@@ -368,11 +368,22 @@ int run_uniform(garage_ec_ctx *ctx, int mode, const uint8_t *src, size_t src_pit
                 size_t n, cudaStream_t st, bool allow_tmap = true)
 {
     const uint32_t ips = items_per_stripe(stride);
-    const size_t max_n = 0xffffffffull / ips;
+    // the kernel's work counter runs past the item count by at most two claimed runs per warp
+    const size_t max_n = (0xffffffffull - (1ull << 24)) / ips;
     TimedLaunch tl(ctx, st);
-    for (size_t s0 = 0; s0 < n; s0 += max_n) {
+    if (n == 0) return GARAGE_EC_OK;
+    // one zeroed work counter per launch (rs_apply_kernel's dynamic schedule): stream-ordered scratch, so the
+    // call stays capturable in a CUDA graph
+    const size_t launches = (n + max_n - 1) / max_n * (size_t)((ctx->m + kRowsPerPass - 1) / kRowsPerPass);
+    void *scratch = nullptr;
+    CU_TRY(ctx, ctx->pool ? cudaMallocFromPoolAsync(&scratch, launches * sizeof(uint32_t), ctx->pool, st)
+                          : cudaMallocAsync(&scratch, launches * sizeof(uint32_t), st));
+    uint32_t *counter = reinterpret_cast<uint32_t *>(scratch);
+    cudaError_t e = cudaMemsetAsync(counter, 0, launches * sizeof(uint32_t), st);
+    int rc = e == cudaSuccess ? GARAGE_EC_OK : set_cuda_error(ctx, e, "cudaMemsetAsync(counter)");
+    for (size_t s0 = 0; s0 < n && rc == GARAGE_EC_OK; s0 += max_n) {
         const size_t cnt = n - s0 < max_n ? n - s0 : max_n;
-        for (int r0 = 0; r0 < ctx->m; r0 += kRowsPerPass) {
+        for (int r0 = 0; r0 < ctx->m && rc == GARAGE_EC_OK; r0 += kRowsPerPass) {
             ApplyParams p;
             memset(&p, 0, sizeof(p));
             p.src = src + s0 * src_pitch;
@@ -381,6 +392,7 @@ int run_uniform(garage_ec_ctx *ctx, int mode, const uint8_t *src, size_t src_pit
             p.dst_pitch = dst_pitch;
             p.shard_len = shard_len ? shard_len + s0 : nullptr;
             p.mismatch = mismatch ? mismatch + s0 : nullptr;
+            p.counter = counter++;
             p.stride = (uint32_t)stride;
             p.n = (uint32_t)cnt;
             p.k = (uint32_t)ctx->k;
@@ -393,12 +405,13 @@ int run_uniform(garage_ec_ctx *ctx, int mode, const uint8_t *src, size_t src_pit
                                               (GEC_SPLIT_STAGE && ctx->k > 16) ? 16 : ctx->k)) ? 1u : 0u;  // box rows: StreamCfg::kSrcRows
             for (uint32_t i = 0; i < p.rows; i++)
                 memcpy(p.coef + i * ctx->k, ctx->P + (r0 + i) * ctx->k, ctx->k);
-            cudaError_t e = mode == kModeEncode ? launch_apply<kModeEncode>(ctx, p, st)
-                                                : launch_apply<kModeVerify>(ctx, p, st);
-            if (e != cudaSuccess) return set_cuda_error(ctx, e, "rs_apply_kernel launch");
+            e = mode == kModeEncode ? launch_apply<kModeEncode>(ctx, p, st) : launch_apply<kModeVerify>(ctx, p, st);
+            if (e != cudaSuccess) rc = set_cuda_error(ctx, e, "rs_apply_kernel launch");
         }
     }
-    return GARAGE_EC_OK;
+    e = cudaFreeAsync(scratch, st);
+    if (e != cudaSuccess && rc == GARAGE_EC_OK) rc = set_cuda_error(ctx, e, "cudaFreeAsync(counter)");
+    return rc;
 }
 
 // Device-resident reconstruct.  plan/counter scratch supplied by the caller (device).

@@ -41,7 +41,8 @@
 //    their own.
 //  * log/antilog tables sit in __constant__ memory and are staged to shared memory by the
 //    decode-planning kernel; the product tables are built from xtime chains (no log lookups).
-//  * Persistent grid: one CTA per SM.
+//  * Persistent grid: one CTA per SM.  Encode / verify warps with whole-item TMA staging claim their work items
+//    from a per-launch counter (StreamCfg::kDynamic); the other uniform shapes keep a fixed stride.
 #pragma once
 #include <cuda.h>  // CUtensorMap (type only; the encoder is fetched through cudaGetDriverEntryPoint)
 #include <cuda_runtime.h>
@@ -88,6 +89,20 @@ namespace garage_ec {
 #endif
 #ifndef GEC_TMA_FROM_K
 #define GEC_TMA_FROM_K 5  // encode / reconstruct use the TMA staging from this k on (k <= 4 is as fast with LDG)
+#endif
+#ifndef GEC_CLAIM_RUN
+#define GEC_CLAIM_RUN 2  // uniform modes, dynamic schedule: consecutive work items a warp claims at once
+#endif
+#ifndef GEC_TAIL_PARTS
+// reconstruct: the last 2 x (CTAs) stripes of a launch are claimed in this many chunk ranges each, so that the end of
+// the launch is shared by every SM instead of the few that claimed the last whole stripes
+#define GEC_TAIL_PARTS 4
+#endif
+#ifndef GEC_NULL_MATH
+// 1 = traffic-ceiling build: column_compute skips the table lookups and the transpose and stores XORs of the
+// staged source vectors, with loads, stages, barriers, item order and stores unchanged.  Its outputs are WRONG;
+// only tools/build_variants.py builds it, to measure what the memory traffic alone allows.
+#define GEC_NULL_MATH 0
 #endif
 
 constexpr int kMaxK = 32;
@@ -150,6 +165,7 @@ struct PlanSlot {
     uint32_t sid;         // stripe index (>= n: no more work)
     int32_t rows;         // rows to produce in this pass (<= 0: nothing to do)
     uint32_t chunk_next;  // next unclaimed 32-column chunk of this stripe
+    uint32_t chunk_end;   // end of the stripe's chunk range claimed in this work unit
     uint32_t len;         // shard_len of the stripe
     uint32_t src_off[kMaxK];             // byte offset of source j inside the stripe
     uint32_t dst_off[kRowsPerPass];      // byte offset of output row i inside the stripe
@@ -175,11 +191,13 @@ __host__ __device__ constexpr int cfg_nw_ldg(int k, int mode)
 }
 // TMA path, k <= 12: measured optimum (total warps; reconstruct includes the builder warp and is then
 // clamped to what the stage memory allows); larger k: by register budget (cfg_nw_tma)
+// RS(10,4) encode and reconstruct: 12 warps measured 0.5 % faster than 16 (encode, with the dynamic schedule) and 20
+// (reconstruct); 8 warps were slower.  Other k were not re-swept.
 __host__ __device__ constexpr int cfg_nw_tma_small(int k, int mode)
 {
-    if (mode == kModePlan) return k <= 6 ? 32 : (k <= 8 ? 28 : 24);
+    if (mode == kModePlan) return k <= 6 ? 32 : (k <= 8 ? 28 : (k == 10 ? 12 : 24));
     if (mode == kModeVerify) return k <= 4 ? 28 : (k <= 8 ? 20 : 16);
-    return k <= 8 ? 20 : 16;
+    return k <= 8 ? 20 : (k == 10 ? 12 : 16);
 }
 // TMA: at most 3 table groups per buffer, fewer (= more zero-table padding) when the table buffers
 // would not leave room for the stages of `want_nw` warps (reconstruct doubles the tables: k = 7 as
@@ -250,6 +268,10 @@ template <int K, int MODE> struct StreamCfg {
         kNwOverride > 0 ? (kTma ? cfg_fit_nw(kNwOverride, kTabBytes, kStageRows, MODE == kModePlan) : kNwOverride) : kWarpsDefault;
     // reconstruct: the last warp is the table builder
     static constexpr int kWarps = MODE == kModePlan ? kWarpsAll - 1 : kWarpsAll;  // consumer warps
+    // uniform modes: warps claim work items from a counter instead of a fixed stride.  Measured on H100 for
+    // k = 4..32: faster with whole-item TMA staging at <= 20 warps (RS(10,4) encode 2.09 -> 1.98 ms), slower with
+    // LDG, with 28 warps (k = 4 verify) and with split staging (k > 16), which keep the fixed stride.
+    static constexpr bool kDynamic = MODE != kModePlan && kTma && !kSplit && kWarps <= 20;
     static constexpr int kThreads = 32 * kWarpsAll;
     static constexpr uint32_t kStageBytes = (uint32_t)kWarps * kStageRows * kStageRowBytes;
     static constexpr uint32_t kSmem = kTabBytes + kStageBytes + kAuxBytes;
@@ -299,7 +321,7 @@ struct ApplyParams {
     const uint32_t *shard_len;  // device, nullable (=> stride)
     const StripePlan *plan;     // kModePlan
     uint32_t *mismatch;         // kModeVerify
-    uint32_t *counter;          // kModePlan dynamic scheduler
+    uint32_t *counter;          // dynamic scheduler, zero at launch: stripes (kModePlan) / work items (uniform modes)
     uint32_t stride;            // bytes between shards
     uint32_t n;                 // stripes
     uint32_t k;                 // sources
@@ -656,6 +678,15 @@ __device__ __forceinline__ void column_compute(uint4 (&d)[CFG::S], uint32_t tab_
 #pragma unroll
         for (int u = 0; u < CFG::S; u++) d[u] = mask_tail(d[u], tail_bytes);
     }
+#if GEC_NULL_MATH
+    (void)acc, (void)tab_addr, (void)lane, (void)row_bytes;
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+        const uint4 a = d[i % CFG::S], b = d[(i + 1) % CFG::S];
+        r[i] = make_uint4(a.x ^ b.x, a.y ^ b.y, a.z ^ b.z, a.w ^ b.w);
+    }
+    return;
+#endif
     // this lane's bank at phase ph of group g: lane xor ph*R
     auto slot_base = [&](auto uc) -> uint32_t {
         constexpr int u = decltype(uc)::value;
@@ -758,8 +789,30 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
         __syncthreads();
 
         const uint32_t ips = p.items_per_stripe;
-        const uint32_t total = p.n * ips;  // host guarantees < 2^32
-        const uint32_t gwarps = gridDim.x * NW;
+        const uint32_t total = p.n * ips;  // host guarantees that total plus the claims past it stay < 2^32
+
+        // Next work item of this warp.  Fixed stride: item = blockIdx.x * NW + warp, then + NW * gridDim.x.
+        // Dynamic: the warp claims runs of GEC_CLAIM_RUN consecutive items from p.counter (zeroed on the stream
+        // before the launch), so SMs that stream faster take more items and none idles at the end while another
+        // still works through a fixed share.  Lane 0 claims the next run one run ahead, so the atomic's latency
+        // hides behind the current run.  Either way a warp's items only grow.
+        uint32_t run_next = CFG::kDynamic ? 0u : blockIdx.x * NW + warp, run_left = 0, run_ahead = 0;
+        if (CFG::kDynamic && lane == 0) run_ahead = atomicAdd(p.counter, (uint32_t)GEC_CLAIM_RUN);
+        auto claim = [&]() -> uint32_t {
+            if constexpr (!CFG::kDynamic) {
+                const uint32_t i = run_next;
+                run_next += gridDim.x * NW;
+                return i;
+            } else {
+                if (run_left == 0) {
+                    run_next = __shfl_sync(0xffffffffu, run_ahead, 0);
+                    run_left = GEC_CLAIM_RUN;
+                    if (lane == 0) run_ahead = atomicAdd(p.counter, (uint32_t)GEC_CLAIM_RUN);
+                }
+                run_left--;
+                return run_next++;
+            }
+        };
 
         // position of this lane's column for a work item (stripe, 32-column chunk)
         struct Pos {
@@ -839,7 +892,7 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
             }
         };
 
-        uint32_t item = blockIdx.x * NW + warp;
+        uint32_t item = claim();
         if constexpr (CFG::kSplit) {
             // k > 16: one table group (<= 16 sources) per phase; the stage is refilled with the next group
             // (or the first group of the next item) as soon as the current one sits in registers
@@ -876,7 +929,7 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
             while (item < total) {
                 const Pos cur = nx;
                 if (!cur.any) {  // chunk past the end of a short stripe: nothing was staged for it
-                    item += gwarps;
+                    item = claim();
                     nx.valid = nx.any = false;
                     if (item < total) {
                         nx = locate(item);
@@ -897,7 +950,7 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
                     if constexpr (g + 1 < NG) {
                         issue_g(cur, std::integral_constant<int, g + 1>{});
                     } else {
-                        item += gwarps;
+                        item = claim();
                         nx.valid = nx.any = false;
                         if (item < total) {
                             nx = locate(item);
@@ -927,7 +980,7 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
                     load_stored(cur, st);
                 }
                 stage_release();  // every lane has its vectors: the stage may be refilled
-                item += gwarps;
+                item = claim();
                 nx.valid = nx.any = false;
                 if (item < total) {
                     nx = locate(item);
@@ -953,7 +1006,7 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
 #pragma unroll
                 for (int i = 0; i < 4; i++) st[i] = stn[i];
                 const Pos cur = nx;
-                item += gwarps;
+                item = claim();
                 nx.valid = nx.any = false;
                 if (item < total) {
                     nx = locate(item);
@@ -970,8 +1023,13 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
         __syncthreads();  // mbarriers initialised
         constexpr uint32_t kTabBuf = CFG::kTabBytes / 2;
         if (warp == (uint32_t)NW) {
-            // ===== builder warp: claim stripes, stage their plans, build their tables one stripe
-            // ahead of the consumers.  Stripe sequence number i uses buffer / slot i & 1.
+            // ===== builder warp: claim work units, stage their plans, build their tables one unit
+            // ahead of the consumers.  Unit sequence number i uses buffer / slot i & 1.
+            // Unit u of the launch's counter: stripe u while u < whole, then the last stripes in GEC_TAIL_PARTS
+            // chunk ranges each (4096 stripes on 132 SMs are 31.03 stripes per SM: with whole stripes only, a
+            // few SMs streamed a 32nd stripe alone at the end).  The parts of a stripe have the same erasure
+            // pattern: a table buffer that gets another part of the stripe it already holds skips the build.
+            const uint32_t whole = p.n > 2 * gridDim.x ? p.n - 2 * gridDim.x : 0;
             uint32_t claimed = 0;
             if (lane == 0) claimed = atomicAdd(p.counter, 1u);
             // pattern whose tables each buffer holds (scalars, not arrays: `b` is a run-time index)
@@ -982,8 +1040,11 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
                 // every consumer warp has left the stripe that used this buffer and slot
                 if (use >= 1) mbar_wait(bar_empty + 8 * b, (use - 1) & 1);
                 PlanSlot &ps = slot[b];
-                const uint32_t s = __shfl_sync(0xffffffffu, claimed, 0);
+                const uint32_t u = __shfl_sync(0xffffffffu, claimed, 0);
                 if (lane == 0) claimed = atomicAdd(p.counter, 1u);  // consumed by the next iteration
+                const bool in_tail = u >= whole;
+                const uint32_t s = in_tail ? whole + (u - whole) / GEC_TAIL_PARTS : u;
+                const uint32_t part = in_tail ? (u - whole) % GEC_TAIL_PARTS : 0u, parts = in_tail ? GEC_TAIL_PARTS : 1u;
                 int rows = 0;
                 unsigned long long kp = 0, ko = 0;
                 if (s < p.n) {
@@ -999,10 +1060,13 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
                     }
                 }
                 if (lane == 0) {
+                    const uint32_t len = s < p.n ? (p.shard_len ? __ldg(p.shard_len + s) : p.stride) : 0;
+                    const uint32_t nch = (((len + 15) >> 4) + 31) >> 5;  // 32-column chunks of the stripe
                     ps.sid = s;
                     ps.rows = rows;
-                    ps.chunk_next = 0;
-                    ps.len = s < p.n ? (p.shard_len ? __ldg(p.shard_len + s) : p.stride) : 0;
+                    ps.chunk_next = part * nch / parts;
+                    ps.chunk_end = (part + 1) * nch / parts;
+                    ps.len = len;
                 }
                 __syncwarp();
                 const bool same = b ? (have1 && kp == bp1 && ko == bo1) : (have0 && kp == bp0 && ko == bo0);
@@ -1060,7 +1124,7 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
                     uint32_t c = 0;
                     if (lane == 0) c = atomicAdd(&ps.chunk_next, 1u);
                     c = __shfl_sync(0xffffffffu, c, 0);
-                    if (c * 32 < nvec) {
+                    if (c < ps.chunk_end) {
                         it.seq = pos;
                         it.s = s;
                         it.chunk = c;
