@@ -36,6 +36,7 @@ ABI_SYMBOLS = [
     "garage_ec_encode_blocks_with_sums", "garage_ec_scrub_repair",
     "garage_ec_numa_info", "garage_ec_bind_thread", "garage_ec_debug_fail_after",
     "garage_ec_set_sum_kind", "garage_ec_set_wait_mode", "garage_ec_copy_for_dma", "garage_ec_shard_sum_host", "garage_ec_reconstruct_stripes",
+    "garage_ec_create_lrc", "garage_ec_code_info", "garage_ec_read_set",
 ]
 
 
@@ -112,6 +113,9 @@ def load_library(build=True):
     L.garage_ec_copy_for_dma.argtypes = [vp, vp, C.c_size_t]
     L.garage_ec_copy_for_dma.restype = None
     L.garage_ec_shard_sum_host.argtypes = [i32, vp, sz, vp]
+    L.garage_ec_create_lrc.argtypes = [C.POINTER(vp), i32, i32, i32, i32]
+    L.garage_ec_code_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32)]
+    L.garage_ec_read_set.argtypes = [vp, vp, vp, vp]
     _lib = L
     return L
 
@@ -169,10 +173,14 @@ class GarageEc:
     or numpy uint8 arrays (HOST mode: synchronous, staged through the library's lanes).
     """
 
-    def __init__(self, device=0, k=10, m=4, kind=VANDERMONDE, matrix=None):
+    def __init__(self, device=0, k=10, m=4, kind=VANDERMONDE, matrix=None, _lrc=None):
         self._L = load_library()
         h = C.c_void_p()
-        if matrix is not None:
+        if _lrc is not None:
+            l, r = _lrc
+            m = l + r
+            rc = self._L.garage_ec_create_lrc(C.byref(h), device, k, l, r)
+        elif matrix is not None:
             mat = np.ascontiguousarray(matrix, dtype=np.uint8)
             if mat.shape != (m, k):
                 raise ValueError("matrix must be m x k")
@@ -183,6 +191,11 @@ class GarageEc:
             raise EcError(rc, self._L.garage_ec_strerror(rc).decode())
         self._h = h
         self.device, self.k, self.m = device, k, m
+
+    @classmethod
+    def lrc(cls, device=0, k=10, l=2, r=2):
+        """LRC(k, l, r) context: l local XOR parities (one per group of k/l data shards), then r Cauchy parities"""
+        return cls(device, k, l + r, _lrc=(l, r))
 
     # -- lifecycle
     def close(self):
@@ -222,6 +235,22 @@ class GarageEc:
         out = np.zeros((self.m, self.k), dtype=np.uint8)
         self._check(self._L.garage_ec_matrix(self._h, _ptr(out)))
         return out
+
+    def code_info(self):
+        """(local groups, global parities): (l, r) for LRC, (0, m) for RS"""
+        a, b = C.c_int(0), C.c_int(0)
+        self._check(self._L.garage_ec_code_info(self._h, C.byref(a), C.byref(b)))
+        return a.value, b.value
+
+    def read_set(self, present, want=None):
+        """shards to fetch to rebuild the wanted absent shards of one stripe: (k+m,) uint8 array, or None if
+        they cannot be rebuilt"""
+        pr = np.ascontiguousarray(present, dtype=np.uint8)
+        wn = None if want is None else np.ascontiguousarray(want, dtype=np.uint8)
+        assert pr.shape == (self.k + self.m,) and (wn is None or wn.shape == pr.shape)
+        out = np.zeros(self.k + self.m, dtype=np.uint8)
+        rc = self._check(self._L.garage_ec_read_set(self._h, _ptr(pr), _ptr(wn), _ptr(out)), (E_UNRECOVERABLE,))
+        return None if rc == E_UNRECOVERABLE else out
 
     def shard_len(self, block_len):
         return int(self._L.garage_ec_shard_len(block_len, self.k))

@@ -243,7 +243,8 @@ struct ShardFileHeader {
     uint32_t shard_len;
     uint8_t sum[32];
     uint32_t hdr_check;  // Adler-32 of bytes [0, 48)
-    uint8_t pad[12];
+    uint8_t pad[12];     // pad[0]: LRC local groups (0 = RS, so files written before it existed read as RS); outside
+                         // hdr_check, so the reader compares it with its own code and quarantines a mismatch
 };
 static_assert(sizeof(ShardFileHeader) == 64, "shard file header is 64 bytes");
 
@@ -265,7 +266,7 @@ struct Node {
     bool up = true;
     bool fsync_data = false;  // data_fsync (util/config.rs), manager.rs:775-789
     std::string dir;          // empty: in-memory store
-    int k = 0, m = 0;
+    int k = 0, m = 0, l = 0;  // l: LRC local groups, 0 = RS
     // in-memory mode: immutable shards behind shared pointers, so the node lock only covers the map operation -- the
     // 100 KB copies happen outside it (the reference shards its lock 256 ways per node, manager.rs:114,679-689; with
     // one lock per node and the copies inside it, 128 clients serialised on 14 mutexes at ~12 GiB/s)
@@ -315,6 +316,7 @@ struct Node {
         hd.shard_len = (uint32_t)n;
         memcpy(hd.sum, mt.sum.data(), 32);
         hd.hdr_check = adler32_small(reinterpret_cast<const uint8_t *>(&hd), 48);
+        hd.pad[0] = (uint8_t)l;
         FILE *f = fopen(tmp.c_str(), "wb");
         if (!f) return false;
         bool ok = fwrite(&hd, sizeof(hd), 1, f) == 1 && (n == 0 || fwrite(bytes, n, 1, f) == 1);
@@ -349,7 +351,7 @@ struct Node {
         // what it claims (a flipped shard_len must not become a 4 GiB resize)
         if (fread(&hd, sizeof(hd), 1, f) == 1 && memcmp(hd.magic, "GEC1", 4) == 0 &&
             hd.hdr_check == adler32_small(reinterpret_cast<const uint8_t *>(&hd), 48) && hd.k == k && hd.m == m &&
-            fstat(fileno(f), &sb) == 0 && (uint64_t)sb.st_size == (uint64_t)hd.shard_len + sizeof(hd)) {
+            hd.pad[0] == l && fstat(fileno(f), &sb) == 0 && (uint64_t)sb.st_size == (uint64_t)hd.shard_len + sizeof(hd)) {
             mt.index = hd.index;
             mt.block_len = hd.block_len;
             mt.shard_len = hd.shard_len;
@@ -735,7 +737,8 @@ struct garage_bm {
     // metrics (src/block/metrics.rs)
     std::atomic<uint64_t> bytes_written{0}, bytes_read{0}, corruption_counter{0}, resync_counter{0},
         resync_error_counter{0}, resync_recv_counter{0}, delete_counter{0}, put_calls{0}, reconstruct_calls{0},
-        scrub_checked{0}, scrub_corrupt{0}, enc_gpu_us{0}, rec_gpu_us{0}, corrupt_data_errors{0}, write_errors{0};
+        scrub_checked{0}, scrub_corrupt{0}, enc_gpu_us{0}, rec_gpu_us{0}, corrupt_data_errors{0}, write_errors{0},
+        resync_shards_read{0};
     std::atomic<uint64_t> put_ns_slot{0}, put_ns_land{0}, put_ns_wait{0}, put_ns_store{0};
 
     size_t shard_len_of(uint32_t block_len) const { return garage_ec_shard_len(block_len, k); }
@@ -906,13 +909,16 @@ struct garage_bm {
     }
 
     // Read the valid shards of `h` from every up node except `skip_node` into the stripe slot
-    // (shard i at slot + i*slot_stride).  Data shards first (a complete set needs no GPU), then only
-    // as many parity shards as it takes to reach k -- the reference likewise stops at the first good
-    // copy (manager.rs:292-334); RpcHelper::try_call_many with quorum k is the real-cluster form.
+    // (shard i at slot + i*slot_stride).  GET (want_in NULL): data shards first (a complete set needs no
+    // GPU), then the survivors garage_ec_read_set names for the missing data shards -- for RS the first
+    // parity shards up to k; the reference likewise stops at the first good copy (manager.rs:292-334).
+    // Resync (want_in = this node's shard): exactly the read set, k/l shards for an LRC local repair.
+    // A shard that cannot be read is taken out of the assumed-present set and the read set recomputed.
     // A shard whose header disagrees with the others on the block length, or that sits under the
-    // wrong index, is treated like a corrupt one.  `all`: do not stop at k (corruption hunting).
+    // wrong index, is treated like a corrupt one.  `all`: read every shard (corruption hunting).
+    // Returns the number of shards read; *ok = the wanted shards can be rebuilt from `have`.
     int gather_into(const Hash &h, int skip_node, uint8_t *slot, uint8_t *have, uint32_t &block_len, bool all = false,
-                    bool for_gpu = false)
+                    bool for_gpu = false, const uint8_t *want_in = nullptr, bool *ok = nullptr)
     {
         int who[64];
         storage_nodes_of(h, who);
@@ -943,11 +949,44 @@ struct garage_bm {
             have[i] = 1;
             count++;
         };
-        for (int i = 0; i < k; i++) {
+        uint8_t tried[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0}, want[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
+        auto attempt = [&](int i) {
+            tried[i] = 1;
             try_shard(i);
-            for_gpu |= !have[i];  // a data shard is missing: this stripe goes through the GPU
+        };
+        if (all) {
+            for (int i = 0; i < tot; i++) attempt(i);
+        } else {
+            if (want_in) {
+                memcpy(want, want_in, tot);
+            } else {
+                for (int i = 0; i < k; i++) {
+                    attempt(i);
+                    for_gpu |= !have[i];  // a data shard is missing: this stripe goes through the GPU
+                    want[i] = !have[i];
+                }
+            }
+            for (;;) {
+                // assume every shard not yet tried on an up node is there; fetch what the read set still lacks
+                uint8_t guess[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M], rd[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
+                for (int i = 0; i < tot; i++) guess[i] = have[i] || (!tried[i] && who[i] != skip_node);
+                if (garage_ec_read_set(ec, guess, want, rd) != GARAGE_EC_OK) break;
+                bool fetched = false, missing = false;
+                for (int i = 0; i < tot; i++) {
+                    if (!rd[i] || have[i]) continue;
+                    missing = true;
+                    attempt(i);
+                    fetched = true;
+                }
+                if (!missing || !fetched) break;
+            }
         }
-        for (int i = k; i < tot && (all || count < k); i++) try_shard(i);
+        if (ok) {
+            uint8_t rd[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
+            if (all)
+                for (int i = 0; i < k; i++) want[i] = !have[i];
+            *ok = garage_ec_read_set(ec, have, want, rd) == GARAGE_EC_OK;
+        }
         block_len = expect;
         return count;
     }
@@ -1061,8 +1100,9 @@ struct garage_bm {
         SlotLease slot(stripe_slots);
         uint8_t have[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M], want[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
         uint32_t block_len = 0;
-        const int count = gather_into(h, -1, slot.p, have, block_len);
-        if (count < k) return GARAGE_BM_E_MISSING_BLOCK;  // manager.rs:336-338
+        bool ok = false;
+        gather_into(h, -1, slot.p, have, block_len, false, false, nullptr, &ok);
+        if (!ok) return GARAGE_BM_E_MISSING_BLOCK;  // manager.rs:336-338
         *out_len = block_len;
         if (block_len > cap) return GARAGE_EC_E_INVALID;
         bool all_data = true;
@@ -1149,12 +1189,13 @@ struct garage_bm {
         SlotLease slot(stripe_slots);
         uint8_t have[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M], want[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
         uint32_t block_len = 0;
-        const int count = gather_into(h, node, slot.p, have, block_len, false, /*for_gpu=*/true);
-        if (count < k) {
+        bool ok = false;
+        want[idx] = 1;
+        resync_shards_read += (uint64_t)gather_into(h, node, slot.p, have, block_len, false, /*for_gpu=*/true, want, &ok);
+        if (!ok) {
             resync_error_counter++;
             return GARAGE_BM_E_MISSING_BLOCK;  // resync.rs:488-494
         }
-        want[idx] = 1;
         int rc2 = reconstruct_in_slot(slot.p, block_len, have, want);
         if (rc2 != GARAGE_BM_OK) {
             resync_error_counter++;
@@ -1492,6 +1533,7 @@ void garage_bm_default_config(garage_bm_config *c)
     c->verify_content_hash = 1;
     c->data_fsync = 0;             // util/config.rs data_fsync default
     c->block_gc_delay_ms = 600000;  // BLOCK_GC_DELAY, manager.rs:49-52
+    c->local_groups = 0;            // RS
 }
 
 static int bm_create(garage_bm **out, const garage_bm_config *cfg)
@@ -1501,6 +1543,13 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
     if (k < 1 || m < 1 || k > GARAGE_EC_MAX_K || m > GARAGE_EC_MAX_M || cfg->n_nodes < k + m || cfg->n_nodes > 256)
         return GARAGE_EC_E_INVALID;
     if (cfg->shard_sum_kind != GARAGE_EC_SUM_BLAKE2 && cfg->shard_sum_kind != GARAGE_EC_SUM_ADLER8) return GARAGE_EC_E_INVALID;
+    const int l = cfg->local_groups;
+    if (l < 0 || (l > 0 && (l >= m || k % l))) return GARAGE_EC_E_INVALID;
+    // every context of the manager runs the same code: RS(k, m), or LRC(k, l, m - l)
+    auto make_ctx = [&](garage_ec_ctx **c) {
+        return l ? garage_ec_create_lrc(c, cfg->cuda_device, k, l, m - l)
+                 : garage_ec_create(c, cfg->cuda_device, k, m, GARAGE_EC_VANDERMONDE);
+    };
     std::unique_ptr<garage_bm> bm(new garage_bm());
     bm->cfg = *cfg;
     if (!bm->cfg.block_size) bm->cfg.block_size = 1u << 20;
@@ -1509,7 +1558,7 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
     bm->tot = k + m;
     bm->sum_kind = cfg->shard_sum_kind;
     bm->slot_stride = garage_ec_stride_for(garage_ec_shard_len(bm->cfg.block_size, k));
-    int rc = garage_ec_create(&bm->ec, cfg->cuda_device, k, m, GARAGE_EC_VANDERMONDE);
+    int rc = make_ctx(&bm->ec);
     if (rc != GARAGE_EC_OK) return rc;  // no GPU => no block manager: there is no CPU fallback
     garage_ec_set_sum_kind(bm->ec, bm->sum_kind);
     if (cfg->n_nodes <= GARAGE_LAYOUT_MAX_NODES) {
@@ -1527,6 +1576,7 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
         Node &nd = *bm->nodes.back();
         nd.k = k;
         nd.m = m;
+        nd.l = cfg->local_groups;
         nd.fsync_data = cfg->data_fsync != 0;
         if (cfg->data_dir && cfg->data_dir[0]) {
             nd.dir = std::string(cfg->data_dir) + "/node" + std::to_string(i);
@@ -1549,8 +1599,8 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
         return code;
     };
     for (int w = 0; w < garage_bm::kWorkers; w++) {
-        rc = garage_ec_create(&bm->enc_ctx[w], cfg->cuda_device, k, m, GARAGE_EC_VANDERMONDE);
-        if (rc == GARAGE_EC_OK) rc = garage_ec_create(&bm->rec_ctx[w], cfg->cuda_device, k, m, GARAGE_EC_VANDERMONDE);
+        rc = make_ctx(&bm->enc_ctx[w]);
+        if (rc == GARAGE_EC_OK) rc = make_ctx(&bm->rec_ctx[w]);
         if (rc != GARAGE_EC_OK) return destroy_on_error(rc);
         garage_ec_set_sum_kind(bm->enc_ctx[w], bm->sum_kind);
         garage_ec_set_sum_kind(bm->rec_ctx[w], bm->sum_kind);
@@ -1867,6 +1917,7 @@ void garage_bm_get_metrics(garage_bm *bm, garage_bm_metrics *o)
     o->reconstruct_call_us = bm->rec_gpu_us;
     o->corrupt_data_errors = bm->corrupt_data_errors;
     o->write_errors = bm->write_errors;
+    o->resync_shards_read = bm->resync_shards_read;
     uint64_t ql = 0;
     for (auto &n : bm->nodes) {
         std::lock_guard<std::mutex> lk(n->mu);

@@ -60,6 +60,7 @@ constexpr int kMaxLaneSets = 4;
 
 struct garage_ec_ctx {
     int device = 0, k = 0, m = 0;
+    int l = 0;  // LRC local groups (garage_ec_create_lrc); 0 = RS (MDS: any k shards decode)
     uint8_t P[kMaxM * kMaxK] = {0};
     int sm_count = 0;
     size_t smem_optin = 0;
@@ -429,13 +430,15 @@ int run_reconstruct(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *present,
     q.n = (uint32_t)n;
     q.k = (uint32_t)ctx->k;
     q.m = (uint32_t)ctx->m;
+    q.l = (uint32_t)ctx->l;
     q.present_is_bad = present_is_bad ? 1u : 0u;
     memcpy(q.P, ctx->P, (size_t)ctx->k * ctx->m);
     const unsigned blocks = (unsigned)((n + kPlanWarps - 1) / kPlanWarps);
-    rs_plan_kernel<<<blocks, kPlanWarps * 32, 0, st>>>(q);
+    if (ctx->l) lrc_plan_kernel<<<blocks, kPlanWarps * 32, 0, st>>>(q);
+    else rs_plan_kernel<<<blocks, kPlanWarps * 32, 0, st>>>(q);
     ctx->launches.fetch_add(1, std::memory_order_relaxed);
     cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_cuda_error(ctx, e, "rs_plan_kernel launch");
+    if (e != cudaSuccess) return set_cuda_error(ctx, e, ctx->l ? "lrc_plan_kernel launch" : "rs_plan_kernel launch");
 
     TimedLaunch tl(ctx, st);
     const size_t pitch = (size_t)(ctx->k + ctx->m) * stride;
@@ -464,6 +467,18 @@ int run_reconstruct(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *present,
 }
 
 size_t plan_scratch_bytes(size_t n) { return n * sizeof(StripePlan) + 16; }
+
+// The shards the plan kernels read for one stripe (present / want: k+m bytes, want nullable = every absent
+// shard), as a bit mask; false if a wanted shard cannot be rebuilt.  HOST paths upload only these.
+bool stripe_read_set(const garage_ec_ctx *ctx, const uint8_t *present, const uint8_t *want, uint64_t *read)
+{
+    uint64_t pm = 0, wm = 0;
+    for (int i = 0; i < ctx->k + ctx->m; i++) {
+        pm |= (uint64_t)(present[i] != 0) << i;
+        wm |= (uint64_t)(!want || want[i] != 0) << i;
+    }
+    return h_read_set(ctx->k, ctx->m, ctx->l, ctx->P, pm, wm, read);
+}
 
 // ---- batched async copies ---------------------------------------------------------------
 // Reconstruct moves many shard-sized pieces per stripe (only the k survivors go up, only the
@@ -548,7 +563,7 @@ int lane_reserve(garage_ec_ctx *ctx, HostLane &L, size_t buf_bytes, size_t small
 
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
-int create_common(garage_ec_ctx **out, int device, int k, int m, const uint8_t *P, int kind)
+int create_common(garage_ec_ctx **out, int device, int k, int m, const uint8_t *P, int kind, int l = 0)
 {
     if (!out) return GARAGE_EC_E_INVALID;
     *out = nullptr;
@@ -567,6 +582,7 @@ int create_common(garage_ec_ctx **out, int device, int k, int m, const uint8_t *
     ctx->device = device;
     ctx->k = k;
     ctx->m = m;
+    ctx->l = l;
     if (P) {
         memcpy(ctx->P, P, (size_t)k * m);
     } else if (!h_build_matrix(k, m, kind, ctx->P)) {
@@ -616,7 +632,7 @@ const char *garage_ec_strerror(int code)
     case GARAGE_EC_E_INVALID: return "invalid argument or geometry";
     case GARAGE_EC_E_CUDA: return "CUDA runtime error";
     case GARAGE_EC_E_NOMEM: return "out of memory";
-    case GARAGE_EC_E_UNRECOVERABLE: return "stripe unrecoverable: fewer than k shards present";
+    case GARAGE_EC_E_UNRECOVERABLE: return "stripe unrecoverable: the present shards do not determine a wanted shard";
     case GARAGE_EC_E_NODEVICE: return "no usable sm_90 CUDA device (no CPU fallback)";
     case GARAGE_EC_E_ALIGN: return "pointer or stride not 16-byte aligned";
     default: return "unknown error";
@@ -631,6 +647,33 @@ int garage_ec_create(garage_ec_ctx **out, int cuda_device, int k, int m, int mat
     }
     if (matrix_kind == GARAGE_EC_CAUCHY && k + m > 256) return GARAGE_EC_E_INVALID;
     return create_common(out, cuda_device, k, m, nullptr, matrix_kind);
+}
+
+int garage_ec_create_lrc(garage_ec_ctx **out, int cuda_device, int k, int l, int r)
+{
+    uint8_t P[kMaxM * kMaxK];
+    if (!h_build_lrc(k, l, r, P)) {
+        if (out) *out = nullptr;
+        return GARAGE_EC_E_INVALID;
+    }
+    return create_common(out, cuda_device, k, l + r, P, 0, l);
+}
+
+int garage_ec_code_info(const garage_ec_ctx *ctx, int *local_groups, int *global_parity)
+{
+    if (!ctx) return GARAGE_EC_E_INVALID;
+    if (local_groups) *local_groups = ctx->l;
+    if (global_parity) *global_parity = ctx->m - ctx->l;
+    return GARAGE_EC_OK;
+}
+
+int garage_ec_read_set(const garage_ec_ctx *ctx, const uint8_t *present, const uint8_t *want, uint8_t *read_out)
+{
+    if (!ctx || !present || !read_out) return GARAGE_EC_E_INVALID;
+    uint64_t rd = 0;
+    const bool ok = stripe_read_set(ctx, present, want, &rd);
+    for (int i = 0; i < ctx->k + ctx->m; i++) read_out[i] = (uint8_t)((rd >> i) & 1);
+    return ok ? GARAGE_EC_OK : GARAGE_EC_E_UNRECOVERABLE;
 }
 
 int garage_ec_create_with_matrix(garage_ec_ctx **out, int cuda_device, int k, int m,
@@ -1011,10 +1054,11 @@ static int reconstruct_host(garage_ec_ctx *ctx, uint8_t *shards, uint8_t *const 
             if (st_o[s] != 0) return GARAGE_EC_E_UNRECOVERABLE;
         return GARAGE_EC_OK;
     }
-    const size_t k = ctx->k, tot = ctx->k + ctx->m;
+    const size_t tot = ctx->k + ctx->m;
     size_t cs = kHostChunkBytes / (tot * stride);
     if (cs < 1) cs = 1;
     if (cs > n) cs = n;
+    std::vector<uint8_t> rec_ok(cs);  // per stripe of the chunk: stripe_read_set succeeded
     // small buffer layout per lane: present | want | status | shard_len | plan+counter
     const size_t o_present = 0, o_want = align_up(cs * tot, 16), o_status = o_want + align_up(cs * tot, 16);
     const size_t o_len = o_status + align_up(cs * 4, 16), o_plan = o_len + align_up(cs * 4, 16);
@@ -1030,22 +1074,15 @@ static int reconstruct_host(garage_ec_ctx *ctx, uint8_t *shards, uint8_t *const 
         HostLane &L = lanes[c % kHostLanes];
         const size_t cnt = n - s0 < cs ? n - s0 : cs;
         uint8_t *d_sh = L.d_buf;
-        // H2D: only the k survivors (first k present shards) of stripes that have work to do
+        // H2D: only the survivors the kernel reads (stripe_read_set) of stripes that have work to do
         for (size_t s = s0; s < s0 + cnt; s++) {
-            const uint8_t *pr = present + s * tot;
-            size_t np = 0;
-            bool work = false;
-            for (size_t i = 0; i < tot; i++) {
-                np += pr[i] ? 1 : 0;
-                work |= !pr[i] && (!want || want[s * tot + i]);
-            }
-            if (np < k || !work) continue;
-            size_t used = 0;
-            for (size_t i = 0; i < tot && used < k; i++) {
-                if (!pr[i]) continue;
-                up.add(d_sh + ((s - s0) * tot + i) * stride, shard_at(s, i), stride);
-                used++;
-            }
+            uint64_t rd = 0;
+            bool work = false;  // a wanted shard is absent
+            for (size_t i = 0; i < tot; i++) work |= !present[s * tot + i] && (!want || want[s * tot + i]);
+            rec_ok[s - s0] = stripe_read_set(ctx, present + s * tot, want ? want + s * tot : nullptr, &rd);
+            if (!rec_ok[s - s0] || !work) continue;
+            for (size_t i = 0; i < tot; i++)
+                if ((rd >> i) & 1) up.add(d_sh + ((s - s0) * tot + i) * stride, shard_at(s, i), stride);
         }
         rc = up.flush(ctx, cudaMemcpyHostToDevice, L.stream);
         if (rc) return rc;
@@ -1074,9 +1111,7 @@ static int reconstruct_host(garage_ec_ctx *ctx, uint8_t *shards, uint8_t *const 
         // D2H: exactly the shards that were rebuilt
         for (size_t s = s0; s < s0 + cnt; s++) {
             const uint8_t *pr = present + s * tot;
-            size_t np = 0;
-            for (size_t i = 0; i < tot; i++) np += pr[i] ? 1 : 0;
-            if (np < k) continue;
+            if (!rec_ok[s - s0]) continue;
             const size_t len = shard_len ? shard_len[s] : stride;
             const size_t bytes = align_up(len, 16);
             for (size_t i = 0; i < tot; i++) {
@@ -1626,15 +1661,18 @@ int garage_ec_decode_blocks(garage_ec_ctx *ctx, const uint8_t *shards, const uin
 
     // stripes with an absent data shard go to the GPU; the rest is a host-side join
     std::vector<size_t> need;
+    std::vector<uint64_t> reads(n_blocks);  // survivors the kernel reads (data shards wanted)
+    std::vector<uint8_t> ok(n_blocks);
+    std::vector<uint8_t> want_data(tot);
+    for (size_t i = 0; i < tot; i++) want_data[i] = i < k ? 1 : 0;
     bool any_bad = false;
     for (size_t s = 0; s < n_blocks; s++) {
         const uint8_t *pr = present + s * tot;
-        size_t np = 0;
         bool data_missing = false;
-        for (size_t i = 0; i < tot; i++) np += pr[i] ? 1 : 0;
         for (size_t j = 0; j < k; j++) data_missing |= !pr[j];
         if (garage_ec_shard_len(block_len[s], (int)k) > stride) return GARAGE_EC_E_INVALID;
-        if (np < k) {
+        ok[s] = stripe_read_set(ctx, pr, want_data.data(), &reads[s]);
+        if (!ok[s]) {
             if (status) status[s] = GARAGE_EC_E_UNRECOVERABLE;
             any_bad = true;
             continue;
@@ -1671,14 +1709,11 @@ int garage_ec_decode_blocks(garage_ec_ctx *ctx, const uint8_t *shards, const uin
                 memcpy(hp + q * tot, present + s * tot, tot);
                 for (size_t i = 0; i < tot; i++) hw[q * tot + i] = i < k ? 1 : 0;  // data shards only
                 hl[q] = garage_ec_shard_len(block_len[s], (int)k);
-                // H2D: only the k survivors the kernel reads (the first k present shards) -- the
-                // GET path is PCIe-bound, absent and surplus shards stay on the host
-                size_t used = 0;
-                for (size_t i = 0; i < tot && used < k; i++) {
-                    if (!present[s * tot + i]) continue;
-                    up.add(L.d_buf + (q * tot + i) * stride, shards + (s * tot + i) * stride, align_up(hl[q], 16));
-                    used++;
-                }
+                // H2D: only the survivors the kernel reads -- the GET path is PCIe-bound, absent and
+                // surplus shards stay on the host
+                for (size_t i = 0; i < tot; i++)
+                    if ((reads[s] >> i) & 1)
+                        up.add(L.d_buf + (q * tot + i) * stride, shards + (s * tot + i) * stride, align_up(hl[q], 16));
             }
             rc = up.flush(ctx, cudaMemcpyHostToDevice, L.stream);
             if (rc) return rc;
@@ -1711,9 +1746,7 @@ int garage_ec_decode_blocks(garage_ec_ctx *ctx, const uint8_t *shards, const uin
         // (framing: block = shard0|shard1|...)
         for (size_t s = 0; s < n_blocks; s++) {
             const uint8_t *pr = present + s * tot;
-            size_t np = 0;
-            for (size_t i = 0; i < tot; i++) np += pr[i] ? 1 : 0;
-            if (np < k) continue;
+            if (!ok[s]) continue;
             const size_t Ls = garage_ec_shard_len(block_len[s], (int)k);
             for (size_t j = 0; j < k; j++) {
                 if (!pr[j]) continue;
@@ -1727,10 +1760,7 @@ int garage_ec_decode_blocks(garage_ec_ctx *ctx, const uint8_t *shards, const uin
         return any_bad ? GARAGE_EC_E_UNRECOVERABLE : GARAGE_EC_OK;
     }
     for (size_t s = 0; s < n_blocks; s++) {
-        const uint8_t *pr = present + s * tot;
-        size_t np = 0;
-        for (size_t i = 0; i < tot; i++) np += pr[i] ? 1 : 0;
-        if (np < k) continue;
+        if (!ok[s]) continue;
         const size_t Ls = garage_ec_shard_len(block_len[s], (int)k);
         for (size_t j = 0; j < k; j++) {
             const size_t off = j * Ls;

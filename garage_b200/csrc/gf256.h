@@ -85,4 +85,87 @@ inline bool h_build_matrix(int k, int m, int kind, uint8_t *P)
     return true;
 }
 
+// LRC(k, l, r) parity rows (DESIGN.md section 2): l local rows (row g = 1 on data [g*k/l, (g+1)*k/l)), then the
+// r Cauchy rows of RS(k, r).  P is (l + r) x k.
+inline bool h_build_lrc(int k, int l, int r, uint8_t *P)
+{
+    if (k < 1 || k > GARAGE_EC_MAX_K_HOST || l < 1 || r < 1 || k % l || l + r > GARAGE_EC_MAX_M_HOST) return false;
+    const int gs = k / l;
+    for (int g = 0; g < l; g++)
+        for (int j = 0; j < k; j++) P[g * k + j] = (uint8_t)(j / gs == g);
+    return h_build_matrix(k, r, 1, P + l * k);
+}
+
+// Survivor set of one stripe, the host twin of the plan kernels (DESIGN.md section 2).  Bit i of present / want:
+// shard i present / wanted (only absent wanted shards are rebuilt).  l = 0: RS, the first k present shards.
+// l > 0: LRC rule 1 (local repair) if it applies, else rule 2 (greedy rank basis in index order).  Returns false
+// if a wanted shard cannot be rebuilt; *read = the shards to read.
+inline bool h_read_set(int k, int m, int l, const uint8_t *P, uint64_t present, uint64_t want, uint64_t *read)
+{
+    const int tot = k + m;
+    const uint64_t all = tot >= 64 ? ~0ull : ((1ull << tot) - 1);
+    present &= all;
+    want &= all & ~present;
+    *read = 0;
+    if (l == 0) {
+        int used = 0;
+        for (int i = 0; i < tot && used < k; i++)
+            if ((present >> i) & 1) {
+                *read |= 1ull << i;
+                used++;
+            }
+        return used == k;
+    }
+    const int gs = k / l;
+    auto group_mask = [&](int g) { return (((1ull << gs) - 1) << (g * gs)) | (1ull << (k + g)); };
+    bool local = true;
+    uint64_t rmask = 0;
+    for (int o = 0; o < tot && local; o++) {
+        if (!((want >> o) & 1)) continue;
+        if (o >= k + l) {
+            local = false;
+            break;
+        }
+        const uint64_t gm = group_mask(o < k ? o / gs : o - k);
+        if ((gm & ~present) != (1ull << o)) local = false;
+        rmask |= gm & ~(1ull << o);
+    }
+    if (local) {
+        *read = rmask;
+        return true;
+    }
+    auto row = [&](int c, int j) -> uint8_t { return c < k ? (uint8_t)(c == j) : P[(c - k) * k + j]; };
+    uint8_t R[GARAGE_EC_MAX_K_HOST][GARAGE_EC_MAX_K_HOST];
+    int piv[GARAGE_EC_MAX_K_HOST], nb = 0;
+    auto reduce = [&](uint8_t *v) {
+        for (int b = 0; b < nb; b++) {
+            const uint8_t f = v[piv[b]];
+            if (f)
+                for (int j = 0; j < k; j++) v[j] ^= h_mul(f, R[b][j]);
+        }
+    };
+    for (int c = 0; c < tot && nb < k; c++) {
+        if (!((present >> c) & 1)) continue;
+        uint8_t v[GARAGE_EC_MAX_K_HOST];
+        for (int j = 0; j < k; j++) v[j] = row(c, j);
+        reduce(v);
+        int p = 0;
+        while (p < k && !v[p]) p++;
+        if (p == k) continue;
+        const uint8_t iv = h_inv(v[p]);
+        for (int j = 0; j < k; j++) R[nb][j] = h_mul(v[j], iv);
+        piv[nb++] = p;
+        *read |= 1ull << c;
+    }
+    for (int o = 0; o < tot; o++) {
+        if (!((want >> o) & 1)) continue;
+        uint8_t v[GARAGE_EC_MAX_K_HOST];
+        for (int j = 0; j < k; j++) v[j] = row(o, j);
+        reduce(v);
+        for (int j = 0; j < k; j++)
+            if (v[j]) return false;
+    }
+    return true;
+}
+
 }  // namespace garage_ec

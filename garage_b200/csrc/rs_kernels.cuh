@@ -167,6 +167,7 @@ struct PlanSlot {
     uint32_t chunk_next;  // next unclaimed 32-column chunk of this stripe
     uint32_t chunk_end;   // end of the stripe's chunk range claimed in this work unit
     uint32_t len;         // shard_len of the stripe
+    uint32_t nsurv;       // sources read; sources >= nsurv are neither fetched nor looked up (zero vectors)
     uint32_t src_off[kMaxK];             // byte offset of source j inside the stripe
     uint32_t dst_off[kRowsPerPass];      // byte offset of output row i inside the stripe
     uint8_t coef[kRowsPerPass * kMaxK];  // coef[i*kMaxK + j]
@@ -306,9 +307,10 @@ struct __align__(16) StripePlan {
     unsigned long long key_present;  // bit i: shard i present
     unsigned long long key_out;      // bit i: shard i is rebuilt
     uint8_t nrows;                   // number of shards rebuilt (0..m)
-    uint8_t unrecoverable;           // 1 if < k present
-    uint8_t pad[6];
-    uint8_t surv[kMaxK];           // source shard indices (first k present)
+    uint8_t unrecoverable;           // 1 if a wanted shard cannot be rebuilt
+    uint8_t nsurv;                   // sources read: surv[0..nsurv) (k for RS; <= k for LRC)
+    uint8_t pad[5];
+    uint8_t surv[kMaxK];           // source shard indices, ascending (RS: the first k present)
     uint8_t out_idx[kMaxM];        // rebuilt shard indices
     uint8_t coef[kMaxM][kMaxK];  // out[r] = XOR_j coef[r][j] * shard[surv[j]]
 };
@@ -494,6 +496,7 @@ __device__ __forceinline__ void build_tables(uint32_t *tab, const uint8_t *coef,
         constexpr int g = decltype(gc)::value;
         constexpr int lg = LAY.lg[g];
         constexpr int NTQ = lg <= 3 ? 1 : (lg == 4 ? 2 : 4);  // tables inside one bank quad
+        if (LAY.base[g] >= K && LAY.base[g] < LAYC::kK) return;  // plan mode, K = nsurv: no source of this group is read
         // does this warp own a unit of this group at all?
         bool any = false;
 #pragma unroll
@@ -642,26 +645,29 @@ template <class CFG, int U> __device__ __forceinline__ constexpr bool slot_may_p
 // LDG: one 16-byte column of every source straight into registers.
 //   sp     : address of this lane's column in source 0 (uniform modes) / shard 0 (plan mode)
 //   kPlan  : source j lives at sp + src_off[j] (smem) instead of sp + j*stride
+//   nsrc   : sources j >= nsrc read as zero (plan mode: an LRC local repair reads only its group)
 template <class CFG, bool kPlan>
 __device__ __forceinline__ void column_load(const uint8_t *sp, uint32_t stride, const uint32_t *src_off,
-                                            uint32_t lane, uint4 (&d)[CFG::S])
+                                            uint32_t lane, uint4 (&d)[CFG::S], uint32_t nsrc = CFG::kK)
 {
     static_for<0, CFG::S>([&](auto uc) {
         constexpr int u = decltype(uc)::value;
         const uint32_t j = lane_source<CFG, u>(lane);
-        if (!slot_may_pad<CFG, u>() || j < (uint32_t)CFG::kK) d[u] = ldg_stream(sp + (kPlan ? src_off[j] : j * stride));
+        if ((!slot_may_pad<CFG, u>() || j < (uint32_t)CFG::kK) && (!kPlan || j < nsrc))
+            d[u] = ldg_stream(sp + (kPlan ? src_off[j] : j * stride));
         else d[u] = make_uint4(0, 0, 0, 0);
     });
 }
 // TMA: the same vectors out of the warp's stage (row j = source j, 512 B per row)
+// (rows j >= nsrc were not fetched: they read as zero, and entry 0 of every table is 0)
 template <class CFG>
 __device__ __forceinline__ void stage_read(uint32_t stage_lane_addr /* stage + lane*16 */, uint32_t lane,
-                                           uint4 (&d)[CFG::S])
+                                           uint4 (&d)[CFG::S], uint32_t nsrc = CFG::kK)
 {
     static_for<0, CFG::S>([&](auto uc) {
         constexpr int u = decltype(uc)::value;
         const uint32_t j = lane_source<CFG, u>(lane);
-        if (!slot_may_pad<CFG, u>() || j < (uint32_t)CFG::kK) d[u] = lds_v4(stage_lane_addr + j * kStageRowBytes);
+        if ((!slot_may_pad<CFG, u>() || j < (uint32_t)CFG::kK) && j < nsrc) d[u] = lds_v4(stage_lane_addr + j * kStageRowBytes);
         else d[u] = make_uint4(0, 0, 0, 0);
     });
 }
@@ -714,14 +720,14 @@ __device__ __forceinline__ void column_compute(uint4 (&d)[CFG::S], uint32_t tab_
 
 // ---- one table group at a time (split staging): rows of group g sit at stage rows 0..size-1
 template <class CFG, int G>
-__device__ __forceinline__ void group_read(uint32_t stage_lane_addr, uint32_t lane, uint4 (&d)[16])
+__device__ __forceinline__ void group_read(uint32_t stage_lane_addr, uint32_t lane, uint4 (&d)[16], uint32_t nsrc = CFG::kK)
 {
     constexpr TabLayout LAY = CFG::kLay;
     constexpr int lg = LAY.lg[G], n = 1 << lg;
     static_for<0, n>([&](auto pc) {
         constexpr int ph = decltype(pc)::value;
         const uint32_t row = (uint32_t)ph ^ (lg ? (lane >> (5 - lg)) : 0u);  // source base + row
-        if (LAY.base[G] + n <= (int)CFG::kK || (uint32_t)LAY.base[G] + row < (uint32_t)CFG::kK)
+        if ((LAY.base[G] + n <= (int)CFG::kK || (uint32_t)LAY.base[G] + row < (uint32_t)CFG::kK) && (uint32_t)LAY.base[G] + row < nsrc)
             d[ph] = lds_v4(stage_lane_addr + row * kStageRowBytes);
         else d[ph] = make_uint4(0, 0, 0, 0);
     });
@@ -1020,7 +1026,10 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
         }
     } else {
         // ---- per-stripe matrices, no block-wide barrier after this one --------------------------
-        __syncthreads();  // mbarriers initialised
+        // Sources past a plan's nsurv read as zero vectors, and the builder skips table groups that hold none of its
+        // sources: those lookups hit row 0 of tables that may never have been built.  Row 0 of every table is 0.
+        for (uint32_t i = tid; i < 2 * CFG::kLay.ngroups * 32; i += blockDim.x) tab[(i >> 5) * (kGroupBytes / 4) + (i & 31)] = 0;
+        __syncthreads();  // mbarriers initialised, row 0 of the tables zeroed
         constexpr uint32_t kTabBuf = CFG::kTabBytes / 2;
         if (warp == (uint32_t)NW) {
             // ===== builder warp: claim work units, stage their plans, build their tables one unit
@@ -1046,12 +1055,14 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
                 const uint32_t s = in_tail ? whole + (u - whole) / GEC_TAIL_PARTS : u;
                 const uint32_t part = in_tail ? (u - whole) % GEC_TAIL_PARTS : 0u, parts = in_tail ? GEC_TAIL_PARTS : 1u;
                 int rows = 0;
+                uint32_t ns = 0;
                 unsigned long long kp = 0, ko = 0;
                 if (s < p.n) {
                     const StripePlan *pl = p.plan + s;
                     rows = pl->unrecoverable ? 0 : min(kRowsPerPass, (int)pl->nrows - (int)p.row_off);
                     if (rows > 0) {
-                        if (lane < (uint32_t)K) ps.src_off[lane] = (uint32_t)pl->surv[lane] * p.stride;
+                        ns = pl->nsurv;
+                        if (lane < ns) ps.src_off[lane] = (uint32_t)pl->surv[lane] * p.stride;
                         if (lane < (uint32_t)rows) ps.dst_off[lane] = (uint32_t)pl->out_idx[p.row_off + lane] * p.stride;
                         for (uint32_t e = lane; e < (uint32_t)rows * kMaxK; e += 32)
                             ps.coef[e] = pl->coef[p.row_off + e / kMaxK][e % kMaxK];
@@ -1067,11 +1078,12 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
                     ps.chunk_next = part * nch / parts;
                     ps.chunk_end = (part + 1) * nch / parts;
                     ps.len = len;
+                    ps.nsurv = ns;
                 }
                 __syncwarp();
                 const bool same = b ? (have1 && kp == bp1 && ko == bo1) : (have0 && kp == bp0 && ko == bo0);
                 if (rows > 0 && !same) {
-                    build_tables<CFG>(tab + b * (kTabBuf / 4), ps.coef, kMaxK, (uint32_t)rows, 0, 1, K);
+                    build_tables<CFG>(tab + b * (kTabBuf / 4), ps.coef, kMaxK, (uint32_t)rows, 0, 1, (int)ns);
                     if (b) {
                         bp1 = kp;
                         bo1 = ko;
@@ -1095,7 +1107,7 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
         bool ended = false;    // the terminal slot (sid >= n) was seen
         uint32_t pend = kNone; // sequence number of the item whose lookups are still to run
         struct It {
-            uint32_t seq, s, chunk, nvec, len;
+            uint32_t seq, s, chunk, nvec, len, nsurv;
             int rows;
             bool valid;
         };
@@ -1130,6 +1142,7 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
                         it.chunk = c;
                         it.nvec = nvec;
                         it.len = len;
+                        it.nsurv = ps.nsurv;
                         it.rows = rows;
                         it.valid = true;
                         return;
@@ -1151,10 +1164,11 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
                 const PlanSlot &ps = slot[it.seq & 1];
                 const uint8_t *sbase = p.src + (unsigned long long)it.s * p.src_pitch + (size_t)it.chunk * kStageRowBytes;
                 const uint32_t rb = min(kStageRowBytes, (it.nvec - it.chunk * 32) * 16);
-                mbar_arrive_expect_tx(bar_stage, rb * nrow);
+                const uint32_t nr = it.nsurv > (uint32_t)LAY.base[g] ? min((uint32_t)nrow, it.nsurv - LAY.base[g]) : 0u;
+                mbar_arrive_expect_tx(bar_stage, rb * nr);
 #pragma unroll
                 for (int r = 0; r < nrow; r++)
-                    bulk_g2s(stage_addr + r * kStageRowBytes, sbase + ps.src_off[LAY.base[g] + r], rb, bar_stage);
+                    if ((uint32_t)r < nr) bulk_g2s(stage_addr + r * kStageRowBytes, sbase + ps.src_off[LAY.base[g] + r], rb, bar_stage);
             }
         };
         auto fetch = [&](const It &it) {
@@ -1165,15 +1179,16 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
             } else if constexpr (TMA) {
                 if (lane == 0) {
                     const uint32_t rb = min(kStageRowBytes, (it.nvec - it.chunk * 32) * 16);
-                    mbar_arrive_expect_tx(bar_stage, rb * K);
+                    mbar_arrive_expect_tx(bar_stage, rb * it.nsurv);
 #pragma unroll
                     for (int j = 0; j < K; j++)
-                        bulk_g2s(stage_addr + j * kStageRowBytes, sbase + ps.src_off[j] + (size_t)it.chunk * kStageRowBytes, rb,
-                                 bar_stage);
+                        if ((uint32_t)j < it.nsurv)
+                            bulk_g2s(stage_addr + j * kStageRowBytes, sbase + ps.src_off[j] + (size_t)it.chunk * kStageRowBytes, rb,
+                                     bar_stage);
                 }
             } else {
                 const uint32_t col = it.chunk * 32 + lane;
-                if (col < it.nvec) column_load<CFG, true>(sbase + (size_t)col * 16, p.stride, ps.src_off, lane, dn);
+                if (col < it.nvec) column_load<CFG, true>(sbase + (size_t)col * 16, p.stride, ps.src_off, lane, dn, it.nsurv);
             }
         };
 
@@ -1193,7 +1208,7 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
                     uint4 d[16];
                     mbar_wait(bar_stage, stage_parity);
                     stage_parity ^= 1;
-                    group_read<CFG, g>(stage_addr + lane * 16, lane, d);
+                    group_read<CFG, g>(stage_addr + lane * 16, lane, d, cur.nsurv);
                     stage_release();  // every lane has its vectors: the stage may be refilled
                     if constexpr (g + 1 < NG) {
                         fetch_group(cur, std::integral_constant<int, g + 1>{});  // next group of the same item
@@ -1228,7 +1243,7 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
             if constexpr (TMA) {
                 mbar_wait(bar_stage, stage_parity);
                 stage_parity ^= 1;
-                stage_read<CFG>(stage_addr + lane * 16, lane, d);
+                stage_read<CFG>(stage_addr + lane * 16, lane, d, cur.nsurv);
                 stage_release();  // every lane has its vectors: the stage may be refilled
             } else {
 #pragma unroll
@@ -1268,6 +1283,7 @@ struct PlanParams {
     StripePlan *plan;        // n
     uint32_t *counter;       // reset to 0 for the apply kernel's scheduler
     uint32_t n, k, m;
+    uint32_t l;               // LRC local groups (lrc_plan_kernel); 0 for RS
     uint32_t present_is_bad;  // 1: `present` holds "bad" flags (scrub): a shard is present iff flag == 0
     alignas(16) uint8_t P[kMaxM * kMaxK];  // parity rows, P[i*k + j] (16-byte aligned: staged with uint4 loads)
 };
@@ -1343,6 +1359,7 @@ __global__ void __launch_bounds__(kPlanWarps * 32) rs_plan_kernel(const __grid_c
         pl->key_out = outmask;
         pl->nrows = (uint8_t)nrows;
         pl->unrecoverable = bad ? 1 : 0;
+        pl->nsurv = (uint8_t)k;
         if (q.status) q.status[s] = bad ? -4 : 0;
     }
     __syncwarp();
@@ -1437,6 +1454,148 @@ __global__ void __launch_bounds__(kPlanWarps * 32) rs_plan_kernel(const __grid_c
     }
     if (lane < k) pl->surv[lane] = s_surv[warp][lane];
     if (lane < (uint32_t)nrows) pl->out_idx[lane] = s_out[warp][lane];
+}
+
+// LRC(k, l, r) planning (DESIGN.md section 2), one warp per stripe.  Generator rows: data j = e_j, parity i = P[i]
+// (the l all-ones local rows, then the r Cauchy rows).  A wanted row is rebuildable iff it lies in the span of the
+// present rows, so fewer than k present shards may do.  Survivors:
+//   rule 1 (local repair): every wanted shard is a data shard or a local parity and is the only absent member of its
+//          group (the group's data plus its local parity): the survivors are the other members, coefficients all 1;
+//   rule 2 otherwise: present rows greedily in index order, kept if they raise the rank (<= k rows); every wanted
+//          row is expressed in that basis.
+// Rule 2 is an incremental Gauss-Jordan over lanes = columns: basis row b is stored reduced ([row | T_b], where
+// T_b gives it as a combination of the chosen survivors), and a new row is reduced against the basis rows in
+// insertion order, which zeroes it at every earlier pivot.
+__global__ void __launch_bounds__(kPlanWarps * 32) lrc_plan_kernel(const __grid_constant__ PlanParams q)
+{
+    __shared__ __align__(16) uint8_t s_gf[sizeof(GfTables)];
+    uint8_t *const s_exp = s_gf, *const s_log = s_gf + 512;
+    __shared__ uint8_t s_R[kPlanWarps][kMaxK][2 * kMaxK];
+    __shared__ uint8_t s_piv[kPlanWarps][kMaxK];
+    __shared__ uint8_t s_surv[kPlanWarps][kMaxK];
+    __shared__ __align__(16) uint8_t s_P[kMaxM * kMaxK];
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    stage_gf_tables(s_gf);
+    {
+        const uint4 *src = reinterpret_cast<const uint4 *>(q.P);
+        for (uint32_t i = warp; i < sizeof(q.P) / 16; i += blockDim.x >> 5) {
+            const uint4 v = src[i];
+            if (lane < 4) reinterpret_cast<uint32_t *>(s_P)[i * 4 + lane] = lane == 0 ? v.x : (lane == 1 ? v.y : (lane == 2 ? v.z : v.w));
+        }
+    }
+    if (blockIdx.x == 0 && tid == 0) *q.counter = 0;
+    __syncthreads();
+    auto mul = [&](uint32_t a, uint32_t b) -> uint32_t {
+        return (a && b) ? s_exp[s_log[a] + s_log[b]] : 0u;
+    };
+
+    const uint32_t s = blockIdx.x * kPlanWarps + warp;
+    if (s >= q.n) return;
+    const uint32_t k = q.k, m = q.m, l = q.l, tot = k + m, gs = k / l;
+    StripePlan *pl = q.plan + s;
+    const uint8_t *pr = q.present + (size_t)s * tot;
+    const uint8_t *wn = q.want ? q.want + (size_t)s * tot : nullptr;
+    const bool inv = q.present_is_bad != 0;
+    const bool p0 = lane < tot && ((pr[lane] != 0) != inv);
+    const bool p1 = lane + 32 < tot && ((pr[lane + 32] != 0) != inv);
+    const unsigned long long present =
+        (unsigned long long)__ballot_sync(0xffffffffu, p0) | ((unsigned long long)__ballot_sync(0xffffffffu, p1) << 32);
+    const bool w0 = lane < tot && !p0 && (!wn || wn[lane] != 0);
+    const bool w1 = lane + 32 < tot && !p1 && (!wn || wn[lane + 32] != 0);
+    const unsigned long long outmask =
+        (unsigned long long)__ballot_sync(0xffffffffu, w0) | ((unsigned long long)__ballot_sync(0xffffffffu, w1) << 32);
+    const int nrows = __popcll(outmask);
+    // generator row c, column j
+    auto grow = [&](uint32_t c, uint32_t j) -> uint32_t { return c < k ? (uint32_t)(c == j) : (uint32_t)s_P[(c - k) * k + j]; };
+    auto group_mask = [&](uint32_t g) -> unsigned long long {
+        return (((1ull << gs) - 1) << (g * gs)) | (1ull << (k + g));
+    };
+
+    // rule 1 (warp-uniform)
+    bool local = true;
+    unsigned long long rmask = 0;
+    for (unsigned long long om = outmask; om; om &= om - 1) {
+        const uint32_t o = (uint32_t)(__ffsll((long long)om) - 1);
+        if (o >= k + l) {
+            local = false;
+            break;
+        }
+        const unsigned long long gm = group_mask(o < k ? o / gs : o - k);
+        if ((gm & ~present) != (1ull << o)) {
+            local = false;
+            break;
+        }
+        rmask |= gm & ~(1ull << o);
+    }
+    uint32_t nsurv = 0;
+    bool ok = true;
+    if (local) {
+        nsurv = (uint32_t)__popcll(rmask);
+        // lane j < nsurv: survivor j = the j-th set bit of rmask
+        unsigned long long mm = rmask;
+        for (uint32_t j = 0; j < lane && mm; j++) mm &= mm - 1;
+        const uint32_t sj = mm ? (uint32_t)(__ffsll((long long)mm) - 1) : 0u;
+        int r = 0;
+        for (unsigned long long om = outmask; om; om &= om - 1, r++) {
+            const uint32_t o = (uint32_t)(__ffsll((long long)om) - 1);
+            const unsigned long long gm = group_mask(o < k ? o / gs : o - k);
+            if (lane < k) pl->coef[r][lane] = (lane < nsurv && ((gm >> sj) & 1)) ? 1 : 0;
+        }
+        if (lane < nsurv) pl->surv[lane] = (uint8_t)sj;
+    } else {
+        // rule 2: greedy basis in index order
+        uint8_t(*R)[2 * kMaxK] = s_R[warp];
+        for (unsigned long long pm = present; pm && nsurv < k; pm &= pm - 1) {
+            const uint32_t c = (uint32_t)(__ffsll((long long)pm) - 1);
+            uint32_t v = lane < k ? grow(c, lane) : 0u, t = lane == nsurv ? 1u : 0u;
+            for (uint32_t b = 0; b < nsurv; b++) {
+                const uint32_t f = __shfl_sync(0xffffffffu, v, s_piv[warp][b]);
+                if (f) {
+                    v ^= mul(f, R[b][lane]);
+                    t ^= mul(f, R[b][kMaxK + lane]);
+                }
+            }
+            const uint32_t nz = __ballot_sync(0xffffffffu, v != 0);
+            if (!nz) continue;  // in the span of the rows already chosen
+            const uint32_t piv = __ffs(nz) - 1;
+            const uint32_t iv = s_exp[255 - s_log[__shfl_sync(0xffffffffu, v, piv)]];
+            R[nsurv][lane] = (uint8_t)mul(v, iv);
+            R[nsurv][kMaxK + lane] = (uint8_t)mul(t, iv);
+            if (lane == 0) {
+                s_piv[warp][nsurv] = (uint8_t)piv;
+                s_surv[warp][nsurv] = (uint8_t)c;
+            }
+            __syncwarp();
+            nsurv++;
+        }
+        int r = 0;
+        for (unsigned long long om = outmask; om && ok; om &= om - 1, r++) {
+            const uint32_t o = (uint32_t)(__ffsll((long long)om) - 1);
+            uint32_t v = lane < k ? grow(o, lane) : 0u, t = 0;
+            for (uint32_t b = 0; b < nsurv; b++) {
+                const uint32_t f = __shfl_sync(0xffffffffu, v, s_piv[warp][b]);
+                if (f) {
+                    v ^= mul(f, R[b][lane]);
+                    t ^= mul(f, R[b][kMaxK + lane]);
+                }
+            }
+            ok = __ballot_sync(0xffffffffu, v != 0) == 0;  // else outside the span of the present rows
+            // (while ok, r < m: rows in the span of fewer than k independent rows are at most l more than them)
+            if (ok && lane < k) pl->coef[r][lane] = (uint8_t)t;
+        }
+        if (lane < nsurv) pl->surv[lane] = s_surv[warp][lane];
+    }
+    if (lane == 0) {
+        int r = 0;
+        if (ok)  // an unrecoverable stripe may have up to k+m-1 absent shards: out_idx holds m
+            for (unsigned long long om = outmask; om; om &= om - 1, r++) pl->out_idx[r] = (uint8_t)(__ffsll((long long)om) - 1);
+        pl->key_present = present;
+        pl->key_out = outmask;
+        pl->nrows = ok ? (uint8_t)nrows : 0;
+        pl->unrecoverable = ok ? 0 : 1;
+        pl->nsurv = (uint8_t)nsurv;
+        if (q.status) q.status[s] = ok ? 0 : -4;
+    }
 }
 
 // ------------------------------------------------------------------ synthetic data

@@ -138,12 +138,13 @@ bool decode_map(const uint8_t *bytes, size_t len, garage_shard_header *h, bool f
             else if (!strcmp(key, "block_len")) h->block_len = (uint32_t)v, seen |= 64;
             else if (!strcmp(key, "shard_len")) h->shard_len = (uint32_t)v, seen |= 128;
             else if (!strcmp(key, "sum_kind")) h->sum_kind = (uint8_t)v, seen |= 256;
+            else if (full && !strcmp(key, "l") && v > 0) h->l = (uint8_t)v, seen |= 512;
             else return false;  // unknown field: not this format
             if (v > 0xffffffffull) return false;
         }
     }
     if (r.n != len) return false;
-    return full ? seen == 511 : seen == 3;
+    return full ? (seen & 511) == 511 : seen == 3;
 }
 
 }  // namespace
@@ -153,9 +154,10 @@ extern "C" {
 size_t garage_shard_wire_encode(const garage_shard_header *h, uint8_t *out, size_t cap)
 {
     if (!h || !out || h->k < 1 || h->index >= h->k + h->m || h->header > 1) return 0;
+    if (h->l && (h->l >= h->m || h->k % h->l)) return 0;
     Writer w{out, cap};
     w.put(GARAGE_SHARD_WIRE_MARKER, 8);
-    w.byte(0x89);  // fixmap, 9 fields, in declaration order like serde
+    w.byte(h->l ? 0x8a : 0x89);  // fixmap, 9 fields (10 with "l"), in declaration order like serde
     w.str("hash");
     w.bin32(h->hash);
     w.str("header");
@@ -174,6 +176,10 @@ size_t garage_shard_wire_encode(const garage_shard_header *h, uint8_t *out, size
     w.uint(h->sum_kind);
     w.str("sum");
     w.bin32(h->sum);
+    if (h->l) {  // skip_serializing_if = 0: RS messages keep their bytes
+        w.str("l");
+        w.uint(h->l);
+    }
     return w.ok ? w.n : 0;
 }
 
@@ -196,7 +202,7 @@ int garage_shard_wire_decode(const uint8_t *bytes, size_t len, garage_shard_head
     memset(&h, 0, sizeof(h));
     // Migrate::decode: the marker and the current format first ...
     if (len > 8 && !memcmp(bytes, GARAGE_SHARD_WIRE_MARKER, 8) && decode_map(bytes + 8, len - 8, &h, true)) {
-        if (h.k < 1 || h.index >= h.k + h.m) return -1;
+        if (h.k < 1 || h.index >= h.k + h.m || (h.l && (h.l >= h.m || h.k % h.l))) return -1;
         *out = h;
         return 0;
     }

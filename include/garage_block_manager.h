@@ -60,6 +60,10 @@ typedef struct {
     int data_fsync;                 /* util/config.rs data_fsync: fsync file + directory before/after the rename  */
     uint32_t block_gc_delay_ms;     /* BLOCK_GC_DELAY (manager.rs:49-52, 10 min): a shard whose block dropped to
                                        rc 0 is deleted by resync only after this delay                            */
+    int local_groups;               /* 0 (default): RS(k, m).  l > 0: LRC(k, l, m - l) (garage_ec_create_lrc): one
+                                       lost shard is resynced from the k/l other shards of its group.  Recorded in
+                                       every shard file header and wire message; a shard of another code is
+                                       quarantined like a k / m mismatch                                          */
 } garage_bm_config;
 
 typedef struct {
@@ -74,6 +78,9 @@ typedef struct {
     uint64_t encode_call_us, reconstruct_call_us; /* wall time spent inside garage_ec_* batch calls */
     uint64_t corrupt_data_errors;            /* GETs whose reassembled block failed the content hash */
     uint64_t write_errors;                   /* shard writes that failed (ENOSPC, EACCES, ...)      */
+    uint64_t resync_shards_read;             /* shards read by resync_block's fetch branch (the read
+                                                set of garage_ec_read_set: k for RS, k/l for an LRC
+                                                local repair)                                       */
 } garage_bm_metrics;
 
 void garage_bm_default_config(garage_bm_config *cfg);
@@ -100,8 +107,8 @@ int garage_bm_block_incref(garage_bm *bm, const uint8_t hash[32]);
 int garage_bm_block_decref(garage_bm *bm, const uint8_t hash[32]);
 long long garage_bm_get_block_rc(garage_bm *bm, const uint8_t hash[32]);
 
-/* resync.rs:354-503 for storage node `node`: fetch branch (rc > 0, shard absent: rebuild it from k
- * survivors) and the deletion half of the offload branch (rc == 0, shard present: delete it).   */
+/* resync.rs:354-503 for storage node `node`: fetch branch (rc > 0, shard absent: rebuild it from the
+ * survivors garage_ec_read_set names -- k for RS, the shard's local group for LRC) and the deletion half of the offload branch (rc == 0, shard present: delete it).   */
 int garage_bm_resync_block(garage_bm *bm, int node, const uint8_t hash[32]);
 /* drain node's resync queue with `workers` concurrent workers (resync.rs:43: up to 8);
  * returns the number of blocks that could not be resynced (they stay queued, with backoff

@@ -55,7 +55,7 @@ extern "C" {
 #define GARAGE_EC_E_INVALID (-1)       /* bad argument / geometry */
 #define GARAGE_EC_E_CUDA (-2)          /* CUDA runtime error, see garage_ec_last_error */
 #define GARAGE_EC_E_NOMEM (-3)         /* host or device allocation failed */
-#define GARAGE_EC_E_UNRECOVERABLE (-4) /* >= 1 stripe had < k shards; see status[] */
+#define GARAGE_EC_E_UNRECOVERABLE (-4) /* >= 1 stripe could not be rebuilt; see status[] */
 #define GARAGE_EC_E_NODEVICE (-5)      /* no CUDA device / wrong architecture */
 #define GARAGE_EC_E_ALIGN (-6)         /* pointer or stride alignment violated */
 
@@ -82,10 +82,27 @@ int garage_ec_create(garage_ec_ctx **out, int cuda_device, int k, int m, int mat
  * the NCCL broadcast of rank 0's matrix (SURVEY.md section 8(e)).                          */
 int garage_ec_create_with_matrix(garage_ec_ctx **out, int cuda_device, int k, int m,
                                  const uint8_t *parity_rows);
+/* Locally repairable code LRC(k, l, r): m = l + r parity shards.  The k data shards form l groups of k/l;
+ * parity k+g (g < l) is the XOR of group g, parities k+l.. are the r Cauchy rows of RS(k, r)
+ * (P[i][j] = 1/((k+i) xor j)).  One lost shard of a group is rebuilt from the other k/l shards of the
+ * group instead of from k shards.  Needs l >= 1, r >= 1, k % l == 0, l + r <= GARAGE_EC_MAX_M,
+ * k <= GARAGE_EC_MAX_K; GARAGE_EC_E_INVALID otherwise, before any CUDA call.  Encode / verify /
+ * reconstruct / scrub_repair / *_blocks work unchanged; reconstruct decides recoverability by rank
+ * (DESIGN.md section 2), so some patterns with fewer than k present shards decode.                   */
+int garage_ec_create_lrc(garage_ec_ctx **out, int cuda_device, int k, int l, int r);
 void garage_ec_destroy(garage_ec_ctx *ctx);
 
 int garage_ec_matrix(const garage_ec_ctx *ctx, uint8_t *out_m_by_k); /* parity rows, row-major */
 int garage_ec_params(const garage_ec_ctx *ctx, int *k, int *m, int *cuda_device);
+/* LRC contexts: (l, r); RS contexts: (0, m).  garage_ec_matrix returns the l local rows, then the r global rows. */
+int garage_ec_code_info(const garage_ec_ctx *ctx, int *local_groups, int *global_parity);
+/* Which shards a gatherer should fetch to rebuild the wanted absent shards of ONE stripe (host only, no GPU
+ * work): read_out[i] = 1 iff reconstruct reads shard i.  present / want / read_out: k+m bytes; want NULL =
+ * every absent shard.  RS: the first k present shards.  LRC: the other members of each wanted shard's
+ * local group when every wanted shard is the only absent member of its group, else a rank basis of the
+ * present shards taken greedily in index order (DESIGN.md section 2).  GARAGE_EC_E_UNRECOVERABLE if a
+ * wanted shard cannot be rebuilt.  Presenting only these shards to reconstruct rebuilds the same bytes. */
+int garage_ec_read_set(const garage_ec_ctx *ctx, const uint8_t *present, const uint8_t *want, uint8_t *read_out);
 const char *garage_ec_strerror(int code);
 /* detail of the last GARAGE_EC_E_CUDA on this context (thread-unsafe snapshot; "" if none) */
 const char *garage_ec_last_error(const garage_ec_ctx *ctx);
@@ -112,8 +129,10 @@ int garage_ec_encode(garage_ec_ctx *ctx, const uint8_t *data, uint8_t *parity,
  *   present : n * (k+m) bytes in {0,1}
  *   want    : NULL = rebuild every absent shard; else n*(k+m) bytes, only absent shards
  *             with want != 0 are rebuilt (GET wants data shards only; resync wants one)
- *   status  : n int32: 0 ok, GARAGE_EC_E_UNRECOVERABLE if < k present (stripe untouched)
- * Survivors used: the first k present shards in index order.  HOST calls return
+ *   status  : n int32: 0 ok, GARAGE_EC_E_UNRECOVERABLE if a wanted shard cannot be rebuilt (RS: < k
+ *             present; stripe untouched)
+ * Survivors used: those of garage_ec_read_set (RS: the first k present shards in index order); only
+ * they are read, and HOST calls copy only them to the GPU.  HOST calls return
  * GARAGE_EC_E_UNRECOVERABLE if any stripe was; DEVICE calls only fill status[].            */
 int garage_ec_reconstruct(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *present,
                           const uint8_t *want, int32_t *status, const uint32_t *shard_len,

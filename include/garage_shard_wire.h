@@ -12,7 +12,9 @@
  *
  *   v1 (erasure coded)  marker "GEC1shdr" + msgpack map
  *        { "hash": bin32, "header": "Plain" | "Compressed", "k": uint, "m": uint, "index": uint,
- *          "block_len": uint, "shard_len": uint, "sum_kind": uint, "sum": bin32 }
+ *          "block_len": uint, "shard_len": uint, "sum_kind": uint, "sum": bin32[, "l": uint] }
+ *        "l" (LRC local groups, garage_ec_create_lrc) is present only for an LRC code (l > 0), so RS
+ *        messages are byte for byte what they were before it existed.
  *   v0 (Previous)       the reference's replicated PutBlock payload, no marker:
  *        { "hash": bin32, "header": "Plain" | "Compressed" }
  *        migrate(v0) = the whole block as the only shard of a (k = 1, m = 0) code, index 0,
@@ -45,6 +47,7 @@ typedef struct {
     uint32_t block_len; /* unpadded length of the whole block                                     */
     uint32_t shard_len; /* ceil(block_len / k)                                                    */
     uint8_t sum[32];    /* integrity tag of this shard's bytes                                    */
+    uint8_t l;          /* LRC local groups (0 < l < m, k % l == 0); 0 = RS                        */
 } garage_shard_header;
 
 /* returns the encoded length, or 0 if `cap` is too small / the header is invalid (<= 160 bytes)   */

@@ -24,9 +24,15 @@ extern "C" {
                             matrix_kind: c_int) -> c_int;
     pub fn garage_ec_create_with_matrix(out: *mut *mut garage_ec_ctx, cuda_device: c_int, k: c_int,
                             m: c_int, parity_rows: *const u8) -> c_int;
+    pub fn garage_ec_create_lrc(out: *mut *mut garage_ec_ctx, cuda_device: c_int, k: c_int, l: c_int,
+                            r: c_int) -> c_int;
     pub fn garage_ec_destroy(ctx: *mut garage_ec_ctx);
     pub fn garage_ec_matrix(ctx: *const garage_ec_ctx, out_m_by_k: *mut u8) -> c_int;
     pub fn garage_ec_params(ctx: *const garage_ec_ctx, k: *mut c_int, m: *mut c_int, dev: *mut c_int) -> c_int;
+    pub fn garage_ec_code_info(ctx: *const garage_ec_ctx, local_groups: *mut c_int,
+                            global_parity: *mut c_int) -> c_int;
+    pub fn garage_ec_read_set(ctx: *const garage_ec_ctx, present: *const u8, want: *const u8,
+                            read_out: *mut u8) -> c_int;
     pub fn garage_ec_strerror(code: c_int) -> *const c_char;
     pub fn garage_ec_last_error(ctx: *const garage_ec_ctx) -> *const c_char;
     pub fn garage_ec_abi_version() -> c_int;

@@ -3,6 +3,9 @@
 of one .so variant on the BASELINE config-2/3 workload.  Not the contract bench (bench.py).
 
     python tools/kbench.py [--so path/to/libgarage_ec.so] [--k 10 --m 4 --blocks 4096 --iters 10]
+    python tools/kbench.py --k 10 --lrc 2 --m 4              # LRC(10,2,2): l = 2 local groups, m = l + r
+    python tools/kbench.py --k 10 --lrc 2 --m 4 --erasures 1 --local   # one lost data / local-parity shard
+Reconstruct bytes are (survivors read + shards rebuilt) x shard_len, the survivors being garage_ec_read_set's.
 """
 import argparse
 import json
@@ -20,6 +23,8 @@ ap.add_argument("--blocks", type=int, default=4096)
 ap.add_argument("--iters", type=int, default=10)
 ap.add_argument("--erasures", type=int, default=None)
 ap.add_argument("--same-pattern", action="store_true", help="all stripes lose the same shards")
+ap.add_argument("--lrc", type=int, default=0, help="LRC with this many local groups (m = local + global parities)")
+ap.add_argument("--local", action="store_true", help="erase only data / local-parity shards (LRC local repair)")
 ap.add_argument("--tag", default="")
 ap.add_argument("--stride-pad", type=int, default=0, help="extra bytes between shards (multiple of 16)")
 args = ap.parse_args()
@@ -37,7 +42,7 @@ k, m, n = args.k, args.m, args.blocks
 tot = k + m
 e = args.erasures if args.erasures is not None else m
 B = 1 << 20
-ec = G.GarageEc(0, k, m)
+ec = G.GarageEc.lrc(0, k, args.lrc, m - args.lrc) if args.lrc else G.GarageEc(0, k, m)
 L = ec.shard_len(B)
 stride = ec.stride_for(L) + args.stride_pad
 shards = torch.zeros(n * tot * stride, dtype=torch.uint8, device="cuda")
@@ -52,10 +57,11 @@ sh3[:, :k] = data.view(n, k, stride)
 sh3[:, k:] = parity.view(n, m, stride)
 orig = shards.clone()
 g = torch.Generator().manual_seed(7)
+span = k + args.lrc if args.local else tot  # --local: erase among the data and local-parity shards
 if args.same_pattern:
     erased = torch.arange(e).repeat(n, 1)
 else:
-    erased = torch.rand(n, tot, generator=g).argsort(dim=1)[:, :e]
+    erased = torch.rand(n, span, generator=g).argsort(dim=1)[:, :e]
 present = torch.ones(n, tot, dtype=torch.uint8)
 if e:
     present.scatter_(1, erased, 0)
@@ -101,12 +107,29 @@ def copy_gbs():
     return 2 * cp_n / (best * 1e-3) / 1e9
 
 
+def power_limit():
+    import subprocess
+
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", "0"],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        return float(out.splitlines()[0])
+    except Exception:
+        return None
+
+
 peak = copy_gbs()
 enc_b = n * (k + m) * L
-dec_b = n * (k + e) * L
+pres_np = present.numpy()
+nsurv = 0
+for s in range(n):
+    rs = ec.read_set(pres_np[s])
+    nsurv += int(rs.sum()) if rs is not None else 0
+dec_b = (nsurv + n * e) * L
 print(json.dumps({
-    "tag": args.tag or (args.so or "default"), "k": k, "m": m, "blocks": n, "erasures": e, "ok": bool(ok),
-    "copy_GBs": round(peak, 1), "gpu": torch.cuda.get_device_name(0),
+    "tag": args.tag or (args.so or "default"), "k": k, "m": m, "lrc_local_groups": args.lrc, "blocks": n, "erasures": e,
+    "local": bool(args.local), "survivors_per_stripe": round(nsurv / n, 3), "ok": bool(ok),
+    "copy_GBs": round(peak, 1), "gpu": torch.cuda.get_device_name(0), "power_limit_W": power_limit(),
     "encode_ms": round(t_enc, 4), "encode_GBs": round(enc_b / t_enc / 1e6, 1), "encode_frac": round(enc_b / t_enc / 1e6 / peak, 4),
     "decode_ms": round(t_dec, 4), "decode_GBs": round(dec_b / t_dec / 1e6, 1), "decode_frac": round(dec_b / t_dec / 1e6 / peak, 4),
     "verify_ms": round(t_ver, 4), "verify_GBs": round(enc_b / t_ver / 1e6, 1), "verify_frac": round(enc_b / t_ver / 1e6 / peak, 4),
