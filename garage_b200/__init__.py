@@ -37,6 +37,8 @@ ABI_SYMBOLS = [
     "garage_ec_numa_info", "garage_ec_bind_thread", "garage_ec_debug_fail_after",
     "garage_ec_set_sum_kind", "garage_ec_set_wait_mode", "garage_ec_copy_for_dma", "garage_ec_shard_sum_host", "garage_ec_reconstruct_stripes",
     "garage_ec_create_lrc", "garage_ec_code_info", "garage_ec_read_set",
+    "garage_ec_create_piggyback", "garage_ec_piggyback_info", "garage_ec_code_shard_len", "garage_ec_read_plan",
+    "garage_ec_check_shard_half_host",
 ]
 
 
@@ -116,6 +118,11 @@ def load_library(build=True):
     L.garage_ec_create_lrc.argtypes = [C.POINTER(vp), i32, i32, i32, i32]
     L.garage_ec_code_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32)]
     L.garage_ec_read_set.argtypes = [vp, vp, vp, vp]
+    L.garage_ec_create_piggyback.argtypes = [C.POINTER(vp), i32, i32, i32, i32]
+    L.garage_ec_piggyback_info.argtypes = [vp, C.POINTER(i32), vp]
+    L.garage_ec_code_shard_len.argtypes = [vp, u32, C.POINTER(u32)]
+    L.garage_ec_read_plan.argtypes = [vp, vp, vp, vp]
+    L.garage_ec_check_shard_half_host.argtypes = [i32, vp, u32, i32, vp]
     _lib = L
     return L
 
@@ -141,6 +148,16 @@ def shard_sum_host(kind, data) -> bytes:
     if rc:
         raise EcError(rc, "shard_sum_host")
     return out.tobytes()
+
+
+def check_shard_half_host(kind, half, shard_len, which, tag) -> int:
+    """garage_ec_check_shard_half_host: 0 if `half` (shard_len/2 bytes, which = 0 a-half / 1 b-half) matches its 4
+    Adler-32 values in the 32-byte adler8 tag `tag`, 1 if not, or an E_* code"""
+    L = load_library()
+    a = np.frombuffer(bytes(half), dtype=np.uint8) if not isinstance(half, np.ndarray) else np.ascontiguousarray(half)
+    t = np.frombuffer(bytes(tag), dtype=np.uint8)
+    return L.garage_ec_check_shard_half_host(kind, C.c_void_p(a.ctypes.data) if a.size else None, shard_len, which,
+                                             C.c_void_p(t.ctypes.data))
 
 
 def copy_for_dma(dst, src):
@@ -173,10 +190,12 @@ class GarageEc:
     or numpy uint8 arrays (HOST mode: synchronous, staged through the library's lanes).
     """
 
-    def __init__(self, device=0, k=10, m=4, kind=VANDERMONDE, matrix=None, _lrc=None):
+    def __init__(self, device=0, k=10, m=4, kind=VANDERMONDE, matrix=None, _lrc=None, _pb=False):
         self._L = load_library()
         h = C.c_void_p()
-        if _lrc is not None:
+        if _pb:
+            rc = self._L.garage_ec_create_piggyback(C.byref(h), device, k, m, kind)
+        elif _lrc is not None:
             l, r = _lrc
             m = l + r
             rc = self._L.garage_ec_create_lrc(C.byref(h), device, k, l, r)
@@ -196,6 +215,11 @@ class GarageEc:
     def lrc(cls, device=0, k=10, l=2, r=2):
         """LRC(k, l, r) context: l local XOR parities (one per group of k/l data shards), then r Cauchy parities"""
         return cls(device, k, l + r, _lrc=(l, r))
+
+    @classmethod
+    def piggyback(cls, device=0, k=10, m=4, kind=VANDERMONDE):
+        """PB(k, m) context: RS(k, m) over two half-shards, b-halves of parities 1..m-1 carry the group XORs of a"""
+        return cls(device, k, m, kind, _pb=True)
 
     # -- lifecycle
     def close(self):
@@ -251,6 +275,28 @@ class GarageEc:
         out = np.zeros(self.k + self.m, dtype=np.uint8)
         rc = self._check(self._L.garage_ec_read_set(self._h, _ptr(pr), _ptr(wn), _ptr(out)), (E_UNRECOVERABLE,))
         return None if rc == E_UNRECOVERABLE else out
+
+    def piggyback_info(self):
+        """(groups, group_of): m-1 and the group (1..m-1) of every data shard for PB, (0, zeros) otherwise"""
+        g = C.c_int(0)
+        out = np.zeros(self.k, dtype=np.uint8)
+        self._check(self._L.garage_ec_piggyback_info(self._h, C.byref(g), _ptr(out)))
+        return g.value, out
+
+    def read_plan(self, present, want=None):
+        """halves to fetch per shard (bit 0 a-half, bit 1 b-half): (k+m,) uint8 array, or None if unrecoverable"""
+        pr = np.ascontiguousarray(present, dtype=np.uint8)
+        wn = None if want is None else np.ascontiguousarray(want, dtype=np.uint8)
+        assert pr.shape == (self.k + self.m,) and (wn is None or wn.shape == pr.shape)
+        out = np.zeros(self.k + self.m, dtype=np.uint8)
+        rc = self._check(self._L.garage_ec_read_plan(self._h, _ptr(pr), _ptr(wn), _ptr(out)), (E_UNRECOVERABLE,))
+        return None if rc == E_UNRECOVERABLE else out
+
+    def code_shard_len(self, block_len):
+        """shard length of a block under this context's code (PB: rounded up to 128 bytes)"""
+        v = C.c_uint32(0)
+        self._check(self._L.garage_ec_code_shard_len(self._h, block_len, C.byref(v)))
+        return v.value
 
     def shard_len(self, block_len):
         return int(self._L.garage_ec_shard_len(block_len, self.k))

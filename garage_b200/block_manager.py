@@ -27,7 +27,7 @@ class Config(C.Structure):
                 ("n_nodes", C.c_int), ("block_size", C.c_uint32), ("block_ram_buffer_max", C.c_uint64),
                 ("batch_max_blocks", C.c_uint32), ("batch_linger_us", C.c_uint32), ("data_dir", C.c_char_p),
                 ("shard_sum_kind", C.c_int), ("verify_content_hash", C.c_int), ("data_fsync", C.c_int),
-                ("block_gc_delay_ms", C.c_uint32), ("local_groups", C.c_int)]
+                ("block_gc_delay_ms", C.c_uint32), ("local_groups", C.c_int), ("piggyback", C.c_int)]
 
 
 class Metrics(C.Structure):
@@ -35,7 +35,7 @@ class Metrics(C.Structure):
         "bytes_written", "bytes_read", "corruption_counter", "resync_counter", "resync_error_counter",
         "resync_recv_counter", "delete_counter", "put_calls", "put_batches", "reconstruct_calls",
         "reconstruct_batches", "scrub_shards_checked", "scrub_corruptions", "resync_queue_length",
-        "encode_call_us", "reconstruct_call_us", "corrupt_data_errors", "write_errors", "resync_shards_read")]
+        "encode_call_us", "reconstruct_call_us", "corrupt_data_errors", "write_errors", "resync_shards_read", "resync_bytes_read")]
 
 
 _lib = None
@@ -99,9 +99,10 @@ class BlockManager:
 
     def __init__(self, k=10, m=4, n_nodes=None, cuda_device=0, batch_max_blocks=64, batch_linger_us=100,
                  block_ram_buffer_max=256 << 20, data_dir=None, shard_sum_kind=SUM_ADLER8, verify_content_hash=True,
-                 data_fsync=False, block_gc_delay_ms=0, local_groups=0):
+                 data_fsync=False, block_gc_delay_ms=0, local_groups=0, piggyback=False):
         """block_gc_delay_ms defaults to 0 HERE (tests delete at once); the library's default is the
-        reference's BLOCK_GC_DELAY of 10 minutes.  local_groups > 0: LRC(k, local_groups, m - local_groups)."""
+        reference's BLOCK_GC_DELAY of 10 minutes.  local_groups > 0: LRC(k, local_groups, m - local_groups).
+        piggyback: PB(k, m), half-shard repair reads."""
         self._L = load_library()
         cfg = Config()
         self._L.garage_bm_default_config(C.byref(cfg))
@@ -112,6 +113,7 @@ class BlockManager:
         cfg.shard_sum_kind, cfg.verify_content_hash = shard_sum_kind, 1 if verify_content_hash else 0
         cfg.data_fsync, cfg.block_gc_delay_ms = 1 if data_fsync else 0, block_gc_delay_ms
         cfg.local_groups = local_groups
+        cfg.piggyback = 1 if piggyback else 0
         self._dir = data_dir.encode() if data_dir else None  # keep the bytes alive
         cfg.data_dir = self._dir
         h = C.c_void_p()
@@ -228,7 +230,8 @@ class BlockManager:
 class ShardHeader(C.Structure):
     _fields_ = [("hash", C.c_uint8 * 32), ("header", C.c_uint8), ("k", C.c_uint8), ("m", C.c_uint8),
                 ("index", C.c_uint8), ("sum_kind", C.c_uint8), ("migrated", C.c_uint8),
-                ("block_len", C.c_uint32), ("shard_len", C.c_uint32), ("sum", C.c_uint8 * 32), ("l", C.c_uint8)]
+                ("block_len", C.c_uint32), ("shard_len", C.c_uint32), ("sum", C.c_uint8 * 32), ("l", C.c_uint8),
+                ("pb", C.c_uint8)]
 
     def as_dict(self):
         d = {"hash": bytes(self.hash), "header": int(self.header), "k": int(self.k), "m": int(self.m),
@@ -236,6 +239,8 @@ class ShardHeader(C.Structure):
              "block_len": int(self.block_len), "shard_len": int(self.shard_len), "sum": bytes(self.sum)}
         if self.l:  # like the wire: only LRC shards carry it
             d["l"] = int(self.l)
+        if self.pb:  # only PB shards carry it
+            d["pb"] = int(self.pb)
         return d
 
 
@@ -252,12 +257,12 @@ def _wire():
     return L
 
 
-def wire_encode(hash32, header, k, m, index, block_len, shard_len, sum_kind, sum32, l=0) -> bytes:
+def wire_encode(hash32, header, k, m, index, block_len, shard_len, sum_kind, sum32, l=0, pb=0) -> bytes:
     h = ShardHeader()
     C.memmove(h.hash, bytes(hash32), 32)
     C.memmove(h.sum, bytes(sum32), 32)
     h.header, h.k, h.m, h.index, h.sum_kind = header, k, m, index, sum_kind
-    h.block_len, h.shard_len, h.l = block_len, shard_len, l
+    h.block_len, h.shard_len, h.l, h.pb = block_len, shard_len, l, pb
     buf = (C.c_uint8 * 256)()
     n = _wire().garage_shard_wire_encode(C.byref(h), buf, 256)
     return bytes(buf[:n])

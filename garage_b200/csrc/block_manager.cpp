@@ -243,8 +243,9 @@ struct ShardFileHeader {
     uint32_t shard_len;
     uint8_t sum[32];
     uint32_t hdr_check;  // Adler-32 of bytes [0, 48)
-    uint8_t pad[12];     // pad[0]: LRC local groups (0 = RS, so files written before it existed read as RS); outside
-                         // hdr_check, so the reader compares it with its own code and quarantines a mismatch
+    uint8_t pad[12];     // pad[0]: LRC local groups (0 = RS, so files written before it existed read as RS); pad[1]: 1 =
+                         // piggybacked RS PB(k, m) (0 = not PB).  Outside hdr_check, so the reader compares them with
+                         // its own code and quarantines a mismatch
 };
 static_assert(sizeof(ShardFileHeader) == 64, "shard file header is 64 bytes");
 
@@ -267,6 +268,7 @@ struct Node {
     bool fsync_data = false;  // data_fsync (util/config.rs), manager.rs:775-789
     std::string dir;          // empty: in-memory store
     int k = 0, m = 0, l = 0;  // l: LRC local groups, 0 = RS
+    bool pb = false;          // piggybacked RS PB(k, m): shard_len = ceil(block_len / k) rounded up to 128
     // in-memory mode: immutable shards behind shared pointers, so the node lock only covers the map operation -- the
     // 100 KB copies happen outside it (the reference shards its lock 256 ways per node, manager.rs:114,679-689; with
     // one lock per node and the copies inside it, 128 clients serialised on 14 mutexes at ~12 GiB/s)
@@ -289,7 +291,8 @@ struct Node {
     bool meta_valid(const ShardMeta &mt) const
     {
         if (mt.index < 0 || mt.index >= k + m) return false;
-        return mt.shard_len == (uint32_t)(((uint64_t)mt.block_len + (unsigned)k - 1) / (unsigned)k);
+        const uint64_t L = ((uint64_t)mt.block_len + (unsigned)k - 1) / (unsigned)k;
+        return mt.shard_len == (pb ? (L + 127) / 128 * 128 : L);
     }
     // all store_* are called with `mu` held
     bool store_put(const Hash &h, const ShardMeta &mt, const uint8_t *bytes, size_t n)
@@ -317,6 +320,7 @@ struct Node {
         memcpy(hd.sum, mt.sum.data(), 32);
         hd.hdr_check = adler32_small(reinterpret_cast<const uint8_t *>(&hd), 48);
         hd.pad[0] = (uint8_t)l;
+        hd.pad[1] = pb ? 1 : 0;
         FILE *f = fopen(tmp.c_str(), "wb");
         if (!f) return false;
         bool ok = fwrite(&hd, sizeof(hd), 1, f) == 1 && (n == 0 || fwrite(bytes, n, 1, f) == 1);
@@ -334,13 +338,15 @@ struct Node {
         if (!ok) ::remove(tmp.c_str());
         return ok;
     }
-    // shard bytes straight into `dst` (cap bytes available), metadata into `mt`
-    ReadResult store_read_into(const Hash &h, uint8_t *dst, size_t cap, ShardMeta &mt) const
+    // shard bytes straight into `dst` (cap bytes available), metadata into `mt`.  half = 0 / 1: only the a- / b-half
+    // [half * shard_len/2, (half+1) * shard_len/2) of a PB shard, one ranged read at 64 + half * shard_len/2 of the
+    // file, into dst (which then holds shard_len/2 bytes)
+    ReadResult store_read_into(const Hash &h, uint8_t *dst, size_t cap, ShardMeta &mt, int half = -1) const
     {
         if (dir.empty()) {
             auto it = shards.find(h);
             if (it == shards.end()) return kReadMissing;
-            return copy_out(*it->second, dst, cap, mt);
+            return copy_out(*it->second, dst, cap, mt, false, half);
         }
         FILE *f = fopen(path_of(h, ".shard").c_str(), "rb");  // find_block (manager.rs:627-662)
         if (!f) return kReadMissing;
@@ -351,24 +357,34 @@ struct Node {
         // what it claims (a flipped shard_len must not become a 4 GiB resize)
         if (fread(&hd, sizeof(hd), 1, f) == 1 && memcmp(hd.magic, "GEC1", 4) == 0 &&
             hd.hdr_check == adler32_small(reinterpret_cast<const uint8_t *>(&hd), 48) && hd.k == k && hd.m == m &&
-            hd.pad[0] == l && fstat(fileno(f), &sb) == 0 && (uint64_t)sb.st_size == (uint64_t)hd.shard_len + sizeof(hd)) {
+            hd.pad[0] == l && hd.pad[1] == (pb ? 1 : 0) && fstat(fileno(f), &sb) == 0 &&
+            (uint64_t)sb.st_size == (uint64_t)hd.shard_len + sizeof(hd)) {
             mt.index = hd.index;
             mt.block_len = hd.block_len;
             mt.shard_len = hd.shard_len;
             mt.sum_kind = hd.sum_kind;
             memcpy(mt.sum.data(), hd.sum, 32);
-            if (meta_valid(mt) && mt.shard_len <= cap && (mt.shard_len == 0 || fread(dst, mt.shard_len, 1, f) == 1))
-                r = kReadOk;
+            if (half < 0) {
+                if (meta_valid(mt) && mt.shard_len <= cap && (mt.shard_len == 0 || fread(dst, mt.shard_len, 1, f) == 1))
+                    r = kReadOk;
+            } else {
+                const size_t hl = mt.shard_len / 2;
+                if (pb && meta_valid(mt) && hl <= cap &&
+                    (hl == 0 || ::pread(fileno(f), dst, hl, (off_t)(sizeof(hd) + (size_t)half * hl)) == (ssize_t)hl))
+                    r = kReadOk;
+            }
         }
         fclose(f);
         return r;
     }
-    ReadResult copy_out(const StoredShard &sh, uint8_t *dst, size_t cap, ShardMeta &mt, bool for_dma = false) const
+    ReadResult copy_out(const StoredShard &sh, uint8_t *dst, size_t cap, ShardMeta &mt, bool for_dma = false,
+                        int half = -1) const
     {
         mt = sh;
-        if (!meta_valid(mt) || sh.bytes.size() != mt.shard_len || mt.shard_len > cap) return kReadInvalid;
-        if (for_dma) copy_for_dma(dst, sh.bytes.data(), mt.shard_len);
-        else if (mt.shard_len) memcpy(dst, sh.bytes.data(), mt.shard_len);
+        const size_t off = half < 0 ? 0 : (size_t)half * (mt.shard_len / 2), n = half < 0 ? mt.shard_len : mt.shard_len / 2;
+        if (!meta_valid(mt) || sh.bytes.size() != mt.shard_len || n > cap || (half >= 0 && !pb)) return kReadInvalid;
+        if (for_dma) copy_for_dma(dst, sh.bytes.data() + off, n);
+        else if (n) memcpy(dst, sh.bytes.data() + off, n);
         return kReadOk;
     }
     bool store_get(const Hash &h, StoredShard &out) const  // a copy (scrub snapshots, inspection)
@@ -738,10 +754,15 @@ struct garage_bm {
     std::atomic<uint64_t> bytes_written{0}, bytes_read{0}, corruption_counter{0}, resync_counter{0},
         resync_error_counter{0}, resync_recv_counter{0}, delete_counter{0}, put_calls{0}, reconstruct_calls{0},
         scrub_checked{0}, scrub_corrupt{0}, enc_gpu_us{0}, rec_gpu_us{0}, corrupt_data_errors{0}, write_errors{0},
-        resync_shards_read{0};
+        resync_shards_read{0}, resync_bytes_read{0};
     std::atomic<uint64_t> put_ns_slot{0}, put_ns_land{0}, put_ns_wait{0}, put_ns_store{0};
 
-    size_t shard_len_of(uint32_t block_len) const { return garage_ec_shard_len(block_len, k); }
+    bool pb = false;  // PB(k, m) contexts (garage_bm_config.piggyback)
+    size_t shard_len_of(uint32_t block_len) const
+    {
+        uint32_t L = 0;  // a length that does not fit in 32 bits is larger than any slot: every caller rejects it
+        return garage_ec_code_shard_len(ec, block_len, &L) == GARAGE_EC_OK ? L : SIZE_MAX;
+    }
 
     // rpc/layout/version.rs:117-137: top 8 bits of the hash -> partition -> k+m distinct nodes, shard i on the
     // i-th of them.  The ring is a garage_layout (row f4, include/garage_placement.h) filled at create with
@@ -847,6 +868,34 @@ struct garage_bm {
         quarantine(node, h);
         return false;
     }
+    // PB: one half of a shard (a ranged read of shard_len/2 bytes into dst), checked against the half's 4 adler8
+    // segment tags (garage_ec_check_shard_half_host); a bad header or tag quarantines the shard like a whole read
+    bool read_half_into(int node, const Hash &h, int half, uint8_t *dst, size_t cap, ShardMeta &mt, bool for_dma = false)
+    {
+        Node &nd = *nodes[node];
+        ReadResult r;
+        Node::ShardPtr sp;
+        if (nd.dir.empty()) {
+            {
+                std::lock_guard<std::mutex> lk(nd.mu);
+                if (!nd.up) return false;
+                sp = nd.store_find(h);
+            }
+            r = sp ? nd.copy_out(*sp, dst, cap, mt, for_dma, half) : kReadMissing;
+        } else {
+            std::lock_guard<std::mutex> lk(nd.mu);
+            if (!nd.up) return false;
+            r = nd.store_read_into(h, dst, cap, mt, half);
+        }
+        if (r == kReadMissing) return false;
+        if (r == kReadOk) {
+            bytes_read += mt.shard_len / 2;
+            if (garage_ec_check_shard_half_host(mt.sum_kind, dst, mt.shard_len, half, mt.sum.data()) == GARAGE_EC_OK)
+                return true;
+        }
+        quarantine(node, h);
+        return false;
+    }
 
     // ---- batch runners (dispatcher threads) -------------------------------------------------
     void run_encode(int w, std::vector<EncodeItem *> &b)
@@ -860,7 +909,7 @@ struct garage_bm {
             lens[i] = b[i]->len;
             max_len = std::max(max_len, b[i]->len);
         }
-        const size_t stride = garage_ec_stride_for(garage_ec_shard_len(max_len, k));
+        const size_t stride = garage_ec_stride_for((uint32_t)shard_len_of(max_len));
         EncBatchBuf &bb = enc_out[w][enc_next[w] = (enc_next[w] + 1) % kEncBufs];
         bb.wait_idle();  // the callers of the batch that last used this buffer have stored their shards
         uint8_t *par = bb.get(n * m * stride + n * tot * 32);
@@ -913,12 +962,14 @@ struct garage_bm {
     // GPU), then the survivors garage_ec_read_set names for the missing data shards -- for RS the first
     // parity shards up to k; the reference likewise stops at the first good copy (manager.rs:292-334).
     // Resync (want_in = this node's shard): exactly the read set, k/l shards for an LRC local repair.
+    // PB: the halves garage_ec_read_plan names (a half at slot + i*slot_stride + half*shard_len/2, one ranged read
+    // each, checked against its 4 adler8 segment tags), k + |G_i| halves for one lost data shard.
     // A shard that cannot be read is taken out of the assumed-present set and the read set recomputed.
     // A shard whose header disagrees with the others on the block length, or that sits under the
     // wrong index, is treated like a corrupt one.  `all`: read every shard (corruption hunting).
-    // Returns the number of shards read; *ok = the wanted shards can be rebuilt from `have`.
+    // Returns the number of shards read (*bytes_out += the bytes); *ok = the wanted shards can be rebuilt from `have`.
     int gather_into(const Hash &h, int skip_node, uint8_t *slot, uint8_t *have, uint32_t &block_len, bool all = false,
-                    bool for_gpu = false, const uint8_t *want_in = nullptr, bool *ok = nullptr)
+                    bool for_gpu = false, const uint8_t *want_in = nullptr, bool *ok = nullptr, uint64_t *bytes_out = nullptr)
     {
         int who[64];
         storage_nodes_of(h, who);
@@ -934,20 +985,45 @@ struct garage_bm {
             }
         }
         int count = 0;
-        auto try_shard = [&](int i) {
-            if (who[i] == skip_node || have[i]) return;
+        uint64_t nbytes = 0;
+        uint8_t have_h[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};  // halves held: bit 0 a, bit 1 b (3 = whole shard)
+        // whole shard (half < 0) or one half of it
+        auto try_shard = [&](int i, int half = -1) {
+            if (who[i] == skip_node || have_h[i] == 3) return;
             ShardMeta mt;
-            if (!read_shard_into(who[i], h, slot + (size_t)i * slot_stride, slot_stride, mt, for_gpu)) return;
+            uint8_t *dst = slot + (size_t)i * slot_stride;
+            bool got;
+            if (half < 0) {
+                got = read_shard_into(who[i], h, dst, slot_stride, mt, for_gpu);
+            } else {
+                const size_t hl = (have_expect ? shard_len_of(expect) : slot_stride) / 2;  // placement of the b-half
+                got = read_half_into(who[i], h, half, dst + (size_t)half * hl, slot_stride - (size_t)half * hl, mt, for_gpu);
+                if (got && !have_expect && half == 1 && mt.shard_len / 2 != hl)  // first read of the block: move it
+                    memmove(dst + mt.shard_len / 2, dst + hl, mt.shard_len / 2);
+            }
+            if (!got) {
+                if (have_h[i]) {  // the other half came from a shard that turned out bad: drop the shard
+                    have_h[i] = 0;
+                    have[i] = 0;
+                    count--;
+                }
+                return;
+            }
             if (mt.index != i || (have_expect && mt.block_len != expect)) {
                 quarantine(who[i], h);  // a stale or misplaced shard with a self-consistent tag
+                if (have_h[i]) count--;
+                have_h[i] = 0;
+                have[i] = 0;
                 return;
             }
             if (!have_expect) {
                 expect = mt.block_len;
                 have_expect = true;
             }
+            nbytes += half < 0 ? mt.shard_len : mt.shard_len / 2;
+            if (!have_h[i]) count++;
+            have_h[i] |= half < 0 ? 3 : (uint8_t)(1 << half);
             have[i] = 1;
-            count++;
         };
         uint8_t tried[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0}, want[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
         auto attempt = [&](int i) {
@@ -967,16 +1043,27 @@ struct garage_bm {
                 }
             }
             for (;;) {
-                // assume every shard not yet tried on an up node is there; fetch what the read set still lacks
+                // assume every shard not yet tried on an up node is there; fetch what the read plan still lacks
+                // (RS / LRC: whole shards of the read set; PB: the planned halves)
                 uint8_t guess[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M], rd[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
                 for (int i = 0; i < tot; i++) guess[i] = have[i] || (!tried[i] && who[i] != skip_node);
-                if (garage_ec_read_set(ec, guess, want, rd) != GARAGE_EC_OK) break;
+                if (garage_ec_read_plan(ec, guess, want, rd) != GARAGE_EC_OK) break;
                 bool fetched = false, missing = false;
                 for (int i = 0; i < tot; i++) {
-                    if (!rd[i] || have[i]) continue;
+                    const int need = rd[i] & ~have_h[i];
+                    if (!need) continue;
                     missing = true;
-                    attempt(i);
                     fetched = true;
+                    if (!pb || (need == 3 && !have_h[i])) {
+                        attempt(i);
+                    } else {
+                        tried[i] = 1;
+                        for (int half = 0; half < 2; half++) {
+                            if (!((need >> half) & 1)) continue;
+                            try_shard(i, half);
+                            if (!((have_h[i] >> half) & 1)) break;  // unreadable: the shard is out, re-plan
+                        }
+                    }
                 }
                 if (!missing || !fetched) break;
             }
@@ -985,8 +1072,10 @@ struct garage_bm {
             uint8_t rd[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
             if (all)
                 for (int i = 0; i < k; i++) want[i] = !have[i];
-            *ok = garage_ec_read_set(ec, have, want, rd) == GARAGE_EC_OK;
+            *ok = garage_ec_read_plan(ec, have, want, rd) == GARAGE_EC_OK;
+            for (int i = 0; i < tot && *ok; i++) *ok = (rd[i] & ~have_h[i]) == 0;  // every planned half is here
         }
+        if (bytes_out) *bytes_out += nbytes;
         block_len = expect;
         return count;
     }
@@ -1191,7 +1280,10 @@ struct garage_bm {
         uint32_t block_len = 0;
         bool ok = false;
         want[idx] = 1;
-        resync_shards_read += (uint64_t)gather_into(h, node, slot.p, have, block_len, false, /*for_gpu=*/true, want, &ok);
+        uint64_t nbytes = 0;
+        resync_shards_read += (uint64_t)gather_into(h, node, slot.p, have, block_len, false, /*for_gpu=*/true, want, &ok,
+                                                    &nbytes);
+        resync_bytes_read += nbytes;
         if (!ok) {
             resync_error_counter++;
             return GARAGE_BM_E_MISSING_BLOCK;  // resync.rs:488-494
@@ -1534,6 +1626,7 @@ void garage_bm_default_config(garage_bm_config *c)
     c->data_fsync = 0;             // util/config.rs data_fsync default
     c->block_gc_delay_ms = 600000;  // BLOCK_GC_DELAY, manager.rs:49-52
     c->local_groups = 0;            // RS
+    c->piggyback = 0;
 }
 
 static int bm_create(garage_bm **out, const garage_bm_config *cfg)
@@ -1545,10 +1638,15 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
     if (cfg->shard_sum_kind != GARAGE_EC_SUM_BLAKE2 && cfg->shard_sum_kind != GARAGE_EC_SUM_ADLER8) return GARAGE_EC_E_INVALID;
     const int l = cfg->local_groups;
     if (l < 0 || (l > 0 && (l >= m || k % l))) return GARAGE_EC_E_INVALID;
-    // every context of the manager runs the same code: RS(k, m), or LRC(k, l, m - l)
+    const bool pb = cfg->piggyback != 0;
+    // PB is not combined with LRC, and its half reads need per-segment (adler8) tags
+    if ((cfg->piggyback != 0 && cfg->piggyback != 1) || (pb && (l > 0 || cfg->shard_sum_kind == GARAGE_EC_SUM_BLAKE2)))
+        return GARAGE_EC_E_INVALID;
+    // every context of the manager runs the same code: RS(k, m), LRC(k, l, m - l) or PB(k, m)
     auto make_ctx = [&](garage_ec_ctx **c) {
-        return l ? garage_ec_create_lrc(c, cfg->cuda_device, k, l, m - l)
-                 : garage_ec_create(c, cfg->cuda_device, k, m, GARAGE_EC_VANDERMONDE);
+        return pb ? garage_ec_create_piggyback(c, cfg->cuda_device, k, m, GARAGE_EC_VANDERMONDE)
+                  : l ? garage_ec_create_lrc(c, cfg->cuda_device, k, l, m - l)
+                      : garage_ec_create(c, cfg->cuda_device, k, m, GARAGE_EC_VANDERMONDE);
     };
     std::unique_ptr<garage_bm> bm(new garage_bm());
     bm->cfg = *cfg;
@@ -1557,10 +1655,11 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
     bm->m = m;
     bm->tot = k + m;
     bm->sum_kind = cfg->shard_sum_kind;
-    bm->slot_stride = garage_ec_stride_for(garage_ec_shard_len(bm->cfg.block_size, k));
+    bm->pb = pb;
     int rc = make_ctx(&bm->ec);
     if (rc != GARAGE_EC_OK) return rc;  // no GPU => no block manager: there is no CPU fallback
     garage_ec_set_sum_kind(bm->ec, bm->sum_kind);
+    bm->slot_stride = garage_ec_stride_for((uint32_t)bm->shard_len_of(bm->cfg.block_size));
     if (cfg->n_nodes <= GARAGE_LAYOUT_MAX_NODES) {
         const int n = cfg->n_nodes, tot = k + m;
         std::vector<uint8_t> ring((size_t)GARAGE_NB_PARTITIONS * tot);
@@ -1577,6 +1676,7 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
         nd.k = k;
         nd.m = m;
         nd.l = cfg->local_groups;
+        nd.pb = pb;
         nd.fsync_data = cfg->data_fsync != 0;
         if (cfg->data_dir && cfg->data_dir[0]) {
             nd.dir = std::string(cfg->data_dir) + "/node" + std::to_string(i);
@@ -1918,6 +2018,7 @@ void garage_bm_get_metrics(garage_bm *bm, garage_bm_metrics *o)
     o->corrupt_data_errors = bm->corrupt_data_errors;
     o->write_errors = bm->write_errors;
     o->resync_shards_read = bm->resync_shards_read;
+    o->resync_bytes_read = bm->resync_bytes_read;
     uint64_t ql = 0;
     for (auto &n : bm->nodes) {
         std::lock_guard<std::mutex> lk(n->mu);

@@ -61,6 +61,7 @@ constexpr int kMaxLaneSets = 4;
 struct garage_ec_ctx {
     int device = 0, k = 0, m = 0;
     int l = 0;  // LRC local groups (garage_ec_create_lrc); 0 = RS (MDS: any k shards decode)
+    bool pb = false;  // piggybacked RS PB(k, m) (garage_ec_create_piggyback, DESIGN.md section 2.2)
     uint8_t P[kMaxM * kMaxK] = {0};
     int sm_count = 0;
     size_t smem_optin = 0;
@@ -322,6 +323,65 @@ cudaError_t launch_apply(garage_ec_ctx *ctx, const ApplyParams &p, cudaStream_t 
 
 uint32_t items_per_stripe(size_t stride) { return (uint32_t)((stride / 16 + 31) / 32); }
 
+template <int K, int MODE>
+cudaError_t launch_pb_t(const garage_ec_ctx *ctx, const ApplyParams &p, cudaStream_t st)
+{
+    static std::atomic<int> configured_for_device{-1};  // per instantiation
+    using CFG = PbCfg<K, MODE>;
+    auto kern = pb_apply_kernel<K, MODE>;
+    if ((size_t)CFG::kSmem > ctx->smem_optin) return cudaErrorInvalidConfiguration;
+    if (configured_for_device.load(std::memory_order_acquire) != ctx->device) {
+        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CFG::kSmem);
+        if (e != cudaSuccess) return e;
+        configured_for_device.store(ctx->device, std::memory_order_release);
+    }
+    kern<<<ctx->sm_count, CFG::kThreads, CFG::kSmem, st>>>(p);
+    return cudaGetLastError();
+}
+
+template <int MODE>
+cudaError_t launch_pb(garage_ec_ctx *ctx, const ApplyParams &p, cudaStream_t st)
+{
+    ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    switch (p.k) {
+#define GEC_CASE(KK) case KK: return launch_pb_t<KK, MODE>(ctx, p, st);
+        GEC_CASE(1) GEC_CASE(2) GEC_CASE(3) GEC_CASE(4) GEC_CASE(5) GEC_CASE(6) GEC_CASE(7) GEC_CASE(8)
+        GEC_CASE(9) GEC_CASE(10) GEC_CASE(11) GEC_CASE(12) GEC_CASE(13) GEC_CASE(14) GEC_CASE(15) GEC_CASE(16)
+#undef GEC_CASE
+    default: return cudaErrorInvalidConfiguration;
+    }
+}
+
+// PB encode / verify: one launch per batch slice, all m <= 4 rows in one pass (pb_apply_kernel)
+int run_pb_uniform(garage_ec_ctx *ctx, int mode, const uint8_t *src, size_t src_pitch, uint8_t *dst, size_t dst_pitch,
+                   uint32_t *mismatch, const uint32_t *shard_len, size_t stride, size_t n, cudaStream_t st)
+{
+    const uint32_t ips = (uint32_t)((stride / 32 + 31) / 32);  // 32-column chunks of the longest half
+    const size_t max_n = 0xffffffffull / ips;
+    TimedLaunch tl(ctx, st);
+    for (size_t s0 = 0; s0 < n; s0 += max_n) {
+        const size_t cnt = n - s0 < max_n ? n - s0 : max_n;
+        ApplyParams p;
+        memset(&p, 0, sizeof(p));
+        p.src = src + s0 * src_pitch;
+        p.src_pitch = src_pitch;
+        p.dst = dst ? dst + s0 * dst_pitch : nullptr;
+        p.dst_pitch = dst_pitch;
+        p.shard_len = shard_len ? shard_len + s0 : nullptr;
+        p.mismatch = mismatch ? mismatch + s0 : nullptr;
+        p.stride = (uint32_t)stride;
+        p.n = (uint32_t)cnt;
+        p.k = (uint32_t)ctx->k;
+        p.rows = (uint32_t)ctx->m;
+        p.items_per_stripe = ips;
+        p.row_bytes = 128;
+        memcpy(p.coef, ctx->P, (size_t)ctx->k * ctx->m);
+        cudaError_t e = mode == kModeEncode ? launch_pb<kModeEncode>(ctx, p, st) : launch_pb<kModeVerify>(ctx, p, st);
+        if (e != cudaSuccess) return set_cuda_error(ctx, e, "pb_apply_kernel launch");
+    }
+    return GARAGE_EC_OK;
+}
+
 // cuTensorMapEncodeTiled through the runtime (no link against libcuda)
 using TensorMapEncodeFn = CUresult (*)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
                                        const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
@@ -368,6 +428,7 @@ int run_uniform(garage_ec_ctx *ctx, int mode, const uint8_t *src, size_t src_pit
                 size_t dst_pitch, uint32_t *mismatch, const uint32_t *shard_len, size_t stride,
                 size_t n, cudaStream_t st, bool allow_tmap = true)
 {
+    if (ctx->pb) return run_pb_uniform(ctx, mode, src, src_pitch, dst, dst_pitch, mismatch, shard_len, stride, n, st);
     const uint32_t ips = items_per_stripe(stride);
     // the kernel's work counter runs past the item count by at most two claimed runs per warp
     const size_t max_n = (0xffffffffull - (1ull << 24)) / ips;
@@ -432,17 +493,23 @@ int run_reconstruct(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *present,
     q.m = (uint32_t)ctx->m;
     q.l = (uint32_t)ctx->l;
     q.present_is_bad = present_is_bad ? 1u : 0u;
+    q.shard_len = shard_len;
+    q.stride = (uint32_t)stride;
     memcpy(q.P, ctx->P, (size_t)ctx->k * ctx->m);
     const unsigned blocks = (unsigned)((n + kPlanWarps - 1) / kPlanWarps);
-    if (ctx->l) lrc_plan_kernel<<<blocks, kPlanWarps * 32, 0, st>>>(q);
+    if (ctx->pb) pb_plan_kernel<<<blocks, kPlanWarps * 32, 0, st>>>(q);
+    else if (ctx->l) lrc_plan_kernel<<<blocks, kPlanWarps * 32, 0, st>>>(q);
     else rs_plan_kernel<<<blocks, kPlanWarps * 32, 0, st>>>(q);
     ctx->launches.fetch_add(1, std::memory_order_relaxed);
     cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_cuda_error(ctx, e, ctx->l ? "lrc_plan_kernel launch" : "rs_plan_kernel launch");
+    if (e != cudaSuccess)
+        return set_cuda_error(ctx, e, ctx->pb ? "pb_plan_kernel launch" : (ctx->l ? "lrc_plan_kernel launch" : "rs_plan_kernel launch"));
 
     TimedLaunch tl(ctx, st);
     const size_t pitch = (size_t)(ctx->k + ctx->m) * stride;
-    for (int r0 = 0; r0 < ctx->m; r0 += kRowsPerPass) {
+    // PB: the plan is over half-rows, 2k sources and up to 2m outputs of length shard_len/2
+    const int nout = ctx->pb ? 2 * ctx->m : ctx->m;
+    for (int r0 = 0; r0 < nout; r0 += kRowsPerPass) {
         if (r0 > 0) {
             e = cudaMemsetAsync(counter, 0, sizeof(uint32_t), st);
             if (e != cudaSuccess) return set_cuda_error(ctx, e, "cudaMemsetAsync(counter)");
@@ -457,7 +524,8 @@ int run_reconstruct(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *present,
         p.counter = counter;
         p.stride = (uint32_t)stride;
         p.n = (uint32_t)n;
-        p.k = (uint32_t)ctx->k;
+        p.k = (uint32_t)(ctx->pb ? 2 * ctx->k : ctx->k);
+        p.half = ctx->pb ? 1u : 0u;
         p.row_off = (uint32_t)r0;
         p.row_bytes = 128;
         e = launch_apply<kModePlan>(ctx, p, st);
@@ -470,14 +538,56 @@ size_t plan_scratch_bytes(size_t n) { return n * sizeof(StripePlan) + 16; }
 
 // The shards the plan kernels read for one stripe (present / want: k+m bytes, want nullable = every absent
 // shard), as a bit mask; false if a wanted shard cannot be rebuilt.  HOST paths upload only these.
-bool stripe_read_set(const garage_ec_ctx *ctx, const uint8_t *present, const uint8_t *want, uint64_t *read)
+// PB contexts: bit 2i / 2i+1 of *halves = a- / b-half of shard i (h_pb_read_plan); other codes: 3 << 2i for every
+// shard of the read set.
+bool stripe_read_plan(const garage_ec_ctx *ctx, const uint8_t *present, const uint8_t *want, uint64_t *halves)
 {
     uint64_t pm = 0, wm = 0;
     for (int i = 0; i < ctx->k + ctx->m; i++) {
         pm |= (uint64_t)(present[i] != 0) << i;
         wm |= (uint64_t)(!want || want[i] != 0) << i;
     }
-    return h_read_set(ctx->k, ctx->m, ctx->l, ctx->P, pm, wm, read);
+    if (ctx->pb) return h_pb_read_plan(ctx->k, ctx->m, ctx->P, pm, wm, halves);
+    uint64_t rd = 0;
+    const bool ok = h_read_set(ctx->k, ctx->m, ctx->l, ctx->P, pm, wm, &rd);
+    *halves = 0;
+    for (int i = 0; i < ctx->k + ctx->m; i++)
+        if ((rd >> i) & 1) *halves |= 3ull << (2 * i);
+    return ok;
+}
+bool stripe_read_set(const garage_ec_ctx *ctx, const uint8_t *present, const uint8_t *want, uint64_t *read)
+{
+    uint64_t hv = 0;
+    const bool ok = stripe_read_plan(ctx, present, want, &hv);
+    *read = 0;
+    for (int i = 0; i < ctx->k + ctx->m; i++)
+        if ((hv >> (2 * i)) & 3) *read |= 1ull << i;
+    return ok;
+}
+// The pieces of shard i a HOST upload copies, as f(offset, bytes): `whole` bytes from 0 for a shard of the read set,
+// or (PB) each planned half of shard_len/2 bytes
+template <class F>
+void for_each_read_piece(const garage_ec_ctx *ctx, uint64_t halves, size_t i, size_t len, size_t whole, F &&f)
+{
+    const unsigned b = (unsigned)(halves >> (2 * i)) & 3u;
+    if (!b) return;
+    if (!ctx->pb) f((size_t)0, whole);
+    else if (b == 3) f((size_t)0, len);
+    else f(b == 1 ? (size_t)0 : len / 2, len / 2);
+}
+// PB: every stripe's shard_len (NULL: stride) must be a multiple of 32 so that the halves are 16-byte aligned
+bool pb_lens_ok(const garage_ec_ctx *ctx, const uint32_t *shard_len, size_t stride, size_t n)
+{
+    if (!ctx->pb) return true;
+    if (!shard_len) return (stride & 31) == 0;
+    for (size_t s = 0; s < n; s++)
+        if ((shard_len[s] & 31) || shard_len[s] > stride) return false;
+    return true;
+}
+// 64-bit: a PB length that does not fit in 32 bits is larger than any stride, so the stride checks reject it
+uint64_t code_shard_len(const garage_ec_ctx *ctx, uint32_t block_len)
+{
+    return ctx->pb ? pb_shard_len(block_len, ctx->k) : garage_ec_shard_len(block_len, ctx->k);
 }
 
 // ---- batched async copies ---------------------------------------------------------------
@@ -563,7 +673,7 @@ int lane_reserve(garage_ec_ctx *ctx, HostLane &L, size_t buf_bytes, size_t small
 
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
-int create_common(garage_ec_ctx **out, int device, int k, int m, const uint8_t *P, int kind, int l = 0)
+int create_common(garage_ec_ctx **out, int device, int k, int m, const uint8_t *P, int kind, int l = 0, bool pb = false)
 {
     if (!out) return GARAGE_EC_E_INVALID;
     *out = nullptr;
@@ -583,6 +693,7 @@ int create_common(garage_ec_ctx **out, int device, int k, int m, const uint8_t *
     ctx->k = k;
     ctx->m = m;
     ctx->l = l;
+    ctx->pb = pb;
     if (P) {
         memcpy(ctx->P, P, (size_t)k * m);
     } else if (!h_build_matrix(k, m, kind, ctx->P)) {
@@ -657,6 +768,43 @@ int garage_ec_create_lrc(garage_ec_ctx **out, int cuda_device, int k, int l, int
         return GARAGE_EC_E_INVALID;
     }
     return create_common(out, cuda_device, k, l + r, P, 0, l);
+}
+
+int garage_ec_create_piggyback(garage_ec_ctx **out, int cuda_device, int k, int m, int matrix_kind)
+{
+    if (k < 1 || k > kPbMaxK || m < kPbMinM || m > kPbMaxM ||
+        (matrix_kind != GARAGE_EC_VANDERMONDE && matrix_kind != GARAGE_EC_CAUCHY)) {
+        if (out) *out = nullptr;
+        return GARAGE_EC_E_INVALID;
+    }
+    return create_common(out, cuda_device, k, m, nullptr, matrix_kind, 0, true);
+}
+
+int garage_ec_piggyback_info(const garage_ec_ctx *ctx, int *groups, uint8_t *group_of)
+{
+    if (!ctx) return GARAGE_EC_E_INVALID;
+    if (groups) *groups = ctx->pb ? ctx->m - 1 : 0;
+    if (group_of)
+        for (int j = 0; j < ctx->k; j++) group_of[j] = ctx->pb ? (uint8_t)pb_group_of(ctx->k, ctx->m, j) : 0;
+    return GARAGE_EC_OK;
+}
+
+int garage_ec_code_shard_len(const garage_ec_ctx *ctx, uint32_t block_len, uint32_t *shard_len)
+{
+    if (!ctx || !shard_len) return GARAGE_EC_E_INVALID;
+    const uint64_t L = code_shard_len(ctx, block_len);
+    if (L > 0xffffffffull) return GARAGE_EC_E_INVALID;  // PB with k = 1 and block_len > 2^32 - 128
+    *shard_len = (uint32_t)L;
+    return GARAGE_EC_OK;
+}
+
+int garage_ec_read_plan(const garage_ec_ctx *ctx, const uint8_t *present, const uint8_t *want, uint8_t *halves_out)
+{
+    if (!ctx || !present || !halves_out) return GARAGE_EC_E_INVALID;
+    uint64_t hv = 0;
+    const bool ok = stripe_read_plan(ctx, present, want, &hv);
+    for (int i = 0; i < ctx->k + ctx->m; i++) halves_out[i] = (uint8_t)((hv >> (2 * i)) & 3);
+    return ok ? GARAGE_EC_OK : GARAGE_EC_E_UNRECOVERABLE;
 }
 
 int garage_ec_code_info(const garage_ec_ctx *ctx, int *local_groups, int *global_parity)
@@ -946,6 +1094,7 @@ int garage_ec_encode(garage_ec_ctx *ctx, const uint8_t *data, uint8_t *parity,
     if (n_stripes == 0) return GARAGE_EC_OK;
     if (!data || !parity) return GARAGE_EC_E_INVALID;
     if (!aligned16(data) || !aligned16(parity)) return GARAGE_EC_E_ALIGN;
+    if (mem_kind == GARAGE_EC_MEM_HOST && !pb_lens_ok(ctx, shard_len, stride, n_stripes)) return GARAGE_EC_E_INVALID;
     CU_TRY(ctx, cudaSetDevice(ctx->device));
     if (mem_kind == GARAGE_EC_MEM_HOST) return encode_host(ctx, data, parity, shard_len, stride, n_stripes);
     return run_uniform(ctx, kModeEncode, data, (size_t)ctx->k * stride, parity, (size_t)ctx->m * stride,
@@ -1000,6 +1149,7 @@ int garage_ec_verify(garage_ec_ctx *ctx, const uint8_t *shards, uint32_t *mismat
     if (n_stripes == 0) return GARAGE_EC_OK;
     if (!shards || !mismatch) return GARAGE_EC_E_INVALID;
     if (!aligned16(shards)) return GARAGE_EC_E_ALIGN;
+    if (mem_kind == GARAGE_EC_MEM_HOST && !pb_lens_ok(ctx, shard_len, stride, n_stripes)) return GARAGE_EC_E_INVALID;
     CU_TRY(ctx, cudaSetDevice(ctx->device));
     if (mem_kind == GARAGE_EC_MEM_HOST) return verify_host(ctx, shards, mismatch, shard_len, stride, n_stripes);
     cudaStream_t st = (cudaStream_t)cuda_stream;
@@ -1076,13 +1226,16 @@ static int reconstruct_host(garage_ec_ctx *ctx, uint8_t *shards, uint8_t *const 
         uint8_t *d_sh = L.d_buf;
         // H2D: only the survivors the kernel reads (stripe_read_set) of stripes that have work to do
         for (size_t s = s0; s < s0 + cnt; s++) {
-            uint64_t rd = 0;
+            uint64_t hv = 0;
             bool work = false;  // a wanted shard is absent
             for (size_t i = 0; i < tot; i++) work |= !present[s * tot + i] && (!want || want[s * tot + i]);
-            rec_ok[s - s0] = stripe_read_set(ctx, present + s * tot, want ? want + s * tot : nullptr, &rd);
+            rec_ok[s - s0] = stripe_read_plan(ctx, present + s * tot, want ? want + s * tot : nullptr, &hv);
             if (!rec_ok[s - s0] || !work) continue;
+            const size_t len = shard_len ? shard_len[s] : stride;
             for (size_t i = 0; i < tot; i++)
-                if ((rd >> i) & 1) up.add(d_sh + ((s - s0) * tot + i) * stride, shard_at(s, i), stride);
+                for_each_read_piece(ctx, hv, i, len, stride, [&](size_t off, size_t bytes) {
+                    up.add(d_sh + ((s - s0) * tot + i) * stride + off, shard_at(s, i) + off, bytes);
+                });
         }
         rc = up.flush(ctx, cudaMemcpyHostToDevice, L.stream);
         if (rc) return rc;
@@ -1139,6 +1292,7 @@ int garage_ec_reconstruct(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *pr
     if (n_stripes == 0) return GARAGE_EC_OK;
     if (!shards || !present) return GARAGE_EC_E_INVALID;
     if (!aligned16(shards)) return GARAGE_EC_E_ALIGN;
+    if (mem_kind == GARAGE_EC_MEM_HOST && !pb_lens_ok(ctx, shard_len, stride, n_stripes)) return GARAGE_EC_E_INVALID;
     CU_TRY(ctx, cudaSetDevice(ctx->device));
     if (mem_kind == GARAGE_EC_MEM_HOST)
         return reconstruct_host(ctx, shards, nullptr, present, want, status, shard_len, stride, n_stripes);
@@ -1169,6 +1323,7 @@ int garage_ec_reconstruct_stripes(garage_ec_ctx *ctx, uint8_t *const *stripes, c
         if (!stripes[s]) return GARAGE_EC_E_INVALID;
         if (!aligned16(stripes[s])) return GARAGE_EC_E_ALIGN;
     }
+    if (!pb_lens_ok(ctx, shard_len, stride, n_stripes)) return GARAGE_EC_E_INVALID;
     CU_TRY(ctx, cudaSetDevice(ctx->device));
     return reconstruct_host(ctx, nullptr, stripes, present, want, status, shard_len, stride, n_stripes);
 }
@@ -1410,12 +1565,51 @@ static void adler8_host_fast(const uint8_t *data, size_t len, uint8_t out[32])
 static void adler8_host_fast(const uint8_t *data, size_t len, uint8_t out[32]) { adler8_host(data, len, out); }
 #endif
 
+// zlib Adler-32 of one buffer
+static uint32_t adler32_one(const uint8_t *p, size_t n)
+{
+#if defined(__x86_64__)
+    static const bool avx2 = __builtin_cpu_supports("avx2");
+    if (avx2) return adler32_avx2(p, n);
+#endif
+    uint32_t a = 1, b = 0;
+    while (n) {
+        const size_t run = n > 5552 ? 5552 : n;  // zlib's NMAX: the sums cannot overflow 32 bits
+        for (size_t i = 0; i < run; i++) {
+            a += p[i];
+            b += a;
+        }
+        a %= 65521;
+        b %= 65521;
+        p += run;
+        n -= run;
+    }
+    return (b << 16) | a;
+}
+
 int garage_ec_shard_sum_host(int kind, const uint8_t *data, size_t len, uint8_t out32[32])
 {
     if (!out32 || (!data && len)) return GARAGE_EC_E_INVALID;
     if (kind == GARAGE_EC_SUM_BLAKE2) blake2sum_host(data, len, out32);
     else if (kind == GARAGE_EC_SUM_ADLER8) adler8_host_fast(data, len, out32);
     else return GARAGE_EC_E_INVALID;
+    return GARAGE_EC_OK;
+}
+
+int garage_ec_check_shard_half_host(int kind, const uint8_t *half_bytes, uint32_t shard_len, int which,
+                                    const uint8_t tag32[32])
+{
+    if (kind != GARAGE_EC_SUM_ADLER8 || (shard_len % 128) || (which != 0 && which != 1) || !tag32 ||
+        (!half_bytes && shard_len))
+        return GARAGE_EC_E_INVALID;
+    // shard_len % 128 == 0: the 8 segments are shard_len/8 bytes each, and half `which` is segments 4*which..+3
+    const size_t seg = shard_len / 8;
+    for (int t = 0; t < 4; t++) {
+        const uint32_t v = seg ? adler32_one(half_bytes + t * seg, seg) : 1u;
+        uint32_t want;
+        memcpy(&want, tag32 + 4 * (4 * which + t), 4);  // little endian
+        if (v != want) return 1;
+    }
     return GARAGE_EC_OK;
 }
 
@@ -1432,6 +1626,7 @@ int garage_ec_scrub_repair(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *e
     if (!aligned16(shards)) return GARAGE_EC_E_ALIGN;
     const size_t tot = ctx->k + ctx->m;
     if (n_stripes * tot > 0xffffffffull) return GARAGE_EC_E_INVALID;
+    if (mem_kind == GARAGE_EC_MEM_HOST && !pb_lens_ok(ctx, shard_len, stride, n_stripes)) return GARAGE_EC_E_INVALID;
     CU_TRY(ctx, cudaSetDevice(ctx->device));
     if (mem_kind == GARAGE_EC_MEM_DEVICE) {
         cudaStream_t st = (cudaStream_t)cuda_stream;
@@ -1547,7 +1742,7 @@ int garage_ec_encode_blocks_with_sums(garage_ec_ctx *ctx, const uint8_t *const *
     uint32_t max_len = 0;
     for (size_t s = 0; s < n_blocks; s++) {
         if (!blocks[s] && block_len[s]) return GARAGE_EC_E_INVALID;
-        if (garage_ec_shard_len(block_len[s], (int)k) > stride) return GARAGE_EC_E_INVALID;
+        if (code_shard_len(ctx, block_len[s]) > stride) return GARAGE_EC_E_INVALID;
         max_len = block_len[s] > max_len ? block_len[s] : max_len;
     }
     const auto tr0 = std::chrono::steady_clock::now();
@@ -1584,7 +1779,7 @@ int garage_ec_encode_blocks_with_sums(garage_ec_ctx *ctx, const uint8_t *const *
         uint32_t *hl = lens.data() + lane_i * 2 * cs, *hb = hl + cs;
         uint8_t *d_blk = L.d_buf, *d_data = L.d_buf + blk_b, *d_par = d_data + in_b;
         for (size_t s = 0; s < cnt; s++) {
-            hl[s] = garage_ec_shard_len(block_len[s0 + s], (int)k);
+            hl[s] = code_shard_len(ctx, block_len[s0 + s]);
             hb[s] = block_len[s0 + s];
             // H2D: the block as ONE contiguous copy; the framing happens on the device
             up.add(d_blk + s * pitch, blocks[s0 + s], block_len[s0 + s]);
@@ -1602,6 +1797,7 @@ int garage_ec_encode_blocks_with_sums(garage_ec_ctx *ctx, const uint8_t *const *
         sp.stride = (uint32_t)stride;
         sp.k = (uint32_t)k;
         sp.n = (uint32_t)cnt;
+        sp.round128 = ctx->pb ? 1u : 0u;
         // ~4 CTAs per SM whatever the batch size (one CTA per block left 13 SMs copying 1 MiB each: 150 us)
         sp.parts = (uint32_t)std::max<size_t>(1, std::min<size_t>(64, ((size_t)ctx->sm_count * 4 + cnt - 1) / cnt));
         split_blocks_kernel<<<(unsigned)std::min<size_t>(cnt * sp.parts, (size_t)ctx->sm_count * 8), 256, 0, L.stream>>>(sp);
@@ -1661,7 +1857,7 @@ int garage_ec_decode_blocks(garage_ec_ctx *ctx, const uint8_t *shards, const uin
 
     // stripes with an absent data shard go to the GPU; the rest is a host-side join
     std::vector<size_t> need;
-    std::vector<uint64_t> reads(n_blocks);  // survivors the kernel reads (data shards wanted)
+    std::vector<uint64_t> reads(n_blocks);  // survivors (halves) the kernel reads, data shards wanted
     std::vector<uint8_t> ok(n_blocks);
     std::vector<uint8_t> want_data(tot);
     for (size_t i = 0; i < tot; i++) want_data[i] = i < k ? 1 : 0;
@@ -1670,8 +1866,8 @@ int garage_ec_decode_blocks(garage_ec_ctx *ctx, const uint8_t *shards, const uin
         const uint8_t *pr = present + s * tot;
         bool data_missing = false;
         for (size_t j = 0; j < k; j++) data_missing |= !pr[j];
-        if (garage_ec_shard_len(block_len[s], (int)k) > stride) return GARAGE_EC_E_INVALID;
-        ok[s] = stripe_read_set(ctx, pr, want_data.data(), &reads[s]);
+        if (code_shard_len(ctx, block_len[s]) > stride) return GARAGE_EC_E_INVALID;
+        ok[s] = stripe_read_plan(ctx, pr, want_data.data(), &reads[s]);
         if (!ok[s]) {
             if (status) status[s] = GARAGE_EC_E_UNRECOVERABLE;
             any_bad = true;
@@ -1708,12 +1904,13 @@ int garage_ec_decode_blocks(garage_ec_ctx *ctx, const uint8_t *shards, const uin
                 const size_t s = need[q0 + q];
                 memcpy(hp + q * tot, present + s * tot, tot);
                 for (size_t i = 0; i < tot; i++) hw[q * tot + i] = i < k ? 1 : 0;  // data shards only
-                hl[q] = garage_ec_shard_len(block_len[s], (int)k);
+                hl[q] = code_shard_len(ctx, block_len[s]);
                 // H2D: only the survivors the kernel reads -- the GET path is PCIe-bound, absent and
                 // surplus shards stay on the host
                 for (size_t i = 0; i < tot; i++)
-                    if ((reads[s] >> i) & 1)
-                        up.add(L.d_buf + (q * tot + i) * stride, shards + (s * tot + i) * stride, align_up(hl[q], 16));
+                    for_each_read_piece(ctx, reads[s], i, hl[q], align_up(hl[q], 16), [&](size_t off, size_t bytes) {
+                        up.add(L.d_buf + (q * tot + i) * stride + off, shards + (s * tot + i) * stride + off, bytes);
+                    });
             }
             rc = up.flush(ctx, cudaMemcpyHostToDevice, L.stream);
             if (rc) return rc;
@@ -1747,7 +1944,7 @@ int garage_ec_decode_blocks(garage_ec_ctx *ctx, const uint8_t *shards, const uin
         for (size_t s = 0; s < n_blocks; s++) {
             const uint8_t *pr = present + s * tot;
             if (!ok[s]) continue;
-            const size_t Ls = garage_ec_shard_len(block_len[s], (int)k);
+            const size_t Ls = code_shard_len(ctx, block_len[s]);
             for (size_t j = 0; j < k; j++) {
                 if (!pr[j]) continue;
                 const size_t off = j * Ls;
@@ -1761,7 +1958,7 @@ int garage_ec_decode_blocks(garage_ec_ctx *ctx, const uint8_t *shards, const uin
     }
     for (size_t s = 0; s < n_blocks; s++) {
         if (!ok[s]) continue;
-        const size_t Ls = garage_ec_shard_len(block_len[s], (int)k);
+        const size_t Ls = code_shard_len(ctx, block_len[s]);
         for (size_t j = 0; j < k; j++) {
             const size_t off = j * Ls;
             if (off >= block_len[s]) continue;

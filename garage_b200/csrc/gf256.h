@@ -12,6 +12,12 @@
 #define GARAGE_EC_MAX_K_HOST 32
 #define GARAGE_EC_MAX_M_HOST 8
 
+#ifdef __CUDACC__
+#define GEC_GF_HD __host__ __device__
+#else
+#define GEC_GF_HD
+#endif
+
 namespace garage_ec {
 
 // host copies
@@ -164,6 +170,97 @@ inline bool h_read_set(int k, int m, int l, const uint8_t *P, uint64_t present, 
         reduce(v);
         for (int j = 0; j < k; j++)
             if (v[j]) return false;
+    }
+    return true;
+}
+
+// ---- piggybacked RS, PB(k, m) (DESIGN.md section 2.2) ------------------------------------------------------------
+// The k data shards form m-1 contiguous groups G_1..G_{m-1}, sizes as equal as possible, larger groups first.  The
+// b-half of parity i >= 1 carries the XOR of the a-halves of G_i on top of its RS value.
+constexpr int kPbMaxK = 16, kPbMinM = 2, kPbMaxM = 4;
+// first data shard of group g (1 <= g <= m-1); g = m gives k
+GEC_GF_HD inline int pb_group_start(int k, int m, int g)
+{
+    const int ng = m - 1, base = k / ng, rem = k % ng, i = g - 1;
+    return i * base + (i < rem ? i : rem);
+}
+GEC_GF_HD inline int pb_group_of(int k, int m, int j)
+{
+    int g = 1;
+    while (g < m - 1 && j >= pb_group_start(k, m, g + 1)) g++;
+    return g;
+}
+// shard length of a block: ceil(block_len / k) rounded up to 128 bytes, so that both halves are 16-byte aligned and
+// each half is exactly 4 of the 8 adler8 segments.  64-bit: with k = 1 a block_len near 2^32 rounds past 32 bits.
+inline uint64_t pb_shard_len(uint32_t block_len, int k)
+{
+    const uint64_t L = ((uint64_t)block_len + (unsigned)k - 1) / (unsigned)k;
+    return (L + 127) / 128 * 128;
+}
+// Generator over half-symbols: row q = 2*shard + half (0..2(k+m)), column c = 2*data + half (0..2k).
+GEC_GF_HD inline uint8_t pb_grow(int k, int m, const uint8_t *P, int q, int c)
+{
+    const int sh = q >> 1, h = q & 1, j = c >> 1, hc = c & 1;
+    if (sh < k) return (uint8_t)(q == c);
+    const int i = sh - k;
+    if (hc == h) return P[i * k + j];
+    return (uint8_t)(h == 1 && i >= 1 && pb_group_of(k, m, j) == i);  // the piggyback: a_j in b of parity i
+}
+// Half-row read plan of one PB stripe (host twin of pb_plan_kernel).  Bit i of present / want: shard i present /
+// wanted.  *halves: bit 2i = a-half of shard i read, bit 2i+1 = b-half.  Rule 1 when the only wanted absent shard is
+// a data shard j of G_i, every other data shard is present and so are parities 0 and i; rule 2 (greedy rank basis of
+// the present half-rows in q order) otherwise.  False if a wanted shard cannot be rebuilt.
+inline bool h_pb_read_plan(int k, int m, const uint8_t *P, uint64_t present, uint64_t want, uint64_t *halves)
+{
+    const int tot = k + m, K2 = 2 * k;
+    const uint64_t all = (1ull << tot) - 1, data = (1ull << k) - 1;
+    present &= all;
+    want &= all & ~present;
+    *halves = 0;
+    uint64_t hp = 0;
+    for (int i = 0; i < tot; i++)
+        if ((present >> i) & 1) hp |= 3ull << (2 * i);
+    if (want && !(want & (want - 1)) && (want & data)) {
+        const int j = __builtin_ctzll(want), g = pb_group_of(k, m, j);
+        if ((present & data) == (data & ~want) && ((present >> k) & 1) && ((present >> (k + g)) & 1)) {
+            uint64_t r = (1ull << (2 * k + 1)) | (1ull << (2 * (k + g) + 1));
+            for (int x = 0; x < k; x++)
+                if (x != j) r |= 1ull << (2 * x + 1);
+            for (int x = pb_group_start(k, m, g); x < pb_group_start(k, m, g + 1); x++)
+                if (x != j) r |= 1ull << (2 * x);
+            *halves = r;
+            return true;
+        }
+    }
+    uint8_t R[2 * kPbMaxK][2 * kPbMaxK];
+    int piv[2 * kPbMaxK], nb = 0;
+    auto reduce = [&](uint8_t *v) {
+        for (int b = 0; b < nb; b++) {
+            const uint8_t f = v[piv[b]];
+            if (f)
+                for (int c = 0; c < K2; c++) v[c] ^= h_mul(f, R[b][c]);
+        }
+    };
+    for (int q = 0; q < 2 * tot && nb < K2; q++) {
+        if (!((hp >> q) & 1)) continue;
+        uint8_t v[2 * kPbMaxK];
+        for (int c = 0; c < K2; c++) v[c] = pb_grow(k, m, P, q, c);
+        reduce(v);
+        int p = 0;
+        while (p < K2 && !v[p]) p++;
+        if (p == K2) continue;
+        const uint8_t iv = h_inv(v[p]);
+        for (int c = 0; c < K2; c++) R[nb][c] = h_mul(v[c], iv);
+        piv[nb++] = p;
+        *halves |= 1ull << q;
+    }
+    for (int q = 0; q < 2 * tot; q++) {
+        if (!((want >> (q >> 1)) & 1)) continue;
+        uint8_t v[2 * kPbMaxK];
+        for (int c = 0; c < K2; c++) v[c] = pb_grow(k, m, P, q, c);
+        reduce(v);
+        for (int c = 0; c < K2; c++)
+            if (v[c]) return false;
     }
     return true;
 }

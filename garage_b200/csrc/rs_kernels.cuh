@@ -333,6 +333,7 @@ struct ApplyParams {
     uint32_t row_bytes;         // 128: bytes per table row (a register operand keeps x*128 an IMAD)
     uint32_t use_tmap;          // 1: `tmap` is valid (uniform modes, TMA path)
     uint32_t rows_per_stripe;   // shards per stripe in `src` (k for encode, k+m for verify): tensor row of (s, j) = s*rows_per_stripe + j
+    uint32_t half;              // kModePlan, PB contexts: plan indices are half-rows q = 2*shard + half (DESIGN.md 2.2)
     uint8_t coef[kRowsPerPass * kMaxK];  // uniform modes: coef[i*k + j]
     // 2-D view of `src` for TMA: dim0 = stride/4 uint32 elements, dim1 = n*rows_per_stripe shards
     // (pitch `stride`), box = 128 elements (512 B = 32 columns) x k rows
@@ -1057,13 +1058,18 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
                 int rows = 0;
                 uint32_t ns = 0;
                 unsigned long long kp = 0, ko = 0;
+                const uint32_t slen = s < p.n ? (p.shard_len ? __ldg(p.shard_len + s) : p.stride) : 0;
+                // source / output index -> byte offset: a shard, or (PB) the half-row q = 2*shard + half
+                auto idx_off = [&](uint32_t i) -> uint32_t {
+                    return p.half ? (i >> 1) * p.stride + (i & 1) * (slen >> 1) : i * p.stride;
+                };
                 if (s < p.n) {
                     const StripePlan *pl = p.plan + s;
                     rows = pl->unrecoverable ? 0 : min(kRowsPerPass, (int)pl->nrows - (int)p.row_off);
                     if (rows > 0) {
                         ns = pl->nsurv;
-                        if (lane < ns) ps.src_off[lane] = (uint32_t)pl->surv[lane] * p.stride;
-                        if (lane < (uint32_t)rows) ps.dst_off[lane] = (uint32_t)pl->out_idx[p.row_off + lane] * p.stride;
+                        if (lane < ns) ps.src_off[lane] = idx_off(pl->surv[lane]);
+                        if (lane < (uint32_t)rows) ps.dst_off[lane] = idx_off(pl->out_idx[p.row_off + lane]);
                         for (uint32_t e = lane; e < (uint32_t)rows * kMaxK; e += 32)
                             ps.coef[e] = pl->coef[p.row_off + e / kMaxK][e % kMaxK];
                         kp = pl->key_present;
@@ -1071,7 +1077,7 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
                     }
                 }
                 if (lane == 0) {
-                    const uint32_t len = s < p.n ? (p.shard_len ? __ldg(p.shard_len + s) : p.stride) : 0;
+                    const uint32_t len = p.half ? slen >> 1 : slen;  // PB: chunks of one half
                     const uint32_t nch = (((len + 15) >> 4) + 31) >> 5;  // 32-column chunks of the stripe
                     ps.sid = s;
                     ps.rows = rows;
@@ -1285,6 +1291,8 @@ struct PlanParams {
     uint32_t n, k, m;
     uint32_t l;               // LRC local groups (lrc_plan_kernel); 0 for RS
     uint32_t present_is_bad;  // 1: `present` holds "bad" flags (scrub): a shard is present iff flag == 0
+    const uint32_t *shard_len;  // pb_plan_kernel: per stripe, nullable (=> stride); a length % 32 != 0 is malformed
+    uint32_t stride;
     alignas(16) uint8_t P[kMaxM * kMaxK];  // parity rows, P[i*k + j] (16-byte aligned: staged with uint4 loads)
 };
 
@@ -1598,6 +1606,280 @@ __global__ void __launch_bounds__(kPlanWarps * 32) lrc_plan_kernel(const __grid_
     }
 }
 
+// PB(k, m) planning (DESIGN.md section 2.2), one warp per stripe, over half-rows q = 2*shard + half: 2(k+m) <= 40
+// generator rows over 2k <= 32 half-data columns (lane = column), generator row q from pb_grow.  Rule 1 (a lone lost
+// data shard j of G_i with every other data shard and parities 0 and i present) is rule 2 run on the present
+// half-rows restricted to its k + |G_i| repair halves, which are independent: the greedy basis keeps them all.  Rule
+// 2 is the greedy rank basis of lrc_plan_kernel.  surv[] / out_idx[] hold half-row indices; rs_apply_kernel<2k,
+// kModePlan> with ApplyParams::half turns them into byte offsets.  A stripe whose shard_len is not a multiple of 32
+// has no 16-byte aligned halves: status GARAGE_EC_E_INVALID (-1), nothing is rebuilt.
+__global__ void __launch_bounds__(kPlanWarps * 32) pb_plan_kernel(const __grid_constant__ PlanParams q)
+{
+    __shared__ __align__(16) uint8_t s_gf[sizeof(GfTables)];
+    uint8_t *const s_exp = s_gf, *const s_log = s_gf + 512;
+    __shared__ uint8_t s_R[kPlanWarps][kMaxK][2 * kMaxK];
+    __shared__ uint8_t s_piv[kPlanWarps][kMaxK];
+    __shared__ uint8_t s_surv[kPlanWarps][kMaxK];
+    __shared__ __align__(16) uint8_t s_P[kMaxM * kMaxK];
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    stage_gf_tables(s_gf);
+    {
+        const uint4 *src = reinterpret_cast<const uint4 *>(q.P);
+        for (uint32_t i = warp; i < sizeof(q.P) / 16; i += blockDim.x >> 5) {
+            const uint4 v = src[i];
+            if (lane < 4) reinterpret_cast<uint32_t *>(s_P)[i * 4 + lane] = lane == 0 ? v.x : (lane == 1 ? v.y : (lane == 2 ? v.z : v.w));
+        }
+    }
+    if (blockIdx.x == 0 && tid == 0) *q.counter = 0;
+    __syncthreads();
+    auto mul = [&](uint32_t a, uint32_t b) -> uint32_t {
+        return (a && b) ? s_exp[s_log[a] + s_log[b]] : 0u;
+    };
+
+    const uint32_t s = blockIdx.x * kPlanWarps + warp;
+    if (s >= q.n) return;
+    const uint32_t k = q.k, m = q.m, tot = k + m, K2 = 2 * k;  // tot <= 20
+    StripePlan *pl = q.plan + s;
+    const uint8_t *pr = q.present + (size_t)s * tot;
+    const uint8_t *wn = q.want ? q.want + (size_t)s * tot : nullptr;
+    const bool inv = q.present_is_bad != 0;
+    const bool p0 = lane < tot && ((pr[lane] != 0) != inv);
+    const unsigned long long present = __ballot_sync(0xffffffffu, p0);
+    const unsigned long long outmask = __ballot_sync(0xffffffffu, lane < tot && !p0 && (!wn || wn[lane] != 0));
+    const uint32_t len = q.shard_len ? q.shard_len[s] : q.stride;
+    if (len & 31) {
+        if (lane == 0) {
+            pl->key_present = present;
+            pl->key_out = outmask;
+            pl->nrows = 0;
+            pl->unrecoverable = 1;
+            pl->nsurv = 0;
+            if (q.status) q.status[s] = -1;
+        }
+        return;
+    }
+    auto grow = [&](uint32_t r, uint32_t c) -> uint32_t { return c < K2 ? pb_grow((int)k, (int)m, s_P, (int)r, (int)c) : 0u; };
+    unsigned long long hp = 0, hout = 0;  // half-row masks
+    for (uint32_t i = 0; i < tot; i++) {
+        if ((present >> i) & 1) hp |= 3ull << (2 * i);
+        if ((outmask >> i) & 1) hout |= 3ull << (2 * i);
+    }
+    const unsigned long long data = (1ull << k) - 1;
+    if (outmask && !(outmask & (outmask - 1)) && (outmask & data)) {  // rule 1
+        const uint32_t j = (uint32_t)(__ffsll((long long)outmask) - 1), g = (uint32_t)pb_group_of((int)k, (int)m, (int)j);
+        if ((present & data) == (data & ~outmask) && ((present >> k) & 1) && ((present >> (k + g)) & 1)) {
+            unsigned long long r = (1ull << (2 * k + 1)) | (1ull << (2 * (k + g) + 1));
+            for (uint32_t x = 0; x < k; x++)
+                if (x != j) r |= 1ull << (2 * x + 1);
+            for (int x = pb_group_start((int)k, (int)m, (int)g); x < pb_group_start((int)k, (int)m, (int)g + 1); x++)
+                if ((uint32_t)x != j) r |= 1ull << (2 * x);
+            hp = r;
+        }
+    }
+    // rule 2: greedy basis in q order (as lrc_plan_kernel, 2k columns)
+    uint8_t(*R)[2 * kMaxK] = s_R[warp];
+    uint32_t nsurv = 0;
+    for (unsigned long long pm = hp; pm && nsurv < K2; pm &= pm - 1) {
+        const uint32_t c = (uint32_t)(__ffsll((long long)pm) - 1);
+        uint32_t v = grow(c, lane), t = lane == nsurv ? 1u : 0u;
+        for (uint32_t b = 0; b < nsurv; b++) {
+            const uint32_t f = __shfl_sync(0xffffffffu, v, s_piv[warp][b]);
+            if (f) {
+                v ^= mul(f, R[b][lane]);
+                t ^= mul(f, R[b][kMaxK + lane]);
+            }
+        }
+        const uint32_t nz = __ballot_sync(0xffffffffu, v != 0);
+        if (!nz) continue;
+        const uint32_t piv = __ffs(nz) - 1;
+        const uint32_t iv = s_exp[255 - s_log[__shfl_sync(0xffffffffu, v, piv)]];
+        R[nsurv][lane] = (uint8_t)mul(v, iv);
+        R[nsurv][kMaxK + lane] = (uint8_t)mul(t, iv);
+        if (lane == 0) {
+            s_piv[warp][nsurv] = (uint8_t)piv;
+            s_surv[warp][nsurv] = (uint8_t)c;
+        }
+        __syncwarp();
+        nsurv++;
+    }
+    bool ok = true;
+    int r = 0;
+    for (unsigned long long om = hout; om && ok; om &= om - 1, r++) {
+        const uint32_t o = (uint32_t)(__ffsll((long long)om) - 1);
+        uint32_t v = grow(o, lane), t = 0;
+        for (uint32_t b = 0; b < nsurv; b++) {
+            const uint32_t f = __shfl_sync(0xffffffffu, v, s_piv[warp][b]);
+            if (f) {
+                v ^= mul(f, R[b][lane]);
+                t ^= mul(f, R[b][kMaxK + lane]);
+            }
+        }
+        ok = __ballot_sync(0xffffffffu, v != 0) == 0;
+        if (ok) pl->coef[r][lane] = (uint8_t)t;  // r < 2m <= kMaxM while ok: at most m shards are absent
+    }
+    if (lane < nsurv) pl->surv[lane] = s_surv[warp][lane];
+    if (lane == 0) {
+        int n_out = 0;
+        if (ok)
+            for (unsigned long long om = hout; om; om &= om - 1, n_out++) pl->out_idx[n_out] = (uint8_t)(__ffsll((long long)om) - 1);
+        pl->key_present = hp;
+        pl->key_out = hout;
+        pl->nrows = ok ? (uint8_t)n_out : 0;
+        pl->unrecoverable = ok ? 0 : 1;
+        pl->nsurv = (uint8_t)nsurv;
+        if (q.status) q.status[s] = ok ? 0 : -4;
+    }
+}
+
+// ---- PB(k, m) encode / verify (DESIGN.md section 2.2) -----------------------------------------------------------
+// The RS(k, m) product tables, built once.  A work item is 32 columns of the a-half and the same 32 columns of the
+// b-half of every shard of a stripe, streamed through the warp's stage in two phases (a, then b) with k 1-D bulk
+// copies each (+ m stored parity halves for verify): the b-phase copy flies while the a-rows are looked up, the next
+// item's a-phase copy while the b-rows are.  Every data vector is looked up once; the piggybacks are plain XORs of
+// the staged a-vectors of each group into the b-outputs.  HBM traffic is the RS(k, m) encode's, (k+m)*L per stripe.
+// shard_len must be a multiple of 32 (16-byte aligned halves): a malformed stripe gets every mismatch bit (verify)
+// or no write at all (encode).
+template <int K, int MODE> struct PbCfg {
+    static constexpr int kK = K;
+    static constexpr TabLayout kLay = make_layout(K, 5, 2);  // RS(10,4): 8 + 2 tables, 64 KB
+    static constexpr int S = kLay.nslots;
+    static constexpr uint32_t kTabBytes = (uint32_t)kLay.ngroups * kGroupBytes;
+    static constexpr int kStageRows = K + (MODE == kModeVerify ? kRowsPerPass : 0);
+    // register budget: S x 4 words of column data + piggybacks + stored rows + accumulators (12 warps: 168 registers)
+    static constexpr int kWarps = cfg_fit_nw(K <= 8 ? 16 : 12, kTabBytes, kStageRows, false);
+    static constexpr int kThreads = 32 * kWarps;
+    static constexpr uint32_t kStageBytes = (uint32_t)kWarps * kStageRows * kStageRowBytes;
+    static constexpr uint32_t kSmem = kTabBytes + kStageBytes + kAuxBytes;
+    static_assert(K >= 1 && K <= kPbMaxK && kLay.nslots >= K, "no table layout for this k");
+    static_assert(kSmem <= kSmemLimit, "shared memory budget exceeded");
+};
+
+template <int K, int MODE>
+__global__ void __launch_bounds__(PbCfg<K, MODE>::kThreads, 1) pb_apply_kernel(const __grid_constant__ ApplyParams p)
+{
+    using CFG = PbCfg<K, MODE>;
+    constexpr int S = CFG::S;
+    constexpr int NW = CFG::kWarps;
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    uint32_t *const tab = reinterpret_cast<uint32_t *>(smem_raw);
+    const uint32_t tab_addr = (uint32_t)__cvta_generic_to_shared(smem_raw);
+    const uint32_t stage = tab_addr + CFG::kTabBytes + warp * (CFG::kStageRows * kStageRowBytes);
+    const uint32_t bar = tab_addr + CFG::kTabBytes + CFG::kStageBytes + warp * 8;
+    if (lane == 0) mbar_init(bar, 1);
+    mbar_fence_init();
+    build_tables<CFG>(tab, p.coef, K, p.rows, warp, (uint32_t)NW, K);
+    __syncthreads();
+
+    const uint32_t m = p.rows;  // 2..4: one pass
+    const int gb2 = m > 2 ? pb_group_start(K, (int)m, 2) : K, gb3 = m > 3 ? pb_group_start(K, (int)m, 3) : K;
+    const uint32_t ips = p.items_per_stripe, total = p.n * ips, step = gridDim.x * NW;
+    struct Pos {
+        const uint8_t *sp;  // chunk start in data shard 0, a-half
+        uint32_t s, col, h, rb;
+        bool valid;  // this lane has a column
+    };
+    // next item at or after `it` with columns to stream; malformed stripes are flagged (verify) and skipped
+    auto advance = [&](uint32_t &it, Pos &z) -> bool {
+        for (; it < total; it += step) {
+            const uint32_t s = it / ips, c = it - s * ips;
+            const uint32_t len = p.shard_len ? __ldg(p.shard_len + s) : p.stride;
+            if (len & 31) {
+                if (MODE == kModeVerify && c == 0 && lane == 0) atomicOr(p.mismatch + s, (1u << m) - 1);
+                continue;
+            }
+            const uint32_t nvec = len >> 5;  // 16-byte vectors per half
+            if (c * 32 >= nvec) continue;
+            z.s = s;
+            z.h = len >> 1;
+            z.col = c * 32 + lane;
+            z.valid = z.col < nvec;
+            z.rb = min(kStageRowBytes, (nvec - c * 32) * 16);
+            z.sp = p.src + (unsigned long long)s * p.src_pitch + (size_t)c * kStageRowBytes;
+            return true;
+        }
+        return false;
+    };
+    auto issue = [&](const Pos &z, uint32_t off) {
+        if (lane != 0) return;
+        const uint32_t prow = MODE == kModeVerify ? m : 0u;
+        mbar_arrive_expect_tx(bar, z.rb * ((uint32_t)K + prow));
+#pragma unroll
+        for (int j = 0; j < K; j++) bulk_g2s(stage + j * kStageRowBytes, z.sp + (size_t)j * p.stride + off, z.rb, bar);
+        for (uint32_t i = 0; i < prow; i++)
+            bulk_g2s(stage + (K + i) * kStageRowBytes, z.sp + (size_t)(K + i) * p.stride + off, z.rb, bar);
+    };
+    auto load_stored = [&](uint4 (&st)[kRowsPerPass]) {
+#pragma unroll
+        for (int i = 0; i < kRowsPerPass; i++)
+            st[i] = (MODE == kModeVerify && (uint32_t)i < m) ? lds_v4(stage + lane * 16 + (K + i) * kStageRowBytes) : make_uint4(0, 0, 0, 0);
+    };
+    auto finish = [&](const Pos &z, uint32_t off, const uint4 (&r)[4], const uint4 (&st)[kRowsPerPass], uint32_t &mm) {
+        if (!z.valid) return;
+        if (MODE == kModeEncode) {
+            uint8_t *dp = p.dst + (unsigned long long)z.s * p.dst_pitch + off + (size_t)z.col * 16;
+#pragma unroll
+            for (int i = 0; i < kRowsPerPass; i++)
+                if ((uint32_t)i < m) stg_stream(dp + (size_t)i * p.stride, r[i]);
+        } else {
+#pragma unroll
+            for (int i = 0; i < kRowsPerPass; i++)
+                if ((uint32_t)i < m && ((st[i].x ^ r[i].x) | (st[i].y ^ r[i].y) | (st[i].z ^ r[i].z) | (st[i].w ^ r[i].w))) mm |= 1u << i;
+        }
+    };
+
+    uint32_t it = blockIdx.x * NW + warp, parity = 0;
+    Pos cur;
+    bool have = advance(it, cur);
+    if (have) issue(cur, 0);
+    while (have) {
+        uint4 d[S], st[kRowsPerPass], pg[kPbMaxM - 1], r[4];
+        uint32_t mm = 0;
+        // ---- a-phase: look up the a-rows; keep the group XORs of the raw a-vectors for the piggybacks
+        mbar_wait(bar, parity);
+        parity ^= 1;
+        stage_read<CFG>(stage + lane * 16, lane, d);
+#pragma unroll
+        for (int i = 0; i < kPbMaxM - 1; i++) pg[i] = make_uint4(0, 0, 0, 0);
+#pragma unroll
+        for (int j = 0; j < K; j++) {
+            const uint4 v = lds_v4(stage + lane * 16 + j * kStageRowBytes);
+            auto acc = [&](uint4 &g) { g = make_uint4(g.x ^ v.x, g.y ^ v.y, g.z ^ v.z, g.w ^ v.w); };
+            if (j < gb2) acc(pg[0]);  // warp-uniform branches: pg stays in registers
+            else if (j < gb3) acc(pg[1]);
+            else acc(pg[2]);
+        }
+        load_stored(st);
+        stage_release();
+        issue(cur, cur.h);
+        if (cur.valid) column_compute<CFG>(d, tab_addr, lane, p.row_bytes, 0, r);
+        finish(cur, 0, r, st, mm);
+        // ---- b-phase: RS value of the b-rows, then the piggybacks into parities 1..m-1
+        mbar_wait(bar, parity);
+        parity ^= 1;
+        stage_read<CFG>(stage + lane * 16, lane, d);
+        load_stored(st);
+        stage_release();
+        Pos nx;
+        it += step;
+        const bool have_next = advance(it, nx);
+        if (have_next) issue(nx, 0);
+        if (cur.valid) {
+            column_compute<CFG>(d, tab_addr, lane, p.row_bytes, 0, r);
+#pragma unroll
+            for (int i = 1; i < kRowsPerPass; i++)
+                r[i] = make_uint4(r[i].x ^ pg[i - 1].x, r[i].y ^ pg[i - 1].y, r[i].z ^ pg[i - 1].z, r[i].w ^ pg[i - 1].w);
+        }
+        finish(cur, cur.h, r, st, mm);
+        if (MODE == kModeVerify) {
+            mm = __reduce_or_sync(0xffffffffu, mm);
+            if (mm && lane == 0) atomicOr(p.mismatch + cur.s, mm);
+        }
+        cur = nx;
+        have = have_next;
+    }
+}
+
 // ------------------------------------------------------------------ synthetic data
 // splitmix64 counter stream of SURVEY.md 8(d) (the CPU checker generates the same stream).
 __global__ void fill_random_kernel(unsigned long long *dst, size_t nwords, unsigned long long seed,
@@ -1831,13 +2113,14 @@ struct SplitParams {
     unsigned long long block_pitch;
     uint32_t stride, k, n;
     uint32_t parts;              // CTAs per block: a dispatcher batch of a dozen blocks still has to fill every SM
+    uint32_t round128;           // PB contexts: shard length ceil(len/k) rounded up to 128 bytes (DESIGN.md 2.2)
 };
 __global__ void __launch_bounds__(256) split_blocks_kernel(const __grid_constant__ SplitParams q)
 {
     for (uint32_t w = blockIdx.x; w < q.n * q.parts; w += gridDim.x) {
         const uint32_t s = w / q.parts, part = w - s * q.parts;
         const uint32_t len = __ldg(q.block_len + s);
-        const uint32_t L = (len + q.k - 1) / q.k, nvec = (L + 15) >> 4;
+        const uint32_t L0 = (len + q.k - 1) / q.k, L = q.round128 ? (L0 + 127) & ~127u : L0, nvec = (L + 15) >> 4;
         const uint8_t *src = q.blocks + (unsigned long long)s * q.block_pitch;
         uint8_t *dst = q.shards + (unsigned long long)s * q.k * q.stride;
         const uint32_t total = q.k * nvec, per = ((total + q.parts - 1) / q.parts + 255u) & ~255u;

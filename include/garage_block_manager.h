@@ -64,6 +64,12 @@ typedef struct {
                                        lost shard is resynced from the k/l other shards of its group.  Recorded in
                                        every shard file header and wire message; a shard of another code is
                                        quarantined like a k / m mismatch                                          */
+    int piggyback;                  /* 0 (default).  1: piggybacked RS PB(k, m) (garage_ec_create_piggyback, needs
+                                       2 <= m <= 4, k <= 16): resync and a degraded GET fetch only the planned
+                                       halves (ranged reads, each checked against its adler8 segment tags), k + |G_i|
+                                       halves for one lost data shard.  GARAGE_EC_E_INVALID with local_groups > 0 or
+                                       shard_sum_kind = GARAGE_EC_SUM_BLAKE2.  Recorded in the shard file header; a
+                                       shard of another code is quarantined                                       */
 } garage_bm_config;
 
 typedef struct {
@@ -81,6 +87,7 @@ typedef struct {
     uint64_t resync_shards_read;             /* shards read by resync_block's fetch branch (the read
                                                 set of garage_ec_read_set: k for RS, k/l for an LRC
                                                 local repair)                                       */
+    uint64_t resync_bytes_read;              /* bytes read by that fetch branch (PB reads half shards) */
 } garage_bm_metrics;
 
 void garage_bm_default_config(garage_bm_config *cfg);

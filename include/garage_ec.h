@@ -90,6 +90,15 @@ int garage_ec_create_with_matrix(garage_ec_ctx **out, int cuda_device, int k, in
  * reconstruct / scrub_repair / *_blocks work unchanged; reconstruct decides recoverability by rank
  * (DESIGN.md section 2), so some patterns with fewer than k present shards decode.                   */
 int garage_ec_create_lrc(garage_ec_ctx **out, int cuda_device, int k, int l, int r);
+/* Piggybacked Reed-Solomon PB(k, m) (DESIGN.md section 2.2): RS(k, m) with parity rows of `matrix_kind`, every
+ * shard cut in an a-half and a b-half; the b-half of parity i >= 1 also carries the XOR of the a-halves of data
+ * group G_i (m-1 contiguous groups).  Same storage and the same any-m-loss tolerance as RS(k, m); one lost data
+ * shard is rebuilt from k + |G_i| halves instead of 2k (PB(10,4): 0.65-0.70 of the bytes).  Every stripe's
+ * shard_len must be a multiple of 32 (garage_ec_code_shard_len gives a multiple of 128).  For a stripe where it is
+ * not, a DEVICE call rebuilds and encodes nothing (encode writes nothing for it, verify sets every mismatch bit,
+ * reconstruct reports GARAGE_EC_E_INVALID in status[]); a HOST call returns GARAGE_EC_E_INVALID before any GPU work.  Needs
+ * 1 <= k <= 16, 2 <= m <= 4; GARAGE_EC_E_INVALID otherwise, before any CUDA call.                                  */
+int garage_ec_create_piggyback(garage_ec_ctx **out, int cuda_device, int k, int m, int matrix_kind);
 void garage_ec_destroy(garage_ec_ctx *ctx);
 
 int garage_ec_matrix(const garage_ec_ctx *ctx, uint8_t *out_m_by_k); /* parity rows, row-major */
@@ -103,6 +112,17 @@ int garage_ec_code_info(const garage_ec_ctx *ctx, int *local_groups, int *global
  * present shards taken greedily in index order (DESIGN.md section 2).  GARAGE_EC_E_UNRECOVERABLE if a
  * wanted shard cannot be rebuilt.  Presenting only these shards to reconstruct rebuilds the same bytes. */
 int garage_ec_read_set(const garage_ec_ctx *ctx, const uint8_t *present, const uint8_t *want, uint8_t *read_out);
+/* PB contexts: *groups = m-1 and group_of[j] = i (1..m-1) for data shard j of G_i (k bytes, nullable); RS and LRC
+ * contexts: 0 groups, group_of[] all 0.                                                                          */
+int garage_ec_piggyback_info(const garage_ec_ctx *ctx, int *groups, uint8_t *group_of);
+/* Shard length of a block_len-byte block under this context's code: ceil(block_len / k) for RS and LRC, that
+ * rounded up to a multiple of 128 for PB.  The block-level calls frame blocks with it.  GARAGE_EC_E_INVALID if
+ * that length does not fit in 32 bits (PB(1, m) with block_len > 2^32 - 128).                                   */
+int garage_ec_code_shard_len(const garage_ec_ctx *ctx, uint32_t block_len, uint32_t *shard_len);
+/* Half-shard form of garage_ec_read_set: halves_out[i] bit 0 = read the a-half [0, shard_len/2) of shard i,
+ * bit 1 = read the b-half.  PB: rule 1 (k + |G_i| halves) or rule 2 (DESIGN.md section 2.2); RS and LRC: 3 for every
+ * shard of garage_ec_read_set.  garage_ec_read_set on a PB context reports a shard iff any of its halves is read. */
+int garage_ec_read_plan(const garage_ec_ctx *ctx, const uint8_t *present, const uint8_t *want, uint8_t *halves_out);
 const char *garage_ec_strerror(int code);
 /* detail of the last GARAGE_EC_E_CUDA on this context (thread-unsafe snapshot; "" if none) */
 const char *garage_ec_last_error(const garage_ec_ctx *ctx);
@@ -199,6 +219,12 @@ int garage_ec_set_sum_kind(garage_ec_ctx *ctx, int kind);
  * rpc_put_block: three spinning waiters are three of the ~12 CPUs a host has per GPU.                   */
 int garage_ec_set_wait_mode(garage_ec_ctx *ctx, int blocking);
 int garage_ec_shard_sum_host(int kind, const uint8_t *data, size_t len, uint8_t out32[32]);
+/* Check one half of a shard (a ranged read, half_bytes = shard_len/2 bytes, which = 0 for the a-half, 1 for the
+ * b-half) against the shard's stored adler8 tag: with shard_len % 128 == 0 a half is exactly 4 of the 8 segments.
+ * 0 if the 4 Adler-32 values match, 1 if not; GARAGE_EC_E_INVALID for GARAGE_EC_SUM_BLAKE2 (a whole-shard hash)
+ * and for shard_len % 128 != 0.                                                                                   */
+int garage_ec_check_shard_half_host(int kind, const uint8_t *half_bytes, uint32_t shard_len, int which,
+                                    const uint8_t tag32[32]);
 
 /* ---- BLOCK-LEVEL convenience (host memory only) -----------------------------------------
  * What rpc_put_block hands over is a contiguous block (bytes::Bytes), not shards.  These do

@@ -12,9 +12,10 @@
  *
  *   v1 (erasure coded)  marker "GEC1shdr" + msgpack map
  *        { "hash": bin32, "header": "Plain" | "Compressed", "k": uint, "m": uint, "index": uint,
- *          "block_len": uint, "shard_len": uint, "sum_kind": uint, "sum": bin32[, "l": uint] }
- *        "l" (LRC local groups, garage_ec_create_lrc) is present only for an LRC code (l > 0), so RS
- *        messages are byte for byte what they were before it existed.
+ *          "block_len": uint, "shard_len": uint, "sum_kind": uint, "sum": bin32[, "l": uint][, "pb": 1] }
+ *        "l" (LRC local groups, garage_ec_create_lrc) is present only for an LRC code (l > 0) and "pb" only
+ *        for a piggybacked RS code (garage_ec_create_piggyback), so RS messages are byte for byte what they
+ *        were before either existed.
  *   v0 (Previous)       the reference's replicated PutBlock payload, no marker:
  *        { "hash": bin32, "header": "Plain" | "Compressed" }
  *        migrate(v0) = the whole block as the only shard of a (k = 1, m = 0) code, index 0,
@@ -48,6 +49,7 @@ typedef struct {
     uint32_t shard_len; /* ceil(block_len / k)                                                    */
     uint8_t sum[32];    /* integrity tag of this shard's bytes                                    */
     uint8_t l;          /* LRC local groups (0 < l < m, k % l == 0); 0 = RS                        */
+    uint8_t pb;         /* 1: piggybacked RS PB(k, m) (l = 0, 2 <= m <= 4, k <= 16); 0 = not PB     */
 } garage_shard_header;
 
 /* returns the encoded length, or 0 if `cap` is too small / the header is invalid (<= 160 bytes)   */

@@ -33,6 +33,14 @@ extern "C" {
                             global_parity: *mut c_int) -> c_int;
     pub fn garage_ec_read_set(ctx: *const garage_ec_ctx, present: *const u8, want: *const u8,
                             read_out: *mut u8) -> c_int;
+    pub fn garage_ec_create_piggyback(out: *mut *mut garage_ec_ctx, cuda_device: c_int, k: c_int, m: c_int,
+                            matrix_kind: c_int) -> c_int;
+    pub fn garage_ec_piggyback_info(ctx: *const garage_ec_ctx, groups: *mut c_int, group_of: *mut u8) -> c_int;
+    pub fn garage_ec_code_shard_len(ctx: *const garage_ec_ctx, block_len: u32, shard_len: *mut u32) -> c_int;
+    pub fn garage_ec_read_plan(ctx: *const garage_ec_ctx, present: *const u8, want: *const u8,
+                            halves_out: *mut u8) -> c_int;
+    pub fn garage_ec_check_shard_half_host(kind: c_int, half_bytes: *const u8, shard_len: u32, which: c_int,
+                            tag32: *const u8) -> c_int;
     pub fn garage_ec_strerror(code: c_int) -> *const c_char;
     pub fn garage_ec_last_error(ctx: *const garage_ec_ctx) -> *const c_char;
     pub fn garage_ec_abi_version() -> c_int;

@@ -5,7 +5,9 @@ of one .so variant on the BASELINE config-2/3 workload.  Not the contract bench 
     python tools/kbench.py [--so path/to/libgarage_ec.so] [--k 10 --m 4 --blocks 4096 --iters 10]
     python tools/kbench.py --k 10 --lrc 2 --m 4              # LRC(10,2,2): l = 2 local groups, m = l + r
     python tools/kbench.py --k 10 --lrc 2 --m 4 --erasures 1 --local   # one lost data / local-parity shard
-Reconstruct bytes are (survivors read + shards rebuilt) x shard_len, the survivors being garage_ec_read_set's.
+    python tools/kbench.py --k 10 --m 4 --pb [--erasures 1 --local]     # PB(10,4) and RS(10,4), one line each
+Reconstruct bytes are (survivors read + shards rebuilt) x shard_len, the survivors being garage_ec_read_set's
+(PB: the halves of garage_ec_read_plan, shard_len / 2 each).
 """
 import argparse
 import json
@@ -25,6 +27,7 @@ ap.add_argument("--erasures", type=int, default=None)
 ap.add_argument("--same-pattern", action="store_true", help="all stripes lose the same shards")
 ap.add_argument("--lrc", type=int, default=0, help="LRC with this many local groups (m = local + global parities)")
 ap.add_argument("--local", action="store_true", help="erase only data / local-parity shards (LRC local repair)")
+ap.add_argument("--pb", action="store_true", help="piggybacked RS PB(k, m), reported next to RS(k, m)")
 ap.add_argument("--tag", default="")
 ap.add_argument("--stride-pad", type=int, default=0, help="extra bytes between shards (multiple of 16)")
 args = ap.parse_args()
@@ -42,33 +45,42 @@ k, m, n = args.k, args.m, args.blocks
 tot = k + m
 e = args.erasures if args.erasures is not None else m
 B = 1 << 20
-ec = G.GarageEc.lrc(0, k, args.lrc, m - args.lrc) if args.lrc else G.GarageEc(0, k, m)
-L = ec.shard_len(B)
-stride = ec.stride_for(L) + args.stride_pad
-shards = torch.zeros(n * tot * stride, dtype=torch.uint8, device="cuda")
-sh3 = shards.view(n, tot, stride)
-data = torch.empty(n * k * stride, dtype=torch.uint8, device="cuda")
-ec.fill_random(data, n * k * stride, 1, 0)
-data.view(n, k, stride)[:, :, L:] = 0
-lens = torch.full((n,), L, dtype=torch.int32, device="cuda")
-parity = torch.zeros(n * m * stride, dtype=torch.uint8, device="cuda")
-ec.encode(data, parity, stride, n, shard_len=lens)
-sh3[:, :k] = data.view(n, k, stride)
-sh3[:, k:] = parity.view(n, m, stride)
-orig = shards.clone()
-g = torch.Generator().manual_seed(7)
-span = k + args.lrc if args.local else tot  # --local: erase among the data and local-parity shards
-if args.same_pattern:
-    erased = torch.arange(e).repeat(n, 1)
-else:
-    erased = torch.rand(n, span, generator=g).argsort(dim=1)[:, :e]
-present = torch.ones(n, tot, dtype=torch.uint8)
-if e:
-    present.scatter_(1, erased, 0)
-pd = present.cuda()
-sh3[~pd.bool()] = 0
-status = torch.zeros(n, dtype=torch.int32, device="cuda")
-mm = torch.zeros(n, dtype=torch.int32, device="cuda")
+
+
+def measure(ec):
+    """encode / reconstruct / verify of one context on the workload: (times, shard_len, present, ok, shards)"""
+    L = ec.code_shard_len(B)
+    stride = ec.stride_for(L) + args.stride_pad
+    shards = torch.zeros(n * tot * stride, dtype=torch.uint8, device="cuda")
+    sh3 = shards.view(n, tot, stride)
+    data = torch.empty(n * k * stride, dtype=torch.uint8, device="cuda")
+    ec.fill_random(data, n * k * stride, 1, 0)
+    data.view(n, k, stride)[:, :, L:] = 0
+    lens = torch.full((n,), L, dtype=torch.int32, device="cuda")
+    parity = torch.zeros(n * m * stride, dtype=torch.uint8, device="cuda")
+    ec.encode(data, parity, stride, n, shard_len=lens)
+    sh3[:, :k] = data.view(n, k, stride)
+    sh3[:, k:] = parity.view(n, m, stride)
+    orig = shards.clone()
+    g = torch.Generator().manual_seed(7)
+    span = k + args.lrc if args.local else tot  # --local: erase among the data and local-parity shards
+    if args.same_pattern:
+        erased = torch.arange(e).repeat(n, 1)
+    else:
+        erased = torch.rand(n, span, generator=g).argsort(dim=1)[:, :e]
+    present = torch.ones(n, tot, dtype=torch.uint8)
+    if e:
+        present.scatter_(1, erased, 0)
+    pd = present.cuda()
+    sh3[~pd.bool()] = 0
+    status = torch.zeros(n, dtype=torch.int32, device="cuda")
+    mm = torch.zeros(n, dtype=torch.int32, device="cuda")
+    t_enc = timeit(lambda: ec.encode(data, parity, stride, n, shard_len=lens), ec)
+    t_dec = timeit(lambda: ec.reconstruct(shards, pd, stride, n, status=status, shard_len=lens), ec)
+    ok = torch.equal(shards, orig) and int(status.abs().sum()) == 0
+    t_ver = timeit(lambda: ec.verify(shards, mm, stride, n, shard_len=lens), ec)
+    ok = ok and int(mm.abs().sum()) == 0
+    return (t_enc, t_dec, t_ver), L, present.numpy(), ok, orig
 
 
 def timeit(fn, ctx):
@@ -85,14 +97,7 @@ def timeit(fn, ctx):
     return ms / max(cnt, 1)
 
 
-t_enc = timeit(lambda: ec.encode(data, parity, stride, n, shard_len=lens), ec)
-t_dec = timeit(lambda: ec.reconstruct(shards, pd, stride, n, status=status, shard_len=lens), ec)
-ok = torch.equal(shards, orig) and int(status.abs().sum()) == 0
-t_ver = timeit(lambda: ec.verify(shards, mm, stride, n, shard_len=lens), ec)
-ok = ok and int(mm.abs().sum()) == 0
-
-
-def copy_gbs():
+def copy_gbs(orig):
     """read+write GB/s of a plain device copy of <= 1 GiB on this GPU in this run (best of 6): the peak of the fractions"""
     cp_n = min(1 << 30, orig.numel() // 2)
     src, dst = orig[:cp_n], orig[cp_n:2 * cp_n]
@@ -118,19 +123,35 @@ def power_limit():
         return None
 
 
-peak = copy_gbs()
-enc_b = n * (k + m) * L
-pres_np = present.numpy()
-nsurv = 0
-for s in range(n):
-    rs = ec.read_set(pres_np[s])
-    nsurv += int(rs.sum()) if rs is not None else 0
-dec_b = (nsurv + n * e) * L
-print(json.dumps({
-    "tag": args.tag or (args.so or "default"), "k": k, "m": m, "lrc_local_groups": args.lrc, "blocks": n, "erasures": e,
-    "local": bool(args.local), "survivors_per_stripe": round(nsurv / n, 3), "ok": bool(ok),
-    "copy_GBs": round(peak, 1), "gpu": torch.cuda.get_device_name(0), "power_limit_W": power_limit(),
-    "encode_ms": round(t_enc, 4), "encode_GBs": round(enc_b / t_enc / 1e6, 1), "encode_frac": round(enc_b / t_enc / 1e6 / peak, 4),
-    "decode_ms": round(t_dec, 4), "decode_GBs": round(dec_b / t_dec / 1e6, 1), "decode_frac": round(dec_b / t_dec / 1e6 / peak, 4),
-    "verify_ms": round(t_ver, 4), "verify_GBs": round(enc_b / t_ver / 1e6, 1), "verify_frac": round(enc_b / t_ver / 1e6 / peak, 4),
-}))
+def report(ec, code):
+    (t_enc, t_dec, t_ver), L, pres_np, ok, orig = measure(ec)
+    peak = copy_gbs(orig)
+    del orig
+    enc_b = n * (k + m) * L
+    nsurv = 0  # shards' worth of survivor bytes read
+    for s in range(n):
+        hv = ec.read_plan(pres_np[s])
+        nsurv += sum(bin(int(x)).count("1") for x in hv) / 2 if hv is not None else 0
+    dec_b = int((nsurv + n * e) * L)
+    print(json.dumps({
+        "tag": args.tag or (args.so or "default"), "code": code, "k": k, "m": m, "lrc_local_groups": args.lrc,
+        "blocks": n, "erasures": e, "shard_len": L,
+        "local": bool(args.local), "survivors_per_stripe": round(nsurv / n, 3),
+        "survivor_bytes_per_stripe": int(nsurv / n * L), "ok": bool(ok),
+        "copy_GBs": round(peak, 1), "gpu": torch.cuda.get_device_name(0), "power_limit_W": power_limit(),
+        "encode_ms": round(t_enc, 4), "encode_GBs": round(enc_b / t_enc / 1e6, 1), "encode_frac": round(enc_b / t_enc / 1e6 / peak, 4),
+        "decode_ms": round(t_dec, 4), "decode_GBs": round(dec_b / t_dec / 1e6, 1), "decode_frac": round(dec_b / t_dec / 1e6 / peak, 4),
+        "verify_ms": round(t_ver, 4), "verify_GBs": round(enc_b / t_ver / 1e6, 1), "verify_frac": round(enc_b / t_ver / 1e6 / peak, 4),
+    }), flush=True)
+
+
+if args.pb:  # PB(k, m) next to RS(k, m) on the same workload, one line each
+    for code, make in (("RS(%d,%d)" % (k, m), lambda: G.GarageEc(0, k, m)),
+                       ("PB(%d,%d)" % (k, m), lambda: G.GarageEc.piggyback(0, k, m))):
+        with make() as ctx:
+            report(ctx, code)
+            torch.cuda.empty_cache()
+elif args.lrc:
+    report(G.GarageEc.lrc(0, k, args.lrc, m - args.lrc), "LRC(%d,%d,%d)" % (k, args.lrc, m - args.lrc))
+else:
+    report(G.GarageEc(0, k, m), "RS(%d,%d)" % (k, m))
