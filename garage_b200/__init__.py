@@ -38,7 +38,7 @@ ABI_SYMBOLS = [
     "garage_ec_set_sum_kind", "garage_ec_set_wait_mode", "garage_ec_copy_for_dma", "garage_ec_shard_sum_host", "garage_ec_reconstruct_stripes",
     "garage_ec_create_lrc", "garage_ec_code_info", "garage_ec_read_set",
     "garage_ec_create_piggyback", "garage_ec_piggyback_info", "garage_ec_code_shard_len", "garage_ec_read_plan",
-    "garage_ec_check_shard_half_host",
+    "garage_ec_check_shard_half_host", "garage_ec_transcode",
 ]
 
 
@@ -123,6 +123,7 @@ def load_library(build=True):
     L.garage_ec_code_shard_len.argtypes = [vp, u32, C.POINTER(u32)]
     L.garage_ec_read_plan.argtypes = [vp, vp, vp, vp]
     L.garage_ec_check_shard_half_host.argtypes = [i32, vp, u32, i32, vp]
+    L.garage_ec_transcode.argtypes = [vp, vp, vp, vp, vp, sz, vp, sz, vp, vp, sz, i32, vp]
     _lib = L
     return L
 
@@ -376,6 +377,17 @@ class GarageEc:
         lens = np.ascontiguousarray(block_lens, dtype=np.uint32)
         return self._check(self._L.garage_ec_decode_blocks(self._h, _ptr(shards), _ptr(present), _ptr(lens), n,
                                                            stride, C.cast(ptrs, C.c_void_p), _ptr(status)),
+                           (E_UNRECOVERABLE,))
+
+    # -- code conversion
+    def transcode(self, src, src_shards, block_lens, src_stride, dst_shards, dst_stride, n, src_present=None,
+                  dst_sums=None, status=None):
+        """garage_ec_transcode: rewrite n blocks stored under `src` (a GarageEc, or None for whole blocks
+        `src_stride` apart) as this context's code; returns 0 or E_UNRECOVERABLE (HOST mode)"""
+        kind, st = self._stream(src_shards, dst_shards)
+        return self._check(self._L.garage_ec_transcode(self._h, src._h if src is not None else None, _ptr(src_shards),
+                                                       _ptr(src_present), _ptr(block_lens), src_stride, _ptr(dst_shards),
+                                                       dst_stride, _ptr(dst_sums), _ptr(status), n, kind, st),
                            (E_UNRECOVERABLE,))
 
     # -- harness utilities

@@ -587,7 +587,7 @@ bool pb_lens_ok(const garage_ec_ctx *ctx, const uint32_t *shard_len, size_t stri
 // 64-bit: a PB length that does not fit in 32 bits is larger than any stride, so the stride checks reject it
 uint64_t code_shard_len(const garage_ec_ctx *ctx, uint32_t block_len)
 {
-    return ctx->pb ? pb_shard_len(block_len, ctx->k) : garage_ec_shard_len(block_len, ctx->k);
+    return ::garage_ec::code_shard_len(block_len, ctx->k, ctx->pb);
 }
 
 // ---- batched async copies ---------------------------------------------------------------
@@ -1967,6 +1967,207 @@ int garage_ec_decode_blocks(garage_ec_ctx *ctx, const uint8_t *shards, const uin
         }
     }
     return any_bad ? GARAGE_EC_E_UNRECOVERABLE : GARAGE_EC_OK;
+}
+
+// --------------------------------------------------------------------------- TRANSCODE
+}  // extern "C"
+namespace {
+
+// device scratch of run_transcode for n stripes: src_len | dst_len | geo | status (caller passed none) | want | plan
+struct TranscodeScratch {
+    size_t o_src_len, o_dst_len, o_geo, o_status, o_want, o_plan, bytes;
+    TranscodeScratch(size_t n, size_t src_tot, bool degraded)
+    {
+        const size_t a = align_up(n * 4, 16);
+        o_src_len = 0;
+        o_dst_len = a;
+        o_geo = 2 * a;
+        o_status = 3 * a;
+        o_want = 4 * a;
+        o_plan = o_want + (degraded ? align_up(n * src_tot, 16) : 0);
+        bytes = o_plan + (degraded ? plan_scratch_bytes(n) : 0);
+    }
+};
+
+// Device-resident transcode of n stripes (DESIGN.md 2.3): lengths, the source reconstruct of absent data shards (only
+// when `present` is given), the reframe into dst's data shards, dst's encode in place and dst's tags.  src == NULL:
+// whole blocks, `s_stride` apart.  status: device, nullable.
+int run_transcode(garage_ec_ctx *dst, garage_ec_ctx *src, uint8_t *s_sh, size_t s_stride, const uint8_t *present,
+                  const uint32_t *block_len, uint8_t *d_sh, size_t d_stride, uint8_t *sums, int32_t *status, size_t n,
+                  uint8_t *scratch, cudaStream_t st)
+{
+    const size_t s_tot = src ? src->k + src->m : 1, d_tot = dst->k + dst->m;
+    const TranscodeScratch L(n, s_tot, present != nullptr);
+    TranscodeParams q;
+    memset(&q, 0, sizeof(q));
+    q.src = s_sh;
+    q.block_len = block_len;
+    q.dst = d_sh;
+    q.src_len = reinterpret_cast<uint32_t *>(scratch + L.o_src_len);
+    q.dst_len = reinterpret_cast<uint32_t *>(scratch + L.o_dst_len);
+    q.geo = reinterpret_cast<int32_t *>(scratch + L.o_geo);
+    q.status = status ? status : reinterpret_cast<int32_t *>(scratch + L.o_status);
+    q.rec_status = present ? q.status : nullptr;
+    q.src_pitch = s_tot * s_stride;
+    q.dst_pitch = d_tot * d_stride;
+    q.src_stride = (uint32_t)s_stride;
+    q.dst_stride = (uint32_t)d_stride;
+    q.ks = src ? (uint32_t)src->k : 1u;
+    q.kd = (uint32_t)dst->k;
+    q.src_whole = src ? 0u : 1u;
+    q.src_pb = src && src->pb ? 1u : 0u;
+    q.dst_pb = dst->pb ? 1u : 0u;
+    q.n = (uint32_t)n;
+    q.parts = (uint32_t)std::max<size_t>(1, std::min<size_t>(64, ((size_t)dst->sm_count * 4 + n - 1) / n));
+    transcode_lens_kernel<<<(unsigned)std::min<size_t>((n + 255) / 256, (size_t)dst->sm_count * 4), 256, 0, st>>>(q);
+    dst->launches.fetch_add(1, std::memory_order_relaxed);
+    CU_TRY(dst, cudaGetLastError());
+    if (present) {
+        // absent source data shards first, by the source code's own plan; the plan kernel skips intact stripes
+        uint8_t *want = scratch + L.o_want;
+        CU_TRY(dst, cudaMemsetAsync(want, 0, n * s_tot, st));
+        CU_TRY(dst, cudaMemset2DAsync(want, s_tot, 1, q.ks, n, st));
+        StripePlan *plan = reinterpret_cast<StripePlan *>(scratch + L.o_plan);
+        uint32_t *counter = reinterpret_cast<uint32_t *>(scratch + L.o_plan + n * sizeof(StripePlan));
+        int rc = run_reconstruct(src, s_sh, present, want, q.status, q.src_len, s_stride, n, plan, counter, st);
+        if (rc) return rc;
+    }
+    {
+        TimedLaunch tl(dst, st);
+        transcode_reframe_kernel<<<(unsigned)std::min<size_t>(n * q.parts, (size_t)dst->sm_count * 8), 256, 0, st>>>(q);
+        dst->launches.fetch_add(1, std::memory_order_relaxed);
+        CU_TRY(dst, cudaGetLastError());
+    }
+    int rc = run_uniform(dst, kModeEncode, d_sh, q.dst_pitch, d_sh + (size_t)dst->k * d_stride, q.dst_pitch, nullptr, q.dst_len,
+                         d_stride, n, st);
+    if (rc) return rc;
+    if (sums) return run_sums(dst, d_sh, nullptr, q.dst_len, d_stride, n * d_tot, (int)d_tot, sums, nullptr, st);
+    return GARAGE_EC_OK;
+}
+
+// HOST mode: chunks through the lanes.  Uploads the present source data shards and, for a stripe with an absent data
+// shard, the pieces of the source read plan; downloads the destination shards (and tags) of the stripes that
+// converted.  src_shards is never written.
+int transcode_host(garage_ec_ctx *dst, garage_ec_ctx *src, const uint8_t *src_shards, const uint8_t *src_present,
+                   const uint32_t *block_len, size_t s_stride, uint8_t *dst_shards, size_t d_stride, uint8_t *dst_sums,
+                   int32_t *status, size_t n)
+{
+    const size_t ks = src ? src->k : 1, s_tot = src ? src->k + src->m : 1, d_tot = dst->k + dst->m;
+    std::vector<uint64_t> reads(n, 0);
+    std::vector<uint8_t> ok(n, 1), degraded(n, 0);
+    std::vector<uint8_t> want_data(s_tot, 0);
+    for (size_t i = 0; i < ks; i++) want_data[i] = 1;
+    for (size_t s = 0; s < n && src_present; s++) {
+        const uint8_t *pr = src_present + s * s_tot;
+        for (size_t j = 0; j < ks; j++) degraded[s] |= !pr[j];
+        if (degraded[s]) ok[s] = stripe_read_plan(src, pr, want_data.data(), &reads[s]);
+    }
+    auto src_len = [&](size_t s) -> size_t { return src ? (size_t)code_shard_len(src, block_len[s]) : block_len[s]; };
+    size_t cs = kHostChunkBytes / (s_tot * s_stride + d_tot * d_stride);
+    if (cs < 1) cs = 1;
+    if (cs > n) cs = n;
+    const size_t o_len = 0, o_present = align_up(cs * 4, 16), o_status = o_present + align_up(cs * s_tot, 16);
+    const size_t o_sums = o_status + align_up(cs * 4, 16), o_scr = o_sums + (dst_sums ? cs * d_tot * 32 : 0);
+    const TranscodeScratch scr(cs, s_tot, src_present != nullptr);
+    const size_t d_src_b = cs * s_tot * s_stride;
+    // copy lists are declared before the lane lease: they outlive its stream work
+    CopyBatch up, down;
+    LEASE_LANES(dst, lanes);
+    for (HostLane &Ln : lanes.set->lanes) {
+        int rc = lane_reserve(dst, Ln, d_src_b + cs * d_tot * d_stride, o_scr + scr.bytes);
+        if (rc) return rc;
+    }
+    size_t c = 0;
+    for (size_t s0 = 0; s0 < n; s0 += cs, c++) {
+        HostLane &Ln = lanes[c % kHostLanes];
+        const size_t cnt = n - s0 < cs ? n - s0 : cs;
+        uint8_t *d_src = Ln.d_buf, *d_dst = Ln.d_buf + d_src_b;
+        bool any_degraded = false;
+        for (size_t s = s0; s < s0 + cnt; s++) {
+            if (!ok[s]) continue;
+            any_degraded |= degraded[s] != 0;
+            const size_t Ls = src_len(s), q = s - s0;
+            for (size_t i = 0; i < s_tot; i++) {
+                const uint8_t *from = src_shards + (s * s_tot + i) * s_stride;
+                uint8_t *to = d_src + (q * s_tot + i) * s_stride;
+                if (i < ks) {
+                    if (!src_present || src_present[s * s_tot + i]) up.add(to, from, align_up(Ls, 16));
+                } else if (degraded[s]) {
+                    for_each_read_piece(src, reads[s], i, Ls, align_up(Ls, 16),
+                                        [&](size_t off, size_t bytes) { up.add(to + off, from + off, bytes); });
+                }
+            }
+        }
+        int rc = up.flush(dst, cudaMemcpyHostToDevice, Ln.stream);
+        if (rc) return rc;
+        CU_TRY(dst, cudaMemcpyAsync(Ln.d_small + o_len, block_len + s0, cnt * 4, cudaMemcpyHostToDevice, Ln.stream));
+        const uint8_t *d_present = nullptr;
+        if (any_degraded) {
+            CU_TRY(dst, cudaMemcpyAsync(Ln.d_small + o_present, src_present + s0 * s_tot, cnt * s_tot, cudaMemcpyHostToDevice,
+                                        Ln.stream));
+            d_present = Ln.d_small + o_present;
+        }
+        rc = run_transcode(dst, src, d_src, s_stride, d_present, reinterpret_cast<const uint32_t *>(Ln.d_small + o_len), d_dst,
+                           d_stride, dst_sums ? Ln.d_small + o_sums : nullptr,
+                           reinterpret_cast<int32_t *>(Ln.d_small + o_status), cnt, Ln.d_small + o_scr, Ln.stream);
+        if (rc) return rc;
+        for (size_t s = s0; s < s0 + cnt; s++) {
+            if (!ok[s]) continue;
+            const size_t bytes = align_up(code_shard_len(dst, block_len[s]), 16), q = s - s0;
+            for (size_t i = 0; i < d_tot; i++)
+                down.add(dst_shards + (s * d_tot + i) * d_stride, d_dst + (q * d_tot + i) * d_stride, bytes);
+            if (dst_sums) down.add(dst_sums + s * d_tot * 32, Ln.d_small + o_sums + q * d_tot * 32, d_tot * 32);
+        }
+        rc = down.flush(dst, cudaMemcpyDeviceToHost, Ln.stream);
+        if (rc) return rc;
+    }
+    for (HostLane &Ln : lanes.set->lanes) CU_TRY(dst, lane_wait(dst, Ln));
+    bool any_bad = false;
+    for (size_t s = 0; s < n; s++) {
+        if (status) status[s] = ok[s] ? 0 : GARAGE_EC_E_UNRECOVERABLE;
+        any_bad |= !ok[s];
+    }
+    return any_bad ? GARAGE_EC_E_UNRECOVERABLE : GARAGE_EC_OK;
+}
+
+}  // namespace
+extern "C" {
+
+int garage_ec_transcode(garage_ec_ctx *dst, garage_ec_ctx *src, uint8_t *src_shards, const uint8_t *src_present,
+                        const uint32_t *block_len, size_t src_stride, uint8_t *dst_shards, size_t dst_stride,
+                        uint8_t *dst_sums, int32_t *status, size_t n_stripes, int mem_kind, void *cuda_stream)
+{
+    if (!dst || (mem_kind != GARAGE_EC_MEM_HOST && mem_kind != GARAGE_EC_MEM_DEVICE)) return GARAGE_EC_E_INVALID;
+    if (src && src->device != dst->device) return GARAGE_EC_E_INVALID;
+    if (!src && src_present) return GARAGE_EC_E_INVALID;
+    int rc = check_geometry(dst, dst_stride, n_stripes, dst->k + dst->m);
+    if (rc) return rc;
+    rc = src ? check_geometry(src, src_stride, n_stripes, src->k + src->m) : check_geometry(dst, src_stride, n_stripes, 1);
+    if (rc) return rc;
+    if (n_stripes == 0) return GARAGE_EC_OK;
+    if (!src_shards || !block_len || !dst_shards) return GARAGE_EC_E_INVALID;
+    if (!aligned16(src_shards) || !aligned16(dst_shards)) return GARAGE_EC_E_ALIGN;
+    if (dst_sums && n_stripes * (size_t)(dst->k + dst->m) > 0xffffffffull) return GARAGE_EC_E_INVALID;
+    if (mem_kind == GARAGE_EC_MEM_HOST) {
+        for (size_t s = 0; s < n_stripes; s++) {
+            const uint64_t ls = src ? code_shard_len(src, block_len[s]) : block_len[s];
+            if (ls > src_stride || code_shard_len(dst, block_len[s]) > dst_stride) return GARAGE_EC_E_INVALID;
+        }
+        CU_TRY(dst, cudaSetDevice(dst->device));
+        return transcode_host(dst, src, src_shards, src_present, block_len, src_stride, dst_shards, dst_stride, dst_sums,
+                              status, n_stripes);
+    }
+    CU_TRY(dst, cudaSetDevice(dst->device));
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    const TranscodeScratch scr(n_stripes, src ? src->k + src->m : 1, src_present != nullptr);
+    void *scratch = nullptr;
+    CU_TRY(dst, dst->pool ? cudaMallocFromPoolAsync(&scratch, scr.bytes, dst->pool, st) : cudaMallocAsync(&scratch, scr.bytes, st));
+    rc = run_transcode(dst, src, src_shards, src_stride, src_present, block_len, dst_shards, dst_stride, dst_sums, status,
+                       n_stripes, reinterpret_cast<uint8_t *>(scratch), st);
+    cudaError_t e = cudaFreeAsync(scratch, st);
+    if (rc) return rc;
+    if (e != cudaSuccess) return set_cuda_error(dst, e, "cudaFreeAsync");
+    return GARAGE_EC_OK;
 }
 
 // ---- test hook -------------------------------------------------------------------------------

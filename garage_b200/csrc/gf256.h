@@ -192,11 +192,13 @@ GEC_GF_HD inline int pb_group_of(int k, int m, int j)
 }
 // shard length of a block: ceil(block_len / k) rounded up to 128 bytes, so that both halves are 16-byte aligned and
 // each half is exactly 4 of the 8 adler8 segments.  64-bit: with k = 1 a block_len near 2^32 rounds past 32 bits.
-inline uint64_t pb_shard_len(uint32_t block_len, int k)
+// code_shard_len: the same for every code -- ceil(block_len / k), PB rounded as above (host and device share it).
+GEC_GF_HD inline uint64_t code_shard_len(uint32_t block_len, int k, bool pb)
 {
     const uint64_t L = ((uint64_t)block_len + (unsigned)k - 1) / (unsigned)k;
-    return (L + 127) / 128 * 128;
+    return pb ? (L + 127) / 128 * 128 : L;
 }
+inline uint64_t pb_shard_len(uint32_t block_len, int k) { return code_shard_len(block_len, k, true); }
 // Generator over half-symbols: row q = 2*shard + half (0..2(k+m)), column c = 2*data + half (0..2k).
 GEC_GF_HD inline uint8_t pb_grow(int k, int m, const uint8_t *P, int q, int c)
 {

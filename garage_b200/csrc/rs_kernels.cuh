@@ -50,6 +50,7 @@
 
 #include <type_traits>
 
+#include "../../include/garage_ec.h"  // GARAGE_EC_E_* status codes
 #include "blake2b.h"
 #include "gf256.h"
 
@@ -2148,6 +2149,103 @@ __global__ void __launch_bounds__(256) split_blocks_kernel(const __grid_constant
     }
 }
 
+// ------------------------------------------------------------------ code conversion (DESIGN.md 2.3)
+// A block stored under source code S is the first block_len bytes of S's data shards 0..k_s-1 concatenated (a whole
+// block: k_s = 1, L_s = block_len).  The transcode to code D writes D's data shard j = block bytes [j*L_d, (j+1)*L_d),
+// zero padded, gathered straight from the source data shards, and D's parities.
+struct TranscodeParams {
+    const uint8_t *src;          // source stripe s at src + s*src_pitch, data shard i at + i*src_stride
+    const uint32_t *block_len;   // per stripe
+    uint8_t *dst;                // destination shard i of stripe s at dst + s*dst_pitch + i*dst_stride
+    uint32_t *src_len, *dst_len; // per stripe: L_s, L_d (0 for a stripe that is skipped)
+    int32_t *geo;                // per stripe: GARAGE_EC_E_INVALID if a length does not fit its stride, else 0
+    int32_t *status;             // per stripe, out
+    const int32_t *rec_status;   // nullable: verdict of the source reconstruct (== status when set)
+    unsigned long long src_pitch, dst_pitch;
+    uint32_t src_stride, dst_stride;
+    uint32_t ks, kd;             // data shards of the source (1: whole blocks) and destination codes
+    uint32_t src_whole;          // 1: the source is the block itself, L_s = block_len
+    uint32_t src_pb, dst_pb;     // PB codes: shard lengths rounded up to 128 bytes
+    uint32_t n, parts;           // parts: reframe CTAs per stripe
+};
+// per-stripe lengths and their geometry verdict; runs before the source reconstruct, which needs L_s
+__global__ void __launch_bounds__(256) transcode_lens_kernel(const __grid_constant__ TranscodeParams q)
+{
+    for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < q.n; s += gridDim.x * blockDim.x) {
+        const uint32_t len = __ldg(q.block_len + s);
+        const uint64_t ls = q.src_whole ? len : code_shard_len(len, (int)q.ks, q.src_pb != 0);
+        const uint64_t ld = code_shard_len(len, (int)q.kd, q.dst_pb != 0);
+        const bool bad = ls > q.src_stride || ld > q.dst_stride;
+        q.geo[s] = bad ? GARAGE_EC_E_INVALID : 0;
+        q.src_len[s] = bad ? 0u : (uint32_t)ls;  // a reconstruct of an empty stripe touches nothing
+        q.dst_len[s] = bad ? 0u : (uint32_t)ld;
+        if (!q.rec_status) q.status[s] = q.geo[s];
+    }
+}
+// Stripe s failed (geometry, or an unrecoverable source): true, and one caller (`first`) records it -- the status, and
+// dst_len = 0, so that the encode and tag launches write nothing for the stripe.  No caller reads dst_len of a failed
+// stripe.
+__device__ __forceinline__ bool transcode_failed(const TranscodeParams &q, uint32_t s, bool first)
+{
+    const int32_t geo = q.geo[s];
+    const int32_t verdict = geo ? geo : (q.rec_status ? q.rec_status[s] : 0);
+    if (verdict && first) {
+        if (geo) q.status[s] = geo;  // else status already holds the reconstruct's verdict
+        q.dst_len[s] = 0;
+    }
+    return verdict != 0;
+}
+// Vector v of destination data row j of one stripe (src = the stripe's source base).  A vector inside one source
+// piece comes from five aligned 32-bit loads and funnel shifts (as in split_blocks_kernel); one that crosses a piece
+// boundary or ends the row is gathered byte by byte.
+__device__ __forceinline__ uint4 transcode_gather(const uint8_t *src, uint32_t src_stride, uint32_t Ls, uint32_t Ld,
+                                                  uint32_t len, uint32_t j, uint32_t v)
+{
+    const uint64_t pos = (uint64_t)j * Ld + v * 16;  // block offset of the vector's first byte
+    uint32_t nvalid = min(16u, Ld - v * 16);
+    nvalid = pos >= len ? 0 : (uint32_t)min((uint64_t)nvalid, len - pos);
+    if (!nvalid) return make_uint4(0, 0, 0, 0);
+    const uint32_t p32 = (uint32_t)pos;  // < block_len: 32-bit division
+    const uint32_t i = p32 / Ls, off = p32 - i * Ls;
+    if (nvalid == 16 && off + 16 <= Ls) {
+        // words a .. a+16 stay inside roundup4(off + 16) <= roundup16(L_s): readable
+        const uint32_t a = off & ~3u, sh = (off & 3u) * 8;
+        const uint32_t *wp = reinterpret_cast<const uint32_t *>(src + (size_t)i * src_stride + a);
+        const uint32_t w0 = __ldg(wp), w1 = __ldg(wp + 1), w2 = __ldg(wp + 2), w3 = __ldg(wp + 3), w4 = sh ? __ldg(wp + 4) : 0;
+        return make_uint4(__funnelshift_r(w0, w1, sh), __funnelshift_r(w1, w2, sh), __funnelshift_r(w2, w3, sh),
+                          __funnelshift_r(w3, w4, sh));
+    }
+    uint32_t wv[4] = {0, 0, 0, 0};
+#pragma unroll
+    for (int b = 0; b < 16; b++) {
+        if ((uint32_t)b < nvalid) {
+            const uint32_t ob = p32 + b;
+            const uint32_t ib = ob / Ls, offb = ob - ib * Ls;
+            wv[b >> 2] |= (uint32_t)src[(size_t)ib * src_stride + offb] << (8 * (b & 3));
+        }
+    }
+    return make_uint4(wv[0], wv[1], wv[2], wv[3]);
+}
+// The destination data shards, one vector per thread; the destination's own encode follows (DESIGN.md 4.5: a one-pass
+// kernel that also looked the gathered vectors up in the parity tables measured no faster).
+__global__ void __launch_bounds__(256) transcode_reframe_kernel(const __grid_constant__ TranscodeParams q)
+{
+    for (uint32_t w = blockIdx.x; w < q.n * q.parts; w += gridDim.x) {
+        const uint32_t s = w / q.parts, part = w - s * q.parts;
+        if (transcode_failed(q, s, part == 0 && threadIdx.x == 0)) continue;
+        const uint32_t len = __ldg(q.block_len + s), Ls = q.src_len[s], Ld = q.dst_len[s], nvec = (Ld + 15) >> 4;
+        const uint8_t *src = q.src + (unsigned long long)s * q.src_pitch;
+        uint8_t *dst = q.dst + (unsigned long long)s * q.dst_pitch;
+        const uint32_t total = q.kd * nvec, per = ((total + q.parts - 1) / q.parts + 255u) & ~255u;
+        const uint32_t lo = part * per, hi = min(total, lo + per);
+#pragma unroll 4
+        for (uint32_t idx = lo + threadIdx.x; idx < hi; idx += 256) {
+            const uint32_t j = idx / nvec, v = idx - j * nvec;
+            *reinterpret_cast<uint4 *>(dst + (size_t)j * q.dst_stride + (size_t)v * 16) =
+                transcode_gather(src, q.src_stride, Ls, Ld, len, j, v);
+        }
+    }
+}
 // ---- fast per-shard integrity tag: 8 x Adler-32 ("adler8") -----------------------------------
 // BLAKE2b is compute-bound on CUDA cores (~20 integer instructions per byte: at most ~1.3 TB/s,
 // round 1 measured 0.45-0.6 TB/s), which capped the scrub sweep at 7 % of HBM bandwidth.  Scrub

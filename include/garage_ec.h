@@ -250,6 +250,31 @@ int garage_ec_decode_blocks(garage_ec_ctx *ctx, const uint8_t *shards, const uin
                             const uint32_t *block_len, size_t n_blocks, size_t stride,
                             uint8_t *const *blocks_out, int32_t *status);
 
+/* ---- TRANSCODE -- changing a cluster's code (DESIGN.md section 2.3): resync after an `erasure_coding` config change
+ * rewrites every block stored under an old code -- a whole-block replica (src = NULL), RS, LRC or PB -- under the
+ * configured one.  A block under code S is the first block_len bytes of S's data shards concatenated; the output is
+ * exactly dst's encode of that block: data shard j = block bytes [j*L_d, (j+1)*L_d) zero padded, L_d =
+ * garage_ec_code_shard_len(dst, block_len), and dst's own parities.
+ *   src_shards  : shard layout of `src` (stride src_stride); src = NULL: block s at s*src_stride
+ *   src_present : n*(k_s+m_s) bytes, nullable (= all present); must be NULL when src = NULL.  A stripe with an absent
+ *                 data shard first has it rebuilt by src's own plan (garage_ec_read_plan: only those pieces are read)
+ *   block_len   : n values
+ *   dst_shards  : shard layout of `dst` (stride dst_stride).  Nothing is written past roundup16(L_d) of a shard
+ *   dst_sums    : nullable; (k_d+m_d)*32 bytes per stripe, dst's tag kind (garage_ec_set_sum_kind) of every shard
+ *   status      : n int32, nullable: 0; GARAGE_EC_E_UNRECOVERABLE (the source stripe cannot be rebuilt: its destination
+ *                 shards are not written); GARAGE_EC_E_INVALID (PB geometry, DESIGN.md section 2.2, or -- DEVICE mode --
+ *                 a length that does not fit its stride: nothing written)
+ * Strides follow the shard-layout rules of each code.  GARAGE_EC_E_INVALID before any CUDA call for dst = NULL,
+ * contexts on different devices, a stride too small for a block (HOST mode) or a length past 32 bits.
+ * DEVICE: all pointers device memory of dst's GPU; enqueues only kernels and stream-ordered allocations on `stream`
+ * (capturable in a CUDA graph).  The absent source data shards of src_shards are OVERWRITTEN with their rebuilt bytes,
+ * as garage_ec_reconstruct does.  dst_sums of a failed stripe is unspecified.
+ * HOST: all pointers host; uploads only what the source plan reads, never writes src_shards, downloads the destination
+ * shards and tags of the stripes that converted; returns GARAGE_EC_E_UNRECOVERABLE if any stripe failed.           */
+int garage_ec_transcode(garage_ec_ctx *dst, garage_ec_ctx *src, uint8_t *src_shards, const uint8_t *src_present,
+                        const uint32_t *block_len, size_t src_stride, uint8_t *dst_shards, size_t dst_stride,
+                        uint8_t *dst_sums, int32_t *status, size_t n_stripes, int mem_kind, void *cuda_stream);
+
 /* ---- utilities used by the harness ------------------------------------------------------
  * device-side synthetic data (same splitmix64 counter stream as the oracle's
  * generator): fills dst[0..len) (device) with stream bytes at `offset`

@@ -61,6 +61,10 @@ extern "C" {
     pub fn garage_ec_decode_blocks(ctx: *mut garage_ec_ctx, shards: *const u8, present: *const u8,
                             block_len: *const u32, n_blocks: usize, stride: usize,
                             blocks_out: *const *mut u8, status: *mut i32) -> c_int;
+    pub fn garage_ec_transcode(dst: *mut garage_ec_ctx, src: *mut garage_ec_ctx, src_shards: *mut u8,
+                            src_present: *const u8, block_len: *const u32, src_stride: usize, dst_shards: *mut u8,
+                            dst_stride: usize, dst_sums: *mut u8, status: *mut i32, n_stripes: usize,
+                            mem_kind: c_int, stream: *mut c_void) -> c_int;
     pub fn garage_ec_encode_blocks_with_sums(ctx: *mut garage_ec_ctx, blocks: *const *const u8,
                             block_len: *const u32, n_blocks: usize, parity_out: *mut u8,
                             sums_out: *mut u8, stride: usize) -> c_int;

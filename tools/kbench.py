@@ -6,6 +6,7 @@ of one .so variant on the BASELINE config-2/3 workload.  Not the contract bench 
     python tools/kbench.py --k 10 --lrc 2 --m 4              # LRC(10,2,2): l = 2 local groups, m = l + r
     python tools/kbench.py --k 10 --lrc 2 --m 4 --erasures 1 --local   # one lost data / local-parity shard
     python tools/kbench.py --k 10 --m 4 --pb [--erasures 1 --local]     # PB(10,4) and RS(10,4), one line each
+    python tools/kbench.py --transcode 6,3:10,4 [--rounds 3]  # code conversion; also lrc:10,2,2  pb:10,4  rep
 Reconstruct bytes are (survivors read + shards rebuilt) x shard_len, the survivors being garage_ec_read_set's
 (PB: the halves of garage_ec_read_plan, shard_len / 2 each).
 """
@@ -28,6 +29,8 @@ ap.add_argument("--same-pattern", action="store_true", help="all stripes lose th
 ap.add_argument("--lrc", type=int, default=0, help="LRC with this many local groups (m = local + global parities)")
 ap.add_argument("--local", action="store_true", help="erase only data / local-parity shards (LRC local repair)")
 ap.add_argument("--pb", action="store_true", help="piggybacked RS PB(k, m), reported next to RS(k, m)")
+ap.add_argument("--transcode", default=None, help="SRC:DST codes: k,m | lrc:k,l,r | pb:k,m | rep (whole blocks)")
+ap.add_argument("--rounds", type=int, default=3, help="--transcode: alternating rounds of the compared paths")
 ap.add_argument("--tag", default="")
 ap.add_argument("--stride-pad", type=int, default=0, help="extra bytes between shards (multiple of 16)")
 args = ap.parse_args()
@@ -145,7 +148,87 @@ def report(ec, code):
     }), flush=True)
 
 
-if args.pb:  # PB(k, m) next to RS(k, m) on the same workload, one line each
+def parse_code(t):
+    if t == "rep":
+        return None, "rep", 1, 0
+    kind, _, nums = t.rpartition(":")
+    v = [int(x) for x in nums.split(",")]
+    if kind == "lrc":
+        return G.GarageEc.lrc(0, *v), "LRC(%d,%d,%d)" % tuple(v), v[0], v[1] + v[2]
+    if kind == "pb":
+        return G.GarageEc.piggyback(0, *v), "PB(%d,%d)" % tuple(v), v[0], v[1]
+    return G.GarageEc(0, *v), "RS(%d,%d)" % tuple(v), v[0], v[1]
+
+
+def event_ms(fn):
+    """mean device time of fn over args.iters calls, after 3 warm-up calls"""
+    for _ in range(3):
+        fn()
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    torch.cuda.synchronize()
+    a.record()
+    for _ in range(args.iters):
+        fn()
+    b.record()
+    torch.cuda.synchronize()
+    return a.elapsed_time(b) / args.iters
+
+
+def transcode_bench():
+    """garage_ec_transcode (reframe + the destination's encode) against torch reframe + garage_ec_encode, same batch,
+    alternating; algorithmic bytes = k_s*L_s read + (k_d+m_d)*L_d written per block"""
+    toks, codes = args.transcode.split(":"), []
+    while toks:  # "lrc" / "pb" take the next token as their numbers
+        t = toks.pop(0)
+        codes.append(t + ":" + toks.pop(0) if t in ("lrc", "pb") else t)
+    (src, sname, ks, ms), (dst, dname, kd, md) = (parse_code(t) for t in codes)
+    Ls = src.code_shard_len(B) if src else B
+    Ld = dst.code_shard_len(B)
+    ss, ds = (src.stride_for(Ls) if src else (B + 15) // 16 * 16), dst.stride_for(Ld)
+    st, dt = ks + ms, kd + md
+    sh = torch.zeros((n, st, ss), dtype=torch.uint8, device="cuda")
+    fill = torch.empty(n * ks * ss, dtype=torch.uint8, device="cuda")
+    dst.fill_random(fill, fill.numel(), 3, 0)
+    sh[:, :ks] = fill.view(n, ks, ss)
+    del fill
+    sh[:, :ks, Ls:] = 0
+    out = torch.zeros((n, dt, ds), dtype=torch.uint8, device="cuda")
+    bl = torch.full((n,), B, dtype=torch.int32, device="cuda")
+    data = torch.zeros((n, kd, ds), dtype=torch.uint8, device="cuda")
+    par = torch.zeros((n, md, ds), dtype=torch.uint8, device="cuda")
+    flat = torch.zeros((n, kd * Ld), dtype=torch.uint8, device="cuda")
+    lens = torch.full((n,), Ld, dtype=torch.int32, device="cuda")
+
+    def transcode():
+        dst.transcode(src, sh.view(-1), bl, ss, out.view(-1), ds, n)
+
+    def torch_encode():
+        flat[:, :B] = sh[:, :ks, :Ls].reshape(n, ks * Ls)[:, :B]
+        data[:, :, :Ld] = flat.view(n, kd, Ld)
+        dst.encode(data.view(-1), par.view(-1), ds, n, shard_len=lens)
+
+    transcode()
+    torch_encode()
+    torch.cuda.synchronize()
+    ok = torch.equal(out[:, :kd, :Ld], data[:, :, :Ld]) and torch.equal(out[:, kd:, :Ld], par[:, :, :Ld])
+    peak = copy_gbs(out.view(-1))
+    alg = n * (ks * Ls + dt * Ld)
+    res = {"transcode_ms": [], "torch_reframe_encode_ms": []}
+    for _ in range(args.rounds):
+        res["transcode_ms"].append(round(event_ms(transcode), 4))
+        res["torch_reframe_encode_ms"].append(round(event_ms(torch_encode), 4))
+    best = {key: min(v) for key, v in res.items()}
+    print(json.dumps({
+        "tag": args.tag or (args.so or "default"), "transcode": "%s->%s" % (sname, dname), "blocks": n, "block_len": B,
+        "ok": bool(ok), "alg_bytes": alg, "copy_GBs": round(peak, 1), "gpu": torch.cuda.get_device_name(0),
+        "power_limit_W": power_limit(), **res,
+        **{key.replace("_ms", "_frac"): round(alg / v / 1e6 / peak, 4) for key, v in best.items()},
+    }), flush=True)
+
+
+if args.transcode:
+    transcode_bench()
+elif args.pb:  # PB(k, m) next to RS(k, m) on the same workload, one line each
     for code, make in (("RS(%d,%d)" % (k, m), lambda: G.GarageEc(0, k, m)),
                        ("PB(%d,%d)" % (k, m), lambda: G.GarageEc.piggyback(0, k, m))):
         with make() as ctx:
