@@ -492,18 +492,15 @@ int run_reconstruct(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *present,
     q.k = (uint32_t)ctx->k;
     q.m = (uint32_t)ctx->m;
     q.l = (uint32_t)ctx->l;
+    q.pb = ctx->pb ? 1u : 0u;
     q.present_is_bad = present_is_bad ? 1u : 0u;
     q.shard_len = shard_len;
     q.stride = (uint32_t)stride;
     memcpy(q.P, ctx->P, (size_t)ctx->k * ctx->m);
-    const unsigned blocks = (unsigned)((n + kPlanWarps - 1) / kPlanWarps);
-    if (ctx->pb) pb_plan_kernel<<<blocks, kPlanWarps * 32, 0, st>>>(q);
-    else if (ctx->l) lrc_plan_kernel<<<blocks, kPlanWarps * 32, 0, st>>>(q);
-    else rs_plan_kernel<<<blocks, kPlanWarps * 32, 0, st>>>(q);
+    plan_kernel<<<(unsigned)((n + kPlanWarps - 1) / kPlanWarps), kPlanWarps * 32, 0, st>>>(q);
     ctx->launches.fetch_add(1, std::memory_order_relaxed);
     cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess)
-        return set_cuda_error(ctx, e, ctx->pb ? "pb_plan_kernel launch" : (ctx->l ? "lrc_plan_kernel launch" : "rs_plan_kernel launch"));
+    if (e != cudaSuccess) return set_cuda_error(ctx, e, "plan_kernel launch");
 
     TimedLaunch tl(ctx, st);
     const size_t pitch = (size_t)(ctx->k + ctx->m) * stride;
@@ -536,10 +533,9 @@ int run_reconstruct(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *present,
 
 size_t plan_scratch_bytes(size_t n) { return n * sizeof(StripePlan) + 16; }
 
-// The shards the plan kernels read for one stripe (present / want: k+m bytes, want nullable = every absent
-// shard), as a bit mask; false if a wanted shard cannot be rebuilt.  HOST paths upload only these.
-// PB contexts: bit 2i / 2i+1 of *halves = a- / b-half of shard i (h_pb_read_plan); other codes: 3 << 2i for every
-// shard of the read set.
+// The half-shards plan_kernel reads for one stripe (present / want: k+m bytes, want nullable = every absent
+// shard): bit 2i / 2i+1 of *halves = a- / b-half of shard i, both for every shard read by RS and LRC.  False if a
+// wanted shard cannot be rebuilt.  HOST paths upload only these.
 bool stripe_read_plan(const garage_ec_ctx *ctx, const uint8_t *present, const uint8_t *want, uint64_t *halves)
 {
     uint64_t pm = 0, wm = 0;
@@ -547,12 +543,11 @@ bool stripe_read_plan(const garage_ec_ctx *ctx, const uint8_t *present, const ui
         pm |= (uint64_t)(present[i] != 0) << i;
         wm |= (uint64_t)(!want || want[i] != 0) << i;
     }
-    if (ctx->pb) return h_pb_read_plan(ctx->k, ctx->m, ctx->P, pm, wm, halves);
-    uint64_t rd = 0;
-    const bool ok = h_read_set(ctx->k, ctx->m, ctx->l, ctx->P, pm, wm, &rd);
-    *halves = 0;
-    for (int i = 0; i < ctx->k + ctx->m; i++)
-        if ((rd >> i) & 1) *halves |= 3ull << (2 * i);
+    uint64_t rows = 0;
+    const bool ok = h_read_plan(PlanCode{ctx->k, ctx->m, ctx->l, ctx->pb, ctx->P}, pm, wm, &rows);
+    *halves = rows;
+    if (!ctx->pb)  // RS and LRC rows are shards
+        for (*halves = 0; rows; rows &= rows - 1) *halves |= 3ull << (2 * ctz64(rows));
     return ok;
 }
 bool stripe_read_set(const garage_ec_ctx *ctx, const uint8_t *present, const uint8_t *want, uint64_t *read)

@@ -102,78 +102,6 @@ inline bool h_build_lrc(int k, int l, int r, uint8_t *P)
     return h_build_matrix(k, r, 1, P + l * k);
 }
 
-// Survivor set of one stripe, the host twin of the plan kernels (DESIGN.md section 2).  Bit i of present / want:
-// shard i present / wanted (only absent wanted shards are rebuilt).  l = 0: RS, the first k present shards.
-// l > 0: LRC rule 1 (local repair) if it applies, else rule 2 (greedy rank basis in index order).  Returns false
-// if a wanted shard cannot be rebuilt; *read = the shards to read.
-inline bool h_read_set(int k, int m, int l, const uint8_t *P, uint64_t present, uint64_t want, uint64_t *read)
-{
-    const int tot = k + m;
-    const uint64_t all = tot >= 64 ? ~0ull : ((1ull << tot) - 1);
-    present &= all;
-    want &= all & ~present;
-    *read = 0;
-    if (l == 0) {
-        int used = 0;
-        for (int i = 0; i < tot && used < k; i++)
-            if ((present >> i) & 1) {
-                *read |= 1ull << i;
-                used++;
-            }
-        return used == k;
-    }
-    const int gs = k / l;
-    auto group_mask = [&](int g) { return (((1ull << gs) - 1) << (g * gs)) | (1ull << (k + g)); };
-    bool local = true;
-    uint64_t rmask = 0;
-    for (int o = 0; o < tot && local; o++) {
-        if (!((want >> o) & 1)) continue;
-        if (o >= k + l) {
-            local = false;
-            break;
-        }
-        const uint64_t gm = group_mask(o < k ? o / gs : o - k);
-        if ((gm & ~present) != (1ull << o)) local = false;
-        rmask |= gm & ~(1ull << o);
-    }
-    if (local) {
-        *read = rmask;
-        return true;
-    }
-    auto row = [&](int c, int j) -> uint8_t { return c < k ? (uint8_t)(c == j) : P[(c - k) * k + j]; };
-    uint8_t R[GARAGE_EC_MAX_K_HOST][GARAGE_EC_MAX_K_HOST];
-    int piv[GARAGE_EC_MAX_K_HOST], nb = 0;
-    auto reduce = [&](uint8_t *v) {
-        for (int b = 0; b < nb; b++) {
-            const uint8_t f = v[piv[b]];
-            if (f)
-                for (int j = 0; j < k; j++) v[j] ^= h_mul(f, R[b][j]);
-        }
-    };
-    for (int c = 0; c < tot && nb < k; c++) {
-        if (!((present >> c) & 1)) continue;
-        uint8_t v[GARAGE_EC_MAX_K_HOST];
-        for (int j = 0; j < k; j++) v[j] = row(c, j);
-        reduce(v);
-        int p = 0;
-        while (p < k && !v[p]) p++;
-        if (p == k) continue;
-        const uint8_t iv = h_inv(v[p]);
-        for (int j = 0; j < k; j++) R[nb][j] = h_mul(v[j], iv);
-        piv[nb++] = p;
-        *read |= 1ull << c;
-    }
-    for (int o = 0; o < tot; o++) {
-        if (!((want >> o) & 1)) continue;
-        uint8_t v[GARAGE_EC_MAX_K_HOST];
-        for (int j = 0; j < k; j++) v[j] = row(o, j);
-        reduce(v);
-        for (int j = 0; j < k; j++)
-            if (v[j]) return false;
-    }
-    return true;
-}
-
 // ---- piggybacked RS, PB(k, m) (DESIGN.md section 2.2) ------------------------------------------------------------
 // The k data shards form m-1 contiguous groups G_1..G_{m-1}, sizes as equal as possible, larger groups first.  The
 // b-half of parity i >= 1 carries the XOR of the a-halves of G_i on top of its RS value.
@@ -208,63 +136,122 @@ GEC_GF_HD inline uint8_t pb_grow(int k, int m, const uint8_t *P, int q, int c)
     if (hc == h) return P[i * k + j];
     return (uint8_t)(h == 1 && i >= 1 && pb_group_of(k, m, j) == i);  // the piggyback: a_j in b of parity i
 }
-// Half-row read plan of one PB stripe (host twin of pb_plan_kernel).  Bit i of present / want: shard i present /
-// wanted.  *halves: bit 2i = a-half of shard i read, bit 2i+1 = b-half.  Rule 1 when the only wanted absent shard is
-// a data shard j of G_i, every other data shard is present and so are parities 0 and i; rule 2 (greedy rank basis of
-// the present half-rows in q order) otherwise.  False if a wanted shard cannot be rebuilt.
-inline bool h_pb_read_plan(int k, int m, const uint8_t *P, uint64_t present, uint64_t want, uint64_t *halves)
+// ---- decode planning (DESIGN.md sections 2.1, 2.2) ---------------------------------------------------------------
+GEC_GF_HD inline int ctz64(uint64_t x)
 {
-    const int tot = k + m, K2 = 2 * k;
-    const uint64_t all = (1ull << tot) - 1, data = (1ull << k) - 1;
+#ifdef __CUDA_ARCH__
+    return __ffsll((long long)x) - 1;
+#else
+    return __builtin_ctzll(x);
+#endif
+}
+GEC_GF_HD inline int popc64(uint64_t x)
+{
+#ifdef __CUDA_ARCH__
+    return __popcll(x);
+#else
+    return __builtin_popcountll(x);
+#endif
+}
+
+// The code a stripe is planned for: RS (l = 0), LRC(k, l, m - l) or PB(k, m) (pb), with parity rows P (m x k).  The
+// planner picks survivors among generator rows: shards, or for PB the half-rows q = 2*shard + half.  Row masks have
+// bit q for row q.  Rows are taken in index order, and the data rows come first and are identity rows: row q < cols()
+// is e_q.  plan_kernel and h_read_plan share everything here.
+struct PlanCode {
+    int k, m, l;
+    bool pb;
+    const uint8_t *P;
+
+    GEC_GF_HD int cols() const { return pb ? 2 * k : k; }
+    GEC_GF_HD uint8_t row(int q, int c) const
+    {
+        if (pb) return pb_grow(k, m, P, q, c);
+        return q < k ? (uint8_t)(q == c) : P[(q - k) * k + c];
+    }
+    // shard mask -> row mask (PB: both halves of every shard)
+    GEC_GF_HD uint64_t shard_rows(uint64_t shards) const
+    {
+        if (!pb) return shards;
+        uint64_t r = 0;
+        for (; shards; shards &= shards - 1) r |= 3ull << (2 * ctz64(shards));
+        return r;
+    }
+    // The rows the survivors are picked from, given the present shards and the wanted absent shards: the present
+    // rows, or only those of rule 1 when it applies.
+    //   LRC (local repair): every wanted shard is a data shard or a local parity and the only absent member of its
+    //     group (the group's data plus its local parity): the other members of those groups.  Holds for want = 0.
+    //   PB (piggyback repair): the only wanted shard is a data shard j of G_i, every other data shard is present and
+    //     so are parities 0 and i: the b-halves of the other data shards and of parities 0 and i, and the a-halves
+    //     of G_i \ {j}, k + |G_i| halves (P[0][j] != 0 gives b_j).
+    // RS has no rule 1.  Rule 1 rows are independent, so the greedy basis keeps them all.
+    GEC_GF_HD uint64_t candidate_rows(uint64_t present, uint64_t want) const
+    {
+        if (l) {
+            const int gs = k / l;
+            uint64_t r = 0;
+            for (uint64_t w = want; w; w &= w - 1) {
+                const int o = ctz64(w);
+                if (o >= k + l) return present;
+                const int g = o < k ? o / gs : o - k;
+                const uint64_t gm = (((1ull << gs) - 1) << (g * gs)) | (1ull << (k + g));
+                if ((gm & ~present) != (1ull << o)) return present;
+                r |= gm & ~(1ull << o);
+            }
+            return r;
+        }
+        const uint64_t all = shard_rows(present), data = (1ull << k) - 1;
+        if (!pb || !want || (want & (want - 1)) || !(want & data)) return all;
+        const int j = ctz64(want), g = pb_group_of(k, m, j);
+        if ((present & data) != (data & ~want) || !((present >> k) & 1) || !((present >> (k + g)) & 1)) return all;
+        uint64_t r = (1ull << (2 * k + 1)) | (1ull << (2 * (k + g) + 1));
+        for (int x = 0; x < k; x++)
+            if (x != j) r |= 1ull << (2 * x + 1);
+        for (int x = pb_group_start(k, m, g); x < pb_group_start(k, m, g + 1); x++)
+            if (x != j) r |= 1ull << (2 * x);
+        return r;
+    }
+    // RS reports a stripe with fewer than k present shards unrecoverable even when nothing is wanted (garage_ec.h);
+    // LRC and PB judge the wanted rows only.
+    GEC_GF_HD bool below_k(uint64_t present) const { return !l && !pb && popc64(present) < k; }
+};
+
+// Survivors of one stripe, the host twin of plan_kernel (DESIGN.md section 2).  Bit i of present / want: shard i
+// present / wanted (only absent wanted shards are rebuilt).  *rows = the rows to read: the greedy rank basis, in row
+// order, of the candidate rows.  False if a wanted row is outside its span.
+inline bool h_read_plan(const PlanCode &c, uint64_t present, uint64_t want, uint64_t *rows)
+{
+    static_assert(2 * kPbMaxK <= GARAGE_EC_MAX_K_HOST, "PB columns");
+    const int K = c.cols();
+    const uint64_t all = (1ull << (c.k + c.m)) - 1;
     present &= all;
     want &= all & ~present;
-    *halves = 0;
-    uint64_t hp = 0;
-    for (int i = 0; i < tot; i++)
-        if ((present >> i) & 1) hp |= 3ull << (2 * i);
-    if (want && !(want & (want - 1)) && (want & data)) {
-        const int j = __builtin_ctzll(want), g = pb_group_of(k, m, j);
-        if ((present & data) == (data & ~want) && ((present >> k) & 1) && ((present >> (k + g)) & 1)) {
-            uint64_t r = (1ull << (2 * k + 1)) | (1ull << (2 * (k + g) + 1));
-            for (int x = 0; x < k; x++)
-                if (x != j) r |= 1ull << (2 * x + 1);
-            for (int x = pb_group_start(k, m, g); x < pb_group_start(k, m, g + 1); x++)
-                if (x != j) r |= 1ull << (2 * x);
-            *halves = r;
-            return true;
-        }
-    }
-    uint8_t R[2 * kPbMaxK][2 * kPbMaxK];
-    int piv[2 * kPbMaxK], nb = 0;
-    auto reduce = [&](uint8_t *v) {
+    uint8_t R[GARAGE_EC_MAX_K_HOST][GARAGE_EC_MAX_K_HOST], v[GARAGE_EC_MAX_K_HOST];
+    int piv[GARAGE_EC_MAX_K_HOST], nb = 0;
+    // row q reduced against the basis into v; returns its first nonzero column, K if it lies in the span
+    auto reduce = [&](int q) {
+        for (int j = 0; j < K; j++) v[j] = c.row(q, j);
         for (int b = 0; b < nb; b++) {
             const uint8_t f = v[piv[b]];
             if (f)
-                for (int c = 0; c < K2; c++) v[c] ^= h_mul(f, R[b][c]);
+                for (int j = 0; j < K; j++) v[j] ^= h_mul(f, R[b][j]);
         }
-    };
-    for (int q = 0; q < 2 * tot && nb < K2; q++) {
-        if (!((hp >> q) & 1)) continue;
-        uint8_t v[2 * kPbMaxK];
-        for (int c = 0; c < K2; c++) v[c] = pb_grow(k, m, P, q, c);
-        reduce(v);
         int p = 0;
-        while (p < K2 && !v[p]) p++;
-        if (p == K2) continue;
+        while (p < K && !v[p]) p++;
+        return p;
+    };
+    *rows = 0;
+    for (uint64_t cm = c.candidate_rows(present, want); cm && nb < K; cm &= cm - 1) {
+        const int q = ctz64(cm), p = reduce(q);
+        if (p == K) continue;
         const uint8_t iv = h_inv(v[p]);
-        for (int c = 0; c < K2; c++) R[nb][c] = h_mul(v[c], iv);
+        for (int j = 0; j < K; j++) R[nb][j] = h_mul(v[j], iv);
         piv[nb++] = p;
-        *halves |= 1ull << q;
+        *rows |= 1ull << q;
     }
-    for (int q = 0; q < 2 * tot; q++) {
-        if (!((want >> (q >> 1)) & 1)) continue;
-        uint8_t v[2 * kPbMaxK];
-        for (int c = 0; c < K2; c++) v[c] = pb_grow(k, m, P, q, c);
-        reduce(v);
-        for (int c = 0; c < K2; c++)
-            if (v[c]) return false;
-    }
-    return true;
+    for (uint64_t wm = c.shard_rows(want); wm; wm &= wm - 1)
+        if (reduce(ctz64(wm)) != K) return false;
+    return !c.below_k(present);
 }
 
 }  // namespace garage_ec

@@ -285,7 +285,7 @@ template <int K, int MODE> struct StreamCfg {
 // GF(2^8) antilog / log tables, pinned in constant memory.  Kernels that need general products
 // (decode planning) stage them into shared memory with warp-UNIFORM 16-byte constant loads:
 // a per-lane byte index into __constant__ memory serialises 32-way in the constant cache (the
-// first version of rs_plan_kernel spent 30 of its 40 us there).
+// first version of the RS plan kernel spent 30 of its 40 us there).
 struct GfTables {
     uint8_t exp[512];
     uint8_t log[256];
@@ -303,17 +303,18 @@ __device__ __forceinline__ void stage_gf_tables(uint8_t *s_gf /* 768 B, 16-byte 
     }
 }
 
-// Per-stripe decode plan, produced by rs_plan_kernel, consumed by rs_apply_kernel<kModePlan>.
+// Per-stripe decode plan, produced by plan_kernel, consumed by rs_apply_kernel<kModePlan>.  Indices are generator
+// rows: shards, or PB half-rows q = 2*shard + half.
 struct __align__(16) StripePlan {
-    unsigned long long key_present;  // bit i: shard i present
-    unsigned long long key_out;      // bit i: shard i is rebuilt
-    uint8_t nrows;                   // number of shards rebuilt (0..m)
+    unsigned long long key_present;  // bit i: row i present (PB: candidate)
+    unsigned long long key_out;      // bit i: row i is rebuilt
+    uint8_t nrows;                   // number of rows rebuilt (0..kMaxM)
     uint8_t unrecoverable;           // 1 if a wanted shard cannot be rebuilt
-    uint8_t nsurv;                   // sources read: surv[0..nsurv) (k for RS; <= k for LRC)
+    uint8_t nsurv;                   // sources read: surv[0..nsurv) (k for RS; <= k for LRC, <= 2k for PB)
     uint8_t pad[5];
-    uint8_t surv[kMaxK];           // source shard indices, ascending (RS: the first k present)
-    uint8_t out_idx[kMaxM];        // rebuilt shard indices
-    uint8_t coef[kMaxM][kMaxK];  // out[r] = XOR_j coef[r][j] * shard[surv[j]]
+    uint8_t surv[kMaxK];           // source row indices, ascending (RS: the first k present)
+    uint8_t out_idx[kMaxM];        // rebuilt row indices
+    uint8_t coef[kMaxM][kMaxK];  // out[r] = XOR_j coef[r][j] * row[surv[j]]
 };
 
 struct ApplyParams {
@@ -1290,27 +1291,34 @@ struct PlanParams {
     StripePlan *plan;        // n
     uint32_t *counter;       // reset to 0 for the apply kernel's scheduler
     uint32_t n, k, m;
-    uint32_t l;               // LRC local groups (lrc_plan_kernel); 0 for RS
+    uint32_t l;               // LRC local groups; 0 for RS and PB
+    uint32_t pb;              // 1: PB(k, m), planned over half-rows
     uint32_t present_is_bad;  // 1: `present` holds "bad" flags (scrub): a shard is present iff flag == 0
-    const uint32_t *shard_len;  // pb_plan_kernel: per stripe, nullable (=> stride); a length % 32 != 0 is malformed
+    const uint32_t *shard_len;  // PB: per stripe, nullable (=> stride); a length % 32 != 0 is malformed
     uint32_t stride;
     alignas(16) uint8_t P[kMaxM * kMaxK];  // parity rows, P[i*k + j] (16-byte aligned: staged with uint4 loads)
 };
 
 constexpr int kPlanWarps = 4;
+static_assert(2 * kPbMaxM <= kMaxM && 2 * kPbMaxK <= kMaxK, "PB half-rows fit a StripePlan");
 
-// One warp per stripe: pick the first k present shards, solve the a x a system that couples the
-// a absent data shards to the a parity survivors (Gauss-Jordan, lanes own columns), compose the
-// rows that map the survivors straight to every wanted absent shard.
-__global__ void __launch_bounds__(kPlanWarps * 32) rs_plan_kernel(const __grid_constant__ PlanParams q)
+// Decode planning for every code (DESIGN.md section 4.2), one warp per stripe, lanes own the cols() <= 32 generator
+// columns.  The survivors are a greedy rank basis, in row order, of PlanCode::candidate_rows; every wanted row is then
+// expressed in that basis, or the stripe is unrecoverable.  h_read_plan (gf256.h) is the host twin.
+// The basis is an incremental Gauss-Jordan: basis row b is stored reduced as [row | T_b], T_b giving it as a
+// combination of the survivors, and a row is reduced against the basis rows in insertion order, which zeroes it at
+// every earlier pivot.  The data rows come first and are identity rows, so the candidate data rows enter the basis
+// as they are (pivot = their column, T = e_position), and reducing a row against all of them is one lane-parallel
+// step.  Only parity rows and wanted rows are reduced serially, against the parity rows of the basis: fewer than the
+// absent data columns and at most kMaxM.  A PB stripe whose shard_len is not a multiple of 32 has no 16-byte aligned
+// halves: status GARAGE_EC_E_INVALID (-1), nothing is rebuilt.  16 CTAs per SM keep it at 32 registers, no spills.
+__global__ void __launch_bounds__(kPlanWarps * 32, 16) plan_kernel(const __grid_constant__ PlanParams q)
 {
     __shared__ __align__(16) uint8_t s_gf[sizeof(GfTables)];
     uint8_t *const s_exp = s_gf, *const s_log = s_gf + 512;
-    __shared__ uint8_t s_A[kPlanWarps][kMaxK][2 * kMaxK];
+    __shared__ uint8_t s_R[kPlanWarps][kMaxM][2 * kMaxK];  // parity rows of the basis, [row | T]
+    __shared__ uint8_t s_piv[kPlanWarps][kMaxM];
     __shared__ uint8_t s_surv[kPlanWarps][kMaxK];
-    __shared__ uint8_t s_out[kPlanWarps][kMaxM];
-    __shared__ uint8_t s_col[kPlanWarps][kMaxK];
-    __shared__ uint8_t s_dm[kPlanWarps][kMaxM];
     __shared__ __align__(16) uint8_t s_P[kMaxM * kMaxK];
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     stage_gf_tables(s_gf);
@@ -1329,181 +1337,12 @@ __global__ void __launch_bounds__(kPlanWarps * 32) rs_plan_kernel(const __grid_c
 
     const uint32_t s = blockIdx.x * kPlanWarps + warp;
     if (s >= q.n) return;
-    const uint32_t k = q.k, m = q.m, tot = k + m;
+    const uint32_t tot = q.k + q.m;
     StripePlan *pl = q.plan + s;
     const uint8_t *pr = q.present + (size_t)s * tot;
     const uint8_t *wn = q.want ? q.want + (size_t)s * tot : nullptr;
 
-    // presence / wanted masks (tot <= 40: two ballot rounds)
-    const bool inv = q.present_is_bad != 0;
-    const bool p0 = lane < tot && ((pr[lane] != 0) != inv);
-    const bool p1 = lane + 32 < tot && ((pr[lane + 32] != 0) != inv);
-    const unsigned long long present =
-        (unsigned long long)__ballot_sync(0xffffffffu, p0) |
-        ((unsigned long long)__ballot_sync(0xffffffffu, p1) << 32);
-    const bool w0 = lane < tot && !p0 && (!wn || wn[lane] != 0);
-    const bool w1 = lane + 32 < tot && !p1 && (!wn || wn[lane + 32] != 0);
-    unsigned long long outmask = (unsigned long long)__ballot_sync(0xffffffffu, w0) |
-                                 ((unsigned long long)__ballot_sync(0xffffffffu, w1) << 32);
-    const int npresent = __popcll(present);
-    const bool bad = npresent < (int)k;
-    if (bad) outmask = 0;
-    int nrows = __popcll(outmask);
-
-    if (lane == 0) {
-        // survivors: first k present; outputs: wanted absent shards in index order
-        unsigned long long pm = present;
-        for (uint32_t r = 0; r < k && pm; r++) {
-            const int i = __ffsll((long long)pm) - 1;
-            s_surv[warp][r] = (uint8_t)i;
-            pm &= pm - 1;
-        }
-        unsigned long long om = outmask;
-        for (int r = 0; r < nrows; r++) {
-            const int i = __ffsll((long long)om) - 1;
-            s_out[warp][r] = (uint8_t)i;
-            om &= om - 1;
-        }
-        pl->key_present = present;
-        pl->key_out = outmask;
-        pl->nrows = (uint8_t)nrows;
-        pl->unrecoverable = bad ? 1 : 0;
-        pl->nsurv = (uint8_t)k;
-        if (q.status) q.status[s] = bad ? -4 : 0;
-    }
-    __syncwarp();
-    if (bad || nrows == 0) return;
-
-    // The survivors are the present data shards (identity rows of the generator) followed by the
-    // first `a` present parity shards, a = number of absent data shards.  Only an a x a system
-    // couples the unknowns:   y_Pu = A x_Dm + B x_Dp,   A = P[Pu][Dm], B = P[Pu][Dp]
-    //   =>  x_Dm = Ainv y_Pu + (Ainv B) x_Dp          (characteristic 2)
-    // so a full k x k inversion is never needed (a <= m <= 8).
-    uint8_t(*A)[2 * kMaxK] = s_A[warp];  // rows 0..7: [A | I] -> [I | Ainv]; rows 8..15: Ainv*B; rows 16..23: decode rows
-    const unsigned long long datamask = (k >= 64 ? ~0ull : ((1ull << k) - 1));
-    const unsigned long long mdmask = ~present & datamask;
-    const uint32_t a = (uint32_t)__popcll(mdmask);
-    const uint32_t nd = k - a;  // data survivors occupy positions [0, nd) of surv[], parity survivors [nd, k)
-    if (lane == 0) {
-        unsigned long long mm = mdmask;
-        for (uint32_t t = 0; t < a; t++) {
-            s_dm[warp][t] = (uint8_t)(__ffsll((long long)mm) - 1);
-            mm &= mm - 1;
-        }
-    }
-    __syncwarp();
-    if (a) {
-        for (uint32_t r = 0; r < a; r++) {
-            const uint32_t prow = (uint32_t)s_surv[warp][nd + r] - k;
-            if (lane < 2 * a) A[r][lane] = lane < a ? s_P[prow * k + s_dm[warp][lane]] : (uint8_t)(lane - a == r);
-        }
-        __syncwarp();
-        for (uint32_t c = 0; c < a; c++) {
-            const bool cand = lane < a && lane >= c && A[lane][c] != 0;  // pivot search: lanes are rows
-            const uint32_t bal = __ballot_sync(0xffffffffu, cand);
-            if (!bal) {  // singular: cannot happen for an MDS generator; report unrecoverable
-                if (lane == 0) {
-                    pl->nrows = 0;
-                    pl->unrecoverable = 1;
-                    if (q.status) q.status[s] = -4;
-                }
-                return;
-            }
-            const uint32_t piv = __ffs(bal) - 1;
-            const uint32_t iv = s_exp[255 - s_log[A[piv][c]]];
-            __syncwarp();
-            if (lane < 2 * a) {
-                const uint8_t x = A[piv][lane], y = A[c][lane];
-                A[piv][lane] = y;                  // swap (no-op when piv == c)
-                A[c][lane] = (uint8_t)mul(x, iv);  // scaled pivot row
-            }
-            __syncwarp();
-            const uint32_t pv = lane < 2 * a ? A[c][lane] : 0;
-            if (lane < a) s_col[warp][lane] = lane == c ? 0 : A[lane][c];
-            __syncwarp();
-            for (uint32_t r = 0; r < a; r++) {
-                const uint32_t f = s_col[warp][r];  // broadcast; lanes own columns
-                if (f && lane < 2 * a) A[r][lane] ^= (uint8_t)mul(f, pv);
-            }
-            __syncwarp();
-        }
-        // decode row of missing data shard dm[t] over the survivor positions:
-        //   data survivors:   (Ainv B)[t][j] = XOR_r Ainv[t][r] * P[Pu_r][surv[j]]
-        //   parity survivors: Ainv[t][j - nd]
-        for (uint32_t t = 0; t < a; t++) {
-            uint32_t v = 0;
-            if (lane < nd) {
-                const uint32_t col = s_surv[warp][lane];
-                for (uint32_t r = 0; r < a; r++)
-                    v ^= mul(A[t][a + r], s_P[((uint32_t)s_surv[warp][nd + r] - k) * k + col]);
-            } else if (lane < k) {
-                v = A[t][a + (lane - nd)];
-            }
-            if (lane < k) A[16 + t][lane] = (uint8_t)v;
-        }
-        __syncwarp();
-    }
-    // rows for the wanted outputs
-    for (int r = 0; r < nrows; r++) {
-        const uint32_t o = s_out[warp][r];
-        if (lane < k) {
-            uint32_t v = 0;
-            if (o < k) {
-                // rank of o among the absent data shards
-                const uint32_t t = (uint32_t)__popcll(mdmask & ((1ull << o) - 1));
-                v = A[16 + t][lane];
-            } else {
-                // absent parity row i: P[i][Dp] on the data survivors, plus P[i][Dm] through the rows above
-                const uint32_t i = o - k;
-                if (lane < nd) v = s_P[i * k + s_surv[warp][lane]];
-                for (uint32_t t = 0; t < a; t++) v ^= mul(s_P[i * k + s_dm[warp][t]], A[16 + t][lane]);
-            }
-            pl->coef[r][lane] = (uint8_t)v;
-        }
-    }
-    if (lane < k) pl->surv[lane] = s_surv[warp][lane];
-    if (lane < (uint32_t)nrows) pl->out_idx[lane] = s_out[warp][lane];
-}
-
-// LRC(k, l, r) planning (DESIGN.md section 2), one warp per stripe.  Generator rows: data j = e_j, parity i = P[i]
-// (the l all-ones local rows, then the r Cauchy rows).  A wanted row is rebuildable iff it lies in the span of the
-// present rows, so fewer than k present shards may do.  Survivors:
-//   rule 1 (local repair): every wanted shard is a data shard or a local parity and is the only absent member of its
-//          group (the group's data plus its local parity): the survivors are the other members, coefficients all 1;
-//   rule 2 otherwise: present rows greedily in index order, kept if they raise the rank (<= k rows); every wanted
-//          row is expressed in that basis.
-// Rule 2 is an incremental Gauss-Jordan over lanes = columns: basis row b is stored reduced ([row | T_b], where
-// T_b gives it as a combination of the chosen survivors), and a new row is reduced against the basis rows in
-// insertion order, which zeroes it at every earlier pivot.
-__global__ void __launch_bounds__(kPlanWarps * 32) lrc_plan_kernel(const __grid_constant__ PlanParams q)
-{
-    __shared__ __align__(16) uint8_t s_gf[sizeof(GfTables)];
-    uint8_t *const s_exp = s_gf, *const s_log = s_gf + 512;
-    __shared__ uint8_t s_R[kPlanWarps][kMaxK][2 * kMaxK];
-    __shared__ uint8_t s_piv[kPlanWarps][kMaxK];
-    __shared__ uint8_t s_surv[kPlanWarps][kMaxK];
-    __shared__ __align__(16) uint8_t s_P[kMaxM * kMaxK];
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    stage_gf_tables(s_gf);
-    {
-        const uint4 *src = reinterpret_cast<const uint4 *>(q.P);
-        for (uint32_t i = warp; i < sizeof(q.P) / 16; i += blockDim.x >> 5) {
-            const uint4 v = src[i];
-            if (lane < 4) reinterpret_cast<uint32_t *>(s_P)[i * 4 + lane] = lane == 0 ? v.x : (lane == 1 ? v.y : (lane == 2 ? v.z : v.w));
-        }
-    }
-    if (blockIdx.x == 0 && tid == 0) *q.counter = 0;
-    __syncthreads();
-    auto mul = [&](uint32_t a, uint32_t b) -> uint32_t {
-        return (a && b) ? s_exp[s_log[a] + s_log[b]] : 0u;
-    };
-
-    const uint32_t s = blockIdx.x * kPlanWarps + warp;
-    if (s >= q.n) return;
-    const uint32_t k = q.k, m = q.m, l = q.l, tot = k + m, gs = k / l;
-    StripePlan *pl = q.plan + s;
-    const uint8_t *pr = q.present + (size_t)s * tot;
-    const uint8_t *wn = q.want ? q.want + (size_t)s * tot : nullptr;
+    // presence / wanted shard masks (tot <= 40: two ballot rounds)
     const bool inv = q.present_is_bad != 0;
     const bool p0 = lane < tot && ((pr[lane] != 0) != inv);
     const bool p1 = lane + 32 < tot && ((pr[lane + 32] != 0) != inv);
@@ -1513,142 +1352,7 @@ __global__ void __launch_bounds__(kPlanWarps * 32) lrc_plan_kernel(const __grid_
     const bool w1 = lane + 32 < tot && !p1 && (!wn || wn[lane + 32] != 0);
     const unsigned long long outmask =
         (unsigned long long)__ballot_sync(0xffffffffu, w0) | ((unsigned long long)__ballot_sync(0xffffffffu, w1) << 32);
-    const int nrows = __popcll(outmask);
-    // generator row c, column j
-    auto grow = [&](uint32_t c, uint32_t j) -> uint32_t { return c < k ? (uint32_t)(c == j) : (uint32_t)s_P[(c - k) * k + j]; };
-    auto group_mask = [&](uint32_t g) -> unsigned long long {
-        return (((1ull << gs) - 1) << (g * gs)) | (1ull << (k + g));
-    };
-
-    // rule 1 (warp-uniform)
-    bool local = true;
-    unsigned long long rmask = 0;
-    for (unsigned long long om = outmask; om; om &= om - 1) {
-        const uint32_t o = (uint32_t)(__ffsll((long long)om) - 1);
-        if (o >= k + l) {
-            local = false;
-            break;
-        }
-        const unsigned long long gm = group_mask(o < k ? o / gs : o - k);
-        if ((gm & ~present) != (1ull << o)) {
-            local = false;
-            break;
-        }
-        rmask |= gm & ~(1ull << o);
-    }
-    uint32_t nsurv = 0;
-    bool ok = true;
-    if (local) {
-        nsurv = (uint32_t)__popcll(rmask);
-        // lane j < nsurv: survivor j = the j-th set bit of rmask
-        unsigned long long mm = rmask;
-        for (uint32_t j = 0; j < lane && mm; j++) mm &= mm - 1;
-        const uint32_t sj = mm ? (uint32_t)(__ffsll((long long)mm) - 1) : 0u;
-        int r = 0;
-        for (unsigned long long om = outmask; om; om &= om - 1, r++) {
-            const uint32_t o = (uint32_t)(__ffsll((long long)om) - 1);
-            const unsigned long long gm = group_mask(o < k ? o / gs : o - k);
-            if (lane < k) pl->coef[r][lane] = (lane < nsurv && ((gm >> sj) & 1)) ? 1 : 0;
-        }
-        if (lane < nsurv) pl->surv[lane] = (uint8_t)sj;
-    } else {
-        // rule 2: greedy basis in index order
-        uint8_t(*R)[2 * kMaxK] = s_R[warp];
-        for (unsigned long long pm = present; pm && nsurv < k; pm &= pm - 1) {
-            const uint32_t c = (uint32_t)(__ffsll((long long)pm) - 1);
-            uint32_t v = lane < k ? grow(c, lane) : 0u, t = lane == nsurv ? 1u : 0u;
-            for (uint32_t b = 0; b < nsurv; b++) {
-                const uint32_t f = __shfl_sync(0xffffffffu, v, s_piv[warp][b]);
-                if (f) {
-                    v ^= mul(f, R[b][lane]);
-                    t ^= mul(f, R[b][kMaxK + lane]);
-                }
-            }
-            const uint32_t nz = __ballot_sync(0xffffffffu, v != 0);
-            if (!nz) continue;  // in the span of the rows already chosen
-            const uint32_t piv = __ffs(nz) - 1;
-            const uint32_t iv = s_exp[255 - s_log[__shfl_sync(0xffffffffu, v, piv)]];
-            R[nsurv][lane] = (uint8_t)mul(v, iv);
-            R[nsurv][kMaxK + lane] = (uint8_t)mul(t, iv);
-            if (lane == 0) {
-                s_piv[warp][nsurv] = (uint8_t)piv;
-                s_surv[warp][nsurv] = (uint8_t)c;
-            }
-            __syncwarp();
-            nsurv++;
-        }
-        int r = 0;
-        for (unsigned long long om = outmask; om && ok; om &= om - 1, r++) {
-            const uint32_t o = (uint32_t)(__ffsll((long long)om) - 1);
-            uint32_t v = lane < k ? grow(o, lane) : 0u, t = 0;
-            for (uint32_t b = 0; b < nsurv; b++) {
-                const uint32_t f = __shfl_sync(0xffffffffu, v, s_piv[warp][b]);
-                if (f) {
-                    v ^= mul(f, R[b][lane]);
-                    t ^= mul(f, R[b][kMaxK + lane]);
-                }
-            }
-            ok = __ballot_sync(0xffffffffu, v != 0) == 0;  // else outside the span of the present rows
-            // (while ok, r < m: rows in the span of fewer than k independent rows are at most l more than them)
-            if (ok && lane < k) pl->coef[r][lane] = (uint8_t)t;
-        }
-        if (lane < nsurv) pl->surv[lane] = s_surv[warp][lane];
-    }
-    if (lane == 0) {
-        int r = 0;
-        if (ok)  // an unrecoverable stripe may have up to k+m-1 absent shards: out_idx holds m
-            for (unsigned long long om = outmask; om; om &= om - 1, r++) pl->out_idx[r] = (uint8_t)(__ffsll((long long)om) - 1);
-        pl->key_present = present;
-        pl->key_out = outmask;
-        pl->nrows = ok ? (uint8_t)nrows : 0;
-        pl->unrecoverable = ok ? 0 : 1;
-        pl->nsurv = (uint8_t)nsurv;
-        if (q.status) q.status[s] = ok ? 0 : -4;
-    }
-}
-
-// PB(k, m) planning (DESIGN.md section 2.2), one warp per stripe, over half-rows q = 2*shard + half: 2(k+m) <= 40
-// generator rows over 2k <= 32 half-data columns (lane = column), generator row q from pb_grow.  Rule 1 (a lone lost
-// data shard j of G_i with every other data shard and parities 0 and i present) is rule 2 run on the present
-// half-rows restricted to its k + |G_i| repair halves, which are independent: the greedy basis keeps them all.  Rule
-// 2 is the greedy rank basis of lrc_plan_kernel.  surv[] / out_idx[] hold half-row indices; rs_apply_kernel<2k,
-// kModePlan> with ApplyParams::half turns them into byte offsets.  A stripe whose shard_len is not a multiple of 32
-// has no 16-byte aligned halves: status GARAGE_EC_E_INVALID (-1), nothing is rebuilt.
-__global__ void __launch_bounds__(kPlanWarps * 32) pb_plan_kernel(const __grid_constant__ PlanParams q)
-{
-    __shared__ __align__(16) uint8_t s_gf[sizeof(GfTables)];
-    uint8_t *const s_exp = s_gf, *const s_log = s_gf + 512;
-    __shared__ uint8_t s_R[kPlanWarps][kMaxK][2 * kMaxK];
-    __shared__ uint8_t s_piv[kPlanWarps][kMaxK];
-    __shared__ uint8_t s_surv[kPlanWarps][kMaxK];
-    __shared__ __align__(16) uint8_t s_P[kMaxM * kMaxK];
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    stage_gf_tables(s_gf);
-    {
-        const uint4 *src = reinterpret_cast<const uint4 *>(q.P);
-        for (uint32_t i = warp; i < sizeof(q.P) / 16; i += blockDim.x >> 5) {
-            const uint4 v = src[i];
-            if (lane < 4) reinterpret_cast<uint32_t *>(s_P)[i * 4 + lane] = lane == 0 ? v.x : (lane == 1 ? v.y : (lane == 2 ? v.z : v.w));
-        }
-    }
-    if (blockIdx.x == 0 && tid == 0) *q.counter = 0;
-    __syncthreads();
-    auto mul = [&](uint32_t a, uint32_t b) -> uint32_t {
-        return (a && b) ? s_exp[s_log[a] + s_log[b]] : 0u;
-    };
-
-    const uint32_t s = blockIdx.x * kPlanWarps + warp;
-    if (s >= q.n) return;
-    const uint32_t k = q.k, m = q.m, tot = k + m, K2 = 2 * k;  // tot <= 20
-    StripePlan *pl = q.plan + s;
-    const uint8_t *pr = q.present + (size_t)s * tot;
-    const uint8_t *wn = q.want ? q.want + (size_t)s * tot : nullptr;
-    const bool inv = q.present_is_bad != 0;
-    const bool p0 = lane < tot && ((pr[lane] != 0) != inv);
-    const unsigned long long present = __ballot_sync(0xffffffffu, p0);
-    const unsigned long long outmask = __ballot_sync(0xffffffffu, lane < tot && !p0 && (!wn || wn[lane] != 0));
-    const uint32_t len = q.shard_len ? q.shard_len[s] : q.stride;
-    if (len & 31) {
+    if (q.pb && ((q.shard_len ? q.shard_len[s] : q.stride) & 31)) {
         if (lane == 0) {
             pl->key_present = present;
             pl->key_out = outmask;
@@ -1659,73 +1363,71 @@ __global__ void __launch_bounds__(kPlanWarps * 32) pb_plan_kernel(const __grid_c
         }
         return;
     }
-    auto grow = [&](uint32_t r, uint32_t c) -> uint32_t { return c < K2 ? pb_grow((int)k, (int)m, s_P, (int)r, (int)c) : 0u; };
-    unsigned long long hp = 0, hout = 0;  // half-row masks
-    for (uint32_t i = 0; i < tot; i++) {
-        if ((present >> i) & 1) hp |= 3ull << (2 * i);
-        if ((outmask >> i) & 1) hout |= 3ull << (2 * i);
-    }
-    const unsigned long long data = (1ull << k) - 1;
-    if (outmask && !(outmask & (outmask - 1)) && (outmask & data)) {  // rule 1
-        const uint32_t j = (uint32_t)(__ffsll((long long)outmask) - 1), g = (uint32_t)pb_group_of((int)k, (int)m, (int)j);
-        if ((present & data) == (data & ~outmask) && ((present >> k) & 1) && ((present >> (k + g)) & 1)) {
-            unsigned long long r = (1ull << (2 * k + 1)) | (1ull << (2 * (k + g) + 1));
-            for (uint32_t x = 0; x < k; x++)
-                if (x != j) r |= 1ull << (2 * x + 1);
-            for (int x = pb_group_start((int)k, (int)m, (int)g); x < pb_group_start((int)k, (int)m, (int)g + 1); x++)
-                if ((uint32_t)x != j) r |= 1ull << (2 * x);
-            hp = r;
-        }
-    }
-    // rule 2: greedy basis in q order (as lrc_plan_kernel, 2k columns)
+    const PlanCode code{(int)q.k, (int)q.m, (int)q.l, q.pb != 0, s_P};
+    const uint32_t K = (uint32_t)code.cols();
+    const unsigned long long cand = code.candidate_rows(present, outmask);
+    const unsigned long long wrows = code.below_k(present) ? 0ull : code.shard_rows(outmask);
+
+    // the candidate data rows: basis positions 0..nd in column order
+    const unsigned long long dmask = cand & ((1ull << K) - 1);
+    const uint32_t nd = (uint32_t)__popcll(dmask);
+    const bool dcol = (dmask >> lane) & 1;
+    if (dcol) s_surv[warp][__popcll(dmask & ((1ull << lane) - 1))] = (uint8_t)lane;
+    __syncwarp();
+    const uint32_t dsrc = lane < nd ? s_surv[warp][lane] : 0u;  // the column of basis position `lane`
     uint8_t(*R)[2 * kMaxK] = s_R[warp];
-    uint32_t nsurv = 0;
-    for (unsigned long long pm = hp; pm && nsurv < K2; pm &= pm - 1) {
-        const uint32_t c = (uint32_t)(__ffsll((long long)pm) - 1);
-        uint32_t v = grow(c, lane), t = lane == nsurv ? 1u : 0u;
-        for (uint32_t b = 0; b < nsurv; b++) {
+    uint32_t np = 0;  // parity rows in the basis
+    // v (lane = column) reduced against the basis, t accumulating the combination of survivors
+    auto reduce = [&](uint32_t &v, uint32_t &t) {
+        const uint32_t vd = __shfl_sync(0xffffffffu, v, dsrc);
+        if (lane < nd) t ^= vd;
+        if (dcol) v = 0;
+        for (uint32_t b = 0; b < np; b++) {
             const uint32_t f = __shfl_sync(0xffffffffu, v, s_piv[warp][b]);
             if (f) {
                 v ^= mul(f, R[b][lane]);
                 t ^= mul(f, R[b][kMaxK + lane]);
             }
         }
+    };
+    uint32_t nsurv = nd;
+    for (unsigned long long pm = cand & ~dmask; pm && nsurv < K; pm &= pm - 1) {
+        const uint32_t c = (uint32_t)(__ffsll((long long)pm) - 1);
+        uint32_t v = lane < K ? code.row((int)c, (int)lane) : 0u, t = lane == nsurv ? 1u : 0u;
+        reduce(v, t);
         const uint32_t nz = __ballot_sync(0xffffffffu, v != 0);
-        if (!nz) continue;
+        if (!nz) continue;  // in the span of the rows already chosen
         const uint32_t piv = __ffs(nz) - 1;
         const uint32_t iv = s_exp[255 - s_log[__shfl_sync(0xffffffffu, v, piv)]];
-        R[nsurv][lane] = (uint8_t)mul(v, iv);
-        R[nsurv][kMaxK + lane] = (uint8_t)mul(t, iv);
+        R[np][lane] = (uint8_t)mul(v, iv);
+        R[np][kMaxK + lane] = (uint8_t)mul(t, iv);
         if (lane == 0) {
-            s_piv[warp][nsurv] = (uint8_t)piv;
+            s_piv[warp][np] = (uint8_t)piv;
             s_surv[warp][nsurv] = (uint8_t)c;
         }
         __syncwarp();
+        np++;
         nsurv++;
     }
-    bool ok = true;
-    int r = 0;
-    for (unsigned long long om = hout; om && ok; om &= om - 1, r++) {
+    bool ok = !code.below_k(present);
+    int nrows = 0;
+    for (unsigned long long om = wrows; om && ok; om &= om - 1, nrows++) {
         const uint32_t o = (uint32_t)(__ffsll((long long)om) - 1);
-        uint32_t v = grow(o, lane), t = 0;
-        for (uint32_t b = 0; b < nsurv; b++) {
-            const uint32_t f = __shfl_sync(0xffffffffu, v, s_piv[warp][b]);
-            if (f) {
-                v ^= mul(f, R[b][lane]);
-                t ^= mul(f, R[b][kMaxK + lane]);
-            }
-        }
-        ok = __ballot_sync(0xffffffffu, v != 0) == 0;
-        if (ok) pl->coef[r][lane] = (uint8_t)t;  // r < 2m <= kMaxM while ok: at most m shards are absent
+        uint32_t v = lane < K ? code.row((int)o, (int)lane) : 0u, t = 0;
+        reduce(v, t);
+        ok = __ballot_sync(0xffffffffu, v != 0) == 0;  // else outside the span of the candidate rows
+        // (while ok, nrows < kMaxM: RS and PB rebuild at most m shards, 2m <= kMaxM halves; LRC rows in the span of
+        // fewer than k independent rows are at most l more than them)
+        if (ok) pl->coef[nrows][lane] = (uint8_t)t;
     }
     if (lane < nsurv) pl->surv[lane] = s_surv[warp][lane];
     if (lane == 0) {
-        int n_out = 0;
-        if (ok)
-            for (unsigned long long om = hout; om; om &= om - 1, n_out++) pl->out_idx[n_out] = (uint8_t)(__ffsll((long long)om) - 1);
-        pl->key_present = hp;
-        pl->key_out = hout;
-        pl->nrows = ok ? (uint8_t)n_out : 0;
+        int r = 0;
+        if (ok)  // an unrecoverable stripe may have up to k+m-1 absent shards: out_idx holds kMaxM
+            for (unsigned long long om = wrows; om; om &= om - 1, r++) pl->out_idx[r] = (uint8_t)(__ffsll((long long)om) - 1);
+        pl->key_present = code.pb ? cand : present;  // with key_out, the apply kernel's table reuse key
+        pl->key_out = wrows;
+        pl->nrows = ok ? (uint8_t)nrows : 0;
         pl->unrecoverable = ok ? 0 : 1;
         pl->nsurv = (uint8_t)nsurv;
         if (q.status) q.status[s] = ok ? 0 : -4;

@@ -96,7 +96,7 @@ int main(int argc, char **argv)
     unsigned long long pm, wm;
     while (scanf("%llx %llx", &pm, &wm) == 2) {
         uint64_t rd = 0;
-        const bool ok = h_read_set(k, m, l, P, pm, wm, &rd);
+        const bool ok = h_read_plan(PlanCode{k, m, l, false, P}, pm, wm, &rd);
         printf("%d %llx\n", ok ? 1 : 0, (unsigned long long)rd);
     }
     return 0;
@@ -115,9 +115,10 @@ def read_set_harness(tmp_path_factory):
 
 
 @pytest.mark.parametrize("k,l,r", [(6, 2, 2), (10, 2, 2), (6, 0, 3)])
-def test_library_read_set_matches_rules(read_set_harness, k, l, r):
-    """the survivor selection the library uses (garage_ec_read_set and the HOST upload paths) against the Python
-    statement of rules 1 and 2, every erasure pattern, want = every absent shard and each absent shard alone"""
+def test_host_read_plan_matches_rules(read_set_harness, k, l, r):
+    """the survivor selection the library uses (h_read_plan: garage_ec_read_set and the HOST upload paths) against
+    the Python statement of rules 1 and 2, every erasure pattern, want = every absent shard and each absent shard
+    alone"""
     m = l + r
     tot = k + m
     P = LO.build_lrc(k, l, r) if l else O.build_matrix(k, m, 0)

@@ -135,7 +135,7 @@ int main()
     unsigned long long pm, wm;
     while (scanf("%llx %llx", &pm, &wm) == 2) {
         uint64_t hv = 0;
-        const bool ok = h_pb_read_plan(k, m, P, pm, wm, &hv);
+        const bool ok = h_read_plan(PlanCode{k, m, 0, true, P}, pm, wm, &hv);
         printf("%d %llx\n", ok ? 1 : 0, (unsigned long long)hv);
     }
     return 0;
@@ -154,9 +154,10 @@ def read_plan_harness(tmp_path_factory):
 
 
 @pytest.mark.parametrize("k,m,kind", [(6, 3, 0), (10, 4, 1)])
-def test_library_read_plan_matches_rules(read_plan_harness, k, m, kind):
-    """the half-row plan the library uses (garage_ec_read_plan, the HOST upload paths) against the Python rules for
-    every pattern with up to 4 absent shards, want = every absent shard and each absent shard alone"""
+def test_host_read_plan_matches_rules(read_plan_harness, k, m, kind):
+    """the half-row plan the library uses (h_read_plan: garage_ec_read_plan, the HOST upload paths) against the
+    Python rules for every pattern with up to 4 absent shards, want = every absent shard and each absent shard
+    alone"""
     tot = k + m
     P = PB.build(k, m, kind)
     cases = []
