@@ -18,8 +18,14 @@ SYMBOLS = [
     "garage_bm_drop_shard", "garage_bm_node_shard_index", "garage_bm_storage_nodes_of", "garage_bm_get_metrics",
     "garage_bm_block_incref", "garage_bm_block_decref", "garage_bm_get_block_rc", "garage_bm_scrub_step",
     "garage_bm_bench", "garage_bm_corrupt_shard_header", "garage_bm_plant_stale_shard", "garage_bm_set_node_readonly",
+    "garage_bm_convert_step", "garage_bm_debug_convert_stop_after",
 ]
 SUM_BLAKE2, SUM_ADLER8 = 0, 1
+
+
+class Code(C.Structure):
+    """garage_bm_code: a code the store may still hold shards of"""
+    _fields_ = [("k", C.c_int), ("m", C.c_int), ("local_groups", C.c_int), ("piggyback", C.c_int)]
 
 
 class Config(C.Structure):
@@ -27,7 +33,8 @@ class Config(C.Structure):
                 ("n_nodes", C.c_int), ("block_size", C.c_uint32), ("block_ram_buffer_max", C.c_uint64),
                 ("batch_max_blocks", C.c_uint32), ("batch_linger_us", C.c_uint32), ("data_dir", C.c_char_p),
                 ("shard_sum_kind", C.c_int), ("verify_content_hash", C.c_int), ("data_fsync", C.c_int),
-                ("block_gc_delay_ms", C.c_uint32), ("local_groups", C.c_int), ("piggyback", C.c_int)]
+                ("block_gc_delay_ms", C.c_uint32), ("local_groups", C.c_int), ("piggyback", C.c_int),
+                ("previous_codes", C.POINTER(Code)), ("n_previous_codes", C.c_int), ("legacy_replicas", C.c_int)]
 
 
 class Metrics(C.Structure):
@@ -35,7 +42,9 @@ class Metrics(C.Structure):
         "bytes_written", "bytes_read", "corruption_counter", "resync_counter", "resync_error_counter",
         "resync_recv_counter", "delete_counter", "put_calls", "put_batches", "reconstruct_calls",
         "reconstruct_batches", "scrub_shards_checked", "scrub_corruptions", "resync_queue_length",
-        "encode_call_us", "reconstruct_call_us", "corrupt_data_errors", "write_errors", "resync_shards_read", "resync_bytes_read")]
+        "encode_call_us", "reconstruct_call_us", "corrupt_data_errors", "write_errors", "resync_shards_read", "resync_bytes_read",
+        "convert_blocks", "convert_bytes_read", "convert_bytes_written", "convert_errors", "convert_call_us", "legacy_gets",
+        "legacy_deleted")]
 
 
 _lib = None
@@ -76,6 +85,8 @@ def load_library():
         L.garage_bm_corrupt_shard_header.argtypes = [vp, i32, vp, i32]
         L.garage_bm_plant_stale_shard.argtypes = [vp, i32, vp]
         L.garage_bm_set_node_readonly.argtypes = [vp, i32, i32]
+        L.garage_bm_convert_step.argtypes = [vp, i32, vp, sz, vp, C.POINTER(i32), C.POINTER(C.c_uint64)]
+        L.garage_bm_debug_convert_stop_after.argtypes = [vp, C.c_long]
         _lib = L
     return _lib
 
@@ -99,10 +110,12 @@ class BlockManager:
 
     def __init__(self, k=10, m=4, n_nodes=None, cuda_device=0, batch_max_blocks=64, batch_linger_us=100,
                  block_ram_buffer_max=256 << 20, data_dir=None, shard_sum_kind=SUM_ADLER8, verify_content_hash=True,
-                 data_fsync=False, block_gc_delay_ms=0, local_groups=0, piggyback=False):
+                 data_fsync=False, block_gc_delay_ms=0, local_groups=0, piggyback=False, previous_codes=(),
+                 legacy_replicas=0):
         """block_gc_delay_ms defaults to 0 HERE (tests delete at once); the library's default is the
         reference's BLOCK_GC_DELAY of 10 minutes.  local_groups > 0: LRC(k, local_groups, m - local_groups).
-        piggyback: PB(k, m), half-shard repair reads."""
+        piggyback: PB(k, m), half-shard repair reads.  previous_codes: (k, m, local_groups, piggyback) tuples of
+        codes the store may still hold; legacy_replicas: replication factor of a previous replicated layout."""
         self._L = load_library()
         cfg = Config()
         self._L.garage_bm_default_config(C.byref(cfg))
@@ -114,6 +127,9 @@ class BlockManager:
         cfg.data_fsync, cfg.block_gc_delay_ms = 1 if data_fsync else 0, block_gc_delay_ms
         cfg.local_groups = local_groups
         cfg.piggyback = 1 if piggyback else 0
+        self._prev = (Code * max(1, len(previous_codes)))(*[Code(*map(int, c)) for c in previous_codes])  # kept alive
+        cfg.previous_codes = C.cast(self._prev, C.POINTER(Code)) if previous_codes else None
+        cfg.n_previous_codes, cfg.legacy_replicas = len(previous_codes), legacy_replicas
         self._dir = data_dir.encode() if data_dir else None  # keep the bytes alive
         cfg.data_dir = self._dir
         h = C.c_void_p()
@@ -187,6 +203,27 @@ class BlockManager:
         rc = self._L.garage_bm_scrub_step(self._h, node, C.c_char_p(bytes(cursor)) if cursor else None, max_shards,
                                           C.cast(out, C.c_void_p), C.byref(fin), C.byref(a), C.byref(b))
         return rc, out.raw, bool(fin.value), a.value, b.value
+
+    def convert_step(self, node, cursor=None, max_blocks=0):
+        """-> (rc, cursor_out bytes, finished, converted)"""
+        out = C.create_string_buffer(32)
+        fin, n = C.c_int(0), C.c_uint64(0)
+        rc = self._L.garage_bm_convert_step(self._h, node, C.c_char_p(bytes(cursor)) if cursor else None, max_blocks,
+                                            C.cast(out, C.c_void_p), C.byref(fin), C.byref(n))
+        return rc, out.raw, bool(fin.value), n.value
+
+    def convert_all(self):
+        """one full convert_step sweep over every node -> blocks converted"""
+        total = 0
+        for node in range(self.n_nodes):
+            rc, _, finished, n = self.convert_step(node)
+            if rc == OK:
+                assert finished
+                total += n
+        return total
+
+    def debug_convert_stop_after(self, n_ops):
+        return self._L.garage_bm_debug_convert_stop_after(self._h, n_ops)
 
     def set_node_up(self, node, up):
         return self._L.garage_bm_set_node_up(self._h, node, 1 if up else 0)

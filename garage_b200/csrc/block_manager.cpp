@@ -262,13 +262,26 @@ std::string hex_of(const uint8_t *p, size_t n)
 
 enum ReadResult { kReadOk = 0, kReadMissing = 1, kReadInvalid = 2 };
 
+// a code shards are stored under: RS(k, m), LRC(k, l, m - l) or PB(k, m)
+struct CodeDesc {
+    int k = 0, m = 0, l = 0;  // l: LRC local groups, 0 = RS
+    bool pb = false;          // piggybacked RS PB(k, m): shard_len = ceil(block_len / k) rounded up to 128
+    bool operator==(const CodeDesc &o) const { return k == o.k && m == o.m && l == o.l && pb == o.pb; }
+    bool named_by(const ShardFileHeader &hd) const { return hd.k == k && hd.m == m && hd.pad[0] == l && hd.pad[1] == (pb ? 1 : 0); }
+};
+
+// A node's files for one hash (file store): <hash>.shard, written by this manager or an earlier one; <hash>.legacy,
+// a shard of a previous code moved aside so that a configured-code shard can take the .shard name; <hash> (no
+// extension), a whole-block replica of a replicated layout (Garage's own file: plain bytes, no header).
 struct Node {
     std::mutex mu;  // stands in for the 256 hash-sharded mutexes (manager.rs:114,679-689)
     bool up = true;
     bool fsync_data = false;  // data_fsync (util/config.rs), manager.rs:775-789
     std::string dir;          // empty: in-memory store
-    int k = 0, m = 0, l = 0;  // l: LRC local groups, 0 = RS
-    bool pb = false;          // piggybacked RS PB(k, m): shard_len = ceil(block_len / k) rounded up to 128
+    int k = 0, m = 0, l = 0;  // the configured code (codes[0])
+    bool pb = false;
+    std::vector<CodeDesc> codes;  // [0] the configured code, then garage_bm_config.previous_codes (file store only)
+    bool replicas = false;        // legacy_replicas > 0: whole-block replica files are read, listed and converted
     // in-memory mode: immutable shards behind shared pointers, so the node lock only covers the map operation -- the
     // 100 KB copies happen outside it (the reference shards its lock 256 ways per node, manager.rs:114,679-689; with
     // one lock per node and the copies inside it, 128 clients serialised on 14 mutexes at ~12 GiB/s)
@@ -288,15 +301,104 @@ struct Node {
         auto it = shards.find(h);
         return it == shards.end() ? ShardPtr() : it->second;
     }
-    bool meta_valid(const ShardMeta &mt) const
+    bool meta_valid(const ShardMeta &mt, int code = 0) const
     {
-        if (mt.index < 0 || mt.index >= k + m) return false;
-        const uint64_t L = ((uint64_t)mt.block_len + (unsigned)k - 1) / (unsigned)k;
-        return mt.shard_len == (pb ? (L + 127) / 128 * 128 : L);
+        const CodeDesc &c = codes[code];
+        if (mt.index < 0 || mt.index >= c.k + c.m) return false;
+        const uint64_t L = ((uint64_t)mt.block_len + (unsigned)c.k - 1) / (unsigned)c.k;
+        return mt.shard_len == (c.pb ? (L + 127) / 128 * 128 : L);
     }
     // all store_* are called with `mu` held
+    // the code a shard file's header names: an index into `codes`, -1 for another code or a damaged header, -2 if the
+    // file does not exist
+    int file_code(const std::string &path) const
+    {
+        FILE *f = fopen(path.c_str(), "rb");
+        if (!f) return -2;
+        ShardFileHeader hd;
+        int c = -1;
+        if (fread(&hd, sizeof(hd), 1, f) == 1 && memcmp(hd.magic, "GEC1", 4) == 0 &&
+            hd.hdr_check == adler32_small(reinterpret_cast<const uint8_t *>(&hd), 48))
+            for (size_t i = 0; i < codes.size() && c < 0; i++)
+                if (codes[i].named_by(hd)) c = (int)i;
+        fclose(f);
+        return c;
+    }
+    // the file holding this node's shard of `code` ("" = none).  The configured code lives in .shard; a shard of a
+    // previous code in .shard (written before the code changed) or .legacy.  A file whose header names no listed code
+    // is the configured code's to read, which quarantines it, as before previous codes existed.
+    std::string path_for(const Hash &h, int code) const
+    {
+        const std::string sh = path_of(h, ".shard");
+        if (codes.size() < 2) return code == 0 ? sh : std::string();
+        const int c = file_code(sh);
+        if (code == 0) return c >= 1 || c == -2 ? std::string() : sh;
+        if (c == code) return sh;
+        const std::string lg = path_of(h, ".legacy");
+        const int c2 = file_code(lg);
+        return c2 == code || c2 == -1 ? lg : std::string();
+    }
+    bool has_legacy_shard(const Hash &h) const
+    {
+        if (codes.size() < 2) return false;
+        const int c = file_code(path_of(h, ".shard"));
+        return c >= 1 || file_code(path_of(h, ".legacy")) != -2;
+    }
+    bool has_replica(const Hash &h) const
+    {
+        struct stat sb;
+        return replicas && ::stat(path_of(h, "").c_str(), &sb) == 0 && S_ISREG(sb.st_mode);
+    }
+    bool fsync_dir_of(const Hash &h) const
+    {
+        const int dfd = ::open((dir + "/" + hex_of(h.data(), 1) + "/" + hex_of(h.data() + 1, 1)).c_str(), O_RDONLY | O_DIRECTORY);
+        if (dfd < 0) return false;
+        const bool ok = ::fsync(dfd) == 0;
+        ::close(dfd);
+        return ok;
+    }
+    // before a configured-code shard takes the .shard name: a previous code's shard there moves to .legacy
+    // (atomic rename, then the directory entry under data_fsync).  false if that failed: nothing may be written then.
+    bool store_move_legacy_aside(const Hash &h)
+    {
+        if (dir.empty() || codes.size() < 2) return true;
+        const std::string sh = path_of(h, ".shard");
+        if (file_code(sh) < 1) return true;
+        if (::rename(sh.c_str(), path_of(h, ".legacy").c_str()) != 0) return false;
+        return !fsync_data || fsync_dir_of(h);
+    }
+    // this node's legacy copies of h (a previous code's shard, the replica): removed, their number returned
+    int store_erase_legacy(const Hash &h, const std::function<bool()> &allow)
+    {
+        int n = 0;
+        if (codes.size() >= 2) {
+            const std::string sh = path_of(h, ".shard"), lg = path_of(h, ".legacy");
+            if (file_code(sh) >= 1 && allow() && ::remove(sh.c_str()) == 0) n++;
+            if (file_code(lg) != -2 && allow() && ::remove(lg.c_str()) == 0) n++;
+        }
+        if (has_replica(h) && allow() && ::remove(path_of(h, "").c_str()) == 0) n++;
+        return n;
+    }
+    // a whole-block replica into dst (cap bytes); its length is the file size.  The caller checks the content hash.
+    ReadResult replica_read_into(const Hash &h, uint8_t *dst, size_t cap, uint32_t &len) const
+    {
+        if (!replicas) return kReadMissing;
+        FILE *f = fopen(path_of(h, "").c_str(), "rb");
+        if (!f) return kReadMissing;
+        struct stat sb;
+        ReadResult r = kReadInvalid;
+        if (fstat(fileno(f), &sb) == 0 && S_ISREG(sb.st_mode) && (uint64_t)sb.st_size <= cap && sb.st_size > 0 &&
+            fread(dst, (size_t)sb.st_size, 1, f) == 1) {
+            len = (uint32_t)sb.st_size;
+            r = kReadOk;
+        }
+        fclose(f);
+        return r;
+    }
+    void replica_quarantine(const Hash &h) { ::rename(path_of(h, "").c_str(), path_of(h, ".corrupted").c_str()); }
     bool store_put(const Hash &h, const ShardMeta &mt, const uint8_t *bytes, size_t n)
     {
+        if (!dir.empty() && !store_move_legacy_aside(h)) return false;
         if (dir.empty()) {
             auto sp = std::make_shared<StoredShard>();
             static_cast<ShardMeta &>(*sp) = mt;
@@ -341,35 +443,41 @@ struct Node {
     // shard bytes straight into `dst` (cap bytes available), metadata into `mt`.  half = 0 / 1: only the a- / b-half
     // [half * shard_len/2, (half+1) * shard_len/2) of a PB shard, one ranged read at 64 + half * shard_len/2 of the
     // file, into dst (which then holds shard_len/2 bytes)
-    ReadResult store_read_into(const Hash &h, uint8_t *dst, size_t cap, ShardMeta &mt, int half = -1) const
+    ReadResult store_read_into(const Hash &h, uint8_t *dst, size_t cap, ShardMeta &mt, int half = -1, int code = 0) const
     {
         if (dir.empty()) {
-            auto it = shards.find(h);
+            auto it = code == 0 ? shards.find(h) : shards.end();
             if (it == shards.end()) return kReadMissing;
             return copy_out(*it->second, dst, cap, mt, false, half);
         }
-        FILE *f = fopen(path_of(h, ".shard").c_str(), "rb");  // find_block (manager.rs:627-662)
+        return file_read_into(path_for(h, code), code, dst, cap, mt, half);
+    }
+    // one shard file read as a shard of `code`
+    ReadResult file_read_into(const std::string &path, int code, uint8_t *dst, size_t cap, ShardMeta &mt, int half = -1) const
+    {
+        if (path.empty()) return kReadMissing;
+        FILE *f = fopen(path.c_str(), "rb");  // find_block (manager.rs:627-662)
         if (!f) return kReadMissing;
+        const CodeDesc &c = codes[code];
         ShardFileHeader hd;
         ReadResult r = kReadInvalid;
         struct stat sb;
         // a header that fails any of these is a corrupt shard, never a reason to allocate or read
         // what it claims (a flipped shard_len must not become a 4 GiB resize)
         if (fread(&hd, sizeof(hd), 1, f) == 1 && memcmp(hd.magic, "GEC1", 4) == 0 &&
-            hd.hdr_check == adler32_small(reinterpret_cast<const uint8_t *>(&hd), 48) && hd.k == k && hd.m == m &&
-            hd.pad[0] == l && hd.pad[1] == (pb ? 1 : 0) && fstat(fileno(f), &sb) == 0 &&
-            (uint64_t)sb.st_size == (uint64_t)hd.shard_len + sizeof(hd)) {
+            hd.hdr_check == adler32_small(reinterpret_cast<const uint8_t *>(&hd), 48) && c.named_by(hd) &&
+            fstat(fileno(f), &sb) == 0 && (uint64_t)sb.st_size == (uint64_t)hd.shard_len + sizeof(hd)) {
             mt.index = hd.index;
             mt.block_len = hd.block_len;
             mt.shard_len = hd.shard_len;
             mt.sum_kind = hd.sum_kind;
             memcpy(mt.sum.data(), hd.sum, 32);
             if (half < 0) {
-                if (meta_valid(mt) && mt.shard_len <= cap && (mt.shard_len == 0 || fread(dst, mt.shard_len, 1, f) == 1))
+                if (meta_valid(mt, code) && mt.shard_len <= cap && (mt.shard_len == 0 || fread(dst, mt.shard_len, 1, f) == 1))
                     r = kReadOk;
             } else {
                 const size_t hl = mt.shard_len / 2;
-                if (pb && meta_valid(mt) && hl <= cap &&
+                if (c.pb && meta_valid(mt, code) && hl <= cap &&
                     (hl == 0 || ::pread(fileno(f), dst, hl, (off_t)(sizeof(hd) + (size_t)half * hl)) == (ssize_t)hl))
                     r = kReadOk;
             }
@@ -407,6 +515,7 @@ struct Node {
     bool store_has(const Hash &h) const
     {
         if (dir.empty()) return shards.count(h) != 0;
+        if (codes.size() >= 2) return !path_for(h, 0).empty();
         std::error_code ec;
         return std::filesystem::exists(path_of(h, ".shard"), ec);
     }
@@ -415,7 +524,7 @@ struct Node {
         if (dir.empty()) return shards.erase(h) != 0;
         return ::remove(path_of(h, ".shard").c_str()) == 0;
     }
-    void store_quarantine(const Hash &h)  // move_block_to_corrupted (manager.rs:807-819)
+    void store_quarantine(const Hash &h, int code = 0)  // move_block_to_corrupted (manager.rs:807-819)
     {
         if (dir.empty()) {
             auto it = shards.find(h);
@@ -425,19 +534,24 @@ struct Node {
             }
             return;
         }
-        ::rename(path_of(h, ".shard").c_str(), path_of(h, ".corrupted").c_str());
+        const std::string p = codes.size() < 2 ? path_of(h, ".shard") : path_for(h, code);
+        if (!p.empty()) ::rename(p.c_str(), path_of(h, ".corrupted").c_str());
     }
-    void store_list(std::vector<Hash> &out) const  // BlockStoreIterator (repair.rs:634-764)
+    // BlockStoreIterator (repair.rs:634-764).  legacy: also hashes held only as a .legacy shard or a replica
+    void store_list(std::vector<Hash> &out, bool legacy = false) const
     {
         if (dir.empty()) {
             for (auto &kv : shards) out.push_back(kv.first);
             return;
         }
-        std::error_code ec;
+        std::error_code ec, ec2;
         for (auto it = std::filesystem::recursive_directory_iterator(dir, ec);
              !ec && it != std::filesystem::recursive_directory_iterator(); it.increment(ec)) {
             const std::string name = it->path().filename().string();
-            if (name.size() != 64 + 6 || name.compare(64, 6, ".shard") != 0) continue;
+            const bool listed = (name.size() == 64 + 6 && name.compare(64, 6, ".shard") == 0) ||
+                                (legacy && codes.size() >= 2 && name.size() == 64 + 7 && name.compare(64, 7, ".legacy") == 0) ||
+                                (legacy && replicas && name.size() == 64 && it->is_regular_file(ec2));
+            if (!listed) continue;
             Hash h;
             bool ok = true;
             for (int i = 0; i < 32 && ok; i++) {
@@ -756,12 +870,42 @@ struct garage_bm {
         scrub_checked{0}, scrub_corrupt{0}, enc_gpu_us{0}, rec_gpu_us{0}, corrupt_data_errors{0}, write_errors{0},
         resync_shards_read{0}, resync_bytes_read{0};
     std::atomic<uint64_t> put_ns_slot{0}, put_ns_land{0}, put_ns_wait{0}, put_ns_store{0};
+    std::atomic<uint64_t> convert_blocks{0}, convert_bytes_read{0}, convert_bytes_written{0}, convert_errors{0},
+        convert_call_us{0}, legacy_gets{0}, legacy_deleted{0};
 
     bool pb = false;  // PB(k, m) contexts (garage_bm_config.piggyback)
-    size_t shard_len_of(uint32_t block_len) const
+    // codes[0]: the configured code (ctx = ec); codes[1..]: garage_bm_config.previous_codes, one context each.  Shard i
+    // of every code lives on the i-th node of the block's ring row.
+    struct Code : CodeDesc {
+        int tot = 0;
+        garage_ec_ctx *ctx = nullptr;
+    };
+    std::vector<Code> codes;
+    int legacy_rf = 0;  // garage_bm_config.legacy_replicas
+    bool has_legacy() const { return codes.size() > 1 || legacy_rf > 0; }
+    std::atomic<long> convert_ops_left{-1};  // garage_bm_debug_convert_stop_after: < 0 = off
+    bool convert_op_allowed()
+    {
+        long v = convert_ops_left.load();
+        while (v >= 0) {
+            if (v == 0) return false;
+            if (convert_ops_left.compare_exchange_weak(v, v - 1)) return true;
+        }
+        return true;
+    }
+    std::mutex convert_mu;         // one conversion batch at a time (owns the pinned batch buffers)
+    PinnedBuf conv_src, conv_dst, conv_blk;  // old shards / replicas in, new shards + tags out, one block
+    size_t shard_len_of(uint32_t block_len, int code = 0) const
     {
         uint32_t L = 0;  // a length that does not fit in 32 bits is larger than any slot: every caller rejects it
-        return garage_ec_code_shard_len(ec, block_len, &L) == GARAGE_EC_OK ? L : SIZE_MAX;
+        return garage_ec_code_shard_len(codes[code].ctx, block_len, &L) == GARAGE_EC_OK ? L : SIZE_MAX;
+    }
+    // the nodes holding shards 0 .. tot-1 of h under `code`
+    void nodes_of(const Hash &h, int code, int *out) const
+    {
+        if (code == 0) return storage_nodes_of(h, out);
+        const int n = (int)nodes.size(), p = h[0] % n;
+        for (int i = 0; i < codes[code].tot; i++) out[i] = (p + i) % n;
     }
 
     // rpc/layout/version.rs:117-137: top 8 bits of the hash -> partition -> k+m distinct nodes, shard i on the
@@ -825,13 +969,15 @@ struct garage_bm {
         return ok;
     }
 
-    void quarantine(int node, const Hash &h)
+    // code -1: the node's replica of h
+    void quarantine(int node, const Hash &h, int code = 0)
     {
         corruption_counter++;
         {
             Node &nd = *nodes[node];
             std::lock_guard<std::mutex> lk(nd.mu);
-            nd.store_quarantine(h);
+            if (code < 0) nd.replica_quarantine(h);
+            else nd.store_quarantine(h, code);
         }
         put_to_resync(node, h);
     }
@@ -839,7 +985,7 @@ struct garage_bm {
     // manager.rs:554-609 read_block + read_block_from: the verified shard bytes land in `dst`.
     // A bad header or a tag mismatch quarantines the shard and queues a resync, like the reference.
     // `for_dma`: the GPU reads `dst` next (degraded GET, resync): see copy_for_dma
-    bool read_shard_into(int node, const Hash &h, uint8_t *dst, size_t cap, ShardMeta &mt, bool for_dma = false)
+    bool read_shard_into(int node, const Hash &h, uint8_t *dst, size_t cap, ShardMeta &mt, bool for_dma = false, int code = 0)
     {
         Node &nd = *nodes[node];
         ReadResult r;
@@ -856,7 +1002,7 @@ struct garage_bm {
         } else {
             std::lock_guard<std::mutex> lk(nd.mu);
             if (!nd.up) return false;
-            r = nd.store_read_into(h, dst, cap, mt);
+            r = nd.store_read_into(h, dst, cap, mt, -1, code);
         }
         if (r == kReadMissing) return false;
         if (r == kReadOk) {
@@ -865,12 +1011,13 @@ struct garage_bm {
             if (garage_ec_shard_sum_host(mt.sum_kind, check, mt.shard_len, got.data()) == GARAGE_EC_OK && got == mt.sum)
                 return true;
         }
-        quarantine(node, h);
+        quarantine(node, h, code);
         return false;
     }
     // PB: one half of a shard (a ranged read of shard_len/2 bytes into dst), checked against the half's 4 adler8
     // segment tags (garage_ec_check_shard_half_host); a bad header or tag quarantines the shard like a whole read
-    bool read_half_into(int node, const Hash &h, int half, uint8_t *dst, size_t cap, ShardMeta &mt, bool for_dma = false)
+    bool read_half_into(int node, const Hash &h, int half, uint8_t *dst, size_t cap, ShardMeta &mt, bool for_dma = false,
+                        int code = 0)
     {
         Node &nd = *nodes[node];
         ReadResult r;
@@ -885,7 +1032,7 @@ struct garage_bm {
         } else {
             std::lock_guard<std::mutex> lk(nd.mu);
             if (!nd.up) return false;
-            r = nd.store_read_into(h, dst, cap, mt, half);
+            r = nd.store_read_into(h, dst, cap, mt, half, code);
         }
         if (r == kReadMissing) return false;
         if (r == kReadOk) {
@@ -893,7 +1040,7 @@ struct garage_bm {
             if (garage_ec_check_shard_half_host(mt.sum_kind, dst, mt.shard_len, half, mt.sum.data()) == GARAGE_EC_OK)
                 return true;
         }
-        quarantine(node, h);
+        quarantine(node, h, code);
         return false;
     }
 
@@ -968,11 +1115,17 @@ struct garage_bm {
     // A shard whose header disagrees with the others on the block length, or that sits under the
     // wrong index, is treated like a corrupt one.  `all`: read every shard (corruption hunting).
     // Returns the number of shards read (*bytes_out += the bytes); *ok = the wanted shards can be rebuilt from `have`.
+    // `code`: the stripe of that code (0 = the configured one; others: a previous code's shards, .shard or .legacy)
     int gather_into(const Hash &h, int skip_node, uint8_t *slot, uint8_t *have, uint32_t &block_len, bool all = false,
-                    bool for_gpu = false, const uint8_t *want_in = nullptr, bool *ok = nullptr, uint64_t *bytes_out = nullptr)
+                    bool for_gpu = false, const uint8_t *want_in = nullptr, bool *ok = nullptr, uint64_t *bytes_out = nullptr,
+                    int code = 0)
     {
+        const Code &cd = codes[code];
+        const int k = cd.k, tot = cd.tot;
+        const bool pb = cd.pb;
+        garage_ec_ctx *const ec = cd.ctx;
         int who[64];
-        storage_nodes_of(h, who);
+        nodes_of(h, code, who);
         memset(have, 0, tot);
         uint32_t expect = 0;
         bool have_expect = false;
@@ -994,10 +1147,11 @@ struct garage_bm {
             uint8_t *dst = slot + (size_t)i * slot_stride;
             bool got;
             if (half < 0) {
-                got = read_shard_into(who[i], h, dst, slot_stride, mt, for_gpu);
+                got = read_shard_into(who[i], h, dst, slot_stride, mt, for_gpu, code);
             } else {
-                const size_t hl = (have_expect ? shard_len_of(expect) : slot_stride) / 2;  // placement of the b-half
-                got = read_half_into(who[i], h, half, dst + (size_t)half * hl, slot_stride - (size_t)half * hl, mt, for_gpu);
+                const size_t hl = (have_expect ? shard_len_of(expect, code) : slot_stride) / 2;  // placement of the b-half
+                got = read_half_into(who[i], h, half, dst + (size_t)half * hl, slot_stride - (size_t)half * hl, mt, for_gpu,
+                                     code);
                 if (got && !have_expect && half == 1 && mt.shard_len / 2 != hl)  // first read of the block: move it
                     memmove(dst + mt.shard_len / 2, dst + hl, mt.shard_len / 2);
             }
@@ -1010,7 +1164,7 @@ struct garage_bm {
                 return;
             }
             if (mt.index != i || (have_expect && mt.block_len != expect)) {
-                quarantine(who[i], h);  // a stale or misplaced shard with a self-consistent tag
+                quarantine(who[i], h, code);  // a stale or misplaced shard with a self-consistent tag
                 if (have_h[i]) count--;
                 have_h[i] = 0;
                 have[i] = 0;
@@ -1080,9 +1234,18 @@ struct garage_bm {
         return count;
     }
 
-    int reconstruct_in_slot(uint8_t *slot, uint32_t block_len, const uint8_t *have, const uint8_t *want)
+    int reconstruct_in_slot(uint8_t *slot, uint32_t block_len, const uint8_t *have, const uint8_t *want, int code = 0)
     {
         reconstruct_calls++;
+        if (code != 0) {  // a previous code's stripe (legacy GET): one stripe, straight on that code's context
+            const uint32_t L = (uint32_t)shard_len_of(block_len, code);
+            int32_t st = 0;
+            const auto t0 = Clock::now();
+            int rc = garage_ec_reconstruct_stripes(codes[code].ctx, &slot, have, want, &st, &L, slot_stride, 1);
+            rec_gpu_us += (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count();
+            if (rc == GARAGE_EC_OK || rc == GARAGE_EC_E_UNRECOVERABLE) rc = st ? GARAGE_BM_E_MISSING_BLOCK : GARAGE_BM_OK;
+            return rc;
+        }
         ReconItem it;
         it.stripe = slot;
         it.stride = slot_stride;
@@ -1092,10 +1255,10 @@ struct garage_bm {
         return rec_batcher->submit(it);
     }
 
-    void assemble(const uint8_t *slot, uint32_t block_len, uint8_t *out) const
+    void assemble(const uint8_t *slot, uint32_t block_len, uint8_t *out, int code = 0) const
     {
-        const size_t L = shard_len_of(block_len);
-        for (int j = 0; j < k; j++) {
+        const size_t L = shard_len_of(block_len, code);
+        for (int j = 0; j < codes[code].k; j++) {
             const size_t off = (size_t)j * L;
             if (off >= block_len) break;
             memcpy(out + off, slot + (size_t)j * slot_stride, std::min(L, (size_t)block_len - off));
@@ -1186,11 +1349,61 @@ struct garage_bm {
     // manager.rs:344-363 + 276-339.  `out` must hold block_size bytes; *out_len = the block's length.
     int rpc_get_block(const Hash &h, uint8_t *out, size_t cap, size_t *out_len)
     {
+        const int rc = get_from_stripe(h, out, cap, out_len, 0);
+        if (rc == GARAGE_BM_OK || !has_legacy()) return rc;
+        // the configured stripe cannot serve it (yet): a block stored before the code changed
+        for (int c = 1; c < (int)codes.size(); c++)
+            if (get_from_stripe(h, out, cap, out_len, c) == GARAGE_BM_OK) {
+                legacy_gets++;
+                return GARAGE_BM_OK;
+            }
+        uint32_t len = 0;
+        if (read_replica(h, out, cap, len)) {
+            *out_len = len;
+            legacy_gets++;
+            return GARAGE_BM_OK;
+        }
+        return rc;
+    }
+
+    // the block from the first of its first legacy_rf ring nodes whose replica matches its content hash (a replica
+    // that does not is quarantined)
+    bool read_replica(const Hash &h, uint8_t *out, size_t cap, uint32_t &len, int *from = nullptr)
+    {
+        for (int i = 0; i < legacy_rf; i++) {
+            const int node = ((int)h[0] % (int)nodes.size() + i) % (int)nodes.size();
+            Node &nd = *nodes[node];
+            ReadResult r;
+            {
+                std::lock_guard<std::mutex> lk(nd.mu);
+                if (!nd.up) continue;
+                r = nd.replica_read_into(h, out, cap, len);
+            }
+            if (r == kReadMissing) continue;
+            Hash got;
+            if (r == kReadOk) {
+                bytes_read += len;
+                garage_ec_blake2sum(out, len, got.data());
+                if (got == h) {
+                    if (from) *from = node;
+                    return true;
+                }
+            }
+            quarantine(node, h, -1);
+        }
+        return false;
+    }
+
+    // manager.rs:344-363 + 276-339 on the stripe of `code`: gather, rebuild missing data shards, check the content
+    // hash, and on a mismatch hunt the shard that is stale
+    int get_from_stripe(const Hash &h, uint8_t *out, size_t cap, size_t *out_len, int code)
+    {
+        const int k = codes[code].k;
         SlotLease slot(stripe_slots);
         uint8_t have[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M], want[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
         uint32_t block_len = 0;
         bool ok = false;
-        gather_into(h, -1, slot.p, have, block_len, false, false, nullptr, &ok);
+        gather_into(h, -1, slot.p, have, block_len, false, false, nullptr, &ok, nullptr, code);
         if (!ok) return GARAGE_BM_E_MISSING_BLOCK;  // manager.rs:336-338
         *out_len = block_len;
         if (block_len > cap) return GARAGE_EC_E_INVALID;
@@ -1200,19 +1413,28 @@ struct garage_bm {
             want[j] = !have[j];
         }
         if (!all_data) {
-            int rc = reconstruct_in_slot(slot.p, block_len, have, want);
+            int rc = reconstruct_in_slot(slot.p, block_len, have, want, code);
             if (rc != GARAGE_BM_OK) return rc;
         }
-        assemble(slot.p, block_len, out);
+        assemble(slot.p, block_len, out, code);
         if (content_ok(h, out, block_len)) return GARAGE_BM_OK;
-        // Every shard passed its own tag, yet the block is not the one `h` names: some shard is
-        // stale or was rebuilt wrongly.  Find it: gather everything, drop one shard at a time,
-        // rebuild, re-check (manager.rs read path: CorruptData -> quarantine + resync).
+        return hunt_stale_shard(h, slot.p, out, cap, out_len, code);
+    }
+
+    // Every shard passed its own tag, yet the block is not the one `h` names: some shard is
+    // stale or was rebuilt wrongly.  Find it: gather everything (into the stripe slot `sp`), drop one shard at a
+    // time, rebuild, re-check (manager.rs read path: CorruptData -> quarantine + resync).
+    int hunt_stale_shard(const Hash &h, uint8_t *sp, uint8_t *out, size_t cap, size_t *out_len, int code)
+    {
+        const int k = codes[code].k, tot = codes[code].tot;
+        uint8_t have[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
+        uint32_t block_len = 0;
         corrupt_data_errors++;
-        const int avail = gather_into(h, -1, slot.p, have, block_len, /*all=*/true, /*for_gpu=*/true);
+        const int avail = gather_into(h, -1, sp, have, block_len, /*all=*/true, /*for_gpu=*/true, nullptr, nullptr,
+                                      nullptr, code);
         if (avail > k && block_len <= cap) {
             int who[64];
-            storage_nodes_of(h, who);
+            nodes_of(h, code, who);
             SlotLease trial(stripe_slots);
             for (int x = 0; x < tot; x++) {
                 if (!have[x]) continue;
@@ -1224,11 +1446,11 @@ struct garage_bm {
                     w2[j] = !h2[j];
                     need |= w2[j] != 0;
                 }
-                memcpy(trial.p, slot.p, (size_t)tot * slot_stride);
-                if (need && reconstruct_in_slot(trial.p, block_len, h2, w2) != GARAGE_BM_OK) continue;
-                assemble(trial.p, block_len, out);
+                memcpy(trial.p, sp, (size_t)tot * slot_stride);
+                if (need && reconstruct_in_slot(trial.p, block_len, h2, w2, code) != GARAGE_BM_OK) continue;
+                assemble(trial.p, block_len, out, code);
                 if (content_ok(h, out, block_len)) {
-                    quarantine(who[x], h);  // the culprit
+                    quarantine(who[x], h, code);  // the culprit
                     *out_len = block_len;
                     return GARAGE_BM_OK;
                 }
@@ -1285,6 +1507,11 @@ struct garage_bm {
                                                     &nbytes);
         resync_bytes_read += nbytes;
         if (!ok) {
+            // no configured stripe to rebuild from, but maybe a block stored before the code changed: convert it
+            if (has_legacy() && convert_batch({h}) == 1) {
+                resync_counter++;
+                return GARAGE_BM_OK;
+            }
             resync_error_counter++;
             return GARAGE_BM_E_MISSING_BLOCK;  // resync.rs:488-494
         }
@@ -1303,6 +1530,276 @@ struct garage_bm {
             return GARAGE_BM_E_MESSAGE;  // Error::Io: stays queued, the caller backs off (resync.rs:300-315)
         }
         resync_counter++;
+        return GARAGE_BM_OK;
+    }
+
+    // ---- changing the store's code (DESIGN.md section 5.1) ----------------------------------
+    // the configured stripe of h holds its write quorum: k+1 configured-code shards with valid tags on their nodes
+    bool configured_at_quorum(const Hash &h)
+    {
+        int who[64];
+        storage_nodes_of(h, who);
+        const int quorum = garage_ec_write_quorum(k, m, GARAGE_CONSISTENT);
+        SlotLease scratch(stripe_slots);
+        int good = 0;
+        for (int i = 0; i < tot && good < quorum && good + (tot - i) >= quorum; i++) {
+            ShardMeta mt;
+            if (read_shard_into(who[i], h, scratch.p, slot_stride, mt) && mt.index == i) good++;
+        }
+        return good >= quorum;
+    }
+    // every node that may hold a legacy copy of a block is among the first legacy_row() nodes of its ring row
+    int legacy_row() const
+    {
+        int r = legacy_rf;
+        for (size_t c = 1; c < codes.size(); c++) r = std::max(r, codes[c].tot);
+        return r;
+    }
+    int ring_node(const Hash &h, int i) const { return ((int)h[0] % (int)nodes.size() + i) % (int)nodes.size(); }
+    // the node that converts h: the first up node holding a legacy copy, previous codes in order and their shards in
+    // index order, then the replica holders; -1 if no up node holds one
+    int converter_of(const Hash &h)
+    {
+        for (int c = 1; c < (int)codes.size(); c++)
+            for (int i = 0; i < codes[c].tot; i++) {
+                Node &nd = *nodes[ring_node(h, i)];
+                std::lock_guard<std::mutex> lk(nd.mu);
+                if (nd.up && !nd.path_for(h, c).empty()) return ring_node(h, i);
+            }
+        for (int i = 0; i < legacy_rf; i++) {
+            Node &nd = *nodes[ring_node(h, i)];
+            std::lock_guard<std::mutex> lk(nd.mu);
+            if (nd.up && nd.has_replica(h)) return ring_node(h, i);
+        }
+        return -1;
+    }
+    // node's legacy copies of h are removed, each removal one conversion file operation.  Only called once the
+    // caller has seen the configured stripe at quorum, or for a block whose rc is 0 (then with refs_mu held).
+    void delete_legacy(int node, const Hash &h)
+    {
+        Node &nd = *nodes[node];
+        std::lock_guard<std::mutex> lk(nd.mu);
+        if (nd.up && !nd.dir.empty()) legacy_deleted += nd.store_erase_legacy(h, [this] { return convert_op_allowed(); });
+    }
+    // write_shard for a conversion: a previous code's shard under the .shard name first moves to .legacy; each of
+    // the two steps is one conversion file operation
+    bool write_converted(int node, const Hash &h, int index, uint32_t block_len, const uint8_t *bytes, size_t n,
+                         const uint8_t *sum)
+    {
+        Node &nd = *nodes[node];
+        bool ok = true;
+        {
+            std::lock_guard<std::mutex> lk(nd.mu);
+            if (!nd.up) return false;
+            if (!nd.dir.empty() && nd.file_code(nd.path_of(h, ".shard")) >= 1)
+                ok = convert_op_allowed() && nd.store_move_legacy_aside(h);
+        }
+        ok = ok && convert_op_allowed();
+        if (!ok) {
+            write_errors++;
+            return false;
+        }
+        if (!write_shard(node, h, index, block_len, bytes, n, sum)) return false;
+        convert_bytes_written += n;
+        return true;
+    }
+
+    // Rewrite blocks stored under a previous code or as replicas under the configured code: one garage_ec_transcode
+    // per source (previous codes in order, then replicas) and batch of batch_max_blocks.  Nothing is written for a
+    // block whose new data shards do not hash to it; then the old stripe's stale shard is hunted and quarantined and
+    // the block converted from the consistent rest.  A block is converted once k+1 new shards are durable; then the
+    // legacy copies on the up nodes are deleted.  Returns the number converted; a block that fails keeps every legacy
+    // copy and counts in convert_errors.
+    size_t convert_batch(const std::vector<Hash> &hs)
+    {
+        std::lock_guard<std::mutex> cl(convert_mu);
+        const size_t bmax = std::max<uint32_t>(cfg.batch_max_blocks, 1);
+        const int nsrc = (int)codes.size() + (legacy_rf > 0 ? 1 : 0);  // source codes.size(): the replicas
+        const size_t rep_stride = garage_ec_stride_for(cfg.block_size);
+        const int quorum = garage_ec_write_quorum(k, m, GARAGE_CONSISTENT);
+        uint8_t *blk = conv_blk.get(rep_stride);
+        if (!blk) return 0;
+        std::atomic<size_t> converted{0};
+        for (size_t b0 = 0; b0 < hs.size(); b0 += bmax) {
+            const size_t nb = std::min(bmax, hs.size() - b0);
+            std::vector<uint8_t> pending(nb, 1);
+            for (int c = 1; c < nsrc; c++) {
+                const bool rep = c == (int)codes.size();
+                const int s_tot = rep ? 1 : codes[c].tot;
+                const size_t s_stride = rep ? rep_stride : slot_stride;
+                uint8_t *src = conv_src.get(nb * s_tot * s_stride);
+                uint8_t *dst = conv_dst.get(nb * tot * (slot_stride + 32));
+                if (!src || !dst) break;
+                uint8_t *sums = dst + nb * tot * slot_stride;
+                std::vector<uint8_t> present(nb * s_tot);
+                std::vector<uint32_t> lens(nb);
+                // the old stripes (or replicas) of the batch, read by several threads: block j at position j ...
+                std::vector<uint8_t> got_src(nb, 0);
+                parallel_for(nb, [&](size_t j, std::vector<uint8_t> &) {
+                    if (!pending[j]) return;
+                    const Hash &h = hs[b0 + j];
+                    uint8_t *slot = src + j * s_tot * s_stride;
+                    uint32_t len = 0;
+                    bool ok = false;
+                    uint64_t nbytes = 0;
+                    if (rep) {
+                        ok = read_replica(h, slot, s_stride, len);
+                        nbytes = len;
+                    } else {
+                        uint8_t *have = present.data() + j * s_tot;
+                        gather_into(h, -1, slot, have, len, false, true, nullptr, &ok, &nbytes, c);
+                        bool degraded = false;
+                        for (int i = 0; i < codes[c].k; i++) degraded |= !have[i];
+                        if (ok && degraded)  // every survivor whole: the transcode reads what its own plan names
+                            gather_into(h, -1, slot, have, len, true, true, nullptr, &ok, &nbytes, c);
+                    }
+                    convert_bytes_read += nbytes;
+                    lens[j] = len;
+                    got_src[j] = ok && len > 0 && len <= cfg.block_size;
+                });
+                // ... then the readable ones packed to the front
+                std::vector<size_t> which;  // batch position -> block
+                for (size_t j = 0; j < nb; j++) {
+                    if (!got_src[j]) continue;
+                    const size_t q = which.size();
+                    if (q != j) {
+                        memmove(src + q * s_tot * s_stride, src + j * s_tot * s_stride, (size_t)s_tot * s_stride);
+                        memmove(present.data() + q * s_tot, present.data() + j * s_tot, s_tot);
+                        lens[q] = lens[j];
+                    }
+                    which.push_back(j);
+                }
+                const size_t n = which.size();
+                if (n == 0) continue;
+                std::vector<int32_t> status(n, GARAGE_EC_E_UNRECOVERABLE);
+                auto t0 = Clock::now();
+                int rc = garage_ec_transcode(ec, rep ? nullptr : codes[c].ctx, src, rep ? nullptr : present.data(), lens.data(),
+                                             s_stride, dst, slot_stride, sums, status.data(), n, GARAGE_EC_MEM_HOST, nullptr);
+                convert_call_us += (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count();
+                if (rc != GARAGE_EC_OK && rc != GARAGE_EC_E_UNRECOVERABLE) continue;
+                // the new data shards must hash to the block before anything is written
+                std::vector<uint8_t> good(n, 0);
+                parallel_for(n, [&](size_t q, std::vector<uint8_t> &tmp) {
+                    if (status[q] != GARAGE_EC_OK) return;
+                    tmp.resize(lens[q]);
+                    assemble(dst + q * tot * slot_stride, lens[q], tmp.data());
+                    Hash got;
+                    garage_ec_blake2sum(tmp.data(), lens[q], got.data());
+                    good[q] = got == hs[b0 + which[q]];
+                });
+                for (size_t q = 0; q < n; q++) {
+                    const Hash &h = hs[b0 + which[q]];
+                    if (status[q] != GARAGE_EC_OK) continue;
+                    if (!good[q] && !rep) {
+                        // a shard of the old stripe passed its tag with other bytes: the hunt quarantines it and
+                        // returns the block, which is converted on its own
+                        size_t olen = 0;
+                        uint32_t l32 = lens[q];
+                        int32_t st = 0;
+                        if (get_from_stripe(h, blk, cfg.block_size, &olen, c) == GARAGE_BM_OK && olen == lens[q]) {
+                            t0 = Clock::now();
+                            rc = garage_ec_transcode(ec, nullptr, blk, nullptr, &l32, rep_stride, dst + q * tot * slot_stride,
+                                                     slot_stride, sums + q * tot * 32, &st, 1, GARAGE_EC_MEM_HOST, nullptr);
+                            convert_call_us +=
+                                (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count();
+                            std::vector<uint8_t> tmp(lens[q]);
+                            assemble(dst + q * tot * slot_stride, lens[q], tmp.data());
+                            Hash got;
+                            garage_ec_blake2sum(tmp.data(), lens[q], got.data());
+                            good[q] = rc == GARAGE_EC_OK && got == h;
+                        }
+                    }
+                }
+                // the new stripes go to their nodes, several blocks at a time
+                parallel_for(n, [&](size_t q, std::vector<uint8_t> &) {
+                    if (!good[q]) return;
+                    const Hash &h = hs[b0 + which[q]];
+                    pending[which[q]] = 0;
+                    int who[64];
+                    storage_nodes_of(h, who);
+                    const size_t L = shard_len_of(lens[q]);
+                    int stored = 0;
+                    for (int i = 0; i < tot; i++)  // only a durable write counts towards the quorum
+                        stored += write_converted(who[i], h, i, lens[q], dst + (q * tot + i) * slot_stride, L,
+                                                  sums + (q * tot + i) * 32);
+                    {
+                        std::lock_guard<std::mutex> lk(refs_mu);
+                        refs[h] = lens[q];
+                    }
+                    if (stored < quorum) {
+                        convert_errors++;  // every legacy copy stays; the next sweep tries again
+                        return;
+                    }
+                    convert_blocks++;
+                    converted++;
+                    for (int i = 0; i < legacy_row(); i++) delete_legacy(ring_node(h, i), h);
+                });
+            }
+            for (size_t j = 0; j < nb; j++) convert_errors += pending[j];
+        }
+        return converted;
+    }
+    // fn(i, per-thread scratch) for i < n on up to 16 threads (reads, content hashes and writes of a batch)
+    static void parallel_for(size_t n, const std::function<void(size_t, std::vector<uint8_t> &)> &fn)
+    {
+        const size_t nt = std::min<size_t>(n, std::min(16u, std::max(1u, std::thread::hardware_concurrency())));
+        std::atomic<size_t> next{0};
+        auto run = [&] {
+            std::vector<uint8_t> tmp;
+            for (size_t i; (i = next++) < n;) fn(i, tmp);
+        };
+        std::vector<std::thread> th;
+        for (size_t t = 1; t < nt; t++) th.emplace_back(run);
+        run();
+        for (auto &t : th) t.join();
+    }
+
+    // garage_bm_convert_step: see include/garage_block_manager.h
+    int convert_step(int node, const Hash *cursor, size_t max_blocks, Hash *cursor_out, int *finished, uint64_t *converted)
+    {
+        Node &nd = *nodes[node];
+        std::vector<Hash> hs;
+        {
+            std::lock_guard<std::mutex> lk(nd.mu);
+            if (!nd.up) return GARAGE_BM_E_MESSAGE;
+            if (!nd.dir.empty() && has_legacy()) {
+                std::vector<Hash> all;
+                nd.store_list(all, true);
+                for (const Hash &h : all)
+                    if (nd.has_legacy_shard(h) || nd.has_replica(h)) hs.push_back(h);
+            }
+        }
+        std::sort(hs.begin(), hs.end());
+        hs.erase(std::unique(hs.begin(), hs.end()), hs.end());
+        if (cursor) hs.erase(hs.begin(), std::upper_bound(hs.begin(), hs.end(), *cursor));
+        bool done = true;
+        if (max_blocks && hs.size() > max_blocks) {
+            hs.resize(max_blocks);
+            done = false;
+        }
+        if (finished) *finished = done ? 1 : 0;
+        if (cursor_out) {
+            if (!hs.empty()) *cursor_out = hs.back();
+            else if (cursor) *cursor_out = *cursor;
+            else cursor_out->fill(0);
+        }
+        std::vector<Hash> todo;
+        for (const Hash &h : hs) {
+            {
+                // rc 0: never converted; the legacy copies go once the GC delay has passed, decided and deleted under
+                // both locks like resync_block's offload branch
+                std::lock_guard<std::mutex> rl(refs_mu);
+                auto it = rc.find(h);
+                if (it != rc.end() && it->second.count <= 0) {
+                    if (deletable_now(h)) delete_legacy(node, h);
+                    continue;
+                }
+            }
+            if (configured_at_quorum(h)) delete_legacy(node, h);  // converted already
+            else if (converter_of(h) == node) todo.push_back(h);
+        }
+        const size_t n = todo.empty() ? 0 : convert_batch(todo);
+        if (converted) *converted = n;
         return GARAGE_BM_OK;
     }
 
@@ -1434,9 +1931,10 @@ struct garage_bm {
         {
             std::lock_guard<std::mutex> lk(nd.mu);
             if (!nd.up) return GARAGE_BM_E_MESSAGE;
-            nd.store_list(hashes);
+            nd.store_list(hashes, has_legacy());
         }
         std::sort(hashes.begin(), hashes.end());
+        hashes.erase(std::unique(hashes.begin(), hashes.end()), hashes.end());
         if (cursor) hashes.erase(hashes.begin(), std::upper_bound(hashes.begin(), hashes.end(), *cursor));
         bool done = true;
         if (max_shards && hashes.size() > max_shards) {
@@ -1449,22 +1947,59 @@ struct garage_bm {
             else if (cursor) *cursor_out = *cursor;
             else cursor_out->fill(0);
         }
+        // the files to check: (hash, 0) the .shard; with previous codes or replicas configured also (hash, 1) a .legacy
+        // shard and (hash, 2) a replica
+        const bool legacy = has_legacy() && !nd.dir.empty();
+        std::vector<std::pair<Hash, int>> items;
+        {
+            std::lock_guard<std::mutex> lk(nd.mu);
+            for (const Hash &h : hashes) {
+                if (!legacy || nd.file_code(nd.path_of(h, ".shard")) != -2) items.emplace_back(h, 0);
+                if (legacy && nd.file_code(nd.path_of(h, ".legacy")) != -2) items.emplace_back(h, 1);
+                if (legacy && nd.has_replica(h)) items.emplace_back(h, 2);
+            }
+        }
         uint64_t nchecked = 0, nbad = 0;
         const size_t chunk = std::max<size_t>(1, (size_t)cfg.batch_max_blocks * tot);
         const size_t stride = slot_stride;
-        for (size_t c0 = 0; c0 < hashes.size(); c0 += chunk) {
-            const size_t n = std::min(chunk, hashes.size() - c0);
+        std::vector<uint8_t> replica;
+        for (size_t c0 = 0; c0 < items.size(); c0 += chunk) {
+            const size_t n = std::min(chunk, items.size() - c0);
             uint8_t *buf = scrub_buf.get(n * stride + n * 32 + n + n * 4);
             if (!buf) return GARAGE_EC_E_NOMEM;
             uint8_t *expect = buf + n * stride, *bad = expect + n * 32;
             std::vector<uint32_t> lens(n, 0);
             std::vector<uint8_t> state(n, 0);  // 0 gone, 1 to be checked on the GPU, 2 corrupt already, 3 checked on the CPU
+            std::vector<int> code(n, 0);       // the code the file holds a shard of (-1: a replica)
             {
                 std::lock_guard<std::mutex> lk(nd.mu);
                 for (size_t i = 0; i < n; i++) {
                     ShardMeta mt;
                     memset(expect + i * 32, 0, 32);
-                    const ReadResult r = nd.store_read_into(hashes[c0 + i], buf + i * stride, stride, mt);
+                    const Hash &h = items[c0 + i].first;
+                    const int kind = items[c0 + i].second;
+                    ReadResult r;
+                    if (kind == 2) {  // a replica is checked against its content hash
+                        replica.resize(cfg.block_size);
+                        uint32_t len = 0;
+                        code[i] = -1;
+                        r = nd.replica_read_into(h, replica.data(), replica.size(), len);
+                        if (r == kReadMissing) continue;
+                        Hash got;
+                        if (r == kReadOk) {
+                            bytes_read += len;
+                            garage_ec_blake2sum(replica.data(), len, got.data());
+                        }
+                        state[i] = r == kReadOk && got == h ? 3 : 2;
+                        continue;
+                    }
+                    if (!legacy) {
+                        r = nd.store_read_into(h, buf + i * stride, stride, mt);
+                    } else {  // read the file as the code its header names; an unknown code is corrupt, as before
+                        const std::string path = nd.path_of(h, kind ? ".legacy" : ".shard");
+                        code[i] = std::max(kind, nd.file_code(path));
+                        r = nd.file_read_into(path, code[i], buf + i * stride, stride, mt);
+                    }
                     if (r == kReadMissing) continue;
                     if (r == kReadInvalid) {
                         state[i] = 2;
@@ -1490,7 +2025,7 @@ struct garage_bm {
                 nchecked++;
                 if (state[i] == 3 || (state[i] == 1 && !bad[i])) continue;
                 nbad++;
-                quarantine(node, hashes[c0 + i]);
+                quarantine(node, items[c0 + i].first, code[i]);
             }
         }
         scrub_checked += nchecked;
@@ -1627,6 +2162,19 @@ void garage_bm_default_config(garage_bm_config *c)
     c->block_gc_delay_ms = 600000;  // BLOCK_GC_DELAY, manager.rs:49-52
     c->local_groups = 0;            // RS
     c->piggyback = 0;
+    c->previous_codes = nullptr;    // no code change in progress
+    c->n_previous_codes = 0;
+    c->legacy_replicas = 0;
+}
+
+// a code garage_ec_create / _lrc / _piggyback accepts, with tags the block manager can check: the same rules as the
+// configured code's (PB: 1 <= k <= 16, 2 <= m <= 4, no LRC groups, adler8 tags)
+static bool code_ok(int k, int m, int l, int piggyback, int sum_kind)
+{
+    if (k < 1 || m < 1 || k > GARAGE_EC_MAX_K || m > GARAGE_EC_MAX_M) return false;
+    if (l < 0 || (l > 0 && (l >= m || k % l))) return false;
+    if (piggyback != 0 && piggyback != 1) return false;
+    return !piggyback || (l == 0 && k <= 16 && m >= 2 && m <= 4 && sum_kind != GARAGE_EC_SUM_BLAKE2);
 }
 
 static int bm_create(garage_bm **out, const garage_bm_config *cfg)
@@ -1642,6 +2190,21 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
     // PB is not combined with LRC, and its half reads need per-segment (adler8) tags
     if ((cfg->piggyback != 0 && cfg->piggyback != 1) || (pb && (l > 0 || cfg->shard_sum_kind == GARAGE_EC_SUM_BLAKE2)))
         return GARAGE_EC_E_INVALID;
+    // previous codes and replicas (all checked before any CUDA call)
+    const int np = cfg->n_previous_codes;
+    if (np < 0 || np > GARAGE_BM_MAX_PREVIOUS_CODES || (np > 0 && !cfg->previous_codes)) return GARAGE_EC_E_INVALID;
+    if (cfg->legacy_replicas < 0 || cfg->legacy_replicas > cfg->n_nodes) return GARAGE_EC_E_INVALID;
+    for (int i = 0; i < np; i++) {
+        const garage_bm_code &p = cfg->previous_codes[i];
+        if (!code_ok(p.k, p.m, p.local_groups, p.piggyback, cfg->shard_sum_kind) || p.k + p.m > cfg->n_nodes)
+            return GARAGE_EC_E_INVALID;
+        if (p.k == k && p.m == m && p.local_groups == l && (p.piggyback != 0) == pb) return GARAGE_EC_E_INVALID;
+        for (int j = 0; j < i; j++) {
+            const garage_bm_code &q = cfg->previous_codes[j];
+            if (p.k == q.k && p.m == q.m && p.local_groups == q.local_groups && p.piggyback == q.piggyback)
+                return GARAGE_EC_E_INVALID;
+        }
+    }
     // every context of the manager runs the same code: RS(k, m), LRC(k, l, m - l) or PB(k, m)
     auto make_ctx = [&](garage_ec_ctx **c) {
         return pb ? garage_ec_create_piggyback(c, cfg->cuda_device, k, m, GARAGE_EC_VANDERMONDE)
@@ -1659,7 +2222,35 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
     int rc = make_ctx(&bm->ec);
     if (rc != GARAGE_EC_OK) return rc;  // no GPU => no block manager: there is no CPU fallback
     garage_ec_set_sum_kind(bm->ec, bm->sum_kind);
+    bm->codes.resize(1 + np);
+    bm->codes[0].k = k;
+    bm->codes[0].m = m;
+    bm->codes[0].l = l;
+    bm->codes[0].pb = pb;
+    bm->codes[0].tot = k + m;
+    bm->codes[0].ctx = bm->ec;
+    bm->legacy_rf = cfg->legacy_replicas;
+    bm->cfg.previous_codes = nullptr;  // not kept: the caller's array may go away
     bm->slot_stride = garage_ec_stride_for((uint32_t)bm->shard_len_of(bm->cfg.block_size));
+    for (int i = 0; i < np; i++) {  // one context per previous code, same tag kind and matrices as the configured one
+        const garage_bm_code &p = cfg->previous_codes[i];
+        garage_bm::Code &c = bm->codes[1 + i];
+        c.k = p.k;
+        c.m = p.m;
+        c.l = p.local_groups;
+        c.pb = p.piggyback != 0;
+        c.tot = p.k + p.m;
+        rc = c.pb ? garage_ec_create_piggyback(&c.ctx, cfg->cuda_device, p.k, p.m, GARAGE_EC_VANDERMONDE)
+             : c.l ? garage_ec_create_lrc(&c.ctx, cfg->cuda_device, p.k, c.l, p.m - c.l)
+                   : garage_ec_create(&c.ctx, cfg->cuda_device, p.k, p.m, GARAGE_EC_VANDERMONDE);
+        if (rc != GARAGE_EC_OK) {
+            garage_bm_destroy(bm.release());
+            return rc;
+        }
+        garage_ec_set_sum_kind(c.ctx, bm->sum_kind);
+        // slots and the scrub buffer hold a shard of the largest code in play
+        bm->slot_stride = std::max(bm->slot_stride, garage_ec_stride_for((uint32_t)bm->shard_len_of(bm->cfg.block_size, 1 + i)));
+    }
     if (cfg->n_nodes <= GARAGE_LAYOUT_MAX_NODES) {
         const int n = cfg->n_nodes, tot = k + m;
         std::vector<uint8_t> ring((size_t)GARAGE_NB_PARTITIONS * tot);
@@ -1677,18 +2268,30 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
         nd.m = m;
         nd.l = cfg->local_groups;
         nd.pb = pb;
+        nd.codes.assign(1, bm->codes[0]);
         nd.fsync_data = cfg->data_fsync != 0;
         if (cfg->data_dir && cfg->data_dir[0]) {
             nd.dir = std::string(cfg->data_dir) + "/node" + std::to_string(i);
+            nd.codes.assign(bm->codes.begin(), bm->codes.end());  // previous codes exist on disk only
+            nd.replicas = bm->legacy_rf > 0;
             std::error_code ec;
             std::filesystem::create_directories(nd.dir, ec);
-            // restart: what is on disk is what exists (the block_ref table would say the same)
+            // restart: what is on disk is what exists (the block_ref table would say the same), shards of previous
+            // codes and replicas included
             std::vector<Hash> have;
-            nd.store_list(have);
+            nd.store_list(have, bm->has_legacy());
             std::vector<uint8_t> tmp(bm->slot_stride);
             for (const Hash &h : have) {
                 ShardMeta mt;
-                if (nd.store_read_into(h, tmp.data(), tmp.size(), mt) == kReadOk) bm->refs[h] = mt.block_len;
+                struct stat sb;
+                for (int c = 0; c < (int)nd.codes.size(); c++)
+                    if (nd.store_read_into(h, tmp.data(), tmp.size(), mt, -1, c) == kReadOk) {
+                        bm->refs[h] = mt.block_len;
+                        break;
+                    }
+                if (!bm->refs.count(h) && nd.has_replica(h) && ::stat(nd.path_of(h, "").c_str(), &sb) == 0 && sb.st_size > 0 &&
+                    (uint64_t)sb.st_size <= bm->cfg.block_size)
+                    bm->refs[h] = (uint32_t)sb.st_size;
             }
         }
     }
@@ -1718,7 +2321,10 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
     }
     const size_t nslots = (size_t)std::max<uint32_t>(cfg->batch_max_blocks, 1) * (garage_bm::kWorkers + 1);
     if (!bm->put_slots.init(bm->ec, nslots, bm->cfg.block_size)) return destroy_on_error(GARAGE_EC_E_NOMEM);
-    if (!bm->stripe_slots.init(bm->ec, nslots, (size_t)bm->tot * bm->slot_stride)) return destroy_on_error(GARAGE_EC_E_NOMEM);
+    int max_tot = bm->tot;  // a stripe slot holds a stripe of any code in play
+    for (const auto &c : bm->codes) max_tot = std::max(max_tot, c.tot);
+    if (!bm->stripe_slots.init(bm->ec, nslots, (size_t)max_tot * bm->slot_stride)) return destroy_on_error(GARAGE_EC_E_NOMEM);
+    bm->conv_src.ctx = bm->conv_dst.ctx = bm->conv_blk.ctx = bm->ec;
     // Warm every dispatcher's context now: streams, lane buffers, and the first launch of each kernel (CUDA
     // loads kernels lazily) cost tens of milliseconds that would otherwise land on the first real batches.
     {
@@ -1775,10 +2381,17 @@ void garage_bm_destroy(garage_bm *bm)
         ctxs[2 * w + 1] = bm->rec_ctx[w];
     }
     bm->scrub_buf.release();
+    bm->conv_src.release();
+    bm->conv_dst.release();
+    bm->conv_blk.release();
     bm->put_slots.destroy();
     bm->stripe_slots.destroy();
+    std::vector<garage_ec_ctx *> previous;
+    for (size_t c = 1; c < bm->codes.size(); c++) previous.push_back(bm->codes[c].ctx);
     delete bm;
     for (garage_ec_ctx *c : ctxs)
+        if (c) garage_ec_destroy(c);
+    for (garage_ec_ctx *c : previous)
         if (c) garage_ec_destroy(c);
     if (ec) garage_ec_destroy(ec);
 }
@@ -1854,6 +2467,30 @@ int garage_bm_scrub_step(garage_bm *bm, int node, const uint8_t *cursor32, size_
     } catch (...) {
         return GARAGE_BM_E_MESSAGE;
     }
+}
+
+int garage_bm_convert_step(garage_bm *bm, int node, const uint8_t *cursor32, size_t max_blocks, uint8_t cursor_out32[32],
+                           int *finished, uint64_t *converted)
+{
+    if (!bm || node < 0 || node >= (int)bm->nodes.size()) return GARAGE_EC_E_INVALID;
+    try {
+        Hash cur, out;
+        if (cursor32) cur = to_hash(cursor32);
+        int rc = bm->convert_step(node, cursor32 ? &cur : nullptr, max_blocks, &out, finished, converted);
+        if (rc == GARAGE_BM_OK && cursor_out32) memcpy(cursor_out32, out.data(), 32);
+        return rc;
+    } catch (const std::bad_alloc &) {
+        return GARAGE_EC_E_NOMEM;
+    } catch (...) {
+        return GARAGE_BM_E_MESSAGE;
+    }
+}
+
+int garage_bm_debug_convert_stop_after(garage_bm *bm, long n_ops)
+{
+    if (!bm) return GARAGE_EC_E_INVALID;
+    bm->convert_ops_left.store(n_ops < 0 ? -1 : n_ops);
+    return GARAGE_BM_OK;
 }
 
 int garage_bm_bench(garage_bm *bm, int threads, int blocks_per_thread, uint32_t block_len, int mode, uint64_t seed,
@@ -2019,6 +2656,13 @@ void garage_bm_get_metrics(garage_bm *bm, garage_bm_metrics *o)
     o->write_errors = bm->write_errors;
     o->resync_shards_read = bm->resync_shards_read;
     o->resync_bytes_read = bm->resync_bytes_read;
+    o->convert_blocks = bm->convert_blocks;
+    o->convert_bytes_read = bm->convert_bytes_read;
+    o->convert_bytes_written = bm->convert_bytes_written;
+    o->convert_errors = bm->convert_errors;
+    o->convert_call_us = bm->convert_call_us;
+    o->legacy_gets = bm->legacy_gets;
+    o->legacy_deleted = bm->legacy_deleted;
     uint64_t ql = 0;
     for (auto &n : bm->nodes) {
         std::lock_guard<std::mutex> lk(n->mu);

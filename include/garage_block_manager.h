@@ -42,6 +42,15 @@ extern "C" {
 
 typedef struct garage_bm garage_bm;
 
+/* a code the store may still hold shards of: RS(k, m), LRC(k, local_groups, m - local_groups) or PB(k, m) */
+typedef struct {
+    int k, m;
+    int local_groups; /* 0: not LRC */
+    int piggyback;    /* 0 or 1 */
+} garage_bm_code;
+
+#define GARAGE_BM_MAX_PREVIOUS_CODES 4
+
 typedef struct {
     int data_shards;                /* k  (config: erasure_coding.data_shards)   */
     int parity_shards;              /* m                                          */
@@ -70,6 +79,16 @@ typedef struct {
                                        halves for one lost data shard.  GARAGE_EC_E_INVALID with local_groups > 0 or
                                        shard_sum_kind = GARAGE_EC_SUM_BLAKE2.  Recorded in the shard file header; a
                                        shard of another code is quarantined                                       */
+    /* Changing a store's code (file store; DESIGN.md section 5.1).  Default: none, and a shard of any code but the
+       configured one is quarantined.  GARAGE_EC_E_INVALID before any CUDA call for: more than
+       GARAGE_BM_MAX_PREVIOUS_CODES entries, a NULL list with entries, an entry equal to the configured code or to
+       another entry, an entry garage_ec_create* would reject or with more than n_nodes shards, a PB entry with
+       GARAGE_EC_SUM_BLAKE2 tags, legacy_replicas < 0 or > n_nodes.                                               */
+    const garage_bm_code *previous_codes; /* codes whose shards are read and converted (old .shard / .legacy files) */
+    int n_previous_codes;
+    int legacy_replicas;            /* replication factor of a previous replicated layout (0 = none): whole-block
+                                       files <node dir>/<hh>/<hh>/<64 hex> on the first legacy_replicas nodes of the
+                                       block's ring row, read and converted like a previous code                   */
 } garage_bm_config;
 
 typedef struct {
@@ -88,6 +107,13 @@ typedef struct {
                                                 set of garage_ec_read_set: k for RS, k/l for an LRC
                                                 local repair)                                       */
     uint64_t resync_bytes_read;              /* bytes read by that fetch branch (PB reads half shards) */
+    uint64_t convert_blocks;                 /* blocks rewritten under the configured code (>= k+1 shards stored) */
+    uint64_t convert_bytes_read;             /* legacy shard / replica bytes read by conversions               */
+    uint64_t convert_bytes_written;          /* configured-code shard bytes durably written by conversions      */
+    uint64_t convert_errors;                 /* conversions that failed (unrecoverable source, no write quorum) */
+    uint64_t convert_call_us;                /* wall time inside garage_ec_transcode                            */
+    uint64_t legacy_gets;                    /* GETs served from a previous code's stripe or a replica          */
+    uint64_t legacy_deleted;                 /* legacy shard / replica files deleted                            */
 } garage_bm_metrics;
 
 void garage_bm_default_config(garage_bm_config *cfg);
@@ -135,6 +161,18 @@ int garage_bm_scrub(garage_bm *bm, int node, uint64_t *checked, uint64_t *corrup
 int garage_bm_scrub_step(garage_bm *bm, int node, const uint8_t *cursor32, size_t max_shards,
                          uint8_t cursor_out32[32], int *finished, uint64_t *checked, uint64_t *corrupt);
 
+/* Conversion sweep of `node` (DESIGN.md section 5.1), resumable in hash order like garage_bm_scrub_step: every block
+ * with a legacy shard or replica on `node`, after cursor32 (NULL = from the start), at most max_blocks (0 = all):
+ *   - the configured stripe holds its write quorum: this node deletes its legacy copies;
+ *   - rc 0: the legacy copies are deleted once block_gc_delay_ms has passed, nothing is converted;
+ *   - this node is the block's converter (the first up node holding a legacy copy, in code order, shard index
+ *     order, then replica order): the old data shards (or the replica) go through garage_ec_transcode in batches
+ *     of batch_max_blocks, the new data shards are checked against the content hash before anything is written,
+ *     the k+m new shards are written, and once k+1 are durable the legacy copies on the up nodes are deleted.
+ * *converted = blocks this call converted.  A block that could not be converted keeps every legacy copy.        */
+int garage_bm_convert_step(garage_bm *bm, int node, const uint8_t *cursor32, size_t max_blocks, uint8_t cursor_out32[32],
+                           int *finished, uint64_t *converted);
+
 /* native closed-loop load generator (row f1: the batching front-end decides real-world throughput):
  * `threads` client threads each PUT (mode 0) or GET (mode 1) `blocks_per_thread` blocks of `block_len`
  * bytes (splitmix64 stream of `seed`; a GET run must follow a PUT run with the same arguments).  The
@@ -153,6 +191,9 @@ int garage_bm_plant_stale_shard(garage_bm *bm, int node, const uint8_t hash[32])
 /* file store only: make every write to the node's directory fail (like ENOSPC / EACCES / a lost mount) */
 int garage_bm_set_node_readonly(garage_bm *bm, int node, int readonly);
 int garage_bm_drop_shard(garage_bm *bm, int node, const uint8_t hash[32]);
+/* after n_ops more file operations of conversions (renames to .legacy, shard writes, legacy deletes), make every
+ * further one fail, as if the process had stopped there; n_ops < 0 turns it off                                  */
+int garage_bm_debug_convert_stop_after(garage_bm *bm, long n_ops);
 int garage_bm_node_shard_index(garage_bm *bm, int node, const uint8_t hash[32]); /* -1 if none */
 int garage_bm_storage_nodes_of(garage_bm *bm, const uint8_t hash[32], int *nodes_out /* k+m */);
 void garage_bm_get_metrics(garage_bm *bm, garage_bm_metrics *out);
