@@ -18,7 +18,8 @@ SYMBOLS = [
     "garage_bm_drop_shard", "garage_bm_node_shard_index", "garage_bm_storage_nodes_of", "garage_bm_get_metrics",
     "garage_bm_block_incref", "garage_bm_block_decref", "garage_bm_get_block_rc", "garage_bm_scrub_step",
     "garage_bm_bench", "garage_bm_corrupt_shard_header", "garage_bm_plant_stale_shard", "garage_bm_set_node_readonly",
-    "garage_bm_convert_step", "garage_bm_debug_convert_stop_after",
+    "garage_bm_convert_step", "garage_bm_debug_convert_stop_after", "garage_bm_apply_layout", "garage_bm_layout_sync_step",
+    "garage_bm_layout_versions",
 ]
 SUM_BLAKE2, SUM_ADLER8 = 0, 1
 
@@ -28,13 +29,27 @@ class Code(C.Structure):
     _fields_ = [("k", C.c_int), ("m", C.c_int), ("local_groups", C.c_int), ("piggyback", C.c_int)]
 
 
+class LayoutSpec(C.Structure):
+    """garage_bm_layout_spec: one layout version over the manager's n_nodes node stores"""
+    _fields_ = [("zone", C.POINTER(C.c_int32)), ("capacity", C.POINTER(C.c_uint64)), ("zone_redundancy", C.c_int),
+                ("max_per_zone", C.c_int)]
+
+
+def _layout_spec(zone, capacity, zone_redundancy=0, max_per_zone=0):
+    """-> (LayoutSpec, the arrays it points into: keep them alive while the spec is used)"""
+    z = (C.c_int32 * max(1, len(zone)))(*map(int, zone))
+    c = (C.c_uint64 * max(1, len(capacity)))(*map(int, capacity))
+    return LayoutSpec(C.cast(z, C.POINTER(C.c_int32)), C.cast(c, C.POINTER(C.c_uint64)), zone_redundancy, max_per_zone), (z, c)
+
+
 class Config(C.Structure):
     _fields_ = [("data_shards", C.c_int), ("parity_shards", C.c_int), ("cuda_device", C.c_int),
                 ("n_nodes", C.c_int), ("block_size", C.c_uint32), ("block_ram_buffer_max", C.c_uint64),
                 ("batch_max_blocks", C.c_uint32), ("batch_linger_us", C.c_uint32), ("data_dir", C.c_char_p),
                 ("shard_sum_kind", C.c_int), ("verify_content_hash", C.c_int), ("data_fsync", C.c_int),
                 ("block_gc_delay_ms", C.c_uint32), ("local_groups", C.c_int), ("piggyback", C.c_int),
-                ("previous_codes", C.POINTER(Code)), ("n_previous_codes", C.c_int), ("legacy_replicas", C.c_int)]
+                ("previous_codes", C.POINTER(Code)), ("n_previous_codes", C.c_int), ("legacy_replicas", C.c_int),
+                ("layout", C.POINTER(LayoutSpec))]
 
 
 class Metrics(C.Structure):
@@ -44,7 +59,8 @@ class Metrics(C.Structure):
         "reconstruct_batches", "scrub_shards_checked", "scrub_corruptions", "resync_queue_length",
         "encode_call_us", "reconstruct_call_us", "corrupt_data_errors", "write_errors", "resync_shards_read", "resync_bytes_read",
         "convert_blocks", "convert_bytes_read", "convert_bytes_written", "convert_errors", "convert_call_us", "legacy_gets",
-        "legacy_deleted")]
+        "legacy_deleted", "layout_shards_copied", "layout_shards_rebuilt", "layout_bytes_read", "layout_bytes_written",
+        "layout_deleted", "layout_sync_errors", "layout_version")]
 
 
 _lib = None
@@ -87,6 +103,9 @@ def load_library():
         L.garage_bm_set_node_readonly.argtypes = [vp, i32, i32]
         L.garage_bm_convert_step.argtypes = [vp, i32, vp, sz, vp, C.POINTER(i32), C.POINTER(C.c_uint64)]
         L.garage_bm_debug_convert_stop_after.argtypes = [vp, C.c_long]
+        L.garage_bm_apply_layout.argtypes = [vp, C.POINTER(LayoutSpec), C.POINTER(C.c_uint64)]
+        L.garage_bm_layout_sync_step.argtypes = [vp, i32, vp, sz, vp, C.POINTER(i32), C.POINTER(C.c_uint64)]
+        L.garage_bm_layout_versions.argtypes = [vp, C.POINTER(C.c_uint64), i32]
         _lib = L
     return _lib
 
@@ -111,11 +130,13 @@ class BlockManager:
     def __init__(self, k=10, m=4, n_nodes=None, cuda_device=0, batch_max_blocks=64, batch_linger_us=100,
                  block_ram_buffer_max=256 << 20, data_dir=None, shard_sum_kind=SUM_ADLER8, verify_content_hash=True,
                  data_fsync=False, block_gc_delay_ms=0, local_groups=0, piggyback=False, previous_codes=(),
-                 legacy_replicas=0):
+                 legacy_replicas=0, layout=None):
         """block_gc_delay_ms defaults to 0 HERE (tests delete at once); the library's default is the
         reference's BLOCK_GC_DELAY of 10 minutes.  local_groups > 0: LRC(k, local_groups, m - local_groups).
         piggyback: PB(k, m), half-shard repair reads.  previous_codes: (k, m, local_groups, piggyback) tuples of
-        codes the store may still hold; legacy_replicas: replication factor of a previous replicated layout."""
+        codes the store may still hold; legacy_replicas: replication factor of a previous replicated layout.
+        layout: None (partition p on nodes (p mod n_nodes) + i) or a dict with zone, capacity and optionally
+        zone_redundancy, max_per_zone: version 1 of the cluster layout."""
         self._L = load_library()
         cfg = Config()
         self._L.garage_bm_default_config(C.byref(cfg))
@@ -132,11 +153,15 @@ class BlockManager:
         cfg.n_previous_codes, cfg.legacy_replicas = len(previous_codes), legacy_replicas
         self._dir = data_dir.encode() if data_dir else None  # keep the bytes alive
         cfg.data_dir = self._dir
+        if layout is not None:
+            self._spec, self._spec_arrays = _layout_spec(**layout)  # kept alive
+            cfg.layout = C.pointer(self._spec)
         h = C.c_void_p()
         rc = self._L.garage_bm_create(C.byref(h), C.byref(cfg))
         if rc != OK:
             raise BlockManagerError(rc)
         self._h, self.k, self.m, self.n_nodes = h, k, m, cfg.n_nodes
+        self._down = set()  # nodes set down through set_node_up
 
     def close(self):
         if getattr(self, "_h", None):
@@ -225,8 +250,46 @@ class BlockManager:
     def debug_convert_stop_after(self, n_ops):
         return self._L.garage_bm_debug_convert_stop_after(self._h, n_ops)
 
+    def apply_layout(self, zone, capacity, zone_redundancy=0, max_per_zone=0):
+        """-> (rc, new version)"""
+        spec, keep = _layout_spec(zone, capacity, zone_redundancy, max_per_zone)
+        v = C.c_uint64(0)
+        rc = self._L.garage_bm_apply_layout(self._h, C.byref(spec), C.byref(v))
+        del keep
+        return rc, v.value
+
+    def layout_sync_step(self, node, cursor=None, max_blocks=0):
+        """-> (rc, cursor_out bytes, finished, shards moved)"""
+        out = C.create_string_buffer(32)
+        fin, n = C.c_int(0), C.c_uint64(0)
+        rc = self._L.garage_bm_layout_sync_step(self._h, node, C.c_char_p(bytes(cursor)) if cursor else None, max_blocks,
+                                                C.cast(out, C.c_void_p), C.byref(fin), C.byref(n))
+        return rc, out.raw, bool(fin.value), n.value
+
+    def layout_sync_all(self, nodes=None):
+        """one full layout_sync_step pass over every node that is up (or over `nodes`) -> shards moved; an error from
+        a node that is up raises BlockManagerError"""
+        total = 0
+        for node in (range(self.n_nodes) if nodes is None else nodes):
+            if node in self._down:
+                continue
+            rc, _, finished, n = self.layout_sync_step(node)
+            if rc != OK:
+                raise BlockManagerError(rc)
+            assert finished
+            total += n
+        return total
+
+    def layout_versions(self):
+        out = (C.c_uint64 * 8)()
+        n = self._L.garage_bm_layout_versions(self._h, out, 8)
+        return list(out[:n])
+
     def set_node_up(self, node, up):
-        return self._L.garage_bm_set_node_up(self._h, node, 1 if up else 0)
+        rc = self._L.garage_bm_set_node_up(self._h, node, 1 if up else 0)
+        if rc == OK:
+            (self._down.discard if up else self._down.add)(node)
+        return rc
 
     def corrupt_shard(self, node, hash32, byte_off=0):
         return self._L.garage_bm_corrupt_shard(self._h, node, self._hp(hash32), byte_off)

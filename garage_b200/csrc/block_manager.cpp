@@ -21,6 +21,8 @@
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
+#include <cctype>
+#include <cerrno>
 #include <cstddef>
 #include <cstdio>
 #include <cstring>
@@ -32,6 +34,7 @@
 #include <mutex>
 #include <new>
 #include <string>
+#include <type_traits>
 #include <thread>
 #include <unordered_map>
 #include <unordered_set>
@@ -282,6 +285,9 @@ struct Node {
     bool pb = false;
     std::vector<CodeDesc> codes;  // [0] the configured code, then garage_bm_config.previous_codes (file store only)
     bool replicas = false;        // legacy_replicas > 0: whole-block replica files are read, listed and converted
+    // the store has a layout file (DESIGN.md section 5.2): a node may hold two indices of a block, the newest version's
+    // in .shard and an older version's in .legacy, and readers of a given index pick the file by its header
+    std::atomic<bool> by_index{false};
     // in-memory mode: immutable shards behind shared pointers, so the node lock only covers the map operation -- the
     // 100 KB copies happen outside it (the reference shards its lock 256 ways per node, manager.rs:114,679-689; with
     // one lock per node and the copies inside it, 128 clients serialised on 14 mutexes at ~12 GiB/s)
@@ -337,6 +343,38 @@ struct Node {
         const std::string lg = path_of(h, ".legacy");
         const int c2 = file_code(lg);
         return c2 == code || c2 == -1 ? lg : std::string();
+    }
+    // the shard index a configured-code file's header names: -1 for another code or a damaged header, -2 if the file
+    // does not exist
+    int file_index(const std::string &path) const
+    {
+        FILE *f = fopen(path.c_str(), "rb");
+        if (!f) return -2;
+        ShardFileHeader hd;
+        int i = -1;
+        if (fread(&hd, sizeof(hd), 1, f) == 1 && memcmp(hd.magic, "GEC1", 4) == 0 &&
+            hd.hdr_check == adler32_small(reinterpret_cast<const uint8_t *>(&hd), 48) && codes[0].named_by(hd))
+            i = hd.index;
+        fclose(f);
+        return i;
+    }
+    // the file holding shard `index` of h ("" = none): .shard or .legacy, whichever header names that index
+    std::string path_at(const Hash &h, int index) const
+    {
+        const std::string sh = path_of(h, ".shard"), lg = path_of(h, ".legacy");
+        if (file_index(sh) == index) return sh;
+        return file_index(lg) == index ? lg : std::string();
+    }
+    // where shard `index` of h goes when the newest layout version gives this node `newest` (-1: none).  .shard holds
+    // the newest index, or the only one the node holds; *aside = .shard must first move to .legacy.
+    const char *place_for(const Hash &h, int index, int newest, bool *aside) const
+    {
+        const int si = file_index(path_of(h, ".shard"));
+        *aside = false;
+        if (si < 0 || si == index) return ".shard";
+        if (index != newest) return ".legacy";
+        *aside = true;
+        return ".shard";
     }
     bool has_legacy_shard(const Hash &h) const
     {
@@ -396,9 +434,9 @@ struct Node {
         return r;
     }
     void replica_quarantine(const Hash &h) { ::rename(path_of(h, "").c_str(), path_of(h, ".corrupted").c_str()); }
-    bool store_put(const Hash &h, const ShardMeta &mt, const uint8_t *bytes, size_t n)
+    bool store_put(const Hash &h, const ShardMeta &mt, const uint8_t *bytes, size_t n, const char *ext = ".shard")
     {
-        if (!dir.empty() && !store_move_legacy_aside(h)) return false;
+        if (!dir.empty() && strcmp(ext, ".shard") == 0 && !store_move_legacy_aside(h)) return false;
         if (dir.empty()) {
             auto sp = std::make_shared<StoredShard>();
             static_cast<ShardMeta &>(*sp) = mt;
@@ -409,7 +447,7 @@ struct Node {
         std::error_code ec;
         const std::string sub = dir + "/" + hex_of(h.data(), 1) + "/" + hex_of(h.data() + 1, 1);
         std::filesystem::create_directories(sub, ec);
-        const std::string fin = path_of(h, ".shard"), tmp = fin + ".tmp" + std::to_string((unsigned long)::getpid());
+        const std::string fin = path_of(h, ext), tmp = fin + ".tmp" + std::to_string((unsigned long)::getpid());
         ShardFileHeader hd;
         memset(&hd, 0, sizeof(hd));
         memcpy(hd.magic, "GEC1", 4);
@@ -443,13 +481,16 @@ struct Node {
     // shard bytes straight into `dst` (cap bytes available), metadata into `mt`.  half = 0 / 1: only the a- / b-half
     // [half * shard_len/2, (half+1) * shard_len/2) of a PB shard, one ranged read at 64 + half * shard_len/2 of the
     // file, into dst (which then holds shard_len/2 bytes)
-    ReadResult store_read_into(const Hash &h, uint8_t *dst, size_t cap, ShardMeta &mt, int half = -1, int code = 0) const
+    // index >= 0 (by_index stores): the file holding that index
+    ReadResult store_read_into(const Hash &h, uint8_t *dst, size_t cap, ShardMeta &mt, int half = -1, int code = 0,
+                               int index = -1) const
     {
         if (dir.empty()) {
             auto it = code == 0 ? shards.find(h) : shards.end();
             if (it == shards.end()) return kReadMissing;
             return copy_out(*it->second, dst, cap, mt, false, half);
         }
+        if (index >= 0 && by_index) return file_read_into(path_at(h, index), 0, dst, cap, mt, half);
         return file_read_into(path_for(h, code), code, dst, cap, mt, half);
     }
     // one shard file read as a shard of `code`
@@ -524,7 +565,8 @@ struct Node {
         if (dir.empty()) return shards.erase(h) != 0;
         return ::remove(path_of(h, ".shard").c_str()) == 0;
     }
-    void store_quarantine(const Hash &h, int code = 0)  // move_block_to_corrupted (manager.rs:807-819)
+    // move_block_to_corrupted (manager.rs:807-819).  index >= 0 (by_index stores): the file holding that index
+    void store_quarantine(const Hash &h, int code = 0, int index = -1)
     {
         if (dir.empty()) {
             auto it = shards.find(h);
@@ -534,7 +576,8 @@ struct Node {
             }
             return;
         }
-        const std::string p = codes.size() < 2 ? path_of(h, ".shard") : path_for(h, code);
+        std::string p = index >= 0 && by_index ? path_at(h, index) : std::string();
+        if (p.empty()) p = codes.size() < 2 ? path_of(h, ".shard") : path_for(h, code);
         if (!p.empty()) ::rename(p.c_str(), path_of(h, ".corrupted").c_str());
     }
     // BlockStoreIterator (repair.rs:634-764).  legacy: also hashes held only as a .legacy shard or a replica
@@ -549,7 +592,8 @@ struct Node {
              !ec && it != std::filesystem::recursive_directory_iterator(); it.increment(ec)) {
             const std::string name = it->path().filename().string();
             const bool listed = (name.size() == 64 + 6 && name.compare(64, 6, ".shard") == 0) ||
-                                (legacy && codes.size() >= 2 && name.size() == 64 + 7 && name.compare(64, 7, ".legacy") == 0) ||
+                                (legacy && (codes.size() >= 2 || by_index) && name.size() == 64 + 7 &&
+                                 name.compare(64, 7, ".legacy") == 0) ||
                                 (legacy && replicas && name.size() == 64 && it->is_regular_file(ec2));
             if (!listed) continue;
             Hash h;
@@ -629,6 +673,19 @@ public:
         cv_.notify_all();
         return f.get();
     }
+    // several items at once (one caller's whole batch): blocks until all are processed, their results in `rc`
+    void submit_all(const std::vector<Item *> &items, std::vector<int> &rc)
+    {
+        std::vector<std::future<int>> fs;
+        for (Item *it : items) fs.push_back(it->done.get_future());
+        {
+            std::lock_guard<std::mutex> lk(mu_);
+            q_.insert(q_.end(), items.begin(), items.end());
+        }
+        cv_.notify_all();
+        rc.resize(items.size());
+        for (size_t i = 0; i < fs.size(); i++) rc[i] = fs[i].get();
+    }
     uint64_t batches() const { return batches_.load(); }
     uint64_t items() const { return items_.load(); }
 
@@ -706,7 +763,24 @@ public:
             std::lock_guard<std::mutex> lk(mu_);
             free_.push_back(p);
         }
-        cv_.notify_one();
+        cv_.notify_all();  // a waiter for n slots must not swallow the wake-up a waiter for one needs
+    }
+    // n slots taken together: a caller never holds some while it waits for the rest (n <= the pool's size)
+    std::vector<uint8_t *> acquire_n(size_t n)
+    {
+        std::unique_lock<std::mutex> lk(mu_);
+        cv_.wait(lk, [&] { return free_.size() >= n; });
+        std::vector<uint8_t *> r(free_.end() - (std::ptrdiff_t)n, free_.end());
+        free_.resize(free_.size() - n);
+        return r;
+    }
+    void release_n(const std::vector<uint8_t *> &ps)
+    {
+        {
+            std::lock_guard<std::mutex> lk(mu_);
+            free_.insert(free_.end(), ps.begin(), ps.end());
+        }
+        cv_.notify_all();
     }
     size_t slot_bytes() const { return slot_bytes_; }
     void destroy()
@@ -872,6 +946,8 @@ struct garage_bm {
     std::atomic<uint64_t> put_ns_slot{0}, put_ns_land{0}, put_ns_wait{0}, put_ns_store{0};
     std::atomic<uint64_t> convert_blocks{0}, convert_bytes_read{0}, convert_bytes_written{0}, convert_errors{0},
         convert_call_us{0}, legacy_gets{0}, legacy_deleted{0};
+    std::atomic<uint64_t> layout_shards_copied{0}, layout_shards_rebuilt{0}, layout_bytes_read{0}, layout_bytes_written{0},
+        layout_deleted{0}, layout_sync_errors{0};
 
     bool pb = false;  // PB(k, m) contexts (garage_bm_config.piggyback)
     // codes[0]: the configured code (ctx = ec); codes[1..]: garage_bm_config.previous_codes, one context each.  Shard i
@@ -909,17 +985,48 @@ struct garage_bm {
     }
 
     // rpc/layout/version.rs:117-137: top 8 bits of the hash -> partition -> k+m distinct nodes, shard i on the
-    // i-th of them.  The ring is a garage_layout (row f4, include/garage_placement.h) filled at create with
-    // partition p -> nodes (p mod n) + i; any other ring (zones, capacities: garage_layout_compute) plugs in here.
-    garage_layout *layout = nullptr;
-    ~garage_bm() { garage_layout_free(layout); }
+    // i-th of them.  Each ring is a garage_layout (row f4, include/garage_placement.h): without garage_bm_config.layout
+    // version 1 is partition p -> nodes (p mod n) + i, otherwise garage_layout_compute's.  During a layout change
+    // (DESIGN.md section 5.2) several versions are active, oldest first; the set is replaced as a whole and readers
+    // work on a snapshot of it.
+    struct Layouts {
+        std::vector<std::shared_ptr<garage_layout>> v;
+        std::vector<std::vector<int32_t>> zone;      // per version: the spec it was computed from
+        std::vector<std::vector<uint64_t>> capacity;
+        const garage_layout *newest() const { return v.empty() ? nullptr : v.back().get(); }
+        std::vector<const garage_layout *> raw() const
+        {
+            std::vector<const garage_layout *> r;
+            for (auto &l : v) r.push_back(l.get());
+            return r;
+        }
+    };
+    std::shared_ptr<const Layouts> layouts_ = std::make_shared<Layouts>();
+    std::shared_ptr<const Layouts> layouts() const { return std::atomic_load(&layouts_); }
+    bool multi_version() const { return layouts()->v.size() > 1; }
+    std::mutex layout_mu;               // apply_layout, the sync bookkeeping below and the layout file
+    bool layout_file = false;           // a file store whose layout history is in <data_dir>/layout
+    std::vector<uint64_t> synced;       // per node: the newest version it has completed a sync pass of
+    std::vector<uint64_t> pass_version; // per node: the newest version when its current sync pass started (0 = none)
+    std::vector<uint8_t> pass_clean;    // per node: that pass has left nothing to receive so far
     void storage_nodes_of(const Hash &h, int *out) const
     {
         static_assert(sizeof(int) == sizeof(int32_t), "node ids are 32-bit");
-        if (layout && garage_layout_nodes_of(layout, h.data(), reinterpret_cast<int32_t *>(out)) == GARAGE_LAYOUT_OK) return;
+        auto ls = layouts();
+        if (ls->newest() && garage_layout_nodes_of(ls->newest(), h.data(), reinterpret_cast<int32_t *>(out)) == GARAGE_LAYOUT_OK)
+            return;
         const int n = (int)nodes.size();  // more nodes than a ring row can name: the same rule, computed
         const int p = h[0] % n;
         for (int i = 0; i < tot; i++) out[i] = (p + i) % n;
+    }
+    // the index the newest version gives `node` for h, -1 if none
+    int newest_index(const Hash &h, int node) const
+    {
+        int who[64];
+        storage_nodes_of(h, who);
+        for (int i = 0; i < tot; i++)
+            if (who[i] == node) return i;
+        return -1;
     }
 
     void put_to_resync(int node, const Hash &h)  // manager.rs:592-605 / resync.rs:put_to_resync
@@ -968,16 +1075,61 @@ struct garage_bm {
         else write_errors++;
         return ok;
     }
+    // write_shard on a store with a layout file: shard `index` takes the name Node::place_for gives it, after the
+    // newest version's index moved .shard aside.  counted: a layout sync's write; the rename and the write are each one
+    // file operation of garage_bm_debug_convert_stop_after.
+    bool write_shard_at(int node, const Hash &h, int index, uint32_t block_len, const uint8_t *bytes, size_t n,
+                        const uint8_t *sum32, bool counted)
+    {
+        Node &nd = *nodes[node];
+        if (nd.dir.empty() || !nd.by_index) {
+            if (counted && !convert_op_allowed()) return false;
+            return write_shard(node, h, index, block_len, bytes, n, sum32);
+        }
+        const int newest = newest_index(h, node);
+        ShardMeta mt;
+        mt.index = index;
+        mt.block_len = block_len;
+        mt.shard_len = (uint32_t)n;
+        mt.sum_kind = (uint8_t)sum_kind;
+        memcpy(mt.sum.data(), sum32, 32);
+        bool ok = true;
+        {
+            std::lock_guard<std::mutex> lk(nd.mu);
+            if (!nd.up) return false;
+            bool aside = false;
+            const char *ext = nd.place_for(h, index, newest, &aside);
+            if (aside)  // the same atomic rename (and directory fsync) as a code change's move to .legacy
+                ok = (!counted || convert_op_allowed()) &&
+                     ::rename(nd.path_of(h, ".shard").c_str(), nd.path_of(h, ".legacy").c_str()) == 0 &&
+                     (!nd.fsync_data || nd.fsync_dir_of(h));
+            ok = ok && (!counted || convert_op_allowed()) && nd.store_put(h, mt, bytes, n, ext);
+        }
+        if (ok) bytes_written += n;
+        else write_errors++;
+        return ok;
+    }
 
-    // code -1: the node's replica of h
-    void quarantine(int node, const Hash &h, int code = 0)
+    // code -1: the node's replica of h.  index >= 0: the file holding that index (by_index stores)
+    void quarantine(int node, const Hash &h, int code = 0, int index = -1)
     {
         corruption_counter++;
         {
             Node &nd = *nodes[node];
             std::lock_guard<std::mutex> lk(nd.mu);
             if (code < 0) nd.replica_quarantine(h);
-            else nd.store_quarantine(h, code);
+            else nd.store_quarantine(h, code, index);
+        }
+        put_to_resync(node, h);
+    }
+    // a file scrub found bad, by name
+    void quarantine_file(int node, const Hash &h, const char *ext)
+    {
+        corruption_counter++;
+        {
+            Node &nd = *nodes[node];
+            std::lock_guard<std::mutex> lk(nd.mu);
+            ::rename(nd.path_of(h, ext).c_str(), nd.path_of(h, ".corrupted").c_str());
         }
         put_to_resync(node, h);
     }
@@ -985,7 +1137,9 @@ struct garage_bm {
     // manager.rs:554-609 read_block + read_block_from: the verified shard bytes land in `dst`.
     // A bad header or a tag mismatch quarantines the shard and queues a resync, like the reference.
     // `for_dma`: the GPU reads `dst` next (degraded GET, resync): see copy_for_dma
-    bool read_shard_into(int node, const Hash &h, uint8_t *dst, size_t cap, ShardMeta &mt, bool for_dma = false, int code = 0)
+    // index >= 0: the node's shard of that index (several active layout versions)
+    bool read_shard_into(int node, const Hash &h, uint8_t *dst, size_t cap, ShardMeta &mt, bool for_dma = false, int code = 0,
+                         int index = -1)
     {
         Node &nd = *nodes[node];
         ReadResult r;
@@ -1002,7 +1156,7 @@ struct garage_bm {
         } else {
             std::lock_guard<std::mutex> lk(nd.mu);
             if (!nd.up) return false;
-            r = nd.store_read_into(h, dst, cap, mt, -1, code);
+            r = nd.store_read_into(h, dst, cap, mt, -1, code, index);
         }
         if (r == kReadMissing) return false;
         if (r == kReadOk) {
@@ -1011,13 +1165,13 @@ struct garage_bm {
             if (garage_ec_shard_sum_host(mt.sum_kind, check, mt.shard_len, got.data()) == GARAGE_EC_OK && got == mt.sum)
                 return true;
         }
-        quarantine(node, h, code);
+        quarantine(node, h, code, index);
         return false;
     }
     // PB: one half of a shard (a ranged read of shard_len/2 bytes into dst), checked against the half's 4 adler8
     // segment tags (garage_ec_check_shard_half_host); a bad header or tag quarantines the shard like a whole read
     bool read_half_into(int node, const Hash &h, int half, uint8_t *dst, size_t cap, ShardMeta &mt, bool for_dma = false,
-                        int code = 0)
+                        int code = 0, int index = -1)
     {
         Node &nd = *nodes[node];
         ReadResult r;
@@ -1032,7 +1186,7 @@ struct garage_bm {
         } else {
             std::lock_guard<std::mutex> lk(nd.mu);
             if (!nd.up) return false;
-            r = nd.store_read_into(h, dst, cap, mt, half, code);
+            r = nd.store_read_into(h, dst, cap, mt, half, code, index);
         }
         if (r == kReadMissing) return false;
         if (r == kReadOk) {
@@ -1040,7 +1194,7 @@ struct garage_bm {
             if (garage_ec_check_shard_half_host(mt.sum_kind, dst, mt.shard_len, half, mt.sum.data()) == GARAGE_EC_OK)
                 return true;
         }
-        quarantine(node, h, code);
+        quarantine(node, h, code, index);
         return false;
     }
 
@@ -1116,16 +1270,45 @@ struct garage_bm {
     // wrong index, is treated like a corrupt one.  `all`: read every shard (corruption hunting).
     // Returns the number of shards read (*bytes_out += the bytes); *ok = the wanted shards can be rebuilt from `have`.
     // `code`: the stripe of that code (0 = the configured one; others: a previous code's shards, .shard or .legacy)
+    // With several active layout versions (code 0) every index has the sources garage_layout_read_plan lists for it,
+    // tried in its order (a source whose file is missing or bad makes way for the next one; a PB shard's halves come
+    // from one source); the wanted indices of skip_node are not read.  from_out[i] = the node shard i came from.
     int gather_into(const Hash &h, int skip_node, uint8_t *slot, uint8_t *have, uint32_t &block_len, bool all = false,
                     bool for_gpu = false, const uint8_t *want_in = nullptr, bool *ok = nullptr, uint64_t *bytes_out = nullptr,
-                    int code = 0)
+                    int code = 0, int *from_out = nullptr)
     {
         const Code &cd = codes[code];
         const int k = cd.k, tot = cd.tot;
         const bool pb = cd.pb;
         garage_ec_ctx *const ec = cd.ctx;
-        int who[64];
-        nodes_of(h, code, who);
+        constexpr int kMaxSrc = GARAGE_BM_MAX_LAYOUT_VERSIONS;
+        int src[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M][kMaxSrc], nsrc[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0},
+            cur[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
+        bool by_index = false;  // read each source's file of that index
+        {
+            auto ls = layouts();
+            if (code == 0 && ls->v.size() > 1) {
+                by_index = true;
+                garage_shard_source plan[(GARAGE_EC_MAX_K + GARAGE_EC_MAX_M) * kMaxSrc];
+                const auto act = ls->raw();
+                const int np = garage_layout_read_plan(act.data(), (int)act.size(), nullptr, 0, h.data(), k, -1, nullptr, plan,
+                                                       (int)(sizeof(plan) / sizeof(plan[0])));
+                for (int s = 0; s < np; s++)
+                    if (plan[s].index < tot && nsrc[plan[s].index] < kMaxSrc) src[plan[s].index][nsrc[plan[s].index]++] = plan[s].node;
+            } else {
+                int who[64];
+                nodes_of(h, code, who);
+                for (int i = 0; i < tot; i++) {
+                    src[i][0] = who[i];
+                    nsrc[i] = 1;
+                }
+            }
+        }
+        // a source of index i is left to try
+        auto left = [&](int i) {
+            while (cur[i] < nsrc[i] && src[i][cur[i]] == skip_node && (!want_in || want_in[i])) cur[i]++;
+            return cur[i] < nsrc[i];
+        };
         memset(have, 0, tot);
         uint32_t expect = 0;
         bool have_expect = false;
@@ -1142,16 +1325,17 @@ struct garage_bm {
         uint8_t have_h[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};  // halves held: bit 0 a, bit 1 b (3 = whole shard)
         // whole shard (half < 0) or one half of it
         auto try_shard = [&](int i, int half = -1) {
-            if (who[i] == skip_node || have_h[i] == 3) return;
+            if (!left(i) || have_h[i] == 3) return;
+            const int node = src[i][cur[i]], fidx = by_index ? i : -1;
             ShardMeta mt;
             uint8_t *dst = slot + (size_t)i * slot_stride;
             bool got;
             if (half < 0) {
-                got = read_shard_into(who[i], h, dst, slot_stride, mt, for_gpu, code);
+                got = read_shard_into(node, h, dst, slot_stride, mt, for_gpu, code, fidx);
             } else {
                 const size_t hl = (have_expect ? shard_len_of(expect, code) : slot_stride) / 2;  // placement of the b-half
-                got = read_half_into(who[i], h, half, dst + (size_t)half * hl, slot_stride - (size_t)half * hl, mt, for_gpu,
-                                     code);
+                got = read_half_into(node, h, half, dst + (size_t)half * hl, slot_stride - (size_t)half * hl, mt, for_gpu,
+                                     code, fidx);
                 if (got && !have_expect && half == 1 && mt.shard_len / 2 != hl)  // first read of the block: move it
                     memmove(dst + mt.shard_len / 2, dst + hl, mt.shard_len / 2);
             }
@@ -1161,15 +1345,18 @@ struct garage_bm {
                     have[i] = 0;
                     count--;
                 }
+                cur[i]++;
                 return;
             }
             if (mt.index != i || (have_expect && mt.block_len != expect)) {
-                quarantine(who[i], h, code);  // a stale or misplaced shard with a self-consistent tag
+                quarantine(node, h, code, fidx);  // a stale or misplaced shard with a self-consistent tag
                 if (have_h[i]) count--;
                 have_h[i] = 0;
                 have[i] = 0;
+                cur[i]++;
                 return;
             }
+            if (from_out) from_out[i] = node;
             if (!have_expect) {
                 expect = mt.block_len;
                 have_expect = true;
@@ -1179,10 +1366,10 @@ struct garage_bm {
             have_h[i] |= half < 0 ? 3 : (uint8_t)(1 << half);
             have[i] = 1;
         };
-        uint8_t tried[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0}, want[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
-        auto attempt = [&](int i) {
-            tried[i] = 1;
-            try_shard(i);
+        uint8_t want[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
+        auto attempt = [&](int i) {  // whole shard i from its sources in order, until one is good
+            do try_shard(i);
+            while (!have[i] && left(i));
         };
         if (all) {
             for (int i = 0; i < tot; i++) attempt(i);
@@ -1197,10 +1384,10 @@ struct garage_bm {
                 }
             }
             for (;;) {
-                // assume every shard not yet tried on an up node is there; fetch what the read plan still lacks
-                // (RS / LRC: whole shards of the read set; PB: the planned halves)
+                // assume every shard with a source not yet tried is there, a wanted one excepted; fetch what the read
+                // plan still lacks (RS / LRC: whole shards of the read set; PB: the planned halves)
                 uint8_t guess[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M], rd[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
-                for (int i = 0; i < tot; i++) guess[i] = have[i] || (!tried[i] && who[i] != skip_node);
+                for (int i = 0; i < tot; i++) guess[i] = have[i] || (!want[i] && left(i));
                 if (garage_ec_read_plan(ec, guess, want, rd) != GARAGE_EC_OK) break;
                 bool fetched = false, missing = false;
                 for (int i = 0; i < tot; i++) {
@@ -1211,7 +1398,6 @@ struct garage_bm {
                     if (!pb || (need == 3 && !have_h[i])) {
                         attempt(i);
                     } else {
-                        tried[i] = 1;
                         for (int half = 0; half < 2; half++) {
                             if (!((need >> half) & 1)) continue;
                             try_shard(i, half);
@@ -1319,31 +1505,48 @@ struct garage_bm {
         } rel{it.buf};
         const size_t L = shard_len_of((uint32_t)len);
         std::vector<uint8_t> pad;
+        auto shard_bytes = [&](int i) -> const uint8_t * {  // valid until the next call
+            if (i >= k) return it.parity + (size_t)(i - k) * it.pstride;
+            const size_t off = (size_t)i * L;
+            const size_t have = off < len ? std::min(L, len - off) : 0;
+            if (have == L) return slot.p + off;
+            pad.assign(L, 0);  // zero padded tail shard (put.rs:611-615 short last block)
+            if (have) memcpy(pad.data(), slot.p + off, have);
+            return pad.data();
+        };
+        const int quorum = garage_ec_write_quorum(k, m, GARAGE_CONSISTENT);  // k+1 capped at k+m (row f4, garage_placement.h)
+        auto ls = layouts();
+        if (ls->v.size() > 1) return put_many_sets(*ls, h, (uint32_t)len, L, shard_bytes, it.sums, quorum);
         int stored = 0;
-        for (int i = 0; i < tot; i++) {  // try_write_many_sets (manager.rs:395-405): all at once
-            const uint8_t *src;
-            if (i < k) {
-                const size_t off = (size_t)i * L;
-                const size_t have = off < len ? std::min(L, len - off) : 0;
-                if (have == L) {
-                    src = slot.p + off;
-                } else {  // zero padded tail shard (put.rs:611-615 short last block)
-                    pad.assign(L, 0);
-                    if (have) memcpy(pad.data(), slot.p + off, have);
-                    src = pad.data();
-                }
-            } else {
-                src = it.parity + (size_t)(i - k) * it.pstride;
-            }
+        for (int i = 0; i < tot; i++)  // try_write_many_sets (manager.rs:395-405): all at once
             // only a shard that is durably stored counts towards the quorum
-            if (write_shard(who[i], h, i, (uint32_t)len, src, L, it.sums + (size_t)i * 32)) stored++;
-        }
+            if (write_shard(who[i], h, i, (uint32_t)len, shard_bytes(i), L, it.sums + (size_t)i * 32)) stored++;
         {
             std::lock_guard<std::mutex> lk(refs_mu);
             refs[h] = (uint32_t)len;
         }
-        const int quorum = garage_ec_write_quorum(k, m, GARAGE_CONSISTENT);  // k+1 capped at k+m (row f4, garage_placement.h)
         return stored >= quorum ? GARAGE_BM_OK : GARAGE_BM_E_QUORUM;
+    }
+    // PUT during a layout change: one shard per (node, index) request of garage_layout_write_plan, and the write quorum
+    // in the node set of every active version (try_write_many_sets, rpc_helper.rs:432-538)
+    int put_many_sets(const Layouts &ls, const Hash &h, uint32_t len, size_t L, const std::function<const uint8_t *(int)> &bytes,
+                      const uint8_t *sums, int quorum)
+    {
+        const auto act = ls.raw();
+        garage_shard_request reqs[(GARAGE_EC_MAX_K + GARAGE_EC_MAX_M) * GARAGE_BM_MAX_LAYOUT_VERSIONS];
+        const int nr = garage_layout_write_plan(act.data(), (int)act.size(), h.data(), reqs, (int)(sizeof(reqs) / sizeof(reqs[0])));
+        garage_quorum_tracker *t = nullptr;
+        if (nr < 1 || garage_quorum_tracker_new(&t, reqs, nr, (int)act.size(), quorum) != GARAGE_LAYOUT_OK) return GARAGE_BM_E_MESSAGE;
+        std::unique_ptr<garage_quorum_tracker, void (*)(garage_quorum_tracker *)> own(t, garage_quorum_tracker_free);
+        for (int r = 0; r < nr; r++) {
+            const int i = reqs[r].index;
+            garage_quorum_tracker_register(t, r, write_shard_at(reqs[r].node, h, i, len, bytes(i), L, sums + (size_t)i * 32, false));
+        }
+        {
+            std::lock_guard<std::mutex> lk(refs_mu);
+            refs[h] = len;
+        }
+        return garage_quorum_tracker_state(t) == GARAGE_QUORUM_OK ? GARAGE_BM_OK : GARAGE_BM_E_QUORUM;
     }
 
     // manager.rs:344-363 + 276-339.  `out` must hold block_size bytes; *out_len = the block's length.
@@ -1430,11 +1633,10 @@ struct garage_bm {
         uint8_t have[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
         uint32_t block_len = 0;
         corrupt_data_errors++;
+        int who[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
         const int avail = gather_into(h, -1, sp, have, block_len, /*all=*/true, /*for_gpu=*/true, nullptr, nullptr,
-                                      nullptr, code);
+                                      nullptr, code, who);
         if (avail > k && block_len <= cap) {
-            int who[64];
-            nodes_of(h, code, who);
             SlotLease trial(stripe_slots);
             for (int x = 0; x < tot; x++) {
                 if (!have[x]) continue;
@@ -1450,7 +1652,7 @@ struct garage_bm {
                 if (need && reconstruct_in_slot(trial.p, block_len, h2, w2, code) != GARAGE_BM_OK) continue;
                 assemble(trial.p, block_len, out, code);
                 if (content_ok(h, out, block_len)) {
-                    quarantine(who[x], h, code);  // the culprit
+                    quarantine(who[x], h, code, code == 0 && multi_version() ? x : -1);  // the culprit
                     *out_len = block_len;
                     return GARAGE_BM_OK;
                 }
@@ -1468,11 +1670,9 @@ struct garage_bm {
 
     int resync_block(int node, const Hash &h)
     {
-        int who[64];
-        storage_nodes_of(h, who);
-        int idx = -1;
-        for (int i = 0; i < tot; i++)
-            if (who[i] == node) idx = i;
+        const auto ls = layouts();
+        const bool multi = ls->v.size() > 1;
+        const int idx = newest_index(h, node);
         if (idx < 0) return GARAGE_BM_OK;  // not a storage node for it any more (resync.rs:466-477)
         bool known, unneeded;
         {
@@ -1485,19 +1685,33 @@ struct garage_bm {
             Node &nd = *nodes[node];
             std::lock_guard<std::mutex> lk(nd.mu);
             if (!nd.up) return GARAGE_BM_E_MESSAGE;
-            const bool exists = nd.store_has(h);
-            if (exists && unneeded) {  // offload branch, resync.rs:369-458: nobody needs it -> delete_if_unneeded
+            const bool exists = multi ? !nd.path_at(h, idx).empty() : nd.store_has(h);
+            // during a layout change the node's files of every index go, .legacy included
+            const auto held = multi ? other_index_files(nd, h, -1) : std::vector<std::pair<const char *, int>>();
+            if ((exists || !held.empty()) && unneeded) {  // offload branch, resync.rs:369-458: delete_if_unneeded
                 if (!deletable_now(h)) {  // still inside the GC delay: look again later
                     if (nd.queued.insert(h).second) nd.resync_queue.push_back(h);
                     return GARAGE_BM_OK;
                 }
-                if (nd.store_erase(h)) delete_counter++;
+                if (!multi) {
+                    if (nd.store_erase(h)) delete_counter++;
+                    return GARAGE_BM_OK;
+                }
+                for (auto &f : held)
+                    if (::remove(nd.path_of(h, f.first).c_str()) == 0) delete_counter++;
                 return GARAGE_BM_OK;
             }
             if (exists) return GARAGE_BM_OK;
         }
         if (!known || unneeded) return GARAGE_BM_OK;  // rc == 0: nothing to fetch
         SlotLease slot(stripe_slots);
+        if (multi) {  // a layout change: the shard's holder in an older version is asked first (DESIGN.md section 5.2)
+            const int c = copy_from_older(node, h, idx, *ls, false, slot.p);
+            if (c != 0) {
+                (c > 0 ? resync_counter : resync_error_counter)++;
+                return c > 0 ? GARAGE_BM_OK : GARAGE_BM_E_MESSAGE;
+            }
+        }
         uint8_t have[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M], want[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
         uint32_t block_len = 0;
         bool ok = false;
@@ -1506,6 +1720,7 @@ struct garage_bm {
         resync_shards_read += (uint64_t)gather_into(h, node, slot.p, have, block_len, false, /*for_gpu=*/true, want, &ok,
                                                     &nbytes);
         resync_bytes_read += nbytes;
+        if (multi) layout_bytes_read += nbytes;
         if (!ok) {
             // no configured stripe to rebuild from, but maybe a block stored before the code changed: convert it
             if (has_legacy() && convert_batch({h}) == 1) {
@@ -1525,12 +1740,419 @@ struct garage_bm {
         const uint8_t *bytes = slot.p + (size_t)idx * slot_stride;
         Hash sum;
         shard_tag(bytes, L, sum);
-        if (!write_shard(node, h, idx, block_len, bytes, L, sum.data())) {  // resync.rs:499
+        if (!(multi ? write_shard_at(node, h, idx, block_len, bytes, L, sum.data(), false)
+                    : write_shard(node, h, idx, block_len, bytes, L, sum.data()))) {  // resync.rs:499
             resync_error_counter++;
             return GARAGE_BM_E_MESSAGE;  // Error::Io: stays queued, the caller backs off (resync.rs:300-315)
         }
+        if (multi) {
+            layout_shards_rebuilt++;
+            layout_bytes_written += L;
+        }
         resync_counter++;
         return GARAGE_BM_OK;
+    }
+
+    // ---- changing the cluster layout (DESIGN.md section 5.2) ---------------------------------
+    // Receive, first choice: shard idx of h, which the newest version gives `node`, copied from the node that holds idx
+    // in an older active version (oldest first), its tag and header checked on read and kept.  1: copied; 0: no valid
+    // copy (rebuild it); -1: the write to `node` failed.  `buf`: slot_stride bytes.
+    int copy_from_older(int node, const Hash &h, int idx, const Layouts &ls, bool counted, uint8_t *buf)
+    {
+        uint32_t expect = 0;
+        bool have_expect = false;
+        {
+            std::lock_guard<std::mutex> lk(refs_mu);
+            auto it = refs.find(h);
+            if (it != refs.end()) expect = it->second, have_expect = true;
+        }
+        for (size_t v = 0; v + 1 < ls.v.size(); v++) {
+            int32_t row[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
+            garage_layout_nodes_of(ls.v[v].get(), h.data(), row);
+            const int y = row[idx];
+            ShardMeta mt;
+            if (y == node || !read_shard_into(y, h, buf, slot_stride, mt, false, 0, idx)) continue;
+            layout_bytes_read += mt.shard_len;
+            if (mt.index != idx || (have_expect && mt.block_len != expect)) {
+                quarantine(y, h, 0, idx);  // a self-consistent shard of another block length: stale
+                continue;
+            }
+            if (!write_shard_at(node, h, idx, mt.block_len, buf, mt.shard_len, mt.sum.data(), counted)) return -1;
+            layout_shards_copied++;
+            layout_bytes_written += mt.shard_len;
+            return 1;
+        }
+        return 0;
+    }
+    // Receive, second choice: rebuild shard idx of each block on `node` from the survivors of every active version,
+    // like resync_block's fetch branch, batch_max_blocks stripes per garage_ec_reconstruct_stripes.  Returns the number
+    // written; *clean = false if one could not be rebuilt or written.
+    // Concurrent syncs run their rebuild batches one at a time (layout_rebuild_mu), and a batch takes its stripe slots
+    // from the shared pool in one step, so it never holds part of the pool while it waits for the rest.
+    std::mutex layout_rebuild_mu;
+    size_t rebuild_batch(int node, const std::vector<std::pair<Hash, int>> &todo, std::atomic<bool> *clean)
+    {
+        std::lock_guard<std::mutex> rl(layout_rebuild_mu);
+        const size_t bmax = std::max<uint32_t>(cfg.batch_max_blocks, 1);
+        std::atomic<size_t> written{0};
+        for (size_t b0 = 0; b0 < todo.size(); b0 += bmax) {
+            const size_t n = std::min(bmax, todo.size() - b0);
+            struct Slots {
+                SlotPool &pool;
+                std::vector<uint8_t *> p;
+                ~Slots() { pool.release_n(p); }
+            } slots{stripe_slots, stripe_slots.acquire_n(n)};
+            std::vector<ReconItem> items(n);
+            std::vector<uint8_t> ok(n, 0);
+            parallel_for(n, [&](size_t j, std::vector<uint8_t> &) {
+                const Hash &h = todo[b0 + j].first;
+                ReconItem &it = items[j];
+                it.stripe = slots.p[j];
+                it.stride = slot_stride;
+                it.want[todo[b0 + j].second] = 1;
+                bool g = false;
+                uint64_t nbytes = 0;
+                gather_into(h, node, it.stripe, it.present, it.block_len, false, /*for_gpu=*/true, it.want, &g, &nbytes);
+                layout_bytes_read += nbytes;
+                ok[j] = g;
+            });
+            std::vector<ReconItem *> batch;
+            for (size_t j = 0; j < n; j++)
+                if (ok[j]) batch.push_back(&items[j]);
+            std::vector<int> rc;
+            reconstruct_calls += batch.size();
+            if (!batch.empty()) rec_batcher->submit_all(batch, rc);
+            for (size_t q = 0, j = 0; j < n; j++)
+                if (ok[j]) ok[j] = rc[q++] == GARAGE_BM_OK;
+            parallel_for(n, [&](size_t j, std::vector<uint8_t> &) {
+                const Hash &h = todo[b0 + j].first;
+                const int idx = todo[b0 + j].second;
+                if (!ok[j]) {
+                    layout_sync_errors++;
+                    *clean = false;
+                    return;
+                }
+                const uint32_t len = items[j].block_len;
+                const size_t L = shard_len_of(len);
+                const uint8_t *bytes = items[j].stripe + (size_t)idx * slot_stride;
+                Hash sum;
+                shard_tag(bytes, L, sum);
+                if (!write_shard_at(node, h, idx, len, bytes, L, sum.data(), true)) {
+                    layout_sync_errors++;
+                    *clean = false;
+                    return;
+                }
+                layout_shards_rebuilt++;
+                layout_bytes_written += L;
+                written++;
+            });
+        }
+        return written;
+    }
+    // the newest version's stripe of h holds its write quorum: k+1 shards with valid tags at their assigned (node, index)
+    bool newest_at_quorum(const Hash &h, uint8_t *buf)
+    {
+        int who[64];
+        storage_nodes_of(h, who);
+        const int quorum = garage_ec_write_quorum(k, m, GARAGE_CONSISTENT);
+        int good = 0;
+        for (int i = 0; i < tot && good < quorum && good + (tot - i) >= quorum; i++) {
+            ShardMeta mt;
+            if (read_shard_into(who[i], h, buf, slot_stride, mt, false, 0, i) && mt.index == i) good++;
+        }
+        return good >= quorum;
+    }
+    // the configured-code files of h on `node` whose index is not `keep`: (".shard" / ".legacy", index)
+    std::vector<std::pair<const char *, int>> other_index_files(Node &nd, const Hash &h, int keep) const  // nd.mu held
+    {
+        std::vector<std::pair<const char *, int>> r;
+        if (nd.dir.empty() || !nd.by_index) return r;
+        for (const char *ext : {".shard", ".legacy"}) {
+            const int i = nd.file_index(nd.path_of(h, ext));
+            if (i >= 0 && i != keep) r.emplace_back(ext, i);
+        }
+        return r;
+    }
+    // Offload of shard i of h from `node` (resync.rs:369-458): the newest version's holder of i gets it first if it
+    // lacks it (a push: the copy a receiver would make), then the file goes once the newest stripe holds k+1.
+    // Returns the number of shards pushed.
+    int offload_shards(int node, const Hash &h, uint8_t *buf)
+    {
+        Node &nd = *nodes[node];
+        int who[64];
+        storage_nodes_of(h, who);
+        const int a = newest_index(h, node);
+        std::vector<std::pair<const char *, int>> held;
+        {
+            std::lock_guard<std::mutex> lk(nd.mu);
+            held = other_index_files(nd, h, a);
+        }
+        int pushed = 0;
+        bool all_held = true;  // every newest holder of an index this node offloads has it
+        for (auto &f : held) {
+            const int i = f.second;
+            ShardMeta mt;
+            if (read_shard_into(who[i], h, buf, slot_stride, mt, false, 0, i) && mt.index == i) continue;
+            if (read_shard_into(node, h, buf, slot_stride, mt, false, 0, i) && mt.index == i &&
+                write_shard_at(who[i], h, i, mt.block_len, buf, mt.shard_len, mt.sum.data(), true)) {
+                layout_shards_copied++;
+                layout_bytes_read += mt.shard_len;
+                layout_bytes_written += mt.shard_len;
+                pushed++;
+            } else {
+                all_held = false;
+            }
+        }
+        if (held.empty() || !all_held || !newest_at_quorum(h, buf)) return pushed;
+        std::lock_guard<std::mutex> lk(nd.mu);
+        if (!nd.up) return pushed;
+        for (auto &f : other_index_files(nd, h, a))
+            if (convert_op_allowed() && ::remove(nd.path_of(h, f.first).c_str()) == 0) layout_deleted++;
+        return pushed;
+    }
+    // garage_bm_layout_sync_step: see include/garage_block_manager.h
+    int layout_sync_step(int node, const Hash *cursor, size_t max_blocks, Hash *cursor_out, int *finished, uint64_t *moved)
+    {
+        Node &nd = *nodes[node];
+        const auto ls = layouts();
+        const uint64_t newest_v = garage_layout_version(ls->newest());
+        std::vector<Hash> hs;
+        {
+            std::lock_guard<std::mutex> lk(refs_mu);
+            for (auto &kv : refs) hs.push_back(kv.first);
+        }
+        hs.erase(std::remove_if(hs.begin(), hs.end(), [&](const Hash &h) { return newest_index(h, node) < 0; }), hs.end());
+        {
+            std::lock_guard<std::mutex> lk(nd.mu);
+            if (!nd.up) return GARAGE_BM_E_MESSAGE;
+            if (!nd.dir.empty()) nd.store_list(hs, true);
+        }
+        std::sort(hs.begin(), hs.end());
+        hs.erase(std::unique(hs.begin(), hs.end()), hs.end());
+        if (cursor) hs.erase(hs.begin(), std::upper_bound(hs.begin(), hs.end(), *cursor));
+        bool done = true;
+        if (max_blocks && hs.size() > max_blocks) {
+            hs.resize(max_blocks);
+            done = false;
+        }
+        if (finished) *finished = done ? 1 : 0;
+        if (cursor_out) {
+            if (!hs.empty()) *cursor_out = hs.back();
+            else if (cursor) *cursor_out = *cursor;
+            else cursor_out->fill(0);
+        }
+        if (!cursor) {
+            std::lock_guard<std::mutex> lk(layout_mu);
+            pass_version[node] = newest_v;
+            pass_clean[node] = 1;
+        }
+        std::vector<std::pair<Hash, int>> receive;
+        std::vector<Hash> offload;  // blocks of which the node holds an index the newest version does not give it
+        {
+            SlotLease scratch(stripe_slots);
+            for (const Hash &h : hs) {
+                {
+                    // rc 0: nothing is received; the node's shards go once the GC delay has passed, decided and deleted
+                    // under both locks like resync_block's offload branch
+                    std::lock_guard<std::mutex> rl(refs_mu);
+                    auto it = rc.find(h);
+                    if (it != rc.end() && it->second.count <= 0) {
+                        if (deletable_now(h)) {
+                            std::lock_guard<std::mutex> lk(nd.mu);
+                            for (auto &f : other_index_files(nd, h, -1))
+                                if (convert_op_allowed() && ::remove(nd.path_of(h, f.first).c_str()) == 0) delete_counter++;
+                        }
+                        continue;
+                    }
+                    if (!refs.count(h)) continue;  // a file of no known block
+                }
+                const int a = newest_index(h, node);
+                ShardMeta mt;
+                if (a >= 0 && !(read_shard_into(node, h, scratch.p, slot_stride, mt, false, 0, a) && mt.index == a))
+                    receive.emplace_back(h, a);
+                std::lock_guard<std::mutex> lk(nd.mu);
+                if (!other_index_files(nd, h, a).empty()) offload.push_back(h);
+            }
+        }
+        std::atomic<bool> clean{true};
+        std::atomic<uint64_t> n_moved{0};
+        std::vector<std::pair<Hash, int>> rebuild;
+        std::mutex rebuild_mu;
+        parallel_for(receive.size(), [&](size_t j, std::vector<uint8_t> &buf) {
+            buf.resize(slot_stride);
+            const int c = copy_from_older(node, receive[j].first, receive[j].second, *ls, true, buf.data());
+            if (c > 0) {
+                n_moved++;
+            } else if (c == 0) {
+                std::lock_guard<std::mutex> lk(rebuild_mu);
+                rebuild.push_back(receive[j]);
+            } else {
+                layout_sync_errors++;
+                clean = false;
+            }
+        });
+        std::sort(rebuild.begin(), rebuild.end());
+        n_moved += rebuild_batch(node, rebuild, &clean);
+        // offload: deleted only once the newest stripe is seen at its write quorum (the deletion rule of DESIGN.md 5.1)
+        parallel_for(offload.size(), [&](size_t j, std::vector<uint8_t> &buf) {
+            buf.resize(slot_stride);
+            n_moved += offload_shards(node, offload[j], buf.data());
+        });
+        if (moved) *moved = n_moved;
+        std::lock_guard<std::mutex> lk(layout_mu);
+        if (!clean) pass_clean[node] = 0;
+        if (done && pass_clean[node] && pass_version[node] == newest_v && synced[node] < newest_v) {
+            synced[node] = newest_v;
+            retire_if_synced();
+            if (layout_file && !save_layout(*layouts())) return GARAGE_BM_E_MESSAGE;
+        }
+        return GARAGE_BM_OK;
+    }
+    // layout_mu held: once every storage node of the newest version has synced it, the older versions are dropped
+    void retire_if_synced()
+    {
+        const auto ls = layouts();
+        if (ls->v.size() < 2) return;
+        const uint64_t newest_v = garage_layout_version(ls->newest());
+        const auto &cap = ls->capacity.back();
+        for (size_t n = 0; n < nodes.size(); n++)
+            if (cap[n] > 0 && synced[n] < newest_v) return;
+        auto nl = std::make_shared<Layouts>();
+        nl->v.push_back(ls->v.back());
+        nl->zone.push_back(ls->zone.back());
+        nl->capacity.push_back(ls->capacity.back());
+        std::atomic_store(&layouts_, std::shared_ptr<const Layouts>(std::move(nl)));
+    }
+    // The layout history, <data_dir>/layout (Garage keeps its cluster layout in metadata, not in its config): every
+    // active version's spec and ring, and each node's synced version.  tmp -> fsync -> rename, then the directory
+    // under data_fsync.  layout_mu held (or the manager not yet shared).
+    std::string layout_path;
+    bool save_layout(const Layouts &ls)
+    {
+        std::string s = "garage-bm-layout 1\nnodes " + std::to_string(nodes.size()) + " shards " + std::to_string(tot) + "\n";
+        std::vector<uint8_t> ring((size_t)GARAGE_NB_PARTITIONS * tot);
+        for (size_t v = 0; v < ls.v.size(); v++) {
+            s += "version " + std::to_string(garage_layout_version(ls.v[v].get())) + "\nzone";
+            for (int32_t z : ls.zone[v]) s += " " + std::to_string(z);
+            s += "\ncapacity";
+            for (uint64_t c : ls.capacity[v]) s += " " + std::to_string(c);
+            garage_layout_ring(ls.v[v].get(), ring.data());
+            s += "\nring " + hex_of(ring.data(), ring.size()) + "\n";
+        }
+        s += "synced";
+        for (uint64_t v : synced) s += " " + std::to_string(v);
+        s += "\n";
+        const std::string tmp = layout_path + ".tmp" + std::to_string((unsigned long)::getpid());
+        FILE *f = fopen(tmp.c_str(), "wb");
+        if (!f) return false;
+        bool ok = fwrite(s.data(), s.size(), 1, f) == 1 && fflush(f) == 0 && ::fsync(fileno(f)) == 0;
+        ok = fclose(f) == 0 && ok;
+        if (ok) ok = ::rename(tmp.c_str(), layout_path.c_str()) == 0;
+        if (ok && cfg.data_fsync) {
+            const int dfd = ::open(std::filesystem::path(layout_path).parent_path().c_str(), O_RDONLY | O_DIRECTORY);
+            ok = dfd >= 0 && ::fsync(dfd) == 0;
+            if (dfd >= 0) ::close(dfd);
+        }
+        if (!ok) ::remove(tmp.c_str());
+        return ok;
+    }
+    // 1: loaded into out / syn; 0: no file; -1: a file this manager cannot use
+    static int load_layout(const std::string &path, int n, int tot, Layouts &out, std::vector<uint64_t> &syn)
+    {
+        FILE *f = fopen(path.c_str(), "rb");
+        if (!f) return 0;
+        std::string s;
+        char buf[65536];
+        for (size_t r; (r = fread(buf, 1, sizeof(buf), f)) > 0;) s.append(buf, r);
+        fclose(f);
+        std::vector<std::string> tok;  // whitespace-separated words
+        for (size_t i = 0; i < s.size();) {
+            while (i < s.size() && isspace((unsigned char)s[i])) i++;
+            const size_t j = i;
+            while (i < s.size() && !isspace((unsigned char)s[i])) i++;
+            if (i > j) tok.push_back(s.substr(j, i - j));
+        }
+        size_t t = 0;
+        auto word = [&](const char *w) { return t < tok.size() && tok[t] == w ? (t++, true) : false; };
+        auto num = [&](auto &v) {
+            if (t >= tok.size()) return false;
+            char *e = nullptr;
+            errno = 0;
+            const long long x = strtoll(tok[t].c_str(), &e, 10);
+            if (errno || *e || tok[t].empty()) return false;
+            v = (std::remove_reference_t<decltype(v)>)x;
+            t++;
+            return true;
+        };
+        int fmt = 0, fn = 0, ft = 0;
+        if (!word("garage-bm-layout") || !num(fmt) || fmt != 1) return -1;
+        if (!word("nodes") || !num(fn) || !word("shards") || !num(ft) || fn != n || ft != tot) return -1;
+        while (word("version")) {
+            uint64_t v = 0;
+            std::vector<int32_t> zone(n);
+            std::vector<uint64_t> cap(n);
+            if (!num(v) || !word("zone")) return -1;
+            for (auto &z : zone)
+                if (!num(z)) return -1;
+            if (!word("capacity")) return -1;
+            for (auto &c : cap)
+                if (!num(c)) return -1;
+            if (!word("ring") || t >= tok.size() || tok[t].size() != (size_t)GARAGE_NB_PARTITIONS * tot * 2) return -1;
+            const std::string &hex = tok[t++];
+            std::vector<uint8_t> ring(hex.size() / 2);
+            for (size_t i = 0; i < ring.size(); i++) {
+                char *e = nullptr;
+                const std::string b = hex.substr(2 * i, 2);
+                ring[i] = (uint8_t)strtoul(b.c_str(), &e, 16);
+                if (*e) return -1;
+            }
+            garage_layout *l = nullptr;
+            if (garage_layout_from_ring(&l, v, n, zone.data(), cap.data(), tot, ring.data()) != GARAGE_LAYOUT_OK) return -1;
+            out.v.emplace_back(l, garage_layout_free);
+            out.zone.push_back(std::move(zone));
+            out.capacity.push_back(std::move(cap));
+        }
+        if (!word("synced") || out.v.empty() || out.v.size() > GARAGE_BM_MAX_LAYOUT_VERSIONS) return -1;
+        syn.assign(n, 0);
+        for (auto &v : syn)
+            if (!num(v)) return -1;
+        return 1;
+    }
+    // garage_bm_apply_layout: see include/garage_block_manager.h
+    int apply_layout(const garage_bm_layout_spec *spec, uint64_t *version_out)
+    {
+        if (nodes[0]->dir.empty() || has_legacy()) return GARAGE_EC_E_INVALID;
+        std::lock_guard<std::mutex> lk(layout_mu);
+        const auto ls = layouts();
+        if (!ls->newest() || ls->v.size() >= GARAGE_BM_MAX_LAYOUT_VERSIONS) return GARAGE_EC_E_INVALID;
+        const uint64_t v = garage_layout_version(ls->newest()) + 1;
+        auto nl = std::make_shared<Layouts>(*ls);
+        if (!layout_from_spec(*nl, v, (int)nodes.size(), k, m, spec, ls->newest())) return GARAGE_EC_E_INVALID;
+        if (!save_layout(*nl)) return GARAGE_BM_E_MESSAGE;  // on disk before any shard goes to the new version
+        for (auto &nd : nodes) nd->by_index = true;           // from now on a node may hold two indices of a block
+        layout_file = true;
+        std::atomic_store(&layouts_, std::shared_ptr<const Layouts>(std::move(nl)));
+        if (version_out) *version_out = v;
+        return GARAGE_BM_OK;
+    }
+    // a spec's layout version appended to `out`; false for a spec garage_bm_config.layout documents as invalid
+    static bool layout_from_spec(Layouts &out, uint64_t version, int n, int k, int m, const garage_bm_layout_spec *s,
+                                 const garage_layout *previous)
+    {
+        if (!s || !s->zone || !s->capacity || s->zone_redundancy < 0 || s->max_per_zone < 0 || s->max_per_zone > m ||
+            n > GARAGE_LAYOUT_MAX_NODES)
+            return false;
+        int storage = 0;
+        for (int i = 0; i < n; i++) storage += s->capacity[i] > 0;
+        if (storage < k + m) return false;
+        garage_layout *l = nullptr;
+        if (garage_layout_compute(&l, version, n, s->zone, s->capacity, k + m, s->zone_redundancy, s->max_per_zone, previous) !=
+            GARAGE_LAYOUT_OK)
+            return false;
+        out.v.emplace_back(l, garage_layout_free);
+        out.zone.emplace_back(s->zone, s->zone + n);
+        out.capacity.emplace_back(s->capacity, s->capacity + n);
+        return true;
     }
 
     // ---- changing the store's code (DESIGN.md section 5.1) ----------------------------------
@@ -1896,16 +2518,14 @@ struct garage_bm {
             for (auto &kv : refs) all.push_back(kv.first);
         }
         uint64_t c = 0;
+        const bool multi = multi_version();
         for (const Hash &h : all) {
-            int who[64];
-            storage_nodes_of(h, who);
-            bool mine = false;
-            for (int i = 0; i < tot; i++) mine |= who[i] == node;
-            if (!mine) continue;
+            const int idx = newest_index(h, node);
+            if (idx < 0) continue;
             bool has;
             {
                 std::lock_guard<std::mutex> lk(nodes[node]->mu);
-                has = nodes[node]->store_has(h);
+                has = multi ? !nodes[node]->path_at(h, idx).empty() : nodes[node]->store_has(h);
             }
             if (!has) {
                 put_to_resync(node, h);
@@ -1931,7 +2551,7 @@ struct garage_bm {
         {
             std::lock_guard<std::mutex> lk(nd.mu);
             if (!nd.up) return GARAGE_BM_E_MESSAGE;
-            nd.store_list(hashes, has_legacy());
+            nd.store_list(hashes, has_legacy() || nd.by_index);
         }
         std::sort(hashes.begin(), hashes.end());
         hashes.erase(std::unique(hashes.begin(), hashes.end()), hashes.end());
@@ -1948,8 +2568,10 @@ struct garage_bm {
             else cursor_out->fill(0);
         }
         // the files to check: (hash, 0) the .shard; with previous codes or replicas configured also (hash, 1) a .legacy
-        // shard and (hash, 2) a replica
-        const bool legacy = has_legacy() && !nd.dir.empty();
+        // shard and (hash, 2) a replica; with a layout file (hash, 1) an older layout version's index
+        const bool by_index = nd.by_index;
+        const bool legacy = (has_legacy() || by_index) && !nd.dir.empty();
+        const bool old_index = by_index && !has_legacy();  // a .legacy file holds the configured code
         std::vector<std::pair<Hash, int>> items;
         {
             std::lock_guard<std::mutex> lk(nd.mu);
@@ -1997,7 +2619,7 @@ struct garage_bm {
                         r = nd.store_read_into(h, buf + i * stride, stride, mt);
                     } else {  // read the file as the code its header names; an unknown code is corrupt, as before
                         const std::string path = nd.path_of(h, kind ? ".legacy" : ".shard");
-                        code[i] = std::max(kind, nd.file_code(path));
+                        code[i] = old_index ? 0 : std::max(kind, nd.file_code(path));
                         r = nd.file_read_into(path, code[i], buf + i * stride, stride, mt);
                     }
                     if (r == kReadMissing) continue;
@@ -2025,7 +2647,8 @@ struct garage_bm {
                 nchecked++;
                 if (state[i] == 3 || (state[i] == 1 && !bad[i])) continue;
                 nbad++;
-                quarantine(node, items[c0 + i].first, code[i]);
+                if (old_index && items[c0 + i].second == 1) quarantine_file(node, items[c0 + i].first, ".legacy");
+                else quarantine(node, items[c0 + i].first, code[i]);
             }
         }
         scrub_checked += nchecked;
@@ -2165,6 +2788,7 @@ void garage_bm_default_config(garage_bm_config *c)
     c->previous_codes = nullptr;    // no code change in progress
     c->n_previous_codes = 0;
     c->legacy_replicas = 0;
+    c->layout = nullptr;            // the fixed ring
 }
 
 // a code garage_ec_create / _lrc / _piggyback accepts, with tags the block manager can check: the same rules as the
@@ -2205,6 +2829,24 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
                 return GARAGE_EC_E_INVALID;
         }
     }
+    // the layout history: <data_dir>/layout wins over cfg->layout; both are checked before any CUDA call
+    auto lays = std::make_shared<garage_bm::Layouts>();
+    std::vector<uint64_t> synced(cfg->n_nodes, 0);
+    const bool file_store = cfg->data_dir && cfg->data_dir[0];
+    const std::string layout_path = file_store ? std::string(cfg->data_dir) + "/layout" : std::string();
+    if (cfg->layout && !garage_bm::layout_from_spec(*lays, 1, cfg->n_nodes, k, m, cfg->layout, nullptr)) return GARAGE_EC_E_INVALID;
+    bool layout_file = file_store && cfg->layout;
+    if (file_store) {
+        auto loaded = std::make_shared<garage_bm::Layouts>();
+        const int r = garage_bm::load_layout(layout_path, cfg->n_nodes, k + m, *loaded, synced);
+        if (r < 0) return GARAGE_EC_E_INVALID;
+        if (r > 0) {
+            lays = loaded;
+            layout_file = true;
+        }
+    }
+    // a store changes its layout or its code, not both at once
+    if (lays->v.size() > 1 && (np > 0 || cfg->legacy_replicas > 0)) return GARAGE_EC_E_INVALID;
     // every context of the manager runs the same code: RS(k, m), LRC(k, l, m - l) or PB(k, m)
     auto make_ctx = [&](garage_ec_ctx **c) {
         return pb ? garage_ec_create_piggyback(c, cfg->cuda_device, k, m, GARAGE_EC_VANDERMONDE)
@@ -2251,16 +2893,27 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
         // slots and the scrub buffer hold a shard of the largest code in play
         bm->slot_stride = std::max(bm->slot_stride, garage_ec_stride_for((uint32_t)bm->shard_len_of(bm->cfg.block_size, 1 + i)));
     }
-    if (cfg->n_nodes <= GARAGE_LAYOUT_MAX_NODES) {
+    if (lays->v.empty() && cfg->n_nodes <= GARAGE_LAYOUT_MAX_NODES) {
         const int n = cfg->n_nodes, tot = k + m;
         std::vector<uint8_t> ring((size_t)GARAGE_NB_PARTITIONS * tot);
         for (int p = 0; p < GARAGE_NB_PARTITIONS; p++)
             for (int i = 0; i < tot; i++) ring[(size_t)p * tot + i] = (uint8_t)((p % n + i) % n);
         std::vector<int32_t> zone(n, 0);
         std::vector<uint64_t> capacity(n, 1);
-        if (garage_layout_from_ring(&bm->layout, 1, n, zone.data(), capacity.data(), tot, ring.data()) != GARAGE_LAYOUT_OK)
-            bm->layout = nullptr;
+        garage_layout *l = nullptr;
+        if (garage_layout_from_ring(&l, 1, n, zone.data(), capacity.data(), tot, ring.data()) == GARAGE_LAYOUT_OK) {
+            lays->v.emplace_back(l, garage_layout_free);
+            lays->zone.push_back(std::move(zone));
+            lays->capacity.push_back(std::move(capacity));
+        }
     }
+    bm->layouts_ = lays;
+    bm->layout_file = layout_file;
+    bm->layout_path = layout_path;
+    bm->synced = synced;
+    bm->pass_version.assign(cfg->n_nodes, 0);
+    bm->pass_clean.assign(cfg->n_nodes, 0);
+    bm->cfg.layout = nullptr;  // not kept: the caller's spec may go away
     for (int i = 0; i < cfg->n_nodes; i++) {
         bm->nodes.emplace_back(new Node());
         Node &nd = *bm->nodes.back();
@@ -2272,6 +2925,7 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
         nd.fsync_data = cfg->data_fsync != 0;
         if (cfg->data_dir && cfg->data_dir[0]) {
             nd.dir = std::string(cfg->data_dir) + "/node" + std::to_string(i);
+            nd.by_index = layout_file;
             nd.codes.assign(bm->codes.begin(), bm->codes.end());  // previous codes exist on disk only
             nd.replicas = bm->legacy_rf > 0;
             std::error_code ec;
@@ -2279,7 +2933,7 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
             // restart: what is on disk is what exists (the block_ref table would say the same), shards of previous
             // codes and replicas included
             std::vector<Hash> have;
-            nd.store_list(have, bm->has_legacy());
+            nd.store_list(have, bm->has_legacy() || nd.by_index);
             std::vector<uint8_t> tmp(bm->slot_stride);
             for (const Hash &h : have) {
                 ShardMeta mt;
@@ -2289,6 +2943,10 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
                         bm->refs[h] = mt.block_len;
                         break;
                     }
+                // a block held only as an older layout version's index
+                if (!bm->refs.count(h) && nd.by_index && !bm->has_legacy() &&
+                    nd.file_read_into(nd.path_of(h, ".legacy"), 0, tmp.data(), tmp.size(), mt) == kReadOk)
+                    bm->refs[h] = mt.block_len;
                 if (!bm->refs.count(h) && nd.has_replica(h) && ::stat(nd.path_of(h, "").c_str(), &sb) == 0 && sb.st_size > 0 &&
                     (uint64_t)sb.st_size <= bm->cfg.block_size)
                     bm->refs[h] = (uint32_t)sb.st_size;
@@ -2301,6 +2959,8 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
         garage_bm_destroy(bm.release());
         return code;
     };
+    // a layout given in the configuration is recorded, so that a restart keeps it and its later versions
+    if (layout_file && !std::filesystem::exists(layout_path) && !bm->save_layout(*lays)) return destroy_on_error(GARAGE_BM_E_MESSAGE);
     for (int w = 0; w < garage_bm::kWorkers; w++) {
         rc = make_ctx(&bm->enc_ctx[w]);
         if (rc == GARAGE_EC_OK) rc = make_ctx(&bm->rec_ctx[w]);
@@ -2486,6 +3146,37 @@ int garage_bm_convert_step(garage_bm *bm, int node, const uint8_t *cursor32, siz
     }
 }
 
+int garage_bm_apply_layout(garage_bm *bm, const garage_bm_layout_spec *spec, uint64_t *version_out)
+{
+    if (!bm || !spec) return GARAGE_EC_E_INVALID;
+    BM_GUARD(bm->apply_layout(spec, version_out));
+}
+
+int garage_bm_layout_sync_step(garage_bm *bm, int node, const uint8_t *cursor32, size_t max_blocks, uint8_t cursor_out32[32],
+                               int *finished, uint64_t *moved)
+{
+    if (!bm || node < 0 || node >= (int)bm->nodes.size()) return GARAGE_EC_E_INVALID;
+    try {
+        Hash cur, out;
+        if (cursor32) cur = to_hash(cursor32);
+        int rc = bm->layout_sync_step(node, cursor32 ? &cur : nullptr, max_blocks, &out, finished, moved);
+        if (rc == GARAGE_BM_OK && cursor_out32) memcpy(cursor_out32, out.data(), 32);
+        return rc;
+    } catch (const std::bad_alloc &) {
+        return GARAGE_EC_E_NOMEM;
+    } catch (...) {
+        return GARAGE_BM_E_MESSAGE;
+    }
+}
+
+int garage_bm_layout_versions(garage_bm *bm, uint64_t *out, int cap)
+{
+    if (!bm || cap < 0 || (cap > 0 && !out)) return GARAGE_EC_E_INVALID;
+    const auto ls = bm->layouts();
+    for (int i = 0; i < (int)ls->v.size() && i < cap; i++) out[i] = garage_layout_version(ls->v[i].get());
+    return (int)ls->v.size();
+}
+
 int garage_bm_debug_convert_stop_after(garage_bm *bm, long n_ops)
 {
     if (!bm) return GARAGE_EC_E_INVALID;
@@ -2663,6 +3354,13 @@ void garage_bm_get_metrics(garage_bm *bm, garage_bm_metrics *o)
     o->convert_call_us = bm->convert_call_us;
     o->legacy_gets = bm->legacy_gets;
     o->legacy_deleted = bm->legacy_deleted;
+    o->layout_shards_copied = bm->layout_shards_copied;
+    o->layout_shards_rebuilt = bm->layout_shards_rebuilt;
+    o->layout_bytes_read = bm->layout_bytes_read;
+    o->layout_bytes_written = bm->layout_bytes_written;
+    o->layout_deleted = bm->layout_deleted;
+    o->layout_sync_errors = bm->layout_sync_errors;
+    o->layout_version = garage_layout_version(bm->layouts()->newest());
     uint64_t ql = 0;
     for (auto &n : bm->nodes) {
         std::lock_guard<std::mutex> lk(n->mu);

@@ -51,6 +51,18 @@ typedef struct {
 
 #define GARAGE_BM_MAX_PREVIOUS_CODES 4
 
+/* One layout version over the manager's n_nodes node stores (DESIGN.md section 5.2).  The fields mean what they mean
+ * to garage_layout_compute: zone[i] = zone of node i, capacity[i] = 0 for a node that stores nothing in this version
+ * (a gateway, or a node being removed), zone_redundancy 0 = maximum, max_per_zone 0 = no limit (at most m).       */
+typedef struct {
+    const int32_t *zone;      /* n_nodes entries */
+    const uint64_t *capacity; /* n_nodes entries */
+    int zone_redundancy;
+    int max_per_zone;
+} garage_bm_layout_spec;
+
+#define GARAGE_BM_MAX_LAYOUT_VERSIONS 4 /* active layout versions at once */
+
 typedef struct {
     int data_shards;                /* k  (config: erasure_coding.data_shards)   */
     int parity_shards;              /* m                                          */
@@ -89,6 +101,12 @@ typedef struct {
     int legacy_replicas;            /* replication factor of a previous replicated layout (0 = none): whole-block
                                        files <node dir>/<hh>/<hh>/<64 hex> on the first legacy_replicas nodes of the
                                        block's ring row, read and converted like a previous code                   */
+    /* Cluster layout (DESIGN.md section 5.2).  NULL: partition p on nodes (p mod n_nodes) + i, as before.  Otherwise
+       version 1 is garage_layout_compute(1, ..., previous = NULL) of this spec.  GARAGE_EC_E_INVALID before any CUDA
+       call for: a NULL array, a negative zone_redundancy or max_per_zone, max_per_zone > m, fewer than k+m nodes with
+       capacity, or a layout garage_layout_compute finds infeasible.  A file store keeps its layout history in
+       <data_dir>/layout; on restart that file wins over this field.                                              */
+    const garage_bm_layout_spec *layout;
 } garage_bm_config;
 
 typedef struct {
@@ -114,6 +132,13 @@ typedef struct {
     uint64_t convert_call_us;                /* wall time inside garage_ec_transcode                            */
     uint64_t legacy_gets;                    /* GETs served from a previous code's stripe or a replica          */
     uint64_t legacy_deleted;                 /* legacy shard / replica files deleted                            */
+    uint64_t layout_shards_copied;           /* shards a layout sync copied from an older version's holder      */
+    uint64_t layout_shards_rebuilt;          /* shards a layout sync (or resync) rebuilt on the GPU             */
+    uint64_t layout_bytes_read;              /* bytes read by those copies and rebuilds                         */
+    uint64_t layout_bytes_written;           /* bytes they wrote                                                */
+    uint64_t layout_deleted;                 /* shards deleted once the newest version no longer assigned them  */
+    uint64_t layout_sync_errors;             /* shards a sync could neither copy nor rebuild (or not write)     */
+    uint64_t layout_version;                 /* the newest active layout version                                */
 } garage_bm_metrics;
 
 void garage_bm_default_config(garage_bm_config *cfg);
@@ -173,6 +198,28 @@ int garage_bm_scrub_step(garage_bm *bm, int node, const uint8_t *cursor32, size_
 int garage_bm_convert_step(garage_bm *bm, int node, const uint8_t *cursor32, size_t max_blocks, uint8_t cursor_out32[32],
                            int *finished, uint64_t *converted);
 
+/* Changing the cluster layout (file store; DESIGN.md section 5.2).  garage_bm_apply_layout computes the next version
+ * with previous = the newest one (nodes that stay keep their shard index) and makes it active; PUTs then write to
+ * every active version and need k+1 shards in each.  GARAGE_EC_E_INVALID for the memory store, with previous_codes or
+ * legacy_replicas configured, for a spec garage_bm_create would reject, or when more than
+ * GARAGE_BM_MAX_LAYOUT_VERSIONS versions would be active.  *version_out = the new version.                       */
+int garage_bm_apply_layout(garage_bm *bm, const garage_bm_layout_spec *spec, uint64_t *version_out);
+/* Layout sync of `node`, resumable in hash order like garage_bm_scrub_step: every block the newest version assigns
+ * to `node` and every shard `node` holds, after cursor32 (NULL = from the start), at most max_blocks (0 = all):
+ *   - receive: the node lacks a valid shard of its newest index: copy it from that index's holder in an older active
+ *     version (oldest first, tag checked), else rebuild it on the GPU from the survivors of every active version;
+ *   - offload: the node holds an index the newest version does not give it: deleted once the newest stripe is seen
+ *     with k+1 valid shards at their assigned (node, index); a block at rc 0 is deleted after block_gc_delay_ms.
+ * A full pass (cursor NULL to *finished) that leaves nothing to receive records the node as synced; once every
+ * storage node of the newest version is, the older versions are retired.  *moved = shards copied or rebuilt.
+ * Its renames, writes and deletes count as file operations for garage_bm_debug_convert_stop_after.  Calls for
+ * different nodes may run concurrently (their GPU rebuild batches then run one at a time); a node's own steps are
+ * made one after another.                                                                                      */
+int garage_bm_layout_sync_step(garage_bm *bm, int node, const uint8_t *cursor32, size_t max_blocks,
+                               uint8_t cursor_out32[32], int *finished, uint64_t *moved);
+/* the active layout versions, oldest first; returns their number (at most cap are written)                       */
+int garage_bm_layout_versions(garage_bm *bm, uint64_t *out, int cap);
+
 /* native closed-loop load generator (row f1: the batching front-end decides real-world throughput):
  * `threads` client threads each PUT (mode 0) or GET (mode 1) `blocks_per_thread` blocks of `block_len`
  * bytes (splitmix64 stream of `seed`; a GET run must follow a PUT run with the same arguments).  The
@@ -191,10 +238,11 @@ int garage_bm_plant_stale_shard(garage_bm *bm, int node, const uint8_t hash[32])
 /* file store only: make every write to the node's directory fail (like ENOSPC / EACCES / a lost mount) */
 int garage_bm_set_node_readonly(garage_bm *bm, int node, int readonly);
 int garage_bm_drop_shard(garage_bm *bm, int node, const uint8_t hash[32]);
-/* after n_ops more file operations of conversions (renames to .legacy, shard writes, legacy deletes), make every
- * further one fail, as if the process had stopped there; n_ops < 0 turns it off                                  */
+/* after n_ops more file operations of conversions and layout syncs (renames to .legacy, shard writes, deletes), make
+ * every further one fail, as if the process had stopped there; n_ops < 0 turns it off                            */
 int garage_bm_debug_convert_stop_after(garage_bm *bm, long n_ops);
 int garage_bm_node_shard_index(garage_bm *bm, int node, const uint8_t hash[32]); /* -1 if none */
+/* the newest active layout version's row: shard i of the block on nodes_out[i]                                  */
 int garage_bm_storage_nodes_of(garage_bm *bm, const uint8_t hash[32], int *nodes_out /* k+m */);
 void garage_bm_get_metrics(garage_bm *bm, garage_bm_metrics *out);
 
