@@ -39,6 +39,7 @@ ABI_SYMBOLS = [
     "garage_ec_create_lrc", "garage_ec_code_info", "garage_ec_read_set",
     "garage_ec_create_piggyback", "garage_ec_piggyback_info", "garage_ec_code_shard_len", "garage_ec_read_plan",
     "garage_ec_check_shard_half_host", "garage_ec_transcode",
+    "garage_ec_create_clay", "garage_ec_clay_info", "garage_ec_read_ranges",
 ]
 
 
@@ -124,6 +125,9 @@ def load_library(build=True):
     L.garage_ec_read_plan.argtypes = [vp, vp, vp, vp]
     L.garage_ec_check_shard_half_host.argtypes = [i32, vp, u32, i32, vp]
     L.garage_ec_transcode.argtypes = [vp, vp, vp, vp, vp, sz, vp, sz, vp, vp, sz, i32, vp]
+    L.garage_ec_create_clay.argtypes = [C.POINTER(vp), i32, i32, i32, i32]
+    L.garage_ec_clay_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), vp]
+    L.garage_ec_read_ranges.argtypes = [vp, vp, vp, u32, vp, sz, C.POINTER(sz)]
     _lib = L
     return L
 
@@ -191,10 +195,12 @@ class GarageEc:
     or numpy uint8 arrays (HOST mode: synchronous, staged through the library's lanes).
     """
 
-    def __init__(self, device=0, k=10, m=4, kind=VANDERMONDE, matrix=None, _lrc=None, _pb=False):
+    def __init__(self, device=0, k=10, m=4, kind=VANDERMONDE, matrix=None, _lrc=None, _pb=False, _clay=False):
         self._L = load_library()
         h = C.c_void_p()
-        if _pb:
+        if _clay:
+            rc = self._L.garage_ec_create_clay(C.byref(h), device, k, m, kind)
+        elif _pb:
             rc = self._L.garage_ec_create_piggyback(C.byref(h), device, k, m, kind)
         elif _lrc is not None:
             l, r = _lrc
@@ -221,6 +227,12 @@ class GarageEc:
     def piggyback(cls, device=0, k=10, m=4, kind=VANDERMONDE):
         """PB(k, m) context: RS(k, m) over two half-shards, b-halves of parities 1..m-1 carry the group XORs of a"""
         return cls(device, k, m, kind, _pb=True)
+
+    @classmethod
+    def clay(cls, device=0, k=10, m=4, kind=VANDERMONDE):
+        """Clay(k, m) context: alpha = m^ceil((k+m)/m) coupled layers of RS(k+s, m); one lost shard is rebuilt from
+        1/m of every other shard"""
+        return cls(device, k, m, kind, _clay=True)
 
     # -- lifecycle
     def close(self):
@@ -292,6 +304,28 @@ class GarageEc:
         out = np.zeros(self.k + self.m, dtype=np.uint8)
         rc = self._check(self._L.garage_ec_read_plan(self._h, _ptr(pr), _ptr(wn), _ptr(out)), (E_UNRECOVERABLE,))
         return None if rc == E_UNRECOVERABLE else out
+
+    def clay_info(self):
+        """(q, t, alpha, virtual nodes, m x (k+s) base rows) of a Clay context; (0, 0, 1, 0, None) otherwise"""
+        v = [C.c_int(0) for _ in range(4)]
+        rows = np.zeros(self.m * self.k + self.m * 4, dtype=np.uint8)
+        self._check(self._L.garage_ec_clay_info(self._h, *[C.byref(x) for x in v], _ptr(rows)))
+        q, t, alpha, s = (x.value for x in v)
+        return q, t, alpha, s, (rows[: self.m * (self.k + s)].reshape(self.m, self.k + s) if q else None)
+
+    def read_ranges(self, present, shard_len, want=None):
+        """[(shard, offset, len)] byte runs to fetch for one stripe, or None if unrecoverable"""
+        pr = np.ascontiguousarray(present, dtype=np.uint8)
+        wn = None if want is None else np.ascontiguousarray(want, dtype=np.uint8)
+        assert pr.shape == (self.k + self.m,) and (wn is None or wn.shape == pr.shape)
+        cap = (self.k + self.m) * 256
+        out = np.zeros(cap * 3, dtype=np.uint32)
+        n = C.c_size_t(0)
+        rc = self._check(self._L.garage_ec_read_ranges(self._h, _ptr(pr), _ptr(wn), shard_len, _ptr(out), cap,
+                                                       C.byref(n)), (E_UNRECOVERABLE,))
+        if rc == E_UNRECOVERABLE:
+            return None
+        return [tuple(int(v) for v in out[3 * i:3 * i + 3]) for i in range(n.value)]
 
     def code_shard_len(self, block_len):
         """shard length of a block under this context's code (PB: rounded up to 128 bytes)"""

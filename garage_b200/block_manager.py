@@ -49,7 +49,7 @@ class Config(C.Structure):
                 ("shard_sum_kind", C.c_int), ("verify_content_hash", C.c_int), ("data_fsync", C.c_int),
                 ("block_gc_delay_ms", C.c_uint32), ("local_groups", C.c_int), ("piggyback", C.c_int),
                 ("previous_codes", C.POINTER(Code)), ("n_previous_codes", C.c_int), ("legacy_replicas", C.c_int),
-                ("layout", C.POINTER(LayoutSpec))]
+                ("layout", C.POINTER(LayoutSpec)), ("clay", C.c_int)]
 
 
 class Metrics(C.Structure):
@@ -60,7 +60,7 @@ class Metrics(C.Structure):
         "encode_call_us", "reconstruct_call_us", "corrupt_data_errors", "write_errors", "resync_shards_read", "resync_bytes_read",
         "convert_blocks", "convert_bytes_read", "convert_bytes_written", "convert_errors", "convert_call_us", "legacy_gets",
         "legacy_deleted", "layout_shards_copied", "layout_shards_rebuilt", "layout_bytes_read", "layout_bytes_written",
-        "layout_deleted", "layout_sync_errors", "layout_version")]
+        "layout_deleted", "layout_sync_errors", "layout_version", "resync_bytes_fetched")]
 
 
 _lib = None
@@ -130,10 +130,10 @@ class BlockManager:
     def __init__(self, k=10, m=4, n_nodes=None, cuda_device=0, batch_max_blocks=64, batch_linger_us=100,
                  block_ram_buffer_max=256 << 20, data_dir=None, shard_sum_kind=SUM_ADLER8, verify_content_hash=True,
                  data_fsync=False, block_gc_delay_ms=0, local_groups=0, piggyback=False, previous_codes=(),
-                 legacy_replicas=0, layout=None):
+                 legacy_replicas=0, layout=None, clay=False):
         """block_gc_delay_ms defaults to 0 HERE (tests delete at once); the library's default is the
         reference's BLOCK_GC_DELAY of 10 minutes.  local_groups > 0: LRC(k, local_groups, m - local_groups).
-        piggyback: PB(k, m), half-shard repair reads.  previous_codes: (k, m, local_groups, piggyback) tuples of
+        piggyback: PB(k, m), half-shard repair reads.  clay: Clay(k, m), a lost shard rebuilt from 1/m of the others.  previous_codes: (k, m, local_groups, piggyback) tuples of
         codes the store may still hold; legacy_replicas: replication factor of a previous replicated layout.
         layout: None (partition p on nodes (p mod n_nodes) + i) or a dict with zone, capacity and optionally
         zone_redundancy, max_per_zone: version 1 of the cluster layout."""
@@ -148,6 +148,7 @@ class BlockManager:
         cfg.data_fsync, cfg.block_gc_delay_ms = 1 if data_fsync else 0, block_gc_delay_ms
         cfg.local_groups = local_groups
         cfg.piggyback = 1 if piggyback else 0
+        cfg.clay = 1 if clay else 0
         self._prev = (Code * max(1, len(previous_codes)))(*[Code(*map(int, c)) for c in previous_codes])  # kept alive
         cfg.previous_codes = C.cast(self._prev, C.POINTER(Code)) if previous_codes else None
         cfg.n_previous_codes, cfg.legacy_replicas = len(previous_codes), legacy_replicas
@@ -331,7 +332,7 @@ class ShardHeader(C.Structure):
     _fields_ = [("hash", C.c_uint8 * 32), ("header", C.c_uint8), ("k", C.c_uint8), ("m", C.c_uint8),
                 ("index", C.c_uint8), ("sum_kind", C.c_uint8), ("migrated", C.c_uint8),
                 ("block_len", C.c_uint32), ("shard_len", C.c_uint32), ("sum", C.c_uint8 * 32), ("l", C.c_uint8),
-                ("pb", C.c_uint8)]
+                ("pb", C.c_uint8), ("clay", C.c_uint8)]
 
     def as_dict(self):
         d = {"hash": bytes(self.hash), "header": int(self.header), "k": int(self.k), "m": int(self.m),
@@ -341,6 +342,8 @@ class ShardHeader(C.Structure):
             d["l"] = int(self.l)
         if self.pb:  # only PB shards carry it
             d["pb"] = int(self.pb)
+        if self.clay:  # only Clay shards carry it
+            d["clay"] = int(self.clay)
         return d
 
 
@@ -357,12 +360,12 @@ def _wire():
     return L
 
 
-def wire_encode(hash32, header, k, m, index, block_len, shard_len, sum_kind, sum32, l=0, pb=0) -> bytes:
+def wire_encode(hash32, header, k, m, index, block_len, shard_len, sum_kind, sum32, l=0, pb=0, clay=0) -> bytes:
     h = ShardHeader()
     C.memmove(h.hash, bytes(hash32), 32)
     C.memmove(h.sum, bytes(sum32), 32)
     h.header, h.k, h.m, h.index, h.sum_kind = header, k, m, index, sum_kind
-    h.block_len, h.shard_len, h.l, h.pb = block_len, shard_len, l, pb
+    h.block_len, h.shard_len, h.l, h.pb, h.clay = block_len, shard_len, l, pb, clay
     buf = (C.c_uint8 * 256)()
     n = _wire().garage_shard_wire_encode(C.byref(h), buf, 256)
     return bytes(buf[:n])

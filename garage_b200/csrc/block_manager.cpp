@@ -247,7 +247,7 @@ struct ShardFileHeader {
     uint8_t sum[32];
     uint32_t hdr_check;  // Adler-32 of bytes [0, 48)
     uint8_t pad[12];     // pad[0]: LRC local groups (0 = RS, so files written before it existed read as RS); pad[1]: 1 =
-                         // piggybacked RS PB(k, m) (0 = not PB).  Outside hdr_check, so the reader compares them with
+                         // piggybacked RS PB(k, m), 2 = Clay(k, m) (0 = neither).  Outside hdr_check, so the reader compares them with
                          // its own code and quarantines a mismatch
 };
 static_assert(sizeof(ShardFileHeader) == 64, "shard file header is 64 bytes");
@@ -269,8 +269,11 @@ enum ReadResult { kReadOk = 0, kReadMissing = 1, kReadInvalid = 2 };
 struct CodeDesc {
     int k = 0, m = 0, l = 0;  // l: LRC local groups, 0 = RS
     bool pb = false;          // piggybacked RS PB(k, m): shard_len = ceil(block_len / k) rounded up to 128
-    bool operator==(const CodeDesc &o) const { return k == o.k && m == o.m && l == o.l && pb == o.pb; }
-    bool named_by(const ShardFileHeader &hd) const { return hd.k == k && hd.m == m && hd.pad[0] == l && hd.pad[1] == (pb ? 1 : 0); }
+    bool clay = false;        // Clay(k, m): shard_len = ceil(block_len / k) rounded up to `quantum` = 16 * alpha
+    uint32_t quantum = 1;
+    bool operator==(const CodeDesc &o) const { return k == o.k && m == o.m && l == o.l && pb == o.pb && clay == o.clay; }
+    uint8_t kind_byte() const { return clay ? 2 : (pb ? 1 : 0); }  // header pad[1]
+    bool named_by(const ShardFileHeader &hd) const { return hd.k == k && hd.m == m && hd.pad[0] == l && hd.pad[1] == kind_byte(); }
 };
 
 // A node's files for one hash (file store): <hash>.shard, written by this manager or an earlier one; <hash>.legacy,
@@ -312,7 +315,7 @@ struct Node {
         const CodeDesc &c = codes[code];
         if (mt.index < 0 || mt.index >= c.k + c.m) return false;
         const uint64_t L = ((uint64_t)mt.block_len + (unsigned)c.k - 1) / (unsigned)c.k;
-        return mt.shard_len == (c.pb ? (L + 127) / 128 * 128 : L);
+        return mt.shard_len == (L + c.quantum - 1) / c.quantum * c.quantum;
     }
     // all store_* are called with `mu` held
     // the code a shard file's header names: an index into `codes`, -1 for another code or a damaged header, -2 if the
@@ -460,7 +463,7 @@ struct Node {
         memcpy(hd.sum, mt.sum.data(), 32);
         hd.hdr_check = adler32_small(reinterpret_cast<const uint8_t *>(&hd), 48);
         hd.pad[0] = (uint8_t)l;
-        hd.pad[1] = pb ? 1 : 0;
+        hd.pad[1] = codes[0].kind_byte();
         FILE *f = fopen(tmp.c_str(), "wb");
         if (!f) return false;
         bool ok = fwrite(&hd, sizeof(hd), 1, f) == 1 && (n == 0 || fwrite(bytes, n, 1, f) == 1);
@@ -942,7 +945,7 @@ struct garage_bm {
     std::atomic<uint64_t> bytes_written{0}, bytes_read{0}, corruption_counter{0}, resync_counter{0},
         resync_error_counter{0}, resync_recv_counter{0}, delete_counter{0}, put_calls{0}, reconstruct_calls{0},
         scrub_checked{0}, scrub_corrupt{0}, enc_gpu_us{0}, rec_gpu_us{0}, corrupt_data_errors{0}, write_errors{0},
-        resync_shards_read{0}, resync_bytes_read{0};
+        resync_shards_read{0}, resync_bytes_read{0}, resync_bytes_fetched{0};
     std::atomic<uint64_t> put_ns_slot{0}, put_ns_land{0}, put_ns_wait{0}, put_ns_store{0};
     std::atomic<uint64_t> convert_blocks{0}, convert_bytes_read{0}, convert_bytes_written{0}, convert_errors{0},
         convert_call_us{0}, legacy_gets{0}, legacy_deleted{0};
@@ -950,6 +953,20 @@ struct garage_bm {
         layout_deleted{0}, layout_sync_errors{0};
 
     bool pb = false;  // PB(k, m) contexts (garage_bm_config.piggyback)
+    // Bytes a rebuild from the shards `have` hands to the GPU, which is what crosses the network in Garage: the runs
+    // garage_ec_read_ranges names for a Clay stripe (1/m of each helper for a lone lost shard), else what was read
+    uint64_t fetched_bytes(const uint8_t *have, const uint8_t *want, uint32_t block_len, uint64_t read_bytes) const
+    {
+        if (!codes[0].clay) return read_bytes;
+        garage_ec_range runs[(GARAGE_EC_MAX_K + GARAGE_EC_MAX_M) * 256];
+        size_t n = 0;
+        if (garage_ec_read_ranges(codes[0].ctx, have, want, (uint32_t)shard_len_of(block_len), runs,
+                                  sizeof(runs) / sizeof(runs[0]), &n) != GARAGE_EC_OK)
+            return read_bytes;
+        uint64_t b = 0;
+        for (size_t i = 0; i < n; i++) b += runs[i].len;
+        return b;
+    }
     // codes[0]: the configured code (ctx = ec); codes[1..]: garage_bm_config.previous_codes, one context each.  Shard i
     // of every code lives on the i-th node of the block's ring row.
     struct Code : CodeDesc {
@@ -1281,6 +1298,15 @@ struct garage_bm {
         const int k = cd.k, tot = cd.tot;
         const bool pb = cd.pb;
         garage_ec_ctx *const ec = cd.ctx;
+        // what to read of each shard: halves (bit 0 a, bit 1 b) from garage_ec_read_plan; Clay: whole shards of
+        // garage_ec_read_set (each holder checks its whole shard's tag; only the garage_ec_read_ranges runs of it are
+        // handed to the rebuild)
+        auto plan = [&](const uint8_t *pr, const uint8_t *wn, uint8_t *rd) {
+            if (!cd.clay) return garage_ec_read_plan(ec, pr, wn, rd);
+            const int rc = garage_ec_read_set(ec, pr, wn, rd);
+            for (int i = 0; i < tot; i++) rd[i] = rd[i] ? 3 : 0;
+            return rc;
+        };
         constexpr int kMaxSrc = GARAGE_BM_MAX_LAYOUT_VERSIONS;
         int src[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M][kMaxSrc], nsrc[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0},
             cur[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
@@ -1388,7 +1414,7 @@ struct garage_bm {
                 // plan still lacks (RS / LRC: whole shards of the read set; PB: the planned halves)
                 uint8_t guess[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M], rd[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
                 for (int i = 0; i < tot; i++) guess[i] = have[i] || (!want[i] && left(i));
-                if (garage_ec_read_plan(ec, guess, want, rd) != GARAGE_EC_OK) break;
+                if (plan(guess, want, rd) != GARAGE_EC_OK) break;
                 bool fetched = false, missing = false;
                 for (int i = 0; i < tot; i++) {
                     const int need = rd[i] & ~have_h[i];
@@ -1412,7 +1438,7 @@ struct garage_bm {
             uint8_t rd[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
             if (all)
                 for (int i = 0; i < k; i++) want[i] = !have[i];
-            *ok = garage_ec_read_plan(ec, have, want, rd) == GARAGE_EC_OK;
+            *ok = plan(have, want, rd) == GARAGE_EC_OK;
             for (int i = 0; i < tot && *ok; i++) *ok = (rd[i] & ~have_h[i]) == 0;  // every planned half is here
         }
         if (bytes_out) *bytes_out += nbytes;
@@ -1720,6 +1746,7 @@ struct garage_bm {
         resync_shards_read += (uint64_t)gather_into(h, node, slot.p, have, block_len, false, /*for_gpu=*/true, want, &ok,
                                                     &nbytes);
         resync_bytes_read += nbytes;
+        resync_bytes_fetched += ok ? fetched_bytes(have, want, block_len, nbytes) : nbytes;
         if (multi) layout_bytes_read += nbytes;
         if (!ok) {
             // no configured stripe to rebuild from, but maybe a block stored before the code changed: convert it
@@ -2121,7 +2148,7 @@ struct garage_bm {
     // garage_bm_apply_layout: see include/garage_block_manager.h
     int apply_layout(const garage_bm_layout_spec *spec, uint64_t *version_out)
     {
-        if (nodes[0]->dir.empty() || has_legacy()) return GARAGE_EC_E_INVALID;
+        if (nodes[0]->dir.empty() || has_legacy() || codes[0].clay) return GARAGE_EC_E_INVALID;
         std::lock_guard<std::mutex> lk(layout_mu);
         const auto ls = layouts();
         if (!ls->newest() || ls->v.size() >= GARAGE_BM_MAX_LAYOUT_VERSIONS) return GARAGE_EC_E_INVALID;
@@ -2789,6 +2816,7 @@ void garage_bm_default_config(garage_bm_config *c)
     c->n_previous_codes = 0;
     c->legacy_replicas = 0;
     c->layout = nullptr;            // the fixed ring
+    c->clay = 0;                    // not Clay
 }
 
 // a code garage_ec_create / _lrc / _piggyback accepts, with tags the block manager can check: the same rules as the
@@ -2814,6 +2842,14 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
     // PB is not combined with LRC, and its half reads need per-segment (adler8) tags
     if ((cfg->piggyback != 0 && cfg->piggyback != 1) || (pb && (l > 0 || cfg->shard_sum_kind == GARAGE_EC_SUM_BLAKE2)))
         return GARAGE_EC_E_INVALID;
+    // Clay(k, m) (garage_ec_create_clay's rules): not combined with LRC or PB, and without layout changes
+    const bool clay = cfg->clay != 0;
+    if (cfg->clay != 0 && cfg->clay != 1) return GARAGE_EC_E_INVALID;
+    if (clay) {
+        int alpha = 1;
+        for (int t = (k + m + m - 1) / m; t > 0 && alpha <= 256; t--) alpha *= m;
+        if (m < 2 || m > 4 || k < 2 || alpha > 256 || pb || l > 0 || cfg->layout) return GARAGE_EC_E_INVALID;
+    }
     // previous codes and replicas (all checked before any CUDA call)
     const int np = cfg->n_previous_codes;
     if (np < 0 || np > GARAGE_BM_MAX_PREVIOUS_CODES || (np > 0 && !cfg->previous_codes)) return GARAGE_EC_E_INVALID;
@@ -2822,7 +2858,7 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
         const garage_bm_code &p = cfg->previous_codes[i];
         if (!code_ok(p.k, p.m, p.local_groups, p.piggyback, cfg->shard_sum_kind) || p.k + p.m > cfg->n_nodes)
             return GARAGE_EC_E_INVALID;
-        if (p.k == k && p.m == m && p.local_groups == l && (p.piggyback != 0) == pb) return GARAGE_EC_E_INVALID;
+        if (!clay && p.k == k && p.m == m && p.local_groups == l && (p.piggyback != 0) == pb) return GARAGE_EC_E_INVALID;
         for (int j = 0; j < i; j++) {
             const garage_bm_code &q = cfg->previous_codes[j];
             if (p.k == q.k && p.m == q.m && p.local_groups == q.local_groups && p.piggyback == q.piggyback)
@@ -2847,9 +2883,11 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
     }
     // a store changes its layout or its code, not both at once
     if (lays->v.size() > 1 && (np > 0 || cfg->legacy_replicas > 0)) return GARAGE_EC_E_INVALID;
+    if (clay && layout_file) return GARAGE_EC_E_INVALID;  // a Clay store keeps the fixed ring
     // every context of the manager runs the same code: RS(k, m), LRC(k, l, m - l) or PB(k, m)
     auto make_ctx = [&](garage_ec_ctx **c) {
-        return pb ? garage_ec_create_piggyback(c, cfg->cuda_device, k, m, GARAGE_EC_VANDERMONDE)
+        return clay ? garage_ec_create_clay(c, cfg->cuda_device, k, m, GARAGE_EC_VANDERMONDE)
+             : pb ? garage_ec_create_piggyback(c, cfg->cuda_device, k, m, GARAGE_EC_VANDERMONDE)
                   : l ? garage_ec_create_lrc(c, cfg->cuda_device, k, l, m - l)
                       : garage_ec_create(c, cfg->cuda_device, k, m, GARAGE_EC_VANDERMONDE);
     };
@@ -2869,6 +2907,13 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
     bm->codes[0].m = m;
     bm->codes[0].l = l;
     bm->codes[0].pb = pb;
+    bm->codes[0].clay = clay;
+    bm->codes[0].quantum = pb ? 128u : 1u;
+    if (clay) {
+        int alpha = 0;
+        garage_ec_clay_info(bm->ec, nullptr, nullptr, &alpha, nullptr, nullptr);
+        bm->codes[0].quantum = 16u * (uint32_t)alpha;
+    }
     bm->codes[0].tot = k + m;
     bm->codes[0].ctx = bm->ec;
     bm->legacy_rf = cfg->legacy_replicas;
@@ -2881,6 +2926,7 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
         c.m = p.m;
         c.l = p.local_groups;
         c.pb = p.piggyback != 0;
+        c.quantum = c.pb ? 128u : 1u;
         c.tot = p.k + p.m;
         rc = c.pb ? garage_ec_create_piggyback(&c.ctx, cfg->cuda_device, p.k, p.m, GARAGE_EC_VANDERMONDE)
              : c.l ? garage_ec_create_lrc(&c.ctx, cfg->cuda_device, p.k, c.l, p.m - c.l)
@@ -3347,6 +3393,7 @@ void garage_bm_get_metrics(garage_bm *bm, garage_bm_metrics *o)
     o->write_errors = bm->write_errors;
     o->resync_shards_read = bm->resync_shards_read;
     o->resync_bytes_read = bm->resync_bytes_read;
+    o->resync_bytes_fetched = bm->resync_bytes_fetched;
     o->convert_blocks = bm->convert_blocks;
     o->convert_bytes_read = bm->convert_bytes_read;
     o->convert_bytes_written = bm->convert_bytes_written;

@@ -29,6 +29,7 @@
 #include <vector>
 
 #include "rs_kernels.cuh"
+#include "clay_kernels.cuh"
 
 using namespace garage_ec;
 
@@ -62,6 +63,9 @@ struct garage_ec_ctx {
     int device = 0, k = 0, m = 0;
     int l = 0;  // LRC local groups (garage_ec_create_lrc); 0 = RS (MDS: any k shards decode)
     bool pb = false;  // piggybacked RS PB(k, m) (garage_ec_create_piggyback, DESIGN.md section 2.2)
+    bool clay = false;  // Clay(k, m) (garage_ec_create_clay, DESIGN.md section 2.4): P is then the m x (k+s) base rows
+    ClayGeo cg{};
+    uint32_t quantum = 1;  // code_shard_len rounding: 1 (RS, LRC), 128 (PB), 16*alpha (Clay)
     uint8_t P[kMaxM * kMaxK] = {0};
     int sm_count = 0;
     size_t smem_optin = 0;
@@ -422,6 +426,66 @@ bool make_src_tensor_map(CUtensorMap *tm, const uint8_t *src, size_t stride, siz
 #endif
 }
 
+// ---- Clay(k, m) (clay_kernels.cuh) ------------------------------------------------------------------------------
+ClayParams clay_params(const garage_ec_ctx *ctx, size_t stride, size_t n)
+{
+    ClayParams c;
+    memset(&c, 0, sizeof(c));
+    c.stride = (uint32_t)stride;
+    c.n = (uint32_t)n;
+    c.k = (uint32_t)ctx->k;
+    c.m = (uint32_t)ctx->m;
+    c.s = (uint32_t)ctx->cg.s;
+    c.q = (uint32_t)ctx->cg.q;
+    c.t = (uint32_t)ctx->cg.t;
+    c.alpha = (uint32_t)ctx->cg.alpha;
+    c.ips = (uint32_t)((stride / ctx->cg.alpha + kClayColBytes - 1) / kClayColBytes);
+    for (int y = 0, v = 1; y <= ctx->cg.t; y++, v *= ctx->cg.q) c.qpow[y] = (uint32_t)v;
+    memcpy(c.coef, ctx->P, (size_t)(ctx->k + ctx->cg.s) * ctx->m);
+    return c;
+}
+template <int MODE>
+cudaError_t launch_clay(garage_ec_ctx *ctx, const ClayParams &c, cudaStream_t st)
+{
+    static std::atomic<int> configured_for_device{-1};  // per instantiation
+    const size_t smem = (size_t)ctx->cg.alpha * clay_layer_words((uint32_t)ctx->cg.n) * 4;
+    auto kern = clay_apply_kernel<MODE>;
+    if (configured_for_device.load(std::memory_order_acquire) != ctx->device) {
+        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             (int)(kClayMaxAlpha * clay_layer_words(kClayMaxNodes) * 4));
+        if (e != cudaSuccess) return e;
+        configured_for_device.store(ctx->device, std::memory_order_release);
+    }
+    ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    const size_t items = (size_t)c.n * c.ips;
+    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>(items, (size_t)ctx->sm_count * 16));
+    kern<<<grid, kClayThreads, smem, st>>>(c);
+    return cudaGetLastError();
+}
+// encode (mode 0) / verify (mode 2): one launch; n * items per stripe stays below 2^32 by the stride check
+int run_clay(garage_ec_ctx *ctx, int mode, const uint8_t *src, size_t src_pitch, uint8_t *dst, size_t dst_pitch,
+             uint32_t *mismatch, const uint32_t *shard_len, size_t stride, size_t n, cudaStream_t st)
+{
+    if (n == 0) return GARAGE_EC_OK;
+    ClayParams c = clay_params(ctx, stride, n);
+    c.src = src;
+    c.src_pitch = src_pitch;
+    c.shard_len = shard_len;
+    c.mismatch = mismatch;
+    if (mode == kModeEncode) {
+        c.dst = dst;
+        c.dst_pitch = dst_pitch;
+    } else {  // verify reads the stored parities of the shard layout
+        c.dst = const_cast<uint8_t *>(src);
+        c.dst_pitch = src_pitch;
+        c.par_off = (uint32_t)ctx->k;
+    }
+    TimedLaunch tl(ctx, st);
+    cudaError_t e = mode == kModeEncode ? launch_clay<kModeEncode>(ctx, c, st) : launch_clay<kModeVerify>(ctx, c, st);
+    if (e != cudaSuccess) return set_cuda_error(ctx, e, "clay_apply_kernel launch");
+    return GARAGE_EC_OK;
+}
+
 // Device-resident encode (mode 0) / verify (mode 2) of n stripes, split so that
 // n * items_per_stripe stays below 2^32 and m > 4 runs in passes of 4 rows.
 int run_uniform(garage_ec_ctx *ctx, int mode, const uint8_t *src, size_t src_pitch, uint8_t *dst,
@@ -429,6 +493,7 @@ int run_uniform(garage_ec_ctx *ctx, int mode, const uint8_t *src, size_t src_pit
                 size_t n, cudaStream_t st, bool allow_tmap = true)
 {
     if (ctx->pb) return run_pb_uniform(ctx, mode, src, src_pitch, dst, dst_pitch, mismatch, shard_len, stride, n, st);
+    if (ctx->clay) return run_clay(ctx, mode, src, src_pitch, dst, dst_pitch, mismatch, shard_len, stride, n, st);
     const uint32_t ips = items_per_stripe(stride);
     // the kernel's work counter runs past the item count by at most two claimed runs per warp
     const size_t max_n = (0xffffffffull - (1ull << 24)) / ips;
@@ -481,6 +546,48 @@ int run_reconstruct(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *present,
                     int32_t *status, const uint32_t *shard_len, size_t stride, size_t n,
                     StripePlan *plan, uint32_t *counter, cudaStream_t st, bool present_is_bad = false)
 {
+    if (ctx->clay) {
+        // the caller's maps onto the n' nodes of the base code (after the counter, plan_scratch_bytes), the base-code
+        // plan by plan_kernel, then the layered decode / repair
+        const int N = ctx->cg.n, kb = ctx->k + ctx->cg.s;
+        uint8_t *present2 = reinterpret_cast<uint8_t *>(counter) + 16, *want2 = present2 + n * N;
+        ClayParams c = clay_params(ctx, stride, n);
+        c.src = shards;
+        c.dst = shards;
+        c.src_pitch = c.dst_pitch = (size_t)(ctx->k + ctx->m) * stride;
+        c.par_off = (uint32_t)ctx->k;
+        c.shard_len = shard_len;
+        c.present = present;
+        c.want = want;
+        c.status = status;
+        c.present_is_bad = present_is_bad ? 1u : 0u;
+        c.plan = plan;
+        clay_prep_kernel<<<(unsigned)std::min<size_t>((n + 255) / 256, (size_t)ctx->sm_count * 4), 256, 0, st>>>(c, present2,
+                                                                                                             want2);
+        ctx->launches.fetch_add(1, std::memory_order_relaxed);
+        cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return set_cuda_error(ctx, e, "clay_prep_kernel launch");
+        PlanParams q;
+        memset(&q, 0, sizeof(q));
+        q.present = present2;
+        q.want = want2;
+        q.status = status;
+        q.plan = plan;
+        q.counter = counter;
+        q.n = (uint32_t)n;
+        q.k = (uint32_t)kb;
+        q.m = (uint32_t)ctx->m;
+        q.stride = (uint32_t)stride;
+        memcpy(q.P, ctx->P, (size_t)kb * ctx->m);
+        plan_kernel<<<(unsigned)((n + kPlanWarps - 1) / kPlanWarps), kPlanWarps * 32, 0, st>>>(q);
+        ctx->launches.fetch_add(1, std::memory_order_relaxed);
+        e = cudaGetLastError();
+        if (e != cudaSuccess) return set_cuda_error(ctx, e, "plan_kernel launch");
+        TimedLaunch tl(ctx, st);
+        e = launch_clay<kModePlan>(ctx, c, st);
+        if (e != cudaSuccess) return set_cuda_error(ctx, e, "clay_apply_kernel<plan> launch");
+        return GARAGE_EC_OK;
+    }
     PlanParams q;
     memset(&q, 0, sizeof(q));
     q.present = present;
@@ -531,7 +638,11 @@ int run_reconstruct(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *present,
     return GARAGE_EC_OK;
 }
 
-size_t plan_scratch_bytes(size_t n) { return n * sizeof(StripePlan) + 16; }
+// StripePlans | apply counter (16 B) | Clay: the present / want maps of the base code, n' bytes each per stripe
+size_t plan_scratch_bytes(const garage_ec_ctx *ctx, size_t n)
+{
+    return n * sizeof(StripePlan) + 16 + (ctx->clay ? (2 * n * (size_t)ctx->cg.n + 15) / 16 * 16 : 0);
+}
 
 // The half-shards plan_kernel reads for one stripe (present / want: k+m bytes, want nullable = every absent
 // shard): bit 2i / 2i+1 of *halves = a- / b-half of shard i, both for every shard read by RS and LRC.  False if a
@@ -544,7 +655,8 @@ bool stripe_read_plan(const garage_ec_ctx *ctx, const uint8_t *present, const ui
         wm |= (uint64_t)(!want || want[i] != 0) << i;
     }
     uint64_t rows = 0;
-    const bool ok = h_read_plan(PlanCode{ctx->k, ctx->m, ctx->l, ctx->pb, ctx->P}, pm, wm, &rows);
+    const bool ok = ctx->clay ? clay_read_set(ctx->k, ctx->m, pm, wm, &rows)
+                              : h_read_plan(PlanCode{ctx->k, ctx->m, ctx->l, ctx->pb, ctx->P}, pm, wm, &rows);
     *halves = rows;
     if (!ctx->pb)  // RS and LRC rows are shards
         for (*halves = 0; rows; rows &= rows - 1) *halves |= 3ull << (2 * ctz64(rows));
@@ -560,29 +672,47 @@ bool stripe_read_set(const garage_ec_ctx *ctx, const uint8_t *present, const uin
     return ok;
 }
 // The pieces of shard i a HOST upload copies, as f(offset, bytes): `whole` bytes from 0 for a shard of the read set,
-// or (PB) each planned half of shard_len/2 bytes
+// (PB) each planned half of shard_len/2 bytes, or (Clay repair: every shard but one is read) the runs of the repair
+// layers {z : z_y0 = x0} of the one absent shard f = (x0, y0), q^y0 sub-chunks every q^(y0+1)
 template <class F>
 void for_each_read_piece(const garage_ec_ctx *ctx, uint64_t halves, size_t i, size_t len, size_t whole, F &&f)
 {
     const unsigned b = (unsigned)(halves >> (2 * i)) & 3u;
     if (!b) return;
+    if (ctx->clay) {
+        const int tot = ctx->k + ctx->m;
+        int nread = 0, f_shard = 0;
+        for (int j = 0; j < tot; j++) {
+            if ((halves >> (2 * j)) & 3) nread++;
+            else f_shard = j;
+        }
+        if (nread != tot - 1) return f((size_t)0, whole);
+        const int a = clay_node(ctx->k, ctx->cg.s, f_shard), q = ctx->cg.q, x0 = a % q, y0 = a / q;
+        size_t run = 1;
+        for (int y = 0; y < y0; y++) run *= (size_t)q;
+        const size_t sub = len / (size_t)ctx->cg.alpha, period = run * q;
+        for (size_t z0 = x0 * run; z0 < (size_t)ctx->cg.alpha; z0 += period) f(z0 * sub, run * sub);
+        return;
+    }
     if (!ctx->pb) f((size_t)0, whole);
     else if (b == 3) f((size_t)0, len);
     else f(b == 1 ? (size_t)0 : len / 2, len / 2);
 }
-// PB: every stripe's shard_len (NULL: stride) must be a multiple of 32 so that the halves are 16-byte aligned
+// PB: every stripe's shard_len (NULL: stride) must be a multiple of 32 so that the halves are 16-byte aligned; Clay: a
+// multiple of 16*alpha, so that every layer's sub-chunk is
 bool pb_lens_ok(const garage_ec_ctx *ctx, const uint32_t *shard_len, size_t stride, size_t n)
 {
-    if (!ctx->pb) return true;
-    if (!shard_len) return (stride & 31) == 0;
+    if (!ctx->pb && !ctx->clay) return true;
+    const size_t unit = ctx->clay ? (size_t)ctx->quantum : 32;
+    if (!shard_len) return stride % unit == 0;
     for (size_t s = 0; s < n; s++)
-        if ((shard_len[s] & 31) || shard_len[s] > stride) return false;
+        if ((shard_len[s] % unit) || shard_len[s] > stride) return false;
     return true;
 }
-// 64-bit: a PB length that does not fit in 32 bits is larger than any stride, so the stride checks reject it
+// 64-bit: a PB or Clay length that does not fit in 32 bits is larger than any stride, so the stride checks reject it
 uint64_t code_shard_len(const garage_ec_ctx *ctx, uint32_t block_len)
 {
-    return ::garage_ec::code_shard_len(block_len, ctx->k, ctx->pb);
+    return ::garage_ec::code_shard_len(block_len, ctx->k, ctx->quantum);
 }
 
 // ---- batched async copies ---------------------------------------------------------------
@@ -668,7 +798,8 @@ int lane_reserve(garage_ec_ctx *ctx, HostLane &L, size_t buf_bytes, size_t small
 
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
-int create_common(garage_ec_ctx **out, int device, int k, int m, const uint8_t *P, int kind, int l = 0, bool pb = false)
+int create_common(garage_ec_ctx **out, int device, int k, int m, const uint8_t *P, int kind, int l = 0, bool pb = false,
+                  const ClayGeo *clay = nullptr)
 {
     if (!out) return GARAGE_EC_E_INVALID;
     *out = nullptr;
@@ -689,9 +820,15 @@ int create_common(garage_ec_ctx **out, int device, int k, int m, const uint8_t *
     ctx->m = m;
     ctx->l = l;
     ctx->pb = pb;
+    ctx->quantum = pb ? kPbQuantum : 1;
+    if (clay) {
+        ctx->clay = true;
+        ctx->cg = *clay;
+        ctx->quantum = kClayColBytes * (uint32_t)clay->alpha;
+    }
     if (P) {
         memcpy(ctx->P, P, (size_t)k * m);
-    } else if (!h_build_matrix(k, m, kind, ctx->P)) {
+    } else if (!h_build_matrix(clay ? k + clay->s : k, m, kind, ctx->P)) {
         delete ctx;
         return GARAGE_EC_E_INVALID;
     }
@@ -775,6 +912,52 @@ int garage_ec_create_piggyback(garage_ec_ctx **out, int cuda_device, int k, int 
     return create_common(out, cuda_device, k, m, nullptr, matrix_kind, 0, true);
 }
 
+int garage_ec_create_clay(garage_ec_ctx **out, int cuda_device, int k, int m, int matrix_kind)
+{
+    ClayGeo g;
+    if (!clay_geometry(k, m, &g) || (matrix_kind != GARAGE_EC_VANDERMONDE && matrix_kind != GARAGE_EC_CAUCHY)) {
+        if (out) *out = nullptr;
+        return GARAGE_EC_E_INVALID;
+    }
+    return create_common(out, cuda_device, k, m, nullptr, matrix_kind, 0, false, &g);
+}
+
+int garage_ec_clay_info(const garage_ec_ctx *ctx, int *q, int *t, int *alpha, int *virtual_nodes, uint8_t *base_rows)
+{
+    if (!ctx) return GARAGE_EC_E_INVALID;
+    if (q) *q = ctx->clay ? ctx->cg.q : 0;
+    if (t) *t = ctx->clay ? ctx->cg.t : 0;
+    if (alpha) *alpha = ctx->clay ? ctx->cg.alpha : 1;
+    if (virtual_nodes) *virtual_nodes = ctx->clay ? ctx->cg.s : 0;
+    if (base_rows && ctx->clay) memcpy(base_rows, ctx->P, (size_t)(ctx->k + ctx->cg.s) * ctx->m);
+    return GARAGE_EC_OK;
+}
+
+int garage_ec_read_ranges(const garage_ec_ctx *ctx, const uint8_t *present, const uint8_t *want, uint32_t shard_len,
+                          garage_ec_range *ranges, size_t cap, size_t *n_ranges)
+{
+    if (!ctx || !present || !n_ranges || (cap && !ranges)) return GARAGE_EC_E_INVALID;
+    *n_ranges = 0;
+    if (ctx->pb && (shard_len & 31)) return GARAGE_EC_E_INVALID;
+    if (ctx->clay && shard_len % ctx->quantum) return GARAGE_EC_E_INVALID;
+    uint64_t hv = 0;
+    const bool ok = stripe_read_plan(ctx, present, want, &hv);
+    if (!ok) return GARAGE_EC_E_UNRECOVERABLE;
+    size_t cnt = 0;
+    for (int i = 0; i < ctx->k + ctx->m; i++)
+        for_each_read_piece(ctx, hv, (size_t)i, shard_len, shard_len, [&](size_t off, size_t bytes) {
+            if (cnt && cnt <= cap && ranges[cnt - 1].shard == (uint32_t)i &&
+                ranges[cnt - 1].offset + ranges[cnt - 1].len == off) {
+                ranges[cnt - 1].len += (uint32_t)bytes;  // adjacent: merged
+                return;
+            }
+            if (cnt < cap) ranges[cnt] = garage_ec_range{(uint32_t)i, (uint32_t)off, (uint32_t)bytes};
+            cnt++;
+        });
+    *n_ranges = cnt;
+    return cnt > cap ? GARAGE_EC_E_INVALID : GARAGE_EC_OK;
+}
+
 int garage_ec_piggyback_info(const garage_ec_ctx *ctx, int *groups, uint8_t *group_of)
 {
     if (!ctx) return GARAGE_EC_E_INVALID;
@@ -795,7 +978,7 @@ int garage_ec_code_shard_len(const garage_ec_ctx *ctx, uint32_t block_len, uint3
 
 int garage_ec_read_plan(const garage_ec_ctx *ctx, const uint8_t *present, const uint8_t *want, uint8_t *halves_out)
 {
-    if (!ctx || !present || !halves_out) return GARAGE_EC_E_INVALID;
+    if (!ctx || !present || !halves_out || ctx->clay) return GARAGE_EC_E_INVALID;
     uint64_t hv = 0;
     const bool ok = stripe_read_plan(ctx, present, want, &hv);
     for (int i = 0; i < ctx->k + ctx->m; i++) halves_out[i] = (uint8_t)((hv >> (2 * i)) & 3);
@@ -865,7 +1048,7 @@ void garage_ec_destroy(garage_ec_ctx *ctx)
 
 int garage_ec_matrix(const garage_ec_ctx *ctx, uint8_t *out_m_by_k)
 {
-    if (!ctx || !out_m_by_k) return GARAGE_EC_E_INVALID;
+    if (!ctx || !out_m_by_k || ctx->clay) return GARAGE_EC_E_INVALID;
     memcpy(out_m_by_k, ctx->P, (size_t)ctx->k * ctx->m);
     return GARAGE_EC_OK;
 }
@@ -1030,7 +1213,7 @@ static int encode_host(garage_ec_ctx *ctx, const uint8_t *data, uint8_t *parity,
                        const uint32_t *shard_len, size_t stride, size_t n)
 {
     LEASE_LANES(ctx, lanes);
-    if (ctx->zero_copy_enc && device_addressable_host(data) && device_addressable_host(parity)) {
+    if (ctx->zero_copy_enc && !ctx->clay && device_addressable_host(data) && device_addressable_host(parity)) {
         // one launch over the whole batch: the TMA / vector loads pull the data shards across PCIe, the parity stores
         // go straight to the caller's buffer -- no staging copies, no chunk boundaries
         HostLane &L = lanes[0];
@@ -1168,13 +1351,13 @@ static int reconstruct_host(garage_ec_ctx *ctx, uint8_t *shards, uint8_t *const 
     std::vector<int32_t> st_host(status ? 0 : n);
     CopyBatch up, down;
     LEASE_LANES(ctx, lanes);
-    if (ctx->zero_copy_rec && !stripes && device_addressable_host(shards)) {
+    if (ctx->zero_copy_rec && !ctx->clay && !stripes && device_addressable_host(shards)) {
         // the kernel reads the k survivors of every stripe and writes the rebuilt shards in the caller's pinned buffer
         const size_t tot_ = ctx->k + ctx->m;
         const size_t zo_present = 0, zo_want = align_up(n * tot_, 16), zo_status = zo_want + align_up(n * tot_, 16);
         const size_t zo_len = zo_status + align_up(n * 4, 16), zo_plan = zo_len + align_up(n * 4, 16);
         HostLane &L = lanes[0];
-        int rcz = lane_reserve(ctx, L, 0, zo_plan + plan_scratch_bytes(n));
+        int rcz = lane_reserve(ctx, L, 0, zo_plan + plan_scratch_bytes(ctx, n));
         if (rcz) return rcz;
         CU_TRY(ctx, cudaMemcpyAsync(L.d_small + zo_present, present, n * tot_, cudaMemcpyHostToDevice, L.stream));
         const uint8_t *d_want = nullptr;
@@ -1207,7 +1390,7 @@ static int reconstruct_host(garage_ec_ctx *ctx, uint8_t *shards, uint8_t *const 
     // small buffer layout per lane: present | want | status | shard_len | plan+counter
     const size_t o_present = 0, o_want = align_up(cs * tot, 16), o_status = o_want + align_up(cs * tot, 16);
     const size_t o_len = o_status + align_up(cs * 4, 16), o_plan = o_len + align_up(cs * 4, 16);
-    const size_t small = o_plan + plan_scratch_bytes(cs);
+    const size_t small = o_plan + plan_scratch_bytes(ctx, cs);
     for (HostLane &L : lanes.set->lanes) {
         int rc = lane_reserve(ctx, L, cs * tot * stride, small);
         if (rc) return rc;
@@ -1293,8 +1476,8 @@ int garage_ec_reconstruct(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *pr
         return reconstruct_host(ctx, shards, nullptr, present, want, status, shard_len, stride, n_stripes);
     cudaStream_t st = (cudaStream_t)cuda_stream;
     void *scratch = nullptr;
-    CU_TRY(ctx, ctx->pool ? cudaMallocFromPoolAsync(&scratch, plan_scratch_bytes(n_stripes), ctx->pool, st)
-                          : cudaMallocAsync(&scratch, plan_scratch_bytes(n_stripes), st));
+    CU_TRY(ctx, ctx->pool ? cudaMallocFromPoolAsync(&scratch, plan_scratch_bytes(ctx, n_stripes), ctx->pool, st)
+                          : cudaMallocAsync(&scratch, plan_scratch_bytes(ctx, n_stripes), st));
     StripePlan *plan = reinterpret_cast<StripePlan *>(scratch);
     uint32_t *counter =
         reinterpret_cast<uint32_t *>(reinterpret_cast<uint8_t *>(scratch) + n_stripes * sizeof(StripePlan));
@@ -1628,8 +1811,8 @@ int garage_ec_scrub_repair(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *e
         rc = run_sums(ctx, shards, expect_sums, shard_len, stride, n_stripes * tot, (int)tot, nullptr, bad_out, st);
         if (rc) return rc;
         void *scratch = nullptr;
-        CU_TRY(ctx, ctx->pool ? cudaMallocFromPoolAsync(&scratch, plan_scratch_bytes(n_stripes), ctx->pool, st)
-                          : cudaMallocAsync(&scratch, plan_scratch_bytes(n_stripes), st));
+        CU_TRY(ctx, ctx->pool ? cudaMallocFromPoolAsync(&scratch, plan_scratch_bytes(ctx, n_stripes), ctx->pool, st)
+                          : cudaMallocAsync(&scratch, plan_scratch_bytes(ctx, n_stripes), st));
         StripePlan *plan = reinterpret_cast<StripePlan *>(scratch);
         uint32_t *counter =
             reinterpret_cast<uint32_t *>(reinterpret_cast<uint8_t *>(scratch) + n_stripes * sizeof(StripePlan));
@@ -1651,7 +1834,7 @@ int garage_ec_scrub_repair(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *e
     if (cs > n_stripes) cs = n_stripes;
     const size_t o_exp = 0, o_bad = o_exp + cs * tot * 32, o_status = o_bad + align_up(cs * tot, 16);
     const size_t o_len = o_status + align_up(cs * 4, 16), o_plan = o_len + align_up(cs * 4, 16);
-    const size_t small = o_plan + plan_scratch_bytes(cs);
+    const size_t small = o_plan + plan_scratch_bytes(ctx, cs);
     for (HostLane &L : lanes.set->lanes) {
         rc = lane_reserve(ctx, L, cs * tot * stride, small);
         if (rc) return rc;
@@ -1792,7 +1975,7 @@ int garage_ec_encode_blocks_with_sums(garage_ec_ctx *ctx, const uint8_t *const *
         sp.stride = (uint32_t)stride;
         sp.k = (uint32_t)k;
         sp.n = (uint32_t)cnt;
-        sp.round128 = ctx->pb ? 1u : 0u;
+        sp.quantum = ctx->quantum;
         // ~4 CTAs per SM whatever the batch size (one CTA per block left 13 SMs copying 1 MiB each: 150 us)
         sp.parts = (uint32_t)std::max<size_t>(1, std::min<size_t>(64, ((size_t)ctx->sm_count * 4 + cnt - 1) / cnt));
         split_blocks_kernel<<<(unsigned)std::min<size_t>(cnt * sp.parts, (size_t)ctx->sm_count * 8), 256, 0, L.stream>>>(sp);
@@ -1877,7 +2060,7 @@ int garage_ec_decode_blocks(garage_ec_ctx *ctx, const uint8_t *shards, const uin
         if (cs > need.size()) cs = need.size();
         const size_t o_present = 0, o_want = align_up(cs * tot, 16), o_status = o_want + align_up(cs * tot, 16);
         const size_t o_len = o_status + align_up(cs * 4, 16), o_plan = o_len + align_up(cs * 4, 16);
-        const size_t small = o_plan + plan_scratch_bytes(cs);
+        const size_t small = o_plan + plan_scratch_bytes(ctx, cs);
         // host staging and copy lists are declared before the lane lease: they outlive its stream work
         std::vector<uint8_t> h_small((2 * cs * tot + cs * 4) * kHostLanes);
         CopyBatch up, down;
@@ -1971,7 +2154,7 @@ namespace {
 // device scratch of run_transcode for n stripes: src_len | dst_len | geo | status (caller passed none) | want | plan
 struct TranscodeScratch {
     size_t o_src_len, o_dst_len, o_geo, o_status, o_want, o_plan, bytes;
-    TranscodeScratch(size_t n, size_t src_tot, bool degraded)
+    TranscodeScratch(const garage_ec_ctx *src, size_t n, size_t src_tot, bool degraded)
     {
         const size_t a = align_up(n * 4, 16);
         o_src_len = 0;
@@ -1980,7 +2163,7 @@ struct TranscodeScratch {
         o_status = 3 * a;
         o_want = 4 * a;
         o_plan = o_want + (degraded ? align_up(n * src_tot, 16) : 0);
-        bytes = o_plan + (degraded ? plan_scratch_bytes(n) : 0);
+        bytes = o_plan + (degraded ? plan_scratch_bytes(src, n) : 0);
     }
 };
 
@@ -1992,7 +2175,7 @@ int run_transcode(garage_ec_ctx *dst, garage_ec_ctx *src, uint8_t *s_sh, size_t 
                   uint8_t *scratch, cudaStream_t st)
 {
     const size_t s_tot = src ? src->k + src->m : 1, d_tot = dst->k + dst->m;
-    const TranscodeScratch L(n, s_tot, present != nullptr);
+    const TranscodeScratch L(src, n, s_tot, present != nullptr);
     TranscodeParams q;
     memset(&q, 0, sizeof(q));
     q.src = s_sh;
@@ -2010,8 +2193,8 @@ int run_transcode(garage_ec_ctx *dst, garage_ec_ctx *src, uint8_t *s_sh, size_t 
     q.ks = src ? (uint32_t)src->k : 1u;
     q.kd = (uint32_t)dst->k;
     q.src_whole = src ? 0u : 1u;
-    q.src_pb = src && src->pb ? 1u : 0u;
-    q.dst_pb = dst->pb ? 1u : 0u;
+    q.src_quantum = src ? src->quantum : 1u;
+    q.dst_quantum = dst->quantum;
     q.n = (uint32_t)n;
     q.parts = (uint32_t)std::max<size_t>(1, std::min<size_t>(64, ((size_t)dst->sm_count * 4 + n - 1) / n));
     transcode_lens_kernel<<<(unsigned)std::min<size_t>((n + 255) / 256, (size_t)dst->sm_count * 4), 256, 0, st>>>(q);
@@ -2063,7 +2246,7 @@ int transcode_host(garage_ec_ctx *dst, garage_ec_ctx *src, const uint8_t *src_sh
     if (cs > n) cs = n;
     const size_t o_len = 0, o_present = align_up(cs * 4, 16), o_status = o_present + align_up(cs * s_tot, 16);
     const size_t o_sums = o_status + align_up(cs * 4, 16), o_scr = o_sums + (dst_sums ? cs * d_tot * 32 : 0);
-    const TranscodeScratch scr(cs, s_tot, src_present != nullptr);
+    const TranscodeScratch scr(src, cs, s_tot, src_present != nullptr);
     const size_t d_src_b = cs * s_tot * s_stride;
     // copy lists are declared before the lane lease: they outlive its stream work
     CopyBatch up, down;
@@ -2154,7 +2337,7 @@ int garage_ec_transcode(garage_ec_ctx *dst, garage_ec_ctx *src, uint8_t *src_sha
     }
     CU_TRY(dst, cudaSetDevice(dst->device));
     cudaStream_t st = (cudaStream_t)cuda_stream;
-    const TranscodeScratch scr(n_stripes, src ? src->k + src->m : 1, src_present != nullptr);
+    const TranscodeScratch scr(src, n_stripes, src ? src->k + src->m : 1, src_present != nullptr);
     void *scratch = nullptr;
     CU_TRY(dst, dst->pool ? cudaMallocFromPoolAsync(&scratch, scr.bytes, dst->pool, st) : cudaMallocAsync(&scratch, scr.bytes, st));
     rc = run_transcode(dst, src, src_shards, src_stride, src_present, block_len, dst_shards, dst_stride, dst_sums, status,

@@ -120,13 +120,17 @@ GEC_GF_HD inline int pb_group_of(int k, int m, int j)
 }
 // shard length of a block: ceil(block_len / k) rounded up to 128 bytes, so that both halves are 16-byte aligned and
 // each half is exactly 4 of the 8 adler8 segments.  64-bit: with k = 1 a block_len near 2^32 rounds past 32 bits.
-// code_shard_len: the same for every code -- ceil(block_len / k), PB rounded as above (host and device share it).
-GEC_GF_HD inline uint64_t code_shard_len(uint32_t block_len, int k, bool pb)
+// code_shard_len: the same for every code -- ceil(block_len / k) rounded up to the code's quantum: 1 for RS and LRC,
+// 128 for PB, 16 * alpha for Clay (host and device share it).
+constexpr uint32_t kPbQuantum = 128;
+GEC_GF_HD inline uint64_t code_shard_len(uint32_t block_len, int k, uint32_t quantum)
 {
     const uint64_t L = ((uint64_t)block_len + (unsigned)k - 1) / (unsigned)k;
-    return pb ? (L + 127) / 128 * 128 : L;
+    return (L + quantum - 1) / quantum * quantum;
 }
-inline uint64_t pb_shard_len(uint32_t block_len, int k) { return code_shard_len(block_len, k, true); }
+inline uint64_t pb_shard_len(uint32_t block_len, int k) { return code_shard_len(block_len, k, kPbQuantum); }
+
+
 // Generator over half-symbols: row q = 2*shard + half (0..2(k+m)), column c = 2*data + half (0..2k).
 GEC_GF_HD inline uint8_t pb_grow(int k, int m, const uint8_t *P, int q, int c)
 {
@@ -152,6 +156,51 @@ GEC_GF_HD inline int popc64(uint64_t x)
 #else
     return __builtin_popcountll(x);
 #endif
+}
+
+// ---- Clay codes, Clay(k, m) (DESIGN.md section 2.4) ---------------------------------------------------------------
+// q = m, t = ceil((k+m)/q), n' = q*t nodes of which s = n' - k - m are virtual (always zero), alpha = q^t layers per
+// shard.  Node i sits at (x, y) = (i mod q, i div q); data shard j is node j, parity shard j is node k+s+j.  Every
+// layer's uncoupled bytes are a codeword of RS(k+s, m).  Accepted: m in {2, 3, 4}, k >= 2, alpha <= 256.
+constexpr int kClayMaxAlpha = 256, kClayMaxNodes = 16;
+struct ClayGeo {
+    int q, t, n, s, alpha;
+};
+GEC_GF_HD inline bool clay_geometry(int k, int m, ClayGeo *g)
+{
+    if (m < 2 || m > 4 || k < 2 || k > GARAGE_EC_MAX_K_HOST) return false;
+    const int q = m, t = (k + m + q - 1) / q;
+    int alpha = 1;
+    for (int i = 0; i < t; i++) {
+        alpha *= q;
+        if (alpha > kClayMaxAlpha) return false;
+    }
+    *g = ClayGeo{q, t, q * t, q * t - k - m, alpha};
+    return true;
+}
+// node of real shard i and back (-1: a virtual node)
+GEC_GF_HD inline int clay_node(int k, int s, int i) { return i < k ? i : i + s; }
+GEC_GF_HD inline int clay_shard(int k, int s, int a) { return a < k ? a : (a < k + s ? -1 : a - s); }
+// The shards one stripe's decode reads (bit i = shard i), given the present and the wanted absent shards: nothing if
+// no wanted shard is absent; every present shard when exactly one shard is absent and wanted (repair: only the layers
+// of clay_repair_runs); else the first k present shards.  False if fewer than k shards are present (as RS).
+GEC_GF_HD inline bool clay_read_set(int k, int m, uint64_t present, uint64_t want, uint64_t *read)
+{
+    const uint64_t all = (1ull << (k + m)) - 1;
+    present &= all;
+    const uint64_t absent = all & ~present;
+    want &= absent;
+    *read = 0;
+    if (popc64(present) < k) return false;
+    if (!want) return true;
+    if (popc64(absent) == 1) {
+        *read = present;
+        return true;
+    }
+    uint64_t r = 0;
+    for (uint64_t p = present; p && popc64(r) < k; p &= p - 1) r |= p & (~p + 1);
+    *read = r;
+    return true;
 }
 
 // The code a stripe is planned for: RS (l = 0), LRC(k, l, m - l) or PB(k, m) (pb), with parity rows P (m x k).  The

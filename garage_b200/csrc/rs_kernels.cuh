@@ -1816,14 +1816,14 @@ struct SplitParams {
     unsigned long long block_pitch;
     uint32_t stride, k, n;
     uint32_t parts;              // CTAs per block: a dispatcher batch of a dozen blocks still has to fill every SM
-    uint32_t round128;           // PB contexts: shard length ceil(len/k) rounded up to 128 bytes (DESIGN.md 2.2)
+    uint32_t quantum;            // shard length = ceil(len/k) rounded up to this (code_shard_len: PB 128, Clay 16*alpha)
 };
 __global__ void __launch_bounds__(256) split_blocks_kernel(const __grid_constant__ SplitParams q)
 {
     for (uint32_t w = blockIdx.x; w < q.n * q.parts; w += gridDim.x) {
         const uint32_t s = w / q.parts, part = w - s * q.parts;
         const uint32_t len = __ldg(q.block_len + s);
-        const uint32_t L0 = (len + q.k - 1) / q.k, L = q.round128 ? (L0 + 127) & ~127u : L0, nvec = (L + 15) >> 4;
+        const uint32_t L = (uint32_t)code_shard_len(len, (int)q.k, q.quantum), nvec = (L + 15) >> 4;
         const uint8_t *src = q.blocks + (unsigned long long)s * q.block_pitch;
         uint8_t *dst = q.shards + (unsigned long long)s * q.k * q.stride;
         const uint32_t total = q.k * nvec, per = ((total + q.parts - 1) / q.parts + 255u) & ~255u;
@@ -1867,7 +1867,7 @@ struct TranscodeParams {
     uint32_t src_stride, dst_stride;
     uint32_t ks, kd;             // data shards of the source (1: whole blocks) and destination codes
     uint32_t src_whole;          // 1: the source is the block itself, L_s = block_len
-    uint32_t src_pb, dst_pb;     // PB codes: shard lengths rounded up to 128 bytes
+    uint32_t src_quantum, dst_quantum;  // code_shard_len rounding of each code (1 for RS and LRC)
     uint32_t n, parts;           // parts: reframe CTAs per stripe
 };
 // per-stripe lengths and their geometry verdict; runs before the source reconstruct, which needs L_s
@@ -1875,8 +1875,8 @@ __global__ void __launch_bounds__(256) transcode_lens_kernel(const __grid_consta
 {
     for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < q.n; s += gridDim.x * blockDim.x) {
         const uint32_t len = __ldg(q.block_len + s);
-        const uint64_t ls = q.src_whole ? len : code_shard_len(len, (int)q.ks, q.src_pb != 0);
-        const uint64_t ld = code_shard_len(len, (int)q.kd, q.dst_pb != 0);
+        const uint64_t ls = q.src_whole ? len : code_shard_len(len, (int)q.ks, q.src_quantum);
+        const uint64_t ld = code_shard_len(len, (int)q.kd, q.dst_quantum);
         const bool bad = ls > q.src_stride || ld > q.dst_stride;
         q.geo[s] = bad ? GARAGE_EC_E_INVALID : 0;
         q.src_len[s] = bad ? 0u : (uint32_t)ls;  // a reconstruct of an empty stripe touches nothing

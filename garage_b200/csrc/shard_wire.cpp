@@ -140,6 +140,7 @@ bool decode_map(const uint8_t *bytes, size_t len, garage_shard_header *h, bool f
             else if (!strcmp(key, "sum_kind")) h->sum_kind = (uint8_t)v, seen |= 256;
             else if (full && !strcmp(key, "l") && v > 0) h->l = (uint8_t)v, seen |= 512;
             else if (full && !strcmp(key, "pb") && v == 1) h->pb = 1, seen |= 1024;
+            else if (full && !strcmp(key, "clay") && v == 1) h->clay = 1, seen |= 2048;
             else return false;  // unknown field: not this format
             if (v > 0xffffffffull) return false;
         }
@@ -157,9 +158,10 @@ size_t garage_shard_wire_encode(const garage_shard_header *h, uint8_t *out, size
     if (!h || !out || h->k < 1 || h->index >= h->k + h->m || h->header > 1) return 0;
     if (h->l && (h->l >= h->m || h->k % h->l)) return 0;
     if (h->pb > 1 || (h->pb && (h->l || h->m < 2 || h->m > 4 || h->k > 16))) return 0;
+    if (h->clay > 1 || (h->clay && (h->l || h->pb || h->m < 2 || h->m > 4))) return 0;
     Writer w{out, cap};
     w.put(GARAGE_SHARD_WIRE_MARKER, 8);
-    w.byte((uint8_t)(0x89 + (h->l ? 1 : 0) + (h->pb ? 1 : 0)));  // fixmap, 9 fields (+ "l", + "pb"), in declaration order like serde
+    w.byte((uint8_t)(0x89 + (h->l ? 1 : 0) + (h->pb ? 1 : 0) + (h->clay ? 1 : 0)));  // fixmap, 9 fields (+ "l", "pb", "clay"), in declaration order like serde
     w.str("hash");
     w.bin32(h->hash);
     w.str("header");
@@ -186,6 +188,10 @@ size_t garage_shard_wire_encode(const garage_shard_header *h, uint8_t *out, size
         w.str("pb");
         w.uint(1);
     }
+    if (h->clay) {
+        w.str("clay");
+        w.uint(1);
+    }
     return w.ok ? w.n : 0;
 }
 
@@ -210,6 +216,7 @@ int garage_shard_wire_decode(const uint8_t *bytes, size_t len, garage_shard_head
     if (len > 8 && !memcmp(bytes, GARAGE_SHARD_WIRE_MARKER, 8) && decode_map(bytes + 8, len - 8, &h, true)) {
         if (h.k < 1 || h.index >= h.k + h.m || (h.l && (h.l >= h.m || h.k % h.l))) return -1;
         if (h.pb && (h.l || h.m < 2 || h.m > 4 || h.k > 16)) return -1;
+        if (h.clay && (h.l || h.pb || h.m < 2 || h.m > 4)) return -1;
         *out = h;
         return 0;
     }

@@ -107,6 +107,15 @@ typedef struct {
        capacity, or a layout garage_layout_compute finds infeasible.  A file store keeps its layout history in
        <data_dir>/layout; on restart that file wins over this field.                                              */
     const garage_bm_layout_spec *layout;
+    int clay;                       /* 0 (default).  1: Clay(k, m) (garage_ec_create_clay: 2 <= m <= 4, k >= 2,
+                                       alpha <= 256).  Resync of one lost shard hands the rebuild only the
+                                       garage_ec_read_ranges runs of every other shard (1/m of each; holders check
+                                       their whole shard's tag first, a bad one is quarantined and the rebuild falls
+                                       back to k whole shards).  Recorded in the shard file header (pad[1] = 2); a
+                                       shard of another code is quarantined.  GARAGE_EC_E_INVALID with
+                                       local_groups > 0, piggyback, `layout` set or a layout file on disk;
+                                       garage_bm_apply_layout refuses a Clay store.  Conversion to Clay works
+                                       through previous_codes                                                     */
 } garage_bm_config;
 
 typedef struct {
@@ -139,6 +148,9 @@ typedef struct {
     uint64_t layout_deleted;                 /* shards deleted once the newest version no longer assigned them  */
     uint64_t layout_sync_errors;             /* shards a sync could neither copy nor rebuild (or not write)     */
     uint64_t layout_version;                 /* the newest active layout version                                */
+    uint64_t resync_bytes_fetched;           /* bytes resync_block's fetch branch handed to the rebuild: what would
+                                                cross the network in Garage.  Clay: the repair runs (1/m of each
+                                                helper); RS, LRC and PB: resync_bytes_read                          */
 } garage_bm_metrics;
 
 void garage_bm_default_config(garage_bm_config *cfg);

@@ -99,6 +99,16 @@ int garage_ec_create_lrc(garage_ec_ctx **out, int cuda_device, int k, int l, int
  * reconstruct reports GARAGE_EC_E_INVALID in status[]); a HOST call returns GARAGE_EC_E_INVALID before any GPU work.  Needs
  * 1 <= k <= 16, 2 <= m <= 4; GARAGE_EC_E_INVALID otherwise, before any CUDA call.                                  */
 int garage_ec_create_piggyback(garage_ec_ctx **out, int cuda_device, int k, int m, int matrix_kind);
+/* Clay code Clay(k, m) (DESIGN.md section 2.4): MDS, any m losses decode, and one lost shard -- data or parity -- is
+ * rebuilt from 1/m of each of the other k+m-1 shards (Clay(10,4): 0.33 of RS(10,4)'s repair bytes).  q = m,
+ * t = ceil((k+m)/q), alpha = q^t layers per shard, s = q*t - k - m virtual nodes; every layer is coupled from a
+ * codeword of RS(k+s, m) with parity rows of `matrix_kind`.  Every stripe's shard_len must be a multiple of 16*alpha
+ * (garage_ec_code_shard_len gives one); for a stripe where it is not, a DEVICE call behaves as for PB (encode writes
+ * nothing, verify sets every mismatch bit, reconstruct reports GARAGE_EC_E_INVALID in status[]) and a HOST call
+ * returns GARAGE_EC_E_INVALID before any GPU work.  Needs m in {2, 3, 4}, k >= 2, alpha <= 256 (Clay(10,4): 256,
+ * Clay(6,3): 27); GARAGE_EC_E_INVALID otherwise, before any CUDA call.  garage_ec_matrix and garage_ec_read_plan
+ * return GARAGE_EC_E_INVALID on a Clay context; garage_ec_read_ranges names what to fetch.                        */
+int garage_ec_create_clay(garage_ec_ctx **out, int cuda_device, int k, int m, int matrix_kind);
 void garage_ec_destroy(garage_ec_ctx *ctx);
 
 int garage_ec_matrix(const garage_ec_ctx *ctx, uint8_t *out_m_by_k); /* parity rows, row-major */
@@ -115,8 +125,23 @@ int garage_ec_read_set(const garage_ec_ctx *ctx, const uint8_t *present, const u
 /* PB contexts: *groups = m-1 and group_of[j] = i (1..m-1) for data shard j of G_i (k bytes, nullable); RS and LRC
  * contexts: 0 groups, group_of[] all 0.                                                                          */
 int garage_ec_piggyback_info(const garage_ec_ctx *ctx, int *groups, uint8_t *group_of);
+/* Clay contexts: q, t, alpha, the virtual node count s and (nullable) the m x (k+s) base-code parity rows, row-major.
+ * Other contexts: alpha = 1, the rest 0, base_rows untouched.                                                       */
+int garage_ec_clay_info(const garage_ec_ctx *ctx, int *q, int *t, int *alpha, int *virtual_nodes, uint8_t *base_rows);
+/* Byte runs of the shards a gatherer fetches to rebuild the wanted absent shards of ONE stripe (host only):
+ * {shard, offset, len} in shard then offset order, adjacent runs merged.  RS and LRC: whole shards of
+ * garage_ec_read_set; PB: the planned halves; Clay: when exactly one shard is absent and wanted, its repair runs in
+ * every other shard (q^y0 sub-chunks of shard_len/alpha bytes every q^(y0+1)), else the first k present shards
+ * whole.  Presenting only these bytes to reconstruct rebuilds the same output.  *n_ranges = the number of runs;
+ * GARAGE_EC_E_INVALID if it exceeds cap (nothing past cap is written) or shard_len breaks the code's framing
+ * (PB: % 32, Clay: % (16*alpha)); GARAGE_EC_E_UNRECOVERABLE if a wanted shard cannot be rebuilt.                    */
+typedef struct garage_ec_range {
+    uint32_t shard, offset, len;
+} garage_ec_range;
+int garage_ec_read_ranges(const garage_ec_ctx *ctx, const uint8_t *present, const uint8_t *want, uint32_t shard_len,
+                          garage_ec_range *ranges, size_t cap, size_t *n_ranges);
 /* Shard length of a block_len-byte block under this context's code: ceil(block_len / k) for RS and LRC, that
- * rounded up to a multiple of 128 for PB.  The block-level calls frame blocks with it.  GARAGE_EC_E_INVALID if
+ * rounded up to a multiple of 128 for PB, of 16*alpha for Clay.  The block-level calls frame blocks with it.  GARAGE_EC_E_INVALID if
  * that length does not fit in 32 bits (PB(1, m) with block_len > 2^32 - 128).                                   */
 int garage_ec_code_shard_len(const garage_ec_ctx *ctx, uint32_t block_len, uint32_t *shard_len);
 /* Half-shard form of garage_ec_read_set: halves_out[i] bit 0 = read the a-half [0, shard_len/2) of shard i,

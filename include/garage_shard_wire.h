@@ -12,9 +12,10 @@
  *
  *   v1 (erasure coded)  marker "GEC1shdr" + msgpack map
  *        { "hash": bin32, "header": "Plain" | "Compressed", "k": uint, "m": uint, "index": uint,
- *          "block_len": uint, "shard_len": uint, "sum_kind": uint, "sum": bin32[, "l": uint][, "pb": 1] }
- *        "l" (LRC local groups, garage_ec_create_lrc) is present only for an LRC code (l > 0) and "pb" only
- *        for a piggybacked RS code (garage_ec_create_piggyback), so RS messages are byte for byte what they
+ *          "block_len": uint, "shard_len": uint, "sum_kind": uint, "sum": bin32[, "l": uint][, "pb": 1][, "clay": 1] }
+ *        "l" (LRC local groups, garage_ec_create_lrc) is present only for an LRC code (l > 0), "pb" only
+ *        for a piggybacked RS code (garage_ec_create_piggyback) and "clay" only for a Clay code
+ *        (garage_ec_create_clay), so RS messages are byte for byte what they
  *        were before either existed.
  *   v0 (Previous)       the reference's replicated PutBlock payload, no marker:
  *        { "hash": bin32, "header": "Plain" | "Compressed" }
@@ -50,6 +51,7 @@ typedef struct {
     uint8_t sum[32];    /* integrity tag of this shard's bytes                                    */
     uint8_t l;          /* LRC local groups (0 < l < m, k % l == 0); 0 = RS                        */
     uint8_t pb;         /* 1: piggybacked RS PB(k, m) (l = 0, 2 <= m <= 4, k <= 16); 0 = not PB     */
+    uint8_t clay;       /* 1: Clay(k, m) (l = 0, pb = 0, 2 <= m <= 4); 0 = not Clay                 */
 } garage_shard_header;
 
 /* returns the encoded length, or 0 if `cap` is too small / the header is invalid (<= 160 bytes)   */

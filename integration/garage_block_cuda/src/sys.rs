@@ -5,6 +5,7 @@
 use std::os::raw::{c_char, c_int, c_void};
 
 #[repr(C)] pub struct garage_ec_ctx { _private: [u8; 0] }
+#[repr(C)] pub struct garage_ec_range { pub shard: u32, pub offset: u32, pub len: u32 }
 
 pub const GARAGE_EC_OK: c_int = 0;
 pub const GARAGE_EC_E_INVALID: c_int = -1;
@@ -41,6 +42,12 @@ extern "C" {
                             halves_out: *mut u8) -> c_int;
     pub fn garage_ec_check_shard_half_host(kind: c_int, half_bytes: *const u8, shard_len: u32, which: c_int,
                             tag32: *const u8) -> c_int;
+    pub fn garage_ec_create_clay(out: *mut *mut garage_ec_ctx, cuda_device: c_int, k: c_int, m: c_int,
+                            matrix_kind: c_int) -> c_int;
+    pub fn garage_ec_clay_info(ctx: *const garage_ec_ctx, q: *mut c_int, t: *mut c_int, alpha: *mut c_int,
+                            virtual_nodes: *mut c_int, base_rows: *mut u8) -> c_int;
+    pub fn garage_ec_read_ranges(ctx: *const garage_ec_ctx, present: *const u8, want: *const u8, shard_len: u32,
+                            ranges: *mut garage_ec_range, cap: usize, n_ranges: *mut usize) -> c_int;
     pub fn garage_ec_strerror(code: c_int) -> *const c_char;
     pub fn garage_ec_last_error(ctx: *const garage_ec_ctx) -> *const c_char;
     pub fn garage_ec_abi_version() -> c_int;

@@ -7,8 +7,9 @@ of one .so variant on the BASELINE config-2/3 workload.  Not the contract bench 
     python tools/kbench.py --k 10 --lrc 2 --m 4 --erasures 1 --local   # one lost data / local-parity shard
     python tools/kbench.py --k 10 --m 4 --pb [--erasures 1 --local]     # PB(10,4) and RS(10,4), one line each
     python tools/kbench.py --transcode 6,3:10,4 [--rounds 3]  # code conversion; also lrc:10,2,2  pb:10,4  rep
-Reconstruct bytes are (survivors read + shards rebuilt) x shard_len, the survivors being garage_ec_read_set's
-(PB: the halves of garage_ec_read_plan, shard_len / 2 each).
+    python tools/kbench.py --k 10 --m 4 --clay [--rounds 3]   # RS, PB and Clay(10,4), alternating; m losses, then 1
+Reconstruct bytes are the survivor bytes garage_ec_read_ranges names (whole shards, PB halves, Clay repair runs) plus
+the shards rebuilt.
 """
 import argparse
 import json
@@ -29,6 +30,7 @@ ap.add_argument("--same-pattern", action="store_true", help="all stripes lose th
 ap.add_argument("--lrc", type=int, default=0, help="LRC with this many local groups (m = local + global parities)")
 ap.add_argument("--local", action="store_true", help="erase only data / local-parity shards (LRC local repair)")
 ap.add_argument("--pb", action="store_true", help="piggybacked RS PB(k, m), reported next to RS(k, m)")
+ap.add_argument("--clay", action="store_true", help="Clay(k, m) next to RS(k, m) and PB(k, m), alternating rounds")
 ap.add_argument("--transcode", default=None, help="SRC:DST codes: k,m | lrc:k,l,r | pb:k,m | rep (whole blocks)")
 ap.add_argument("--rounds", type=int, default=3, help="--transcode: alternating rounds of the compared paths")
 ap.add_argument("--tag", default="")
@@ -46,12 +48,13 @@ import garage_b200 as G  # noqa: E402
 
 k, m, n = args.k, args.m, args.blocks
 tot = k + m
-e = args.erasures if args.erasures is not None else m
+ERASURES = args.erasures if args.erasures is not None else m
 B = 1 << 20
 
 
-def measure(ec):
-    """encode / reconstruct / verify of one context on the workload: (times, shard_len, present, ok, shards)"""
+def measure(ec, e):
+    """encode / reconstruct / verify of one context on the workload, e erasures per stripe: (times, shard_len,
+    present, ok, shards)"""
     L = ec.code_shard_len(B)
     stride = ec.stride_for(L) + args.stride_pad
     shards = torch.zeros(n * tot * stride, dtype=torch.uint8, device="cuda")
@@ -126,15 +129,15 @@ def power_limit():
         return None
 
 
-def report(ec, code):
-    (t_enc, t_dec, t_ver), L, pres_np, ok, orig = measure(ec)
+def report(ec, code, e=ERASURES):
+    (t_enc, t_dec, t_ver), L, pres_np, ok, orig = measure(ec, e)
     peak = copy_gbs(orig)
     del orig
     enc_b = n * (k + m) * L
     nsurv = 0  # shards' worth of survivor bytes read
     for s in range(n):
-        hv = ec.read_plan(pres_np[s])
-        nsurv += sum(bin(int(x)).count("1") for x in hv) / 2 if hv is not None else 0
+        runs = ec.read_ranges(pres_np[s], L)
+        nsurv += sum(r[2] for r in runs) / L if runs is not None else 0
     dec_b = int((nsurv + n * e) * L)
     print(json.dumps({
         "tag": args.tag or (args.so or "default"), "code": code, "k": k, "m": m, "lrc_local_groups": args.lrc,
@@ -228,6 +231,15 @@ def transcode_bench():
 
 if args.transcode:
     transcode_bench()
+elif args.clay:  # Clay(k, m) next to RS(k, m) and PB(k, m): m losses, then one, in alternating rounds
+    for rnd in range(args.rounds):
+        for erasures in (m, 1):
+            for code, make in (("RS(%d,%d)" % (k, m), lambda: G.GarageEc(0, k, m)),
+                               ("PB(%d,%d)" % (k, m), lambda: G.GarageEc.piggyback(0, k, m)),
+                               ("Clay(%d,%d)" % (k, m), lambda: G.GarageEc.clay(0, k, m))):
+                with make() as ctx:
+                    report(ctx, code, erasures)
+                    torch.cuda.empty_cache()
 elif args.pb:  # PB(k, m) next to RS(k, m) on the same workload, one line each
     for code, make in (("RS(%d,%d)" % (k, m), lambda: G.GarageEc(0, k, m)),
                        ("PB(%d,%d)" % (k, m), lambda: G.GarageEc.piggyback(0, k, m))):
