@@ -40,6 +40,7 @@ ABI_SYMBOLS = [
     "garage_ec_create_piggyback", "garage_ec_piggyback_info", "garage_ec_code_shard_len", "garage_ec_read_plan",
     "garage_ec_check_shard_half_host", "garage_ec_transcode",
     "garage_ec_create_clay", "garage_ec_clay_info", "garage_ec_read_ranges",
+    "garage_ec_deep_check",
 ]
 
 
@@ -128,6 +129,7 @@ def load_library(build=True):
     L.garage_ec_create_clay.argtypes = [C.POINTER(vp), i32, i32, i32, i32]
     L.garage_ec_clay_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), vp]
     L.garage_ec_read_ranges.argtypes = [vp, vp, vp, u32, vp, sz, C.POINTER(sz)]
+    L.garage_ec_deep_check.argtypes = [vp, vp, vp, vp, vp, vp, sz, sz, i32, vp]
     _lib = L
     return L
 
@@ -376,6 +378,13 @@ class GarageEc:
         kind, st = self._stream(shards)
         return self._check(self._L.garage_ec_verify(self._h, _ptr(shards), _ptr(mismatch), _ptr(shard_len),
                                                     stride, n, kind, st))
+
+    def deep_check(self, shards, block_len, hashes, hash_bad, mismatch, stride, n):
+        """garage_ec_deep_check: hash_bad[s] = the block read from the data shards does not hash to hashes[s];
+        mismatch[s] = garage_ec_verify's parity bits with the code's shard length"""
+        kind, st = self._stream(shards)
+        return self._check(self._L.garage_ec_deep_check(self._h, _ptr(shards), _ptr(block_len), _ptr(hashes),
+                                                        _ptr(hash_bad), _ptr(mismatch), stride, n, kind, st))
 
     # -- per-shard integrity (blake2sum of every shard)
     def shard_sums(self, shards, sums_out, stride, n, per_stripe, shard_len=None):

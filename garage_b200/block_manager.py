@@ -19,7 +19,7 @@ SYMBOLS = [
     "garage_bm_block_incref", "garage_bm_block_decref", "garage_bm_get_block_rc", "garage_bm_scrub_step",
     "garage_bm_bench", "garage_bm_corrupt_shard_header", "garage_bm_plant_stale_shard", "garage_bm_set_node_readonly",
     "garage_bm_convert_step", "garage_bm_debug_convert_stop_after", "garage_bm_apply_layout", "garage_bm_layout_sync_step",
-    "garage_bm_layout_versions",
+    "garage_bm_layout_versions", "garage_bm_deep_scrub_step",
 ]
 SUM_BLAKE2, SUM_ADLER8 = 0, 1
 
@@ -60,7 +60,8 @@ class Metrics(C.Structure):
         "encode_call_us", "reconstruct_call_us", "corrupt_data_errors", "write_errors", "resync_shards_read", "resync_bytes_read",
         "convert_blocks", "convert_bytes_read", "convert_bytes_written", "convert_errors", "convert_call_us", "legacy_gets",
         "legacy_deleted", "layout_shards_copied", "layout_shards_rebuilt", "layout_bytes_read", "layout_bytes_written",
-        "layout_deleted", "layout_sync_errors", "layout_version", "resync_bytes_fetched")]
+        "layout_deleted", "layout_sync_errors", "layout_version", "resync_bytes_fetched", "deep_scrub_blocks",
+        "deep_scrub_skipped", "deep_scrub_parity_bad", "deep_scrub_content_errors", "deep_check_call_us")]
 
 
 _lib = None
@@ -106,6 +107,8 @@ def load_library():
         L.garage_bm_apply_layout.argtypes = [vp, C.POINTER(LayoutSpec), C.POINTER(C.c_uint64)]
         L.garage_bm_layout_sync_step.argtypes = [vp, i32, vp, sz, vp, C.POINTER(i32), C.POINTER(C.c_uint64)]
         L.garage_bm_layout_versions.argtypes = [vp, C.POINTER(C.c_uint64), i32]
+        L.garage_bm_deep_scrub_step.argtypes = [vp, i32, vp, sz, vp, C.POINTER(i32), C.POINTER(C.c_uint64),
+                                                C.POINTER(C.c_uint64)]
         _lib = L
     return _lib
 
@@ -228,6 +231,14 @@ class BlockManager:
         fin, a, b = C.c_int(0), C.c_uint64(0), C.c_uint64(0)
         rc = self._L.garage_bm_scrub_step(self._h, node, C.c_char_p(bytes(cursor)) if cursor else None, max_shards,
                                           C.cast(out, C.c_void_p), C.byref(fin), C.byref(a), C.byref(b))
+        return rc, out.raw, bool(fin.value), a.value, b.value
+
+    def deep_scrub_step(self, node, cursor=None, max_blocks=0):
+        """-> (rc, cursor_out bytes, finished, blocks checked, shards quarantined)"""
+        out = C.create_string_buffer(32)
+        fin, a, b = C.c_int(0), C.c_uint64(0), C.c_uint64(0)
+        rc = self._L.garage_bm_deep_scrub_step(self._h, node, C.c_char_p(bytes(cursor)) if cursor else None, max_blocks,
+                                               C.cast(out, C.c_void_p), C.byref(fin), C.byref(a), C.byref(b))
         return rc, out.raw, bool(fin.value), a.value, b.value
 
     def convert_step(self, node, cursor=None, max_blocks=0):

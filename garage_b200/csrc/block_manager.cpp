@@ -940,6 +940,9 @@ struct garage_bm {
     int enc_next[kWorkers] = {0};
     PinnedBuf scrub_buf;
     std::mutex scrub_mu;
+    PinnedBuf deep_buf;  // the deep scrub's batch of stripes (not stripe_slots: DESIGN.md section 5.2's pool rule)
+    std::mutex deep_mu;
+    std::atomic<uint64_t> deep_blocks{0}, deep_skipped{0}, deep_parity_bad{0}, deep_content_errors{0}, deep_check_us{0};
     std::atomic<bool> warmed{false};
     // metrics (src/block/metrics.rs)
     std::atomic<uint64_t> bytes_written{0}, bytes_read{0}, corruption_counter{0}, resync_counter{0},
@@ -2403,6 +2406,132 @@ struct garage_bm {
         for (auto &t : th) t.join();
     }
 
+    // the node that deep-scrubs h: the first up node of its row in the newest layout version, -1 if none is up
+    int deep_scrub_owner(const Hash &h)
+    {
+        int who[64];
+        storage_nodes_of(h, who);
+        for (int i = 0; i < tot; i++) {
+            Node &nd = *nodes[who[i]];
+            std::lock_guard<std::mutex> lk(nd.mu);
+            if (nd.up) return who[i];
+        }
+        return -1;
+    }
+
+    // garage_bm_deep_scrub_step: see include/garage_block_manager.h and DESIGN.md section 5.4
+    int deep_scrub_step(int node, const Hash *cursor, size_t max_blocks, Hash *cursor_out, int *finished,
+                        uint64_t *checked, uint64_t *repaired)
+    {
+        {
+            Node &nd = *nodes[node];
+            std::lock_guard<std::mutex> lk(nd.mu);
+            if (!nd.up) return GARAGE_BM_E_MESSAGE;
+        }
+        std::vector<Hash> hs;
+        {
+            std::lock_guard<std::mutex> lk(refs_mu);
+            for (auto &kv : refs) {
+                auto it = rc.find(kv.first);
+                if (it == rc.end() || it->second.count > 0) hs.push_back(kv.first);
+            }
+        }
+        std::sort(hs.begin(), hs.end());
+        if (cursor) hs.erase(hs.begin(), std::upper_bound(hs.begin(), hs.end(), *cursor));
+        std::vector<Hash> mine;
+        bool done = true;
+        for (const Hash &h : hs) {
+            if (deep_scrub_owner(h) != node) continue;
+            if (max_blocks && mine.size() == max_blocks) {
+                done = false;
+                break;
+            }
+            mine.push_back(h);
+        }
+        if (finished) *finished = done ? 1 : 0;
+        if (cursor_out) {
+            if (!mine.empty()) *cursor_out = mine.back();
+            else if (cursor) *cursor_out = *cursor;
+            else cursor_out->fill(0);
+        }
+        uint64_t nchecked = 0, nrep = 0;
+        std::lock_guard<std::mutex> dl(deep_mu);
+        const size_t bmax = std::max<uint32_t>(cfg.batch_max_blocks, 1), sbytes = (size_t)tot * slot_stride;
+        uint8_t *buf = mine.empty() ? nullptr : deep_buf.get(bmax * (sbytes + 32));
+        if (!mine.empty() && !buf) return GARAGE_EC_E_NOMEM;
+        const bool multi = multi_version();
+        std::vector<uint8_t> blk;
+        for (size_t b0 = 0; b0 < mine.size(); b0 += bmax) {
+            const size_t nb = std::min(bmax, mine.size() - b0);
+            uint8_t *const hashes = buf + bmax * sbytes;
+            std::vector<Hash> hv;  // the complete stripes, at buf + i * sbytes
+            std::vector<uint32_t> lens;
+            std::vector<int> from;  // the node each of their shards came from
+            for (size_t b = b0; b < b0 + nb; b++) {
+                const Hash &h = mine[b];
+                uint8_t *sp = buf + hv.size() * sbytes;
+                uint8_t have[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
+                int src[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M], who[64];
+                uint32_t block_len = 0;
+                // tags are checked on read; a bad shard is quarantined (and queued) there
+                const int got = gather_into(h, -1, sp, have, block_len, /*all=*/true, /*for_gpu=*/true, nullptr, nullptr,
+                                            nullptr, 0, src);
+                if (got == 0) continue;  // no configured shard: held under a previous code or as replicas
+                storage_nodes_of(h, who);
+                bool whole = got == tot;
+                for (int i = 0; i < tot; i++) {
+                    // during a layout change only the newest version's stripe counts: a shard read from an older
+                    // holder is missing from it
+                    if (have[i] && (!multi || src[i] == who[i])) continue;
+                    whole = false;
+                    put_to_resync(who[i], h);
+                }
+                if (!whole) {
+                    deep_skipped++;
+                    continue;
+                }
+                memcpy(hashes + hv.size() * 32, h.data(), 32);
+                hv.push_back(h);
+                lens.push_back(block_len);
+                from.insert(from.end(), src, src + tot);
+            }
+            const size_t nc = hv.size();
+            if (!nc) continue;
+            std::vector<uint8_t> hash_bad(nc);
+            std::vector<uint32_t> mm(nc);
+            const auto t0 = Clock::now();
+            const int rc_ = garage_ec_deep_check(ec, buf, lens.data(), hashes, hash_bad.data(), mm.data(), slot_stride, nc,
+                                                 GARAGE_EC_MEM_HOST, nullptr);
+            deep_check_us += (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count();
+            if (rc_ != GARAGE_EC_OK) return rc_;
+            nchecked += nc;
+            deep_blocks += nc;
+            for (size_t s = 0; s < nc; s++) {
+                const Hash &h = hv[s];
+                if (!hash_bad[s]) {
+                    // the data is right, so every flagged parity is stale: all of them go out before any rebuild (a
+                    // Clay repair of one parity reads the others)
+                    for (int i = 0; i < m; i++) {
+                        if (!((mm[s] >> i) & 1)) continue;
+                        quarantine(from[s * tot + k + i], h, 0, multi ? k + i : -1);
+                        deep_parity_bad++;
+                        nrep++;
+                    }
+                    continue;
+                }
+                // the block is wrong: the GET path's hunt finds and quarantines the stale shard, if one set of k is
+                // consistent (the stripe's region of the batch buffer is free by now)
+                blk.resize(std::max<size_t>(cfg.block_size, lens[s]));
+                size_t out_len = 0;
+                if (hunt_stale_shard(h, buf + s * sbytes, blk.data(), blk.size(), &out_len, 0) == GARAGE_BM_OK) nrep++;
+                else deep_content_errors++;
+            }
+        }
+        if (checked) *checked = nchecked;
+        if (repaired) *repaired = nrep;
+        return GARAGE_BM_OK;
+    }
+
     // garage_bm_convert_step: see include/garage_block_manager.h
     int convert_step(int node, const Hash *cursor, size_t max_blocks, Hash *cursor_out, int *finished, uint64_t *converted)
     {
@@ -3001,6 +3130,7 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
     }
     bm->ram.reset(new ByteSemaphore(cfg->block_ram_buffer_max ? cfg->block_ram_buffer_max : (256ull << 20)));
     bm->scrub_buf.ctx = bm->ec;
+    bm->deep_buf.ctx = bm->ec;
     auto destroy_on_error = [&](int code) {
         garage_bm_destroy(bm.release());
         return code;
@@ -3087,6 +3217,7 @@ void garage_bm_destroy(garage_bm *bm)
         ctxs[2 * w + 1] = bm->rec_ctx[w];
     }
     bm->scrub_buf.release();
+    bm->deep_buf.release();
     bm->conv_src.release();
     bm->conv_dst.release();
     bm->conv_blk.release();
@@ -3166,6 +3297,23 @@ int garage_bm_scrub_step(garage_bm *bm, int node, const uint8_t *cursor32, size_
         Hash cur, out;
         if (cursor32) cur = to_hash(cursor32);
         int rc = bm->scrub(node, checked, corrupt, cursor32 ? &cur : nullptr, max_shards, &out, finished);
+        if (rc == GARAGE_BM_OK && cursor_out32) memcpy(cursor_out32, out.data(), 32);
+        return rc;
+    } catch (const std::bad_alloc &) {
+        return GARAGE_EC_E_NOMEM;
+    } catch (...) {
+        return GARAGE_BM_E_MESSAGE;
+    }
+}
+
+int garage_bm_deep_scrub_step(garage_bm *bm, int node, const uint8_t *cursor32, size_t max_blocks,
+                              uint8_t cursor_out32[32], int *finished, uint64_t *checked, uint64_t *repaired)
+{
+    if (!bm || node < 0 || node >= (int)bm->nodes.size()) return GARAGE_EC_E_INVALID;
+    try {
+        Hash cur, out;
+        if (cursor32) cur = to_hash(cursor32);
+        int rc = bm->deep_scrub_step(node, cursor32 ? &cur : nullptr, max_blocks, &out, finished, checked, repaired);
         if (rc == GARAGE_BM_OK && cursor_out32) memcpy(cursor_out32, out.data(), 32);
         return rc;
     } catch (const std::bad_alloc &) {
@@ -3414,6 +3562,11 @@ void garage_bm_get_metrics(garage_bm *bm, garage_bm_metrics *o)
         ql += n->resync_queue.size();
     }
     o->resync_queue_length = ql;
+    o->deep_scrub_blocks = bm->deep_blocks;
+    o->deep_scrub_skipped = bm->deep_skipped;
+    o->deep_scrub_parity_bad = bm->deep_parity_bad;
+    o->deep_scrub_content_errors = bm->deep_content_errors;
+    o->deep_check_call_us = bm->deep_check_us;
 }
 
 }  // extern "C"

@@ -1336,6 +1336,110 @@ int garage_ec_verify(garage_ec_ctx *ctx, const uint8_t *shards, uint32_t *mismat
                        shard_len, stride, n_stripes, st);
 }
 
+// --------------------------------------------------------------------------- DEEP CHECK
+// The block hash of every stripe (blake2sum_blocks_kernel, which also leaves L in shard_len and initialises mismatch),
+// then the code's own verify launch with those lengths.  shard_len: n uint32 of device scratch.
+static int run_deep_check(garage_ec_ctx *ctx, const uint8_t *shards, const uint32_t *block_len, const uint8_t *hashes,
+                          uint8_t *hash_bad, uint32_t *mismatch, uint32_t *shard_len, size_t stride, size_t n,
+                          cudaStream_t st)
+{
+    BlockSumParams q;
+    memset(&q, 0, sizeof(q));
+    q.shards = shards;
+    q.block_len = block_len;
+    q.hashes = hashes;
+    q.hash_bad = hash_bad;
+    q.shard_len = shard_len;
+    q.mismatch = mismatch;
+    q.stride = (uint32_t)stride;
+    q.k = (uint32_t)ctx->k;
+    q.m = (uint32_t)ctx->m;
+    q.n = (uint32_t)n;
+    q.quantum = ctx->quantum;
+    blake2sum_blocks_kernel<<<(unsigned)((n + kQuadThreads / 4 - 1) / (kQuadThreads / 4)), kQuadThreads, 0, st>>>(q);
+    ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return set_cuda_error(ctx, e, "blake2sum_blocks_kernel launch");
+    return run_uniform(ctx, kModeVerify, shards, (size_t)(ctx->k + ctx->m) * stride, nullptr, 0, mismatch, shard_len,
+                       stride, n, st);
+}
+
+// HOST: chunks of whole stripes through the lanes; only roundup16(L) bytes of each shard go up
+static int deep_check_host(garage_ec_ctx *ctx, const uint8_t *shards, const uint32_t *block_len, const uint8_t *hashes,
+                           uint8_t *hash_bad, uint32_t *mismatch, size_t stride, size_t n)
+{
+    CopyBatch up;  // declared before the lane lease: it must outlive the stream work the lease waits for
+    LEASE_LANES(ctx, lanes);
+    const size_t tot = ctx->k + ctx->m;
+    size_t cs = kHostChunkBytes / (tot * stride);
+    if (cs < 1) cs = 1;
+    if (cs > n) cs = n;
+    // small buffer layout per lane: block_len | hashes | shard_len | mismatch | hash_bad
+    const size_t o_blen = 0, o_hash = align_up(cs * 4, 16), o_sl = o_hash + cs * 32, o_mm = o_sl + align_up(cs * 4, 16);
+    const size_t o_bad = o_mm + align_up(cs * 4, 16), small = o_bad + align_up(cs, 16);
+    for (HostLane &L : lanes.set->lanes) {
+        int rc = lane_reserve(ctx, L, cs * tot * stride, small);
+        if (rc) return rc;
+    }
+    size_t c = 0;
+    for (size_t s0 = 0; s0 < n; s0 += cs, c++) {
+        HostLane &L = lanes[c % kHostLanes];
+        const size_t cnt = n - s0 < cs ? n - s0 : cs;
+        for (size_t s = s0; s < s0 + cnt; s++) {
+            const size_t bytes = align_up(code_shard_len(ctx, block_len[s]), 16);
+            for (size_t i = 0; i < tot; i++)
+                up.add(L.d_buf + ((s - s0) * tot + i) * stride, shards + (s * tot + i) * stride, bytes);
+        }
+        int rc = up.flush(ctx, cudaMemcpyHostToDevice, L.stream);
+        if (rc) return rc;
+        CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_blen, block_len + s0, cnt * 4, cudaMemcpyHostToDevice, L.stream));
+        CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_hash, hashes + s0 * 32, cnt * 32, cudaMemcpyHostToDevice, L.stream));
+        uint32_t *d_mm = reinterpret_cast<uint32_t *>(L.d_small + o_mm);
+        rc = run_deep_check(ctx, L.d_buf, reinterpret_cast<const uint32_t *>(L.d_small + o_blen), L.d_small + o_hash,
+                            L.d_small + o_bad, d_mm, reinterpret_cast<uint32_t *>(L.d_small + o_sl), stride, cnt,
+                            L.stream);
+        if (rc) return rc;
+        CU_TRY(ctx, cudaMemcpyAsync(hash_bad + s0, L.d_small + o_bad, cnt, cudaMemcpyDeviceToHost, L.stream));
+        CU_TRY(ctx, cudaMemcpyAsync(mismatch + s0, d_mm, cnt * 4, cudaMemcpyDeviceToHost, L.stream));
+    }
+    for (HostLane &L : lanes.set->lanes) CU_TRY(ctx, lane_wait(ctx, L));
+    return GARAGE_EC_OK;
+}
+
+int garage_ec_deep_check(garage_ec_ctx *ctx, const uint8_t *shards, const uint32_t *block_len, const uint8_t *hashes,
+                         uint8_t *hash_bad, uint32_t *mismatch, size_t stride, size_t n_stripes, int mem_kind,
+                         void *cuda_stream)
+{
+    if (!ctx || (mem_kind != GARAGE_EC_MEM_HOST && mem_kind != GARAGE_EC_MEM_DEVICE)) return GARAGE_EC_E_INVALID;
+    int rc = check_geometry(ctx, stride, n_stripes, ctx->k + ctx->m);
+    if (rc) return rc;
+    if (n_stripes == 0) return GARAGE_EC_OK;
+    if (!shards || !block_len || !hashes || !hash_bad || !mismatch) return GARAGE_EC_E_INVALID;
+    if (!aligned16(shards)) return GARAGE_EC_E_ALIGN;
+    if (mem_kind == GARAGE_EC_MEM_HOST) {
+        // code_shard_len is a multiple of the code's framing unit, so a length that fits its stride is well framed
+        for (size_t s = 0; s < n_stripes; s++)
+            if (code_shard_len(ctx, block_len[s]) > stride) return GARAGE_EC_E_INVALID;
+        CU_TRY(ctx, cudaSetDevice(ctx->device));
+        return deep_check_host(ctx, shards, block_len, hashes, hash_bad, mismatch, stride, n_stripes);
+    }
+    // the kernel reads the hashes as 8-byte words and the lengths / writes the mismatch words as 4-byte words
+    if ((reinterpret_cast<uintptr_t>(hashes) & 7) || (reinterpret_cast<uintptr_t>(block_len) & 3) ||
+        (reinterpret_cast<uintptr_t>(mismatch) & 3))
+        return GARAGE_EC_E_ALIGN;
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    void *scratch = nullptr;
+    CU_TRY(ctx, ctx->pool ? cudaMallocFromPoolAsync(&scratch, n_stripes * 4, ctx->pool, st)
+                          : cudaMallocAsync(&scratch, n_stripes * 4, st));
+    rc = run_deep_check(ctx, shards, block_len, hashes, hash_bad, mismatch, reinterpret_cast<uint32_t *>(scratch),
+                        stride, n_stripes, st);
+    cudaError_t e = cudaFreeAsync(scratch, st);
+    if (rc) return rc;
+    if (e != cudaSuccess) return set_cuda_error(ctx, e, "cudaFreeAsync");
+    return GARAGE_EC_OK;
+}
+
 // --------------------------------------------------------------------------- RECONSTRUCT
 // `stripes` != NULL: stripe s lives at stripes[s] (its k+m shards `stride` apart) instead of
 // shards + s*(k+m)*stride -- the gather form used by batching front-ends whose callers each own

@@ -1718,20 +1718,15 @@ __device__ __forceinline__ uint64_t lds_u64(uint32_t addr)
 
 constexpr int kQuadThreads = 128;  // 32 shards per block
 
-__global__ void __launch_bounds__(kQuadThreads) blake2sum_shards_quad_kernel(const __grid_constant__ SumParams q)
+// BLAKE2b-512 of a len-byte message by one quad; lane c = threadIdx.x & 3 returns h[c], bytes 8c..8c+7 of the digest.
+// load32(o, x, y) gives this lane's 32 message bytes at o + 32c, zero beyond len; it is called for o = 0, 128, ...
+// in order, one block ahead of the compression.  s_row: the quad's 128-byte message row in shared memory.
+template <class Load32>
+__device__ __forceinline__ uint64_t blake2b_quad(uint32_t len, uint8_t *s_row, Load32 load32)
 {
-    // 144-byte pitch: consecutive quads start 4 banks apart (a 128-byte pitch puts the same word
-    // of all 8 quads of a warp in the same bank: 8-way conflicts on every message load)
-    __shared__ __align__(16) uint8_t s_msg[kQuadThreads / 4][144];
-    const uint32_t tid = threadIdx.x, lane = tid & 31, c = tid & 3;
-    const uint32_t i = blockIdx.x * (kQuadThreads / 4) + (tid >> 2);  // shard index
-    if (i >= q.n_shards) return;                                      // whole quads leave together
+    const uint32_t lane = threadIdx.x & 31, c = threadIdx.x & 3;
     const uint32_t qmask = 0xFu << (lane & ~3u), qbase = lane & ~3u;
-    const uint8_t *p;
-    uint32_t len;
-    size_t oi;
-    locate_shard(q, i, p, len, oi);
-    const uint32_t msg = (uint32_t)__cvta_generic_to_shared(&s_msg[tid >> 2][0]);
+    const uint32_t msg = (uint32_t)__cvta_generic_to_shared(s_row);
 
     // per-round message offsets for this lane: {col x, col y, diag x, diag y} * 8 bytes
     uint32_t off[12];
@@ -1745,28 +1740,14 @@ __global__ void __launch_bounds__(kQuadThreads) blake2sum_shards_quad_kernel(con
     const uint64_t ivhi = c == 0 ? IV[4] : (c == 1 ? IV[5] : (c == 2 ? IV[6] : IV[7]));
     uint64_t h0 = ivlo ^ (c == 0 ? 0x01010040ull : 0ull), h1 = ivhi;  // h[c], h[4+c]
 
-    // this lane's 32 bytes of the block starting at byte `o` (zero beyond len)
-    auto load32 = [&](uint32_t o, uint4 &x, uint4 &y) {
-        x = make_uint4(0, 0, 0, 0);
-        y = make_uint4(0, 0, 0, 0);
-        const uint32_t a0 = o + 32 * c;
-        if (a0 < len) {
-            x = *reinterpret_cast<const uint4 *>(p + a0);
-            if (len - a0 < 16) x = mask_tail(x, len - a0);
-        }
-        if (a0 + 16 < len) {
-            y = *reinterpret_cast<const uint4 *>(p + a0 + 16);
-            if (len - a0 - 16 < 16) y = mask_tail(y, len - a0 - 16);
-        }
-    };
     uint4 nx, ny;
     load32(0, nx, ny);
     uint32_t o = 0;
     for (;;) {
-        const bool last = len - o <= 128;  // also true for an empty shard
+        const bool last = len - o <= 128;  // also true for an empty message
         __syncwarp(qmask);                  // previous block's words are no longer needed
-        *reinterpret_cast<uint4 *>(&s_msg[tid >> 2][32 * c]) = nx;
-        *reinterpret_cast<uint4 *>(&s_msg[tid >> 2][32 * c + 16]) = ny;
+        *reinterpret_cast<uint4 *>(s_row + 32 * c) = nx;
+        *reinterpret_cast<uint4 *>(s_row + 32 * c + 16) = ny;
         __syncwarp(qmask);
         if (!last) load32(o + 128, nx, ny);  // prefetch the next block
         const uint64_t t = last ? (uint64_t)len : (uint64_t)o + 128;
@@ -1793,12 +1774,140 @@ __global__ void __launch_bounds__(kQuadThreads) blake2sum_shards_quad_kernel(con
         if (last) break;
         o += 128;
     }
+    return h0;
+}
+
+__global__ void __launch_bounds__(kQuadThreads) blake2sum_shards_quad_kernel(const __grid_constant__ SumParams q)
+{
+    // 144-byte pitch: consecutive quads start 4 banks apart (a 128-byte pitch puts the same word
+    // of all 8 quads of a warp in the same bank: 8-way conflicts on every message load)
+    __shared__ __align__(16) uint8_t s_msg[kQuadThreads / 4][144];
+    const uint32_t tid = threadIdx.x, lane = tid & 31, c = tid & 3;
+    const uint32_t i = blockIdx.x * (kQuadThreads / 4) + (tid >> 2);  // shard index
+    if (i >= q.n_shards) return;                                      // whole quads leave together
+    const uint32_t qmask = 0xFu << (lane & ~3u);
+    const uint8_t *p;
+    uint32_t len;
+    size_t oi;
+    locate_shard(q, i, p, len, oi);
+
+    // this lane's 32 bytes of the shard starting at byte `o` (zero beyond len)
+    auto load32 = [&](uint32_t o, uint4 &x, uint4 &y) {
+        x = make_uint4(0, 0, 0, 0);
+        y = make_uint4(0, 0, 0, 0);
+        const uint32_t a0 = o + 32 * c;
+        if (a0 < len) {
+            x = *reinterpret_cast<const uint4 *>(p + a0);
+            if (len - a0 < 16) x = mask_tail(x, len - a0);
+        }
+        if (a0 + 16 < len) {
+            y = *reinterpret_cast<const uint4 *>(p + a0 + 16);
+            if (len - a0 - 16 < 16) y = mask_tail(y, len - a0 - 16);
+        }
+    };
+    const uint64_t h0 = blake2b_quad(len, &s_msg[tid >> 2][0], load32);
     if (q.sums) *reinterpret_cast<unsigned long long *>(q.sums + oi * 32 + 8 * c) = h0;
     if (q.expect && q.bad) {
         const unsigned long long e = *reinterpret_cast<const unsigned long long *>(q.expect + oi * 32 + 8 * c);
         const uint32_t diff = __ballot_sync(qmask, e != h0) & qmask;
         if (c == 0) q.bad[oi] = diff ? 1 : 0;
     }
+}
+
+// ---- blake2sum of whole blocks, read from their data shards (deep scrub, DESIGN.md 4.7) -------------------------
+// The block is the first block_len bytes of data shards 0..k-1 concatenated (DESIGN.md 2.3): block byte o is byte
+// o % L of shard o / L, L = code_shard_len.  One quad per stripe, as in blake2sum_shards_quad_kernel.  Bytes of a
+// shard at [L, stride) are not part of the block and never enter the hash.
+struct BlockSumParams {
+    const uint8_t *shards;        // stripe s at shards + s*(k+m)*stride, shard i at + i*stride
+    const uint32_t *block_len;    // per stripe
+    const uint8_t *hashes;        // 32 bytes per stripe: the content address
+    uint8_t *hash_bad;            // out: 1 iff the block's blake2sum differs from hashes[s]
+    uint32_t *shard_len;          // out: L, or 0 for a stripe whose L does not fit its stride
+    uint32_t *mismatch;           // out: 0, or every parity bit for such a stripe (the verify launch ORs into it)
+    uint32_t stride, k, m, n, quantum;
+};
+
+// 16 block bytes at offset `off` of data shard `j`, `nvalid` of them valid (zero past that).  Inside one shard at a
+// 16-byte aligned offset: one vector load; inside one shard elsewhere: five aligned 32-bit loads and funnel shifts
+// (as in split_blocks_kernel; the words stay inside roundup4(off + 16) <= roundup16(L)); only the one vector that
+// crosses into the next shard -- or several shards when L < 16 -- is gathered byte by byte.
+__device__ __forceinline__ uint4 block_vec16(const uint8_t *stripe, uint32_t stride, uint32_t L, uint32_t j,
+                                             uint32_t off, uint32_t nvalid)
+{
+    if (!nvalid) return make_uint4(0, 0, 0, 0);
+    const uint8_t *p = stripe + (size_t)j * stride;
+    uint4 v;
+    if (off + 16 <= L) {
+        if (!(off & 15)) {
+            v = __ldg(reinterpret_cast<const uint4 *>(p + off));
+        } else {
+            const uint32_t sh = (off & 3u) * 8;
+            const uint32_t *wp = reinterpret_cast<const uint32_t *>(p + (off & ~3u));
+            const uint32_t w0 = __ldg(wp), w1 = __ldg(wp + 1), w2 = __ldg(wp + 2), w3 = __ldg(wp + 3),
+                           w4 = sh ? __ldg(wp + 4) : 0;
+            v = make_uint4(__funnelshift_r(w0, w1, sh), __funnelshift_r(w1, w2, sh), __funnelshift_r(w2, w3, sh),
+                           __funnelshift_r(w3, w4, sh));
+        }
+        return nvalid < 16 ? mask_tail(v, nvalid) : v;
+    }
+    uint32_t wv[4] = {0, 0, 0, 0};
+#pragma unroll
+    for (int b = 0; b < 16; b++) {
+        if ((uint32_t)b < nvalid) {
+            uint32_t ob = off + b, jb = j;
+            if (ob >= L) {  // crossed into the next shard(s)
+                jb += ob / L;
+                ob %= L;
+            }
+            wv[b >> 2] |= (uint32_t)stripe[(size_t)jb * stride + ob] << (8 * (b & 3));
+        }
+    }
+    return make_uint4(wv[0], wv[1], wv[2], wv[3]);
+}
+
+__global__ void __launch_bounds__(kQuadThreads) blake2sum_blocks_kernel(const __grid_constant__ BlockSumParams q)
+{
+    __shared__ __align__(16) uint8_t s_msg[kQuadThreads / 4][144];  // 144-byte pitch: see the shard kernel
+    const uint32_t tid = threadIdx.x, lane = tid & 31, c = tid & 3;
+    const uint32_t s = blockIdx.x * (kQuadThreads / 4) + (tid >> 2);  // stripe index
+    if (s >= q.n) return;                                             // whole quads leave together
+    const uint32_t qmask = 0xFu << (lane & ~3u);
+    const uint32_t len = __ldg(q.block_len + s);
+    const uint64_t L64 = code_shard_len(len, (int)q.k, q.quantum);
+    const bool bad_geo = L64 > q.stride;  // DEVICE mode reports it; nothing of the stripe is read
+    const uint32_t L = bad_geo ? 0u : (uint32_t)L64;
+    if (c == 0) {
+        q.shard_len[s] = L;
+        q.mismatch[s] = bad_geo ? (1u << q.m) - 1 : 0u;
+    }
+    if (bad_geo) {
+        if (c == 0) q.hash_bad[s] = 1;
+        return;
+    }
+    const uint8_t *stripe = q.shards + (size_t)s * (q.k + q.m) * q.stride;
+    // this lane's 32 block bytes at o + 32c, as two 16-byte vectors; zero past block_len
+    auto load32 = [&](uint32_t o, uint4 &x, uint4 &y) {
+        const uint32_t a0 = o + 32 * c;
+        uint32_t j = 0, off = 0;
+        if (a0 < len) {  // L >= 1 here
+            j = a0 / L;
+            off = a0 - j * L;
+        }
+        const uint32_t nx = a0 < len ? min(16u, len - a0) : 0u, ny = a0 + 16 < len ? min(16u, len - a0 - 16) : 0u;
+        x = block_vec16(stripe, q.stride, L, j, off, nx);
+        if (ny && off + 16 >= L) {  // the second vector starts in the next shard
+            off = off + 16 - L;
+            j++;
+        } else {
+            off += 16;
+        }
+        y = block_vec16(stripe, q.stride, L, j, off, ny);
+    };
+    const uint64_t h0 = blake2b_quad(len, &s_msg[tid >> 2][0], load32);
+    const unsigned long long e = *reinterpret_cast<const unsigned long long *>(q.hashes + (size_t)s * 32 + 8 * c);
+    const uint32_t diff = __ballot_sync(qmask, e != h0) & qmask;
+    if (c == 0) q.hash_bad[s] = diff ? 1 : 0;
 }
 
 // ------------------------------------------------------------------ block -> shard framing on the device

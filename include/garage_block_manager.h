@@ -151,6 +151,11 @@ typedef struct {
     uint64_t resync_bytes_fetched;           /* bytes resync_block's fetch branch handed to the rebuild: what would
                                                 cross the network in Garage.  Clay: the repair runs (1/m of each
                                                 helper); RS, LRC and PB: resync_bytes_read                          */
+    uint64_t deep_scrub_blocks;              /* blocks garage_bm_deep_scrub_step checked (content hash + parity) */
+    uint64_t deep_scrub_skipped;             /* blocks it skipped because a shard was missing or bad            */
+    uint64_t deep_scrub_parity_bad;          /* stale parity shards it quarantined                               */
+    uint64_t deep_scrub_content_errors;      /* blocks whose content hash failed and whose hunt found no culprit */
+    uint64_t deep_check_call_us;             /* wall time inside garage_ec_deep_check                            */
 } garage_bm_metrics;
 
 void garage_bm_default_config(garage_bm_config *cfg);
@@ -197,6 +202,21 @@ int garage_bm_scrub(garage_bm *bm, int node, uint64_t *checked, uint64_t *corrup
  * position to persist, *finished = 1 once the end of the node's store was reached.                */
 int garage_bm_scrub_step(garage_bm *bm, int node, const uint8_t *cursor32, size_t max_shards,
                          uint8_t cursor_out32[32], int *finished, uint64_t *checked, uint64_t *corrupt);
+
+/* Deep scrub (DESIGN.md section 5.4), resumable in hash order like garage_bm_scrub_step: the known blocks not at rc 0
+ * whose deep-scrub owner is `node` -- the first up node of the block's row in the newest layout version -- after
+ * cursor32 (NULL = from the start), at most max_blocks of them (0 = all).  In batches of batch_max_blocks, all k+m
+ * shards of the configured stripe are read (tags checked on read) and garage_ec_deep_check proves the block's content
+ * hash and every parity row on the GPU:
+ *   - hash and parity right: clean;
+ *   - hash right, parity rows wrong: every flagged parity shard is quarantined (and queued for resync);
+ *   - hash wrong: the stale-shard hunt of GET quarantines the culprit, or, if no consistent set exists, the block
+ *     counts in deep_scrub_content_errors and no file is touched.
+ * A block with a configured shard missing or bad is skipped (its resync queued); a block held only under a previous
+ * code or as replicas is skipped without one.  *checked = blocks deep-checked, *repaired = shards quarantined.
+ * GARAGE_BM_E_MESSAGE if `node` is down.                                                                          */
+int garage_bm_deep_scrub_step(garage_bm *bm, int node, const uint8_t *cursor32, size_t max_blocks,
+                              uint8_t cursor_out32[32], int *finished, uint64_t *checked, uint64_t *repaired);
 
 /* Conversion sweep of `node` (DESIGN.md section 5.1), resumable in hash order like garage_bm_scrub_step: every block
  * with a legacy shard or replica on `node`, after cursor32 (NULL = from the start), at most max_blocks (0 = all):

@@ -200,6 +200,22 @@ int garage_ec_verify(garage_ec_ctx *ctx, const uint8_t *shards, uint32_t *mismat
                      const uint32_t *shard_len, size_t stride, size_t n_stripes, int mem_kind,
                      void *cuda_stream);
 
+/* ---- DEEP CHECK (deep scrub) -- what ScrubWorker::work proves for a plain block (src/block/repair.rs:438-490,
+ * DataBlock::verify, src/block/block.rs:69-83: blake2sum(block) == hash), done on a stored stripe, together with
+ * garage_ec_verify.  Per stripe s of the shard layout (k+m shards, `stride` apart):
+ *   block_len : n values; L = garage_ec_code_shard_len(block_len[s]); the block is the first block_len bytes of data
+ *               shards 0..k-1 concatenated (DESIGN.md section 2.3).  Shard bytes in [L, stride) are ignored
+ *   hashes    : n * 32 bytes, the content addresses
+ *   hash_bad  : n bytes out, 1 iff the block's blake2sum differs from hashes[s]
+ *   mismatch  : n uint32 out, exactly garage_ec_verify's result for the stripe with shard_len = L (bit i = parity k+i)
+ * A stripe whose L exceeds `stride`: a HOST call returns GARAGE_EC_E_INVALID before any GPU work; a DEVICE call
+ * reports hash_bad = 1 and all m mismatch bits, and reads nothing of it.  DEVICE: all pointers device memory (hashes
+ * 8-byte aligned), only kernels and stream-ordered scratch are enqueued (capturable in a CUDA graph).  HOST: uploads
+ * roundup16(L) bytes of each shard.                                                                                 */
+int garage_ec_deep_check(garage_ec_ctx *ctx, const uint8_t *shards, const uint32_t *block_len, const uint8_t *hashes,
+                         uint8_t *hash_bad, uint32_t *mismatch, size_t stride, size_t n_stripes, int mem_kind,
+                         void *cuda_stream);
+
 /* ---- PER-SHARD INTEGRITY (SURVEY.md section 8 row f2) -- call sites: DataBlock::verify,
  * src/block/block.rs:69-83 (Plain => blake2sum(data) == hash) and read_block_from,
  * src/block/manager.rs:577-609.  A node stores 1/k of a block, so the whole-block hash cannot be

@@ -90,5 +90,20 @@ impl ErasureCoder {
         check(self.ctx, rc)?;
         Ok(mm)
     }
+
+    /// Deep scrub of gathered stripes: per stripe, (the block read from the data shards does not hash to
+    /// `hashes[s]`, the parity rows that disagree with the data shards).
+    pub fn deep_check(&self, shards_layout: &[u8], block_len: &[u32], hashes: &[[u8; 32]], stride: usize)
+                      -> Result<(Vec<bool>, Vec<u32>), Error> {
+        let n = block_len.len();
+        assert_eq!(hashes.len(), n);
+        let mut bad = vec![0u8; n];
+        let mut mm = vec![0u32; n];
+        let rc = unsafe { sys::garage_ec_deep_check(self.ctx, shards_layout.as_ptr(), block_len.as_ptr(),
+                          hashes.as_ptr() as *const u8, bad.as_mut_ptr(), mm.as_mut_ptr(), stride, n,
+                          sys::GARAGE_EC_MEM_HOST, std::ptr::null_mut()) };
+        check(self.ctx, rc)?;
+        Ok((bad.into_iter().map(|b| b != 0).collect(), mm))
+    }
 }
 impl Drop for ErasureCoder { fn drop(&mut self) { unsafe { sys::garage_ec_destroy(self.ctx) } } }

@@ -62,6 +62,9 @@ extern "C" {
     pub fn garage_ec_verify(ctx: *mut garage_ec_ctx, shards: *const u8, mismatch: *mut u32,
                             shard_len: *const u32, stride: usize, n_stripes: usize,
                             mem_kind: c_int, cuda_stream: *mut c_void) -> c_int;
+    pub fn garage_ec_deep_check(ctx: *mut garage_ec_ctx, shards: *const u8, block_len: *const u32,
+                            hashes: *const u8, hash_bad: *mut u8, mismatch: *mut u32, stride: usize,
+                            n_stripes: usize, mem_kind: c_int, cuda_stream: *mut c_void) -> c_int;
     pub fn garage_ec_encode_blocks(ctx: *mut garage_ec_ctx, blocks: *const *const u8,
                             block_len: *const u32, n_blocks: usize, parity_out: *mut u8,
                             stride: usize) -> c_int;
