@@ -19,10 +19,10 @@
 #include <atomic>
 #include <condition_variable>
 #include <cctype>
-#include <chrono>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <mutex>
 #include <new>
 #include <utility>
@@ -39,8 +39,7 @@ static_assert(GARAGE_EC_MAX_K == GARAGE_EC_MAX_K_HOST && GARAGE_EC_MAX_M == GARA
 
 namespace {
 
-constexpr int kHostLanes = 3;                       // H2D / kernel / D2H overlap across chunks
-constexpr size_t kHostChunkBytes = 48ull << 20;     // target source bytes per pipeline chunk
+constexpr int kHostLanes = 3;  // H2D / kernel / D2H overlap across chunks
 
 struct HostLane {
     cudaStream_t stream = nullptr;
@@ -84,19 +83,9 @@ struct garage_ec_ctx {
     cpu_set_t node_cpus;
     int last_alloc_node = -1;                 // node the last garage_ec_host_alloc landed on (-1 unknown)
     std::atomic<long> fault_countdown{-1};
-    // GARAGE_EC_TRACE=1: host-side time per phase of the block-level encode call, printed at destroy (tuning aid)
-    bool trace = false;
     // how a HOST-mode call waits for its lanes: 0 = cudaStreamSynchronize (the driver spins: lowest latency, one CPU
     // per waiting caller), 1 = block on an event (garage_ec_set_wait_mode)
     std::atomic<int> wait_blocking{0};
-    // HOST-mode calls on pinned (device-addressable) buffers: let the kernel read and write the host memory directly
-    // over PCIe instead of staging chunks through device buffers.  Reconstruct's staged form moves ~130 scattered
-    // 100 KB pieces per chunk in each direction, which the kernel's direct reads and writes avoid; encode moves one
-    // contiguous copy per chunk, which staging handles well.  Default: reconstruct only.  GARAGE_EC_ZEROCOPY=0 turns it
-    // off, =1 also applies it to encode.
-    bool zero_copy_rec = true, zero_copy_enc = false;
-    std::atomic<uint64_t> tr_calls{0}, tr_blocks{0}, tr_prep_us{0}, tr_issue_us{0}, tr_sync_us{0};
-    std::atomic<uint64_t> tr_gpu_ns[4] = {};  // device time of the first chunk: H2D | split+encode | parity D2H | tags + D2H
     // test hook: fail the n-th staged operation (see garage_ec_debug_fail_after)
     std::mutex misc_mu;  // timing list, last_error
     bool timing = false;
@@ -144,44 +133,19 @@ inline cudaError_t lane_wait(garage_ec_ctx *ctx, HostLane &L)
     return e;
 }
 
-// Lease of one lane set for the duration of a HOST-mode call.  The destructor waits for every
-// lane stream BEFORE the set goes back to the pool -- and therefore before the entry point
-// returns, on every path including the early error returns: no DMA touches the caller's buffers
-// after a HOST call has returned ("the library keeps no pointer", include/garage_ec.h).
-struct LaneLease {
-    garage_ec_ctx *ctx;
-    LaneSet *set = nullptr;
-    explicit LaneLease(garage_ec_ctx *c) : ctx(c)
-    {
-        std::unique_lock<std::mutex> lk(ctx->pool_mu);
-        ctx->pool_cv.wait(lk, [&] { return !ctx->free_sets.empty() || ctx->n_sets < kMaxLaneSets; });
-        if (!ctx->free_sets.empty()) {
-            set = ctx->free_sets.back();
-            ctx->free_sets.pop_back();
-        } else {
-            set = new (std::nothrow) LaneSet();
-            if (set) ctx->n_sets++;
-        }
-    }
-    ~LaneLease()
-    {
-        if (!set) return;
-        for (HostLane &L : set->lanes)
-            if (L.stream) (void)cudaStreamSynchronize(L.stream);
-        (void)cudaGetLastError();
-        {
-            std::lock_guard<std::mutex> lk(ctx->pool_mu);
-            ctx->free_sets.push_back(set);
-        }
-        ctx->pool_cv.notify_one();
-    }
-    LaneLease(const LaneLease &) = delete;
-    LaneLease &operator=(const LaneLease &) = delete;
-    HostLane &operator[](size_t i) { return set->lanes[i]; }
-};
-#define LEASE_LANES(ctx, name)  \
-    LaneLease name(ctx);        \
-    if (!name.set) return GARAGE_EC_E_NOMEM
+// Stream-ordered device scratch of `bytes` for the work f(scratch) queues on st, freed on st after it: from the context's
+// pool (the default pool if it has none), so that DEVICE-mode calls stay capturable in a CUDA graph.  f's error first.
+template <class F>
+int with_stream_scratch(garage_ec_ctx *ctx, size_t bytes, cudaStream_t st, F &&f)
+{
+    void *scratch = nullptr;
+    CU_TRY(ctx, ctx->pool ? cudaMallocFromPoolAsync(&scratch, bytes, ctx->pool, st) : cudaMallocAsync(&scratch, bytes, st));
+    const int rc = f(static_cast<uint8_t *>(scratch));
+    const cudaError_t e = cudaFreeAsync(scratch, st);
+    if (rc) return rc;
+    if (e != cudaSuccess) return set_cuda_error(ctx, e, "cudaFreeAsync");
+    return GARAGE_EC_OK;
+}
 
 // ---- NUMA placement of the GPU ------------------------------------------------------------
 // 8-GPU hosts hang 4 GPUs off each socket; pinned buffers that land on the other socket cross
@@ -490,7 +454,7 @@ int run_clay(garage_ec_ctx *ctx, int mode, const uint8_t *src, size_t src_pitch,
 // n * items_per_stripe stays below 2^32 and m > 4 runs in passes of 4 rows.
 int run_uniform(garage_ec_ctx *ctx, int mode, const uint8_t *src, size_t src_pitch, uint8_t *dst,
                 size_t dst_pitch, uint32_t *mismatch, const uint32_t *shard_len, size_t stride,
-                size_t n, cudaStream_t st, bool allow_tmap = true)
+                size_t n, cudaStream_t st)
 {
     if (ctx->pb) return run_pb_uniform(ctx, mode, src, src_pitch, dst, dst_pitch, mismatch, shard_len, stride, n, st);
     if (ctx->clay) return run_clay(ctx, mode, src, src_pitch, dst, dst_pitch, mismatch, shard_len, stride, n, st);
@@ -502,53 +466,59 @@ int run_uniform(garage_ec_ctx *ctx, int mode, const uint8_t *src, size_t src_pit
     // one zeroed work counter per launch (rs_apply_kernel's dynamic schedule): stream-ordered scratch, so the
     // call stays capturable in a CUDA graph
     const size_t launches = (n + max_n - 1) / max_n * (size_t)((ctx->m + kRowsPerPass - 1) / kRowsPerPass);
-    void *scratch = nullptr;
-    CU_TRY(ctx, ctx->pool ? cudaMallocFromPoolAsync(&scratch, launches * sizeof(uint32_t), ctx->pool, st)
-                          : cudaMallocAsync(&scratch, launches * sizeof(uint32_t), st));
-    uint32_t *counter = reinterpret_cast<uint32_t *>(scratch);
-    cudaError_t e = cudaMemsetAsync(counter, 0, launches * sizeof(uint32_t), st);
-    int rc = e == cudaSuccess ? GARAGE_EC_OK : set_cuda_error(ctx, e, "cudaMemsetAsync(counter)");
-    for (size_t s0 = 0; s0 < n && rc == GARAGE_EC_OK; s0 += max_n) {
-        const size_t cnt = n - s0 < max_n ? n - s0 : max_n;
-        for (int r0 = 0; r0 < ctx->m && rc == GARAGE_EC_OK; r0 += kRowsPerPass) {
-            ApplyParams p;
-            memset(&p, 0, sizeof(p));
-            p.src = src + s0 * src_pitch;
-            p.src_pitch = src_pitch;
-            p.dst = dst ? dst + s0 * dst_pitch + (size_t)r0 * stride : nullptr;
-            p.dst_pitch = dst_pitch;
-            p.shard_len = shard_len ? shard_len + s0 : nullptr;
-            p.mismatch = mismatch ? mismatch + s0 : nullptr;
-            p.counter = counter++;
-            p.stride = (uint32_t)stride;
-            p.n = (uint32_t)cnt;
-            p.k = (uint32_t)ctx->k;
-            p.rows = (uint32_t)(ctx->m - r0 < kRowsPerPass ? ctx->m - r0 : kRowsPerPass);
-            p.row_off = (uint32_t)r0;
-            p.items_per_stripe = ips;
-            p.row_bytes = 128;
-            p.rows_per_stripe = (uint32_t)(src_pitch / stride);
-            p.use_tmap = (allow_tmap && GEC_TMAP && ctx->k >= GEC_TMAP_FROM_K && make_src_tensor_map(&p.tmap, p.src, stride, cnt * p.rows_per_stripe,
-                                              (GEC_SPLIT_STAGE && ctx->k > 16) ? 16 : ctx->k)) ? 1u : 0u;  // box rows: StreamCfg::kSrcRows
-            for (uint32_t i = 0; i < p.rows; i++)
-                memcpy(p.coef + i * ctx->k, ctx->P + (r0 + i) * ctx->k, ctx->k);
-            e = mode == kModeEncode ? launch_apply<kModeEncode>(ctx, p, st) : launch_apply<kModeVerify>(ctx, p, st);
-            if (e != cudaSuccess) rc = set_cuda_error(ctx, e, "rs_apply_kernel launch");
+    return with_stream_scratch(ctx, launches * sizeof(uint32_t), st, [&](uint8_t *scratch) -> int {
+        uint32_t *counter = reinterpret_cast<uint32_t *>(scratch);
+        cudaError_t e = cudaMemsetAsync(counter, 0, launches * sizeof(uint32_t), st);
+        if (e != cudaSuccess) return set_cuda_error(ctx, e, "cudaMemsetAsync(counter)");
+        for (size_t s0 = 0; s0 < n; s0 += max_n) {
+            const size_t cnt = n - s0 < max_n ? n - s0 : max_n;
+            for (int r0 = 0; r0 < ctx->m; r0 += kRowsPerPass) {
+                ApplyParams p;
+                memset(&p, 0, sizeof(p));
+                p.src = src + s0 * src_pitch;
+                p.src_pitch = src_pitch;
+                p.dst = dst ? dst + s0 * dst_pitch + (size_t)r0 * stride : nullptr;
+                p.dst_pitch = dst_pitch;
+                p.shard_len = shard_len ? shard_len + s0 : nullptr;
+                p.mismatch = mismatch ? mismatch + s0 : nullptr;
+                p.counter = counter++;
+                p.stride = (uint32_t)stride;
+                p.n = (uint32_t)cnt;
+                p.k = (uint32_t)ctx->k;
+                p.rows = (uint32_t)(ctx->m - r0 < kRowsPerPass ? ctx->m - r0 : kRowsPerPass);
+                p.row_off = (uint32_t)r0;
+                p.items_per_stripe = ips;
+                p.row_bytes = 128;
+                p.rows_per_stripe = (uint32_t)(src_pitch / stride);
+                p.use_tmap = (GEC_TMAP && ctx->k >= GEC_TMAP_FROM_K && make_src_tensor_map(&p.tmap, p.src, stride, cnt * p.rows_per_stripe,
+                                                  (GEC_SPLIT_STAGE && ctx->k > 16) ? 16 : ctx->k)) ? 1u : 0u;  // box rows: StreamCfg::kSrcRows
+                for (uint32_t i = 0; i < p.rows; i++)
+                    memcpy(p.coef + i * ctx->k, ctx->P + (r0 + i) * ctx->k, ctx->k);
+                e = mode == kModeEncode ? launch_apply<kModeEncode>(ctx, p, st) : launch_apply<kModeVerify>(ctx, p, st);
+                if (e != cudaSuccess) return set_cuda_error(ctx, e, "rs_apply_kernel launch");
+            }
         }
-    }
-    e = cudaFreeAsync(scratch, st);
-    if (e != cudaSuccess && rc == GARAGE_EC_OK) rc = set_cuda_error(ctx, e, "cudaFreeAsync(counter)");
-    return rc;
+        return GARAGE_EC_OK;
+    });
 }
 
-// Device-resident reconstruct.  plan/counter scratch supplied by the caller (device).
+// Device scratch of run_reconstruct for n stripes: StripePlans | apply counter (16 B) | Clay: the present / want maps of
+// the base code, n' bytes each per stripe
+size_t plan_scratch_bytes(const garage_ec_ctx *ctx, size_t n)
+{
+    return n * sizeof(StripePlan) + 16 + (ctx->clay ? (2 * n * (size_t)ctx->cg.n + 15) / 16 * 16 : 0);
+}
+
+// Device-resident reconstruct.  plan_scratch: plan_scratch_bytes(ctx, n) of device memory.
 int run_reconstruct(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *present, const uint8_t *want,
                     int32_t *status, const uint32_t *shard_len, size_t stride, size_t n,
-                    StripePlan *plan, uint32_t *counter, cudaStream_t st, bool present_is_bad = false)
+                    uint8_t *plan_scratch, cudaStream_t st, bool present_is_bad = false)
 {
+    StripePlan *plan = reinterpret_cast<StripePlan *>(plan_scratch);
+    uint32_t *counter = reinterpret_cast<uint32_t *>(plan_scratch + n * sizeof(StripePlan));
     if (ctx->clay) {
-        // the caller's maps onto the n' nodes of the base code (after the counter, plan_scratch_bytes), the base-code
-        // plan by plan_kernel, then the layered decode / repair
+        // the caller's maps onto the n' nodes of the base code, the base-code plan by plan_kernel, then the layered
+        // decode / repair
         const int N = ctx->cg.n, kb = ctx->k + ctx->cg.s;
         uint8_t *present2 = reinterpret_cast<uint8_t *>(counter) + 16, *want2 = present2 + n * N;
         ClayParams c = clay_params(ctx, stride, n);
@@ -636,12 +606,6 @@ int run_reconstruct(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *present,
         if (e != cudaSuccess) return set_cuda_error(ctx, e, "rs_apply_kernel<plan> launch");
     }
     return GARAGE_EC_OK;
-}
-
-// StripePlans | apply counter (16 B) | Clay: the present / want maps of the base code, n' bytes each per stripe
-size_t plan_scratch_bytes(const garage_ec_ctx *ctx, size_t n)
-{
-    return n * sizeof(StripePlan) + 16 + (ctx->clay ? (2 * n * (size_t)ctx->cg.n + 15) / 16 * 16 : 0);
 }
 
 // The half-shards plan_kernel reads for one stripe (present / want: k+m bytes, want nullable = every absent
@@ -798,6 +762,149 @@ int lane_reserve(garage_ec_ctx *ctx, HostLane &L, size_t buf_bytes, size_t small
 
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// A lane's small device buffer: 16-byte aligned regions, handed out in the order they are taken
+struct SmallLayout {
+    size_t bytes = 0;
+    size_t take(size_t n)
+    {
+        const size_t o = bytes;
+        bytes += align_up(n, 16);
+        return o;
+    }
+};
+
+// One chunk of a HOST-mode call: stripes [s0, s0 + cnt) on lane L, with the lane's pageable staging
+struct HostChunk {
+    HostLane *L = nullptr;
+    uint8_t *host = nullptr;
+    size_t s0 = 0, cnt = 0;
+    bool pending = false;  // issued, not retired yet
+};
+using Retire = std::function<int(const HostChunk &)>;
+
+// The chunk pipeline every HOST-mode call stages through: n stripes in chunks of cs (about kHostChunkBytes of
+// bytes_per_stripe each), round robin over the three lanes of one leased lane set, so that H2D, kernels and D2H of
+// consecutive chunks overlap.  bytes_per_stripe == 0: one chunk of all n stripes on lane 0 (zero-copy calls).
+//
+// It owns the lease and every host object a queued copy reads or writes: the copy lists, the per-lane pageable
+// staging and the status array of a caller that passed none.  The destructor waits for every lane stream before the
+// set goes back to the pool and before those members are freed, so no DMA touches the caller's buffers after a HOST
+// call has returned, on every path including the early error returns ("the library keeps no pointer",
+// include/garage_ec.h).  n == 0 takes no lease.
+class HostPipeline {
+public:
+    static constexpr size_t kHostChunkBytes = 48ull << 20;  // target source bytes per chunk
+    const size_t n, cs;
+    CopyBatch up, down;  // the chunk being issued (or, in a retire step, the chunk being retired)
+
+    HostPipeline(garage_ec_ctx *ctx, size_t n, size_t bytes_per_stripe)
+        : n(n), cs(bytes_per_stripe ? std::min(std::max<size_t>(kHostChunkBytes / bytes_per_stripe, 1), n) : n),
+          ctx_(ctx), lanes_(bytes_per_stripe ? kHostLanes : 1)
+    {
+    }
+    HostPipeline(const HostPipeline &) = delete;
+    HostPipeline &operator=(const HostPipeline &) = delete;
+    ~HostPipeline()
+    {
+        if (!set_) return;
+        for (HostLane &L : set_->lanes)
+            if (L.stream) (void)cudaStreamSynchronize(L.stream);
+        (void)cudaGetLastError();
+        {
+            std::lock_guard<std::mutex> lk(ctx_->pool_mu);
+            ctx_->free_sets.push_back(set_);
+        }
+        ctx_->pool_cv.notify_one();
+    }
+
+    // lease a lane set and size its lanes: `buf` bytes of chunk buffer, `small` bytes of small buffer (SmallLayout)
+    // and `host` bytes of pageable staging per lane
+    int reserve(size_t buf, size_t small, size_t host = 0)
+    {
+        if (!n) return GARAGE_EC_OK;
+        {
+            std::unique_lock<std::mutex> lk(ctx_->pool_mu);
+            ctx_->pool_cv.wait(lk, [&] { return !ctx_->free_sets.empty() || ctx_->n_sets < kMaxLaneSets; });
+            if (!ctx_->free_sets.empty()) {
+                set_ = ctx_->free_sets.back();
+                ctx_->free_sets.pop_back();
+            } else {
+                set_ = new (std::nothrow) LaneSet();
+                if (set_) ctx_->n_sets++;
+            }
+        }
+        if (!set_) return GARAGE_EC_E_NOMEM;
+        for (int l = 0; l < lanes_; l++) {
+            int rc = lane_reserve(ctx_, set_->lanes[l], buf, small);
+            if (rc) return rc;
+        }
+        host_stride_ = align_up(host, 16);
+        host_.resize(host_stride_ * lanes_);
+        return GARAGE_EC_OK;
+    }
+
+    // the caller's status array, or one of ours for the n stripes
+    int32_t *status_out(int32_t *status)
+    {
+        if (status) return status;
+        own_status_.assign(n, 0);
+        return own_status_.data();
+    }
+
+    // issue(chunk) queues every chunk.  A lane whose previous chunk left work for the host -- a retire step, or the
+    // lane's pageable staging, which the next chunk overwrites -- is waited for before it takes the next chunk, and
+    // retire(previous chunk) runs then.
+    template <class Issue>
+    int run(Issue &&issue, const Retire &retire = nullptr)
+    {
+        size_t c = 0;
+        for (size_t s0 = 0; s0 < n; s0 += cs, c++) {
+            HostChunk &ch = chunks_[c % lanes_];
+            if (ch.pending && (retire || host_stride_)) {
+                int rc = retire_chunk(ch, retire);
+                if (rc) return rc;
+            }
+            ch.L = &set_->lanes[c % lanes_];
+            ch.host = host_.data() + (c % lanes_) * host_stride_;
+            ch.s0 = s0;
+            ch.cnt = n - s0 < cs ? n - s0 : cs;
+            ch.pending = true;
+            int rc = issue(ch);
+            if (rc) return rc;
+        }
+        return GARAGE_EC_OK;
+    }
+
+    // retire every pending chunk, then wait for every lane
+    int drain(const Retire &retire = nullptr)
+    {
+        if (!set_) return GARAGE_EC_OK;
+        for (int l = 0; l < lanes_ && retire; l++) {
+            if (!chunks_[l].pending) continue;
+            int rc = retire_chunk(chunks_[l], retire);
+            if (rc) return rc;
+        }
+        for (int l = 0; l < lanes_; l++) CU_TRY(ctx_, lane_wait(ctx_, set_->lanes[l]));
+        return GARAGE_EC_OK;
+    }
+
+private:
+    int retire_chunk(HostChunk &ch, const Retire &retire)
+    {
+        ch.pending = false;
+        CU_TRY(ctx_, lane_wait(ctx_, *ch.L));
+        return retire ? retire(ch) : GARAGE_EC_OK;
+    }
+
+    garage_ec_ctx *ctx_;
+    const int lanes_;
+    std::vector<uint8_t> host_;
+    size_t host_stride_ = 0;
+    std::vector<int32_t> own_status_;
+    HostChunk chunks_[kHostLanes];
+    LaneSet *set_ = nullptr;
+};
+
 int create_common(garage_ec_ctx **out, int device, int k, int m, const uint8_t *P, int kind, int l = 0, bool pb = false,
                   const ClayGeo *clay = nullptr)
 {
@@ -854,9 +961,7 @@ int create_common(garage_ec_ctx **out, int device, int k, int m, const uint8_t *
         (void)cudaGetLastError();
     }
     probe_numa(ctx);
-    ctx->trace = getenv("GARAGE_EC_TRACE") != nullptr;
     if (const char *b = getenv("GARAGE_EC_BATCHCOPY")) ctx->batch_copy_ok.store(b[0] != '0');
-    if (const char *z = getenv("GARAGE_EC_ZEROCOPY")) ctx->zero_copy_rec = ctx->zero_copy_enc = z[0] == '1';
     *out = ctx;
     return GARAGE_EC_OK;
 }
@@ -1015,15 +1120,6 @@ int garage_ec_create_with_matrix(garage_ec_ctx **out, int cuda_device, int k, in
 void garage_ec_destroy(garage_ec_ctx *ctx)
 {
     if (!ctx) return;
-    if (ctx->trace && ctx->tr_calls.load())
-        fprintf(stderr, "garage_ec trace ctx %p: encode_blocks calls=%llu blocks=%llu  per call: prep %.1f us, issue %.1f us, sync %.1f us\n",
-                (void *)ctx, (unsigned long long)ctx->tr_calls.load(), (unsigned long long)ctx->tr_blocks.load(),
-                (double)ctx->tr_prep_us.load() / ctx->tr_calls.load(), (double)ctx->tr_issue_us.load() / ctx->tr_calls.load(),
-                (double)ctx->tr_sync_us.load() / ctx->tr_calls.load());
-    if (ctx->trace && ctx->tr_calls.load())
-        fprintf(stderr, "    device time of the first chunk per call: H2D %.1f us, split+encode %.1f us, parity D2H %.1f us, tags+D2H %.1f us\n",
-                ctx->tr_gpu_ns[0].load() / 1e3 / ctx->tr_calls.load(), ctx->tr_gpu_ns[1].load() / 1e3 / ctx->tr_calls.load(),
-                ctx->tr_gpu_ns[2].load() / 1e3 / ctx->tr_calls.load(), ctx->tr_gpu_ns[3].load() / 1e3 / ctx->tr_calls.load());
     cudaSetDevice(ctx->device);
     for (LaneSet *set : ctx->free_sets) {
         for (HostLane &L : set->lanes) {
@@ -1212,53 +1308,29 @@ static bool device_addressable_host(const void *p)
 static int encode_host(garage_ec_ctx *ctx, const uint8_t *data, uint8_t *parity,
                        const uint32_t *shard_len, size_t stride, size_t n)
 {
-    LEASE_LANES(ctx, lanes);
-    if (ctx->zero_copy_enc && !ctx->clay && device_addressable_host(data) && device_addressable_host(parity)) {
-        // one launch over the whole batch: the TMA / vector loads pull the data shards across PCIe, the parity stores
-        // go straight to the caller's buffer -- no staging copies, no chunk boundaries
-        HostLane &L = lanes[0];
-        int rc = lane_reserve(ctx, L, 0, align_up(n * 4, 16));
-        if (rc) return rc;
-        const uint32_t *d_len = nullptr;
-        if (shard_len) {
-            CU_TRY(ctx, cudaMemcpyAsync(L.d_small, shard_len, n * 4, cudaMemcpyHostToDevice, L.stream));
-            d_len = reinterpret_cast<const uint32_t *>(L.d_small);
-        }
-        rc = run_uniform(ctx, kModeEncode, data, ctx->k * stride, parity, ctx->m * stride, nullptr, d_len, stride, n, L.stream,
-                         /*allow_tmap=*/false);
-        if (rc) return rc;
-        CU_TRY(ctx, lane_wait(ctx, L));
-        return GARAGE_EC_OK;
-    }
     const size_t k = ctx->k, m = ctx->m;
-    size_t cs = kHostChunkBytes / (k * stride);
-    if (cs < 1) cs = 1;
-    if (cs > n) cs = n;
-    const size_t in_b = cs * k * stride, out_b = cs * m * stride;
-    for (HostLane &L : lanes.set->lanes) {
-        int rc = lane_reserve(ctx, L, in_b + out_b, align_up(cs * 4, 16));
-        if (rc) return rc;
-    }
-    size_t c = 0;
-    for (size_t s0 = 0; s0 < n; s0 += cs, c++) {
-        HostLane &L = lanes[c % kHostLanes];
-        const size_t cnt = n - s0 < cs ? n - s0 : cs;
-        CU_TRY(ctx, cudaMemcpyAsync(L.d_buf, data + s0 * k * stride, cnt * k * stride,
+    HostPipeline p(ctx, n, k * stride);
+    const size_t in_b = p.cs * k * stride, out_b = p.cs * m * stride;
+    int rc = p.reserve(in_b + out_b, align_up(p.cs * 4, 16));
+    if (rc) return rc;
+    rc = p.run([&](const HostChunk &ch) -> int {
+        HostLane &L = *ch.L;
+        CU_TRY(ctx, cudaMemcpyAsync(L.d_buf, data + ch.s0 * k * stride, ch.cnt * k * stride,
                                     cudaMemcpyHostToDevice, L.stream));
         const uint32_t *d_len = nullptr;
         if (shard_len) {
-            CU_TRY(ctx, cudaMemcpyAsync(L.d_small, shard_len + s0, cnt * 4, cudaMemcpyHostToDevice,
+            CU_TRY(ctx, cudaMemcpyAsync(L.d_small, shard_len + ch.s0, ch.cnt * 4, cudaMemcpyHostToDevice,
                                         L.stream));
             d_len = reinterpret_cast<const uint32_t *>(L.d_small);
         }
-        int rc = run_uniform(ctx, kModeEncode, L.d_buf, k * stride, L.d_buf + in_b, m * stride,
-                             nullptr, d_len, stride, cnt, L.stream);
-        if (rc) return rc;
-        CU_TRY(ctx, cudaMemcpyAsync(parity + s0 * m * stride, L.d_buf + in_b, cnt * m * stride,
+        int r = run_uniform(ctx, kModeEncode, L.d_buf, k * stride, L.d_buf + in_b, m * stride,
+                            nullptr, d_len, stride, ch.cnt, L.stream);
+        if (r) return r;
+        CU_TRY(ctx, cudaMemcpyAsync(parity + ch.s0 * m * stride, L.d_buf + in_b, ch.cnt * m * stride,
                                     cudaMemcpyDeviceToHost, L.stream));
-    }
-    for (HostLane &L : lanes.set->lanes) CU_TRY(ctx, lane_wait(ctx, L));
-    return GARAGE_EC_OK;
+        return GARAGE_EC_OK;
+    });
+    return rc ? rc : p.drain();
 }
 
 int garage_ec_encode(garage_ec_ctx *ctx, const uint8_t *data, uint8_t *parity,
@@ -1283,37 +1355,31 @@ int garage_ec_encode(garage_ec_ctx *ctx, const uint8_t *data, uint8_t *parity,
 static int verify_host(garage_ec_ctx *ctx, const uint8_t *shards, uint32_t *mismatch,
                        const uint32_t *shard_len, size_t stride, size_t n)
 {
-    LEASE_LANES(ctx, lanes);
     const size_t tot = ctx->k + ctx->m;
-    size_t cs = kHostChunkBytes / (tot * stride);
-    if (cs < 1) cs = 1;
-    if (cs > n) cs = n;
-    const size_t small = align_up(cs * 4, 16);
-    for (HostLane &L : lanes.set->lanes) {
-        int rc = lane_reserve(ctx, L, cs * tot * stride, 2 * small);
-        if (rc) return rc;
-    }
-    size_t c = 0;
-    for (size_t s0 = 0; s0 < n; s0 += cs, c++) {
-        HostLane &L = lanes[c % kHostLanes];
-        const size_t cnt = n - s0 < cs ? n - s0 : cs;
-        CU_TRY(ctx, cudaMemcpyAsync(L.d_buf, shards + s0 * tot * stride, cnt * tot * stride,
+    HostPipeline p(ctx, n, tot * stride);
+    SmallLayout sl;
+    const size_t o_mm = sl.take(p.cs * 4), o_len = sl.take(p.cs * 4);
+    int rc = p.reserve(p.cs * tot * stride, sl.bytes);
+    if (rc) return rc;
+    rc = p.run([&](const HostChunk &ch) -> int {
+        HostLane &L = *ch.L;
+        CU_TRY(ctx, cudaMemcpyAsync(L.d_buf, shards + ch.s0 * tot * stride, ch.cnt * tot * stride,
                                     cudaMemcpyHostToDevice, L.stream));
-        uint32_t *d_mm = reinterpret_cast<uint32_t *>(L.d_small);
+        uint32_t *d_mm = reinterpret_cast<uint32_t *>(L.d_small + o_mm);
         const uint32_t *d_len = nullptr;
         if (shard_len) {
-            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + small, shard_len + s0, cnt * 4,
+            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_len, shard_len + ch.s0, ch.cnt * 4,
                                         cudaMemcpyHostToDevice, L.stream));
-            d_len = reinterpret_cast<const uint32_t *>(L.d_small + small);
+            d_len = reinterpret_cast<const uint32_t *>(L.d_small + o_len);
         }
-        CU_TRY(ctx, cudaMemsetAsync(d_mm, 0, cnt * 4, L.stream));
-        int rc = run_uniform(ctx, kModeVerify, L.d_buf, tot * stride, nullptr, 0, d_mm, d_len, stride,
-                             cnt, L.stream);
-        if (rc) return rc;
-        CU_TRY(ctx, cudaMemcpyAsync(mismatch + s0, d_mm, cnt * 4, cudaMemcpyDeviceToHost, L.stream));
-    }
-    for (HostLane &L : lanes.set->lanes) CU_TRY(ctx, lane_wait(ctx, L));
-    return GARAGE_EC_OK;
+        CU_TRY(ctx, cudaMemsetAsync(d_mm, 0, ch.cnt * 4, L.stream));
+        int r = run_uniform(ctx, kModeVerify, L.d_buf, tot * stride, nullptr, 0, d_mm, d_len, stride,
+                            ch.cnt, L.stream);
+        if (r) return r;
+        CU_TRY(ctx, cudaMemcpyAsync(mismatch + ch.s0, d_mm, ch.cnt * 4, cudaMemcpyDeviceToHost, L.stream));
+        return GARAGE_EC_OK;
+    });
+    return rc ? rc : p.drain();
 }
 
 int garage_ec_verify(garage_ec_ctx *ctx, const uint8_t *shards, uint32_t *mismatch,
@@ -1368,42 +1434,34 @@ static int run_deep_check(garage_ec_ctx *ctx, const uint8_t *shards, const uint3
 static int deep_check_host(garage_ec_ctx *ctx, const uint8_t *shards, const uint32_t *block_len, const uint8_t *hashes,
                            uint8_t *hash_bad, uint32_t *mismatch, size_t stride, size_t n)
 {
-    CopyBatch up;  // declared before the lane lease: it must outlive the stream work the lease waits for
-    LEASE_LANES(ctx, lanes);
     const size_t tot = ctx->k + ctx->m;
-    size_t cs = kHostChunkBytes / (tot * stride);
-    if (cs < 1) cs = 1;
-    if (cs > n) cs = n;
-    // small buffer layout per lane: block_len | hashes | shard_len | mismatch | hash_bad
-    const size_t o_blen = 0, o_hash = align_up(cs * 4, 16), o_sl = o_hash + cs * 32, o_mm = o_sl + align_up(cs * 4, 16);
-    const size_t o_bad = o_mm + align_up(cs * 4, 16), small = o_bad + align_up(cs, 16);
-    for (HostLane &L : lanes.set->lanes) {
-        int rc = lane_reserve(ctx, L, cs * tot * stride, small);
-        if (rc) return rc;
-    }
-    size_t c = 0;
-    for (size_t s0 = 0; s0 < n; s0 += cs, c++) {
-        HostLane &L = lanes[c % kHostLanes];
-        const size_t cnt = n - s0 < cs ? n - s0 : cs;
-        for (size_t s = s0; s < s0 + cnt; s++) {
+    HostPipeline p(ctx, n, tot * stride);
+    SmallLayout sl;
+    const size_t o_blen = sl.take(p.cs * 4), o_hash = sl.take(p.cs * 32), o_sl = sl.take(p.cs * 4),
+                 o_mm = sl.take(p.cs * 4), o_bad = sl.take(p.cs);
+    int rc = p.reserve(p.cs * tot * stride, sl.bytes);
+    if (rc) return rc;
+    rc = p.run([&](const HostChunk &ch) -> int {
+        HostLane &L = *ch.L;
+        for (size_t s = ch.s0; s < ch.s0 + ch.cnt; s++) {
             const size_t bytes = align_up(code_shard_len(ctx, block_len[s]), 16);
             for (size_t i = 0; i < tot; i++)
-                up.add(L.d_buf + ((s - s0) * tot + i) * stride, shards + (s * tot + i) * stride, bytes);
+                p.up.add(L.d_buf + ((s - ch.s0) * tot + i) * stride, shards + (s * tot + i) * stride, bytes);
         }
-        int rc = up.flush(ctx, cudaMemcpyHostToDevice, L.stream);
-        if (rc) return rc;
-        CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_blen, block_len + s0, cnt * 4, cudaMemcpyHostToDevice, L.stream));
-        CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_hash, hashes + s0 * 32, cnt * 32, cudaMemcpyHostToDevice, L.stream));
+        int r = p.up.flush(ctx, cudaMemcpyHostToDevice, L.stream);
+        if (r) return r;
+        CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_blen, block_len + ch.s0, ch.cnt * 4, cudaMemcpyHostToDevice, L.stream));
+        CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_hash, hashes + ch.s0 * 32, ch.cnt * 32, cudaMemcpyHostToDevice, L.stream));
         uint32_t *d_mm = reinterpret_cast<uint32_t *>(L.d_small + o_mm);
-        rc = run_deep_check(ctx, L.d_buf, reinterpret_cast<const uint32_t *>(L.d_small + o_blen), L.d_small + o_hash,
-                            L.d_small + o_bad, d_mm, reinterpret_cast<uint32_t *>(L.d_small + o_sl), stride, cnt,
-                            L.stream);
-        if (rc) return rc;
-        CU_TRY(ctx, cudaMemcpyAsync(hash_bad + s0, L.d_small + o_bad, cnt, cudaMemcpyDeviceToHost, L.stream));
-        CU_TRY(ctx, cudaMemcpyAsync(mismatch + s0, d_mm, cnt * 4, cudaMemcpyDeviceToHost, L.stream));
-    }
-    for (HostLane &L : lanes.set->lanes) CU_TRY(ctx, lane_wait(ctx, L));
-    return GARAGE_EC_OK;
+        r = run_deep_check(ctx, L.d_buf, reinterpret_cast<const uint32_t *>(L.d_small + o_blen), L.d_small + o_hash,
+                           L.d_small + o_bad, d_mm, reinterpret_cast<uint32_t *>(L.d_small + o_sl), stride, ch.cnt,
+                           L.stream);
+        if (r) return r;
+        CU_TRY(ctx, cudaMemcpyAsync(hash_bad + ch.s0, L.d_small + o_bad, ch.cnt, cudaMemcpyDeviceToHost, L.stream));
+        CU_TRY(ctx, cudaMemcpyAsync(mismatch + ch.s0, d_mm, ch.cnt * 4, cudaMemcpyDeviceToHost, L.stream));
+        return GARAGE_EC_OK;
+    });
+    return rc ? rc : p.drain();
 }
 
 int garage_ec_deep_check(garage_ec_ctx *ctx, const uint8_t *shards, const uint32_t *block_len, const uint8_t *hashes,
@@ -1429,15 +1487,10 @@ int garage_ec_deep_check(garage_ec_ctx *ctx, const uint8_t *shards, const uint32
         return GARAGE_EC_E_ALIGN;
     CU_TRY(ctx, cudaSetDevice(ctx->device));
     cudaStream_t st = (cudaStream_t)cuda_stream;
-    void *scratch = nullptr;
-    CU_TRY(ctx, ctx->pool ? cudaMallocFromPoolAsync(&scratch, n_stripes * 4, ctx->pool, st)
-                          : cudaMallocAsync(&scratch, n_stripes * 4, st));
-    rc = run_deep_check(ctx, shards, block_len, hashes, hash_bad, mismatch, reinterpret_cast<uint32_t *>(scratch),
-                        stride, n_stripes, st);
-    cudaError_t e = cudaFreeAsync(scratch, st);
-    if (rc) return rc;
-    if (e != cudaSuccess) return set_cuda_error(ctx, e, "cudaFreeAsync");
-    return GARAGE_EC_OK;
+    return with_stream_scratch(ctx, n_stripes * 4, st, [&](uint8_t *scratch) {
+        return run_deep_check(ctx, shards, block_len, hashes, hash_bad, mismatch, reinterpret_cast<uint32_t *>(scratch),
+                              stride, n_stripes, st);
+    });
 }
 
 // --------------------------------------------------------------------------- RECONSTRUCT
@@ -1448,66 +1501,27 @@ static int reconstruct_host(garage_ec_ctx *ctx, uint8_t *shards, uint8_t *const 
                             const uint8_t *want, int32_t *status, const uint32_t *shard_len,
                             size_t stride, size_t n)
 {
-    auto shard_at = [&](size_t s, size_t i) -> uint8_t * {
-        return stripes ? stripes[s] + i * stride : shards + (s * (size_t)(ctx->k + ctx->m) + i) * stride;
-    };
-    // declared before the lane lease: they must outlive the stream work the lease waits for
-    std::vector<int32_t> st_host(status ? 0 : n);
-    CopyBatch up, down;
-    LEASE_LANES(ctx, lanes);
-    if (ctx->zero_copy_rec && !ctx->clay && !stripes && device_addressable_host(shards)) {
-        // the kernel reads the k survivors of every stripe and writes the rebuilt shards in the caller's pinned buffer
-        const size_t tot_ = ctx->k + ctx->m;
-        const size_t zo_present = 0, zo_want = align_up(n * tot_, 16), zo_status = zo_want + align_up(n * tot_, 16);
-        const size_t zo_len = zo_status + align_up(n * 4, 16), zo_plan = zo_len + align_up(n * 4, 16);
-        HostLane &L = lanes[0];
-        int rcz = lane_reserve(ctx, L, 0, zo_plan + plan_scratch_bytes(ctx, n));
-        if (rcz) return rcz;
-        CU_TRY(ctx, cudaMemcpyAsync(L.d_small + zo_present, present, n * tot_, cudaMemcpyHostToDevice, L.stream));
-        const uint8_t *d_want = nullptr;
-        if (want) {
-            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + zo_want, want, n * tot_, cudaMemcpyHostToDevice, L.stream));
-            d_want = L.d_small + zo_want;
-        }
-        const uint32_t *d_len = nullptr;
-        if (shard_len) {
-            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + zo_len, shard_len, n * 4, cudaMemcpyHostToDevice, L.stream));
-            d_len = reinterpret_cast<const uint32_t *>(L.d_small + zo_len);
-        }
-        StripePlan *d_plan = reinterpret_cast<StripePlan *>(L.d_small + zo_plan);
-        uint32_t *d_counter = reinterpret_cast<uint32_t *>(L.d_small + zo_plan + n * sizeof(StripePlan));
-        rcz = run_reconstruct(ctx, shards, L.d_small + zo_present, d_want, reinterpret_cast<int32_t *>(L.d_small + zo_status), d_len,
-                              stride, n, d_plan, d_counter, L.stream);
-        if (rcz) return rcz;
-        int32_t *st_o = status ? status : st_host.data();
-        CU_TRY(ctx, cudaMemcpyAsync(st_o, L.d_small + zo_status, n * 4, cudaMemcpyDeviceToHost, L.stream));
-        CU_TRY(ctx, lane_wait(ctx, L));
-        for (size_t s = 0; s < n; s++)
-            if (st_o[s] != 0) return GARAGE_EC_E_UNRECOVERABLE;
-        return GARAGE_EC_OK;
-    }
     const size_t tot = ctx->k + ctx->m;
-    size_t cs = kHostChunkBytes / (tot * stride);
-    if (cs < 1) cs = 1;
-    if (cs > n) cs = n;
-    std::vector<uint8_t> rec_ok(cs);  // per stripe of the chunk: stripe_read_set succeeded
-    // small buffer layout per lane: present | want | status | shard_len | plan+counter
-    const size_t o_present = 0, o_want = align_up(cs * tot, 16), o_status = o_want + align_up(cs * tot, 16);
-    const size_t o_len = o_status + align_up(cs * 4, 16), o_plan = o_len + align_up(cs * 4, 16);
-    const size_t small = o_plan + plan_scratch_bytes(ctx, cs);
-    for (HostLane &L : lanes.set->lanes) {
-        int rc = lane_reserve(ctx, L, cs * tot * stride, small);
-        if (rc) return rc;
-    }
-    int32_t *st_out = status ? status : st_host.data();
-    int rc = GARAGE_EC_OK;
-    size_t c = 0;
-    for (size_t s0 = 0; s0 < n; s0 += cs, c++) {
-        HostLane &L = lanes[c % kHostLanes];
-        const size_t cnt = n - s0 < cs ? n - s0 : cs;
-        uint8_t *d_sh = L.d_buf;
+    auto shard_at = [&](size_t s, size_t i) -> uint8_t * {
+        return stripes ? stripes[s] + i * stride : shards + (s * tot + i) * stride;
+    };
+    // pinned (device-addressable) buffer: one chunk of all n stripes, in which the kernel reads the survivors from, and
+    // writes the rebuilt shards into, the caller's buffer over PCIe -- nothing staged
+    const bool zero_copy = !ctx->clay && !stripes && device_addressable_host(shards);
+    HostPipeline p(ctx, n, zero_copy ? 0 : tot * stride);
+    SmallLayout sl;
+    const size_t o_present = sl.take(p.cs * tot), o_want = sl.take(p.cs * tot), o_status = sl.take(p.cs * 4),
+                 o_len = sl.take(p.cs * 4), o_plan = sl.take(plan_scratch_bytes(ctx, p.cs));
+    int rc = p.reserve(zero_copy ? 0 : p.cs * tot * stride, sl.bytes);
+    if (rc) return rc;
+    int32_t *st_out = p.status_out(status);
+    std::vector<uint8_t> rec_ok(p.cs);  // per stripe of the chunk: stripe_read_set succeeded
+    rc = p.run([&](const HostChunk &ch) -> int {
+        HostLane &L = *ch.L;
+        const size_t s0 = ch.s0, cnt = ch.cnt;
+        uint8_t *d_sh = zero_copy ? shards : L.d_buf;
         // H2D: only the survivors the kernel reads (stripe_read_set) of stripes that have work to do
-        for (size_t s = s0; s < s0 + cnt; s++) {
+        for (size_t s = s0; s < s0 + cnt && !zero_copy; s++) {
             uint64_t hv = 0;
             bool work = false;  // a wanted shard is absent
             for (size_t i = 0; i < tot; i++) work |= !present[s * tot + i] && (!want || want[s * tot + i]);
@@ -1516,11 +1530,11 @@ static int reconstruct_host(garage_ec_ctx *ctx, uint8_t *shards, uint8_t *const 
             const size_t len = shard_len ? shard_len[s] : stride;
             for (size_t i = 0; i < tot; i++)
                 for_each_read_piece(ctx, hv, i, len, stride, [&](size_t off, size_t bytes) {
-                    up.add(d_sh + ((s - s0) * tot + i) * stride + off, shard_at(s, i) + off, bytes);
+                    p.up.add(d_sh + ((s - s0) * tot + i) * stride + off, shard_at(s, i) + off, bytes);
                 });
         }
-        rc = up.flush(ctx, cudaMemcpyHostToDevice, L.stream);
-        if (rc) return rc;
+        int r = p.up.flush(ctx, cudaMemcpyHostToDevice, L.stream);
+        if (r) return r;
         CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_present, present + s0 * tot, cnt * tot,
                                     cudaMemcpyHostToDevice, L.stream));
         const uint8_t *d_want = nullptr;
@@ -1535,29 +1549,26 @@ static int reconstruct_host(garage_ec_ctx *ctx, uint8_t *shards, uint8_t *const 
                                         L.stream));
             d_len = reinterpret_cast<const uint32_t *>(L.d_small + o_len);
         }
-        StripePlan *d_plan = reinterpret_cast<StripePlan *>(L.d_small + o_plan);
-        uint32_t *d_counter = reinterpret_cast<uint32_t *>(L.d_small + o_plan + cnt * sizeof(StripePlan));
-        rc = run_reconstruct(ctx, d_sh, L.d_small + o_present, d_want,
-                             reinterpret_cast<int32_t *>(L.d_small + o_status), d_len, stride, cnt,
-                             d_plan, d_counter, L.stream);
-        if (rc) return rc;
+        r = run_reconstruct(ctx, d_sh, L.d_small + o_present, d_want, reinterpret_cast<int32_t *>(L.d_small + o_status),
+                            d_len, stride, cnt, L.d_small + o_plan, L.stream);
+        if (r) return r;
         CU_TRY(ctx, cudaMemcpyAsync(st_out + s0, L.d_small + o_status, cnt * 4, cudaMemcpyDeviceToHost,
                                     L.stream));
         // D2H: exactly the shards that were rebuilt
-        for (size_t s = s0; s < s0 + cnt; s++) {
+        for (size_t s = s0; s < s0 + cnt && !zero_copy; s++) {
             const uint8_t *pr = present + s * tot;
             if (!rec_ok[s - s0]) continue;
             const size_t len = shard_len ? shard_len[s] : stride;
             const size_t bytes = align_up(len, 16);
             for (size_t i = 0; i < tot; i++) {
                 if (pr[i] || (want && !want[s * tot + i])) continue;
-                down.add(shard_at(s, i), d_sh + ((s - s0) * tot + i) * stride, bytes);
+                p.down.add(shard_at(s, i), d_sh + ((s - s0) * tot + i) * stride, bytes);
             }
         }
-        rc = down.flush(ctx, cudaMemcpyDeviceToHost, L.stream);
-        if (rc) return rc;
-    }
-    for (HostLane &L : lanes.set->lanes) CU_TRY(ctx, lane_wait(ctx, L));
+        return p.down.flush(ctx, cudaMemcpyDeviceToHost, L.stream);
+    });
+    if (!rc) rc = p.drain();
+    if (rc) return rc;
     for (size_t s = 0; s < n; s++)
         if (st_out[s] != 0) return GARAGE_EC_E_UNRECOVERABLE;
     return GARAGE_EC_OK;
@@ -1579,17 +1590,9 @@ int garage_ec_reconstruct(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *pr
     if (mem_kind == GARAGE_EC_MEM_HOST)
         return reconstruct_host(ctx, shards, nullptr, present, want, status, shard_len, stride, n_stripes);
     cudaStream_t st = (cudaStream_t)cuda_stream;
-    void *scratch = nullptr;
-    CU_TRY(ctx, ctx->pool ? cudaMallocFromPoolAsync(&scratch, plan_scratch_bytes(ctx, n_stripes), ctx->pool, st)
-                          : cudaMallocAsync(&scratch, plan_scratch_bytes(ctx, n_stripes), st));
-    StripePlan *plan = reinterpret_cast<StripePlan *>(scratch);
-    uint32_t *counter =
-        reinterpret_cast<uint32_t *>(reinterpret_cast<uint8_t *>(scratch) + n_stripes * sizeof(StripePlan));
-    rc = run_reconstruct(ctx, shards, present, want, status, shard_len, stride, n_stripes, plan, counter, st);
-    cudaError_t e = cudaFreeAsync(scratch, st);
-    if (rc) return rc;
-    if (e != cudaSuccess) return set_cuda_error(ctx, e, "cudaFreeAsync");
-    return GARAGE_EC_OK;
+    return with_stream_scratch(ctx, plan_scratch_bytes(ctx, n_stripes), st, [&](uint8_t *scratch) {
+        return run_reconstruct(ctx, shards, present, want, status, shard_len, stride, n_stripes, scratch, st);
+    });
 }
 
 int garage_ec_reconstruct_stripes(garage_ec_ctx *ctx, uint8_t *const *stripes, const uint8_t *present,
@@ -1676,20 +1679,15 @@ static int sums_common(garage_ec_ctx *ctx, const uint8_t *shards, const uint8_t 
         return run_sums(ctx, shards, expect, shard_len, stride, n * per, per, sums_out, bad_out,
                         (cudaStream_t)cuda_stream);
     // HOST: chunked through the lanes (H2D shards [+ expect], kernel, D2H sums / bad flags)
-    LEASE_LANES(ctx, lanes);
-    size_t cs = kHostChunkBytes / ((size_t)per * stride);
-    if (cs < 1) cs = 1;
-    if (cs > n) cs = n;
-    const size_t o_len = 0, o_exp = align_up(cs * 4, 16), o_sum = o_exp + cs * per * 32, o_bad = o_sum + cs * per * 32;
-    const size_t small = o_bad + align_up(cs * per, 16);
-    for (HostLane &L : lanes.set->lanes) {
-        rc = lane_reserve(ctx, L, cs * per * stride, small);
-        if (rc) return rc;
-    }
-    size_t c = 0;
-    for (size_t s0 = 0; s0 < n; s0 += cs, c++) {
-        HostLane &L = lanes[c % kHostLanes];
-        const size_t cnt = n - s0 < cs ? n - s0 : cs;
+    HostPipeline p(ctx, n, (size_t)per * stride);
+    SmallLayout sl;
+    const size_t o_len = sl.take(p.cs * 4), o_exp = sl.take(p.cs * per * 32), o_sum = sl.take(p.cs * per * 32),
+                 o_bad = sl.take(p.cs * per);
+    rc = p.reserve(p.cs * per * stride, sl.bytes);
+    if (rc) return rc;
+    rc = p.run([&](const HostChunk &ch) -> int {
+        HostLane &L = *ch.L;
+        const size_t s0 = ch.s0, cnt = ch.cnt;
         CU_TRY(ctx, cudaMemcpyAsync(L.d_buf, shards + s0 * per * stride, cnt * per * stride, cudaMemcpyHostToDevice,
                                     L.stream));
         const uint32_t *d_len = nullptr;
@@ -1703,18 +1701,18 @@ static int sums_common(garage_ec_ctx *ctx, const uint8_t *shards, const uint8_t 
                                         cudaMemcpyHostToDevice, L.stream));
             d_exp = L.d_small + o_exp;
         }
-        rc = run_sums(ctx, L.d_buf, d_exp, d_len, stride, cnt * per, per, sums_out ? L.d_small + o_sum : nullptr,
-                      bad_out ? L.d_small + o_bad : nullptr, L.stream);
-        if (rc) return rc;
+        int r = run_sums(ctx, L.d_buf, d_exp, d_len, stride, cnt * per, per, sums_out ? L.d_small + o_sum : nullptr,
+                         bad_out ? L.d_small + o_bad : nullptr, L.stream);
+        if (r) return r;
         if (sums_out)
             CU_TRY(ctx, cudaMemcpyAsync(sums_out + s0 * per * 32, L.d_small + o_sum, cnt * per * 32,
                                         cudaMemcpyDeviceToHost, L.stream));
         if (bad_out)
             CU_TRY(ctx, cudaMemcpyAsync(bad_out + s0 * per, L.d_small + o_bad, cnt * per, cudaMemcpyDeviceToHost,
                                         L.stream));
-    }
-    for (HostLane &L : lanes.set->lanes) CU_TRY(ctx, lane_wait(ctx, L));
-    return GARAGE_EC_OK;
+        return GARAGE_EC_OK;
+    });
+    return rc ? rc : p.drain();
 }
 
 int garage_ec_shard_sums(garage_ec_ctx *ctx, const uint8_t *shards, const uint32_t *shard_len, size_t stride,
@@ -1914,92 +1912,58 @@ int garage_ec_scrub_repair(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *e
         cudaStream_t st = (cudaStream_t)cuda_stream;
         rc = run_sums(ctx, shards, expect_sums, shard_len, stride, n_stripes * tot, (int)tot, nullptr, bad_out, st);
         if (rc) return rc;
-        void *scratch = nullptr;
-        CU_TRY(ctx, ctx->pool ? cudaMallocFromPoolAsync(&scratch, plan_scratch_bytes(ctx, n_stripes), ctx->pool, st)
-                          : cudaMallocAsync(&scratch, plan_scratch_bytes(ctx, n_stripes), st));
-        StripePlan *plan = reinterpret_cast<StripePlan *>(scratch);
-        uint32_t *counter =
-            reinterpret_cast<uint32_t *>(reinterpret_cast<uint8_t *>(scratch) + n_stripes * sizeof(StripePlan));
-        rc = run_reconstruct(ctx, shards, bad_out, nullptr, status, shard_len, stride, n_stripes, plan, counter, st,
-                             /*present_is_bad=*/true);
-        cudaError_t e = cudaFreeAsync(scratch, st);
-        if (rc) return rc;
-        if (e != cudaSuccess) return set_cuda_error(ctx, e, "cudaFreeAsync");
-        return GARAGE_EC_OK;
+        return with_stream_scratch(ctx, plan_scratch_bytes(ctx, n_stripes), st, [&](uint8_t *scratch) {
+            return run_reconstruct(ctx, shards, bad_out, nullptr, status, shard_len, stride, n_stripes, scratch, st,
+                                   /*present_is_bad=*/true);
+        });
     }
     // HOST: every shard goes up (it has to be hashed); only the rebuilt shards come back.  The
-    // rebuilt set is known once the bad flags are on the host, so each lane's chunk is finished
+    // rebuilt set is known once the bad flags are on the host, so each lane's chunk is retired
     // (flags read, copies issued) when the lane comes round again.
-    std::vector<int32_t> st_host(status ? 0 : n_stripes);  // outlives the lane lease below
-    CopyBatch down;
-    LEASE_LANES(ctx, lanes);
-    size_t cs = kHostChunkBytes / (tot * stride);
-    if (cs < 1) cs = 1;
-    if (cs > n_stripes) cs = n_stripes;
-    const size_t o_exp = 0, o_bad = o_exp + cs * tot * 32, o_status = o_bad + align_up(cs * tot, 16);
-    const size_t o_len = o_status + align_up(cs * 4, 16), o_plan = o_len + align_up(cs * 4, 16);
-    const size_t small = o_plan + plan_scratch_bytes(ctx, cs);
-    for (HostLane &L : lanes.set->lanes) {
-        rc = lane_reserve(ctx, L, cs * tot * stride, small);
-        if (rc) return rc;
-    }
-    int32_t *st_out = status ? status : st_host.data();
-    struct Pending {
-        bool active = false;
-        size_t s0 = 0, cnt = 0;
-    } pend[kHostLanes];
-    auto finish = [&](size_t lane_i) -> int {
-        Pending &P = pend[lane_i];
-        if (!P.active) return GARAGE_EC_OK;
-        HostLane &L = lanes[lane_i];
-        CU_TRY(ctx, lane_wait(ctx, L));  // bad flags + status of this chunk are on the host
-        for (size_t s = P.s0; s < P.s0 + P.cnt; s++) {
+    HostPipeline p(ctx, n_stripes, tot * stride);
+    SmallLayout sl;
+    const size_t o_exp = sl.take(p.cs * tot * 32), o_bad = sl.take(p.cs * tot), o_status = sl.take(p.cs * 4),
+                 o_len = sl.take(p.cs * 4), o_plan = sl.take(plan_scratch_bytes(ctx, p.cs));
+    rc = p.reserve(p.cs * tot * stride, sl.bytes);
+    if (rc) return rc;
+    int32_t *st_out = p.status_out(status);
+    const Retire retire = [&](const HostChunk &ch) -> int {  // bad flags + status of this chunk are on the host
+        for (size_t s = ch.s0; s < ch.s0 + ch.cnt; s++) {
             if (st_out[s] != 0) continue;
             const size_t len = shard_len ? shard_len[s] : stride;
             for (size_t i = 0; i < tot; i++)
                 if (bad_out[s * tot + i])
-                    down.add(shards + (s * tot + i) * stride, L.d_buf + ((s - P.s0) * tot + i) * stride,
-                             align_up(len, 16));
+                    p.down.add(shards + (s * tot + i) * stride, ch.L->d_buf + ((s - ch.s0) * tot + i) * stride,
+                               align_up(len, 16));
         }
-        int r = down.flush(ctx, cudaMemcpyDeviceToHost, L.stream);
-        P.active = false;
-        return r;
+        return p.down.flush(ctx, cudaMemcpyDeviceToHost, ch.L->stream);
     };
-    size_t c = 0;
-    for (size_t s0 = 0; s0 < n_stripes; s0 += cs, c++) {
-        const size_t lane_i = c % kHostLanes;
-        HostLane &L = lanes[lane_i];
-        rc = finish(lane_i);
-        if (rc) return rc;
-        const size_t cnt = n_stripes - s0 < cs ? n_stripes - s0 : cs;
-        CU_TRY(ctx, cudaMemcpyAsync(L.d_buf, shards + s0 * tot * stride, cnt * tot * stride, cudaMemcpyHostToDevice,
-                                    L.stream));
-        CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_exp, expect_sums + s0 * tot * 32, cnt * tot * 32,
-                                    cudaMemcpyHostToDevice, L.stream));
-        const uint32_t *d_len = nullptr;
-        if (shard_len) {
-            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_len, shard_len + s0, cnt * 4, cudaMemcpyHostToDevice, L.stream));
-            d_len = reinterpret_cast<const uint32_t *>(L.d_small + o_len);
-        }
-        rc = run_sums(ctx, L.d_buf, L.d_small + o_exp, d_len, stride, cnt * tot, (int)tot, nullptr, L.d_small + o_bad,
-                      L.stream);
-        if (rc) return rc;
-        StripePlan *d_plan = reinterpret_cast<StripePlan *>(L.d_small + o_plan);
-        uint32_t *d_counter = reinterpret_cast<uint32_t *>(L.d_small + o_plan + cnt * sizeof(StripePlan));
-        rc = run_reconstruct(ctx, L.d_buf, L.d_small + o_bad, nullptr, reinterpret_cast<int32_t *>(L.d_small + o_status),
-                             d_len, stride, cnt, d_plan, d_counter, L.stream, true);
-        if (rc) return rc;
-        CU_TRY(ctx, cudaMemcpyAsync(bad_out + s0 * tot, L.d_small + o_bad, cnt * tot, cudaMemcpyDeviceToHost, L.stream));
-        CU_TRY(ctx, cudaMemcpyAsync(st_out + s0, L.d_small + o_status, cnt * 4, cudaMemcpyDeviceToHost, L.stream));
-        pend[lane_i].active = true;
-        pend[lane_i].s0 = s0;
-        pend[lane_i].cnt = cnt;
-    }
-    for (size_t l = 0; l < (size_t)kHostLanes; l++) {
-        rc = finish(l);
-        if (rc) return rc;
-    }
-    for (HostLane &L : lanes.set->lanes) CU_TRY(ctx, lane_wait(ctx, L));
+    rc = p.run(
+        [&](const HostChunk &ch) -> int {
+            HostLane &L = *ch.L;
+            const size_t s0 = ch.s0, cnt = ch.cnt;
+            CU_TRY(ctx, cudaMemcpyAsync(L.d_buf, shards + s0 * tot * stride, cnt * tot * stride, cudaMemcpyHostToDevice,
+                                        L.stream));
+            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_exp, expect_sums + s0 * tot * 32, cnt * tot * 32,
+                                        cudaMemcpyHostToDevice, L.stream));
+            const uint32_t *d_len = nullptr;
+            if (shard_len) {
+                CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_len, shard_len + s0, cnt * 4, cudaMemcpyHostToDevice, L.stream));
+                d_len = reinterpret_cast<const uint32_t *>(L.d_small + o_len);
+            }
+            int r = run_sums(ctx, L.d_buf, L.d_small + o_exp, d_len, stride, cnt * tot, (int)tot, nullptr,
+                             L.d_small + o_bad, L.stream);
+            if (r) return r;
+            r = run_reconstruct(ctx, L.d_buf, L.d_small + o_bad, nullptr, reinterpret_cast<int32_t *>(L.d_small + o_status),
+                                d_len, stride, cnt, L.d_small + o_plan, L.stream, true);
+            if (r) return r;
+            CU_TRY(ctx, cudaMemcpyAsync(bad_out + s0 * tot, L.d_small + o_bad, cnt * tot, cudaMemcpyDeviceToHost, L.stream));
+            CU_TRY(ctx, cudaMemcpyAsync(st_out + s0, L.d_small + o_status, cnt * 4, cudaMemcpyDeviceToHost, L.stream));
+            return GARAGE_EC_OK;
+        },
+        retire);
+    if (!rc) rc = p.drain(retire);
+    if (rc) return rc;
     for (size_t s = 0; s < n_stripes; s++)
         if (st_out[s] != 0) return GARAGE_EC_E_UNRECOVERABLE;
     return GARAGE_EC_OK;
@@ -2027,50 +1991,32 @@ int garage_ec_encode_blocks_with_sums(garage_ec_ctx *ctx, const uint8_t *const *
         if (code_shard_len(ctx, block_len[s]) > stride) return GARAGE_EC_E_INVALID;
         max_len = block_len[s] > max_len ? block_len[s] : max_len;
     }
-    const auto tr0 = std::chrono::steady_clock::now();
     CU_TRY(ctx, cudaSetDevice(ctx->device));
-    size_t cs = kHostChunkBytes / (k * stride);
-    if (cs < 1) cs = 1;
-    if (cs > n_blocks) cs = n_blocks;
+    HostPipeline p(ctx, n_blocks, k * stride);
+    const size_t cs = p.cs;
     // per lane: [blocks as they arrive, contiguous, `pitch` apart][k data shards][m parity shards]
     const size_t pitch = align_up((size_t)max_len + 16, 16);  // + one aligned word of slack for the split kernel
     const size_t blk_b = align_up(cs * pitch, 256), in_b = cs * k * stride, out_b = cs * m * stride;
-    std::vector<uint32_t> lens(2 * cs * kHostLanes);  // [shard_len | block_len] per lane; outlives the lane lease below
-    CopyBatch up;
-    LEASE_LANES(ctx, lanes);
-    for (HostLane &L : lanes.set->lanes) {
-        rc = lane_reserve(ctx, L, blk_b + in_b + out_b, align_up(cs * 8, 16) + cs * (k + m) * 32);
-        if (rc) return rc;
-    }
-    const size_t o_blen = cs * 4, o_sums = align_up(cs * 8, 16);
-    const auto tr1 = std::chrono::steady_clock::now();
-    cudaEvent_t tev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-    if (ctx->trace)
-        for (auto &e : tev) cudaEventCreate(&e);
-    auto mark = [&](int i, size_t chunk, cudaStream_t st) {
-        if (ctx->trace && chunk == 0 && tev[i]) cudaEventRecord(tev[i], st);
-    };
-    size_t c = 0;
-    for (size_t s0 = 0; s0 < n_blocks; s0 += cs, c++) {
-        const size_t lane_i = c % kHostLanes;
-        HostLane &L = lanes[lane_i];
-        const size_t cnt = n_blocks - s0 < cs ? n_blocks - s0 : cs;
-        // the pageable `lens` slot of this lane is reused: wait for the lane's previous chunk
-        if (c >= (size_t)kHostLanes) CU_TRY(ctx, lane_wait(ctx, L));
-        mark(0, c, L.stream);
-        uint32_t *hl = lens.data() + lane_i * 2 * cs, *hb = hl + cs;
+    // small: [shard_len | block_len] (staged through the lane's pageable slot of the same layout) | tags
+    SmallLayout sl;
+    const size_t o_lens = sl.take(cs * 8), o_blen = o_lens + cs * 4, o_sums = sl.take(cs * (k + m) * 32);
+    rc = p.reserve(blk_b + in_b + out_b, sl.bytes, cs * 8);
+    if (rc) return rc;
+    rc = p.run([&](const HostChunk &ch) -> int {
+        HostLane &L = *ch.L;
+        const size_t s0 = ch.s0, cnt = ch.cnt;
+        uint32_t *hl = reinterpret_cast<uint32_t *>(ch.host), *hb = hl + cs;
         uint8_t *d_blk = L.d_buf, *d_data = L.d_buf + blk_b, *d_par = d_data + in_b;
         for (size_t s = 0; s < cnt; s++) {
             hl[s] = code_shard_len(ctx, block_len[s0 + s]);
             hb[s] = block_len[s0 + s];
             // H2D: the block as ONE contiguous copy; the framing happens on the device
-            up.add(d_blk + s * pitch, blocks[s0 + s], block_len[s0 + s]);
+            p.up.add(d_blk + s * pitch, blocks[s0 + s], block_len[s0 + s]);
         }
-        rc = up.flush(ctx, cudaMemcpyHostToDevice, L.stream);
-        if (rc) return rc;
-        CU_TRY(ctx, cudaMemcpyAsync(L.d_small, hl, cnt * 4, cudaMemcpyHostToDevice, L.stream));
+        int r = p.up.flush(ctx, cudaMemcpyHostToDevice, L.stream);
+        if (r) return r;
+        CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_lens, hl, cnt * 4, cudaMemcpyHostToDevice, L.stream));
         CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_blen, hb, cnt * 4, cudaMemcpyHostToDevice, L.stream));
-        mark(1, c, L.stream);
         SplitParams sp;
         sp.blocks = d_blk;
         sp.block_len = reinterpret_cast<const uint32_t *>(L.d_small + o_blen);
@@ -2085,43 +2031,21 @@ int garage_ec_encode_blocks_with_sums(garage_ec_ctx *ctx, const uint8_t *const *
         split_blocks_kernel<<<(unsigned)std::min<size_t>(cnt * sp.parts, (size_t)ctx->sm_count * 8), 256, 0, L.stream>>>(sp);
         ctx->launches.fetch_add(1, std::memory_order_relaxed);
         CU_TRY(ctx, cudaGetLastError());
-        rc = run_uniform(ctx, kModeEncode, d_data, k * stride, d_par, m * stride, nullptr,
-                         reinterpret_cast<const uint32_t *>(L.d_small), stride, cnt, L.stream);
-        if (rc) return rc;
-        mark(2, c, L.stream);
+        const uint32_t *d_len = reinterpret_cast<const uint32_t *>(L.d_small + o_lens);
+        r = run_uniform(ctx, kModeEncode, d_data, k * stride, d_par, m * stride, nullptr, d_len, stride, cnt, L.stream);
+        if (r) return r;
         CU_TRY(ctx, cudaMemcpyAsync(parity_out + s0 * m * stride, d_par, cnt * m * stride, cudaMemcpyDeviceToHost, L.stream));
-        mark(3, c, L.stream);
         if (sums_out) {
             // per-shard tags of all k+m shards while they are on the device (row f2): [s][k+m][32]
-            const uint32_t *d_len = reinterpret_cast<const uint32_t *>(L.d_small);
-            rc = run_sums(ctx, d_data, nullptr, d_len, stride, cnt * k, (int)k, L.d_small + o_sums, nullptr, L.stream,
-                          (int)(k + m), 0, d_par, cnt * m, (int)m, (int)k);
-            if (rc) return rc;
+            r = run_sums(ctx, d_data, nullptr, d_len, stride, cnt * k, (int)k, L.d_small + o_sums, nullptr, L.stream,
+                         (int)(k + m), 0, d_par, cnt * m, (int)m, (int)k);
+            if (r) return r;
             CU_TRY(ctx, cudaMemcpyAsync(sums_out + s0 * (k + m) * 32, L.d_small + o_sums, cnt * (k + m) * 32,
                                         cudaMemcpyDeviceToHost, L.stream));
         }
-        mark(4, c, L.stream);
-    }
-    const auto tr2 = std::chrono::steady_clock::now();
-    for (HostLane &L : lanes.set->lanes) CU_TRY(ctx, lane_wait(ctx, L));
-    if (ctx->trace) {
-        const auto tr3 = std::chrono::steady_clock::now();
-        auto us = [](auto a, auto b) { return (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(b - a).count(); };
-        ctx->tr_calls++;
-        ctx->tr_blocks += n_blocks;
-        ctx->tr_prep_us += us(tr0, tr1);
-        ctx->tr_issue_us += us(tr1, tr2);
-        ctx->tr_sync_us += us(tr2, tr3);
-        for (int i = 0; i < 4; i++) {
-            float ms = 0;
-            if (tev[i] && tev[i + 1] && cudaEventElapsedTime(&ms, tev[i], tev[i + 1]) == cudaSuccess)
-                ctx->tr_gpu_ns[i] += (uint64_t)(ms * 1e6);
-        }
-        (void)cudaGetLastError();
-        for (auto e : tev)
-            if (e) cudaEventDestroy(e);  // (an error return above leaks them: trace mode is a tuning aid only)
-    }
-    return GARAGE_EC_OK;
+        return GARAGE_EC_OK;
+    });
+    return rc ? rc : p.drain();
 }
 
 int garage_ec_decode_blocks(garage_ec_ctx *ctx, const uint8_t *shards, const uint8_t *present,
@@ -2158,96 +2082,65 @@ int garage_ec_decode_blocks(garage_ec_ctx *ctx, const uint8_t *shards, const uin
         if (status) status[s] = 0;
         if (data_missing) need.push_back(s);
     }
-    size_t cs = kHostChunkBytes / (tot * stride);
-    if (cs < 1) cs = 1;
-    if (!need.empty()) {
-        if (cs > need.size()) cs = need.size();
-        const size_t o_present = 0, o_want = align_up(cs * tot, 16), o_status = o_want + align_up(cs * tot, 16);
-        const size_t o_len = o_status + align_up(cs * 4, 16), o_plan = o_len + align_up(cs * 4, 16);
-        const size_t small = o_plan + plan_scratch_bytes(ctx, cs);
-        // host staging and copy lists are declared before the lane lease: they outlive its stream work
-        std::vector<uint8_t> h_small((2 * cs * tot + cs * 4) * kHostLanes);
-        CopyBatch up, down;
-        LEASE_LANES(ctx, lanes);
-        for (HostLane &L : lanes.set->lanes) {
-            rc = lane_reserve(ctx, L, cs * tot * stride, small);
-            if (rc) return rc;
+    // the data-shard pieces of block s (framing: block = shard0|shard1|...), as f(j, offset in the block, bytes)
+    auto for_each_data_piece = [&](size_t s, auto &&f) {
+        const size_t Ls = code_shard_len(ctx, block_len[s]);
+        for (size_t j = 0; j < k && j * Ls < block_len[s]; j++) f(j, j * Ls, std::min<size_t>(block_len[s] - j * Ls, Ls));
+    };
+    HostPipeline p(ctx, need.size(), tot * stride);
+    const size_t cs = p.cs;
+    SmallLayout sl;
+    const size_t o_present = sl.take(cs * tot), o_want = sl.take(cs * tot), o_status = sl.take(cs * 4),
+                 o_len = sl.take(cs * 4), o_plan = sl.take(plan_scratch_bytes(ctx, cs));
+    // pageable staging per lane: shard_len | present | want
+    rc = p.reserve(cs * tot * stride, sl.bytes, cs * 4 + 2 * cs * tot);
+    if (rc) return rc;
+    rc = p.run([&](const HostChunk &ch) -> int {
+        HostLane &L = *ch.L;
+        const size_t q0 = ch.s0, cnt = ch.cnt;
+        uint32_t *hl = reinterpret_cast<uint32_t *>(ch.host);
+        uint8_t *hp = ch.host + cs * 4, *hw = hp + cs * tot;
+        for (size_t q = 0; q < cnt; q++) {
+            const size_t s = need[q0 + q];
+            memcpy(hp + q * tot, present + s * tot, tot);
+            memcpy(hw + q * tot, want_data.data(), tot);  // data shards only
+            hl[q] = code_shard_len(ctx, block_len[s]);
+            // H2D: only the survivors the kernel reads -- the GET path is PCIe-bound, absent and
+            // surplus shards stay on the host
+            for (size_t i = 0; i < tot; i++)
+                for_each_read_piece(ctx, reads[s], i, hl[q], align_up(hl[q], 16), [&](size_t off, size_t bytes) {
+                    p.up.add(L.d_buf + (q * tot + i) * stride + off, shards + (s * tot + i) * stride + off, bytes);
+                });
         }
-        size_t c = 0;
-        for (size_t q0 = 0; q0 < need.size(); q0 += cs, c++) {
-            const size_t lane_i = c % kHostLanes;
-            HostLane &L = lanes[lane_i];
-            const size_t cnt = need.size() - q0 < cs ? need.size() - q0 : cs;
-            if (c >= (size_t)kHostLanes) CU_TRY(ctx, lane_wait(ctx, L));
-            uint8_t *hp = h_small.data() + lane_i * (2 * cs * tot + cs * 4);
-            uint8_t *hw = hp + cs * tot;
-            uint32_t *hl = reinterpret_cast<uint32_t *>(hw + cs * tot);
-            for (size_t q = 0; q < cnt; q++) {
-                const size_t s = need[q0 + q];
-                memcpy(hp + q * tot, present + s * tot, tot);
-                for (size_t i = 0; i < tot; i++) hw[q * tot + i] = i < k ? 1 : 0;  // data shards only
-                hl[q] = code_shard_len(ctx, block_len[s]);
-                // H2D: only the survivors the kernel reads -- the GET path is PCIe-bound, absent and
-                // surplus shards stay on the host
-                for (size_t i = 0; i < tot; i++)
-                    for_each_read_piece(ctx, reads[s], i, hl[q], align_up(hl[q], 16), [&](size_t off, size_t bytes) {
-                        up.add(L.d_buf + (q * tot + i) * stride + off, shards + (s * tot + i) * stride + off, bytes);
-                    });
-            }
-            rc = up.flush(ctx, cudaMemcpyHostToDevice, L.stream);
-            if (rc) return rc;
-            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_present, hp, cnt * tot, cudaMemcpyHostToDevice, L.stream));
-            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_want, hw, cnt * tot, cudaMemcpyHostToDevice, L.stream));
-            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_len, hl, cnt * 4, cudaMemcpyHostToDevice, L.stream));
-            StripePlan *d_plan = reinterpret_cast<StripePlan *>(L.d_small + o_plan);
-            uint32_t *d_counter = reinterpret_cast<uint32_t *>(L.d_small + o_plan + cnt * sizeof(StripePlan));
-            rc = run_reconstruct(ctx, L.d_buf, L.d_small + o_present, L.d_small + o_want,
-                                 reinterpret_cast<int32_t *>(L.d_small + o_status),
-                                 reinterpret_cast<const uint32_t *>(L.d_small + o_len), stride, cnt, d_plan,
-                                 d_counter, L.stream);
-            if (rc) return rc;
-            // rebuilt data shards land directly in the output blocks
-            for (size_t q = 0; q < cnt; q++) {
-                const size_t s = need[q0 + q];
-                const size_t Ls = hl[q];
-                for (size_t j = 0; j < k; j++) {
-                    if (present[s * tot + j]) continue;
-                    const size_t off = j * Ls;
-                    if (off >= block_len[s]) continue;
-                    const size_t have = block_len[s] - off < Ls ? block_len[s] - off : Ls;
-                    down.add(blocks_out[s] + off, L.d_buf + (q * tot + j) * stride, have);
-                }
-            }
-            rc = down.flush(ctx, cudaMemcpyDeviceToHost, L.stream);
-            if (rc) return rc;
+        int r = p.up.flush(ctx, cudaMemcpyHostToDevice, L.stream);
+        if (r) return r;
+        CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_present, hp, cnt * tot, cudaMemcpyHostToDevice, L.stream));
+        CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_want, hw, cnt * tot, cudaMemcpyHostToDevice, L.stream));
+        CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_len, hl, cnt * 4, cudaMemcpyHostToDevice, L.stream));
+        r = run_reconstruct(ctx, L.d_buf, L.d_small + o_present, L.d_small + o_want,
+                            reinterpret_cast<int32_t *>(L.d_small + o_status),
+                            reinterpret_cast<const uint32_t *>(L.d_small + o_len), stride, cnt, L.d_small + o_plan,
+                            L.stream);
+        if (r) return r;
+        // rebuilt data shards land directly in the output blocks
+        for (size_t q = 0; q < cnt; q++) {
+            const size_t s = need[q0 + q];
+            for_each_data_piece(s, [&](size_t j, size_t off, size_t bytes) {
+                if (!present[s * tot + j]) p.down.add(blocks_out[s] + off, L.d_buf + (q * tot + j) * stride, bytes);
+            });
         }
-        // host-side join of the data shards that did arrive, while the GPU works
-        // (framing: block = shard0|shard1|...)
-        for (size_t s = 0; s < n_blocks; s++) {
-            const uint8_t *pr = present + s * tot;
-            if (!ok[s]) continue;
-            const size_t Ls = code_shard_len(ctx, block_len[s]);
-            for (size_t j = 0; j < k; j++) {
-                if (!pr[j]) continue;
-                const size_t off = j * Ls;
-                if (off >= block_len[s]) continue;
-                const size_t have = block_len[s] - off < Ls ? block_len[s] - off : Ls;
-                memcpy(blocks_out[s] + off, shards + (s * tot + j) * stride, have);
-            }
-        }
-        for (HostLane &L : lanes.set->lanes) CU_TRY(ctx, lane_wait(ctx, L));
-        return any_bad ? GARAGE_EC_E_UNRECOVERABLE : GARAGE_EC_OK;
-    }
+        return p.down.flush(ctx, cudaMemcpyDeviceToHost, L.stream);
+    });
+    if (rc) return rc;
+    // host-side join of the data shards that did arrive, while the GPU works
     for (size_t s = 0; s < n_blocks; s++) {
         if (!ok[s]) continue;
-        const size_t Ls = code_shard_len(ctx, block_len[s]);
-        for (size_t j = 0; j < k; j++) {
-            const size_t off = j * Ls;
-            if (off >= block_len[s]) continue;
-            const size_t have = block_len[s] - off < Ls ? block_len[s] - off : Ls;
-            memcpy(blocks_out[s] + off, shards + (s * tot + j) * stride, have);
-        }
+        for_each_data_piece(s, [&](size_t j, size_t off, size_t bytes) {
+            if (present[s * tot + j]) memcpy(blocks_out[s] + off, shards + (s * tot + j) * stride, bytes);
+        });
     }
+    rc = p.drain();
+    if (rc) return rc;
     return any_bad ? GARAGE_EC_E_UNRECOVERABLE : GARAGE_EC_OK;
 }
 
@@ -2309,9 +2202,7 @@ int run_transcode(garage_ec_ctx *dst, garage_ec_ctx *src, uint8_t *s_sh, size_t 
         uint8_t *want = scratch + L.o_want;
         CU_TRY(dst, cudaMemsetAsync(want, 0, n * s_tot, st));
         CU_TRY(dst, cudaMemset2DAsync(want, s_tot, 1, q.ks, n, st));
-        StripePlan *plan = reinterpret_cast<StripePlan *>(scratch + L.o_plan);
-        uint32_t *counter = reinterpret_cast<uint32_t *>(scratch + L.o_plan + n * sizeof(StripePlan));
-        int rc = run_reconstruct(src, s_sh, present, want, q.status, q.src_len, s_stride, n, plan, counter, st);
+        int rc = run_reconstruct(src, s_sh, present, want, q.status, q.src_len, s_stride, n, scratch + L.o_plan, st);
         if (rc) return rc;
     }
     {
@@ -2345,24 +2236,18 @@ int transcode_host(garage_ec_ctx *dst, garage_ec_ctx *src, const uint8_t *src_sh
         if (degraded[s]) ok[s] = stripe_read_plan(src, pr, want_data.data(), &reads[s]);
     }
     auto src_len = [&](size_t s) -> size_t { return src ? (size_t)code_shard_len(src, block_len[s]) : block_len[s]; };
-    size_t cs = kHostChunkBytes / (s_tot * s_stride + d_tot * d_stride);
-    if (cs < 1) cs = 1;
-    if (cs > n) cs = n;
-    const size_t o_len = 0, o_present = align_up(cs * 4, 16), o_status = o_present + align_up(cs * s_tot, 16);
-    const size_t o_sums = o_status + align_up(cs * 4, 16), o_scr = o_sums + (dst_sums ? cs * d_tot * 32 : 0);
+    HostPipeline p(dst, n, s_tot * s_stride + d_tot * d_stride);
+    const size_t cs = p.cs;
     const TranscodeScratch scr(src, cs, s_tot, src_present != nullptr);
+    SmallLayout sl;
+    const size_t o_len = sl.take(cs * 4), o_present = sl.take(cs * s_tot), o_status = sl.take(cs * 4),
+                 o_sums = sl.take(dst_sums ? cs * d_tot * 32 : 0), o_scr = sl.take(scr.bytes);
     const size_t d_src_b = cs * s_tot * s_stride;
-    // copy lists are declared before the lane lease: they outlive its stream work
-    CopyBatch up, down;
-    LEASE_LANES(dst, lanes);
-    for (HostLane &Ln : lanes.set->lanes) {
-        int rc = lane_reserve(dst, Ln, d_src_b + cs * d_tot * d_stride, o_scr + scr.bytes);
-        if (rc) return rc;
-    }
-    size_t c = 0;
-    for (size_t s0 = 0; s0 < n; s0 += cs, c++) {
-        HostLane &Ln = lanes[c % kHostLanes];
-        const size_t cnt = n - s0 < cs ? n - s0 : cs;
+    int rc = p.reserve(d_src_b + cs * d_tot * d_stride, sl.bytes);
+    if (rc) return rc;
+    rc = p.run([&](const HostChunk &ch) -> int {
+        HostLane &Ln = *ch.L;
+        const size_t s0 = ch.s0, cnt = ch.cnt;
         uint8_t *d_src = Ln.d_buf, *d_dst = Ln.d_buf + d_src_b;
         bool any_degraded = false;
         for (size_t s = s0; s < s0 + cnt; s++) {
@@ -2373,15 +2258,15 @@ int transcode_host(garage_ec_ctx *dst, garage_ec_ctx *src, const uint8_t *src_sh
                 const uint8_t *from = src_shards + (s * s_tot + i) * s_stride;
                 uint8_t *to = d_src + (q * s_tot + i) * s_stride;
                 if (i < ks) {
-                    if (!src_present || src_present[s * s_tot + i]) up.add(to, from, align_up(Ls, 16));
+                    if (!src_present || src_present[s * s_tot + i]) p.up.add(to, from, align_up(Ls, 16));
                 } else if (degraded[s]) {
                     for_each_read_piece(src, reads[s], i, Ls, align_up(Ls, 16),
-                                        [&](size_t off, size_t bytes) { up.add(to + off, from + off, bytes); });
+                                        [&](size_t off, size_t bytes) { p.up.add(to + off, from + off, bytes); });
                 }
             }
         }
-        int rc = up.flush(dst, cudaMemcpyHostToDevice, Ln.stream);
-        if (rc) return rc;
+        int r = p.up.flush(dst, cudaMemcpyHostToDevice, Ln.stream);
+        if (r) return r;
         CU_TRY(dst, cudaMemcpyAsync(Ln.d_small + o_len, block_len + s0, cnt * 4, cudaMemcpyHostToDevice, Ln.stream));
         const uint8_t *d_present = nullptr;
         if (any_degraded) {
@@ -2389,21 +2274,21 @@ int transcode_host(garage_ec_ctx *dst, garage_ec_ctx *src, const uint8_t *src_sh
                                         Ln.stream));
             d_present = Ln.d_small + o_present;
         }
-        rc = run_transcode(dst, src, d_src, s_stride, d_present, reinterpret_cast<const uint32_t *>(Ln.d_small + o_len), d_dst,
-                           d_stride, dst_sums ? Ln.d_small + o_sums : nullptr,
-                           reinterpret_cast<int32_t *>(Ln.d_small + o_status), cnt, Ln.d_small + o_scr, Ln.stream);
-        if (rc) return rc;
+        r = run_transcode(dst, src, d_src, s_stride, d_present, reinterpret_cast<const uint32_t *>(Ln.d_small + o_len), d_dst,
+                          d_stride, dst_sums ? Ln.d_small + o_sums : nullptr,
+                          reinterpret_cast<int32_t *>(Ln.d_small + o_status), cnt, Ln.d_small + o_scr, Ln.stream);
+        if (r) return r;
         for (size_t s = s0; s < s0 + cnt; s++) {
             if (!ok[s]) continue;
             const size_t bytes = align_up(code_shard_len(dst, block_len[s]), 16), q = s - s0;
             for (size_t i = 0; i < d_tot; i++)
-                down.add(dst_shards + (s * d_tot + i) * d_stride, d_dst + (q * d_tot + i) * d_stride, bytes);
-            if (dst_sums) down.add(dst_sums + s * d_tot * 32, Ln.d_small + o_sums + q * d_tot * 32, d_tot * 32);
+                p.down.add(dst_shards + (s * d_tot + i) * d_stride, d_dst + (q * d_tot + i) * d_stride, bytes);
+            if (dst_sums) p.down.add(dst_sums + s * d_tot * 32, Ln.d_small + o_sums + q * d_tot * 32, d_tot * 32);
         }
-        rc = down.flush(dst, cudaMemcpyDeviceToHost, Ln.stream);
-        if (rc) return rc;
-    }
-    for (HostLane &Ln : lanes.set->lanes) CU_TRY(dst, lane_wait(dst, Ln));
+        return p.down.flush(dst, cudaMemcpyDeviceToHost, Ln.stream);
+    });
+    if (!rc) rc = p.drain();
+    if (rc) return rc;
     bool any_bad = false;
     for (size_t s = 0; s < n; s++) {
         if (status) status[s] = ok[s] ? 0 : GARAGE_EC_E_UNRECOVERABLE;
@@ -2442,14 +2327,10 @@ int garage_ec_transcode(garage_ec_ctx *dst, garage_ec_ctx *src, uint8_t *src_sha
     CU_TRY(dst, cudaSetDevice(dst->device));
     cudaStream_t st = (cudaStream_t)cuda_stream;
     const TranscodeScratch scr(src, n_stripes, src ? src->k + src->m : 1, src_present != nullptr);
-    void *scratch = nullptr;
-    CU_TRY(dst, dst->pool ? cudaMallocFromPoolAsync(&scratch, scr.bytes, dst->pool, st) : cudaMallocAsync(&scratch, scr.bytes, st));
-    rc = run_transcode(dst, src, src_shards, src_stride, src_present, block_len, dst_shards, dst_stride, dst_sums, status,
-                       n_stripes, reinterpret_cast<uint8_t *>(scratch), st);
-    cudaError_t e = cudaFreeAsync(scratch, st);
-    if (rc) return rc;
-    if (e != cudaSuccess) return set_cuda_error(dst, e, "cudaFreeAsync");
-    return GARAGE_EC_OK;
+    return with_stream_scratch(dst, scr.bytes, st, [&](uint8_t *scratch) {
+        return run_transcode(dst, src, src_shards, src_stride, src_present, block_len, dst_shards, dst_stride, dst_sums,
+                             status, n_stripes, scratch, st);
+    });
 }
 
 // ---- test hook -------------------------------------------------------------------------------

@@ -5,6 +5,7 @@ and the survivors-only upload of garage_ec_decode_blocks.
 Reference convention mirrored: blocks are bytes::Bytes owned by the caller and every error is a
 Result (src/util/error.rs:14-82); a Rust caller frees its Vec on Err, so a DMA that is still in
 flight after an error return would be a use-after-free."""
+import contextlib
 import os
 import sys
 import threading
@@ -151,6 +152,151 @@ def test_block_level_host_fault(torch):
         assert ec.decode_blocks(shards.reshape(-1), present, blens, stride, out, st) == 0
         for s in range(n):
             assert np.array_equal(out[s], blocks[s]), s
+
+
+@pytest.fixture(scope="module")
+def big_case():
+    """RS(10,4), 240 stripes of 14 x 104960 bytes: 8 chunks of 48 MB"""
+    k, m, stride, n = 10, 4, 104960, 240
+    _, _, sh = _case(k, m, n, stride, 1618)
+    present = np.ones((n, k + m), dtype=np.uint8)
+    rng = np.random.default_rng(21)
+    for s in range(n):
+        present[s, rng.choice(k + m, m, replace=False)] = 0
+    return k, m, stride, n, sh, present
+
+
+# Each entry: (ec, case, stack) -> (run, outputs, reset, check).  run() makes the HOST call, `outputs` are the caller's
+# arrays it writes, reset() restores the inputs a run consumes and check() asserts the exact result; `stack` (an
+# ExitStack) frees what the entry allocates.
+def _verify_call(ec, case, stack):
+    k, m, stride, n, sh, _ = case
+    work = sh.copy()
+    work[37, k + 1, 11] ^= 1
+    mm = np.zeros(n, dtype=np.uint32)
+
+    def check():
+        assert np.flatnonzero(mm).tolist() == [37]
+
+    return lambda: ec.verify(work.reshape(-1), mm, stride, n), [mm], lambda: None, check
+
+
+def _deep_check_call(ec, case, stack):
+    k, m, stride, n, sh, _ = case
+    work = sh.copy()
+    work[37, k + 1, 11] ^= 1
+    blen = np.full(n, k * stride, dtype=np.uint32)
+    hashes = np.stack([np.frombuffer(G.blake2sum(sh[s, :k].reshape(-1)), dtype=np.uint8) for s in range(n)])
+    hashes[5, 0] ^= 1
+    bad = np.zeros(n, dtype=np.uint8)
+    mm = np.zeros(n, dtype=np.uint32)
+
+    def check():
+        assert np.flatnonzero(bad).tolist() == [5] and np.flatnonzero(mm).tolist() == [37]
+
+    return lambda: ec.deep_check(work.reshape(-1), blen, hashes, bad, mm, stride, n), [bad, mm], lambda: None, check
+
+
+def _shard_sums_call(ec, case, stack):
+    k, m, stride, n, sh, _ = case
+    tot = k + m
+    sums = np.zeros((n, tot, 32), dtype=np.uint8)
+
+    def check():
+        for s in (0, n // 2, n - 1):
+            for i in range(tot):
+                assert sums[s, i].tobytes() == G.blake2sum(sh[s, i]), (s, i)
+
+    return lambda: ec.shard_sums(sh.reshape(-1), sums, stride, n, tot), [sums], lambda: None, check
+
+
+def _check_sums_call(ec, case, stack):
+    k, m, stride, n, sh, _ = case
+    tot = k + m
+    expect = np.zeros(n * tot * 32, dtype=np.uint8)
+    ec.shard_sums(sh.reshape(-1), expect, stride, n, tot)
+    work = sh.copy()
+    work[100, 3, 7] ^= 1
+    bad = np.zeros(n * tot, dtype=np.uint8)
+
+    def check():
+        assert np.flatnonzero(bad).tolist() == [100 * tot + 3]
+
+    return lambda: ec.check_sums(work.reshape(-1), expect, bad, stride, n, tot), [bad], lambda: None, check
+
+
+def _reconstruct_stripes_call(ec, case, stack):
+    k, m, stride, n, sh, present = case
+    work = sh.copy()
+    stripes = [work[s] for s in range(n)]
+    st = np.zeros(n, dtype=np.int32)
+
+    def reset():
+        work[:] = sh
+        work[present == 0] = 0
+
+    def check():
+        assert np.array_equal(work, sh) and not st.any()
+
+    return lambda: ec.reconstruct_stripes(stripes, present, stride, status=st), [work, st], reset, check
+
+
+def _reconstruct_pinned_call(ec, case, stack):
+    """pinned buffer: the zero-copy reconstruct (one launch over the caller's buffer, no staging)"""
+    k, m, stride, n, sh, present = case
+    buf, p = ec.host_alloc(n * (k + m) * stride)
+    stack.callback(ec.host_free, p)
+    v = buf.reshape(n, k + m, stride)
+    want = np.ones((n, k + m), dtype=np.uint8)
+    lens = np.full(n, stride, dtype=np.uint32)
+    st = np.zeros(n, dtype=np.int32)
+
+    def reset():
+        v[:] = sh
+        v[present == 0] = 0x77
+
+    def check():
+        assert np.array_equal(v, sh) and not st.any()
+
+    def run():
+        return ec.reconstruct(buf, present, stride, n, want=want, status=st, shard_len=lens)
+
+    return run, [buf, st], reset, check
+
+
+_FAULT_CALLS = {
+    "verify": _verify_call,
+    "deep_check": _deep_check_call,
+    "shard_sums": _shard_sums_call,
+    "check_sums": _check_sums_call,
+    "reconstruct_stripes": _reconstruct_stripes_call,
+    "reconstruct_pinned": _reconstruct_pinned_call,
+}
+
+
+@pytest.mark.parametrize("fail_at", [0, 1, 3, 5])
+@pytest.mark.parametrize("call", sorted(_FAULT_CALLS))
+def test_host_call_fault_leaves_caller_buffers_alone(torch, big_case, call, fail_at):
+    """the HOST entry points the tests above do not cover, same contract: after an injected fault's error return
+    nothing writes the caller's output buffers any more, and the context still computes exact results"""
+    k, m = big_case[:2]
+    with G.GarageEc(0, k, m) as ec, contextlib.ExitStack() as stack:
+        run, outs, reset, check = _FAULT_CALLS[call](ec, big_case, stack)
+        reset()
+        run()  # lanes sized, streams created
+        check()
+        reset()
+        ec.debug_fail_after(fail_at)
+        with pytest.raises(G.EcError):
+            run()
+        ec.debug_fail_after(-1)
+        for o in outs:
+            o.view(np.uint8)[...] = 0xEE
+        torch.cuda.synchronize()
+        assert all((o.view(np.uint8) == 0xEE).all() for o in outs), "a copy or kernel wrote after the error return"
+        reset()
+        run()
+        check()
 
 
 def test_decode_blocks_uploads_survivors_only(torch):
