@@ -265,6 +265,57 @@ std::string hex_of(const uint8_t *p, size_t n)
 
 enum ReadResult { kReadOk = 0, kReadMissing = 1, kReadInvalid = 2 };
 
+// the header of the shard file at `path`: kReadMissing (no such file), kReadInvalid (short, or a wrong magic or header
+// check) or kReadOk.  keep != NULL: on kReadOk the open file is handed over there, positioned after the header
+ReadResult read_header(const std::string &path, ShardFileHeader &hd, FILE **keep = nullptr)
+{
+    FILE *f = path.empty() ? nullptr : fopen(path.c_str(), "rb");  // find_block (manager.rs:627-662)
+    if (!f) return kReadMissing;
+    const bool ok = fread(&hd, sizeof(hd), 1, f) == 1 && memcmp(hd.magic, "GEC1", 4) == 0 &&
+                    hd.hdr_check == adler32_small(reinterpret_cast<const uint8_t *>(&hd), 48);
+    if (ok && keep) *keep = f;
+    else fclose(f);
+    return ok ? kReadOk : kReadInvalid;
+}
+
+bool fsync_dir(const std::string &dir)
+{
+    const int dfd = ::open(dir.c_str(), O_RDONLY | O_DIRECTORY);
+    if (dfd < 0) return false;
+    const bool ok = ::fsync(dfd) == 0;
+    ::close(dfd);
+    return ok;
+}
+
+// the whole file at `path` into `out`; false if it cannot be opened
+bool read_file(const std::string &path, std::string &out)
+{
+    FILE *f = fopen(path.c_str(), "rb");
+    if (!f) return false;
+    char buf[65536];
+    for (size_t r; (r = fread(buf, 1, sizeof(buf), f)) > 0;) out.append(buf, r);
+    fclose(f);
+    return true;
+}
+
+// `path` replaced atomically by a[0, na) + b[0, nb): a temporary file, fsynced if `fsync_file`, renamed over `path`
+// (manager.rs:790-795), then the directory entry fsynced if `fsync_entry` (manager.rs:797-803).  A directory that
+// cannot be opened for that fsync fails the write.  The temporary file goes on failure.
+bool write_file_atomic(const std::string &path, const void *a, size_t na, const void *b, size_t nb, bool fsync_file,
+                       bool fsync_entry)
+{
+    const std::string tmp = path + ".tmp" + std::to_string((unsigned long)::getpid());
+    FILE *f = fopen(tmp.c_str(), "wb");
+    if (!f) return false;
+    bool ok = (na == 0 || fwrite(a, na, 1, f) == 1) && (nb == 0 || fwrite(b, nb, 1, f) == 1) && fflush(f) == 0;
+    if (ok && fsync_file) ok = ::fsync(fileno(f)) == 0;  // manager.rs:775-777
+    ok = (fclose(f) == 0) && ok;
+    if (ok) ok = ::rename(tmp.c_str(), path.c_str()) == 0;
+    if (ok && fsync_entry) ok = fsync_dir(std::filesystem::path(path).parent_path().string());
+    if (!ok) ::remove(tmp.c_str());
+    return ok;
+}
+
 // a code shards are stored under: RS(k, m), LRC(k, l, m - l) or PB(k, m)
 struct CodeDesc {
     int k = 0, m = 0, l = 0;  // l: LRC local groups, 0 = RS
@@ -284,8 +335,6 @@ struct Node {
     bool up = true;
     bool fsync_data = false;  // data_fsync (util/config.rs), manager.rs:775-789
     std::string dir;          // empty: in-memory store
-    int k = 0, m = 0, l = 0;  // the configured code (codes[0])
-    bool pb = false;
     std::vector<CodeDesc> codes;  // [0] the configured code, then garage_bm_config.previous_codes (file store only)
     bool replicas = false;        // legacy_replicas > 0: whole-block replica files are read, listed and converted
     // the store has a layout file (DESIGN.md section 5.2): a node may hold two indices of a block, the newest version's
@@ -300,11 +349,20 @@ struct Node {
     std::deque<Hash> resync_queue;                                // block_local_resync_queue (resync.rs:90)
     std::unordered_set<Hash, HashHasher> queued;
 
-    std::string path_of(const Hash &h, const char *ext) const
+    // Node is the only owner of the file scheme: the names below, the header and the placement rules of DESIGN.md
+    // sections 5.1 / 5.2.  The files of one hash, by ShardFile:
+    enum ShardFile { kShardFile = 0, kLegacyFile = 1, kReplicaFile = 2 };
+    static constexpr const char *kExt[3] = {".shard", ".legacy", ""};
+    std::string dir_of(const Hash &h) const { return dir + "/" + hex_of(h.data(), 1) + "/" + hex_of(h.data() + 1, 1); }
+    std::string path_of(const Hash &h, const char *ext) const { return dir_of(h) + "/" + hex_of(h.data(), 32) + ext; }
+    // previous codes or replicas are configured (a file store changing its code)
+    bool legacy_store() const { return codes.size() >= 2 || replicas; }
+    // in-memory: the copy was made by the caller; the shard it replaces is returned, to be freed outside the lock
+    ShardPtr store_put_ptr(const Hash &h, ShardPtr sp)
     {
-        return dir + "/" + hex_of(h.data(), 1) + "/" + hex_of(h.data() + 1, 1) + "/" + hex_of(h.data(), 32) + ext;
+        shards[h].swap(sp);
+        return sp;
     }
-    void store_put_ptr(const Hash &h, ShardPtr sp) { shards[h] = std::move(sp); }  // in-memory: the copy was made by the caller
     ShardPtr store_find(const Hash &h) const
     {
         auto it = shards.find(h);
@@ -322,16 +380,12 @@ struct Node {
     // file does not exist
     int file_code(const std::string &path) const
     {
-        FILE *f = fopen(path.c_str(), "rb");
-        if (!f) return -2;
         ShardFileHeader hd;
-        int c = -1;
-        if (fread(&hd, sizeof(hd), 1, f) == 1 && memcmp(hd.magic, "GEC1", 4) == 0 &&
-            hd.hdr_check == adler32_small(reinterpret_cast<const uint8_t *>(&hd), 48))
-            for (size_t i = 0; i < codes.size() && c < 0; i++)
-                if (codes[i].named_by(hd)) c = (int)i;
-        fclose(f);
-        return c;
+        const ReadResult r = read_header(path, hd);
+        if (r == kReadMissing) return -2;
+        for (size_t i = 0; r == kReadOk && i < codes.size(); i++)
+            if (codes[i].named_by(hd)) return (int)i;
+        return -1;
     }
     // the file holding this node's shard of `code` ("" = none).  The configured code lives in .shard; a shard of a
     // previous code in .shard (written before the code changed) or .legacy.  A file whose header names no listed code
@@ -347,19 +401,15 @@ struct Node {
         const int c2 = file_code(lg);
         return c2 == code || c2 == -1 ? lg : std::string();
     }
+    bool has_code(const Hash &h, int code) const { return !path_for(h, code).empty(); }
     // the shard index a configured-code file's header names: -1 for another code or a damaged header, -2 if the file
     // does not exist
     int file_index(const std::string &path) const
     {
-        FILE *f = fopen(path.c_str(), "rb");
-        if (!f) return -2;
         ShardFileHeader hd;
-        int i = -1;
-        if (fread(&hd, sizeof(hd), 1, f) == 1 && memcmp(hd.magic, "GEC1", 4) == 0 &&
-            hd.hdr_check == adler32_small(reinterpret_cast<const uint8_t *>(&hd), 48) && codes[0].named_by(hd))
-            i = hd.index;
-        fclose(f);
-        return i;
+        const ReadResult r = read_header(path, hd);
+        if (r == kReadMissing) return -2;
+        return r == kReadOk && codes[0].named_by(hd) ? hd.index : -1;
     }
     // the file holding shard `index` of h ("" = none): .shard or .legacy, whichever header names that index
     std::string path_at(const Hash &h, int index) const
@@ -368,16 +418,24 @@ struct Node {
         if (file_index(sh) == index) return sh;
         return file_index(lg) == index ? lg : std::string();
     }
-    // where shard `index` of h goes when the newest layout version gives this node `newest` (-1: none).  .shard holds
-    // the newest index, or the only one the node holds; *aside = .shard must first move to .legacy.
-    const char *place_for(const Hash &h, int index, int newest, bool *aside) const
+    // by_index stores: h's configured-code files whose index is not `keep`, as (extension, index)
+    std::vector<std::pair<const char *, int>> other_index_files(const Hash &h, int keep) const
     {
-        const int si = file_index(path_of(h, ".shard"));
-        *aside = false;
-        if (si < 0 || si == index) return ".shard";
-        if (index != newest) return ".legacy";
-        *aside = true;
-        return ".shard";
+        std::vector<std::pair<const char *, int>> r;
+        if (dir.empty() || !by_index) return r;
+        for (const char *ext : {".shard", ".legacy"}) {
+            const int i = file_index(path_of(h, ext));
+            if (i >= 0 && i != keep) r.emplace_back(ext, i);
+        }
+        return r;
+    }
+    // those files removed, allow() gating each removal; the number removed
+    int erase_other_indices(const Hash &h, int keep, const std::function<bool()> &allow)
+    {
+        int n = 0;
+        for (auto &f : other_index_files(h, keep))
+            if (allow() && ::remove(path_of(h, f.first).c_str()) == 0) n++;
+        return n;
     }
     bool has_legacy_shard(const Hash &h) const
     {
@@ -389,24 +447,6 @@ struct Node {
     {
         struct stat sb;
         return replicas && ::stat(path_of(h, "").c_str(), &sb) == 0 && S_ISREG(sb.st_mode);
-    }
-    bool fsync_dir_of(const Hash &h) const
-    {
-        const int dfd = ::open((dir + "/" + hex_of(h.data(), 1) + "/" + hex_of(h.data() + 1, 1)).c_str(), O_RDONLY | O_DIRECTORY);
-        if (dfd < 0) return false;
-        const bool ok = ::fsync(dfd) == 0;
-        ::close(dfd);
-        return ok;
-    }
-    // before a configured-code shard takes the .shard name: a previous code's shard there moves to .legacy
-    // (atomic rename, then the directory entry under data_fsync).  false if that failed: nothing may be written then.
-    bool store_move_legacy_aside(const Hash &h)
-    {
-        if (dir.empty() || codes.size() < 2) return true;
-        const std::string sh = path_of(h, ".shard");
-        if (file_code(sh) < 1) return true;
-        if (::rename(sh.c_str(), path_of(h, ".legacy").c_str()) != 0) return false;
-        return !fsync_data || fsync_dir_of(h);
     }
     // this node's legacy copies of h (a previous code's shard, the replica): removed, their number returned
     int store_erase_legacy(const Hash &h, const std::function<bool()> &allow)
@@ -436,50 +476,46 @@ struct Node {
         fclose(f);
         return r;
     }
-    void replica_quarantine(const Hash &h) { ::rename(path_of(h, "").c_str(), path_of(h, ".corrupted").c_str()); }
-    bool store_put(const Hash &h, const ShardMeta &mt, const uint8_t *bytes, size_t n, const char *ext = ".shard")
+    // Shard mt.index of h (n bytes) stored under the configured code; the file store writes it atomically.  .shard
+    // first moves to .legacy (an atomic rename, then the directory entry under data_fsync) when it holds a previous
+    // code's shard (DESIGN.md section 5.1), or, in a by_index store, another index while the one written is `newest`,
+    // the index the newest layout version gives this node; an older index is written to .legacy instead (section
+    // 5.2).  allow() gates the move and the write, one file operation each.  false: the write did not happen.
+    bool store_put(const Hash &h, const ShardMeta &mt, const uint8_t *bytes, size_t n, int newest = -1,
+                   const std::function<bool()> &allow = [] { return true; })
     {
-        if (!dir.empty() && strcmp(ext, ".shard") == 0 && !store_move_legacy_aside(h)) return false;
         if (dir.empty()) {
             auto sp = std::make_shared<StoredShard>();
             static_cast<ShardMeta &>(*sp) = mt;
             sp->bytes.assign(bytes, bytes + n);
-            shards[h] = std::move(sp);
+            store_put_ptr(h, std::move(sp));
             return true;
         }
+        const std::string sh = path_of(h, ".shard");
+        const int si = by_index ? file_index(sh) : -1;
+        const bool other = si >= 0 && si != mt.index;  // .shard holds another index of h
+        const bool aside = other ? mt.index == newest : codes.size() >= 2 && file_code(sh) >= 1;
+        if (aside && !(allow() && ::rename(sh.c_str(), path_of(h, ".legacy").c_str()) == 0 &&
+                       (!fsync_data || fsync_dir(dir_of(h)))))
+            return false;
+        if (!allow()) return false;
         std::error_code ec;
-        const std::string sub = dir + "/" + hex_of(h.data(), 1) + "/" + hex_of(h.data() + 1, 1);
-        std::filesystem::create_directories(sub, ec);
-        const std::string fin = path_of(h, ext), tmp = fin + ".tmp" + std::to_string((unsigned long)::getpid());
+        std::filesystem::create_directories(dir_of(h), ec);
         ShardFileHeader hd;
         memset(&hd, 0, sizeof(hd));
         memcpy(hd.magic, "GEC1", 4);
-        hd.k = (uint8_t)k;
-        hd.m = (uint8_t)m;
+        hd.k = (uint8_t)codes[0].k;
+        hd.m = (uint8_t)codes[0].m;
         hd.index = (uint8_t)mt.index;
         hd.sum_kind = mt.sum_kind;
         hd.block_len = mt.block_len;
         hd.shard_len = (uint32_t)n;
         memcpy(hd.sum, mt.sum.data(), 32);
         hd.hdr_check = adler32_small(reinterpret_cast<const uint8_t *>(&hd), 48);
-        hd.pad[0] = (uint8_t)l;
+        hd.pad[0] = (uint8_t)codes[0].l;
         hd.pad[1] = codes[0].kind_byte();
-        FILE *f = fopen(tmp.c_str(), "wb");
-        if (!f) return false;
-        bool ok = fwrite(&hd, sizeof(hd), 1, f) == 1 && (n == 0 || fwrite(bytes, n, 1, f) == 1);
-        if (ok) ok = fflush(f) == 0;
-        if (ok && fsync_data) ok = ::fsync(fileno(f)) == 0;  // manager.rs:775-777
-        ok = (fclose(f) == 0) && ok;
-        if (ok) ok = ::rename(tmp.c_str(), fin.c_str()) == 0;  // atomic publish (manager.rs:790-795)
-        if (ok && fsync_data) {                                 // and the directory entry (manager.rs:797-803)
-            const int dfd = ::open(sub.c_str(), O_RDONLY | O_DIRECTORY);
-            if (dfd >= 0) {
-                ok = ::fsync(dfd) == 0;
-                ::close(dfd);
-            }
-        }
-        if (!ok) ::remove(tmp.c_str());
-        return ok;
+        return write_file_atomic(path_of(h, other && !aside ? ".legacy" : ".shard"), &hd, sizeof(hd), bytes, n, fsync_data,
+                                 fsync_data);
     }
     // shard bytes straight into `dst` (cap bytes available), metadata into `mt`.  half = 0 / 1: only the a- / b-half
     // [half * shard_len/2, (half+1) * shard_len/2) of a PB shard, one ranged read at 64 + half * shard_len/2 of the
@@ -499,18 +535,16 @@ struct Node {
     // one shard file read as a shard of `code`
     ReadResult file_read_into(const std::string &path, int code, uint8_t *dst, size_t cap, ShardMeta &mt, int half = -1) const
     {
-        if (path.empty()) return kReadMissing;
-        FILE *f = fopen(path.c_str(), "rb");  // find_block (manager.rs:627-662)
-        if (!f) return kReadMissing;
-        const CodeDesc &c = codes[code];
         ShardFileHeader hd;
+        FILE *f = nullptr;
+        const ReadResult hr = read_header(path, hd, &f);
+        if (hr != kReadOk) return hr;
+        const CodeDesc &c = codes[code];
         ReadResult r = kReadInvalid;
         struct stat sb;
         // a header that fails any of these is a corrupt shard, never a reason to allocate or read
         // what it claims (a flipped shard_len must not become a 4 GiB resize)
-        if (fread(&hd, sizeof(hd), 1, f) == 1 && memcmp(hd.magic, "GEC1", 4) == 0 &&
-            hd.hdr_check == adler32_small(reinterpret_cast<const uint8_t *>(&hd), 48) && c.named_by(hd) &&
-            fstat(fileno(f), &sb) == 0 && (uint64_t)sb.st_size == (uint64_t)hd.shard_len + sizeof(hd)) {
+        if (c.named_by(hd) && fstat(fileno(f), &sb) == 0 && (uint64_t)sb.st_size == (uint64_t)hd.shard_len + sizeof(hd)) {
             mt.index = hd.index;
             mt.block_len = hd.block_len;
             mt.shard_len = hd.shard_len;
@@ -534,10 +568,46 @@ struct Node {
     {
         mt = sh;
         const size_t off = half < 0 ? 0 : (size_t)half * (mt.shard_len / 2), n = half < 0 ? mt.shard_len : mt.shard_len / 2;
-        if (!meta_valid(mt) || sh.bytes.size() != mt.shard_len || n > cap || (half >= 0 && !pb)) return kReadInvalid;
+        if (!meta_valid(mt) || sh.bytes.size() != mt.shard_len || n > cap || (half >= 0 && !codes[0].pb)) return kReadInvalid;
         if (for_dma) copy_for_dma(dst, sh.bytes.data() + off, n);
         else if (n) memcpy(dst, sh.bytes.data() + off, n);
         return kReadOk;
+    }
+    // the files scrub checks for h (ShardFile values): only .shard in a store without previous codes, replicas or a
+    // layout file; otherwise each of .shard, .legacy and the replica that exists
+    std::vector<int> scrub_files(const Hash &h) const
+    {
+        if (dir.empty() || !(legacy_store() || by_index)) return {kShardFile};
+        std::vector<int> r;
+        if (file_code(path_of(h, ".shard")) != -2) r.push_back(kShardFile);
+        if (file_code(path_of(h, ".legacy")) != -2) r.push_back(kLegacyFile);
+        if (has_replica(h)) r.push_back(kReplicaFile);
+        return r;
+    }
+    // scrub's read of file (kShardFile / kLegacyFile) of h, as the code its header names.  A header naming no listed
+    // code is read as the configured code (.shard) or the first previous one (.legacy), which fails it, as before
+    // previous codes existed; a store with a layout file and no previous codes holds the configured code in both.
+    ReadResult scrub_read_into(const Hash &h, int file, uint8_t *dst, size_t cap, ShardMeta &mt) const
+    {
+        if (dir.empty() || !(legacy_store() || by_index)) return store_read_into(h, dst, cap, mt);
+        const std::string path = path_of(h, kExt[file]);
+        return file_read_into(path, legacy_store() ? std::max(file, file_code(path)) : 0, dst, cap, mt);
+    }
+    // restart: the length of block h as a readable shard of any listed code on this node gives it; unless `known`
+    // (another node gave it already), also an older layout version's index in .legacy, or the size of the replica (at
+    // most max_len).  `tmp` holds a shard of the largest code.  false: no file gives it.
+    bool block_len_of(const Hash &h, std::vector<uint8_t> &tmp, uint32_t max_len, bool known, uint32_t &len) const
+    {
+        ShardMeta mt;
+        for (int c = 0; c < (int)codes.size(); c++)
+            if (store_read_into(h, tmp.data(), tmp.size(), mt, -1, c) == kReadOk) return len = mt.block_len, true;
+        if (known) return false;
+        if (by_index && !legacy_store() && file_read_into(path_of(h, ".legacy"), 0, tmp.data(), tmp.size(), mt) == kReadOk)
+            return len = mt.block_len, true;
+        struct stat sb;
+        if (has_replica(h) && ::stat(path_of(h, "").c_str(), &sb) == 0 && sb.st_size > 0 && (uint64_t)sb.st_size <= max_len)
+            return len = (uint32_t)sb.st_size, true;
+        return false;
     }
     bool store_get(const Hash &h, StoredShard &out) const  // a copy (scrub snapshots, inspection)
     {
@@ -556,9 +626,11 @@ struct Node {
         static_cast<ShardMeta &>(out) = mt;
         return true;
     }
-    bool store_has(const Hash &h) const
+    // a configured-code shard of h is here; index >= 0: the file holding that index
+    bool store_has(const Hash &h, int index = -1) const
     {
         if (dir.empty()) return shards.count(h) != 0;
+        if (index >= 0) return !path_at(h, index).empty();
         if (codes.size() >= 2) return !path_for(h, 0).empty();
         std::error_code ec;
         return std::filesystem::exists(path_of(h, ".shard"), ec);
@@ -568,8 +640,9 @@ struct Node {
         if (dir.empty()) return shards.erase(h) != 0;
         return ::remove(path_of(h, ".shard").c_str()) == 0;
     }
-    // move_block_to_corrupted (manager.rs:807-819).  index >= 0 (by_index stores): the file holding that index
-    void store_quarantine(const Hash &h, int code = 0, int index = -1)
+    // move_block_to_corrupted (manager.rs:807-819): file >= 0 that ShardFile of h; code -1 the replica; index >= 0
+    // (by_index stores) the file holding that index; otherwise the file holding the shard of `code`
+    void store_quarantine(const Hash &h, int code = 0, int index = -1, int file = -1)
     {
         if (dir.empty()) {
             auto it = shards.find(h);
@@ -579,12 +652,53 @@ struct Node {
             }
             return;
         }
-        std::string p = index >= 0 && by_index ? path_at(h, index) : std::string();
+        std::string p;
+        if (file >= 0 || code < 0) p = path_of(h, kExt[file >= 0 ? file : kReplicaFile]);
+        else if (index >= 0 && by_index) p = path_at(h, index);
         if (p.empty()) p = codes.size() < 2 ? path_of(h, ".shard") : path_for(h, code);
         if (!p.empty()) ::rename(p.c_str(), path_of(h, ".corrupted").c_str());
     }
-    // BlockStoreIterator (repair.rs:634-764).  legacy: also hashes held only as a .legacy shard or a replica
-    void store_list(std::vector<Hash> &out, bool legacy = false) const
+    // fault injection (garage_bm_corrupt_shard*): what = 0 flips a bit of the shard's bytes at byte_off, 1 rewrites the
+    // stored block_len (+1), 2 rewrites the stored index (+1 mod k+m); the stored tag / header check are left alone in
+    // every case -- that is the corruption.
+    int store_corrupt(const Hash &h, size_t byte_off, int what)
+    {
+        if (dir.empty()) {
+            auto it = shards.find(h);
+            if (it == shards.end()) return GARAGE_BM_E_MISSING_BLOCK;
+            auto mod = std::make_shared<StoredShard>(*it->second);  // stored shards are immutable: replace by a damaged copy
+            if (what == 0) {
+                if (mod->bytes.empty()) return GARAGE_BM_E_MISSING_BLOCK;
+                mod->bytes[byte_off % mod->bytes.size()] ^= 0x01;
+            } else if (what == 1) {
+                mod->block_len += 1;
+            } else {
+                mod->index = (mod->index + 1) % (codes[0].k + codes[0].m);
+            }
+            it->second = std::move(mod);
+            return GARAGE_BM_OK;
+        }
+        FILE *f = fopen(path_of(h, ".shard").c_str(), "r+b");
+        if (!f) return GARAGE_BM_E_MISSING_BLOCK;
+        ShardFileHeader hd;
+        int rc = GARAGE_BM_E_MISSING_BLOCK;
+        if (fread(&hd, sizeof(hd), 1, f) == 1) {
+            long off = -1;
+            uint8_t b = 0;
+            if (what == 0 && hd.shard_len) off = (long)sizeof(hd) + (long)(byte_off % hd.shard_len);
+            else if (what == 1) off = offsetof(ShardFileHeader, block_len);
+            else if (what == 2) off = offsetof(ShardFileHeader, index);
+            if (off >= 0 && fseek(f, off, SEEK_SET) == 0 && fread(&b, 1, 1, f) == 1) {
+                b = what == 0 ? (uint8_t)(b ^ 1) : (uint8_t)(b + 1);
+                if (fseek(f, off, SEEK_SET) == 0 && fwrite(&b, 1, 1, f) == 1) rc = GARAGE_BM_OK;
+            }
+        }
+        fclose(f);
+        return rc;
+    }
+    // BlockStoreIterator (repair.rs:634-764): every hash this node holds a file of that it reads -- .shard, and with
+    // previous codes or a layout file .legacy, with replicas configured the replica
+    void store_list(std::vector<Hash> &out) const
     {
         if (dir.empty()) {
             for (auto &kv : shards) out.push_back(kv.first);
@@ -595,9 +709,8 @@ struct Node {
              !ec && it != std::filesystem::recursive_directory_iterator(); it.increment(ec)) {
             const std::string name = it->path().filename().string();
             const bool listed = (name.size() == 64 + 6 && name.compare(64, 6, ".shard") == 0) ||
-                                (legacy && (codes.size() >= 2 || by_index) && name.size() == 64 + 7 &&
-                                 name.compare(64, 7, ".legacy") == 0) ||
-                                (legacy && replicas && name.size() == 64 && it->is_regular_file(ec2));
+                                ((codes.size() >= 2 || by_index) && name.size() == 64 + 7 && name.compare(64, 7, ".legacy") == 0) ||
+                                (replicas && name.size() == 64 && it->is_regular_file(ec2));
             if (!listed) continue;
             Hash h;
             bool ok = true;
@@ -909,6 +1022,24 @@ struct RcEntry {
     Clock::time_point zero_since{};  // when the count last dropped to 0 (BLOCK_GC_DELAY, manager.rs:49-52)
 };
 
+// One page of a resumable sweep (the scrub iterator checkpoint, repair.rs:186-193,460-464): `hs` sorted and
+// deduplicated, then cut to the hashes after *cursor (NULL: from the start), at most `max` of them (0: all).
+// *finished: the page reaches the end; *cursor_out: its last hash (none: *cursor, or zeros from the start).
+void sweep_page(std::vector<Hash> &hs, const Hash *cursor, size_t max, Hash *cursor_out, int *finished)
+{
+    std::sort(hs.begin(), hs.end());
+    hs.erase(std::unique(hs.begin(), hs.end()), hs.end());
+    if (cursor) hs.erase(hs.begin(), std::upper_bound(hs.begin(), hs.end(), *cursor));
+    const bool done = !max || hs.size() <= max;
+    if (!done) hs.resize(max);
+    if (finished) *finished = done ? 1 : 0;
+    if (cursor_out) {
+        if (!hs.empty()) *cursor_out = hs.back();
+        else if (cursor) *cursor_out = *cursor;
+        else cursor_out->fill(0);
+    }
+}
+
 }  // namespace
 
 // ================================================================= the manager
@@ -955,7 +1086,6 @@ struct garage_bm {
     std::atomic<uint64_t> layout_shards_copied{0}, layout_shards_rebuilt{0}, layout_bytes_read{0}, layout_bytes_written{0},
         layout_deleted{0}, layout_sync_errors{0};
 
-    bool pb = false;  // PB(k, m) contexts (garage_bm_config.piggyback)
     // Bytes a rebuild from the shards `have` hands to the GPU, which is what crosses the network in Garage: the runs
     // garage_ec_read_ranges names for a Clay stripe (1/m of each helper for a lone lost shard), else what was read
     uint64_t fetched_bytes(const uint8_t *have, const uint8_t *want, uint32_t block_len, uint64_t read_bytes) const
@@ -1000,9 +1130,10 @@ struct garage_bm {
     void nodes_of(const Hash &h, int code, int *out) const
     {
         if (code == 0) return storage_nodes_of(h, out);
-        const int n = (int)nodes.size(), p = h[0] % n;
-        for (int i = 0; i < codes[code].tot; i++) out[i] = (p + i) % n;
+        for (int i = 0; i < codes[code].tot; i++) out[i] = ring_node(h, i);
     }
+    // the fixed ring: shard i of h on node (h[0] mod n) + i
+    int ring_node(const Hash &h, int i) const { return ((int)h[0] % (int)nodes.size() + i) % (int)nodes.size(); }
 
     // rpc/layout/version.rs:117-137: top 8 bits of the hash -> partition -> k+m distinct nodes, shard i on the
     // i-th of them.  Each ring is a garage_layout (row f4, include/garage_placement.h): without garage_bm_config.layout
@@ -1035,9 +1166,7 @@ struct garage_bm {
         auto ls = layouts();
         if (ls->newest() && garage_layout_nodes_of(ls->newest(), h.data(), reinterpret_cast<int32_t *>(out)) == GARAGE_LAYOUT_OK)
             return;
-        const int n = (int)nodes.size();  // more nodes than a ring row can name: the same rule, computed
-        const int p = h[0] % n;
-        for (int i = 0; i < tot; i++) out[i] = (p + i) % n;
+        for (int i = 0; i < tot; i++) out[i] = ring_node(h, i);  // more nodes than a ring row can name: the same rule
     }
     // the index the newest version gives `node` for h, -1 if none
     int newest_index(const Hash &h, int node) const
@@ -1061,9 +1190,11 @@ struct garage_bm {
         garage_ec_shard_sum_host(sum_kind, bytes, n, out.data());
     }
 
-    // manager.rs:517-530 write_block: false if the node is down or the store failed (ENOSPC, EACCES ...)
+    // manager.rs:517-530 write_block: false if the node is down or the store failed (ENOSPC, EACCES ...).  The node
+    // places the shard (Node::store_put).  counted: a conversion's or layout sync's write, whose move of another shard
+    // aside and write are each one file operation of garage_bm_debug_convert_stop_after.
     bool write_shard(int node, const Hash &h, int index, uint32_t block_len, const uint8_t *bytes, size_t n,
-                     const uint8_t *sum32)
+                     const uint8_t *sum32, bool counted = false)
     {
         ShardMeta mt;
         mt.index = index;
@@ -1072,6 +1203,7 @@ struct garage_bm {
         mt.sum_kind = (uint8_t)sum_kind;
         memcpy(mt.sum.data(), sum32, 32);
         Node &nd = *nodes[node];
+        auto allow = [&] { return !counted || convert_op_allowed(); };
         bool ok;
         if (nd.dir.empty()) {
             auto sp = std::make_shared<StoredShard>();  // the copy happens before the node lock is taken
@@ -1081,75 +1213,30 @@ struct garage_bm {
             {
                 std::lock_guard<std::mutex> lk(nd.mu);
                 if (!nd.up) return false;
-                auto &slot_ref = nd.shards[h];
-                old.swap(slot_ref);
-                slot_ref = std::move(sp);
+                ok = allow();
+                if (ok) old = nd.store_put_ptr(h, std::move(sp));
             }
-            ok = true;  // `old` (a replaced shard) is freed here, outside the lock
+            // `old` (a replaced shard) is freed here, outside the lock
         } else {
+            const int newest = nd.by_index ? newest_index(h, node) : -1;
             std::lock_guard<std::mutex> lk(nd.mu);
             if (!nd.up) return false;
-            ok = nd.store_put(h, mt, bytes, n);
-        }
-        if (ok) bytes_written += n;
-        else write_errors++;
-        return ok;
-    }
-    // write_shard on a store with a layout file: shard `index` takes the name Node::place_for gives it, after the
-    // newest version's index moved .shard aside.  counted: a layout sync's write; the rename and the write are each one
-    // file operation of garage_bm_debug_convert_stop_after.
-    bool write_shard_at(int node, const Hash &h, int index, uint32_t block_len, const uint8_t *bytes, size_t n,
-                        const uint8_t *sum32, bool counted)
-    {
-        Node &nd = *nodes[node];
-        if (nd.dir.empty() || !nd.by_index) {
-            if (counted && !convert_op_allowed()) return false;
-            return write_shard(node, h, index, block_len, bytes, n, sum32);
-        }
-        const int newest = newest_index(h, node);
-        ShardMeta mt;
-        mt.index = index;
-        mt.block_len = block_len;
-        mt.shard_len = (uint32_t)n;
-        mt.sum_kind = (uint8_t)sum_kind;
-        memcpy(mt.sum.data(), sum32, 32);
-        bool ok = true;
-        {
-            std::lock_guard<std::mutex> lk(nd.mu);
-            if (!nd.up) return false;
-            bool aside = false;
-            const char *ext = nd.place_for(h, index, newest, &aside);
-            if (aside)  // the same atomic rename (and directory fsync) as a code change's move to .legacy
-                ok = (!counted || convert_op_allowed()) &&
-                     ::rename(nd.path_of(h, ".shard").c_str(), nd.path_of(h, ".legacy").c_str()) == 0 &&
-                     (!nd.fsync_data || nd.fsync_dir_of(h));
-            ok = ok && (!counted || convert_op_allowed()) && nd.store_put(h, mt, bytes, n, ext);
+            ok = nd.store_put(h, mt, bytes, n, newest, allow);
         }
         if (ok) bytes_written += n;
         else write_errors++;
         return ok;
     }
 
-    // code -1: the node's replica of h.  index >= 0: the file holding that index (by_index stores)
-    void quarantine(int node, const Hash &h, int code = 0, int index = -1)
+    // code -1: the node's replica of h.  index >= 0: the file holding that index (by_index stores).  file >= 0: that
+    // Node::ShardFile of h
+    void quarantine(int node, const Hash &h, int code = 0, int index = -1, int file = -1)
     {
         corruption_counter++;
         {
             Node &nd = *nodes[node];
             std::lock_guard<std::mutex> lk(nd.mu);
-            if (code < 0) nd.replica_quarantine(h);
-            else nd.store_quarantine(h, code, index);
-        }
-        put_to_resync(node, h);
-    }
-    // a file scrub found bad, by name
-    void quarantine_file(int node, const Hash &h, const char *ext)
-    {
-        corruption_counter++;
-        {
-            Node &nd = *nodes[node];
-            std::lock_guard<std::mutex> lk(nd.mu);
-            ::rename(nd.path_of(h, ext).c_str(), nd.path_of(h, ".corrupted").c_str());
+            nd.store_quarantine(h, code, index, file);
         }
         put_to_resync(node, h);
     }
@@ -1158,8 +1245,10 @@ struct garage_bm {
     // A bad header or a tag mismatch quarantines the shard and queues a resync, like the reference.
     // `for_dma`: the GPU reads `dst` next (degraded GET, resync): see copy_for_dma
     // index >= 0: the node's shard of that index (several active layout versions)
+    // half = 0 / 1 (PB): one half of the shard (a ranged read of shard_len/2 bytes into dst), checked against the
+    // half's 4 adler8 segment tags (garage_ec_check_shard_half_host)
     bool read_shard_into(int node, const Hash &h, uint8_t *dst, size_t cap, ShardMeta &mt, bool for_dma = false, int code = 0,
-                         int index = -1)
+                         int index = -1, int half = -1)
     {
         Node &nd = *nodes[node];
         ReadResult r;
@@ -1171,38 +1260,8 @@ struct garage_bm {
                 if (!nd.up) return false;
                 sp = nd.store_find(h);
             }
-            r = sp ? nd.copy_out(*sp, dst, cap, mt, for_dma) : kReadMissing;  // the copy happens outside the node lock
-            if (sp && for_dma) check = sp->bytes.data();  // same bytes, and these are still in the cache
-        } else {
-            std::lock_guard<std::mutex> lk(nd.mu);
-            if (!nd.up) return false;
-            r = nd.store_read_into(h, dst, cap, mt, -1, code, index);
-        }
-        if (r == kReadMissing) return false;
-        if (r == kReadOk) {
-            bytes_read += mt.shard_len;
-            Hash got;
-            if (garage_ec_shard_sum_host(mt.sum_kind, check, mt.shard_len, got.data()) == GARAGE_EC_OK && got == mt.sum)
-                return true;
-        }
-        quarantine(node, h, code, index);
-        return false;
-    }
-    // PB: one half of a shard (a ranged read of shard_len/2 bytes into dst), checked against the half's 4 adler8
-    // segment tags (garage_ec_check_shard_half_host); a bad header or tag quarantines the shard like a whole read
-    bool read_half_into(int node, const Hash &h, int half, uint8_t *dst, size_t cap, ShardMeta &mt, bool for_dma = false,
-                        int code = 0, int index = -1)
-    {
-        Node &nd = *nodes[node];
-        ReadResult r;
-        Node::ShardPtr sp;
-        if (nd.dir.empty()) {
-            {
-                std::lock_guard<std::mutex> lk(nd.mu);
-                if (!nd.up) return false;
-                sp = nd.store_find(h);
-            }
-            r = sp ? nd.copy_out(*sp, dst, cap, mt, for_dma, half) : kReadMissing;
+            r = sp ? nd.copy_out(*sp, dst, cap, mt, for_dma, half) : kReadMissing;  // the copy happens outside the node lock
+            if (sp && for_dma && half < 0) check = sp->bytes.data();  // same bytes, and these are still in the cache
         } else {
             std::lock_guard<std::mutex> lk(nd.mu);
             if (!nd.up) return false;
@@ -1210,9 +1269,16 @@ struct garage_bm {
         }
         if (r == kReadMissing) return false;
         if (r == kReadOk) {
-            bytes_read += mt.shard_len / 2;
-            if (garage_ec_check_shard_half_host(mt.sum_kind, dst, mt.shard_len, half, mt.sum.data()) == GARAGE_EC_OK)
-                return true;
+            if (half >= 0) {
+                bytes_read += mt.shard_len / 2;
+                if (garage_ec_check_shard_half_host(mt.sum_kind, dst, mt.shard_len, half, mt.sum.data()) == GARAGE_EC_OK)
+                    return true;
+            } else {
+                bytes_read += mt.shard_len;
+                Hash got;
+                if (garage_ec_shard_sum_host(mt.sum_kind, check, mt.shard_len, got.data()) == GARAGE_EC_OK && got == mt.sum)
+                    return true;
+            }
         }
         quarantine(node, h, code, index);
         return false;
@@ -1289,7 +1355,7 @@ struct garage_bm {
     // A shard whose header disagrees with the others on the block length, or that sits under the
     // wrong index, is treated like a corrupt one.  `all`: read every shard (corruption hunting).
     // Returns the number of shards read (*bytes_out += the bytes); *ok = the wanted shards can be rebuilt from `have`.
-    // `code`: the stripe of that code (0 = the configured one; others: a previous code's shards, .shard or .legacy)
+    // `code`: the stripe of that code (0 = the configured one; others: a previous code's shards, moved aside or not)
     // With several active layout versions (code 0) every index has the sources garage_layout_read_plan lists for it,
     // tried in its order (a source whose file is missing or bad makes way for the next one; a PB shard's halves come
     // from one source); the wanted indices of skip_node are not read.  from_out[i] = the node shard i came from.
@@ -1363,8 +1429,8 @@ struct garage_bm {
                 got = read_shard_into(node, h, dst, slot_stride, mt, for_gpu, code, fidx);
             } else {
                 const size_t hl = (have_expect ? shard_len_of(expect, code) : slot_stride) / 2;  // placement of the b-half
-                got = read_half_into(node, h, half, dst + (size_t)half * hl, slot_stride - (size_t)half * hl, mt, for_gpu,
-                                     code, fidx);
+                got = read_shard_into(node, h, dst + (size_t)half * hl, slot_stride - (size_t)half * hl, mt, for_gpu, code,
+                                      fidx, half);
                 if (got && !have_expect && half == 1 && mt.shard_len / 2 != hl)  // first read of the block: move it
                     memmove(dst + mt.shard_len / 2, dst + hl, mt.shard_len / 2);
             }
@@ -1569,7 +1635,7 @@ struct garage_bm {
         std::unique_ptr<garage_quorum_tracker, void (*)(garage_quorum_tracker *)> own(t, garage_quorum_tracker_free);
         for (int r = 0; r < nr; r++) {
             const int i = reqs[r].index;
-            garage_quorum_tracker_register(t, r, write_shard_at(reqs[r].node, h, i, len, bytes(i), L, sums + (size_t)i * 32, false));
+            garage_quorum_tracker_register(t, r, write_shard(reqs[r].node, h, i, len, bytes(i), L, sums + (size_t)i * 32));
         }
         {
             std::lock_guard<std::mutex> lk(refs_mu);
@@ -1714,20 +1780,15 @@ struct garage_bm {
             Node &nd = *nodes[node];
             std::lock_guard<std::mutex> lk(nd.mu);
             if (!nd.up) return GARAGE_BM_E_MESSAGE;
-            const bool exists = multi ? !nd.path_at(h, idx).empty() : nd.store_has(h);
-            // during a layout change the node's files of every index go, .legacy included
-            const auto held = multi ? other_index_files(nd, h, -1) : std::vector<std::pair<const char *, int>>();
-            if ((exists || !held.empty()) && unneeded) {  // offload branch, resync.rs:369-458: delete_if_unneeded
+            const bool exists = nd.store_has(h, multi ? idx : -1);
+            // during a layout change the node's files of every index go, an older index moved aside included
+            const bool held = multi && !nd.other_index_files(h, -1).empty();
+            if ((exists || held) && unneeded) {  // offload branch, resync.rs:369-458: delete_if_unneeded
                 if (!deletable_now(h)) {  // still inside the GC delay: look again later
                     if (nd.queued.insert(h).second) nd.resync_queue.push_back(h);
                     return GARAGE_BM_OK;
                 }
-                if (!multi) {
-                    if (nd.store_erase(h)) delete_counter++;
-                    return GARAGE_BM_OK;
-                }
-                for (auto &f : held)
-                    if (::remove(nd.path_of(h, f.first).c_str()) == 0) delete_counter++;
+                delete_counter += multi ? nd.erase_other_indices(h, -1, [] { return true; }) : nd.store_erase(h);
                 return GARAGE_BM_OK;
             }
             if (exists) return GARAGE_BM_OK;
@@ -1770,8 +1831,7 @@ struct garage_bm {
         const uint8_t *bytes = slot.p + (size_t)idx * slot_stride;
         Hash sum;
         shard_tag(bytes, L, sum);
-        if (!(multi ? write_shard_at(node, h, idx, block_len, bytes, L, sum.data(), false)
-                    : write_shard(node, h, idx, block_len, bytes, L, sum.data()))) {  // resync.rs:499
+        if (!write_shard(node, h, idx, block_len, bytes, L, sum.data())) {  // resync.rs:499
             resync_error_counter++;
             return GARAGE_BM_E_MESSAGE;  // Error::Io: stays queued, the caller backs off (resync.rs:300-315)
         }
@@ -1807,7 +1867,7 @@ struct garage_bm {
                 quarantine(y, h, 0, idx);  // a self-consistent shard of another block length: stale
                 continue;
             }
-            if (!write_shard_at(node, h, idx, mt.block_len, buf, mt.shard_len, mt.sum.data(), counted)) return -1;
+            if (!write_shard(node, h, idx, mt.block_len, buf, mt.shard_len, mt.sum.data(), counted)) return -1;
             layout_shards_copied++;
             layout_bytes_written += mt.shard_len;
             return 1;
@@ -1867,7 +1927,7 @@ struct garage_bm {
                 const uint8_t *bytes = items[j].stripe + (size_t)idx * slot_stride;
                 Hash sum;
                 shard_tag(bytes, L, sum);
-                if (!write_shard_at(node, h, idx, len, bytes, L, sum.data(), true)) {
+                if (!write_shard(node, h, idx, len, bytes, L, sum.data(), true)) {
                     layout_sync_errors++;
                     *clean = false;
                     return;
@@ -1879,8 +1939,9 @@ struct garage_bm {
         }
         return written;
     }
-    // the newest version's stripe of h holds its write quorum: k+1 shards with valid tags at their assigned (node, index)
-    bool newest_at_quorum(const Hash &h, uint8_t *buf)
+    // the newest version's stripe of h holds its write quorum: k+1 configured-code shards with valid tags on their nodes.
+    // by_index: each read from the file holding its assigned index (the newest stripe during a layout change)
+    bool at_quorum(const Hash &h, uint8_t *buf, bool by_index)
     {
         int who[64];
         storage_nodes_of(h, who);
@@ -1888,20 +1949,9 @@ struct garage_bm {
         int good = 0;
         for (int i = 0; i < tot && good < quorum && good + (tot - i) >= quorum; i++) {
             ShardMeta mt;
-            if (read_shard_into(who[i], h, buf, slot_stride, mt, false, 0, i) && mt.index == i) good++;
+            if (read_shard_into(who[i], h, buf, slot_stride, mt, false, 0, by_index ? i : -1) && mt.index == i) good++;
         }
         return good >= quorum;
-    }
-    // the configured-code files of h on `node` whose index is not `keep`: (".shard" / ".legacy", index)
-    std::vector<std::pair<const char *, int>> other_index_files(Node &nd, const Hash &h, int keep) const  // nd.mu held
-    {
-        std::vector<std::pair<const char *, int>> r;
-        if (nd.dir.empty() || !nd.by_index) return r;
-        for (const char *ext : {".shard", ".legacy"}) {
-            const int i = nd.file_index(nd.path_of(h, ext));
-            if (i >= 0 && i != keep) r.emplace_back(ext, i);
-        }
-        return r;
     }
     // Offload of shard i of h from `node` (resync.rs:369-458): the newest version's holder of i gets it first if it
     // lacks it (a push: the copy a receiver would make), then the file goes once the newest stripe holds k+1.
@@ -1915,7 +1965,7 @@ struct garage_bm {
         std::vector<std::pair<const char *, int>> held;
         {
             std::lock_guard<std::mutex> lk(nd.mu);
-            held = other_index_files(nd, h, a);
+            held = nd.other_index_files(h, a);
         }
         int pushed = 0;
         bool all_held = true;  // every newest holder of an index this node offloads has it
@@ -1924,7 +1974,7 @@ struct garage_bm {
             ShardMeta mt;
             if (read_shard_into(who[i], h, buf, slot_stride, mt, false, 0, i) && mt.index == i) continue;
             if (read_shard_into(node, h, buf, slot_stride, mt, false, 0, i) && mt.index == i &&
-                write_shard_at(who[i], h, i, mt.block_len, buf, mt.shard_len, mt.sum.data(), true)) {
+                write_shard(who[i], h, i, mt.block_len, buf, mt.shard_len, mt.sum.data(), true)) {
                 layout_shards_copied++;
                 layout_bytes_read += mt.shard_len;
                 layout_bytes_written += mt.shard_len;
@@ -1933,11 +1983,9 @@ struct garage_bm {
                 all_held = false;
             }
         }
-        if (held.empty() || !all_held || !newest_at_quorum(h, buf)) return pushed;
+        if (held.empty() || !all_held || !at_quorum(h, buf, true)) return pushed;
         std::lock_guard<std::mutex> lk(nd.mu);
-        if (!nd.up) return pushed;
-        for (auto &f : other_index_files(nd, h, a))
-            if (convert_op_allowed() && ::remove(nd.path_of(h, f.first).c_str()) == 0) layout_deleted++;
+        if (nd.up) layout_deleted += nd.erase_other_indices(h, a, [this] { return convert_op_allowed(); });
         return pushed;
     }
     // garage_bm_layout_sync_step: see include/garage_block_manager.h
@@ -1955,22 +2003,11 @@ struct garage_bm {
         {
             std::lock_guard<std::mutex> lk(nd.mu);
             if (!nd.up) return GARAGE_BM_E_MESSAGE;
-            if (!nd.dir.empty()) nd.store_list(hs, true);
+            if (!nd.dir.empty()) nd.store_list(hs);
         }
-        std::sort(hs.begin(), hs.end());
-        hs.erase(std::unique(hs.begin(), hs.end()), hs.end());
-        if (cursor) hs.erase(hs.begin(), std::upper_bound(hs.begin(), hs.end(), *cursor));
-        bool done = true;
-        if (max_blocks && hs.size() > max_blocks) {
-            hs.resize(max_blocks);
-            done = false;
-        }
-        if (finished) *finished = done ? 1 : 0;
-        if (cursor_out) {
-            if (!hs.empty()) *cursor_out = hs.back();
-            else if (cursor) *cursor_out = *cursor;
-            else cursor_out->fill(0);
-        }
+        int done = 0;
+        sweep_page(hs, cursor, max_blocks, cursor_out, &done);
+        if (finished) *finished = done;
         if (!cursor) {
             std::lock_guard<std::mutex> lk(layout_mu);
             pass_version[node] = newest_v;
@@ -1989,8 +2026,7 @@ struct garage_bm {
                     if (it != rc.end() && it->second.count <= 0) {
                         if (deletable_now(h)) {
                             std::lock_guard<std::mutex> lk(nd.mu);
-                            for (auto &f : other_index_files(nd, h, -1))
-                                if (convert_op_allowed() && ::remove(nd.path_of(h, f.first).c_str()) == 0) delete_counter++;
+                            delete_counter += nd.erase_other_indices(h, -1, [this] { return convert_op_allowed(); });
                         }
                         continue;
                     }
@@ -2001,7 +2037,7 @@ struct garage_bm {
                 if (a >= 0 && !(read_shard_into(node, h, scratch.p, slot_stride, mt, false, 0, a) && mt.index == a))
                     receive.emplace_back(h, a);
                 std::lock_guard<std::mutex> lk(nd.mu);
-                if (!other_index_files(nd, h, a).empty()) offload.push_back(h);
+                if (!nd.other_index_files(h, a).empty()) offload.push_back(h);
             }
         }
         std::atomic<bool> clean{true};
@@ -2072,29 +2108,13 @@ struct garage_bm {
         s += "synced";
         for (uint64_t v : synced) s += " " + std::to_string(v);
         s += "\n";
-        const std::string tmp = layout_path + ".tmp" + std::to_string((unsigned long)::getpid());
-        FILE *f = fopen(tmp.c_str(), "wb");
-        if (!f) return false;
-        bool ok = fwrite(s.data(), s.size(), 1, f) == 1 && fflush(f) == 0 && ::fsync(fileno(f)) == 0;
-        ok = fclose(f) == 0 && ok;
-        if (ok) ok = ::rename(tmp.c_str(), layout_path.c_str()) == 0;
-        if (ok && cfg.data_fsync) {
-            const int dfd = ::open(std::filesystem::path(layout_path).parent_path().c_str(), O_RDONLY | O_DIRECTORY);
-            ok = dfd >= 0 && ::fsync(dfd) == 0;
-            if (dfd >= 0) ::close(dfd);
-        }
-        if (!ok) ::remove(tmp.c_str());
-        return ok;
+        return write_file_atomic(layout_path, s.data(), s.size(), nullptr, 0, true, cfg.data_fsync != 0);
     }
     // 1: loaded into out / syn; 0: no file; -1: a file this manager cannot use
     static int load_layout(const std::string &path, int n, int tot, Layouts &out, std::vector<uint64_t> &syn)
     {
-        FILE *f = fopen(path.c_str(), "rb");
-        if (!f) return 0;
         std::string s;
-        char buf[65536];
-        for (size_t r; (r = fread(buf, 1, sizeof(buf), f)) > 0;) s.append(buf, r);
-        fclose(f);
+        if (!read_file(path, s)) return 0;
         std::vector<std::string> tok;  // whitespace-separated words
         for (size_t i = 0; i < s.size();) {
             while (i < s.size() && isspace((unsigned char)s[i])) i++;
@@ -2186,20 +2206,6 @@ struct garage_bm {
     }
 
     // ---- changing the store's code (DESIGN.md section 5.1) ----------------------------------
-    // the configured stripe of h holds its write quorum: k+1 configured-code shards with valid tags on their nodes
-    bool configured_at_quorum(const Hash &h)
-    {
-        int who[64];
-        storage_nodes_of(h, who);
-        const int quorum = garage_ec_write_quorum(k, m, GARAGE_CONSISTENT);
-        SlotLease scratch(stripe_slots);
-        int good = 0;
-        for (int i = 0; i < tot && good < quorum && good + (tot - i) >= quorum; i++) {
-            ShardMeta mt;
-            if (read_shard_into(who[i], h, scratch.p, slot_stride, mt) && mt.index == i) good++;
-        }
-        return good >= quorum;
-    }
     // every node that may hold a legacy copy of a block is among the first legacy_row() nodes of its ring row
     int legacy_row() const
     {
@@ -2207,7 +2213,6 @@ struct garage_bm {
         for (size_t c = 1; c < codes.size(); c++) r = std::max(r, codes[c].tot);
         return r;
     }
-    int ring_node(const Hash &h, int i) const { return ((int)h[0] % (int)nodes.size() + i) % (int)nodes.size(); }
     // the node that converts h: the first up node holding a legacy copy, previous codes in order and their shards in
     // index order, then the replica holders; -1 if no up node holds one
     int converter_of(const Hash &h)
@@ -2216,7 +2221,7 @@ struct garage_bm {
             for (int i = 0; i < codes[c].tot; i++) {
                 Node &nd = *nodes[ring_node(h, i)];
                 std::lock_guard<std::mutex> lk(nd.mu);
-                if (nd.up && !nd.path_for(h, c).empty()) return ring_node(h, i);
+                if (nd.up && nd.has_code(h, c)) return ring_node(h, i);
             }
         for (int i = 0; i < legacy_rf; i++) {
             Node &nd = *nodes[ring_node(h, i)];
@@ -2233,29 +2238,6 @@ struct garage_bm {
         std::lock_guard<std::mutex> lk(nd.mu);
         if (nd.up && !nd.dir.empty()) legacy_deleted += nd.store_erase_legacy(h, [this] { return convert_op_allowed(); });
     }
-    // write_shard for a conversion: a previous code's shard under the .shard name first moves to .legacy; each of
-    // the two steps is one conversion file operation
-    bool write_converted(int node, const Hash &h, int index, uint32_t block_len, const uint8_t *bytes, size_t n,
-                         const uint8_t *sum)
-    {
-        Node &nd = *nodes[node];
-        bool ok = true;
-        {
-            std::lock_guard<std::mutex> lk(nd.mu);
-            if (!nd.up) return false;
-            if (!nd.dir.empty() && nd.file_code(nd.path_of(h, ".shard")) >= 1)
-                ok = convert_op_allowed() && nd.store_move_legacy_aside(h);
-        }
-        ok = ok && convert_op_allowed();
-        if (!ok) {
-            write_errors++;
-            return false;
-        }
-        if (!write_shard(node, h, index, block_len, bytes, n, sum)) return false;
-        convert_bytes_written += n;
-        return true;
-    }
-
     // Rewrite blocks stored under a previous code or as replicas under the configured code: one garage_ec_transcode
     // per source (previous codes in order, then replicas) and batch of batch_max_blocks.  Nothing is written for a
     // block whose new data shards do not hash to it; then the old stripe's stale shard is hunted and quarantined and
@@ -2372,8 +2354,11 @@ struct garage_bm {
                     const size_t L = shard_len_of(lens[q]);
                     int stored = 0;
                     for (int i = 0; i < tot; i++)  // only a durable write counts towards the quorum
-                        stored += write_converted(who[i], h, i, lens[q], dst + (q * tot + i) * slot_stride, L,
-                                                  sums + (q * tot + i) * 32);
+                        if (write_shard(who[i], h, i, lens[q], dst + (q * tot + i) * slot_stride, L, sums + (q * tot + i) * 32,
+                                        true)) {
+                            stored++;
+                            convert_bytes_written += L;
+                        }
                     {
                         std::lock_guard<std::mutex> lk(refs_mu);
                         refs[h] = lens[q];
@@ -2436,24 +2421,10 @@ struct garage_bm {
                 if (it == rc.end() || it->second.count > 0) hs.push_back(kv.first);
             }
         }
-        std::sort(hs.begin(), hs.end());
-        if (cursor) hs.erase(hs.begin(), std::upper_bound(hs.begin(), hs.end(), *cursor));
         std::vector<Hash> mine;
-        bool done = true;
-        for (const Hash &h : hs) {
-            if (deep_scrub_owner(h) != node) continue;
-            if (max_blocks && mine.size() == max_blocks) {
-                done = false;
-                break;
-            }
-            mine.push_back(h);
-        }
-        if (finished) *finished = done ? 1 : 0;
-        if (cursor_out) {
-            if (!mine.empty()) *cursor_out = mine.back();
-            else if (cursor) *cursor_out = *cursor;
-            else cursor_out->fill(0);
-        }
+        for (const Hash &h : hs)
+            if (deep_scrub_owner(h) == node) mine.push_back(h);
+        sweep_page(mine, cursor, max_blocks, cursor_out, finished);
         uint64_t nchecked = 0, nrep = 0;
         std::lock_guard<std::mutex> dl(deep_mu);
         const size_t bmax = std::max<uint32_t>(cfg.batch_max_blocks, 1), sbytes = (size_t)tot * slot_stride;
@@ -2542,39 +2513,29 @@ struct garage_bm {
             if (!nd.up) return GARAGE_BM_E_MESSAGE;
             if (!nd.dir.empty() && has_legacy()) {
                 std::vector<Hash> all;
-                nd.store_list(all, true);
+                nd.store_list(all);
                 for (const Hash &h : all)
                     if (nd.has_legacy_shard(h) || nd.has_replica(h)) hs.push_back(h);
             }
         }
-        std::sort(hs.begin(), hs.end());
-        hs.erase(std::unique(hs.begin(), hs.end()), hs.end());
-        if (cursor) hs.erase(hs.begin(), std::upper_bound(hs.begin(), hs.end(), *cursor));
-        bool done = true;
-        if (max_blocks && hs.size() > max_blocks) {
-            hs.resize(max_blocks);
-            done = false;
-        }
-        if (finished) *finished = done ? 1 : 0;
-        if (cursor_out) {
-            if (!hs.empty()) *cursor_out = hs.back();
-            else if (cursor) *cursor_out = *cursor;
-            else cursor_out->fill(0);
-        }
+        sweep_page(hs, cursor, max_blocks, cursor_out, finished);
         std::vector<Hash> todo;
-        for (const Hash &h : hs) {
-            {
-                // rc 0: never converted; the legacy copies go once the GC delay has passed, decided and deleted under
-                // both locks like resync_block's offload branch
-                std::lock_guard<std::mutex> rl(refs_mu);
-                auto it = rc.find(h);
-                if (it != rc.end() && it->second.count <= 0) {
-                    if (deletable_now(h)) delete_legacy(node, h);
-                    continue;
+        {
+            SlotLease scratch(stripe_slots);  // the quorum check's reads
+            for (const Hash &h : hs) {
+                {
+                    // rc 0: never converted; the legacy copies go once the GC delay has passed, decided and deleted
+                    // under both locks like resync_block's offload branch
+                    std::lock_guard<std::mutex> rl(refs_mu);
+                    auto it = rc.find(h);
+                    if (it != rc.end() && it->second.count <= 0) {
+                        if (deletable_now(h)) delete_legacy(node, h);
+                        continue;
+                    }
                 }
+                if (at_quorum(h, scratch.p, false)) delete_legacy(node, h);  // converted already
+                else if (converter_of(h) == node) todo.push_back(h);
             }
-            if (configured_at_quorum(h)) delete_legacy(node, h);  // converted already
-            else if (converter_of(h) == node) todo.push_back(h);
         }
         const size_t n = todo.empty() ? 0 : convert_batch(todo);
         if (converted) *converted = n;
@@ -2681,7 +2642,7 @@ struct garage_bm {
             bool has;
             {
                 std::lock_guard<std::mutex> lk(nodes[node]->mu);
-                has = multi ? !nodes[node]->path_at(h, idx).empty() : nodes[node]->store_has(h);
+                has = nodes[node]->store_has(h, multi ? idx : -1);
             }
             if (!has) {
                 put_to_resync(node, h);
@@ -2707,35 +2668,14 @@ struct garage_bm {
         {
             std::lock_guard<std::mutex> lk(nd.mu);
             if (!nd.up) return GARAGE_BM_E_MESSAGE;
-            nd.store_list(hashes, has_legacy() || nd.by_index);
+            nd.store_list(hashes);
         }
-        std::sort(hashes.begin(), hashes.end());
-        hashes.erase(std::unique(hashes.begin(), hashes.end()), hashes.end());
-        if (cursor) hashes.erase(hashes.begin(), std::upper_bound(hashes.begin(), hashes.end(), *cursor));
-        bool done = true;
-        if (max_shards && hashes.size() > max_shards) {
-            hashes.resize(max_shards);
-            done = false;
-        }
-        if (finished) *finished = done ? 1 : 0;
-        if (cursor_out) {
-            if (!hashes.empty()) *cursor_out = hashes.back();
-            else if (cursor) *cursor_out = *cursor;
-            else cursor_out->fill(0);
-        }
-        // the files to check: (hash, 0) the .shard; with previous codes or replicas configured also (hash, 1) a .legacy
-        // shard and (hash, 2) a replica; with a layout file (hash, 1) an older layout version's index
-        const bool by_index = nd.by_index;
-        const bool legacy = (has_legacy() || by_index) && !nd.dir.empty();
-        const bool old_index = by_index && !has_legacy();  // a .legacy file holds the configured code
-        std::vector<std::pair<Hash, int>> items;
+        sweep_page(hashes, cursor, max_shards, cursor_out, finished);
+        std::vector<std::pair<Hash, int>> items;  // (hash, Node::ShardFile)
         {
             std::lock_guard<std::mutex> lk(nd.mu);
-            for (const Hash &h : hashes) {
-                if (!legacy || nd.file_code(nd.path_of(h, ".shard")) != -2) items.emplace_back(h, 0);
-                if (legacy && nd.file_code(nd.path_of(h, ".legacy")) != -2) items.emplace_back(h, 1);
-                if (legacy && nd.has_replica(h)) items.emplace_back(h, 2);
-            }
+            for (const Hash &h : hashes)
+                for (int f : nd.scrub_files(h)) items.emplace_back(h, f);
         }
         uint64_t nchecked = 0, nbad = 0;
         const size_t chunk = std::max<size_t>(1, (size_t)cfg.batch_max_blocks * tot);
@@ -2748,7 +2688,6 @@ struct garage_bm {
             uint8_t *expect = buf + n * stride, *bad = expect + n * 32;
             std::vector<uint32_t> lens(n, 0);
             std::vector<uint8_t> state(n, 0);  // 0 gone, 1 to be checked on the GPU, 2 corrupt already, 3 checked on the CPU
-            std::vector<int> code(n, 0);       // the code the file holds a shard of (-1: a replica)
             {
                 std::lock_guard<std::mutex> lk(nd.mu);
                 for (size_t i = 0; i < n; i++) {
@@ -2757,10 +2696,9 @@ struct garage_bm {
                     const Hash &h = items[c0 + i].first;
                     const int kind = items[c0 + i].second;
                     ReadResult r;
-                    if (kind == 2) {  // a replica is checked against its content hash
+                    if (kind == Node::kReplicaFile) {  // a replica is checked against its content hash
                         replica.resize(cfg.block_size);
                         uint32_t len = 0;
-                        code[i] = -1;
                         r = nd.replica_read_into(h, replica.data(), replica.size(), len);
                         if (r == kReadMissing) continue;
                         Hash got;
@@ -2771,13 +2709,7 @@ struct garage_bm {
                         state[i] = r == kReadOk && got == h ? 3 : 2;
                         continue;
                     }
-                    if (!legacy) {
-                        r = nd.store_read_into(h, buf + i * stride, stride, mt);
-                    } else {  // read the file as the code its header names; an unknown code is corrupt, as before
-                        const std::string path = nd.path_of(h, kind ? ".legacy" : ".shard");
-                        code[i] = old_index ? 0 : std::max(kind, nd.file_code(path));
-                        r = nd.file_read_into(path, code[i], buf + i * stride, stride, mt);
-                    }
+                    r = nd.scrub_read_into(h, kind, buf + i * stride, stride, mt);
                     if (r == kReadMissing) continue;
                     if (r == kReadInvalid) {
                         state[i] = 2;
@@ -2803,8 +2735,7 @@ struct garage_bm {
                 nchecked++;
                 if (state[i] == 3 || (state[i] == 1 && !bad[i])) continue;
                 nbad++;
-                if (old_index && items[c0 + i].second == 1) quarantine_file(node, items[c0 + i].first, ".legacy");
-                else quarantine(node, items[c0 + i].first, code[i]);
+                quarantine(node, items[c0 + i].first, 0, -1, items[c0 + i].second);
             }
         }
         scrub_checked += nchecked;
@@ -2921,6 +2852,20 @@ struct garage_bm {
         return GARAGE_BM_E_MESSAGE;          \
     }
 
+// the four resumable sweeps: the cursor in and out of one garage_bm_*_step call
+template <class Step>
+static int bm_step(garage_bm *bm, int node, const uint8_t *cursor32, uint8_t *cursor_out32, Step step)
+{
+    if (!bm || node < 0 || node >= (int)bm->nodes.size()) return GARAGE_EC_E_INVALID;
+    BM_GUARD(([&] {
+        Hash cur, out;
+        if (cursor32) cur = to_hash(cursor32);
+        const int rc = step(cursor32 ? &cur : nullptr, &out);
+        if (rc == GARAGE_BM_OK && cursor_out32) memcpy(cursor_out32, out.data(), 32);
+        return rc;
+    }()));
+}
+
 extern "C" {
 
 void garage_bm_default_config(garage_bm_config *c)
@@ -2948,8 +2893,9 @@ void garage_bm_default_config(garage_bm_config *c)
     c->clay = 0;                    // not Clay
 }
 
-// a code garage_ec_create / _lrc / _piggyback accepts, with tags the block manager can check: the same rules as the
-// configured code's (PB: 1 <= k <= 16, 2 <= m <= 4, no LRC groups, adler8 tags)
+// a code garage_ec_create / _lrc / _piggyback accepts, with tags the block manager can check; the rules of the
+// configured code and of every previous code (PB: 1 <= k <= 16, 2 <= m <= 4, no LRC groups, and adler8 tags for its
+// half reads)
 static bool code_ok(int k, int m, int l, int piggyback, int sum_kind)
 {
     if (k < 1 || m < 1 || k > GARAGE_EC_MAX_K || m > GARAGE_EC_MAX_M) return false;
@@ -2958,19 +2904,25 @@ static bool code_ok(int k, int m, int l, int piggyback, int sum_kind)
     return !piggyback || (l == 0 && k <= 16 && m >= 2 && m <= 4 && sum_kind != GARAGE_EC_SUM_BLAKE2);
 }
 
+// a context running code `c` (RS, LRC, PB or Clay) with shard tags of `sum_kind`
+static int create_ctx(const CodeDesc &c, int device, int sum_kind, garage_ec_ctx **out)
+{
+    const int rc = c.clay ? garage_ec_create_clay(out, device, c.k, c.m, GARAGE_EC_VANDERMONDE)
+                   : c.pb ? garage_ec_create_piggyback(out, device, c.k, c.m, GARAGE_EC_VANDERMONDE)
+                   : c.l  ? garage_ec_create_lrc(out, device, c.k, c.l, c.m - c.l)
+                          : garage_ec_create(out, device, c.k, c.m, GARAGE_EC_VANDERMONDE);
+    if (rc == GARAGE_EC_OK) garage_ec_set_sum_kind(*out, sum_kind);
+    return rc;
+}
+
 static int bm_create(garage_bm **out, const garage_bm_config *cfg)
 {
     *out = nullptr;
-    const int k = cfg->data_shards, m = cfg->parity_shards;
-    if (k < 1 || m < 1 || k > GARAGE_EC_MAX_K || m > GARAGE_EC_MAX_M || cfg->n_nodes < k + m || cfg->n_nodes > 256)
+    const int k = cfg->data_shards, m = cfg->parity_shards, l = cfg->local_groups;
+    if (!code_ok(k, m, l, cfg->piggyback, cfg->shard_sum_kind) || cfg->n_nodes < k + m || cfg->n_nodes > 256)
         return GARAGE_EC_E_INVALID;
     if (cfg->shard_sum_kind != GARAGE_EC_SUM_BLAKE2 && cfg->shard_sum_kind != GARAGE_EC_SUM_ADLER8) return GARAGE_EC_E_INVALID;
-    const int l = cfg->local_groups;
-    if (l < 0 || (l > 0 && (l >= m || k % l))) return GARAGE_EC_E_INVALID;
     const bool pb = cfg->piggyback != 0;
-    // PB is not combined with LRC, and its half reads need per-segment (adler8) tags
-    if ((cfg->piggyback != 0 && cfg->piggyback != 1) || (pb && (l > 0 || cfg->shard_sum_kind == GARAGE_EC_SUM_BLAKE2)))
-        return GARAGE_EC_E_INVALID;
     // Clay(k, m) (garage_ec_create_clay's rules): not combined with LRC or PB, and without layout changes
     const bool clay = cfg->clay != 0;
     if (cfg->clay != 0 && cfg->clay != 1) return GARAGE_EC_E_INVALID;
@@ -3013,13 +2965,6 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
     // a store changes its layout or its code, not both at once
     if (lays->v.size() > 1 && (np > 0 || cfg->legacy_replicas > 0)) return GARAGE_EC_E_INVALID;
     if (clay && layout_file) return GARAGE_EC_E_INVALID;  // a Clay store keeps the fixed ring
-    // every context of the manager runs the same code: RS(k, m), LRC(k, l, m - l) or PB(k, m)
-    auto make_ctx = [&](garage_ec_ctx **c) {
-        return clay ? garage_ec_create_clay(c, cfg->cuda_device, k, m, GARAGE_EC_VANDERMONDE)
-             : pb ? garage_ec_create_piggyback(c, cfg->cuda_device, k, m, GARAGE_EC_VANDERMONDE)
-                  : l ? garage_ec_create_lrc(c, cfg->cuda_device, k, l, m - l)
-                      : garage_ec_create(c, cfg->cuda_device, k, m, GARAGE_EC_VANDERMONDE);
-    };
     std::unique_ptr<garage_bm> bm(new garage_bm());
     bm->cfg = *cfg;
     if (!bm->cfg.block_size) bm->cfg.block_size = 1u << 20;
@@ -3027,46 +2972,35 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
     bm->m = m;
     bm->tot = k + m;
     bm->sum_kind = cfg->shard_sum_kind;
-    bm->pb = pb;
-    int rc = make_ctx(&bm->ec);
-    if (rc != GARAGE_EC_OK) return rc;  // no GPU => no block manager: there is no CPU fallback
-    garage_ec_set_sum_kind(bm->ec, bm->sum_kind);
-    bm->codes.resize(1 + np);
-    bm->codes[0].k = k;
-    bm->codes[0].m = m;
-    bm->codes[0].l = l;
-    bm->codes[0].pb = pb;
-    bm->codes[0].clay = clay;
-    bm->codes[0].quantum = pb ? 128u : 1u;
-    if (clay) {
-        int alpha = 0;
-        garage_ec_clay_info(bm->ec, nullptr, nullptr, &alpha, nullptr, nullptr);
-        bm->codes[0].quantum = 16u * (uint32_t)alpha;
-    }
-    bm->codes[0].tot = k + m;
-    bm->codes[0].ctx = bm->ec;
     bm->legacy_rf = cfg->legacy_replicas;
     bm->cfg.previous_codes = nullptr;  // not kept: the caller's array may go away
-    bm->slot_stride = garage_ec_stride_for((uint32_t)bm->shard_len_of(bm->cfg.block_size));
-    for (int i = 0; i < np; i++) {  // one context per previous code, same tag kind and matrices as the configured one
-        const garage_bm_code &p = cfg->previous_codes[i];
-        garage_bm::Code &c = bm->codes[1 + i];
+    // codes[0] the configured code (every dispatcher context runs it too), then one context per previous code, same
+    // tag kind and matrices as the configured one
+    bm->codes.resize(1 + np);
+    int rc = GARAGE_EC_OK;
+    for (int i = 0; i <= np; i++) {
+        garage_bm::Code &c = bm->codes[i];
+        const garage_bm_code p = i ? cfg->previous_codes[i - 1] : garage_bm_code{k, m, l, cfg->piggyback};
         c.k = p.k;
         c.m = p.m;
         c.l = p.local_groups;
         c.pb = p.piggyback != 0;
-        c.quantum = c.pb ? 128u : 1u;
+        c.clay = i == 0 && clay;
         c.tot = p.k + p.m;
-        rc = c.pb ? garage_ec_create_piggyback(&c.ctx, cfg->cuda_device, p.k, p.m, GARAGE_EC_VANDERMONDE)
-             : c.l ? garage_ec_create_lrc(&c.ctx, cfg->cuda_device, p.k, c.l, p.m - c.l)
-                   : garage_ec_create(&c.ctx, cfg->cuda_device, p.k, p.m, GARAGE_EC_VANDERMONDE);
-        if (rc != GARAGE_EC_OK) {
+        rc = create_ctx(c, cfg->cuda_device, bm->sum_kind, &c.ctx);
+        if (rc != GARAGE_EC_OK) {  // no GPU => no block manager: there is no CPU fallback
             garage_bm_destroy(bm.release());
             return rc;
         }
-        garage_ec_set_sum_kind(c.ctx, bm->sum_kind);
+        if (i == 0) bm->ec = c.ctx;
+        c.quantum = c.pb ? 128u : 1u;
+        if (c.clay) {
+            int alpha = 0;
+            garage_ec_clay_info(c.ctx, nullptr, nullptr, &alpha, nullptr, nullptr);
+            c.quantum = 16u * (uint32_t)alpha;
+        }
         // slots and the scrub buffer hold a shard of the largest code in play
-        bm->slot_stride = std::max(bm->slot_stride, garage_ec_stride_for((uint32_t)bm->shard_len_of(bm->cfg.block_size, 1 + i)));
+        bm->slot_stride = std::max(bm->slot_stride, garage_ec_stride_for((uint32_t)bm->shard_len_of(bm->cfg.block_size, i)));
     }
     if (lays->v.empty() && cfg->n_nodes <= GARAGE_LAYOUT_MAX_NODES) {
         const int n = cfg->n_nodes, tot = k + m;
@@ -3092,10 +3026,6 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
     for (int i = 0; i < cfg->n_nodes; i++) {
         bm->nodes.emplace_back(new Node());
         Node &nd = *bm->nodes.back();
-        nd.k = k;
-        nd.m = m;
-        nd.l = cfg->local_groups;
-        nd.pb = pb;
         nd.codes.assign(1, bm->codes[0]);
         nd.fsync_data = cfg->data_fsync != 0;
         if (cfg->data_dir && cfg->data_dir[0]) {
@@ -3108,23 +3038,11 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
             // restart: what is on disk is what exists (the block_ref table would say the same), shards of previous
             // codes and replicas included
             std::vector<Hash> have;
-            nd.store_list(have, bm->has_legacy() || nd.by_index);
+            nd.store_list(have);
             std::vector<uint8_t> tmp(bm->slot_stride);
             for (const Hash &h : have) {
-                ShardMeta mt;
-                struct stat sb;
-                for (int c = 0; c < (int)nd.codes.size(); c++)
-                    if (nd.store_read_into(h, tmp.data(), tmp.size(), mt, -1, c) == kReadOk) {
-                        bm->refs[h] = mt.block_len;
-                        break;
-                    }
-                // a block held only as an older layout version's index
-                if (!bm->refs.count(h) && nd.by_index && !bm->has_legacy() &&
-                    nd.file_read_into(nd.path_of(h, ".legacy"), 0, tmp.data(), tmp.size(), mt) == kReadOk)
-                    bm->refs[h] = mt.block_len;
-                if (!bm->refs.count(h) && nd.has_replica(h) && ::stat(nd.path_of(h, "").c_str(), &sb) == 0 && sb.st_size > 0 &&
-                    (uint64_t)sb.st_size <= bm->cfg.block_size)
-                    bm->refs[h] = (uint32_t)sb.st_size;
+                uint32_t len = 0;
+                if (nd.block_len_of(h, tmp, bm->cfg.block_size, bm->refs.count(h) != 0, len)) bm->refs[h] = len;
             }
         }
     }
@@ -3138,11 +3056,9 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
     // a layout given in the configuration is recorded, so that a restart keeps it and its later versions
     if (layout_file && !std::filesystem::exists(layout_path) && !bm->save_layout(*lays)) return destroy_on_error(GARAGE_BM_E_MESSAGE);
     for (int w = 0; w < garage_bm::kWorkers; w++) {
-        rc = make_ctx(&bm->enc_ctx[w]);
-        if (rc == GARAGE_EC_OK) rc = make_ctx(&bm->rec_ctx[w]);
+        rc = create_ctx(bm->codes[0], cfg->cuda_device, bm->sum_kind, &bm->enc_ctx[w]);
+        if (rc == GARAGE_EC_OK) rc = create_ctx(bm->codes[0], cfg->cuda_device, bm->sum_kind, &bm->rec_ctx[w]);
         if (rc != GARAGE_EC_OK) return destroy_on_error(rc);
-        garage_ec_set_sum_kind(bm->enc_ctx[w], bm->sum_kind);
-        garage_ec_set_sum_kind(bm->rec_ctx[w], bm->sum_kind);
         // Dispatchers wait for their batch spinning in the driver (default) or sleeping on an event
         // (GARAGE_BM_SLEEP_WAIT=1).  With 32 client threads on a 16-CPU host PUT is faster spinning: the wake-up
         // latency costs more than the three CPUs.
@@ -3292,52 +3208,25 @@ int garage_bm_scrub(garage_bm *bm, int node, uint64_t *checked, uint64_t *corrup
 int garage_bm_scrub_step(garage_bm *bm, int node, const uint8_t *cursor32, size_t max_shards, uint8_t cursor_out32[32],
                          int *finished, uint64_t *checked, uint64_t *corrupt)
 {
-    if (!bm || node < 0 || node >= (int)bm->nodes.size()) return GARAGE_EC_E_INVALID;
-    try {
-        Hash cur, out;
-        if (cursor32) cur = to_hash(cursor32);
-        int rc = bm->scrub(node, checked, corrupt, cursor32 ? &cur : nullptr, max_shards, &out, finished);
-        if (rc == GARAGE_BM_OK && cursor_out32) memcpy(cursor_out32, out.data(), 32);
-        return rc;
-    } catch (const std::bad_alloc &) {
-        return GARAGE_EC_E_NOMEM;
-    } catch (...) {
-        return GARAGE_BM_E_MESSAGE;
-    }
+    return bm_step(bm, node, cursor32, cursor_out32, [&](const Hash *cur, Hash *out) {
+        return bm->scrub(node, checked, corrupt, cur, max_shards, out, finished);
+    });
 }
 
 int garage_bm_deep_scrub_step(garage_bm *bm, int node, const uint8_t *cursor32, size_t max_blocks,
                               uint8_t cursor_out32[32], int *finished, uint64_t *checked, uint64_t *repaired)
 {
-    if (!bm || node < 0 || node >= (int)bm->nodes.size()) return GARAGE_EC_E_INVALID;
-    try {
-        Hash cur, out;
-        if (cursor32) cur = to_hash(cursor32);
-        int rc = bm->deep_scrub_step(node, cursor32 ? &cur : nullptr, max_blocks, &out, finished, checked, repaired);
-        if (rc == GARAGE_BM_OK && cursor_out32) memcpy(cursor_out32, out.data(), 32);
-        return rc;
-    } catch (const std::bad_alloc &) {
-        return GARAGE_EC_E_NOMEM;
-    } catch (...) {
-        return GARAGE_BM_E_MESSAGE;
-    }
+    return bm_step(bm, node, cursor32, cursor_out32, [&](const Hash *cur, Hash *out) {
+        return bm->deep_scrub_step(node, cur, max_blocks, out, finished, checked, repaired);
+    });
 }
 
 int garage_bm_convert_step(garage_bm *bm, int node, const uint8_t *cursor32, size_t max_blocks, uint8_t cursor_out32[32],
                            int *finished, uint64_t *converted)
 {
-    if (!bm || node < 0 || node >= (int)bm->nodes.size()) return GARAGE_EC_E_INVALID;
-    try {
-        Hash cur, out;
-        if (cursor32) cur = to_hash(cursor32);
-        int rc = bm->convert_step(node, cursor32 ? &cur : nullptr, max_blocks, &out, finished, converted);
-        if (rc == GARAGE_BM_OK && cursor_out32) memcpy(cursor_out32, out.data(), 32);
-        return rc;
-    } catch (const std::bad_alloc &) {
-        return GARAGE_EC_E_NOMEM;
-    } catch (...) {
-        return GARAGE_BM_E_MESSAGE;
-    }
+    return bm_step(bm, node, cursor32, cursor_out32, [&](const Hash *cur, Hash *out) {
+        return bm->convert_step(node, cur, max_blocks, out, finished, converted);
+    });
 }
 
 int garage_bm_apply_layout(garage_bm *bm, const garage_bm_layout_spec *spec, uint64_t *version_out)
@@ -3349,18 +3238,9 @@ int garage_bm_apply_layout(garage_bm *bm, const garage_bm_layout_spec *spec, uin
 int garage_bm_layout_sync_step(garage_bm *bm, int node, const uint8_t *cursor32, size_t max_blocks, uint8_t cursor_out32[32],
                                int *finished, uint64_t *moved)
 {
-    if (!bm || node < 0 || node >= (int)bm->nodes.size()) return GARAGE_EC_E_INVALID;
-    try {
-        Hash cur, out;
-        if (cursor32) cur = to_hash(cursor32);
-        int rc = bm->layout_sync_step(node, cursor32 ? &cur : nullptr, max_blocks, &out, finished, moved);
-        if (rc == GARAGE_BM_OK && cursor_out32) memcpy(cursor_out32, out.data(), 32);
-        return rc;
-    } catch (const std::bad_alloc &) {
-        return GARAGE_EC_E_NOMEM;
-    } catch (...) {
-        return GARAGE_BM_E_MESSAGE;
-    }
+    return bm_step(bm, node, cursor32, cursor_out32, [&](const Hash *cur, Hash *out) {
+        return bm->layout_sync_step(node, cur, max_blocks, out, finished, moved);
+    });
 }
 
 int garage_bm_layout_versions(garage_bm *bm, uint64_t *out, int cap)
@@ -3393,46 +3273,11 @@ int garage_bm_set_node_up(garage_bm *bm, int node, int up)
     return GARAGE_BM_OK;
 }
 
-// fault injection: what = 0 flips a bit of the shard's bytes at byte_off, 1 rewrites the stored
-// block_len (+1), 2 rewrites the stored index (+1 mod k+m); the stored tag / header check are left
-// alone in every case -- that is the corruption.
 static int bm_corrupt(garage_bm *bm, int node, const uint8_t hash[32], size_t byte_off, int what)
 {
     Node &nd = *bm->nodes[node];
     std::lock_guard<std::mutex> lk(nd.mu);
-    const Hash h = to_hash(hash);
-    if (nd.dir.empty()) {
-        auto it = nd.shards.find(h);
-        if (it == nd.shards.end()) return GARAGE_BM_E_MISSING_BLOCK;
-        auto mod = std::make_shared<StoredShard>(*it->second);  // stored shards are immutable: replace by a damaged copy
-        if (what == 0) {
-            if (mod->bytes.empty()) return GARAGE_BM_E_MISSING_BLOCK;
-            mod->bytes[byte_off % mod->bytes.size()] ^= 0x01;
-        } else if (what == 1) {
-            mod->block_len += 1;
-        } else {
-            mod->index = (mod->index + 1) % (bm->tot);
-        }
-        it->second = std::move(mod);
-        return GARAGE_BM_OK;
-    }
-    FILE *f = fopen(nd.path_of(h, ".shard").c_str(), "r+b");
-    if (!f) return GARAGE_BM_E_MISSING_BLOCK;
-    ShardFileHeader hd;
-    int rc = GARAGE_BM_E_MISSING_BLOCK;
-    if (fread(&hd, sizeof(hd), 1, f) == 1) {
-        long off = -1;
-        uint8_t b = 0;
-        if (what == 0 && hd.shard_len) off = (long)sizeof(hd) + (long)(byte_off % hd.shard_len);
-        else if (what == 1) off = offsetof(ShardFileHeader, block_len);
-        else if (what == 2) off = offsetof(ShardFileHeader, index);
-        if (off >= 0 && fseek(f, off, SEEK_SET) == 0 && fread(&b, 1, 1, f) == 1) {
-            b = what == 0 ? (uint8_t)(b ^ 1) : (uint8_t)(b + 1);
-            if (fseek(f, off, SEEK_SET) == 0 && fwrite(&b, 1, 1, f) == 1) rc = GARAGE_BM_OK;
-        }
-    }
-    fclose(f);
-    return rc;
+    return nd.store_corrupt(to_hash(hash), byte_off, what);
 }
 
 int garage_bm_corrupt_shard(garage_bm *bm, int node, const uint8_t hash[32], size_t byte_off)
