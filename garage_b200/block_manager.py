@@ -26,7 +26,7 @@ SUM_BLAKE2, SUM_ADLER8 = 0, 1
 
 class Code(C.Structure):
     """garage_bm_code: a code the store may still hold shards of"""
-    _fields_ = [("k", C.c_int), ("m", C.c_int), ("local_groups", C.c_int), ("piggyback", C.c_int)]
+    _fields_ = [("k", C.c_int), ("m", C.c_int), ("local_groups", C.c_int), ("piggyback", C.c_int), ("clay", C.c_int)]
 
 
 class LayoutSpec(C.Structure):
@@ -49,7 +49,7 @@ class Config(C.Structure):
                 ("shard_sum_kind", C.c_int), ("verify_content_hash", C.c_int), ("data_fsync", C.c_int),
                 ("block_gc_delay_ms", C.c_uint32), ("local_groups", C.c_int), ("piggyback", C.c_int),
                 ("previous_codes", C.POINTER(Code)), ("n_previous_codes", C.c_int), ("legacy_replicas", C.c_int),
-                ("layout", C.POINTER(LayoutSpec)), ("clay", C.c_int)]
+                ("layout", C.POINTER(LayoutSpec)), ("clay", C.c_int), ("clay_layout", C.c_int)]
 
 
 class Metrics(C.Structure):
@@ -61,7 +61,8 @@ class Metrics(C.Structure):
         "convert_blocks", "convert_bytes_read", "convert_bytes_written", "convert_errors", "convert_call_us", "legacy_gets",
         "legacy_deleted", "layout_shards_copied", "layout_shards_rebuilt", "layout_bytes_read", "layout_bytes_written",
         "layout_deleted", "layout_sync_errors", "layout_version", "resync_bytes_fetched", "deep_scrub_blocks",
-        "deep_scrub_skipped", "deep_scrub_parity_bad", "deep_scrub_content_errors", "deep_check_call_us")]
+        "deep_scrub_skipped", "deep_scrub_parity_bad", "deep_scrub_content_errors", "deep_check_call_us",
+        "layout_bytes_fetched")]
 
 
 _lib = None
@@ -133,11 +134,11 @@ class BlockManager:
     def __init__(self, k=10, m=4, n_nodes=None, cuda_device=0, batch_max_blocks=64, batch_linger_us=100,
                  block_ram_buffer_max=256 << 20, data_dir=None, shard_sum_kind=SUM_ADLER8, verify_content_hash=True,
                  data_fsync=False, block_gc_delay_ms=0, local_groups=0, piggyback=False, previous_codes=(),
-                 legacy_replicas=0, layout=None, clay=False):
+                 legacy_replicas=0, layout=None, clay=False, clay_layout=False):
         """block_gc_delay_ms defaults to 0 HERE (tests delete at once); the library's default is the
         reference's BLOCK_GC_DELAY of 10 minutes.  local_groups > 0: LRC(k, local_groups, m - local_groups).
-        piggyback: PB(k, m), half-shard repair reads.  clay: Clay(k, m), a lost shard rebuilt from 1/m of the others.  previous_codes: (k, m, local_groups, piggyback) tuples of
-        codes the store may still hold; legacy_replicas: replication factor of a previous replicated layout.
+        piggyback: PB(k, m), half-shard repair reads.  clay: Clay(k, m), a lost shard rebuilt from 1/m of the others; clay_layout: that store may change its
+        layout.  previous_codes: (k, m, local_groups, piggyback[, clay]) tuples of codes the store may still hold; legacy_replicas: replication factor of a previous replicated layout.
         layout: None (partition p on nodes (p mod n_nodes) + i) or a dict with zone, capacity and optionally
         zone_redundancy, max_per_zone: version 1 of the cluster layout."""
         self._L = load_library()
@@ -152,6 +153,7 @@ class BlockManager:
         cfg.local_groups = local_groups
         cfg.piggyback = 1 if piggyback else 0
         cfg.clay = 1 if clay else 0
+        cfg.clay_layout = int(clay_layout)
         self._prev = (Code * max(1, len(previous_codes)))(*[Code(*map(int, c)) for c in previous_codes])  # kept alive
         cfg.previous_codes = C.cast(self._prev, C.POINTER(Code)) if previous_codes else None
         cfg.n_previous_codes, cfg.legacy_replicas = len(previous_codes), legacy_replicas

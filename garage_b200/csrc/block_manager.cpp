@@ -316,7 +316,7 @@ bool write_file_atomic(const std::string &path, const void *a, size_t na, const 
     return ok;
 }
 
-// a code shards are stored under: RS(k, m), LRC(k, l, m - l) or PB(k, m)
+// a code shards are stored under: RS(k, m), LRC(k, l, m - l), PB(k, m) or Clay(k, m)
 struct CodeDesc {
     int k = 0, m = 0, l = 0;  // l: LRC local groups, 0 = RS
     bool pb = false;          // piggybacked RS PB(k, m): shard_len = ceil(block_len / k) rounded up to 128
@@ -1084,7 +1084,7 @@ struct garage_bm {
     std::atomic<uint64_t> convert_blocks{0}, convert_bytes_read{0}, convert_bytes_written{0}, convert_errors{0},
         convert_call_us{0}, legacy_gets{0}, legacy_deleted{0};
     std::atomic<uint64_t> layout_shards_copied{0}, layout_shards_rebuilt{0}, layout_bytes_read{0}, layout_bytes_written{0},
-        layout_deleted{0}, layout_sync_errors{0};
+        layout_deleted{0}, layout_sync_errors{0}, layout_bytes_fetched{0};
 
     // Bytes a rebuild from the shards `have` hands to the GPU, which is what crosses the network in Garage: the runs
     // garage_ec_read_ranges names for a Clay stripe (1/m of each helper for a lone lost shard), else what was read
@@ -1809,9 +1809,13 @@ struct garage_bm {
         uint64_t nbytes = 0;
         resync_shards_read += (uint64_t)gather_into(h, node, slot.p, have, block_len, false, /*for_gpu=*/true, want, &ok,
                                                     &nbytes);
+        const uint64_t fetched = ok ? fetched_bytes(have, want, block_len, nbytes) : nbytes;
         resync_bytes_read += nbytes;
-        resync_bytes_fetched += ok ? fetched_bytes(have, want, block_len, nbytes) : nbytes;
-        if (multi) layout_bytes_read += nbytes;
+        resync_bytes_fetched += fetched;
+        if (multi) {
+            layout_bytes_read += nbytes;
+            layout_bytes_fetched += fetched;
+        }
         if (!ok) {
             // no configured stripe to rebuild from, but maybe a block stored before the code changed: convert it
             if (has_legacy() && convert_batch({h}) == 1) {
@@ -1863,6 +1867,7 @@ struct garage_bm {
             ShardMeta mt;
             if (y == node || !read_shard_into(y, h, buf, slot_stride, mt, false, 0, idx)) continue;
             layout_bytes_read += mt.shard_len;
+            layout_bytes_fetched += mt.shard_len;
             if (mt.index != idx || (have_expect && mt.block_len != expect)) {
                 quarantine(y, h, 0, idx);  // a self-consistent shard of another block length: stale
                 continue;
@@ -1904,6 +1909,7 @@ struct garage_bm {
                 uint64_t nbytes = 0;
                 gather_into(h, node, it.stripe, it.present, it.block_len, false, /*for_gpu=*/true, it.want, &g, &nbytes);
                 layout_bytes_read += nbytes;
+                layout_bytes_fetched += g ? fetched_bytes(it.present, it.want, it.block_len, nbytes) : nbytes;
                 ok[j] = g;
             });
             std::vector<ReconItem *> batch;
@@ -1977,6 +1983,7 @@ struct garage_bm {
                 write_shard(who[i], h, i, mt.block_len, buf, mt.shard_len, mt.sum.data(), true)) {
                 layout_shards_copied++;
                 layout_bytes_read += mt.shard_len;
+                layout_bytes_fetched += mt.shard_len;
                 layout_bytes_written += mt.shard_len;
                 pushed++;
             } else {
@@ -2171,7 +2178,7 @@ struct garage_bm {
     // garage_bm_apply_layout: see include/garage_block_manager.h
     int apply_layout(const garage_bm_layout_spec *spec, uint64_t *version_out)
     {
-        if (nodes[0]->dir.empty() || has_legacy() || codes[0].clay) return GARAGE_EC_E_INVALID;
+        if (nodes[0]->dir.empty() || has_legacy() || (codes[0].clay && !cfg.clay_layout)) return GARAGE_EC_E_INVALID;
         std::lock_guard<std::mutex> lk(layout_mu);
         const auto ls = layouts();
         if (!ls->newest() || ls->v.size() >= GARAGE_BM_MAX_LAYOUT_VERSIONS) return GARAGE_EC_E_INVALID;
@@ -2284,7 +2291,9 @@ struct garage_bm {
                         gather_into(h, -1, slot, have, len, false, true, nullptr, &ok, &nbytes, c);
                         bool degraded = false;
                         for (int i = 0; i < codes[c].k; i++) degraded |= !have[i];
-                        if (ok && degraded)  // every survivor whole: the transcode reads what its own plan names
+                        // every survivor whole: the transcode reads what its own plan names (a Clay read set is
+                        // whole shards already)
+                        if (ok && degraded && !codes[c].clay)
                             gather_into(h, -1, slot, have, len, true, true, nullptr, &ok, &nbytes, c);
                     }
                     convert_bytes_read += nbytes;
@@ -2891,16 +2900,22 @@ void garage_bm_default_config(garage_bm_config *c)
     c->legacy_replicas = 0;
     c->layout = nullptr;            // the fixed ring
     c->clay = 0;                    // not Clay
+    c->clay_layout = 0;             // a Clay store keeps the fixed ring
 }
 
-// a code garage_ec_create / _lrc / _piggyback accepts, with tags the block manager can check; the rules of the
+// a code garage_ec_create / _lrc / _piggyback / _clay accepts, with tags the block manager can check; the rules of the
 // configured code and of every previous code (PB: 1 <= k <= 16, 2 <= m <= 4, no LRC groups, and adler8 tags for its
-// half reads)
-static bool code_ok(int k, int m, int l, int piggyback, int sum_kind)
+// half reads; Clay: k >= 2, 2 <= m <= 4, alpha = m^ceil((k+m)/m) <= 256, neither LRC groups nor PB)
+static bool code_ok(int k, int m, int l, int piggyback, int clay, int sum_kind)
 {
     if (k < 1 || m < 1 || k > GARAGE_EC_MAX_K || m > GARAGE_EC_MAX_M) return false;
     if (l < 0 || (l > 0 && (l >= m || k % l))) return false;
-    if (piggyback != 0 && piggyback != 1) return false;
+    if ((piggyback != 0 && piggyback != 1) || (clay != 0 && clay != 1)) return false;
+    if (clay) {
+        int alpha = 1;
+        for (int t = (k + m + m - 1) / m; t > 0 && alpha <= 256; t--) alpha *= m;
+        return m >= 2 && m <= 4 && k >= 2 && alpha <= 256 && !piggyback && l == 0;
+    }
     return !piggyback || (l == 0 && k <= 16 && m >= 2 && m <= 4 && sum_kind != GARAGE_EC_SUM_BLAKE2);
 }
 
@@ -2919,30 +2934,27 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
 {
     *out = nullptr;
     const int k = cfg->data_shards, m = cfg->parity_shards, l = cfg->local_groups;
-    if (!code_ok(k, m, l, cfg->piggyback, cfg->shard_sum_kind) || cfg->n_nodes < k + m || cfg->n_nodes > 256)
+    if (!code_ok(k, m, l, cfg->piggyback, cfg->clay, cfg->shard_sum_kind) || cfg->n_nodes < k + m || cfg->n_nodes > 256)
         return GARAGE_EC_E_INVALID;
     if (cfg->shard_sum_kind != GARAGE_EC_SUM_BLAKE2 && cfg->shard_sum_kind != GARAGE_EC_SUM_ADLER8) return GARAGE_EC_E_INVALID;
     const bool pb = cfg->piggyback != 0;
-    // Clay(k, m) (garage_ec_create_clay's rules): not combined with LRC or PB, and without layout changes
+    // a Clay store changes its layout only with clay_layout
     const bool clay = cfg->clay != 0;
-    if (cfg->clay != 0 && cfg->clay != 1) return GARAGE_EC_E_INVALID;
-    if (clay) {
-        int alpha = 1;
-        for (int t = (k + m + m - 1) / m; t > 0 && alpha <= 256; t--) alpha *= m;
-        if (m < 2 || m > 4 || k < 2 || alpha > 256 || pb || l > 0 || cfg->layout) return GARAGE_EC_E_INVALID;
-    }
+    if ((cfg->clay_layout != 0 && cfg->clay_layout != 1) || (cfg->clay_layout && !clay)) return GARAGE_EC_E_INVALID;
+    if (clay && cfg->layout && !cfg->clay_layout) return GARAGE_EC_E_INVALID;
     // previous codes and replicas (all checked before any CUDA call)
     const int np = cfg->n_previous_codes;
     if (np < 0 || np > GARAGE_BM_MAX_PREVIOUS_CODES || (np > 0 && !cfg->previous_codes)) return GARAGE_EC_E_INVALID;
     if (cfg->legacy_replicas < 0 || cfg->legacy_replicas > cfg->n_nodes) return GARAGE_EC_E_INVALID;
     for (int i = 0; i < np; i++) {
         const garage_bm_code &p = cfg->previous_codes[i];
-        if (!code_ok(p.k, p.m, p.local_groups, p.piggyback, cfg->shard_sum_kind) || p.k + p.m > cfg->n_nodes)
+        if (!code_ok(p.k, p.m, p.local_groups, p.piggyback, p.clay, cfg->shard_sum_kind) || p.k + p.m > cfg->n_nodes)
             return GARAGE_EC_E_INVALID;
-        if (!clay && p.k == k && p.m == m && p.local_groups == l && (p.piggyback != 0) == pb) return GARAGE_EC_E_INVALID;
+        if (p.k == k && p.m == m && p.local_groups == l && (p.piggyback != 0) == pb && (p.clay != 0) == clay)
+            return GARAGE_EC_E_INVALID;
         for (int j = 0; j < i; j++) {
             const garage_bm_code &q = cfg->previous_codes[j];
-            if (p.k == q.k && p.m == q.m && p.local_groups == q.local_groups && p.piggyback == q.piggyback)
+            if (p.k == q.k && p.m == q.m && p.local_groups == q.local_groups && p.piggyback == q.piggyback && p.clay == q.clay)
                 return GARAGE_EC_E_INVALID;
         }
     }
@@ -2964,7 +2976,7 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
     }
     // a store changes its layout or its code, not both at once
     if (lays->v.size() > 1 && (np > 0 || cfg->legacy_replicas > 0)) return GARAGE_EC_E_INVALID;
-    if (clay && layout_file) return GARAGE_EC_E_INVALID;  // a Clay store keeps the fixed ring
+    if (clay && layout_file && !cfg->clay_layout) return GARAGE_EC_E_INVALID;  // a Clay store keeps the fixed ring
     std::unique_ptr<garage_bm> bm(new garage_bm());
     bm->cfg = *cfg;
     if (!bm->cfg.block_size) bm->cfg.block_size = 1u << 20;
@@ -2980,12 +2992,12 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
     int rc = GARAGE_EC_OK;
     for (int i = 0; i <= np; i++) {
         garage_bm::Code &c = bm->codes[i];
-        const garage_bm_code p = i ? cfg->previous_codes[i - 1] : garage_bm_code{k, m, l, cfg->piggyback};
+        const garage_bm_code p = i ? cfg->previous_codes[i - 1] : garage_bm_code{k, m, l, cfg->piggyback, cfg->clay};
         c.k = p.k;
         c.m = p.m;
         c.l = p.local_groups;
         c.pb = p.piggyback != 0;
-        c.clay = i == 0 && clay;
+        c.clay = p.clay != 0;
         c.tot = p.k + p.m;
         rc = create_ctx(c, cfg->cuda_device, bm->sum_kind, &c.ctx);
         if (rc != GARAGE_EC_OK) {  // no GPU => no block manager: there is no CPU fallback
@@ -3400,6 +3412,7 @@ void garage_bm_get_metrics(garage_bm *bm, garage_bm_metrics *o)
     o->layout_bytes_written = bm->layout_bytes_written;
     o->layout_deleted = bm->layout_deleted;
     o->layout_sync_errors = bm->layout_sync_errors;
+    o->layout_bytes_fetched = bm->layout_bytes_fetched;
     o->layout_version = garage_layout_version(bm->layouts()->newest());
     uint64_t ql = 0;
     for (auto &n : bm->nodes) {

@@ -42,11 +42,12 @@ extern "C" {
 
 typedef struct garage_bm garage_bm;
 
-/* a code the store may still hold shards of: RS(k, m), LRC(k, local_groups, m - local_groups) or PB(k, m) */
+/* a code the store may still hold shards of: RS(k, m), LRC(k, local_groups, m - local_groups), PB(k, m) or Clay(k, m) */
 typedef struct {
     int k, m;
     int local_groups; /* 0: not LRC */
     int piggyback;    /* 0 or 1 */
+    int clay;         /* 0 or 1: Clay(k, m), garage_ec_create_clay's rules; not with local_groups or piggyback */
 } garage_bm_code;
 
 #define GARAGE_BM_MAX_PREVIOUS_CODES 4
@@ -94,7 +95,8 @@ typedef struct {
     /* Changing a store's code (file store; DESIGN.md section 5.1).  Default: none, and a shard of any code but the
        configured one is quarantined.  GARAGE_EC_E_INVALID before any CUDA call for: more than
        GARAGE_BM_MAX_PREVIOUS_CODES entries, a NULL list with entries, an entry equal to the configured code or to
-       another entry, an entry garage_ec_create* would reject or with more than n_nodes shards, a PB entry with
+       another entry (k, m, local_groups, piggyback and clay all equal: Clay(6,3) may precede Clay(10,4), and RS(10,4)
+       may), an entry garage_ec_create* would reject or with more than n_nodes shards, a PB entry with
        GARAGE_EC_SUM_BLAKE2 tags, legacy_replicas < 0 or > n_nodes.                                               */
     const garage_bm_code *previous_codes; /* codes whose shards are read and converted (old .shard / .legacy files) */
     int n_previous_codes;
@@ -113,9 +115,15 @@ typedef struct {
                                        their whole shard's tag first, a bad one is quarantined and the rebuild falls
                                        back to k whole shards).  Recorded in the shard file header (pad[1] = 2); a
                                        shard of another code is quarantined.  GARAGE_EC_E_INVALID with
-                                       local_groups > 0, piggyback, `layout` set or a layout file on disk;
-                                       garage_bm_apply_layout refuses a Clay store.  Conversion to Clay works
-                                       through previous_codes                                                     */
+                                       local_groups > 0 or piggyback, and, unless clay_layout is set, with `layout`
+                                       set or a layout file on disk; garage_bm_apply_layout then refuses the store
+                                       too.  Conversion to and from Clay works through previous_codes             */
+    int clay_layout;                /* 0 (default): a Clay store keeps the fixed ring, as above.  1: a Clay store
+                                       takes `layout`, a layout file and garage_bm_apply_layout like any other code
+                                       (DESIGN.md section 5.3): a shard no active version has a copy of is rebuilt
+                                       from the garage_ec_read_ranges runs of the others, each one read whole from
+                                       the first version that has it.  GARAGE_EC_E_INVALID without clay, or for any
+                                       other value                                                                */
 } garage_bm_config;
 
 typedef struct {
@@ -156,6 +164,9 @@ typedef struct {
     uint64_t deep_scrub_parity_bad;          /* stale parity shards it quarantined                               */
     uint64_t deep_scrub_content_errors;      /* blocks whose content hash failed and whose hunt found no culprit */
     uint64_t deep_check_call_us;             /* wall time inside garage_ec_deep_check                            */
+    uint64_t layout_bytes_fetched;           /* bytes handed to layout copies and rebuilds: what would cross the network
+                                                in Garage.  A Clay repair counts its runs (1/m of each helper);
+                                                everything else equals layout_bytes_read                            */
 } garage_bm_metrics;
 
 void garage_bm_default_config(garage_bm_config *cfg);

@@ -1,5 +1,6 @@
-"""Rate of changing a store's code: a file store of N blocks stored under RS(6,3), and separately as rf = 3 plain
-replicas, is restarted as RS(10,4) and converted by one convert_step sweep over every node.
+"""Rate of changing a store's code: a file store of N blocks stored under RS(6,3), separately as rf = 3 plain
+replicas, and separately under Clay(10,4) (--sources clay104), is restarted as RS(10,4) and converted by one
+convert_step sweep over every node.
 
 Reports GiB/s of block bytes over the sweep's wall time, the share of that time spent inside garage_ec_transcode, and
 the bytes read and written per block against the algorithmic k_s*L_s read and (k_d+m_d)*L_d written.  The store lives
@@ -54,6 +55,12 @@ def run(source, nblocks, block_len, base):
                 for h, b in zip(hashes, blocks):
                     assert old.rpc_put_block(h, b) == BM.OK
             kw, read_alg = {"previous_codes": [(6, 3, 0, 0)]}, 6 * -(-block_len // 6)
+        elif source == "clay104":
+            with BM.BlockManager(10, 4, n_nodes=N_NODES, data_dir=d, clay=True) as old:
+                for h, b in zip(hashes, blocks):
+                    assert old.rpc_put_block(h, b) == BM.OK
+            L = -(-(-(-block_len // 10)) // 4096) * 4096  # rounded up to 16 * alpha
+            kw, read_alg = {"previous_codes": [(10, 4, 0, 0, 1)]}, 10 * L
         else:
             for h, b in zip(hashes, blocks):
                 write_replicas(d, h, b, 3)
@@ -82,7 +89,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--blocks", type=int, default=256)
     ap.add_argument("--block-len", type=int, default=1 << 20)
-    ap.add_argument("--sources", default="rs63,rep3")
+    ap.add_argument("--sources", default="rs63,rep3,clay104")
     a = ap.parse_args()
     base = "/dev/shm" if os.path.isdir("/dev/shm") and os.access("/dev/shm", os.W_OK) else None
     res = [run(s, a.blocks, a.block_len, base) for s in a.sources.split(",")]
