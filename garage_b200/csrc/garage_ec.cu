@@ -686,6 +686,7 @@ uint64_t code_shard_len(const garage_ec_ctx *ctx, uint32_t block_len)
 struct CopyBatch {
     std::vector<void *> dst, src;
     std::vector<size_t> sz;
+    bool use_batch = true;  // false: the host side is pageable memory, copied piece by piece
     void add(void *d, const void *s, size_t n)
     {
         if (!n) return;
@@ -709,7 +710,7 @@ struct CopyBatch {
             return set_cuda_error(ctx, cudaErrorUnknown, "injected fault at batched copy");
         }
         bool done = false;
-        if (cnt > 1 && ctx->batch_copy_ok.load(std::memory_order_relaxed)) {
+        if (cnt > 1 && use_batch && ctx->batch_copy_ok.load(std::memory_order_relaxed)) {
             cudaMemcpyAttributes attr;
             memset(&attr, 0, sizeof(attr));
             attr.srcAccessOrder = cudaMemcpySrcAccessOrderStream;
@@ -1509,6 +1510,12 @@ static int reconstruct_host(garage_ec_ctx *ctx, uint8_t *shards, uint8_t *const 
     // writes the rebuilt shards into, the caller's buffer over PCIe -- nothing staged
     const bool zero_copy = !ctx->clay && !stripes && device_addressable_host(shards);
     HostPipeline p(ctx, n, zero_copy ? 0 : tot * stride);
+    // cudaMemcpyBatchAsync gets pinned stripes only.  Batches of thousands of pageable survivor pieces (ragged
+    // lengths, PB halves, Clay repair runs) crashed the process or faulted the context; pageable stripes are copied
+    // piece by piece, which the driver stages through its own pinned buffers.
+    bool pinned = !zero_copy;
+    for (size_t s = 0; pinned && s < (stripes ? n : 1); s++) pinned = device_addressable_host(stripes ? stripes[s] : shards);
+    p.up.use_batch = p.down.use_batch = pinned;
     SmallLayout sl;
     const size_t o_present = sl.take(p.cs * tot), o_want = sl.take(p.cs * tot), o_status = sl.take(p.cs * 4),
                  o_len = sl.take(p.cs * 4), o_plan = sl.take(plan_scratch_bytes(ctx, p.cs));
