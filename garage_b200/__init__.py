@@ -41,6 +41,8 @@ ABI_SYMBOLS = [
     "garage_ec_check_shard_half_host", "garage_ec_transcode",
     "garage_ec_create_clay", "garage_ec_clay_info", "garage_ec_read_ranges",
     "garage_ec_deep_check",
+    "garage_ec_tag_span", "garage_ec_check_shard_span_host", "garage_ec_range_plan", "garage_ec_decode_range",
+    "garage_ec_decode_range_stripes",
 ]
 
 
@@ -130,6 +132,11 @@ def load_library(build=True):
     L.garage_ec_clay_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), vp]
     L.garage_ec_read_ranges.argtypes = [vp, vp, vp, u32, vp, sz, C.POINTER(sz)]
     L.garage_ec_deep_check.argtypes = [vp, vp, vp, vp, vp, vp, sz, sz, i32, vp]
+    L.garage_ec_tag_span.argtypes = [i32, u32, u32, u32, C.POINTER(u32), C.POINTER(u32)]
+    L.garage_ec_check_shard_span_host.argtypes = [i32, vp, u32, u32, u32, vp]
+    L.garage_ec_range_plan.argtypes = [vp, vp, u32, u32, u32, vp, sz, C.POINTER(sz), C.POINTER(i32)]
+    L.garage_ec_decode_range.argtypes = [vp, vp, vp, vp, vp, vp, sz, vp, sz, vp, sz, i32, vp]
+    L.garage_ec_decode_range_stripes.argtypes = [vp, vp, vp, vp, vp, vp, sz, vp, vp, sz]
     _lib = L
     return L
 
@@ -165,6 +172,26 @@ def check_shard_half_host(kind, half, shard_len, which, tag) -> int:
     t = np.frombuffer(bytes(tag), dtype=np.uint8)
     return L.garage_ec_check_shard_half_host(kind, C.c_void_p(a.ctypes.data) if a.size else None, shard_len, which,
                                              C.c_void_p(t.ctypes.data))
+
+
+def tag_span(kind, shard_len, off, length):
+    """garage_ec_tag_span: (span_off, span_len) of the whole tag segments covering [off, off + length) of a shard"""
+    L = load_library()
+    a, b = C.c_uint32(0), C.c_uint32(0)
+    rc = L.garage_ec_tag_span(kind, shard_len, off, length, C.byref(a), C.byref(b))
+    if rc:
+        raise EcError(rc, "tag_span")
+    return a.value, b.value
+
+
+def check_shard_span_host(kind, span, shard_len, span_off, tag) -> int:
+    """garage_ec_check_shard_span_host: 0 if `span` (the bytes of a tag span at span_off) matches the 32-byte tag,
+    1 if not, or an E_* code"""
+    L = load_library()
+    a = np.frombuffer(bytes(span), dtype=np.uint8) if not isinstance(span, np.ndarray) else np.ascontiguousarray(span)
+    t = np.frombuffer(bytes(tag), dtype=np.uint8)
+    return L.garage_ec_check_shard_span_host(kind, C.c_void_p(a.ctypes.data) if a.size else None, shard_len, span_off,
+                                             a.size, C.c_void_p(t.ctypes.data))
 
 
 def copy_for_dma(dst, src):
@@ -328,6 +355,38 @@ class GarageEc:
         if rc == E_UNRECOVERABLE:
             return None
         return [tuple(int(v) for v in out[3 * i:3 * i + 3]) for i in range(n.value)]
+
+    def range_plan(self, present, block_len, offset, length):
+        """(runs [(shard, offset, len)], needs_gpu) for bytes [offset, offset + length) of one block, or (None,
+        needs_gpu) if the absent touched data shards cannot be rebuilt"""
+        pr = np.ascontiguousarray(present, dtype=np.uint8)
+        assert pr.shape == (self.k + self.m,)
+        cap = (self.k + self.m) * 512
+        out = np.zeros(cap * 3, dtype=np.uint32)
+        n, g = C.c_size_t(0), C.c_int(0)
+        rc = self._check(self._L.garage_ec_range_plan(self._h, _ptr(pr), block_len, offset, length, _ptr(out), cap,
+                                                      C.byref(n), C.byref(g)), (E_UNRECOVERABLE,))
+        if rc == E_UNRECOVERABLE:
+            return None, g.value
+        return [tuple(int(v) for v in out[3 * i:3 * i + 3]) for i in range(n.value)], g.value
+
+    def decode_range(self, shards, present, block_len, offset, length, stride, out, out_stride, status=None):
+        """garage_ec_decode_range of n = len(block_len) requests (uint32 arrays, numpy or device tensors)"""
+        kind, st = self._stream(shards)
+        return self._check(self._L.garage_ec_decode_range(self._h, _ptr(shards), _ptr(present), _ptr(block_len),
+                                                          _ptr(offset), _ptr(length), stride, _ptr(out), out_stride,
+                                                          _ptr(status), len(block_len), kind, st),
+                           (E_UNRECOVERABLE,))
+
+    def decode_range_stripes(self, stripes, present, block_len, offset, length, stride, outs, status=None):
+        """gather form: `stripes` / `outs` are lists of numpy arrays, one per request"""
+        n = len(stripes)
+        sp = (C.c_void_p * n)(*[a.ctypes.data for a in stripes])
+        op = (C.c_void_p * n)(*[a.ctypes.data for a in outs])
+        return self._check(self._L.garage_ec_decode_range_stripes(self._h, C.cast(sp, C.c_void_p), _ptr(present),
+                                                                  _ptr(block_len), _ptr(offset), _ptr(length), stride,
+                                                                  C.cast(op, C.c_void_p), _ptr(status), n),
+                           (E_UNRECOVERABLE,))
 
     def code_shard_len(self, block_len):
         """shard length of a block under this context's code (PB: rounded up to 128 bytes)"""

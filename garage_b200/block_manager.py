@@ -19,7 +19,8 @@ SYMBOLS = [
     "garage_bm_block_incref", "garage_bm_block_decref", "garage_bm_get_block_rc", "garage_bm_scrub_step",
     "garage_bm_bench", "garage_bm_corrupt_shard_header", "garage_bm_plant_stale_shard", "garage_bm_set_node_readonly",
     "garage_bm_convert_step", "garage_bm_debug_convert_stop_after", "garage_bm_apply_layout", "garage_bm_layout_sync_step",
-    "garage_bm_layout_versions", "garage_bm_deep_scrub_step",
+    "garage_bm_layout_versions", "garage_bm_deep_scrub_step", "garage_bm_rpc_get_block_range",
+    "garage_bm_get_range_metrics",
 ]
 SUM_BLAKE2, SUM_ADLER8 = 0, 1
 
@@ -65,6 +66,10 @@ class Metrics(C.Structure):
         "layout_bytes_fetched")]
 
 
+class RangeMetrics(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("range_gets", "range_degraded", "range_bytes_read", "range_bytes_fetched")]
+
+
 _lib = None
 
 
@@ -98,6 +103,9 @@ def load_library():
         L.garage_bm_node_shard_index.argtypes = [vp, i32, vp]
         L.garage_bm_storage_nodes_of.argtypes = [vp, vp, C.POINTER(i32)]
         L.garage_bm_get_metrics.argtypes = [vp, C.POINTER(Metrics)]
+        L.garage_bm_get_range_metrics.argtypes = [vp, C.POINTER(RangeMetrics)]
+        L.garage_bm_get_range_metrics.restype = None
+        L.garage_bm_rpc_get_block_range.argtypes = [vp, vp, C.c_uint32, C.c_uint32, vp, sz, C.POINTER(sz)]
         L.garage_bm_get_metrics.restype = None
         L.garage_bm_bench.argtypes = [vp, i32, i32, C.c_uint32, i32, C.c_uint64, C.POINTER(C.c_double), C.POINTER(C.c_uint64)]
         L.garage_bm_corrupt_shard_header.argtypes = [vp, i32, vp, i32]
@@ -198,6 +206,14 @@ class BlockManager:
         out = np.empty(cap, dtype=np.uint8)
         n = C.c_size_t(0)
         rc = self._L.garage_bm_rpc_get_block(self._h, self._hp(hash32), C.c_void_p(out.ctypes.data), cap, C.byref(n))
+        return rc, (out[: n.value].copy() if rc == OK else None)
+
+    def rpc_get_block_range(self, hash32, offset, length):
+        """(rc, bytes [offset, offset + length) of the block or None)"""
+        out = np.empty(max(length, 1), dtype=np.uint8)
+        n = C.c_size_t(0)
+        rc = self._L.garage_bm_rpc_get_block_range(self._h, self._hp(hash32), offset, length, C.c_void_p(out.ctypes.data),
+                                                   length, C.byref(n))
         return rc, (out[: n.value].copy() if rc == OK else None)
 
     def block_incref(self, hash32):
@@ -337,7 +353,11 @@ class BlockManager:
     def metrics(self):
         mt = Metrics()
         self._L.garage_bm_get_metrics(self._h, C.byref(mt))
-        return {n: getattr(mt, n) for n, _ in Metrics._fields_}
+        rm = RangeMetrics()
+        self._L.garage_bm_get_range_metrics(self._h, C.byref(rm))
+        out = {n: getattr(mt, n) for n, _ in Metrics._fields_}
+        out.update({n: getattr(rm, n) for n, _ in RangeMetrics._fields_})
+        return out
 
 
 # ---- shard wire format (include/garage_shard_wire.h) ---------------------------------------------

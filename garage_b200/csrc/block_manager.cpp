@@ -265,6 +265,42 @@ std::string hex_of(const uint8_t *p, size_t n)
 
 enum ReadResult { kReadOk = 0, kReadMissing = 1, kReadInvalid = 2 };
 
+// A run of a shard's bytes for a ranged read: the whole shard (the default), one PB half -- its length comes from the
+// header read with it -- or explicit bytes [off, off + len)
+struct ShardSpan {
+    int half = -1;
+    uint32_t off = 0, len = UINT32_MAX;  // UINT32_MAX: the whole shard
+    static ShardSpan of_half(int h)
+    {
+        ShardSpan s;
+        s.half = h;
+        return s;
+    }
+    static ShardSpan bytes(uint32_t off, uint32_t len)
+    {
+        ShardSpan s;
+        s.off = off;
+        s.len = len;
+        return s;
+    }
+    bool whole() const { return half < 0 && len == UINT32_MAX; }
+    // [off, off + n) of a shard of L bytes; false if the span does not fit in it
+    bool resolve(uint32_t L, size_t &off_out, size_t &n) const
+    {
+        if (half >= 0) {
+            off_out = (size_t)half * (L / 2);
+            n = L / 2;
+        } else if (len == UINT32_MAX) {
+            off_out = 0;
+            n = L;
+        } else {
+            off_out = off;
+            n = len;
+        }
+        return (uint64_t)off_out + n <= L;
+    }
+};
+
 // the header of the shard file at `path`: kReadMissing (no such file), kReadInvalid (short, or a wrong magic or header
 // check) or kReadOk.  keep != NULL: on kReadOk the open file is handed over there, positioned after the header
 ReadResult read_header(const std::string &path, ShardFileHeader &hd, FILE **keep = nullptr)
@@ -517,23 +553,23 @@ struct Node {
         return write_file_atomic(path_of(h, other && !aside ? ".legacy" : ".shard"), &hd, sizeof(hd), bytes, n, fsync_data,
                                  fsync_data);
     }
-    // shard bytes straight into `dst` (cap bytes available), metadata into `mt`.  half = 0 / 1: only the a- / b-half
-    // [half * shard_len/2, (half+1) * shard_len/2) of a PB shard, one ranged read at 64 + half * shard_len/2 of the
-    // file, into dst (which then holds shard_len/2 bytes)
+    // shard bytes straight into `dst` (cap bytes available), metadata into `mt`.  A span other than the whole shard
+    // is one ranged read of its bytes only, into dst (which then holds the span's bytes); an empty span reads and checks
+    // the header alone.  Only the node knows where a shard's bytes sit in its file.
     // index >= 0 (by_index stores): the file holding that index
-    ReadResult store_read_into(const Hash &h, uint8_t *dst, size_t cap, ShardMeta &mt, int half = -1, int code = 0,
+    ReadResult store_read_into(const Hash &h, uint8_t *dst, size_t cap, ShardMeta &mt, ShardSpan span = {}, int code = 0,
                                int index = -1) const
     {
         if (dir.empty()) {
             auto it = code == 0 ? shards.find(h) : shards.end();
             if (it == shards.end()) return kReadMissing;
-            return copy_out(*it->second, dst, cap, mt, false, half);
+            return copy_out(*it->second, dst, cap, mt, false, span);
         }
-        if (index >= 0 && by_index) return file_read_into(path_at(h, index), 0, dst, cap, mt, half);
-        return file_read_into(path_for(h, code), code, dst, cap, mt, half);
+        if (index >= 0 && by_index) return file_read_into(path_at(h, index), 0, dst, cap, mt, span);
+        return file_read_into(path_for(h, code), code, dst, cap, mt, span);
     }
     // one shard file read as a shard of `code`
-    ReadResult file_read_into(const std::string &path, int code, uint8_t *dst, size_t cap, ShardMeta &mt, int half = -1) const
+    ReadResult file_read_into(const std::string &path, int code, uint8_t *dst, size_t cap, ShardMeta &mt, ShardSpan span = {}) const
     {
         ShardFileHeader hd;
         FILE *f = nullptr;
@@ -550,25 +586,26 @@ struct Node {
             mt.shard_len = hd.shard_len;
             mt.sum_kind = hd.sum_kind;
             memcpy(mt.sum.data(), hd.sum, 32);
-            if (half < 0) {
+            size_t off = 0, n = 0;
+            if (span.whole()) {
                 if (meta_valid(mt, code) && mt.shard_len <= cap && (mt.shard_len == 0 || fread(dst, mt.shard_len, 1, f) == 1))
                     r = kReadOk;
-            } else {
-                const size_t hl = mt.shard_len / 2;
-                if (c.pb && meta_valid(mt, code) && hl <= cap &&
-                    (hl == 0 || ::pread(fileno(f), dst, hl, (off_t)(sizeof(hd) + (size_t)half * hl)) == (ssize_t)hl))
-                    r = kReadOk;
+            } else if ((span.half < 0 || c.pb) && meta_valid(mt, code) && span.resolve(mt.shard_len, off, n) && n <= cap &&
+                       (n == 0 || ::pread(fileno(f), dst, n, (off_t)(sizeof(hd) + off)) == (ssize_t)n)) {
+                r = kReadOk;
             }
         }
         fclose(f);
         return r;
     }
     ReadResult copy_out(const StoredShard &sh, uint8_t *dst, size_t cap, ShardMeta &mt, bool for_dma = false,
-                        int half = -1) const
+                        ShardSpan span = {}) const
     {
         mt = sh;
-        const size_t off = half < 0 ? 0 : (size_t)half * (mt.shard_len / 2), n = half < 0 ? mt.shard_len : mt.shard_len / 2;
-        if (!meta_valid(mt) || sh.bytes.size() != mt.shard_len || n > cap || (half >= 0 && !codes[0].pb)) return kReadInvalid;
+        size_t off = 0, n = 0;
+        if (!meta_valid(mt) || sh.bytes.size() != mt.shard_len || !span.resolve(mt.shard_len, off, n) || n > cap ||
+            (span.half >= 0 && !codes[0].pb))
+            return kReadInvalid;
         if (for_dma) copy_for_dma(dst, sh.bytes.data() + off, n);
         else if (n) memcpy(dst, sh.bytes.data() + off, n);
         return kReadOk;
@@ -600,7 +637,7 @@ struct Node {
     {
         ShardMeta mt;
         for (int c = 0; c < (int)codes.size(); c++)
-            if (store_read_into(h, tmp.data(), tmp.size(), mt, -1, c) == kReadOk) return len = mt.block_len, true;
+            if (store_read_into(h, tmp.data(), tmp.size(), mt, {}, c) == kReadOk) return len = mt.block_len, true;
         if (known) return false;
         if (by_index && !legacy_store() && file_read_into(path_of(h, ".legacy"), 0, tmp.data(), tmp.size(), mt) == kReadOk)
             return len = mt.block_len, true;
@@ -988,6 +1025,11 @@ struct ReconItem {
     uint32_t block_len = 0;
     uint8_t present[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
     uint8_t want[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
+    // a ranged GET (garage_ec_decode_range_stripes): `present` is the plan's presence map, bytes [off, off + len) of
+    // the block go to `out`
+    bool range = false;
+    uint32_t off = 0, len = 0;
+    uint8_t *out = nullptr;
     bool fulfilled = false;
     std::promise<int> done;
 };
@@ -1082,7 +1124,8 @@ struct garage_bm {
         resync_shards_read{0}, resync_bytes_read{0}, resync_bytes_fetched{0};
     std::atomic<uint64_t> put_ns_slot{0}, put_ns_land{0}, put_ns_wait{0}, put_ns_store{0};
     std::atomic<uint64_t> convert_blocks{0}, convert_bytes_read{0}, convert_bytes_written{0}, convert_errors{0},
-        convert_call_us{0}, legacy_gets{0}, legacy_deleted{0};
+        convert_call_us{0}, legacy_gets{0}, legacy_deleted{0}, range_gets{0}, range_degraded{0}, range_bytes_read{0},
+        range_bytes_fetched{0};
     std::atomic<uint64_t> layout_shards_copied{0}, layout_shards_rebuilt{0}, layout_bytes_read{0}, layout_bytes_written{0},
         layout_deleted{0}, layout_sync_errors{0}, layout_bytes_fetched{0};
 
@@ -1245,10 +1288,10 @@ struct garage_bm {
     // A bad header or a tag mismatch quarantines the shard and queues a resync, like the reference.
     // `for_dma`: the GPU reads `dst` next (degraded GET, resync): see copy_for_dma
     // index >= 0: the node's shard of that index (several active layout versions)
-    // half = 0 / 1 (PB): one half of the shard (a ranged read of shard_len/2 bytes into dst), checked against the
-    // half's 4 adler8 segment tags (garage_ec_check_shard_half_host)
+    // span other than the whole shard (a PB half, or the tag span of a ranged GET): a ranged read of its bytes into
+    // dst, checked against the tag segments it covers (garage_ec_check_shard_span_host)
     bool read_shard_into(int node, const Hash &h, uint8_t *dst, size_t cap, ShardMeta &mt, bool for_dma = false, int code = 0,
-                         int index = -1, int half = -1)
+                         int index = -1, ShardSpan span = {})
     {
         Node &nd = *nodes[node];
         ReadResult r;
@@ -1260,18 +1303,21 @@ struct garage_bm {
                 if (!nd.up) return false;
                 sp = nd.store_find(h);
             }
-            r = sp ? nd.copy_out(*sp, dst, cap, mt, for_dma, half) : kReadMissing;  // the copy happens outside the node lock
-            if (sp && for_dma && half < 0) check = sp->bytes.data();  // same bytes, and these are still in the cache
+            r = sp ? nd.copy_out(*sp, dst, cap, mt, for_dma, span) : kReadMissing;  // the copy happens outside the node lock
+            if (sp && for_dma && span.whole()) check = sp->bytes.data();  // same bytes, and these are still in the cache
         } else {
             std::lock_guard<std::mutex> lk(nd.mu);
             if (!nd.up) return false;
-            r = nd.store_read_into(h, dst, cap, mt, half, code, index);
+            r = nd.store_read_into(h, dst, cap, mt, span, code, index);
         }
         if (r == kReadMissing) return false;
         if (r == kReadOk) {
-            if (half >= 0) {
-                bytes_read += mt.shard_len / 2;
-                if (garage_ec_check_shard_half_host(mt.sum_kind, dst, mt.shard_len, half, mt.sum.data()) == GARAGE_EC_OK)
+            if (!span.whole()) {
+                size_t off = 0, n = 0;
+                span.resolve(mt.shard_len, off, n);
+                bytes_read += n;
+                if (garage_ec_check_shard_span_host(mt.sum_kind, dst, mt.shard_len, (uint32_t)off, (uint32_t)n,
+                                                    mt.sum.data()) == GARAGE_EC_OK)
                     return true;
             } else {
                 bytes_read += mt.shard_len;
@@ -1319,8 +1365,12 @@ struct garage_bm {
         }
     }
 
-    void run_reconstruct(int w, std::vector<ReconItem *> &b)
+    void run_reconstruct(int w, std::vector<ReconItem *> &all)
     {
+        std::vector<ReconItem *> b, rb;  // whole-shard rebuilds, ranged GETs
+        for (ReconItem *it : all) (it->range ? rb : b).push_back(it);
+        if (!rb.empty()) run_decode_range(w, rb);
+        if (b.empty()) return;
         const size_t n = b.size();
         std::vector<uint8_t *> stripes(n);
         std::vector<uint8_t> present(n * tot), want(n * tot);
@@ -1342,6 +1392,62 @@ struct garage_bm {
             b[i]->fulfilled = true;
             b[i]->done.set_value(r);
         }
+    }
+
+    // the ranged GETs of a dispatcher batch: one garage_ec_decode_range_stripes on their stripe slots
+    void run_decode_range(int w, std::vector<ReconItem *> &b)
+    {
+        const size_t n = b.size();
+        std::vector<const uint8_t *> stripes(n);
+        std::vector<uint8_t *> outs(n);
+        std::vector<uint8_t> present(n * tot);
+        std::vector<uint32_t> blen(n), offs(n), lens(n);
+        std::vector<int32_t> status(n, 0);
+        for (size_t i = 0; i < n; i++) {
+            stripes[i] = b[i]->stripe;
+            outs[i] = b[i]->out;
+            blen[i] = b[i]->block_len;
+            offs[i] = b[i]->off;
+            lens[i] = b[i]->len;
+            memcpy(present.data() + i * tot, b[i]->present, tot);
+        }
+        const auto t0 = Clock::now();
+        int rc = garage_ec_decode_range_stripes(rec_ctx[w], stripes.data(), present.data(), blen.data(), offs.data(),
+                                                lens.data(), slot_stride, outs.data(), status.data(), n);
+        rec_gpu_us += (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count();
+        for (size_t i = 0; i < n; i++) {
+            int r = rc;
+            if (rc == GARAGE_EC_OK || rc == GARAGE_EC_E_UNRECOVERABLE) r = status[i] ? GARAGE_BM_E_MISSING_BLOCK : GARAGE_BM_OK;
+            b[i]->fulfilled = true;
+            b[i]->done.set_value(r);
+        }
+    }
+
+    // The sources of every index of h's stripe of `code`, in the order to try them: with several active layout
+    // versions (code 0) those garage_layout_read_plan lists, and true (read each source's file of that index); else the
+    // index's ring node.
+    bool shard_sources(const Hash &h, int code, int (*src)[GARAGE_BM_MAX_LAYOUT_VERSIONS], int *nsrc)
+    {
+        constexpr int kMaxSrc = GARAGE_BM_MAX_LAYOUT_VERSIONS;
+        const int k = codes[code].k, tot = codes[code].tot;
+        for (int i = 0; i < tot; i++) nsrc[i] = 0;
+        auto ls = layouts();
+        if (code == 0 && ls->v.size() > 1) {
+            garage_shard_source plan[(GARAGE_EC_MAX_K + GARAGE_EC_MAX_M) * kMaxSrc];
+            const auto act = ls->raw();
+            const int np = garage_layout_read_plan(act.data(), (int)act.size(), nullptr, 0, h.data(), k, -1, nullptr, plan,
+                                                   (int)(sizeof(plan) / sizeof(plan[0])));
+            for (int s = 0; s < np; s++)
+                if (plan[s].index < tot && nsrc[plan[s].index] < kMaxSrc) src[plan[s].index][nsrc[plan[s].index]++] = plan[s].node;
+            return true;
+        }
+        int who[64];
+        nodes_of(h, code, who);
+        for (int i = 0; i < tot; i++) {
+            src[i][0] = who[i];
+            nsrc[i] = 1;
+        }
+        return false;
     }
 
     // Read the valid shards of `h` from every up node except `skip_node` into the stripe slot
@@ -1379,26 +1485,7 @@ struct garage_bm {
         constexpr int kMaxSrc = GARAGE_BM_MAX_LAYOUT_VERSIONS;
         int src[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M][kMaxSrc], nsrc[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0},
             cur[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
-        bool by_index = false;  // read each source's file of that index
-        {
-            auto ls = layouts();
-            if (code == 0 && ls->v.size() > 1) {
-                by_index = true;
-                garage_shard_source plan[(GARAGE_EC_MAX_K + GARAGE_EC_MAX_M) * kMaxSrc];
-                const auto act = ls->raw();
-                const int np = garage_layout_read_plan(act.data(), (int)act.size(), nullptr, 0, h.data(), k, -1, nullptr, plan,
-                                                       (int)(sizeof(plan) / sizeof(plan[0])));
-                for (int s = 0; s < np; s++)
-                    if (plan[s].index < tot && nsrc[plan[s].index] < kMaxSrc) src[plan[s].index][nsrc[plan[s].index]++] = plan[s].node;
-            } else {
-                int who[64];
-                nodes_of(h, code, who);
-                for (int i = 0; i < tot; i++) {
-                    src[i][0] = who[i];
-                    nsrc[i] = 1;
-                }
-            }
-        }
+        const bool by_index = shard_sources(h, code, src, nsrc);  // read each source's file of that index
         // a source of index i is left to try
         auto left = [&](int i) {
             while (cur[i] < nsrc[i] && src[i][cur[i]] == skip_node && (!want_in || want_in[i])) cur[i]++;
@@ -1430,7 +1517,7 @@ struct garage_bm {
             } else {
                 const size_t hl = (have_expect ? shard_len_of(expect, code) : slot_stride) / 2;  // placement of the b-half
                 got = read_shard_into(node, h, dst + (size_t)half * hl, slot_stride - (size_t)half * hl, mt, for_gpu, code,
-                                      fidx, half);
+                                      fidx, ShardSpan::of_half(half));
                 if (got && !have_expect && half == 1 && mt.shard_len / 2 != hl)  // first read of the block: move it
                     memmove(dst + mt.shard_len / 2, dst + hl, mt.shard_len / 2);
             }
@@ -1662,6 +1749,133 @@ struct garage_bm {
             return GARAGE_BM_OK;
         }
         return rc;
+    }
+
+    // Bytes [off, off + len) of block h into out (S3 GetObject with a Range header, body_from_blocks_range; the
+    // source ranges of UploadPartCopy).  The block length comes from the first configured-code shard header that
+    // reads.  garage_ec_range_plan names the runs to fetch; each holder reads only the tag span covering its runs
+    // (garage_ec_tag_span) and checks it against the shard's tag; a span that fails quarantines its shard, queues its
+    // resync, and the plan is recomputed without it.  A range whose touched data shards are all present never
+    // touches the GPU; the others go through the reconstruct dispatchers (garage_ec_decode_range_stripes).
+    // Integrity: a ranged read is proven by the shard tags only.  The block's blake2sum needs the whole block, so a
+    // self-consistent stale shard is found by the deep scrub (DESIGN.md section 5.4), not here.  A range equal to the
+    // whole block is rpc_get_block, with its content-hash check and stale-shard hunt; so is a block held only under a
+    // previous code or as replicas, which is then sliced.
+    int rpc_get_block_range(const Hash &h, uint32_t off, uint32_t len, uint8_t *out, size_t cap, size_t *out_len)
+    {
+        range_gets++;
+        const Code &cd = codes[0];
+        const int tot = cd.tot;
+        constexpr int kMaxSrc = GARAGE_BM_MAX_LAYOUT_VERSIONS;
+        int src[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M][kMaxSrc], nsrc[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0},
+            cur[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
+        const bool by_index = shard_sources(h, 0, src, nsrc);
+        auto left = [&](int i) { return cur[i] < nsrc[i]; };
+        // the block length and tag kind: the first header that reads (a bad one quarantines its shard)
+        ShardMeta m0;
+        bool have_len = false;
+        for (int i = 0; i < tot && !have_len; i++) {
+            while (left(i) && !have_len) {
+                Node &nd = *nodes[src[i][cur[i]]];
+                ReadResult r = kReadMissing;
+                ShardMeta mt;
+                Node::ShardPtr sp;
+                {
+                    std::lock_guard<std::mutex> lk(nd.mu);
+                    if (nd.up) {
+                        if (nd.dir.empty()) sp = nd.store_find(h);
+                        else r = nd.store_read_into(h, nullptr, 0, mt, ShardSpan::bytes(0, 0), 0, by_index ? i : -1);
+                    }
+                }
+                if (sp) r = nd.copy_out(*sp, nullptr, 0, mt, false, ShardSpan::bytes(0, 0));
+                if (r == kReadOk && mt.index == i) {
+                    m0 = mt;
+                    have_len = true;
+                    break;
+                }
+                if (r != kReadMissing) quarantine(src[i][cur[i]], h, 0, by_index ? i : -1);
+                cur[i]++;
+            }
+        }
+        auto sliced = [&]() -> int {  // the whole block through rpc_get_block, then the range of it
+            std::vector<uint8_t> whole(cfg.block_size);
+            size_t n = 0;
+            const int rc = rpc_get_block(h, whole.data(), whole.size(), &n);
+            if (rc != GARAGE_BM_OK) return rc;
+            if ((uint64_t)off + len > n || len > cap) return GARAGE_EC_E_INVALID;
+            memcpy(out, whole.data() + off, len);
+            *out_len = len;
+            return GARAGE_BM_OK;
+        };
+        if (!have_len) return has_legacy() ? sliced() : GARAGE_BM_E_MISSING_BLOCK;
+        const uint32_t block_len = m0.block_len, L = (uint32_t)shard_len_of(block_len);
+        if ((uint64_t)off + len > block_len || len > cap) return GARAGE_EC_E_INVALID;
+        if (off == 0 && len == block_len) return sliced();
+        SlotLease slot(stripe_slots);
+        uint8_t fetched[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0}, guess[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
+        uint32_t f_lo[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M], f_hi[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
+        std::vector<garage_ec_range> runs((size_t)tot * ((cd.clay ? cd.quantum / 16 : 1) + 2));
+        size_t nr = 0;
+        int gpu = 0;
+        for (;;) {
+            for (int i = 0; i < tot; i++) guess[i] = fetched[i] || left(i);
+            const int rc = garage_ec_range_plan(cd.ctx, guess, block_len, off, len, runs.data(), runs.size(), &nr, &gpu);
+            if (rc == GARAGE_EC_E_UNRECOVERABLE) return GARAGE_BM_E_MISSING_BLOCK;
+            if (rc != GARAGE_EC_OK) return rc;
+            uint32_t lo[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M], hi[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
+            for (int i = 0; i < tot; i++) lo[i] = UINT32_MAX;
+            for (size_t x = 0; x < nr; x++) {
+                lo[runs[x].shard] = std::min(lo[runs[x].shard], runs[x].offset);
+                hi[runs[x].shard] = std::max(hi[runs[x].shard], runs[x].offset + runs[x].len);
+            }
+            bool replan = false;
+            for (int i = 0; i < tot && !replan; i++) {
+                if (lo[i] == UINT32_MAX || (fetched[i] && f_lo[i] <= lo[i] && hi[i] <= f_hi[i])) continue;
+                uint32_t so = 0, sl = 0;
+                if (garage_ec_tag_span(m0.sum_kind, L, lo[i], hi[i] - lo[i], &so, &sl) != GARAGE_EC_OK) return GARAGE_EC_E_INVALID;
+                fetched[i] = 0;
+                while (left(i)) {  // a shard's runs come from one source
+                    const int node = src[i][cur[i]], fidx = by_index ? i : -1;
+                    ShardMeta mt;
+                    bool got = read_shard_into(node, h, slot.p + (size_t)i * slot_stride + so, slot_stride - so, mt, true, 0,
+                                               fidx, ShardSpan::bytes(so, sl));
+                    if (got) range_bytes_read += sl;
+                    if (got && (mt.index != i || mt.block_len != block_len || mt.shard_len != L)) {
+                        quarantine(node, h, 0, fidx);  // a stale or misplaced shard with a self-consistent tag
+                        got = false;
+                    }
+                    if (got) {
+                        fetched[i] = 1;
+                        f_lo[i] = so;
+                        f_hi[i] = so + sl;
+                        break;
+                    }
+                    cur[i]++;
+                }
+                replan = !fetched[i];  // the shard is out: the plan changes
+            }
+            if (!replan) break;
+        }
+        for (size_t x = 0; x < nr; x++) range_bytes_fetched += runs[x].len;
+        *out_len = len;
+        if (!gpu) {  // every touched data shard is present: their range bytes, no GPU
+            for (uint64_t j = off / L, end = (uint64_t)off + len; j * L < end; j++) {
+                const uint64_t base = j * L, c0 = std::max<uint64_t>(off, base) - base, c1 = std::min<uint64_t>(end, base + L) - base;
+                memcpy(out + (base + c0 - off), slot.p + j * slot_stride + c0, c1 - c0);
+            }
+            return GARAGE_BM_OK;
+        }
+        range_degraded++;
+        ReconItem it;
+        it.stripe = slot.p;
+        it.stride = slot_stride;
+        it.block_len = block_len;
+        memcpy(it.present, guess, tot);
+        it.range = true;
+        it.off = off;
+        it.len = len;
+        it.out = out;
+        return rec_batcher->submit(it);
     }
 
     // the block from the first of its first legacy_rf ring nodes whose replica matches its content hash (a replica
@@ -3175,6 +3389,13 @@ int garage_bm_rpc_get_block(garage_bm *bm, const uint8_t hash[32], uint8_t *out,
     BM_GUARD(bm->rpc_get_block(to_hash(hash), out, cap, out_len));
 }
 
+int garage_bm_rpc_get_block_range(garage_bm *bm, const uint8_t hash[32], uint32_t offset, uint32_t len, uint8_t *out,
+                                  size_t cap, size_t *out_len)
+{
+    if (!bm || !hash || !out_len || (!out && len)) return GARAGE_EC_E_INVALID;
+    BM_GUARD(bm->rpc_get_block_range(to_hash(hash), offset, len, out, cap, out_len));
+}
+
 int garage_bm_resync_block(garage_bm *bm, int node, const uint8_t hash[32])
 {
     if (!bm || !hash || node < 0 || node >= (int)bm->nodes.size()) return GARAGE_EC_E_INVALID;
@@ -3425,6 +3646,15 @@ void garage_bm_get_metrics(garage_bm *bm, garage_bm_metrics *o)
     o->deep_scrub_parity_bad = bm->deep_parity_bad;
     o->deep_scrub_content_errors = bm->deep_content_errors;
     o->deep_check_call_us = bm->deep_check_us;
+}
+
+void garage_bm_get_range_metrics(garage_bm *bm, garage_bm_range_metrics *o)
+{
+    if (!bm || !o) return;
+    o->range_gets = bm->range_gets;
+    o->range_degraded = bm->range_degraded;
+    o->range_bytes_read = bm->range_bytes_read;
+    o->range_bytes_fetched = bm->range_bytes_fetched;
 }
 
 }  // extern "C"

@@ -1620,6 +1620,285 @@ int garage_ec_reconstruct_stripes(garage_ec_ctx *ctx, uint8_t *const *stripes, c
     return reconstruct_host(ctx, nullptr, stripes, present, want, status, shard_len, stride, n_stripes);
 }
 
+// --------------------------------------------------------------------------- RANGED READS (DESIGN.md 2.5)
+}  // extern "C"
+namespace {
+
+// One request's window (rs_kernels.cuh) and the survivor plan of its absent touched data shards.  GARAGE_EC_E_INVALID
+// for a range past the block or a shard length past `stride`.
+struct RangeReq {
+    RangeWindow r{0, 0, 0, 0, 0};
+    uint64_t halves = 0;
+    bool ok = true;  // the absent touched data shards can be rebuilt
+};
+int range_request(const garage_ec_ctx *ctx, const uint8_t *present, uint32_t block_len, uint32_t off,
+                         uint32_t len, uint64_t stride, RangeReq *q)
+{
+    const uint64_t L = code_shard_len(ctx, block_len);
+    if ((uint64_t)off + len > block_len || L > stride) return GARAGE_EC_E_INVALID;
+    q->r = range_window((uint32_t)L, range_unit((uint32_t)L, ctx->pb, ctx->clay ? ctx->cg.alpha : 1), off, len, present);
+    if (!q->r.w) return GARAGE_EC_OK;
+    uint8_t want[kMaxK + kMaxM] = {0};
+    for (int j = 0; j < ctx->k; j++) want[j] = (uint8_t)((q->r.want >> j) & 1);
+    q->ok = stripe_read_plan(ctx, present, want, &q->halves);
+    return GARAGE_EC_OK;
+}
+// The range's bytes in each touched data shard j, as f(j, offset c in the shard, offset in the range, bytes)
+template <class F>
+void for_each_range_piece(const RangeWindow &r, uint64_t off, uint64_t len, F &&f)
+{
+    for (uint64_t j = r.L ? off / r.L : 0, end = off + len; len && j * r.L < end; j++) {
+        const uint64_t base = j * r.L, c0 = std::max(off, base) - base, c1 = std::min(end, base + r.L) - base;
+        f((size_t)j, (size_t)c0, (size_t)(base + c0 - off), (size_t)(c1 - c0));
+    }
+}
+// The window runs of shard i that the sub-stripe decode reads -- the pieces of stripe_read_plan cut to the window --
+// as f(offset in the shard, offset in the sub-stripe's shard, bytes)
+template <class F>
+void for_each_window_run(const garage_ec_ctx *ctx, const RangeReq &q, size_t i, F &&f)
+{
+    const RangeWindow &r = q.r;
+    for_each_read_piece(ctx, q.halves, i, r.L, r.L, [&](size_t off, size_t bytes) {
+        for (size_t z = off / r.unit; z * r.unit < off + bytes; z++) f(z * r.unit + r.w0, z * r.w, (size_t)r.w);
+    });
+}
+// Rebuilt bytes [c0, c0 + bytes) of an absent data shard, cut at run edges, as f(offset in the sub-stripe's shard,
+// offset from c0, bytes)
+template <class F>
+void for_each_rebuilt_piece(const RangeWindow &r, size_t c0, size_t bytes, F &&f)
+{
+    for (size_t c = c0, e = c0 + bytes; c < e;) {
+        const size_t z = c / r.unit, ce = std::min(e, (z + 1) * r.unit);
+        f(z * r.w + (c - z * r.unit) - r.w0, c - c0, ce - c);
+        c = ce;
+    }
+}
+
+}  // namespace
+extern "C" {
+
+int garage_ec_range_plan(const garage_ec_ctx *ctx, const uint8_t *present, uint32_t block_len, uint32_t offset,
+                         uint32_t len, garage_ec_range *ranges, size_t cap, size_t *n_ranges, int *needs_gpu)
+{
+    if (!ctx || !present || !n_ranges || (cap && !ranges)) return GARAGE_EC_E_INVALID;
+    *n_ranges = 0;
+    if (needs_gpu) *needs_gpu = 0;
+    RangeReq q;
+    int rc = range_request(ctx, present, block_len, offset, len, UINT64_MAX, &q);
+    if (rc) return rc;
+    if (needs_gpu) *needs_gpu = q.r.w ? 1 : 0;
+    if (!q.ok) return GARAGE_EC_E_UNRECOVERABLE;
+    std::vector<garage_ec_range> runs;
+    for_each_range_piece(q.r, offset, len, [&](size_t j, size_t c, size_t, size_t bytes) {
+        if (present[j]) runs.push_back(garage_ec_range{(uint32_t)j, (uint32_t)c, (uint32_t)bytes});
+    });
+    for (int i = 0; q.r.w && i < ctx->k + ctx->m; i++)
+        for_each_window_run(ctx, q, (size_t)i, [&](size_t off, size_t, size_t bytes) {
+            runs.push_back(garage_ec_range{(uint32_t)i, (uint32_t)off, (uint32_t)bytes});
+        });
+    std::sort(runs.begin(), runs.end(), [](const garage_ec_range &a, const garage_ec_range &b) {
+        return a.shard != b.shard ? a.shard < b.shard : a.offset < b.offset;
+    });
+    std::vector<garage_ec_range> merged;
+    for (const garage_ec_range &r : runs) {
+        garage_ec_range *b = merged.empty() ? nullptr : &merged.back();
+        if (b && b->shard == r.shard && r.offset <= b->offset + b->len)  // overlapping or adjacent: merged
+            b->len = std::max(b->offset + b->len, r.offset + r.len) - b->offset;
+        else
+            merged.push_back(r);
+    }
+    for (size_t x = 0; x < merged.size() && x < cap; x++) ranges[x] = merged[x];
+    *n_ranges = merged.size();
+    return merged.size() > cap ? GARAGE_EC_E_INVALID : GARAGE_EC_OK;
+}
+
+// HOST ranged decode.  stripes / outs != NULL: the gather form (garage_ec_decode_range_stripes).  Only the window runs
+// of the plan go up, packed into sub-stripes; only the rebuilt range bytes come down; present range bytes are
+// copied on the host.
+static int decode_range_host(garage_ec_ctx *ctx, const uint8_t *shards, const uint8_t *const *stripes,
+                             const uint8_t *present, const uint32_t *block_len, const uint32_t *offset,
+                             const uint32_t *len, size_t stride, uint8_t *out, size_t out_stride, uint8_t *const *outs,
+                             int32_t *status, size_t n)
+{
+    const size_t tot = ctx->k + ctx->m;
+    auto shard_at = [&](size_t s, size_t i) -> const uint8_t * {
+        return stripes ? stripes[s] + i * stride : shards + (s * tot + i) * stride;
+    };
+    auto out_at = [&](size_t s) -> uint8_t * { return outs ? outs[s] : out + s * out_stride; };
+    std::vector<RangeReq> rq(n);
+    std::vector<size_t> need;
+    size_t sub_max = 16;
+    bool any_bad = false, pinned = true;
+    for (size_t s = 0; s < n; s++) {
+        int rc = range_request(ctx, present + s * tot, block_len[s], offset[s], len[s], stride, &rq[s]);
+        if (rc) return rc;
+        if (len[s] && !out_at(s)) return GARAGE_EC_E_INVALID;
+    }
+    for (size_t s = 0; s < n; s++) {
+        if (status) status[s] = rq[s].ok ? 0 : GARAGE_EC_E_UNRECOVERABLE;
+        any_bad |= !rq[s].ok;
+        if (!rq[s].ok || !rq[s].r.w) continue;
+        need.push_back(s);
+        sub_max = std::max<size_t>(sub_max, (size_t)(rq[s].r.L / rq[s].r.unit) * rq[s].r.w);
+        pinned = pinned && device_addressable_host(shard_at(s, 0)) && device_addressable_host(out_at(s));
+    }
+    const size_t sub_stride = align_up(sub_max, 16);
+    std::vector<int32_t> dec_status(need.size(), 0);  // the decode's own verdicts (outlives the pipeline's copies)
+    HostPipeline p(ctx, need.size(), tot * sub_stride);
+    // pageable pieces go one by one (see reconstruct_host)
+    p.up.use_batch = p.down.use_batch = pinned;
+    const size_t cs = p.cs;
+    SmallLayout sl;
+    const size_t o_present = sl.take(cs * tot), o_want = sl.take(cs * tot), o_status = sl.take(cs * 4),
+                 o_len = sl.take(cs * 4), o_plan = sl.take(plan_scratch_bytes(ctx, cs));
+    // pageable staging per lane: sub-stripe length | present | want
+    int rc = p.reserve(cs * tot * sub_stride, sl.bytes, cs * 4 + 2 * cs * tot);
+    if (rc) return rc;
+    rc = p.run([&](const HostChunk &ch) -> int {
+        HostLane &L = *ch.L;
+        const size_t q0 = ch.s0, cnt = ch.cnt;
+        uint32_t *hl = reinterpret_cast<uint32_t *>(ch.host);
+        uint8_t *hp = ch.host + cs * 4, *hw = hp + cs * tot;
+        for (size_t q = 0; q < cnt; q++) {
+            const size_t s = need[q0 + q];
+            const RangeReq &r = rq[s];
+            memcpy(hp + q * tot, present + s * tot, tot);
+            for (size_t i = 0; i < tot; i++) hw[q * tot + i] = (uint8_t)((r.r.want >> i) & 1);
+            hl[q] = (r.r.L / r.r.unit) * r.r.w;
+            uint8_t *d_st = L.d_buf + q * tot * sub_stride;
+            for (size_t i = 0; i < tot; i++)
+                for_each_window_run(ctx, r, i, [&](size_t so, size_t sub, size_t bytes) {
+                    p.up.add(d_st + i * sub_stride + sub, shard_at(s, i) + so, bytes);
+                });
+        }
+        int e = p.up.flush(ctx, cudaMemcpyHostToDevice, L.stream);
+        if (e) return e;
+        CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_present, hp, cnt * tot, cudaMemcpyHostToDevice, L.stream));
+        CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_want, hw, cnt * tot, cudaMemcpyHostToDevice, L.stream));
+        CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_len, hl, cnt * 4, cudaMemcpyHostToDevice, L.stream));
+        e = run_reconstruct(ctx, L.d_buf, L.d_small + o_present, L.d_small + o_want,
+                            reinterpret_cast<int32_t *>(L.d_small + o_status),
+                            reinterpret_cast<const uint32_t *>(L.d_small + o_len), sub_stride, cnt, L.d_small + o_plan,
+                            L.stream);
+        if (e) return e;
+        CU_TRY(ctx, cudaMemcpyAsync(dec_status.data() + q0, L.d_small + o_status, cnt * 4, cudaMemcpyDeviceToHost,
+                                    L.stream));
+        // D2H: the rebuilt range bytes only, straight into the caller's output
+        for (size_t q = 0; q < cnt; q++) {
+            const size_t s = need[q0 + q];
+            const RangeReq &r = rq[s];
+            for_each_range_piece(r.r, offset[s], len[s], [&](size_t j, size_t c, size_t pos, size_t bytes) {
+                if (present[s * tot + j]) return;
+                const uint8_t *d_sh = L.d_buf + (q * tot + j) * sub_stride;
+                for_each_rebuilt_piece(r.r, c, bytes, [&](size_t sub, size_t rel, size_t b) {
+                    p.down.add(out_at(s) + pos + rel, d_sh + sub, b);
+                });
+            });
+        }
+        return p.down.flush(ctx, cudaMemcpyDeviceToHost, L.stream);
+    });
+    if (rc) return rc;
+    // the present range bytes, while the GPU works
+    for (size_t s = 0; s < n; s++) {
+        if (!rq[s].ok) continue;
+        for_each_range_piece(rq[s].r, offset[s], len[s], [&](size_t j, size_t c, size_t pos, size_t bytes) {
+            if (present[s * tot + j]) memcpy(out_at(s) + pos, shard_at(s, j) + c, bytes);
+        });
+    }
+    rc = p.drain();
+    if (rc) return rc;
+    for (size_t q = 0; q < need.size(); q++)  // the host plan said yes; the decode's verdict has the last word
+        if (dec_status[q]) {
+            if (status) status[need[q]] = dec_status[q];
+            any_bad = true;
+        }
+    return any_bad ? GARAGE_EC_E_UNRECOVERABLE : GARAGE_EC_OK;
+}
+
+// DEVICE ranged decode: geometry, pack the window runs into sub-stripes, the code's own decode on them, join
+static int decode_range_device(garage_ec_ctx *ctx, const uint8_t *shards, const uint8_t *present,
+                               const uint32_t *block_len, const uint32_t *offset, const uint32_t *len, size_t stride,
+                               uint8_t *out, size_t out_stride, int32_t *status, size_t n, cudaStream_t st)
+{
+    const size_t tot = ctx->k + ctx->m, pitch = tot * stride;
+    SmallLayout sl;
+    const size_t o_sub = sl.take(n * pitch), o_geo = sl.take(n * 16), o_len = sl.take(n * 4), o_want = sl.take(n * tot),
+                 o_st = sl.take(n * 4), o_plan = sl.take(plan_scratch_bytes(ctx, n));
+    return with_stream_scratch(ctx, sl.bytes, st, [&](uint8_t *sc) -> int {
+        RangeParams q;
+        memset(&q, 0, sizeof(q));
+        q.shards = shards;
+        q.sub = sc + o_sub;
+        q.present = present;
+        q.block_len = block_len;
+        q.offset = offset;
+        q.len = len;
+        q.out = out;
+        q.geo = reinterpret_cast<uint4 *>(sc + o_geo);
+        q.sub_len = reinterpret_cast<uint32_t *>(sc + o_len);
+        q.want = sc + o_want;
+        q.plan_status = reinterpret_cast<const int32_t *>(sc + o_st);
+        q.status = status;
+        q.pitch = pitch;
+        q.out_stride = out_stride;
+        q.stride = (uint32_t)stride;
+        q.k = (uint32_t)ctx->k;
+        q.m = (uint32_t)ctx->m;
+        q.n = (uint32_t)n;
+        q.quantum = ctx->quantum;
+        q.alpha = ctx->clay ? (uint32_t)ctx->cg.alpha : 1u;
+        q.pb = ctx->pb ? 1u : 0u;
+        const unsigned per_req = (unsigned)std::min<size_t>(n, (size_t)ctx->sm_count * 8);
+        range_geo_kernel<<<(unsigned)std::min<size_t>((n + 255) / 256, (size_t)ctx->sm_count * 4), 256, 0, st>>>(q);
+        range_pack_kernel<<<per_req, 256, 0, st>>>(q);
+        ctx->launches.fetch_add(2, std::memory_order_relaxed);
+        CU_TRY(ctx, cudaGetLastError());
+        int r = run_reconstruct(ctx, q.sub, present, q.want, reinterpret_cast<int32_t *>(sc + o_st), q.sub_len, stride, n,
+                                sc + o_plan, st);
+        if (r) return r;
+        range_join_kernel<<<per_req, 256, 0, st>>>(q);
+        ctx->launches.fetch_add(1, std::memory_order_relaxed);
+        CU_TRY(ctx, cudaGetLastError());
+        return GARAGE_EC_OK;
+    });
+}
+
+int garage_ec_decode_range(garage_ec_ctx *ctx, const uint8_t *shards, const uint8_t *present, const uint32_t *block_len,
+                           const uint32_t *offset, const uint32_t *len, size_t stride, uint8_t *out, size_t out_stride,
+                           int32_t *status, size_t n, int mem_kind, void *cuda_stream)
+{
+    if (!ctx || (mem_kind != GARAGE_EC_MEM_HOST && mem_kind != GARAGE_EC_MEM_DEVICE)) return GARAGE_EC_E_INVALID;
+    int rc = check_geometry(ctx, stride, n, ctx->k + ctx->m);
+    if (rc) return rc;
+    if (n == 0) return GARAGE_EC_OK;
+    if (!shards || !present || !block_len || !offset || !len || !out) return GARAGE_EC_E_INVALID;
+    if (!aligned16(shards)) return GARAGE_EC_E_ALIGN;
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    if (mem_kind == GARAGE_EC_MEM_HOST)
+        return decode_range_host(ctx, shards, nullptr, present, block_len, offset, len, stride, out, out_stride, nullptr,
+                                 status, n);
+    if (!aligned16(out) || (out_stride & 15)) return GARAGE_EC_E_ALIGN;
+    return decode_range_device(ctx, shards, present, block_len, offset, len, stride, out, out_stride, status, n,
+                               (cudaStream_t)cuda_stream);
+}
+
+int garage_ec_decode_range_stripes(garage_ec_ctx *ctx, const uint8_t *const *stripes, const uint8_t *present,
+                                   const uint32_t *block_len, const uint32_t *offset, const uint32_t *len, size_t stride,
+                                   uint8_t *const *outs, int32_t *status, size_t n)
+{
+    if (!ctx) return GARAGE_EC_E_INVALID;
+    int rc = check_geometry(ctx, stride, n, ctx->k + ctx->m);
+    if (rc) return rc;
+    if (n == 0) return GARAGE_EC_OK;
+    if (!stripes || !present || !block_len || !offset || !len || !outs) return GARAGE_EC_E_INVALID;
+    for (size_t s = 0; s < n; s++) {
+        if (!stripes[s]) return GARAGE_EC_E_INVALID;
+        if (!aligned16(stripes[s])) return GARAGE_EC_E_ALIGN;
+    }
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    return decode_range_host(ctx, nullptr, stripes, present, block_len, offset, len, stride, nullptr, 0, outs, status, n);
+}
+
 // --------------------------------------------------------------------------- SHARD SUMS
 static int run_sums(garage_ec_ctx *ctx, const uint8_t *shards, const uint8_t *expect, const uint32_t *shard_len,
                     size_t stride, size_t n_shards, int per_stripe, uint8_t *sums, uint8_t *bad, cudaStream_t st,
@@ -1883,21 +2162,68 @@ int garage_ec_shard_sum_host(int kind, const uint8_t *data, size_t len, uint8_t 
     return GARAGE_EC_OK;
 }
 
+int garage_ec_tag_span(int kind, uint32_t shard_len, uint32_t off, uint32_t len, uint32_t *span_off, uint32_t *span_len)
+{
+    if (!span_off || !span_len || (uint64_t)off + len > shard_len) return GARAGE_EC_E_INVALID;
+    if (kind == GARAGE_EC_SUM_BLAKE2) {  // one hash over the whole shard
+        *span_off = 0;
+        *span_len = shard_len;
+        return GARAGE_EC_OK;
+    }
+    if (kind != GARAGE_EC_SUM_ADLER8) return GARAGE_EC_E_INVALID;
+    if (!len) {
+        *span_off = off;
+        *span_len = 0;
+        return GARAGE_EC_OK;
+    }
+    const uint64_t seg = adler8_seg_bytes(shard_len), a = off / seg * seg,
+                   b = std::min<uint64_t>(((uint64_t)off + len + seg - 1) / seg * seg, shard_len);
+    *span_off = (uint32_t)a;
+    *span_len = (uint32_t)(b - a);
+    return GARAGE_EC_OK;
+}
+
+int garage_ec_check_shard_span_host(int kind, const uint8_t *bytes, uint32_t shard_len, uint32_t span_off,
+                                    uint32_t span_len, const uint8_t tag32[32])
+{
+    if (!tag32 || (!bytes && span_len) || (uint64_t)span_off + span_len > shard_len) return GARAGE_EC_E_INVALID;
+    if (kind == GARAGE_EC_SUM_BLAKE2) {
+        if (span_off || span_len != shard_len) return GARAGE_EC_E_INVALID;
+        uint8_t h[32];
+        blake2sum_host(bytes, shard_len, h);
+        return memcmp(h, tag32, 32) ? 1 : GARAGE_EC_OK;
+    }
+    if (kind != GARAGE_EC_SUM_ADLER8) return GARAGE_EC_E_INVALID;
+    if (!span_len) return GARAGE_EC_OK;
+    // whole segments only: the span starts on a segment edge and ends on one or at the shard's end
+    const uint64_t seg = adler8_seg_bytes(shard_len), end = (uint64_t)span_off + span_len;
+    if (span_off % seg || (end % seg && end != shard_len)) return GARAGE_EC_E_INVALID;
+    for (uint64_t a = span_off; a < end; a += seg) {
+        const uint32_t v = adler32_one(bytes + (a - span_off), std::min<uint64_t>(seg, end - a));
+        uint32_t want;
+        memcpy(&want, tag32 + 4 * (a / seg), 4);  // little endian
+        if (v != want) return 1;
+    }
+    return GARAGE_EC_OK;
+}
+
 int garage_ec_check_shard_half_host(int kind, const uint8_t *half_bytes, uint32_t shard_len, int which,
                                     const uint8_t tag32[32])
 {
     if (kind != GARAGE_EC_SUM_ADLER8 || (shard_len % 128) || (which != 0 && which != 1) || !tag32 ||
         (!half_bytes && shard_len))
         return GARAGE_EC_E_INVALID;
-    // shard_len % 128 == 0: the 8 segments are shard_len/8 bytes each, and half `which` is segments 4*which..+3
-    const size_t seg = shard_len / 8;
-    for (int t = 0; t < 4; t++) {
-        const uint32_t v = seg ? adler32_one(half_bytes + t * seg, seg) : 1u;
-        uint32_t want;
-        memcpy(&want, tag32 + 4 * (4 * which + t), 4);  // little endian
-        if (v != want) return 1;
+    if (!shard_len) {  // four empty segments: Adler-32 = 1 each
+        for (int t = 0; t < 4; t++) {
+            uint32_t want;
+            memcpy(&want, tag32 + 4 * (4 * which + t), 4);
+            if (want != 1u) return 1;
+        }
+        return GARAGE_EC_OK;
     }
-    return GARAGE_EC_OK;
+    // shard_len % 128 == 0: the 8 segments are shard_len/8 bytes each, and half `which` is segments 4*which..+3
+    return garage_ec_check_shard_span_host(kind, half_bytes, shard_len, (uint32_t)which * (shard_len / 2), shard_len / 2,
+                                           tag32);
 }
 
 // --------------------------------------------------------------------------- SCRUB + REPAIR

@@ -2145,4 +2145,165 @@ __global__ void __launch_bounds__(256) adler8_shards_kernel(const __grid_constan
     }
 }
 
+// ------------------------------------------------------------------ ranged reads (DESIGN.md 2.5)
+// Block byte o is byte c = o % L of data shard o / L.  Every code here is column-local: byte c of a rebuilt shard
+// depends on the survivors only at the bytes of the same window coordinate, c (RS, LRC), c mod L/2 (PB: a-half column
+// c pairs with b-half column c) or c mod L/alpha (Clay: the in-layer column across all alpha layers).  With unit = L,
+// L/2 or L/alpha, a shard is L/unit runs of `unit` bytes; the window [w0, w0 + w) is the smallest 16-byte aligned
+// interval (capped at unit) covering the window coordinates of the range's bytes in absent data shards.  The
+// sub-stripe holds the window of every run of every shard, run z at z*w: a stripe of shard length (L/unit)*w that the
+// code's own decode rebuilds into exactly the window of the full decode.
+struct RangeWindow {
+    uint32_t L, unit, w0, w;  // w = 0: no touched data shard is absent
+    uint64_t want;            // the absent touched data shards
+};
+__host__ __device__ inline uint32_t range_unit(uint32_t L, bool pb, uint32_t alpha)
+{
+    return pb ? L / 2 : L / alpha;  // alpha = 1 for RS, LRC and PB
+}
+// present: the stripe's k+m map; off + len <= block_len is the caller's check
+__host__ __device__ inline RangeWindow range_window(uint32_t L, uint32_t unit, uint64_t off, uint64_t len,
+                                                    const uint8_t *present)
+{
+    RangeWindow r{L, unit, 0, 0, 0};
+    if (!len || !unit) return r;
+    uint64_t lo = unit, hi = 0;
+    const uint64_t end = off + len;
+    for (uint64_t j = off / L; j * L < end; j++) {
+        if (present[j]) continue;
+        r.want |= 1ull << j;
+        const uint64_t base = j * L, c0 = (off > base ? off : base) - base, c1 = (end < base + L ? end : base + L) - base;
+        if (c1 - c0 >= unit || c0 / unit != (c1 - 1) / unit) {  // wraps around a run: every window coordinate
+            lo = 0;
+            hi = unit;
+        } else {
+            lo = c0 % unit < lo ? c0 % unit : lo;
+            hi = (c1 - 1) % unit + 1 > hi ? (c1 - 1) % unit + 1 : hi;
+        }
+    }
+    if (!r.want) return r;
+    r.w0 = (uint32_t)(lo & ~15ull);
+    const uint64_t w1 = (hi + 15) & ~15ull;
+    r.w = (uint32_t)((w1 < unit ? w1 : unit) - r.w0);
+    return r;
+}
+
+struct RangeParams {
+    const uint8_t *shards;          // the caller's shard layout: stripe s at shards + s*pitch, shard i at + i*stride
+    uint8_t *sub;                   // the sub-stripes, same layout (a window never exceeds its shard)
+    const uint8_t *present;         // n*(k+m)
+    const uint32_t *block_len, *offset, *len;  // per request
+    uint8_t *out;                   // request s at out + s*out_stride
+    uint4 *geo;                     // per request: L, unit (0: invalid request), w0, w
+    uint32_t *sub_len;              // per request: (L/unit)*w, the sub-stripe's shard length
+    uint8_t *want;                  // n*(k+m): the absent touched data shards
+    const int32_t *plan_status;     // the decode's status of the sub-stripes
+    int32_t *status;                // nullable, out
+    unsigned long long pitch, out_stride;
+    uint32_t stride, k, m, n, quantum, alpha, pb;
+};
+
+// one thread per request: the window, the decode's want map and sub-stripe length
+__global__ void __launch_bounds__(256) range_geo_kernel(const __grid_constant__ RangeParams q)
+{
+    const uint32_t tot = q.k + q.m;
+    for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < q.n; s += gridDim.x * blockDim.x) {
+        const uint32_t blen = __ldg(q.block_len + s), off = __ldg(q.offset + s), len = __ldg(q.len + s);
+        const uint64_t L64 = code_shard_len(blen, (int)q.k, q.quantum);
+        const bool bad = L64 > q.stride || (uint64_t)off + len > blen;
+        RangeWindow r{0, 0, 0, 0, 0};
+        if (!bad) {
+            const uint32_t L = (uint32_t)L64;
+            r = range_window(L, range_unit(L, q.pb != 0, q.alpha), off, len, q.present + (size_t)s * tot);
+            r.unit = r.unit ? r.unit : 1u;  // a valid empty block
+        }
+        q.geo[s] = make_uint4(r.L, r.unit, r.w0, r.w);
+        q.sub_len[s] = r.w ? (r.L / r.unit) * r.w : 0u;
+        for (uint32_t i = 0; i < tot; i++) q.want[(size_t)s * tot + i] = (uint8_t)((r.want >> i) & 1);
+    }
+}
+
+// The window runs of every present shard into the sub-stripes, one 16-byte vector per thread (window starts are
+// 16-byte aligned; the last vector of an RS / LRC run may read past the window, inside roundup16(L) <= stride).
+// CTAs walk the requests.
+__global__ void __launch_bounds__(256) range_pack_kernel(const __grid_constant__ RangeParams q)
+{
+    const uint32_t tot = q.k + q.m;
+    for (uint32_t s = blockIdx.x; s < q.n; s += gridDim.x) {
+        const uint4 g = q.geo[s];
+        if (!g.w) continue;
+        const uint32_t nz = g.x / g.y, nv = (g.w + 15) >> 4, per = nz * nv;
+        const uint8_t *src = q.shards + s * q.pitch, *pr = q.present + (size_t)s * tot;
+        uint8_t *dst = q.sub + s * q.pitch;
+        for (uint32_t idx = threadIdx.x; idx < tot * per; idx += blockDim.x) {
+            const uint32_t i = idx / per, r = idx - i * per, z = r / nv, v = r - z * nv;
+            if (!pr[i]) continue;
+            const uint4 x = __ldg(reinterpret_cast<const uint4 *>(src + (size_t)i * q.stride + z * g.y + g.z + 16 * v));
+            *reinterpret_cast<uint4 *>(dst + (size_t)i * q.stride + z * g.w + 16 * v) = x;
+        }
+    }
+}
+
+// Where block byte o of request s lives: in the caller's layout for a present shard, in the rebuilt sub-stripe for an
+// absent one; *rem = the bytes from there to the end of that contiguous piece.
+__device__ __forceinline__ const uint8_t *range_src(const RangeParams &q, uint32_t s, const uint4 &g, uint32_t o,
+                                                    uint32_t *rem)
+{
+    const uint32_t j = o / g.x, c = o - j * g.x;
+    if (q.present[(size_t)s * (q.k + q.m) + j]) {
+        *rem = g.x - c;
+        return q.shards + s * q.pitch + (size_t)j * q.stride + c;
+    }
+    const uint32_t z = c / g.y, cc = c - z * g.y;
+    *rem = g.z + g.w - cc;
+    return q.sub + s * q.pitch + (size_t)j * q.stride + z * g.w + (cc - g.z);
+}
+
+// Every request's bytes into out, 16 per thread, zero past len up to roundup16(len).  A vector inside one piece is one
+// aligned vector load, or five aligned 32-bit loads and funnel shifts (as block_vec16: the words stay inside the
+// piece's 16-byte rounding); a vector whose 16 bytes would run past the end of its piece -- one that crosses a shard,
+// PB half or Clay layer edge, or the range's last vector near such an edge -- is gathered byte by byte.  status: invalid requests GARAGE_EC_E_INVALID, requests without an absent touched data
+// shard 0, the others the decode's verdict; nothing is written for a failed request.
+__global__ void __launch_bounds__(256) range_join_kernel(const __grid_constant__ RangeParams q)
+{
+    for (uint32_t s = blockIdx.x; s < q.n; s += gridDim.x) {
+        const uint4 g = q.geo[s];
+        const int32_t verdict = !g.y ? GARAGE_EC_E_INVALID : (g.w ? q.plan_status[s] : 0);
+        if (threadIdx.x == 0 && q.status) q.status[s] = verdict;
+        if (verdict) continue;
+        const uint32_t off = __ldg(q.offset + s), len = __ldg(q.len + s);
+        uint8_t *dst = q.out + s * q.out_stride;
+        for (uint32_t v = threadIdx.x; v < (len + 15) >> 4; v += blockDim.x) {
+            const uint32_t o = off + 16 * v, nvalid = min(16u, len - 16 * v);
+            uint32_t rem;
+            const uint8_t *p = range_src(q, s, g, o, &rem);
+            uint4 x;
+            if (rem >= 16) {
+                if (!(reinterpret_cast<uintptr_t>(p) & 15)) {
+                    x = __ldg(reinterpret_cast<const uint4 *>(p));
+                } else {
+                    const uint32_t sh = (uint32_t)(reinterpret_cast<uintptr_t>(p) & 3u) * 8;
+                    const uint32_t *wp = reinterpret_cast<const uint32_t *>(reinterpret_cast<uintptr_t>(p) & ~(uintptr_t)3);
+                    const uint32_t w0 = __ldg(wp), w1 = __ldg(wp + 1), w2 = __ldg(wp + 2), w3 = __ldg(wp + 3),
+                                   w4 = sh ? __ldg(wp + 4) : 0;
+                    x = make_uint4(__funnelshift_r(w0, w1, sh), __funnelshift_r(w1, w2, sh), __funnelshift_r(w2, w3, sh),
+                                   __funnelshift_r(w3, w4, sh));
+                }
+                if (nvalid < 16) x = mask_tail(x, nvalid);
+            } else {
+                uint32_t wv[4] = {0, 0, 0, 0};
+#pragma unroll
+                for (int b = 0; b < 16; b++) {
+                    if ((uint32_t)b < nvalid) {
+                        uint32_t rb;
+                        wv[b >> 2] |= (uint32_t)*range_src(q, s, g, o + b, &rb) << (8 * (b & 3));
+                    }
+                }
+                x = make_uint4(wv[0], wv[1], wv[2], wv[3]);
+            }
+            *reinterpret_cast<uint4 *>(dst + 16 * (size_t)v) = x;
+        }
+    }
+}
+
 }  // namespace garage_ec

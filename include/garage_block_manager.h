@@ -168,6 +168,14 @@ typedef struct {
                                                 in Garage.  A Clay repair counts its runs (1/m of each helper);
                                                 everything else equals layout_bytes_read                            */
 } garage_bm_metrics;
+/* Counters of garage_bm_rpc_get_block_range, in a struct of their own so that garage_bm_metrics keeps the layout older
+ * callers were built against. */
+typedef struct garage_bm_range_metrics {
+    uint64_t range_gets;          /* garage_bm_rpc_get_block_range calls                                   */
+    uint64_t range_degraded;      /* ranged GETs whose range needed an absent data shard (went to the GPU)  */
+    uint64_t range_bytes_read;    /* tag-span bytes those GETs read from shard files                      */
+    uint64_t range_bytes_fetched; /* the planned run bytes: what would cross the network in Garage         */
+} garage_bm_range_metrics;
 
 void garage_bm_default_config(garage_bm_config *cfg);
 int garage_bm_create(garage_bm **out, const garage_bm_config *cfg);
@@ -184,6 +192,17 @@ int garage_bm_rpc_put_block(garage_bm *bm, const uint8_t hash[32], const uint8_t
  * GARAGE_BM_E_MISSING_BLOCK if fewer than k valid shards can be gathered.                       */
 int garage_bm_rpc_get_block(garage_bm *bm, const uint8_t hash[32], uint8_t *out, size_t cap,
                             size_t *out_len);
+/* Bytes [offset, offset + len) of a block (body_from_blocks_range, src/api/s3/get.rs:650-743; the source range of
+ * UploadPartCopy, src/api/s3/copy.rs:396-469), reading only the shards and columns garage_ec_range_plan names, each as
+ * the adler8 tag span that covers its runs (BLAKE2 stores: whole shards).  *out_len = len.  A range whose touched data
+ * shards are all present never reaches the GPU; the others are rebuilt by the reconstruct dispatchers.
+ * Integrity: a ranged read is proven by the shard tags only -- the block's blake2sum needs the whole block -- so a
+ * stale shard that is consistent with its own tag is found by the deep scrub (garage_bm_deep_scrub_step), not here.
+ * The whole block (offset 0, len = block length), and blocks held only under a previous code or as replicas, are
+ * served by garage_bm_rpc_get_block (content hash checked) and sliced.  GARAGE_EC_E_INVALID if offset + len exceeds
+ * the block or len > cap; GARAGE_BM_E_MISSING_BLOCK as garage_bm_rpc_get_block.                               */
+int garage_bm_rpc_get_block_range(garage_bm *bm, const uint8_t hash[32], uint32_t offset, uint32_t len, uint8_t *out,
+                                  size_t cap, size_t *out_len);
 
 /* manager.rs:452-500 block_incref / block_decref (called by BlockRefTable::updated,
  * src/model/s3/block_ref_table.rs:69-85): 0 -> 1 and 1 -> 0 transitions queue a resync on every
@@ -288,6 +307,7 @@ int garage_bm_node_shard_index(garage_bm *bm, int node, const uint8_t hash[32]);
 /* the newest active layout version's row: shard i of the block on nodes_out[i]                                  */
 int garage_bm_storage_nodes_of(garage_bm *bm, const uint8_t hash[32], int *nodes_out /* k+m */);
 void garage_bm_get_metrics(garage_bm *bm, garage_bm_metrics *out);
+void garage_bm_get_range_metrics(garage_bm *bm, garage_bm_range_metrics *out);
 
 #ifdef __cplusplus
 }

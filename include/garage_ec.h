@@ -266,6 +266,16 @@ int garage_ec_shard_sum_host(int kind, const uint8_t *data, size_t len, uint8_t 
  * and for shard_len % 128 != 0.                                                                                   */
 int garage_ec_check_shard_half_host(int kind, const uint8_t *half_bytes, uint32_t shard_len, int which,
                                     const uint8_t tag32[32]);
+/* The part of a shard's tag that proves the run [off, off + len) of a shard_len-byte shard: *span_off / *span_len =
+ * the smallest run of whole adler8 segments covering it (GARAGE_EC_SUM_ADLER8; segments of
+ * roundup16(ceil(shard_len/8)) bytes, the last one cut at shard_len; len = 0: an empty span at off), or the whole
+ * shard (GARAGE_EC_SUM_BLAKE2).  GARAGE_EC_E_INVALID for an unknown kind or off + len > shard_len.
+ * garage_ec_check_shard_span_host checks such a span (`bytes` = its span_len bytes) against the shard's 32-byte
+ * tag: 0 if every covered segment (BLAKE2: the shard's hash) matches, 1 if not; GARAGE_EC_E_INVALID for a span that
+ * is not whole segments (BLAKE2: not the whole shard).                                                            */
+int garage_ec_tag_span(int kind, uint32_t shard_len, uint32_t off, uint32_t len, uint32_t *span_off, uint32_t *span_len);
+int garage_ec_check_shard_span_host(int kind, const uint8_t *bytes, uint32_t shard_len, uint32_t span_off,
+                                    uint32_t span_len, const uint8_t tag32[32]);
 
 /* ---- BLOCK-LEVEL convenience (host memory only) -----------------------------------------
  * What rpc_put_block hands over is a contiguous block (bytes::Bytes), not shards.  These do
@@ -290,6 +300,45 @@ int garage_ec_encode_blocks_with_sums(garage_ec_ctx *ctx, const uint8_t *const *
 int garage_ec_decode_blocks(garage_ec_ctx *ctx, const uint8_t *shards, const uint8_t *present,
                             const uint32_t *block_len, size_t n_blocks, size_t stride,
                             uint8_t *const *blocks_out, int32_t *status);
+
+/* ---- RANGED READS -- call sites: body_from_blocks_range (S3 GetObject with a Range header, src/api/s3/get.rs:650-743)
+ * and UploadPartCopy with x-amz-copy-source-range (src/api/s3/copy.rs:396-469, 511-540): bytes [offset, offset + len)
+ * of a block, reading only the shards and columns they need (DESIGN.md section 2.5).  Block byte o is byte o % L of
+ * data shard o / L, L = garage_ec_code_shard_len.  A range whose touched data shards are all present needs their
+ * range bytes only, and no GPU.  Otherwise the absent touched data shards are rebuilt over one window [w0, w0 + w):
+ * the smallest 16-byte aligned interval covering the window coordinates of the range's bytes in them -- c for RS and
+ * LRC, c mod L/2 for PB, c mod L/alpha for Clay (a range that wraps round a half / layer, or spans two absent shards
+ * across their boundary, may widen it to the whole half / layer / shard) -- of every half (PB) or layer (Clay).
+ *
+ * garage_ec_range_plan (host only, one request): the byte runs a gatherer fetches, in the format, order and merge
+ * rule of garage_ec_read_ranges (overlapping runs are merged too): the range bytes of the present touched data
+ * shards, and, if a touched data shard is absent, the runs the code's own plan names for want = the absent touched
+ * data shards, cut to the window (RS / LRC: garage_ec_read_set shards; PB: garage_ec_read_plan halves; Clay: the
+ * repair layers of garage_ec_read_ranges when that shard is the only absent one, else every layer of the first k
+ * present shards).  *needs_gpu (nullable) = 1 iff a touched data shard is absent.  GARAGE_EC_E_INVALID for
+ * offset + len > block_len or more than cap runs; GARAGE_EC_E_UNRECOVERABLE if the absent touched data shards cannot
+ * be rebuilt.  A Clay range of a layer (L/alpha bytes) or more in an absent shard costs a whole-shard repair.
+ *
+ * garage_ec_decode_range: n requests on the shard layout (stride rules of reconstruct; only the planned runs need
+ * hold valid bytes).  block_len / offset / len: n values each.  Request s writes its len[s] bytes at
+ * out + s*out_stride; status (nullable, n int32): 0, GARAGE_EC_E_UNRECOVERABLE (nothing written) or -- DEVICE --
+ * GARAGE_EC_E_INVALID for offset + len > block_len or a shard length past `stride`.
+ *   DEVICE: all pointers device memory; out 16-byte aligned, out_stride a multiple of 16 >= roundup16(len[s]), bytes
+ *           [len, roundup16(len)) of a request are written as zero.  Only kernels and stream-ordered scratch of about
+ *           n*(k+m)*stride bytes are enqueued (capturable in a CUDA graph).  shards is never written.
+ *   HOST:   synchronous; any output alignment.  Uploads only the planned window runs, packed into sub-stripes,
+ *           downloads only the rebuilt range bytes; present range bytes are copied on the host.  GARAGE_EC_E_INVALID
+ *           before any GPU work for an invalid request; GARAGE_EC_E_UNRECOVERABLE if any request was.
+ * garage_ec_decode_range_stripes: the HOST gather form -- stripe s at stripes[s] (its k+m shards `stride` apart),
+ * request s writes at outs[s] -- as garage_ec_reconstruct_stripes is to garage_ec_reconstruct.                     */
+int garage_ec_range_plan(const garage_ec_ctx *ctx, const uint8_t *present, uint32_t block_len, uint32_t offset,
+                         uint32_t len, garage_ec_range *ranges, size_t cap, size_t *n_ranges, int *needs_gpu);
+int garage_ec_decode_range(garage_ec_ctx *ctx, const uint8_t *shards, const uint8_t *present, const uint32_t *block_len,
+                           const uint32_t *offset, const uint32_t *len, size_t stride, uint8_t *out, size_t out_stride,
+                           int32_t *status, size_t n, int mem_kind, void *cuda_stream);
+int garage_ec_decode_range_stripes(garage_ec_ctx *ctx, const uint8_t *const *stripes, const uint8_t *present,
+                                   const uint32_t *block_len, const uint32_t *offset, const uint32_t *len, size_t stride,
+                                   uint8_t *const *outs, int32_t *status, size_t n);
 
 /* ---- TRANSCODE -- changing a cluster's code (DESIGN.md section 2.3): resync after an `erasure_coding` config change
  * rewrites every block stored under an old code -- a whole-block replica (src = NULL), RS, LRC or PB -- under the

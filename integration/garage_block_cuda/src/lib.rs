@@ -81,6 +81,41 @@ impl ErasureCoder {
         Ok(())
     }
 
+    /// Ranged read (body_from_blocks_range; UploadPartCopy's source range), step 1: the byte runs
+    /// (shard, offset, len) to fetch for bytes [offset, offset+len) of a block, and whether a touched data shard is
+    /// absent (the range then needs `read_range`; otherwise it is the runs' bytes in order).  Plain blocks only: an
+    /// SSE-C or `Compressed` block is decrypted / decompressed as a whole, so those keep the whole-block GET.
+    pub fn range_plan(&self, hash: &Hash, present: &[bool], block_len: usize, offset: usize, len: usize)
+        -> Result<(Vec<(u32, u32, u32)>, bool), Error>
+    {
+        let pr: Vec<u8> = present.iter().map(|p| *p as u8).collect();
+        let cap = (self.k + self.m) * 512;
+        let mut runs: Vec<sys::garage_ec_range> = (0..cap).map(|_| sys::garage_ec_range { shard: 0, offset: 0, len: 0 }).collect();
+        let (mut n, mut gpu) = (0usize, 0i32);
+        let rc = unsafe { sys::garage_ec_range_plan(self.ctx, pr.as_ptr(), block_len as u32, offset as u32, len as u32,
+                          runs.as_mut_ptr(), cap, &mut n, &mut gpu) };
+        if rc == sys::GARAGE_EC_E_UNRECOVERABLE { return Err(Error::MissingBlock(*hash)); }
+        check(self.ctx, rc)?;
+        Ok((runs[..n].iter().map(|r| (r.shard, r.offset, r.len)).collect(), gpu != 0))
+    }
+
+    /// Ranged read, step 2: `stripe` holds the k+m shards `stride` apart with (at least) the planned runs filled in;
+    /// returns bytes [offset, offset+len) of the block, rebuilding absent columns on the GPU.  Only the shard tags
+    /// prove these bytes: the block's blake2sum needs the whole block (the deep scrub finds stale shards).
+    pub fn read_range(&self, hash: &Hash, stripe: &[u8], stride: usize, present: &[bool], block_len: usize,
+                      offset: usize, len: usize) -> Result<Vec<u8>, Error>
+    {
+        let pr: Vec<u8> = present.iter().map(|p| *p as u8).collect();
+        let mut out = vec![0u8; len];
+        let (bl, off, ln, mut st) = ([block_len as u32], [offset as u32], [len as u32], [0i32]);
+        let (sp, op) = ([stripe.as_ptr()], [out.as_mut_ptr()]);
+        let rc = unsafe { sys::garage_ec_decode_range_stripes(self.ctx, sp.as_ptr(), pr.as_ptr(), bl.as_ptr(),
+                          off.as_ptr(), ln.as_ptr(), stride, op.as_ptr(), st.as_mut_ptr(), 1) };
+        if rc == sys::GARAGE_EC_E_UNRECOVERABLE { return Err(Error::MissingBlock(*hash)); }
+        check(self.ctx, rc)?;
+        Ok(out)
+    }
+
     /// Scrub: bit i of the result set = stored parity row i disagrees with the data shards.
     pub fn verify(&self, shards_layout: &[u8], shard_len: &[u32], stride: usize) -> Result<Vec<u32>, Error> {
         let n = shard_len.len();

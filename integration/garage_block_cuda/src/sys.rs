@@ -48,6 +48,20 @@ extern "C" {
                             virtual_nodes: *mut c_int, base_rows: *mut u8) -> c_int;
     pub fn garage_ec_read_ranges(ctx: *const garage_ec_ctx, present: *const u8, want: *const u8, shard_len: u32,
                             ranges: *mut garage_ec_range, cap: usize, n_ranges: *mut usize) -> c_int;
+    pub fn garage_ec_tag_span(kind: c_int, shard_len: u32, off: u32, len: u32, span_off: *mut u32,
+                            span_len: *mut u32) -> c_int;
+    pub fn garage_ec_check_shard_span_host(kind: c_int, bytes: *const u8, shard_len: u32, span_off: u32,
+                            span_len: u32, tag32: *const u8) -> c_int;
+    pub fn garage_ec_range_plan(ctx: *const garage_ec_ctx, present: *const u8, block_len: u32, offset: u32, len: u32,
+                            ranges: *mut garage_ec_range, cap: usize, n_ranges: *mut usize,
+                            needs_gpu: *mut c_int) -> c_int;
+    pub fn garage_ec_decode_range(ctx: *mut garage_ec_ctx, shards: *const u8, present: *const u8,
+                            block_len: *const u32, offset: *const u32, len: *const u32, stride: usize, out: *mut u8,
+                            out_stride: usize, status: *mut i32, n: usize, mem_kind: c_int,
+                            cuda_stream: *mut c_void) -> c_int;
+    pub fn garage_ec_decode_range_stripes(ctx: *mut garage_ec_ctx, stripes: *const *const u8, present: *const u8,
+                            block_len: *const u32, offset: *const u32, len: *const u32, stride: usize,
+                            outs: *const *mut u8, status: *mut i32, n: usize) -> c_int;
     pub fn garage_ec_strerror(code: c_int) -> *const c_char;
     pub fn garage_ec_last_error(ctx: *const garage_ec_ctx) -> *const c_char;
     pub fn garage_ec_abi_version() -> c_int;
