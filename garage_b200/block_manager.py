@@ -20,7 +20,7 @@ SYMBOLS = [
     "garage_bm_bench", "garage_bm_corrupt_shard_header", "garage_bm_plant_stale_shard", "garage_bm_set_node_readonly",
     "garage_bm_convert_step", "garage_bm_debug_convert_stop_after", "garage_bm_apply_layout", "garage_bm_layout_sync_step",
     "garage_bm_layout_versions", "garage_bm_deep_scrub_step", "garage_bm_rpc_get_block_range",
-    "garage_bm_get_range_metrics",
+    "garage_bm_get_range_metrics", "garage_bm_stripe_repair_step", "garage_bm_get_stripe_repair_metrics",
 ]
 SUM_BLAKE2, SUM_ADLER8 = 0, 1
 
@@ -68,6 +68,12 @@ class Metrics(C.Structure):
 
 class RangeMetrics(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("range_gets", "range_degraded", "range_bytes_read", "range_bytes_fetched")]
+
+
+class StripeRepairMetrics(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in (
+        "stripe_repairs", "stripe_repair_shards", "stripe_repair_bytes_read", "stripe_repair_bytes_fetched",
+        "stripe_repair_bytes_written", "stripe_repair_errors", "stripe_repair_call_us")]
 
 
 _lib = None
@@ -118,6 +124,10 @@ def load_library():
         L.garage_bm_layout_versions.argtypes = [vp, C.POINTER(C.c_uint64), i32]
         L.garage_bm_deep_scrub_step.argtypes = [vp, i32, vp, sz, vp, C.POINTER(i32), C.POINTER(C.c_uint64),
                                                 C.POINTER(C.c_uint64)]
+        L.garage_bm_stripe_repair_step.argtypes = [vp, i32, vp, sz, i32, vp, C.POINTER(i32), C.POINTER(C.c_uint64),
+                                                   C.POINTER(C.c_uint64)]
+        L.garage_bm_get_stripe_repair_metrics.argtypes = [vp, C.POINTER(StripeRepairMetrics)]
+        L.garage_bm_get_stripe_repair_metrics.restype = None
         _lib = L
     return _lib
 
@@ -258,6 +268,34 @@ class BlockManager:
         rc = self._L.garage_bm_deep_scrub_step(self._h, node, C.c_char_p(bytes(cursor)) if cursor else None, max_blocks,
                                                C.cast(out, C.c_void_p), C.byref(fin), C.byref(a), C.byref(b))
         return rc, out.raw, bool(fin.value), a.value, b.value
+
+    def stripe_repair_step(self, node, cursor=None, max_blocks=0, min_missing=0):
+        """-> (rc, cursor_out bytes, finished, stripes repaired, shards rebuilt)"""
+        out = C.create_string_buffer(32)
+        fin, a, b = C.c_int(0), C.c_uint64(0), C.c_uint64(0)
+        rc = self._L.garage_bm_stripe_repair_step(self._h, node, C.c_char_p(bytes(cursor)) if cursor else None, max_blocks,
+                                                  min_missing, C.cast(out, C.c_void_p), C.byref(fin), C.byref(a),
+                                                  C.byref(b))
+        return rc, out.raw, bool(fin.value), a.value, b.value
+
+    def stripe_repair_all(self, min_missing=0):
+        """one full stripe_repair_step sweep of every node that is up -> (stripes repaired, shards rebuilt); an error
+        from a node that is up raises BlockManagerError"""
+        repaired = rebuilt = 0
+        for node in range(self.n_nodes):
+            if node in self._down:
+                continue
+            rc, _, finished, a, b = self.stripe_repair_step(node, min_missing=min_missing)
+            if rc != OK:
+                raise BlockManagerError(rc)
+            assert finished
+            repaired, rebuilt = repaired + a, rebuilt + b
+        return repaired, rebuilt
+
+    def stripe_repair_metrics(self):
+        mt = StripeRepairMetrics()
+        self._L.garage_bm_get_stripe_repair_metrics(self._h, C.byref(mt))
+        return {n: getattr(mt, n) for n, _ in StripeRepairMetrics._fields_}
 
     def convert_step(self, node, cursor=None, max_blocks=0):
         """-> (rc, cursor_out bytes, finished, converted)"""

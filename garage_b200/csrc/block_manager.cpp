@@ -672,6 +672,14 @@ struct Node {
         std::error_code ec;
         return std::filesystem::exists(path_of(h, ".shard"), ec);
     }
+    // a configured-code shard of h with this index whose header checks out is here (the stripe repair's probe, Garage's
+    // NeedBlockQuery): no shard bytes are read, so a shard with bad bytes is found when it is read
+    bool store_probe(const Hash &h, int index) const
+    {
+        if (!dir.empty()) return !path_at(h, index).empty();
+        const ShardPtr sp = store_find(h);
+        return sp && sp->index == index && meta_valid(*sp);
+    }
     bool store_erase(const Hash &h)
     {
         if (dir.empty()) return shards.erase(h) != 0;
@@ -1030,6 +1038,7 @@ struct ReconItem {
     bool range = false;
     uint32_t off = 0, len = 0;
     uint8_t *out = nullptr;
+    std::atomic<uint64_t> *call_us = nullptr;  // non-NULL: also gets the wall time of the call that rebuilt this stripe
     bool fulfilled = false;
     std::promise<int> done;
 };
@@ -1128,6 +1137,8 @@ struct garage_bm {
         range_bytes_fetched{0};
     std::atomic<uint64_t> layout_shards_copied{0}, layout_shards_rebuilt{0}, layout_bytes_read{0}, layout_bytes_written{0},
         layout_deleted{0}, layout_sync_errors{0}, layout_bytes_fetched{0};
+    std::atomic<uint64_t> stripe_repairs{0}, stripe_repair_shards{0}, stripe_repair_bytes_read{0},
+        stripe_repair_bytes_fetched{0}, stripe_repair_bytes_written{0}, stripe_repair_errors{0}, stripe_repair_call_us{0};
 
     // Bytes a rebuild from the shards `have` hands to the GPU, which is what crosses the network in Garage: the runs
     // garage_ec_read_ranges names for a Clay stripe (1/m of each helper for a lone lost shard), else what was read
@@ -1385,7 +1396,14 @@ struct garage_bm {
         const auto t0 = Clock::now();
         int rc = garage_ec_reconstruct_stripes(rec_ctx[w], stripes.data(), present.data(), want.data(), status.data(),
                                                lens.data(), slot_stride, n);
-        rec_gpu_us += (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count();
+        const uint64_t us = (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count();
+        rec_gpu_us += us;
+        std::vector<std::atomic<uint64_t> *> counted;  // each extra counter gets the call's time once
+        for (size_t i = 0; i < n; i++)
+            if (b[i]->call_us && std::find(counted.begin(), counted.end(), b[i]->call_us) == counted.end()) {
+                counted.push_back(b[i]->call_us);
+                *b[i]->call_us += us;
+            }
         for (size_t i = 0; i < n; i++) {
             int r = rc;
             if (rc == GARAGE_EC_OK || rc == GARAGE_EC_E_UNRECOVERABLE) r = status[i] ? GARAGE_BM_E_MISSING_BLOCK : GARAGE_BM_OK;
@@ -2093,19 +2111,36 @@ struct garage_bm {
         }
         return 0;
     }
-    // Receive, second choice: rebuild shard idx of each block on `node` from the survivors of every active version,
-    // like resync_block's fetch branch, batch_max_blocks stripes per garage_ec_reconstruct_stripes.  Returns the number
-    // written; *clean = false if one could not be rebuilt or written.
-    // Concurrent syncs run their rebuild batches one at a time (layout_rebuild_mu), and a batch takes its stripe slots
-    // from the shared pool in one step, so it never holds part of the pool while it waits for the rest.
-    std::mutex layout_rebuild_mu;
-    size_t rebuild_batch(int node, const std::vector<std::pair<Hash, int>> &todo, std::atomic<bool> *clean)
+    // One stripe of a rebuild batch: the shards `want` of h are rebuilt and shard i is written to node to[i].  skip: a
+    // node whose wanted shards are not read (a layout sync's receiver), -1 none.  grow: a survivor the gather
+    // quarantines becomes one more wanted shard if its holder to[i] is up, and the stripe is gathered again for it.
+    struct RebuildJob {
+        Hash h{};
+        uint8_t want[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
+        int to[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
+        int skip = -1;
+        bool grow = false;
+        int written = 0;  // out: the shards written; -1: the stripe could not be rebuilt
+    };
+    // where a rebuild batch counts: the bytes read and handed to the rebuild, the shards and bytes written, the errors
+    // (an unrecoverable stripe, a failed write: one each) and the time of its reconstruct calls (nullable)
+    struct RebuildCounters {
+        std::atomic<uint64_t> &read, &fetched, &shards, &written, &errors;
+        std::atomic<uint64_t> *call_us;
+        bool counted;  // the writes are file operations of garage_bm_debug_convert_stop_after
+    };
+    // Rebuild the jobs' stripes from their survivors, like resync_block's fetch branch, batch_max_blocks stripes per
+    // garage_ec_reconstruct_stripes.  Returns the number of shards written; *errors = the errors counted.
+    // Concurrent callers run their batches one at a time (rebuild_mu), and a batch takes its stripe slots from the
+    // shared pool in one step, so it never holds part of the pool while it waits for the rest.
+    std::mutex rebuild_mu;
+    size_t rebuild_batch(std::vector<RebuildJob> &jobs, const RebuildCounters &c, size_t *errors = nullptr)
     {
-        std::lock_guard<std::mutex> rl(layout_rebuild_mu);
+        std::lock_guard<std::mutex> rl(rebuild_mu);
         const size_t bmax = std::max<uint32_t>(cfg.batch_max_blocks, 1);
-        std::atomic<size_t> written{0};
-        for (size_t b0 = 0; b0 < todo.size(); b0 += bmax) {
-            const size_t n = std::min(bmax, todo.size() - b0);
+        std::atomic<size_t> written{0}, nerr{0};
+        for (size_t b0 = 0; b0 < jobs.size(); b0 += bmax) {
+            const size_t n = std::min(bmax, jobs.size() - b0);
             struct Slots {
                 SlotPool &pool;
                 std::vector<uint8_t *> p;
@@ -2114,17 +2149,28 @@ struct garage_bm {
             std::vector<ReconItem> items(n);
             std::vector<uint8_t> ok(n, 0);
             parallel_for(n, [&](size_t j, std::vector<uint8_t> &) {
-                const Hash &h = todo[b0 + j].first;
+                const RebuildJob &jb = jobs[b0 + j];
                 ReconItem &it = items[j];
                 it.stripe = slots.p[j];
                 it.stride = slot_stride;
-                it.want[todo[b0 + j].second] = 1;
-                bool g = false;
-                uint64_t nbytes = 0;
-                gather_into(h, node, it.stripe, it.present, it.block_len, false, /*for_gpu=*/true, it.want, &g, &nbytes);
-                layout_bytes_read += nbytes;
-                layout_bytes_fetched += g ? fetched_bytes(it.present, it.want, it.block_len, nbytes) : nbytes;
-                ok[j] = g;
+                it.call_us = c.call_us;
+                memcpy(it.want, jb.want, tot);
+                for (;;) {
+                    bool g = false;
+                    uint64_t nbytes = 0;
+                    gather_into(jb.h, jb.skip, it.stripe, it.present, it.block_len, false, /*for_gpu=*/true, it.want, &g,
+                                &nbytes);
+                    c.read += nbytes;
+                    c.fetched += g ? fetched_bytes(it.present, it.want, it.block_len, nbytes) : nbytes;
+                    ok[j] = g;
+                    bool more = false;
+                    for (int i = 0; jb.grow && i < tot; i++)
+                        if (!it.want[i] && !it.present[i] && probe(jb.to[i], jb.h, i) == 0) {
+                            it.want[i] = 1;
+                            more = true;
+                        }
+                    if (!more) break;
+                }
             });
             std::vector<ReconItem *> batch;
             for (size_t j = 0; j < n; j++)
@@ -2135,29 +2181,42 @@ struct garage_bm {
             for (size_t q = 0, j = 0; j < n; j++)
                 if (ok[j]) ok[j] = rc[q++] == GARAGE_BM_OK;
             parallel_for(n, [&](size_t j, std::vector<uint8_t> &) {
-                const Hash &h = todo[b0 + j].first;
-                const int idx = todo[b0 + j].second;
+                RebuildJob &jb = jobs[b0 + j];
                 if (!ok[j]) {
-                    layout_sync_errors++;
-                    *clean = false;
+                    jb.written = -1;
+                    c.errors++;
+                    nerr++;
                     return;
                 }
                 const uint32_t len = items[j].block_len;
                 const size_t L = shard_len_of(len);
-                const uint8_t *bytes = items[j].stripe + (size_t)idx * slot_stride;
-                Hash sum;
-                shard_tag(bytes, L, sum);
-                if (!write_shard(node, h, idx, len, bytes, L, sum.data(), true)) {
-                    layout_sync_errors++;
-                    *clean = false;
-                    return;
+                for (int i = 0; i < tot; i++) {
+                    if (!items[j].want[i]) continue;
+                    const uint8_t *bytes = items[j].stripe + (size_t)i * slot_stride;
+                    Hash sum;
+                    shard_tag(bytes, L, sum);
+                    if (!write_shard(jb.to[i], jb.h, i, len, bytes, L, sum.data(), c.counted)) {
+                        c.errors++;
+                        nerr++;
+                        continue;
+                    }
+                    c.shards++;
+                    c.written += L;
+                    jb.written++;
+                    written++;
                 }
-                layout_shards_rebuilt++;
-                layout_bytes_written += L;
-                written++;
             });
         }
+        if (errors) *errors = nerr;
         return written;
+    }
+    // what holder `node` says of shard i of h: 1 it holds a valid-looking one (Node::store_probe), 0 it does not, -1 down
+    int probe(int node, const Hash &h, int i)
+    {
+        Node &nd = *nodes[node];
+        std::lock_guard<std::mutex> lk(nd.mu);
+        if (!nd.up) return -1;
+        return nd.store_probe(h, i) ? 1 : 0;
     }
     // the newest version's stripe of h holds its write quorum: k+1 configured-code shards with valid tags on their nodes.
     // by_index: each read from the file holding its assigned index (the newest stripe during a layout change)
@@ -2279,7 +2338,18 @@ struct garage_bm {
             }
         });
         std::sort(rebuild.begin(), rebuild.end());
-        n_moved += rebuild_batch(node, rebuild, &clean);
+        std::vector<RebuildJob> jobs(rebuild.size());
+        for (size_t j = 0; j < rebuild.size(); j++) {
+            jobs[j].h = rebuild[j].first;
+            jobs[j].want[rebuild[j].second] = 1;
+            jobs[j].to[rebuild[j].second] = node;
+            jobs[j].skip = node;
+        }
+        size_t errs = 0;
+        n_moved += rebuild_batch(jobs, {layout_bytes_read, layout_bytes_fetched, layout_shards_rebuilt, layout_bytes_written,
+                                        layout_sync_errors, nullptr, true},
+                                 &errs);
+        if (errs) clean = false;
         // offload: deleted only once the newest stripe is seen at its write quorum (the deletion rule of DESIGN.md 5.1)
         parallel_for(offload.size(), [&](size_t j, std::vector<uint8_t> &buf) {
             buf.resize(slot_stride);
@@ -2614,8 +2684,9 @@ struct garage_bm {
         for (auto &t : th) t.join();
     }
 
-    // the node that deep-scrubs h: the first up node of its row in the newest layout version, -1 if none is up
-    int deep_scrub_owner(const Hash &h)
+    // the node that deep-scrubs and stripe-repairs h: the first up node of its row in the newest layout version, -1 if
+    // none is up
+    int repair_owner(const Hash &h)
     {
         int who[64];
         storage_nodes_of(h, who);
@@ -2625,6 +2696,22 @@ struct garage_bm {
             if (nd.up) return who[i];
         }
         return -1;
+    }
+    // the known blocks not at rc 0 whose repair owner is `node`
+    std::vector<Hash> owned_blocks(int node)
+    {
+        std::vector<Hash> hs;
+        {
+            std::lock_guard<std::mutex> lk(refs_mu);
+            for (auto &kv : refs) {
+                auto it = rc.find(kv.first);
+                if (it == rc.end() || it->second.count > 0) hs.push_back(kv.first);
+            }
+        }
+        std::vector<Hash> mine;
+        for (const Hash &h : hs)
+            if (repair_owner(h) == node) mine.push_back(h);
+        return mine;
     }
 
     // garage_bm_deep_scrub_step: see include/garage_block_manager.h and DESIGN.md section 5.4
@@ -2636,17 +2723,7 @@ struct garage_bm {
             std::lock_guard<std::mutex> lk(nd.mu);
             if (!nd.up) return GARAGE_BM_E_MESSAGE;
         }
-        std::vector<Hash> hs;
-        {
-            std::lock_guard<std::mutex> lk(refs_mu);
-            for (auto &kv : refs) {
-                auto it = rc.find(kv.first);
-                if (it == rc.end() || it->second.count > 0) hs.push_back(kv.first);
-            }
-        }
-        std::vector<Hash> mine;
-        for (const Hash &h : hs)
-            if (deep_scrub_owner(h) == node) mine.push_back(h);
+        std::vector<Hash> mine = owned_blocks(node);
         sweep_page(mine, cursor, max_blocks, cursor_out, finished);
         uint64_t nchecked = 0, nrep = 0;
         std::lock_guard<std::mutex> dl(deep_mu);
@@ -2723,6 +2800,51 @@ struct garage_bm {
         }
         if (checked) *checked = nchecked;
         if (repaired) *repaired = nrep;
+        return GARAGE_BM_OK;
+    }
+
+    // garage_bm_stripe_repair_step: see include/garage_block_manager.h and DESIGN.md section 5.6
+    int stripe_repair_step(int node, const Hash *cursor, size_t max_blocks, int min_missing, Hash *cursor_out,
+                           int *finished, uint64_t *repaired, uint64_t *rebuilt)
+    {
+        {
+            Node &nd = *nodes[node];
+            std::lock_guard<std::mutex> lk(nd.mu);
+            if (!nd.up) return GARAGE_BM_E_MESSAGE;
+        }
+        if (multi_version()) return GARAGE_EC_E_INVALID;  // layout sync rebuilds (DESIGN.md section 5.2)
+        std::vector<Hash> mine = owned_blocks(node);
+        sweep_page(mine, cursor, max_blocks, cursor_out, finished);
+        std::vector<RebuildJob> jobs;
+        for (const Hash &h : mine) {
+            RebuildJob jb;
+            jb.h = h;
+            jb.grow = true;
+            storage_nodes_of(h, jb.to);
+            int present = 0, targets = 0;
+            for (int i = 0; i < tot; i++) {
+                const int p = probe(jb.to[i], h, i);
+                present += p > 0;
+                if (p == 0) {
+                    jb.want[i] = 1;
+                    targets++;
+                }
+            }
+            // nothing of the configured code while older copies may exist: the conversion sweep's block
+            if (!targets || tot - present < min_missing || (present == 0 && has_legacy())) continue;
+            jobs.push_back(jb);
+        }
+        rebuild_batch(jobs, {stripe_repair_bytes_read, stripe_repair_bytes_fetched, stripe_repair_shards,
+                             stripe_repair_bytes_written, stripe_repair_errors, &stripe_repair_call_us, false});
+        uint64_t nrep = 0, nshards = 0;
+        for (const RebuildJob &jb : jobs)
+            if (jb.written > 0) {
+                nrep++;
+                nshards += (uint64_t)jb.written;
+            }
+        stripe_repairs += nrep;
+        if (repaired) *repaired = nrep;
+        if (rebuilt) *rebuilt = nshards;
         return GARAGE_BM_OK;
     }
 
@@ -3075,7 +3197,7 @@ struct garage_bm {
         return GARAGE_BM_E_MESSAGE;          \
     }
 
-// the four resumable sweeps: the cursor in and out of one garage_bm_*_step call
+// the resumable sweeps: the cursor in and out of one garage_bm_*_step call
 template <class Step>
 static int bm_step(garage_bm *bm, int node, const uint8_t *cursor32, uint8_t *cursor_out32, Step step)
 {
@@ -3454,6 +3576,15 @@ int garage_bm_deep_scrub_step(garage_bm *bm, int node, const uint8_t *cursor32, 
     });
 }
 
+int garage_bm_stripe_repair_step(garage_bm *bm, int node, const uint8_t *cursor32, size_t max_blocks, int min_missing,
+                                 uint8_t cursor_out32[32], int *finished, uint64_t *repaired_blocks,
+                                 uint64_t *rebuilt_shards)
+{
+    return bm_step(bm, node, cursor32, cursor_out32, [&](const Hash *cur, Hash *out) {
+        return bm->stripe_repair_step(node, cur, max_blocks, min_missing, out, finished, repaired_blocks, rebuilt_shards);
+    });
+}
+
 int garage_bm_convert_step(garage_bm *bm, int node, const uint8_t *cursor32, size_t max_blocks, uint8_t cursor_out32[32],
                            int *finished, uint64_t *converted)
 {
@@ -3655,6 +3786,18 @@ void garage_bm_get_range_metrics(garage_bm *bm, garage_bm_range_metrics *o)
     o->range_degraded = bm->range_degraded;
     o->range_bytes_read = bm->range_bytes_read;
     o->range_bytes_fetched = bm->range_bytes_fetched;
+}
+
+void garage_bm_get_stripe_repair_metrics(garage_bm *bm, garage_bm_stripe_repair_metrics *o)
+{
+    if (!bm || !o) return;
+    o->stripe_repairs = bm->stripe_repairs;
+    o->stripe_repair_shards = bm->stripe_repair_shards;
+    o->stripe_repair_bytes_read = bm->stripe_repair_bytes_read;
+    o->stripe_repair_bytes_fetched = bm->stripe_repair_bytes_fetched;
+    o->stripe_repair_bytes_written = bm->stripe_repair_bytes_written;
+    o->stripe_repair_errors = bm->stripe_repair_errors;
+    o->stripe_repair_call_us = bm->stripe_repair_call_us;
 }
 
 }  // extern "C"

@@ -176,6 +176,17 @@ typedef struct garage_bm_range_metrics {
     uint64_t range_bytes_read;    /* tag-span bytes those GETs read from shard files                      */
     uint64_t range_bytes_fetched; /* the planned run bytes: what would cross the network in Garage         */
 } garage_bm_range_metrics;
+/* Counters of garage_bm_stripe_repair_step, in a struct of their own for the same reason. */
+typedef struct garage_bm_stripe_repair_metrics {
+    uint64_t stripe_repairs;              /* stripes with at least one shard written                            */
+    uint64_t stripe_repair_shards;        /* shards written                                                     */
+    uint64_t stripe_repair_bytes_read;    /* bytes the holders read from their shard files                      */
+    uint64_t stripe_repair_bytes_fetched; /* bytes handed to the rebuild: what would cross the network in Garage.
+                                             Clay: the repair runs (1/m of each helper for one absent shard)    */
+    uint64_t stripe_repair_bytes_written; /* bytes of the shards written                                        */
+    uint64_t stripe_repair_errors;        /* unrecoverable stripes + shard writes that failed                   */
+    uint64_t stripe_repair_call_us;       /* wall time inside garage_ec_reconstruct_stripes                     */
+} garage_bm_stripe_repair_metrics;
 
 void garage_bm_default_config(garage_bm_config *cfg);
 int garage_bm_create(garage_bm **out, const garage_bm_config *cfg);
@@ -248,6 +259,26 @@ int garage_bm_scrub_step(garage_bm *bm, int node, const uint8_t *cursor32, size_
 int garage_bm_deep_scrub_step(garage_bm *bm, int node, const uint8_t *cursor32, size_t max_blocks,
                               uint8_t cursor_out32[32], int *finished, uint64_t *checked, uint64_t *repaired);
 
+/* Stripe repair (DESIGN.md section 5.6), resumable in hash order like garage_bm_deep_scrub_step over the same blocks:
+ * the known blocks not at rc 0 whose owner is `node` (the deep-scrub owner rule).  For each block:
+ *   - probe: each of the k+m holders is asked whether it holds a shard of its index whose file header checks out (no
+ *     shard bytes are read; Garage's NeedBlockQuery).  missing = k+m - present, a down holder counting as missing;
+ *     the targets are the missing indices whose holder is up;
+ *   - skip the block if it has no target or missing < min_missing (min_missing <= 1: every block with a target), or
+ *     if no shard of the configured code is present and previous codes or replicas are configured;
+ *   - gather once, want = the targets, through the code's own plan (RS: the first k; LRC: the union of the local
+ *     groups; PB: the planned halves; Clay: the repair runs when exactly one shard is absent, k whole shards
+ *     otherwise), tags checked on read.  A bad survivor is quarantined and the plan recomputed; if its holder is up
+ *     it becomes one more target;
+ *   - rebuild batch_max_blocks stripes per garage_ec_reconstruct_stripes, and write each rebuilt shard to its holder.
+ * Nothing is fatal: an unrecoverable stripe and a failed shard write each count one stripe_repair_errors, and the
+ * other targets of the stripe are still written.  *repaired_blocks = stripes with a shard written, *rebuilt_shards =
+ * shards written.  GARAGE_BM_E_MESSAGE if `node` is down; GARAGE_EC_E_INVALID while more than one layout version is
+ * active (layout sync rebuilds then).  Calls for different owners, and resync_all, may run concurrently.          */
+int garage_bm_stripe_repair_step(garage_bm *bm, int node, const uint8_t *cursor32, size_t max_blocks, int min_missing,
+                                 uint8_t cursor_out32[32], int *finished, uint64_t *repaired_blocks,
+                                 uint64_t *rebuilt_shards);
+
 /* Conversion sweep of `node` (DESIGN.md section 5.1), resumable in hash order like garage_bm_scrub_step: every block
  * with a legacy shard or replica on `node`, after cursor32 (NULL = from the start), at most max_blocks (0 = all):
  *   - the configured stripe holds its write quorum: this node deletes its legacy copies;
@@ -308,6 +339,7 @@ int garage_bm_node_shard_index(garage_bm *bm, int node, const uint8_t hash[32]);
 int garage_bm_storage_nodes_of(garage_bm *bm, const uint8_t hash[32], int *nodes_out /* k+m */);
 void garage_bm_get_metrics(garage_bm *bm, garage_bm_metrics *out);
 void garage_bm_get_range_metrics(garage_bm *bm, garage_bm_range_metrics *out);
+void garage_bm_get_stripe_repair_metrics(garage_bm *bm, garage_bm_stripe_repair_metrics *out);
 
 #ifdef __cplusplus
 }
