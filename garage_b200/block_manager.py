@@ -21,6 +21,7 @@ SYMBOLS = [
     "garage_bm_convert_step", "garage_bm_debug_convert_stop_after", "garage_bm_apply_layout", "garage_bm_layout_sync_step",
     "garage_bm_layout_versions", "garage_bm_deep_scrub_step", "garage_bm_rpc_get_block_range",
     "garage_bm_get_range_metrics", "garage_bm_stripe_repair_step", "garage_bm_get_stripe_repair_metrics",
+    "garage_bm_set_data_dirs", "garage_bm_rebalance_step", "garage_bm_get_drive_metrics", "garage_bm_create_with_drives",
 ]
 SUM_BLAKE2, SUM_ADLER8 = 0, 1
 
@@ -41,6 +42,24 @@ def _layout_spec(zone, capacity, zone_redundancy=0, max_per_zone=0):
     z = (C.c_int32 * max(1, len(zone)))(*map(int, zone))
     c = (C.c_uint64 * max(1, len(capacity)))(*map(int, capacity))
     return LayoutSpec(C.cast(z, C.POINTER(C.c_int32)), C.cast(c, C.POINTER(C.c_uint64)), zone_redundancy, max_per_zone), (z, c)
+
+
+class DataDir(C.Structure):
+    """garage_bm_data_dir: one drive of a node, path relative to the node directory"""
+    _fields_ = [("path", C.c_char_p), ("capacity", C.c_uint64), ("read_only", C.c_int)]
+
+
+def _data_dirs(dirs):
+    """(path, capacity) / (path, capacity, read_only) tuples or dicts -> (DataDir array or None, n)"""
+    rows = []
+    for d in dirs:
+        if isinstance(d, dict):
+            rows.append((d["path"], d.get("capacity", 0), d.get("read_only", False)))
+        else:
+            rows.append((d[0], d[1], d[2] if len(d) > 2 else False))
+    arr = (DataDir * max(1, len(rows)))(*[DataDir(p.encode() if isinstance(p, str) else p, int(c), int(bool(ro)))
+                                          for p, c, ro in rows])
+    return arr, len(rows)
 
 
 class Config(C.Structure):
@@ -68,6 +87,11 @@ class Metrics(C.Structure):
 
 class RangeMetrics(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("range_gets", "range_degraded", "range_bytes_read", "range_bytes_fetched")]
+
+
+class DriveMetrics(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in (
+        "rebalance_files_moved", "rebalance_bytes_moved", "rebalance_errors", "drive_marker_errors")]
 
 
 class StripeRepairMetrics(C.Structure):
@@ -128,6 +152,11 @@ def load_library():
                                                    C.POINTER(C.c_uint64)]
         L.garage_bm_get_stripe_repair_metrics.argtypes = [vp, C.POINTER(StripeRepairMetrics)]
         L.garage_bm_get_stripe_repair_metrics.restype = None
+        L.garage_bm_create_with_drives.argtypes = [C.POINTER(vp), C.POINTER(Config), C.POINTER(DataDir), i32]
+        L.garage_bm_set_data_dirs.argtypes = [vp, i32, C.POINTER(DataDir), i32]
+        L.garage_bm_rebalance_step.argtypes = [vp, i32, vp, sz, vp, C.POINTER(i32), C.POINTER(C.c_uint64)]
+        L.garage_bm_get_drive_metrics.argtypes = [vp, C.POINTER(DriveMetrics)]
+        L.garage_bm_get_drive_metrics.restype = None
         _lib = L
     return _lib
 
@@ -152,13 +181,15 @@ class BlockManager:
     def __init__(self, k=10, m=4, n_nodes=None, cuda_device=0, batch_max_blocks=64, batch_linger_us=100,
                  block_ram_buffer_max=256 << 20, data_dir=None, shard_sum_kind=SUM_ADLER8, verify_content_hash=True,
                  data_fsync=False, block_gc_delay_ms=0, local_groups=0, piggyback=False, previous_codes=(),
-                 legacy_replicas=0, layout=None, clay=False, clay_layout=False):
+                 legacy_replicas=0, layout=None, clay=False, clay_layout=False, data_dirs=None):
         """block_gc_delay_ms defaults to 0 HERE (tests delete at once); the library's default is the
         reference's BLOCK_GC_DELAY of 10 minutes.  local_groups > 0: LRC(k, local_groups, m - local_groups).
         piggyback: PB(k, m), half-shard repair reads.  clay: Clay(k, m), a lost shard rebuilt from 1/m of the others; clay_layout: that store may change its
         layout.  previous_codes: (k, m, local_groups, piggyback[, clay]) tuples of codes the store may still hold; legacy_replicas: replication factor of a previous replicated layout.
         layout: None (partition p on nodes (p mod n_nodes) + i) or a dict with zone, capacity and optionally
-        zone_redundancy, max_per_zone: version 1 of the cluster layout."""
+        zone_redundancy, max_per_zone: version 1 of the cluster layout.  data_dirs: None (one directory per node) or a list
+        of (path, capacity[, read_only]) tuples or {path, capacity, read_only} dicts, paths relative to each node's
+        directory: the drives every node spreads its files over."""
         self._L = load_library()
         cfg = Config()
         self._L.garage_bm_default_config(C.byref(cfg))
@@ -181,7 +212,11 @@ class BlockManager:
             self._spec, self._spec_arrays = _layout_spec(**layout)  # kept alive
             cfg.layout = C.pointer(self._spec)
         h = C.c_void_p()
-        rc = self._L.garage_bm_create(C.byref(h), C.byref(cfg))
+        if data_dirs is None:
+            rc = self._L.garage_bm_create(C.byref(h), C.byref(cfg))
+        else:
+            drives, n = _data_dirs(data_dirs)
+            rc = self._L.garage_bm_create_with_drives(C.byref(h), C.byref(cfg), drives, n)
         if rc != OK:
             raise BlockManagerError(rc)
         self._h, self.k, self.m, self.n_nodes = h, k, m, cfg.n_nodes
@@ -296,6 +331,44 @@ class BlockManager:
         mt = StripeRepairMetrics()
         self._L.garage_bm_get_stripe_repair_metrics(self._h, C.byref(mt))
         return {n: getattr(mt, n) for n, _ in StripeRepairMetrics._fields_}
+
+    def set_data_dirs(self, node, dirs):
+        """node restarts with this data_dir list ((path, capacity[, read_only]) tuples or dicts) -> rc; a failed marker
+        check (E_MESSAGE) leaves the node down, success brings it up"""
+        arr, n = _data_dirs(dirs)
+        rc = self._L.garage_bm_set_data_dirs(self._h, node, C.cast(arr, C.POINTER(DataDir)) if n else None, n)
+        if rc == OK:
+            self._down.discard(node)
+        elif rc == E_MESSAGE:
+            self._down.add(node)
+        return rc
+
+    def rebalance_step(self, node, cursor=None, max_files=0):
+        """-> (rc, cursor_out bytes, finished, files moved)"""
+        out = C.create_string_buffer(32)
+        fin, n = C.c_int(0), C.c_uint64(0)
+        rc = self._L.garage_bm_rebalance_step(self._h, node, C.c_char_p(bytes(cursor)) if cursor else None, max_files,
+                                              C.cast(out, C.c_void_p), C.byref(fin), C.byref(n))
+        return rc, out.raw, bool(fin.value), n.value
+
+    def rebalance_all(self, nodes=None):
+        """one full rebalance_step pass over every node that is up (or over `nodes`) -> files moved; an error from a
+        node that is up raises BlockManagerError"""
+        total = 0
+        for node in (range(self.n_nodes) if nodes is None else nodes):
+            if node in self._down:
+                continue
+            rc, _, finished, n = self.rebalance_step(node)
+            if rc != OK:
+                raise BlockManagerError(rc)
+            assert finished
+            total += n
+        return total
+
+    def drive_metrics(self):
+        mt = DriveMetrics()
+        self._L.garage_bm_get_drive_metrics(self._h, C.byref(mt))
+        return {n: getattr(mt, n) for n, _ in DriveMetrics._fields_}
 
     def convert_step(self, node, cursor=None, max_blocks=0):
         """-> (rc, cursor_out bytes, finished, converted)"""

@@ -33,6 +33,7 @@
 #include <memory>
 #include <mutex>
 #include <new>
+#include <random>
 #include <string>
 #include <type_traits>
 #include <thread>
@@ -386,11 +387,271 @@ struct Node {
     std::unordered_set<Hash, HashHasher> queued;
 
     // Node is the only owner of the file scheme: the names below, the header and the placement rules of DESIGN.md
-    // sections 5.1 / 5.2.  The files of one hash, by ShardFile:
+    // sections 5.1 / 5.2 / 5.7.  The files of one hash, by ShardFile:
     enum ShardFile { kShardFile = 0, kLegacyFile = 1, kReplicaFile = 2 };
     static constexpr const char *kExt[3] = {".shard", ".legacy", ""};
-    std::string dir_of(const Hash &h) const { return dir + "/" + hex_of(h.data(), 1) + "/" + hex_of(h.data() + 1, 1); }
-    std::string path_of(const Hash &h, const char *ext) const { return dir_of(h) + "/" + hex_of(h.data(), 32) + ext; }
+    // Drives (DESIGN.md section 5.7): with a drive layout the files of h live in <root>/<hh>/<hh>/ of one of `drives`,
+    // the primary of h's drive partition (where every write goes) or one of its secondaries (where reads look after
+    // the primary).  Drives are separate filesystems: a rename never crosses from one drive to another.  No drives:
+    // every file under `dir`, as before.
+    struct Drive {
+        std::string path;    // as configured, relative to `dir`
+        std::string root;    // dir + "/" + path, or dir for "."
+        std::string marker;  // the garage-marker id recorded for it ("" = none yet)
+        uint64_t capacity = 0;
+        bool read_only = false;
+    };
+    std::vector<Drive> drives;
+    std::shared_ptr<garage_drive_layout> dlayout;
+    // the drives of h's partition: the primary, then the secondaries in read order
+    std::vector<int> drives_of(const Hash &h) const
+    {
+        const int p = garage_drive_partition_of(h.data());
+        uint8_t sec[GARAGE_DRIVE_MAX_DIRS];
+        const int n = std::max(0, std::min(GARAGE_DRIVE_MAX_DIRS, garage_drive_layout_secondaries(dlayout.get(), p, sec, GARAGE_DRIVE_MAX_DIRS)));
+        std::vector<int> r{garage_drive_layout_primary(dlayout.get(), p)};
+        r.insert(r.end(), sec, sec + n);
+        return r;
+    }
+    static std::string dir_in(const std::string &root, const Hash &h)
+    {
+        return root + "/" + hex_of(h.data(), 1) + "/" + hex_of(h.data() + 1, 1);
+    }
+    static std::string name_of(const Hash &h, const char *ext) { return hex_of(h.data(), 32) + ext; }
+    // where a new file of h goes: the primary drive's directory
+    std::string dir_of(const Hash &h) const { return dir_in(drives.empty() ? dir : drives[drives_of(h)[0]].root, h); }
+    std::string primary_path(const Hash &h, const char *ext) const { return dir_of(h) + "/" + name_of(h, ext); }
+    // the file `ext` of h: the first of the primary and the secondaries that has it, else the primary's
+    std::string path_of(const Hash &h, const char *ext) const
+    {
+        if (drives.empty()) return primary_path(h, ext);
+        for (int d : drives_of(h)) {
+            const std::string p = dir_in(drives[d].root, h) + "/" + name_of(h, ext);
+            if (::access(p.c_str(), F_OK) == 0) return p;
+        }
+        return primary_path(h, ext);
+    }
+    // the name `ext` of h next to the file at `path` (the same directory, so a rename to it stays on its drive)
+    static std::string sibling(const std::string &path, const Hash &h, const char *ext)
+    {
+        return path.substr(0, path.rfind('/') + 1) + name_of(h, ext);
+    }
+    // the name `ext` of h removed from the primary and every secondary; true if a file was removed
+    bool remove_file(const Hash &h, const char *ext)
+    {
+        if (drives.empty()) return ::remove(path_of(h, ext).c_str()) == 0;
+        bool any = false;
+        for (int d : drives_of(h)) any = ::remove((dir_in(drives[d].root, h) + "/" + name_of(h, ext)).c_str()) == 0 || any;
+        return any;
+    }
+    // copies of the name `ext` of h other than the one at `keep`, removed: a write to the primary replaces them, as a
+    // rename over the name does in one directory
+    void remove_copies(const Hash &h, const char *ext, const std::string &keep)
+    {
+        if (drives.empty()) return;
+        for (int d : drives_of(h)) {
+            const std::string p = dir_in(drives[d].root, h) + "/" + name_of(h, ext);
+            if (p != keep) ::remove(p.c_str());
+        }
+    }
+    // ---- the drive layout's own files: <dir>/data_layout and a garage-marker in every drive
+    uint64_t drive_gen = 0;  // bumped by every change of `drives` (a rebalance pass drops secondaries of its own layout only)
+    std::string drive_layout_path() const { return dir + "/data_layout"; }
+    // Garage's dir_not_empty: a garage-marker file or a hex-named subdirectory
+    static bool dir_non_empty(const std::string &root)
+    {
+        std::error_code ec;
+        if (std::filesystem::exists(root + "/garage-marker", ec)) return true;
+        for (const auto &e : std::filesystem::directory_iterator(root, ec)) {
+            std::error_code ec2;
+            const std::string n = e.path().filename().string();
+            std::vector<uint8_t> b(n.size() / 2 + 1);
+            if (!n.empty() && n.size() % 2 == 0 && hex_to(n, n.size() / 2, b.data()) && e.is_directory(ec2)) return true;
+        }
+        return false;
+    }
+    // <dir>/data_layout, atomically: format version, every drive (path, capacity, read-only, marker), the layout image,
+    // and an Adler-32 of all of that
+    bool save_drives() const
+    {
+        std::string s = "garage-bm-data-layout 1\n";
+        for (const Drive &d : drives) {
+            s += "dir " + hex_of(reinterpret_cast<const uint8_t *>(d.path.data()), d.path.size()) + " " +
+                 std::to_string(d.capacity) + " " + (d.read_only ? "1" : "0") + " " +
+                 (d.marker.empty() ? std::string("-") : hex_of(reinterpret_cast<const uint8_t *>(d.marker.data()), d.marker.size())) +
+                 "\n";
+        }
+        std::vector<uint8_t> img(garage_drive_layout_serialize(dlayout.get(), nullptr, 0));
+        garage_drive_layout_serialize(dlayout.get(), img.data(), img.size());
+        s += "layout " + hex_of(img.data(), img.size()) + "\n";
+        s += "check " + std::to_string(adler32_small(reinterpret_cast<const uint8_t *>(s.data()), s.size())) + "\n";
+        return write_file_atomic(drive_layout_path(), s.data(), s.size(), nullptr, 0, true, fsync_data);
+    }
+    // 1: `drives` and `dlayout` loaded from <dir>/data_layout; 0: no file; -1: a file that fails its check or format
+    int load_drives()
+    {
+        std::string s;
+        if (!read_file(drive_layout_path(), s)) return 0;
+        const size_t c = s.rfind("check ");
+        if (c == std::string::npos || (c > 0 && s[c - 1] != '\n')) return -1;
+        if (std::to_string(adler32_small(reinterpret_cast<const uint8_t *>(s.data()), c)) + "\n" != s.substr(c + 6)) return -1;
+        std::vector<std::string> tok;
+        for (size_t i = 0; i < c;) {
+            while (i < c && isspace((unsigned char)s[i])) i++;
+            const size_t j = i;
+            while (i < c && !isspace((unsigned char)s[i])) i++;
+            if (i > j) tok.push_back(s.substr(j, i - j));
+        }
+        auto unhex = [](const std::string &h, std::string &out) {
+            out.assign(h.size() / 2, '\0');
+            return h.size() % 2 == 0 && hex_to(h, h.size() / 2, reinterpret_cast<uint8_t *>(&out[0]));
+        };
+        size_t t = 0;
+        if (tok.size() < 2 || tok[t++] != "garage-bm-data-layout" || tok[t++] != "1") return -1;
+        std::vector<Drive> ds;
+        while (t + 5 <= tok.size() && tok[t] == "dir") {
+            Drive d;
+            char *e = nullptr;
+            errno = 0;
+            d.capacity = strtoull(tok[t + 2].c_str(), &e, 10);
+            if (errno || *e || !unhex(tok[t + 1], d.path) || d.path.empty() || (tok[t + 3] != "0" && tok[t + 3] != "1")) return -1;
+            d.read_only = tok[t + 3] == "1";
+            if (tok[t + 4] != "-" && !unhex(tok[t + 4], d.marker)) return -1;
+            d.root = root_of(d.path);
+            ds.push_back(std::move(d));
+            t += 5;
+        }
+        std::string img;
+        if (t + 2 != tok.size() || tok[t] != "layout" || !unhex(tok[t + 1], img)) return -1;
+        garage_drive_layout *l = nullptr;
+        if (garage_drive_layout_deserialize(&l, reinterpret_cast<const uint8_t *>(img.data()), img.size()) != GARAGE_LAYOUT_OK)
+            return -1;
+        dlayout.reset(l, garage_drive_layout_free);
+        bool ok = garage_drive_layout_n_dirs(l) == (int)ds.size();
+        std::vector<uint8_t> img2(img.size());
+        garage_drive_layout_serialize(l, img2.data(), img2.size());
+        for (size_t i = 0; ok && i < ds.size(); i++) {  // the image's capacities are the drives'
+            uint64_t cap = 0;
+            memcpy(&cap, img2.data() + 5 + 8 * i, 8);
+            ok = cap == (ds[i].read_only ? 0 : ds[i].capacity);
+        }
+        if (!ok) {
+            dlayout.reset();
+            return -1;
+        }
+        drives = std::move(ds);
+        drive_gen++;
+        return 1;
+    }
+    std::string root_of(const std::string &path) const { return path == "." ? dir : dir + "/" + path; }
+    // Garage's check_markers over `ds`: a recorded marker must be in its drive's garage-marker file; a drive without one
+    // records the file's, or writes a new random one.  false: a drive fails (unmounted, or another disk).
+    static bool check_markers(std::vector<Drive> &ds)
+    {
+        for (Drive &d : ds) {
+            std::string have;
+            const bool found = read_file(d.root + "/garage-marker", have);
+            if (!d.marker.empty()) {
+                if (!found || have != d.marker) return false;
+            } else if (found && !have.empty()) {
+                d.marker = have;
+            } else {
+                std::error_code ec;
+                std::filesystem::create_directories(d.root, ec);
+                std::random_device rd;
+                uint8_t id[16];
+                for (auto &b : id) b = (uint8_t)rd();
+                d.marker = hex_of(id, sizeof(id));
+                if (!write_file_atomic(d.root + "/garage-marker", d.marker.data(), d.marker.size(), nullptr, 0, true, true))
+                    return false;
+            }
+        }
+        return true;
+    }
+    // Garage restarting with the data_dir list `cfg` (garage_bm_data_dir, checked by the caller): the layout updated
+    // from the current one (initialised if there is none), markers checked, <dir>/data_layout written.  false: a marker
+    // check or the write failed, and nothing changed.
+    bool set_drives(const garage_bm_data_dir *cfg, int n)
+    {
+        std::vector<Drive> ds(n);
+        std::vector<int> prev_index(n, -1);
+        std::vector<uint64_t> cap(n);
+        std::vector<uint8_t> non_empty(n);
+        for (int i = 0; i < n; i++) {
+            ds[i].path = normal_path(cfg[i].path);
+            ds[i].root = root_of(ds[i].path);
+            ds[i].read_only = cfg[i].read_only != 0;
+            ds[i].capacity = ds[i].read_only ? 0 : cfg[i].capacity;
+            cap[i] = ds[i].capacity;
+            for (size_t j = 0; j < drives.size(); j++)
+                if (drives[j].path == ds[i].path) {
+                    prev_index[i] = (int)j;
+                    ds[i].marker = drives[j].marker;
+                }
+            non_empty[i] = dir_non_empty(ds[i].root);
+        }
+        garage_drive_layout *l = nullptr;
+        const int rc = dlayout ? garage_drive_layout_update(&l, dlayout.get(), prev_index.data(), n, cap.data(), non_empty.data())
+                               : garage_drive_layout_init(&l, n, cap.data(), non_empty.data());
+        if (rc != GARAGE_LAYOUT_OK) return false;
+        std::shared_ptr<garage_drive_layout> nl(l, garage_drive_layout_free);
+        if (!check_markers(ds)) return false;
+        std::swap(drives, ds);
+        std::swap(dlayout, nl);
+        if (!save_drives()) {
+            std::swap(drives, ds);
+            std::swap(dlayout, nl);
+            return false;
+        }
+        drive_gen++;
+        return true;
+    }
+    static std::string normal_path(const char *p)
+    {
+        std::string s = std::filesystem::path(p).lexically_normal().string();
+        while (s.size() > 1 && s.back() == '/') s.pop_back();
+        return s;
+    }
+    // the hashes with a file on a drive that is not the primary of their partition (duplicates possible)
+    void misplaced(std::vector<Hash> &out) const
+    {
+        for (size_t d = 0; d < drives.size(); d++) {
+            std::vector<Hash> hs;
+            drive_list(d, hs);
+            for (const Hash &h : hs)
+                if (drives_of(h)[0] != (int)d) out.push_back(h);
+        }
+    }
+    enum MoveResult { kMoveGone = 0, kMoved, kMoveStale, kMoveQuarantined, kMoveFailed };
+    // RebalanceWorker's move of file `ext` of h off drive d (not h's primary): read and checked (a shard by its header
+    // and tag; a replica is moved as it is, convert_step checks its content hash), written whole to the primary, then
+    // the old copy removed -- a file never changes drive by a rename.  A copy the primary already has is removed only.  A
+    // shard that fails is quarantined where it is.  allow() gates the write and the removal.  *bytes: the file's size.
+    MoveResult move_to_primary(const Hash &h, int d, const char *ext, const std::function<bool()> &allow, uint64_t *bytes)
+    {
+        const std::string from = dir_in(drives[d].root, h) + "/" + name_of(h, ext);
+        std::string buf;
+        if (!read_file(from, buf)) return kMoveGone;
+        *bytes = buf.size();
+        if (ext[0]) {
+            ShardFileHeader hd;
+            bool good = buf.size() >= sizeof(hd);
+            if (good) memcpy(&hd, buf.data(), sizeof(hd));
+            good = good && memcmp(hd.magic, "GEC1", 4) == 0 && hd.hdr_check == adler32_small(reinterpret_cast<const uint8_t *>(&hd), 48) &&
+                   (uint64_t)buf.size() == sizeof(hd) + (uint64_t)hd.shard_len;
+            Hash got;
+            good = good && garage_ec_shard_sum_host(hd.sum_kind, reinterpret_cast<const uint8_t *>(buf.data()) + sizeof(hd),
+                                                    hd.shard_len, got.data()) == GARAGE_EC_OK &&
+                   memcmp(got.data(), hd.sum, 32) == 0;
+            if (!good) return ::rename(from.c_str(), sibling(from, h, ".corrupted").c_str()) == 0 ? kMoveQuarantined : kMoveFailed;
+        }
+        const std::string to = primary_path(h, ext);
+        if (::access(to.c_str(), F_OK) == 0) return allow() && ::remove(from.c_str()) == 0 ? kMoveStale : kMoveFailed;
+        std::error_code ec;
+        std::filesystem::create_directories(dir_of(h), ec);
+        if (!allow() || !write_file_atomic(to, buf.data(), buf.size(), nullptr, 0, fsync_data, fsync_data)) return kMoveFailed;
+        return allow() && ::remove(from.c_str()) == 0 ? kMoved : kMoveFailed;
+    }
     // previous codes or replicas are configured (a file store changing its code)
     bool legacy_store() const { return codes.size() >= 2 || replicas; }
     // in-memory: the copy was made by the caller; the shard it replaces is returned, to be freed outside the lock
@@ -470,7 +731,7 @@ struct Node {
     {
         int n = 0;
         for (auto &f : other_index_files(h, keep))
-            if (allow() && ::remove(path_of(h, f.first).c_str()) == 0) n++;
+            if (allow() && remove_file(h, f.first)) n++;
         return n;
     }
     bool has_legacy_shard(const Hash &h) const
@@ -490,10 +751,10 @@ struct Node {
         int n = 0;
         if (codes.size() >= 2) {
             const std::string sh = path_of(h, ".shard"), lg = path_of(h, ".legacy");
-            if (file_code(sh) >= 1 && allow() && ::remove(sh.c_str()) == 0) n++;
-            if (file_code(lg) != -2 && allow() && ::remove(lg.c_str()) == 0) n++;
+            if (file_code(sh) >= 1 && allow() && remove_file(h, ".shard")) n++;
+            if (file_code(lg) != -2 && allow() && remove_file(h, ".legacy")) n++;
         }
-        if (has_replica(h) && allow() && ::remove(path_of(h, "").c_str()) == 0) n++;
+        if (has_replica(h) && allow() && remove_file(h, "")) n++;
         return n;
     }
     // a whole-block replica into dst (cap bytes); its length is the file size.  The caller checks the content hash.
@@ -531,9 +792,11 @@ struct Node {
         const int si = by_index ? file_index(sh) : -1;
         const bool other = si >= 0 && si != mt.index;  // .shard holds another index of h
         const bool aside = other ? mt.index == newest : codes.size() >= 2 && file_code(sh) >= 1;
-        if (aside && !(allow() && ::rename(sh.c_str(), path_of(h, ".legacy").c_str()) == 0 &&
-                       (!fsync_data || fsync_dir(dir_of(h)))))
+        const std::string lg = sibling(sh, h, ".legacy");
+        if (aside && !(allow() && ::rename(sh.c_str(), lg.c_str()) == 0 &&
+                       (!fsync_data || fsync_dir(lg.substr(0, lg.rfind('/'))))))
             return false;
+        if (aside) remove_copies(h, ".legacy", lg);
         if (!allow()) return false;
         std::error_code ec;
         std::filesystem::create_directories(dir_of(h), ec);
@@ -550,8 +813,11 @@ struct Node {
         hd.hdr_check = adler32_small(reinterpret_cast<const uint8_t *>(&hd), 48);
         hd.pad[0] = (uint8_t)codes[0].l;
         hd.pad[1] = codes[0].kind_byte();
-        return write_file_atomic(path_of(h, other && !aside ? ".legacy" : ".shard"), &hd, sizeof(hd), bytes, n, fsync_data,
-                                 fsync_data);
+        const char *ext = other && !aside ? ".legacy" : ".shard";
+        const std::string to = primary_path(h, ext);
+        if (!write_file_atomic(to, &hd, sizeof(hd), bytes, n, fsync_data, fsync_data)) return false;
+        remove_copies(h, ext, to);
+        return true;
     }
     // shard bytes straight into `dst` (cap bytes available), metadata into `mt`.  A span other than the whole shard
     // is one ranged read of its bytes only, into dst (which then holds the span's bytes); an empty span reads and checks
@@ -683,7 +949,7 @@ struct Node {
     bool store_erase(const Hash &h)
     {
         if (dir.empty()) return shards.erase(h) != 0;
-        return ::remove(path_of(h, ".shard").c_str()) == 0;
+        return remove_file(h, ".shard");
     }
     // move_block_to_corrupted (manager.rs:807-819): file >= 0 that ShardFile of h; code -1 the replica; index >= 0
     // (by_index stores) the file holding that index; otherwise the file holding the shard of `code`
@@ -701,7 +967,7 @@ struct Node {
         if (file >= 0 || code < 0) p = path_of(h, kExt[file >= 0 ? file : kReplicaFile]);
         else if (index >= 0 && by_index) p = path_at(h, index);
         if (p.empty()) p = codes.size() < 2 ? path_of(h, ".shard") : path_for(h, code);
-        if (!p.empty()) ::rename(p.c_str(), path_of(h, ".corrupted").c_str());
+        if (!p.empty()) ::rename(p.c_str(), sibling(p, h, ".corrupted").c_str());
     }
     // fault injection (garage_bm_corrupt_shard*): what = 0 flips a bit of the shard's bytes at byte_off, 1 rewrites the
     // stored block_len (+1), 2 rewrites the stored index (+1 mod k+m); the stored tag / header check are left alone in
@@ -749,23 +1015,63 @@ struct Node {
             for (auto &kv : shards) out.push_back(kv.first);
             return;
         }
-        std::error_code ec, ec2;
+        if (!drives.empty()) {
+            for (size_t d = 0; d < drives.size(); d++) drive_list(d, out);
+            std::sort(out.begin(), out.end());
+            out.erase(std::unique(out.begin(), out.end()), out.end());
+            return;
+        }
+        std::error_code ec;
         for (auto it = std::filesystem::recursive_directory_iterator(dir, ec);
              !ec && it != std::filesystem::recursive_directory_iterator(); it.increment(ec)) {
-            const std::string name = it->path().filename().string();
-            const bool listed = (name.size() == 64 + 6 && name.compare(64, 6, ".shard") == 0) ||
-                                ((codes.size() >= 2 || by_index) && name.size() == 64 + 7 && name.compare(64, 7, ".legacy") == 0) ||
-                                (replicas && name.size() == 64 && it->is_regular_file(ec2));
-            if (!listed) continue;
             Hash h;
-            bool ok = true;
-            for (int i = 0; i < 32 && ok; i++) {
-                auto v = [&](char c) { return c >= '0' && c <= '9' ? c - '0' : (c >= 'a' && c <= 'f' ? c - 'a' + 10 : -1); };
-                const int hi = v(name[2 * i]), lo = v(name[2 * i + 1]);
-                ok = hi >= 0 && lo >= 0;
-                h[i] = (uint8_t)((hi << 4) | lo);
+            if (listed_name(*it, h)) out.push_back(h);
+        }
+    }
+    // a file store_list lists: .shard, with previous codes or a layout file .legacy, with replicas configured the replica;
+    // its hash into h
+    bool listed_name(const std::filesystem::directory_entry &e, Hash &h) const
+    {
+        std::error_code ec;
+        const std::string name = e.path().filename().string();
+        const bool listed = (name.size() == 64 + 6 && name.compare(64, 6, ".shard") == 0) ||
+                            ((codes.size() >= 2 || by_index) && name.size() == 64 + 7 && name.compare(64, 7, ".legacy") == 0) ||
+                            (replicas && name.size() == 64 && e.is_regular_file(ec));
+        return listed && hex_to(name, 32, h.data());
+    }
+    static bool hex_to(const std::string &s, size_t n, uint8_t *out)
+    {
+        auto v = [&](char c) { return c >= '0' && c <= '9' ? c - '0' : (c >= 'a' && c <= 'f' ? c - 'a' + 10 : -1); };
+        if (s.size() < 2 * n) return false;
+        for (size_t i = 0; i < n; i++) {
+            const int hi = v(s[2 * i]), lo = v(s[2 * i + 1]);
+            if (hi < 0 || lo < 0) return false;
+            out[i] = (uint8_t)((hi << 4) | lo);
+        }
+        return true;
+    }
+    // the hashes with a listed file in drive d's <hh>/<hh>/ tree (duplicates possible)
+    void drive_list(size_t d, std::vector<Hash> &out) const
+    {
+        namespace fs = std::filesystem;
+        auto hex_dir = [](const fs::directory_entry &e) {
+            std::error_code ec;
+            const std::string n = e.path().filename().string();
+            uint8_t b;
+            return n.size() == 2 && hex_to(n, 1, &b) && e.is_directory(ec);
+        };
+        std::error_code ec;
+        for (const auto &a : fs::directory_iterator(drives[d].root, ec)) {
+            if (!hex_dir(a)) continue;
+            std::error_code ec2;
+            for (const auto &b : fs::directory_iterator(a.path(), ec2)) {
+                if (!hex_dir(b)) continue;
+                std::error_code ec3;
+                for (const auto &f : fs::directory_iterator(b.path(), ec3)) {
+                    Hash h;
+                    if (listed_name(f, h)) out.push_back(h);
+                }
             }
-            if (ok) out.push_back(h);
         }
     }
 };
@@ -1139,6 +1445,12 @@ struct garage_bm {
         layout_deleted{0}, layout_sync_errors{0}, layout_bytes_fetched{0};
     std::atomic<uint64_t> stripe_repairs{0}, stripe_repair_shards{0}, stripe_repair_bytes_read{0},
         stripe_repair_bytes_fetched{0}, stripe_repair_bytes_written{0}, stripe_repair_errors{0}, stripe_repair_call_us{0};
+    std::atomic<uint64_t> rebalance_files_moved{0}, rebalance_bytes_moved{0}, rebalance_errors{0}, drive_marker_errors{0};
+    // per node: the drive layout generation + 1 a rebalance pass started from cursor NULL under (0 = none), and
+    // whether that pass has left no misplaced file behind so far
+    std::mutex rebalance_mu;
+    std::vector<uint64_t> rebalance_gen;
+    std::vector<uint8_t> rebalance_clean;
 
     // Bytes a rebuild from the shards `have` hands to the GPU, which is what crosses the network in Garage: the runs
     // garage_ec_read_ranges names for a Clay stripe (1/m of each helper for a lone lost shard), else what was read
@@ -2804,6 +3116,104 @@ struct garage_bm {
     }
 
     // garage_bm_stripe_repair_step: see include/garage_block_manager.h and DESIGN.md section 5.6
+    // garage_bm_set_data_dirs (DESIGN.md section 5.7)
+    int set_data_dirs(int node, const garage_bm_data_dir *dirs, int n)
+    {
+        Node &nd = *nodes[node];
+        std::lock_guard<std::mutex> lk(nd.mu);
+        if (nd.dir.empty()) return GARAGE_EC_E_INVALID;
+        if (!nd.set_drives(dirs, n)) {
+            drive_marker_errors++;
+            nd.up = false;
+            return GARAGE_BM_E_MESSAGE;
+        }
+        nd.up = true;
+        return GARAGE_BM_OK;
+    }
+
+    // RebalanceWorker (repair.rs:531-626) over node's drives, in hash order
+    int rebalance_step(int node, const Hash *cursor, size_t max_files, Hash *cursor_out, int *finished, uint64_t *moved)
+    {
+        Node &nd = *nodes[node];
+        std::vector<Hash> hs;
+        uint64_t gen;
+        {
+            std::lock_guard<std::mutex> lk(nd.mu);
+            if (nd.drives.empty()) return GARAGE_EC_E_INVALID;
+            if (!nd.up) return GARAGE_BM_E_MESSAGE;
+            nd.misplaced(hs);
+            gen = nd.drive_gen;
+        }
+        int fin = 0;
+        sweep_page(hs, cursor, max_files, cursor_out, &fin);
+        if (finished) *finished = fin;
+        {
+            std::lock_guard<std::mutex> lk(rebalance_mu);
+            if (!cursor) {
+                rebalance_gen[node] = gen + 1;
+                rebalance_clean[node] = 1;
+            }
+        }
+        auto allow = [this] { return convert_op_allowed(); };
+        uint64_t n = 0;
+        bool clean = true;
+        std::vector<Hash> bad;
+        for (const Hash &h : hs) {
+            std::lock_guard<std::mutex> lk(nd.mu);
+            if (!nd.up || nd.drive_gen != gen) {
+                clean = false;
+                break;
+            }
+            const int prim = nd.drives_of(h)[0];
+            for (int d = 0; d < (int)nd.drives.size(); d++) {
+                if (d == prim) continue;
+                for (const char *ext : {".shard", ".legacy", ""}) {
+                    if (!ext[0] && !nd.replicas) continue;
+                    uint64_t b = 0;
+                    switch (nd.move_to_primary(h, d, ext, allow, &b)) {
+                    case Node::kMoved:
+                        n++;
+                        rebalance_files_moved++;
+                        rebalance_bytes_moved += b;
+                        break;
+                    case Node::kMoveQuarantined:
+                        corruption_counter++;
+                        bad.push_back(h);
+                        break;
+                    case Node::kMoveFailed:
+                        rebalance_errors++;
+                        clean = false;
+                        break;
+                    default:
+                        break;
+                    }
+                }
+            }
+        }
+        for (const Hash &h : bad) put_to_resync(node, h);
+        if (moved) *moved = n;
+        std::lock_guard<std::mutex> lk(rebalance_mu);
+        if (!clean) rebalance_clean[node] = 0;
+        if (!fin) return GARAGE_BM_OK;
+        const bool drop = rebalance_gen[node] == gen + 1 && rebalance_clean[node];
+        rebalance_gen[node] = 0;
+        if (!drop) return GARAGE_BM_OK;
+        // every file is in its primary now, and every write since went there: the secondaries can go
+        // (without_secondary_locations)
+        std::lock_guard<std::mutex> nl(nd.mu);
+        if (nd.drive_gen != gen) return GARAGE_BM_OK;
+        garage_drive_layout *l = nullptr;
+        if (garage_drive_layout_drop_secondaries(&l, nd.dlayout.get()) != GARAGE_LAYOUT_OK) return GARAGE_EC_E_NOMEM;
+        std::shared_ptr<garage_drive_layout> keep(l, garage_drive_layout_free);
+        std::swap(nd.dlayout, keep);
+        if (!nd.save_drives()) {
+            std::swap(nd.dlayout, keep);
+            return GARAGE_BM_E_MESSAGE;
+        }
+        nd.drive_gen++;
+        return GARAGE_BM_OK;
+    }
+
     int stripe_repair_step(int node, const Hash *cursor, size_t max_blocks, int min_missing, Hash *cursor_out,
                            int *finished, uint64_t *repaired, uint64_t *rebuilt)
     {
@@ -3255,6 +3665,28 @@ static bool code_ok(int k, int m, int l, int piggyback, int clay, int sum_kind)
     return !piggyback || (l == 0 && k <= 16 && m >= 2 && m <= 4 && sum_kind != GARAGE_EC_SUM_BLAKE2);
 }
 
+// a data_dir list garage_bm_create and garage_bm_set_data_dirs take: 1..GARAGE_BM_MAX_DATA_DIRS entries with relative
+// paths inside the node directory, distinct once normalised, capacity > 0 unless read-only, and at least one with
+// capacity (the drive layout's own rules)
+static bool drive_list_ok(const garage_bm_data_dir *d, int n)
+{
+    if (n < 1 || n > GARAGE_BM_MAX_DATA_DIRS || !d) return false;
+    std::vector<std::string> seen;
+    std::vector<uint64_t> cap(n);
+    for (int i = 0; i < n; i++) {
+        if (!d[i].path || !d[i].path[0] || d[i].path[0] == '/' || (d[i].read_only != 0 && d[i].read_only != 1)) return false;
+        if (!d[i].read_only && d[i].capacity == 0) return false;
+        const std::string p = Node::normal_path(d[i].path);
+        if (p == ".." || p.compare(0, 3, "../") == 0 || std::find(seen.begin(), seen.end(), p) != seen.end()) return false;
+        seen.push_back(p);
+        cap[i] = d[i].read_only ? 0 : d[i].capacity;
+    }
+    garage_drive_layout *l = nullptr;
+    const int rc = garage_drive_layout_init(&l, n, cap.data(), nullptr);
+    garage_drive_layout_free(l);
+    return rc == GARAGE_LAYOUT_OK;
+}
+
 // a context running code `c` (RS, LRC, PB or Clay) with shard tags of `sum_kind`
 static int create_ctx(const CodeDesc &c, int device, int sum_kind, garage_ec_ctx **out)
 {
@@ -3266,7 +3698,7 @@ static int create_ctx(const CodeDesc &c, int device, int sum_kind, garage_ec_ctx
     return rc;
 }
 
-static int bm_create(garage_bm **out, const garage_bm_config *cfg)
+static int bm_create(garage_bm **out, const garage_bm_config *cfg, const garage_bm_data_dir *data_dirs, int n_data_dirs)
 {
     *out = nullptr;
     const int k = cfg->data_shards, m = cfg->parity_shards, l = cfg->local_groups;
@@ -3294,6 +3726,9 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
                 return GARAGE_EC_E_INVALID;
         }
     }
+    // drives: a file store only, and a list the drive layout takes
+    if (n_data_dirs < 0 || (n_data_dirs > 0 && (!(cfg->data_dir && cfg->data_dir[0]) || !drive_list_ok(data_dirs, n_data_dirs))))
+        return GARAGE_EC_E_INVALID;
     // the layout history: <data_dir>/layout wins over cfg->layout; both are checked before any CUDA call
     auto lays = std::make_shared<garage_bm::Layouts>();
     std::vector<uint64_t> synced(cfg->n_nodes, 0);
@@ -3371,6 +3806,8 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
     bm->pass_version.assign(cfg->n_nodes, 0);
     bm->pass_clean.assign(cfg->n_nodes, 0);
     bm->cfg.layout = nullptr;  // not kept: the caller's spec may go away
+    bm->rebalance_gen.assign(cfg->n_nodes, 0);
+    bm->rebalance_clean.assign(cfg->n_nodes, 0);
     for (int i = 0; i < cfg->n_nodes; i++) {
         bm->nodes.emplace_back(new Node());
         Node &nd = *bm->nodes.back();
@@ -3383,6 +3820,29 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
             nd.replicas = bm->legacy_rf > 0;
             std::error_code ec;
             std::filesystem::create_directories(nd.dir, ec);
+            // drives: <node dir>/data_layout wins over the configured list, which seeds a node without one
+            const int lr = nd.load_drives();
+            if (lr < 0) {
+                garage_bm_destroy(bm.release());
+                return GARAGE_EC_E_INVALID;
+            }
+            bool markers_ok = true;
+            if (lr == 0 && n_data_dirs > 0) {
+                markers_ok = nd.set_drives(data_dirs, n_data_dirs);
+            } else if (lr > 0) {
+                std::vector<Node::Drive> ds = nd.drives;
+                markers_ok = Node::check_markers(ds);
+                bool recorded = false;
+                for (size_t d = 0; markers_ok && d < ds.size(); d++) recorded = recorded || ds[d].marker != nd.drives[d].marker;
+                if (recorded) {
+                    nd.drives = ds;
+                    markers_ok = nd.save_drives();
+                }
+            }
+            if (!markers_ok) {  // Garage refuses to start on an unmounted or swapped disk
+                nd.up = false;
+                bm->drive_marker_errors++;
+            }
             // restart: what is on disk is what exists (the block_ref table would say the same), shards of previous
             // codes and replicas included
             std::vector<Hash> have;
@@ -3465,7 +3925,14 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg)
 int garage_bm_create(garage_bm **out, const garage_bm_config *cfg)
 {
     if (!out || !cfg) return GARAGE_EC_E_INVALID;
-    BM_GUARD(bm_create(out, cfg));
+    BM_GUARD(bm_create(out, cfg, nullptr, 0));
+}
+
+int garage_bm_create_with_drives(garage_bm **out, const garage_bm_config *cfg, const garage_bm_data_dir *data_dirs,
+                                 int n_data_dirs)
+{
+    if (!out || !cfg) return GARAGE_EC_E_INVALID;
+    BM_GUARD(bm_create(out, cfg, data_dirs, n_data_dirs));
 }
 
 void garage_bm_destroy(garage_bm *bm)
@@ -3786,6 +4253,29 @@ void garage_bm_get_range_metrics(garage_bm *bm, garage_bm_range_metrics *o)
     o->range_degraded = bm->range_degraded;
     o->range_bytes_read = bm->range_bytes_read;
     o->range_bytes_fetched = bm->range_bytes_fetched;
+}
+
+int garage_bm_set_data_dirs(garage_bm *bm, int node, const garage_bm_data_dir *dirs, int n)
+{
+    if (!bm || node < 0 || node >= (int)bm->nodes.size() || !drive_list_ok(dirs, n)) return GARAGE_EC_E_INVALID;
+    BM_GUARD(bm->set_data_dirs(node, dirs, n));
+}
+
+int garage_bm_rebalance_step(garage_bm *bm, int node, const uint8_t *cursor32, size_t max_files, uint8_t cursor_out32[32],
+                             int *finished, uint64_t *moved)
+{
+    return bm_step(bm, node, cursor32, cursor_out32, [&](const Hash *cur, Hash *out) {
+        return bm->rebalance_step(node, cur, max_files, out, finished, moved);
+    });
+}
+
+void garage_bm_get_drive_metrics(garage_bm *bm, garage_bm_drive_metrics *o)
+{
+    if (!bm || !o) return;
+    o->rebalance_files_moved = bm->rebalance_files_moved;
+    o->rebalance_bytes_moved = bm->rebalance_bytes_moved;
+    o->rebalance_errors = bm->rebalance_errors;
+    o->drive_marker_errors = bm->drive_marker_errors;
 }
 
 void garage_bm_get_stripe_repair_metrics(garage_bm *bm, garage_bm_stripe_repair_metrics *o)

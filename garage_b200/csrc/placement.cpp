@@ -585,3 +585,241 @@ int garage_layout_read_plan(const garage_layout *const *active, int n_active, co
 }
 
 }  // extern "C"
+
+// ================================================================= drive layout (DESIGN.md section 5.7)
+struct garage_drive_layout {
+    std::vector<uint64_t> capacity;            // per directory: 0 = read-only
+    std::vector<uint8_t> prim;                 // GARAGE_DRIVE_NPART primaries
+    std::vector<std::vector<uint8_t>> sec;     // per partition: secondaries in read order
+};
+
+namespace {
+
+constexpr int DNP = GARAGE_DRIVE_NPART;
+
+bool drive_dirs_ok(int n_dirs, const uint64_t *capacity)
+{
+    if (n_dirs < 1 || n_dirs > GARAGE_DRIVE_MAX_DIRS || !capacity) return false;
+    for (int i = 0; i < n_dirs; i++)
+        if (capacity[i] > 0) return true;
+    return false;
+}
+
+// end of directory i's run of partitions: floor(cumulative capacity through i * NPART / total capacity).  The
+// product fits in 128 bits for any u64 capacities.
+std::vector<int> drive_run_ends(int n_dirs, const uint64_t *capacity)
+{
+    unsigned __int128 total = 0, cum = 0;
+    for (int i = 0; i < n_dirs; i++) total += capacity[i];
+    std::vector<int> end(n_dirs);
+    for (int i = 0; i < n_dirs; i++) {
+        cum += capacity[i];
+        end[i] = (int)(cum * DNP / total);
+    }
+    return end;
+}
+
+// every non-empty directory with only[i] set becomes a secondary of each partition it is not primary of, unless it is one
+// already
+void drive_add_non_empty(garage_drive_layout &l, const uint8_t *non_empty, const std::vector<uint8_t> &only)
+{
+    if (!non_empty) return;
+    for (int i = 0; i < (int)l.capacity.size(); i++) {
+        if (!non_empty[i] || !only[i]) continue;
+        for (int p = 0; p < DNP; p++)
+            if (l.prim[p] != i && std::find(l.sec[p].begin(), l.sec[p].end(), (uint8_t)i) == l.sec[p].end())
+                l.sec[p].push_back((uint8_t)i);
+    }
+}
+
+}  // namespace
+
+extern "C" {
+
+int garage_drive_partition_of(const uint8_t hash[32])
+{
+    if (!hash) return GARAGE_LAYOUT_E_INVALID;
+    return (int)((((unsigned)hash[2] << 8) | hash[3]) % DNP);
+}
+
+int garage_drive_layout_init(garage_drive_layout **out, int n_dirs, const uint64_t *capacity, const uint8_t *non_empty)
+{
+    if (!out) return GARAGE_LAYOUT_E_INVALID;
+    *out = nullptr;
+    if (!drive_dirs_ok(n_dirs, capacity)) return GARAGE_LAYOUT_E_INVALID;
+    try {
+        std::unique_ptr<garage_drive_layout> l(new garage_drive_layout());
+        l->capacity.assign(capacity, capacity + n_dirs);
+        l->prim.assign(DNP, 0);
+        l->sec.assign(DNP, {});
+        const std::vector<int> end = drive_run_ends(n_dirs, capacity);
+        for (int i = 0, p = 0; i < n_dirs; i++)  // a read-only directory's run is empty
+            for (; p < end[i]; p++) l->prim[p] = (uint8_t)i;
+        drive_add_non_empty(*l, non_empty, std::vector<uint8_t>(n_dirs, 1));
+        *out = l.release();
+        return GARAGE_LAYOUT_OK;
+    } catch (const std::bad_alloc &) {
+        return GARAGE_LAYOUT_E_NOMEM;
+    }
+}
+
+int garage_drive_layout_update(garage_drive_layout **out, const garage_drive_layout *prev, const int *prev_index,
+                               int n_dirs, const uint64_t *capacity, const uint8_t *non_empty)
+{
+    if (!out) return GARAGE_LAYOUT_E_INVALID;
+    *out = nullptr;
+    if (!prev || !prev_index || !drive_dirs_ok(n_dirs, capacity)) return GARAGE_LAYOUT_E_INVALID;
+    const int n_prev = (int)prev->capacity.size();
+    try {
+        std::vector<int> old2new(n_prev, -1);
+        for (int i = 0; i < n_dirs; i++) {
+            const int o = prev_index[i];
+            if (o < -1 || o >= n_prev || (o >= 0 && old2new[o] >= 0)) return GARAGE_LAYOUT_E_INVALID;
+            if (o >= 0) old2new[o] = i;
+        }
+        std::unique_ptr<garage_drive_layout> l(new garage_drive_layout());
+        bool same = n_dirs == n_prev;
+        for (int i = 0; same && i < n_dirs; i++) same = prev_index[i] == i && capacity[i] == prev->capacity[i];
+        if (same) {  // the same list: the same layout
+            *l = *prev;
+            *out = l.release();
+            return GARAGE_LAYOUT_OK;
+        }
+        l->capacity.assign(capacity, capacity + n_dirs);
+        l->prim.assign(DNP, 0);
+        l->sec.assign(DNP, {});
+        // secondaries carry over, removed directories dropped
+        for (int p = 0; p < DNP; p++)
+            for (uint8_t o : prev->sec[p])
+                if (old2new[o] >= 0) l->sec[p].push_back((uint8_t)old2new[o]);
+        // each surviving directory keeps its primaries (in partition order)
+        std::vector<std::vector<int>> dir_prim(n_dirs);
+        for (int p = 0; p < DNP; p++)
+            if (old2new[prev->prim[p]] >= 0) dir_prim[old2new[prev->prim[p]]].push_back(p);
+        // targets: differences of the floors of cumulative capacity
+        std::vector<int> target(n_dirs, 0);
+        const std::vector<int> end = drive_run_ends(n_dirs, capacity);
+        for (int i = 0; i < n_dirs; i++) target[i] = end[i] - (i ? end[i - 1] : 0);
+        // over target: give up the highest-numbered partitions, keeping them as a secondary
+        for (int i = 0; i < n_dirs; i++)
+            while ((int)dir_prim[i].size() > target[i]) {
+                const int p = dir_prim[i].back();
+                dir_prim[i].pop_back();
+                if (std::find(l->sec[p].begin(), l->sec[p].end(), (uint8_t)i) == l->sec[p].end())
+                    l->sec[p].push_back((uint8_t)i);
+            }
+        std::vector<int> owner(DNP, -1);
+        for (int i = 0; i < n_dirs; i++)
+            for (int p : dir_prim[i]) owner[p] = i;
+        std::vector<int> unassigned;
+        for (int p = 0; p < DNP; p++)
+            if (owner[p] < 0) unassigned.push_back(p);
+        // below target, in list order: take unassigned partitions, highest-numbered first
+        for (int i = 0; i < n_dirs; i++)
+            for (int need = target[i] - (int)dir_prim[i].size(); need > 0; need--) {
+                const int p = unassigned.back();
+                unassigned.pop_back();
+                owner[p] = i;
+                auto &s = l->sec[p];
+                s.erase(std::remove(s.begin(), s.end(), (uint8_t)i), s.end());
+            }
+        for (int p = 0; p < DNP; p++) l->prim[p] = (uint8_t)owner[p];
+        // newly listed non-empty directories become secondaries everywhere they are not primary
+        std::vector<uint8_t> fresh(n_dirs);
+        for (int i = 0; i < n_dirs; i++) fresh[i] = prev_index[i] < 0;
+        drive_add_non_empty(*l, non_empty, fresh);
+        *out = l.release();
+        return GARAGE_LAYOUT_OK;
+    } catch (const std::bad_alloc &) {
+        return GARAGE_LAYOUT_E_NOMEM;
+    }
+}
+
+int garage_drive_layout_drop_secondaries(garage_drive_layout **out, const garage_drive_layout *l)
+{
+    if (!out) return GARAGE_LAYOUT_E_INVALID;
+    *out = nullptr;
+    if (!l) return GARAGE_LAYOUT_E_INVALID;
+    try {
+        std::unique_ptr<garage_drive_layout> r(new garage_drive_layout(*l));
+        for (auto &s : r->sec) s.clear();
+        *out = r.release();
+        return GARAGE_LAYOUT_OK;
+    } catch (const std::bad_alloc &) {
+        return GARAGE_LAYOUT_E_NOMEM;
+    }
+}
+
+int garage_drive_layout_n_dirs(const garage_drive_layout *l) { return l ? (int)l->capacity.size() : GARAGE_LAYOUT_E_INVALID; }
+
+int garage_drive_layout_primary(const garage_drive_layout *l, int part)
+{
+    if (!l || part < 0 || part >= DNP) return GARAGE_LAYOUT_E_INVALID;
+    return l->prim[part];
+}
+
+int garage_drive_layout_secondaries(const garage_drive_layout *l, int part, uint8_t *out, int cap)
+{
+    if (!l || part < 0 || part >= DNP || cap < 0 || (cap > 0 && !out)) return GARAGE_LAYOUT_E_INVALID;
+    const auto &s = l->sec[part];
+    for (int i = 0; i < (int)s.size() && i < cap; i++) out[i] = s[i];
+    return (int)s.size();
+}
+
+// image: "GDL1", n_dirs, n_dirs little-endian u64 capacities, then per partition: primary, count, secondaries
+size_t garage_drive_layout_serialize(const garage_drive_layout *l, uint8_t *out, size_t cap)
+{
+    if (!l) return 0;
+    std::vector<uint8_t> b = {'G', 'D', 'L', '1', (uint8_t)l->capacity.size()};
+    for (uint64_t c : l->capacity)
+        for (int j = 0; j < 8; j++) b.push_back((uint8_t)(c >> (8 * j)));
+    for (int p = 0; p < DNP; p++) {
+        b.push_back(l->prim[p]);
+        b.push_back((uint8_t)l->sec[p].size());
+        b.insert(b.end(), l->sec[p].begin(), l->sec[p].end());
+    }
+    if (out && cap >= b.size()) memcpy(out, b.data(), b.size());
+    return b.size();
+}
+
+int garage_drive_layout_deserialize(garage_drive_layout **out, const uint8_t *buf, size_t len)
+{
+    if (!out) return GARAGE_LAYOUT_E_INVALID;
+    *out = nullptr;
+    if (!buf || len < 5 || memcmp(buf, "GDL1", 4) != 0) return GARAGE_LAYOUT_E_INVALID;
+    try {
+        std::unique_ptr<garage_drive_layout> l(new garage_drive_layout());
+        const int n = buf[4];
+        size_t at = 5;
+        if (len < at + (size_t)n * 8) return GARAGE_LAYOUT_E_INVALID;
+        l->capacity.assign(n, 0);
+        for (int i = 0; i < n; i++, at += 8)
+            for (int j = 0; j < 8; j++) l->capacity[i] |= (uint64_t)buf[at + j] << (8 * j);
+        if (!drive_dirs_ok(n, l->capacity.data())) return GARAGE_LAYOUT_E_INVALID;
+        l->prim.assign(DNP, 0);
+        l->sec.assign(DNP, {});
+        for (int p = 0; p < DNP; p++) {
+            if (at + 2 > len) return GARAGE_LAYOUT_E_INVALID;
+            const int pr = buf[at], ns = buf[at + 1];
+            at += 2;
+            if (pr >= n || l->capacity[pr] == 0 || ns >= n || at + ns > len) return GARAGE_LAYOUT_E_INVALID;
+            l->prim[p] = (uint8_t)pr;
+            for (int j = 0; j < ns; j++) {
+                const uint8_t d = buf[at + j];
+                auto &s = l->sec[p];
+                if (d >= n || d == pr || std::find(s.begin(), s.end(), d) != s.end()) return GARAGE_LAYOUT_E_INVALID;
+                s.push_back(d);
+            }
+            at += ns;
+        }
+        if (at != len) return GARAGE_LAYOUT_E_INVALID;
+        *out = l.release();
+        return GARAGE_LAYOUT_OK;
+    } catch (const std::bad_alloc &) {
+        return GARAGE_LAYOUT_E_NOMEM;
+    }
+}
+
+void garage_drive_layout_free(garage_drive_layout *l) { delete l; }
+
+}  // extern "C"

@@ -240,3 +240,121 @@ def read_plan(active, hash32, k, our_node=-1, ping_us=None, old=()):
     if n < 0:
         raise PlacementError(n, "garage_layout_read_plan")
     return [(out[i].node, out[i].index, out[i].version) for i in range(n)]
+
+
+# ---- drive layout (DESIGN.md section 5.7): a node's files over several data directories ----------
+DRIVE_NPART = 1024
+DRIVE_MAX_DIRS = 16
+DRIVE_SYMBOLS = [
+    "garage_drive_partition_of", "garage_drive_layout_init", "garage_drive_layout_update",
+    "garage_drive_layout_drop_secondaries", "garage_drive_layout_n_dirs", "garage_drive_layout_primary",
+    "garage_drive_layout_secondaries", "garage_drive_layout_serialize", "garage_drive_layout_deserialize",
+    "garage_drive_layout_free",
+]
+_drive_bound = False
+
+
+def _dlib():
+    global _drive_bound
+    L = _lib()
+    if not _drive_bound:
+        vp, i32 = C.c_void_p, C.c_int
+        L.garage_drive_partition_of.argtypes = [vp]
+        L.garage_drive_layout_init.argtypes = [C.POINTER(vp), i32, vp, vp]
+        L.garage_drive_layout_update.argtypes = [C.POINTER(vp), vp, vp, i32, vp, vp]
+        L.garage_drive_layout_drop_secondaries.argtypes = [C.POINTER(vp), vp]
+        L.garage_drive_layout_n_dirs.argtypes = [vp]
+        L.garage_drive_layout_primary.argtypes = [vp, i32]
+        L.garage_drive_layout_secondaries.argtypes = [vp, i32, vp, i32]
+        L.garage_drive_layout_serialize.argtypes = [vp, vp, C.c_size_t]
+        L.garage_drive_layout_serialize.restype = C.c_size_t
+        L.garage_drive_layout_deserialize.argtypes = [C.POINTER(vp), vp, C.c_size_t]
+        L.garage_drive_layout_free.argtypes = [vp]
+        L.garage_drive_layout_free.restype = None
+        _drive_bound = True
+    return L
+
+
+def drive_partition_of(hash32) -> int:
+    return _dlib().garage_drive_partition_of(_hash_ptr(hash32))
+
+
+class DriveLayout:
+    """a node's drive layout: per partition a primary directory and ordered secondary directories.  capacity 0 marks
+    a read-only directory; non_empty[i]: directory i holds a garage-marker or a hex-named subdirectory."""
+
+    def __init__(self, handle):
+        self._h = handle
+
+    @staticmethod
+    def _arrays(capacity, non_empty):
+        c = np.ascontiguousarray(capacity, dtype=np.uint64)
+        ne = np.ascontiguousarray(non_empty if non_empty is not None else np.zeros(c.size), dtype=np.uint8)
+        return c, ne
+
+    @classmethod
+    def init(cls, capacity, non_empty=None):
+        c, ne = cls._arrays(capacity, non_empty)
+        h = C.c_void_p()
+        rc = _dlib().garage_drive_layout_init(C.byref(h), c.size, c.ctypes.data, ne.ctypes.data)
+        if rc:
+            raise PlacementError(rc, "garage_drive_layout_init")
+        return cls(h)
+
+    def update(self, prev_index, capacity, non_empty=None):
+        c, ne = self._arrays(capacity, non_empty)
+        pi = np.ascontiguousarray(prev_index, dtype=np.int32)
+        assert pi.size == c.size
+        h = C.c_void_p()
+        rc = _dlib().garage_drive_layout_update(C.byref(h), self._h, pi.ctypes.data, c.size, c.ctypes.data, ne.ctypes.data)
+        if rc:
+            raise PlacementError(rc, "garage_drive_layout_update")
+        return DriveLayout(h)
+
+    def drop_secondaries(self):
+        h = C.c_void_p()
+        rc = _dlib().garage_drive_layout_drop_secondaries(C.byref(h), self._h)
+        if rc:
+            raise PlacementError(rc, "garage_drive_layout_drop_secondaries")
+        return DriveLayout(h)
+
+    @property
+    def n_dirs(self):
+        return _dlib().garage_drive_layout_n_dirs(self._h)
+
+    def primary(self, part):
+        return _dlib().garage_drive_layout_primary(self._h, part)
+
+    def secondaries(self, part):
+        out = (C.c_uint8 * DRIVE_MAX_DIRS)()
+        n = _dlib().garage_drive_layout_secondaries(self._h, part, out, DRIVE_MAX_DIRS)
+        return list(out[:n])
+
+    def primaries(self):
+        return [self.primary(p) for p in range(DRIVE_NPART)]
+
+    def all_secondaries(self):
+        return [self.secondaries(p) for p in range(DRIVE_NPART)]
+
+    def serialize(self) -> bytes:
+        n = _dlib().garage_drive_layout_serialize(self._h, None, 0)
+        buf = (C.c_uint8 * n)()
+        _dlib().garage_drive_layout_serialize(self._h, buf, n)
+        return bytes(buf)
+
+    @classmethod
+    def deserialize(cls, data: bytes):
+        b = (C.c_uint8 * max(1, len(data))).from_buffer_copy(data or b"\0")
+        h = C.c_void_p()
+        rc = _dlib().garage_drive_layout_deserialize(C.byref(h), b, len(data))
+        if rc:
+            raise PlacementError(rc, "garage_drive_layout_deserialize")
+        return cls(h)
+
+    def __del__(self):
+        try:
+            if self._h:
+                _dlib().garage_drive_layout_free(self._h)
+                self._h = None
+        except Exception:
+            pass

@@ -64,6 +64,16 @@ typedef struct {
 
 #define GARAGE_BM_MAX_LAYOUT_VERSIONS 4 /* active layout versions at once */
 
+/* One data directory of a node (Garage's data_dir = [{path, capacity}, {path, read_only}]; DESIGN.md section 5.7).
+ * path is relative to the node directory <data_dir>/node<N>; "." is the node directory itself.                      */
+typedef struct {
+    const char *path;
+    uint64_t capacity; /* > 0 unless read_only: the share of the node's partitions the drive is the primary of */
+    int read_only;     /* 1: read and rebalanced off, never written                                            */
+} garage_bm_data_dir;
+
+#define GARAGE_BM_MAX_DATA_DIRS 16
+
 typedef struct {
     int data_shards;                /* k  (config: erasure_coding.data_shards)   */
     int parity_shards;              /* m                                          */
@@ -187,9 +197,26 @@ typedef struct garage_bm_stripe_repair_metrics {
     uint64_t stripe_repair_errors;        /* unrecoverable stripes + shard writes that failed                   */
     uint64_t stripe_repair_call_us;       /* wall time inside garage_ec_reconstruct_stripes                     */
 } garage_bm_stripe_repair_metrics;
+/* Counters of the drives (DESIGN.md section 5.7), in a struct of their own for the same reason. */
+typedef struct garage_bm_drive_metrics {
+    uint64_t rebalance_files_moved; /* files garage_bm_rebalance_step wrote to their primary drive (old copy removed) */
+    uint64_t rebalance_bytes_moved; /* their bytes, file headers included                                            */
+    uint64_t rebalance_errors;      /* moves whose write or removal failed (the file stays readable where it was)   */
+    uint64_t drive_marker_errors;   /* marker checks that failed (at create or garage_bm_set_data_dirs)             */
+} garage_bm_drive_metrics;
 
 void garage_bm_default_config(garage_bm_config *cfg);
 int garage_bm_create(garage_bm **out, const garage_bm_config *cfg);
+/* garage_bm_create with several drives per node (file store; DESIGN.md section 5.7); garage_bm_config keeps the size
+ * older callers allocate, so the drive list comes here.  data_dirs NULL / n_data_dirs 0: garage_bm_create exactly,
+ * every file under the node directory.  Otherwise each node spreads its files over these directories by the drive
+ * layout (include/garage_placement.h), recorded in <data_dir>/node<N>/data_layout with a garage-marker file in every
+ * drive; on restart that file wins over this list, which only seeds nodes without one.  A node whose recorded marker
+ * is missing or different starts down.  GARAGE_EC_E_INVALID before any CUDA call for: drives on the memory store, a
+ * NULL list with entries, a negative count, more than GARAGE_BM_MAX_DATA_DIRS entries, a NULL, empty, absolute or
+ * repeated path or one outside the node directory, capacity 0 without read_only, or no drive with capacity.        */
+int garage_bm_create_with_drives(garage_bm **out, const garage_bm_config *cfg, const garage_bm_data_dir *data_dirs,
+                                 int n_data_dirs);
 void garage_bm_destroy(garage_bm *bm);
 
 /* util/data.rs:130-138 */
@@ -312,6 +339,24 @@ int garage_bm_layout_sync_step(garage_bm *bm, int node, const uint8_t *cursor32,
                                uint8_t cursor_out32[32], int *finished, uint64_t *moved);
 /* the active layout versions, oldest first; returns their number (at most cap are written)                       */
 int garage_bm_layout_versions(garage_bm *bm, uint64_t *out, int cap);
+
+/* Drives (file store; DESIGN.md section 5.7).  garage_bm_set_data_dirs: node `node` restarts with this data_dir list
+ * (the same rules as garage_bm_config.data_dirs): the drive layout is updated by path (initialised if the node has
+ * none), the markers checked and <node dir>/data_layout written.  GARAGE_EC_E_INVALID for a list create would
+ * reject; GARAGE_BM_E_MESSAGE if a drive fails its marker check, which leaves the node down and its layout as it was;
+ * on success the node is up.                                                                                      */
+int garage_bm_set_data_dirs(garage_bm *bm, int node, const garage_bm_data_dir *dirs, int n);
+/* RebalanceWorker (repair.rs:531-626), resumable in hash order like garage_bm_scrub_step: the hashes with a file on a
+ * drive other than their primary, after cursor32 (NULL = from the start), at most max_files of them (0 = all).  Each
+ * such .shard, .legacy or replica file is read and checked (shards by header and tag; a replica is moved as it is),
+ * written to the primary, then the old copy removed; a copy the primary already has is removed only.  A shard that
+ * fails is quarantined next to itself and queued for resync.  A full pass (cursor NULL to *finished) that left no
+ * misplaced file behind, with no drive change meanwhile, drops the secondaries and persists the layout.  Its writes
+ * and removals count as file operations for garage_bm_debug_convert_stop_after.  *moved = files moved.
+ * GARAGE_EC_E_INVALID for a node without drives, GARAGE_BM_E_MESSAGE if the node is down.                         */
+int garage_bm_rebalance_step(garage_bm *bm, int node, const uint8_t *cursor32, size_t max_files, uint8_t cursor_out32[32],
+                             int *finished, uint64_t *moved);
+void garage_bm_get_drive_metrics(garage_bm *bm, garage_bm_drive_metrics *out);
 
 /* native closed-loop load generator (row f1: the batching front-end decides real-world throughput):
  * `threads` client threads each PUT (mode 0) or GET (mode 1) `blocks_per_thread` blocks of `block_len`

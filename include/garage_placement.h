@@ -136,6 +136,34 @@ int garage_layout_read_plan(const garage_layout *const *active, int n_active, co
                             int n_old, const uint8_t hash[32], int k, int our_node, const uint32_t *ping_us,
                             garage_shard_source *out, int cap);
 
+/* ---- drive layout: a node's shards over several data directories (DESIGN.md section 5.7) ---------
+ * Garage's multi-drive data_dir: a hash's drive partition has one primary directory (writes go there)
+ * and an ordered list of secondary directories (reads look there after the primary).  Directory i is
+ * active with capacity[i] > 0, read-only with capacity[i] = 0; at least one is active.  non_empty[i]:
+ * the directory holds a garage-marker file or a hex-named subdirectory (NULL = none is).  Errors:
+ * GARAGE_LAYOUT_E_INVALID (= GARAGE_EC_E_INVALID) for no active directory, more than
+ * GARAGE_DRIVE_MAX_DIRS directories or a prev_index naming a previous directory twice or none. */
+#define GARAGE_DRIVE_NPART 1024
+#define GARAGE_DRIVE_MAX_DIRS 16
+typedef struct garage_drive_layout garage_drive_layout;
+/* the big-endian u16 of hash bytes 2 and 3, mod GARAGE_DRIVE_NPART                                 */
+int garage_drive_partition_of(const uint8_t hash[32]);
+int garage_drive_layout_init(garage_drive_layout **out, int n_dirs, const uint64_t *capacity, const uint8_t *non_empty);
+/* prev_index[i]: new directory i's index in prev (the same path), -1 for a directory prev did not list */
+int garage_drive_layout_update(garage_drive_layout **out, const garage_drive_layout *prev, const int *prev_index,
+                               int n_dirs, const uint64_t *capacity, const uint8_t *non_empty);
+/* the same primaries, no secondaries (a finished rebalance)                                         */
+int garage_drive_layout_drop_secondaries(garage_drive_layout **out, const garage_drive_layout *l);
+int garage_drive_layout_n_dirs(const garage_drive_layout *l);
+int garage_drive_layout_primary(const garage_drive_layout *l, int part);
+/* partition part's secondaries, in read order, into out (at most cap); returns their number          */
+int garage_drive_layout_secondaries(const garage_drive_layout *l, int part, uint8_t *out, int cap);
+/* a byte image of the layout (directories' capacities, primaries, secondaries): the bytes needed are
+ * returned and written if cap allows.  _deserialize checks an image and rebuilds the layout from it. */
+size_t garage_drive_layout_serialize(const garage_drive_layout *l, uint8_t *out, size_t cap);
+int garage_drive_layout_deserialize(garage_drive_layout **out, const uint8_t *buf, size_t len);
+void garage_drive_layout_free(garage_drive_layout *l);
+
 #ifdef __cplusplus
 }
 #endif
