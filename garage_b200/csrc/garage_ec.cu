@@ -662,12 +662,11 @@ void for_each_read_piece(const garage_ec_ctx *ctx, uint64_t halves, size_t i, si
     else if (b == 3) f((size_t)0, len);
     else f(b == 1 ? (size_t)0 : len / 2, len / 2);
 }
-// PB: every stripe's shard_len (NULL: stride) must be a multiple of 32 so that the halves are 16-byte aligned; Clay: a
-// multiple of 16*alpha, so that every layer's sub-chunk is
-bool pb_lens_ok(const garage_ec_ctx *ctx, const uint32_t *shard_len, size_t stride, size_t n)
+// Every stripe's shard_len (NULL: stride) must be at most the stride and, for PB, a multiple of 32 so that the halves
+// are 16-byte aligned; for Clay, a multiple of 16*alpha, so that every layer's sub-chunk is
+bool shard_lens_ok(const garage_ec_ctx *ctx, const uint32_t *shard_len, size_t stride, size_t n)
 {
-    if (!ctx->pb && !ctx->clay) return true;
-    const size_t unit = ctx->clay ? (size_t)ctx->quantum : 32;
+    const size_t unit = ctx->clay ? (size_t)ctx->quantum : ctx->pb ? 32 : 1;
     if (!shard_len) return stride % unit == 0;
     for (size_t s = 0; s < n; s++)
         if ((shard_len[s] % unit) || shard_len[s] > stride) return false;
@@ -1311,6 +1310,8 @@ static int encode_host(garage_ec_ctx *ctx, const uint8_t *data, uint8_t *parity,
 {
     const size_t k = ctx->k, m = ctx->m;
     HostPipeline p(ctx, n, k * stride);
+    // pageable parity rows are copied piece by piece, as in reconstruct_host
+    p.down.use_batch = device_addressable_host(parity);
     const size_t in_b = p.cs * k * stride, out_b = p.cs * m * stride;
     int rc = p.reserve(in_b + out_b, align_up(p.cs * 4, 16));
     if (rc) return rc;
@@ -1327,9 +1328,14 @@ static int encode_host(garage_ec_ctx *ctx, const uint8_t *data, uint8_t *parity,
         int r = run_uniform(ctx, kModeEncode, L.d_buf, k * stride, L.d_buf + in_b, m * stride,
                             nullptr, d_len, stride, ch.cnt, L.stream);
         if (r) return r;
-        CU_TRY(ctx, cudaMemcpyAsync(parity + ch.s0 * m * stride, L.d_buf + in_b, ch.cnt * m * stride,
-                                    cudaMemcpyDeviceToHost, L.stream));
-        return GARAGE_EC_OK;
+        // D2H: roundup16(shard_len) bytes of every parity row, never the caller's bytes past them (the lane buffer
+        // holds stale data there); rows of stripes with shard_len == stride merge into one copy
+        for (size_t s = ch.s0; s < ch.s0 + ch.cnt; s++) {
+            const size_t bytes = shard_len ? align_up(shard_len[s], 16) : stride;
+            for (size_t i = 0; i < m; i++)
+                p.down.add(parity + (s * m + i) * stride, L.d_buf + in_b + ((s - ch.s0) * m + i) * stride, bytes);
+        }
+        return p.down.flush(ctx, cudaMemcpyDeviceToHost, L.stream);
     });
     return rc ? rc : p.drain();
 }
@@ -1345,7 +1351,7 @@ int garage_ec_encode(garage_ec_ctx *ctx, const uint8_t *data, uint8_t *parity,
     if (n_stripes == 0) return GARAGE_EC_OK;
     if (!data || !parity) return GARAGE_EC_E_INVALID;
     if (!aligned16(data) || !aligned16(parity)) return GARAGE_EC_E_ALIGN;
-    if (mem_kind == GARAGE_EC_MEM_HOST && !pb_lens_ok(ctx, shard_len, stride, n_stripes)) return GARAGE_EC_E_INVALID;
+    if (mem_kind == GARAGE_EC_MEM_HOST && !shard_lens_ok(ctx, shard_len, stride, n_stripes)) return GARAGE_EC_E_INVALID;
     CU_TRY(ctx, cudaSetDevice(ctx->device));
     if (mem_kind == GARAGE_EC_MEM_HOST) return encode_host(ctx, data, parity, shard_len, stride, n_stripes);
     return run_uniform(ctx, kModeEncode, data, (size_t)ctx->k * stride, parity, (size_t)ctx->m * stride,
@@ -1394,7 +1400,7 @@ int garage_ec_verify(garage_ec_ctx *ctx, const uint8_t *shards, uint32_t *mismat
     if (n_stripes == 0) return GARAGE_EC_OK;
     if (!shards || !mismatch) return GARAGE_EC_E_INVALID;
     if (!aligned16(shards)) return GARAGE_EC_E_ALIGN;
-    if (mem_kind == GARAGE_EC_MEM_HOST && !pb_lens_ok(ctx, shard_len, stride, n_stripes)) return GARAGE_EC_E_INVALID;
+    if (mem_kind == GARAGE_EC_MEM_HOST && !shard_lens_ok(ctx, shard_len, stride, n_stripes)) return GARAGE_EC_E_INVALID;
     CU_TRY(ctx, cudaSetDevice(ctx->device));
     if (mem_kind == GARAGE_EC_MEM_HOST) return verify_host(ctx, shards, mismatch, shard_len, stride, n_stripes);
     cudaStream_t st = (cudaStream_t)cuda_stream;
@@ -1592,7 +1598,7 @@ int garage_ec_reconstruct(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *pr
     if (n_stripes == 0) return GARAGE_EC_OK;
     if (!shards || !present) return GARAGE_EC_E_INVALID;
     if (!aligned16(shards)) return GARAGE_EC_E_ALIGN;
-    if (mem_kind == GARAGE_EC_MEM_HOST && !pb_lens_ok(ctx, shard_len, stride, n_stripes)) return GARAGE_EC_E_INVALID;
+    if (mem_kind == GARAGE_EC_MEM_HOST && !shard_lens_ok(ctx, shard_len, stride, n_stripes)) return GARAGE_EC_E_INVALID;
     CU_TRY(ctx, cudaSetDevice(ctx->device));
     if (mem_kind == GARAGE_EC_MEM_HOST)
         return reconstruct_host(ctx, shards, nullptr, present, want, status, shard_len, stride, n_stripes);
@@ -1615,7 +1621,7 @@ int garage_ec_reconstruct_stripes(garage_ec_ctx *ctx, uint8_t *const *stripes, c
         if (!stripes[s]) return GARAGE_EC_E_INVALID;
         if (!aligned16(stripes[s])) return GARAGE_EC_E_ALIGN;
     }
-    if (!pb_lens_ok(ctx, shard_len, stride, n_stripes)) return GARAGE_EC_E_INVALID;
+    if (!shard_lens_ok(ctx, shard_len, stride, n_stripes)) return GARAGE_EC_E_INVALID;
     CU_TRY(ctx, cudaSetDevice(ctx->device));
     return reconstruct_host(ctx, nullptr, stripes, present, want, status, shard_len, stride, n_stripes);
 }
@@ -2239,7 +2245,7 @@ int garage_ec_scrub_repair(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *e
     if (!aligned16(shards)) return GARAGE_EC_E_ALIGN;
     const size_t tot = ctx->k + ctx->m;
     if (n_stripes * tot > 0xffffffffull) return GARAGE_EC_E_INVALID;
-    if (mem_kind == GARAGE_EC_MEM_HOST && !pb_lens_ok(ctx, shard_len, stride, n_stripes)) return GARAGE_EC_E_INVALID;
+    if (mem_kind == GARAGE_EC_MEM_HOST && !shard_lens_ok(ctx, shard_len, stride, n_stripes)) return GARAGE_EC_E_INVALID;
     CU_TRY(ctx, cudaSetDevice(ctx->device));
     if (mem_kind == GARAGE_EC_MEM_DEVICE) {
         cudaStream_t st = (cudaStream_t)cuda_stream;

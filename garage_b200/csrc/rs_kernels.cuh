@@ -322,7 +322,7 @@ struct ApplyParams {
     uint8_t *dst;                  // stripe s output base = dst + s*dst_pitch
     unsigned long long src_pitch;  // bytes
     unsigned long long dst_pitch;
-    const uint32_t *shard_len;  // device, nullable (=> stride)
+    const uint32_t *shard_len;  // device, nullable (=> stride); encode / verify: a length past the stride is malformed
     const StripePlan *plan;     // kModePlan
     uint32_t *mismatch;         // kModeVerify
     uint32_t *counter;          // dynamic scheduler, zero at launch: stripes (kModePlan) / work items (uniform modes)
@@ -829,11 +829,17 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
             uint32_t s, col, tail, rb;
             bool valid, any;  // this lane has a column / the warp has at least one
         };
+        // A stripe whose shard_len exceeds the stride is malformed: none of its chunks has columns (encode writes
+        // nothing of it) and verify sets every mismatch bit of this pass, once, from the stripe's first chunk.
         auto locate = [&](uint32_t item) -> Pos {
             Pos z;
             z.s = item / ips;
             const uint32_t c = item - z.s * ips;
-            const uint32_t len = p.shard_len ? __ldg(p.shard_len + z.s) : p.stride;
+            uint32_t len = p.shard_len ? __ldg(p.shard_len + z.s) : p.stride;
+            if (len > p.stride) {
+                if (MODE == kModeVerify && c == 0 && lane == 0) atomicOr(p.mismatch + z.s, ((1u << p.rows) - 1) << p.row_off);
+                len = 0;
+            }
             const uint32_t nvec = (len + 15) >> 4;
             z.col = c * 32 + lane;
             z.valid = z.col < nvec;
@@ -1440,8 +1446,8 @@ __global__ void __launch_bounds__(kPlanWarps * 32, 16) plan_kernel(const __grid_
 // copies each (+ m stored parity halves for verify): the b-phase copy flies while the a-rows are looked up, the next
 // item's a-phase copy while the b-rows are.  Every data vector is looked up once; the piggybacks are plain XORs of
 // the staged a-vectors of each group into the b-outputs.  HBM traffic is the RS(k, m) encode's, (k+m)*L per stripe.
-// shard_len must be a multiple of 32 (16-byte aligned halves): a malformed stripe gets every mismatch bit (verify)
-// or no write at all (encode).
+// shard_len must be a multiple of 32 (16-byte aligned halves) and at most the stride: a malformed stripe gets every
+// mismatch bit (verify) or no write at all (encode).
 template <int K, int MODE> struct PbCfg {
     static constexpr int kK = K;
     static constexpr TabLayout kLay = make_layout(K, 5, 2);  // RS(10,4): 8 + 2 tables, 64 KB
@@ -1487,7 +1493,7 @@ __global__ void __launch_bounds__(PbCfg<K, MODE>::kThreads, 1) pb_apply_kernel(c
         for (; it < total; it += step) {
             const uint32_t s = it / ips, c = it - s * ips;
             const uint32_t len = p.shard_len ? __ldg(p.shard_len + s) : p.stride;
-            if (len & 31) {
+            if ((len & 31) || len > p.stride) {
                 if (MODE == kModeVerify && c == 0 && lane == 0) atomicOr(p.mismatch + s, (1u << m) - 1);
                 continue;
             }

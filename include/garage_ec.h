@@ -161,7 +161,10 @@ size_t garage_ec_stride_for(uint32_t shard_len);         /* shard_len rounded up
  * right after DataBlock::from_buffer (manager.rs:376): the k data shards of each block go in,
  * the m parity shards come out; shard i is then sent to node i of the (k+m)-node set.
  *   data   : n * k * stride bytes, shard j of stripe s at (s*k + j) * stride
- *   parity : n * m * stride bytes, row  i of stripe s at (s*m + i) * stride                */
+ *   parity : n * m * stride bytes, row  i of stripe s at (s*m + i) * stride
+ * A stripe whose shard_len exceeds `stride` is malformed, for every code: a HOST call returns
+ * GARAGE_EC_E_INVALID before any GPU work; a DEVICE call writes nothing of that stripe's parity
+ * and encodes the other stripes.                                                            */
 int garage_ec_encode(garage_ec_ctx *ctx, const uint8_t *data, uint8_t *parity,
                      const uint32_t *shard_len, size_t stride, size_t n_stripes, int mem_kind,
                      void *cuda_stream);
@@ -195,7 +198,10 @@ int garage_ec_reconstruct_stripes(garage_ec_ctx *ctx, uint8_t *const *stripes, c
 /* ---- VERIFY (scrub) -- call sites: DataBlock::verify via BlockManager::read_block,
  * src/block/manager.rs:554-609 / src/block/block.rs:69-83, driven by ScrubWorker::work,
  * src/block/repair.rs:438-490: recompute parity from the k data shards and compare with
- * the stored parity.  mismatch[s] bit i set iff parity row i differs.                      */
+ * the stored parity.  mismatch[s] bit i set iff parity row i differs.  A stripe whose
+ * shard_len exceeds `stride` is malformed, for every code: a HOST call returns
+ * GARAGE_EC_E_INVALID before any GPU work; a DEVICE call sets its m low mismatch bits and
+ * reads nothing of it.                                                                      */
 int garage_ec_verify(garage_ec_ctx *ctx, const uint8_t *shards, uint32_t *mismatch,
                      const uint32_t *shard_len, size_t stride, size_t n_stripes, int mem_kind,
                      void *cuda_stream);
