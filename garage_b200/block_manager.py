@@ -22,6 +22,8 @@ SYMBOLS = [
     "garage_bm_layout_versions", "garage_bm_deep_scrub_step", "garage_bm_rpc_get_block_range",
     "garage_bm_get_range_metrics", "garage_bm_stripe_repair_step", "garage_bm_get_stripe_repair_metrics",
     "garage_bm_set_data_dirs", "garage_bm_rebalance_step", "garage_bm_get_drive_metrics", "garage_bm_create_with_drives",
+    "garage_bm_resync_step", "garage_bm_list_resync_errors", "garage_bm_resync_retry_now", "garage_bm_block_info",
+    "garage_bm_debug_set_clock_ms", "garage_bm_get_resync_metrics",
 ]
 SUM_BLAKE2, SUM_ADLER8 = 0, 1
 
@@ -100,6 +102,30 @@ class StripeRepairMetrics(C.Structure):
         "stripe_repair_bytes_written", "stripe_repair_errors", "stripe_repair_call_us")]
 
 
+class ResyncMetrics(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in (
+        "resync_error_entries", "resync_deferred", "resync_steps", "resync_retry_nows", "resync_failed_bytes_read")]
+
+
+class ResyncError(C.Structure):
+    """garage_bm_resync_error: one entry of a node's resync error table"""
+    _fields_ = [("node", C.c_int32), ("hash", C.c_uint8 * 32), ("rc", C.c_longlong), ("errors", C.c_uint64),
+                ("last_try_ms", C.c_uint64), ("next_try_ms", C.c_uint64), ("last_status", C.c_int32)]
+
+
+# garage_bm_block_status.state values
+SHARD_VALID, SHARD_ABSENT, SHARD_DOWN, SHARD_BAD_HEADER, SHARD_BAD_TAG, SHARD_QUARANTINED, SHARD_PREVIOUS = range(7)
+MAX_SHARDS = 40
+
+
+class BlockStatus(C.Structure):
+    """garage_bm_block_status: what garage_bm_block_info reports of one block"""
+    _fields_ = [("rc", C.c_longlong), ("code", Code), ("block_len", C.c_uint32), ("n_shards", C.c_int32),
+                ("node", C.c_int32 * MAX_SHARDS), ("state", C.c_int32 * MAX_SHARDS),
+                ("resync_errors", C.c_uint64 * MAX_SHARDS), ("recoverable", C.c_int32),
+                ("read_set", C.c_uint8 * MAX_SHARDS)]
+
+
 _lib = None
 
 
@@ -157,6 +183,14 @@ def load_library():
         L.garage_bm_rebalance_step.argtypes = [vp, i32, vp, sz, vp, C.POINTER(i32), C.POINTER(C.c_uint64)]
         L.garage_bm_get_drive_metrics.argtypes = [vp, C.POINTER(DriveMetrics)]
         L.garage_bm_get_drive_metrics.restype = None
+        u64p = C.POINTER(C.c_uint64)
+        L.garage_bm_resync_step.argtypes = [vp, i32, i32, sz, u64p, u64p, u64p, C.POINTER(C.c_int64)]
+        L.garage_bm_list_resync_errors.argtypes = [vp, i32, C.POINTER(ResyncError), sz, C.POINTER(sz)]
+        L.garage_bm_resync_retry_now.argtypes = [vp, i32, vp, u64p]
+        L.garage_bm_block_info.argtypes = [vp, vp, i32, C.POINTER(BlockStatus)]
+        L.garage_bm_debug_set_clock_ms.argtypes = [vp, C.c_uint64]
+        L.garage_bm_get_resync_metrics.argtypes = [vp, C.POINTER(ResyncMetrics)]
+        L.garage_bm_get_resync_metrics.restype = None
         _lib = L
     return _lib
 
@@ -277,6 +311,50 @@ class BlockManager:
         done = C.c_uint64(0)
         failed = self._L.garage_bm_resync_all(self._h, node, workers, C.byref(done))
         return failed, done.value
+
+    def resync_step(self, node, workers=8, max_blocks=0):
+        """one ResyncWorker pass over node's due entries -> (rc, resynced, failed, deferred, wait_ms)"""
+        a, b, c, w = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0), C.c_int64(0)
+        rc = self._L.garage_bm_resync_step(self._h, node, workers, max_blocks, C.byref(a), C.byref(b), C.byref(c),
+                                           C.byref(w))
+        return rc, a.value, b.value, c.value, w.value
+
+    def list_resync_errors(self, node=-1):
+        """-> (rc, [dict of node, hash, rc, errors, last_try_ms, next_try_ms, last_status]) in node then hash order"""
+        n = C.c_size_t(0)
+        rc = self._L.garage_bm_list_resync_errors(self._h, node, None, 0, C.byref(n))  # the size query
+        if rc != OK:
+            return rc, []
+        arr = (ResyncError * max(1, n.value))()
+        rc = self._L.garage_bm_list_resync_errors(self._h, node, arr, len(arr), C.byref(n))
+        out = [{"node": e.node, "hash": bytes(e.hash), "rc": e.rc, "errors": e.errors, "last_try_ms": e.last_try_ms,
+                "next_try_ms": e.next_try_ms, "last_status": e.last_status} for e in arr[:min(n.value, len(arr))]]
+        return rc, out
+
+    def resync_retry_now(self, node, hash32=None):
+        """clear_backoff of hash32 (None: every error entry of node) -> (rc, entries made due)"""
+        n = C.c_uint64(0)
+        rc = self._L.garage_bm_resync_retry_now(self._h, node, self._hp(hash32) if hash32 is not None else None,
+                                                C.byref(n))
+        return rc, n.value
+
+    def block_info(self, hash32, check_tags=False):
+        """-> (rc, dict of rc, code, block_len, node, state, resync_errors (per index), recoverable, read_set)"""
+        st = BlockStatus()
+        rc = self._L.garage_bm_block_info(self._h, self._hp(hash32), 1 if check_tags else 0, C.byref(st))
+        n = st.n_shards
+        return rc, {"rc": st.rc, "code": (st.code.k, st.code.m, st.code.local_groups, st.code.piggyback, st.code.clay),
+                    "block_len": st.block_len, "node": list(st.node[:n]), "state": list(st.state[:n]),
+                    "resync_errors": list(st.resync_errors[:n]), "recoverable": bool(st.recoverable),
+                    "read_set": list(st.read_set[:n])}
+
+    def debug_set_clock_ms(self, now_ms):
+        return self._L.garage_bm_debug_set_clock_ms(self._h, now_ms)
+
+    def resync_metrics(self):
+        mt = ResyncMetrics()
+        self._L.garage_bm_get_resync_metrics(self._h, C.byref(mt))
+        return {n: getattr(mt, n) for n, _ in ResyncMetrics._fields_}
 
     def repair_enqueue_missing(self, node):
         n = C.c_uint64(0)

@@ -23,6 +23,7 @@
 #include <condition_variable>
 #include <cctype>
 #include <cerrno>
+#include <climits>
 #include <cstddef>
 #include <cstdio>
 #include <cstring>
@@ -34,11 +35,11 @@
 #include <mutex>
 #include <new>
 #include <random>
+#include <set>
 #include <string>
 #include <type_traits>
 #include <thread>
 #include <unordered_map>
-#include <unordered_set>
 #include <vector>
 
 #include <fcntl.h>
@@ -383,8 +384,109 @@ struct Node {
     using ShardPtr = std::shared_ptr<const StoredShard>;
     std::unordered_map<Hash, ShardPtr, HashHasher> shards;
     std::unordered_map<Hash, ShardPtr, HashHasher> corrupted;  // the ".corrupted" quarantine
-    std::deque<Hash> resync_queue;                                // block_local_resync_queue (resync.rs:90)
-    std::unordered_set<Hash, HashHasher> queued;
+    // block_local_resync_queue (resync.rs:90, put_to_resync_at :241-256): one entry per hash with the time it falls
+    // due (ms on the manager's clock), iterated in (due, hash) order
+    std::unordered_map<Hash, int64_t, HashHasher> resync_due;
+    std::set<std::pair<int64_t, Hash>> resync_queue;
+    // the hash queued at `when`, or at its current due time if that is earlier
+    void schedule(const Hash &h, int64_t when)
+    {
+        auto it = resync_due.find(h);
+        if (it != resync_due.end()) {
+            if (it->second <= when) return;
+            resync_queue.erase({it->second, h});
+            it->second = when;
+        } else {
+            resync_due.emplace(h, when);
+        }
+        resync_queue.emplace(when, h);
+    }
+    // resync.errors (resync.rs:605-655 ErrorCounter), plus the status of the last failure
+    struct ResyncError {
+        uint64_t errors = 0;
+        uint64_t last_try = 0;  // ms on the manager's clock
+        int32_t status = 0;
+        // RESYNC_RETRY_DELAY << min(errors - 1, RESYNC_RETRY_DELAY_MAX_BACKOFF_POWER): 1 minute up to 64 minutes
+        uint64_t delay_ms() const { return 60000ull << std::min<uint64_t>(errors - 1, 6); }
+        uint64_t next_try() const { return last_try + delay_ms(); }
+    };
+    std::unordered_map<Hash, ResyncError, HashHasher> resync_errors;
+    // <dir>/resync holds the queue and the error table once a scheduled step or a retry-now ran on this node (or the
+    // file was there at start); resync_file_mu orders its writes
+    bool resync_persist = false;
+    std::mutex resync_file_mu;
+    std::mutex resync_step_mu;  // one garage_bm_resync_step of this node at a time
+    std::string resync_path() const { return dir + "/resync"; }
+    // the file's text: format version, the queue in (due, hash) order, the error table in hash order, an Adler-32 of all
+    // of that.  mu held.
+    std::string resync_image() const
+    {
+        std::string s = "garage-bm-resync 1\n";
+        for (const auto &q : resync_queue) s += "queue " + std::to_string(q.first) + " " + hex_of(q.second.data(), 32) + "\n";
+        std::vector<std::pair<Hash, ResyncError>> errs(resync_errors.begin(), resync_errors.end());
+        std::sort(errs.begin(), errs.end(), [](const auto &a, const auto &b) { return a.first < b.first; });
+        for (const auto &e : errs)
+            s += "error " + hex_of(e.first.data(), 32) + " " + std::to_string(e.second.errors) + " " +
+                 std::to_string(e.second.last_try) + " " + std::to_string(e.second.status) + "\n";
+        s += "check " + std::to_string(adler32_small(reinterpret_cast<const uint8_t *>(s.data()), s.size())) + "\n";
+        return s;
+    }
+    // the queue and error table of <dir>/resync merged in (mu held): true if the file was there and read.  A file that
+    // fails its check or format is ignored; garage_bm_repair_enqueue_missing finds the missing shards again.
+    bool load_resync()
+    {
+        std::string s;
+        if (dir.empty() || !read_file(resync_path(), s)) return false;
+        const size_t c = s.rfind("check ");
+        if (c == std::string::npos || (c > 0 && s[c - 1] != '\n')) return false;
+        if (std::to_string(adler32_small(reinterpret_cast<const uint8_t *>(s.data()), c)) + "\n" != s.substr(c + 6)) return false;
+        std::vector<std::string> tok;
+        for (size_t i = 0; i < c;) {
+            while (i < c && isspace((unsigned char)s[i])) i++;
+            const size_t j = i;
+            while (i < c && !isspace((unsigned char)s[i])) i++;
+            if (i > j) tok.push_back(s.substr(j, i - j));
+        }
+        auto num = [](const std::string &t, long long lo, long long &out) {
+            char *e = nullptr;
+            errno = 0;
+            out = strtoll(t.c_str(), &e, 10);
+            return !errno && !*e && !t.empty() && out >= lo;
+        };
+        auto unum = [](const std::string &t, unsigned long long &out) {
+            char *e = nullptr;
+            errno = 0;
+            out = strtoull(t.c_str(), &e, 10);
+            return !errno && !*e && !t.empty() && t[0] != '-';
+        };
+        size_t t = 0;
+        if (tok.size() < 2 || tok[t++] != "garage-bm-resync" || tok[t++] != "1") return false;
+        std::vector<std::pair<int64_t, Hash>> q;
+        std::vector<std::pair<Hash, ResyncError>> errs;
+        while (t < tok.size()) {
+            Hash h;
+            long long a = 0, st = 0;
+            unsigned long long b = 0;
+            if (tok[t] == "queue" && t + 3 <= tok.size() && num(tok[t + 1], LLONG_MIN, a) && tok[t + 2].size() == 64 &&
+                hex_to(tok[t + 2], 32, h.data())) {
+                q.emplace_back(a, h);
+                t += 3;
+            } else if (tok[t] == "error" && t + 5 <= tok.size() && tok[t + 1].size() == 64 && hex_to(tok[t + 1], 32, h.data()) &&
+                       num(tok[t + 2], 1, a) && unum(tok[t + 3], b) && num(tok[t + 4], INT32_MIN, st) && st <= INT32_MAX) {
+                ResyncError e;
+                e.errors = (uint64_t)a;
+                e.last_try = (uint64_t)b;
+                e.status = (int32_t)st;
+                errs.emplace_back(h, e);
+                t += 5;
+            } else {
+                return false;
+            }
+        }
+        for (const auto &x : q) schedule(x.second, x.first);
+        for (const auto &e : errs) resync_errors[e.first] = e.second;
+        return true;
+    }
 
     // Node is the only owner of the file scheme: the names below, the header and the placement rules of DESIGN.md
     // sections 5.1 / 5.2 / 5.7.  The files of one hash, by ShardFile:
@@ -946,6 +1048,59 @@ struct Node {
         const ShardPtr sp = store_find(h);
         return sp && sp->index == index && meta_valid(*sp);
     }
+    // garage_bm_block_info's look at this node's shard `index` of h (mu held, the node up): a GARAGE_BM_SHARD_* state
+    // from the file header alone; nothing is quarantined or queued.  expect: the block's known length (0 = unknown).
+    // Valid: the header names the configured code, this index and consistent lengths; its block length goes to
+    // *block_len, and what tag_state reads goes to *tag_file (file store) or *tag_shard (memory store).
+    int shard_state(const Hash &h, int index, uint32_t expect, uint32_t *block_len, std::string *tag_file,
+                    ShardPtr *tag_shard) const
+    {
+        auto judge = [&](const ShardMeta &mt) {
+            if (mt.index != index || (expect && mt.block_len != expect) || !meta_valid(mt)) return GARAGE_BM_SHARD_BAD_HEADER;
+            *block_len = mt.block_len;
+            return GARAGE_BM_SHARD_VALID;
+        };
+        if (dir.empty()) {
+            const ShardPtr sp = store_find(h);
+            if (!sp) return corrupted.count(h) ? GARAGE_BM_SHARD_QUARANTINED : GARAGE_BM_SHARD_ABSENT;
+            if (sp->bytes.size() != sp->shard_len) return GARAGE_BM_SHARD_BAD_HEADER;
+            *tag_shard = sp;
+            return judge(*sp);
+        }
+        std::string p = by_index ? path_at(h, index) : path_for(h, 0);
+        if (p.empty() && file_code(path_of(h, ".shard")) == -1) p = path_of(h, ".shard");  // a damaged or unknown header
+        ShardMeta mt;
+        const ReadResult r = p.empty() ? kReadMissing : file_read_into(p, 0, nullptr, 0, mt, ShardSpan::bytes(0, 0));
+        if (r == kReadInvalid) return GARAGE_BM_SHARD_BAD_HEADER;
+        if (r == kReadOk) {
+            *tag_file = p;
+            return judge(mt);
+        }
+        std::error_code ec;
+        if (std::filesystem::exists(path_of(h, ".corrupted"), ec)) return GARAGE_BM_SHARD_QUARANTINED;
+        return has_legacy_shard(h) || has_replica(h) ? GARAGE_BM_SHARD_PREVIOUS : GARAGE_BM_SHARD_ABSENT;
+    }
+    // The tag check of a shard shard_state found valid, without the node lock: the whole file (or the immutable
+    // in-memory shard) read into `buf` (room for a shard) and its tag computed.  A file replaced meanwhile is judged as
+    // it is read then.
+    int tag_state(int index, uint32_t expect, const std::string &file, const ShardPtr &sp, std::vector<uint8_t> &buf) const
+    {
+        ShardMeta mt;
+        const uint8_t *bytes = nullptr;
+        if (sp) {
+            mt = *sp;
+            bytes = sp->bytes.data();
+        } else {
+            const ReadResult r = file_read_into(file, 0, buf.data(), buf.size(), mt);
+            if (r == kReadMissing) return GARAGE_BM_SHARD_ABSENT;
+            if (r == kReadInvalid || mt.index != index || (expect && mt.block_len != expect)) return GARAGE_BM_SHARD_BAD_HEADER;
+            bytes = buf.data();
+        }
+        Hash got;
+        if (garage_ec_shard_sum_host(mt.sum_kind, bytes, mt.shard_len, got.data()) != GARAGE_EC_OK || got != mt.sum)
+            return GARAGE_BM_SHARD_BAD_TAG;
+        return GARAGE_BM_SHARD_VALID;
+    }
     bool store_erase(const Hash &h)
     {
         if (dir.empty()) return shards.erase(h) != 0;
@@ -1437,6 +1592,7 @@ struct garage_bm {
         resync_error_counter{0}, resync_recv_counter{0}, delete_counter{0}, put_calls{0}, reconstruct_calls{0},
         scrub_checked{0}, scrub_corrupt{0}, enc_gpu_us{0}, rec_gpu_us{0}, corrupt_data_errors{0}, write_errors{0},
         resync_shards_read{0}, resync_bytes_read{0}, resync_bytes_fetched{0};
+    std::atomic<uint64_t> resync_deferred{0}, resync_steps{0}, resync_retry_nows{0}, resync_failed_bytes_read{0};
     std::atomic<uint64_t> put_ns_slot{0}, put_ns_land{0}, put_ns_wait{0}, put_ns_store{0};
     std::atomic<uint64_t> convert_blocks{0}, convert_bytes_read{0}, convert_bytes_written{0}, convert_errors{0},
         convert_call_us{0}, legacy_gets{0}, legacy_deleted{0}, range_gets{0}, range_degraded{0}, range_bytes_read{0},
@@ -1544,11 +1700,19 @@ struct garage_bm {
         return -1;
     }
 
-    void put_to_resync(int node, const Hash &h)  // manager.rs:592-605 / resync.rs:put_to_resync
+    void put_to_resync(int node, const Hash &h)  // manager.rs:592-605 / resync.rs:put_to_resync: due at once
     {
         Node &nd = *nodes[node];
         std::lock_guard<std::mutex> lk(nd.mu);
-        if (nd.queued.insert(h).second) nd.resync_queue.push_back(h);
+        nd.schedule(h, now_ms());
+    }
+    // now_msec() of the scheduled queue and the error table: ms since the epoch, or garage_bm_debug_set_clock_ms's time
+    std::atomic<int64_t> debug_clock_ms{0};
+    int64_t now_ms() const
+    {
+        const int64_t t = debug_clock_ms.load();
+        if (t) return t;
+        return std::chrono::duration_cast<std::chrono::milliseconds>(std::chrono::system_clock::now().time_since_epoch()).count();
     }
 
     void shard_tag(const uint8_t *bytes, size_t n, Hash &out) const
@@ -2307,8 +2471,19 @@ struct garage_bm {
         return Clock::now() - it->second.zero_since >= std::chrono::milliseconds(cfg.block_gc_delay_ms);
     }
 
-    int resync_block(int node, const Hash &h)
+    // refs_mu held: ms until h, at rc 0, leaves its GC delay (at least 1)
+    int64_t gc_delay_left_ms(const Hash &h)
     {
+        const auto it = rc.find(h);
+        const auto left = std::chrono::milliseconds(cfg.block_gc_delay_ms) - (Clock::now() - it->second.zero_since);
+        return std::max<int64_t>(1, std::chrono::ceil<std::chrono::milliseconds>(left).count());
+    }
+
+    // gc_wait_ms: a block still inside its GC delay is not queued again; *gc_wait_ms = the ms until it leaves it (0 if
+    // it is not such a block)
+    int resync_block(int node, const Hash &h, int64_t *gc_wait_ms = nullptr)
+    {
+        if (gc_wait_ms) *gc_wait_ms = 0;
         const auto ls = layouts();
         const bool multi = ls->v.size() > 1;
         const int idx = newest_index(h, node);
@@ -2329,7 +2504,8 @@ struct garage_bm {
             const bool held = multi && !nd.other_index_files(h, -1).empty();
             if ((exists || held) && unneeded) {  // offload branch, resync.rs:369-458: delete_if_unneeded
                 if (!deletable_now(h)) {  // still inside the GC delay: look again later
-                    if (nd.queued.insert(h).second) nd.resync_queue.push_back(h);
+                    if (gc_wait_ms) *gc_wait_ms = gc_delay_left_ms(h);
+                    else nd.schedule(h, now_ms());
                     return GARAGE_BM_OK;
                 }
                 delete_counter += multi ? nd.erase_other_indices(h, -1, [] { return true; }) : nd.store_erase(h);
@@ -2367,11 +2543,13 @@ struct garage_bm {
                 return GARAGE_BM_OK;
             }
             resync_error_counter++;
+            resync_failed_bytes_read += nbytes;
             return GARAGE_BM_E_MISSING_BLOCK;  // resync.rs:488-494
         }
         int rc2 = reconstruct_in_slot(slot.p, block_len, have, want);
         if (rc2 != GARAGE_BM_OK) {
             resync_error_counter++;
+            resync_failed_bytes_read += nbytes;
             return rc2;
         }
         resync_recv_counter++;
@@ -2381,6 +2559,7 @@ struct garage_bm {
         shard_tag(bytes, L, sum);
         if (!write_shard(node, h, idx, block_len, bytes, L, sum.data())) {  // resync.rs:499
             resync_error_counter++;
+            resync_failed_bytes_read += nbytes;
             return GARAGE_BM_E_MESSAGE;  // Error::Io: stays queued, the caller backs off (resync.rs:300-315)
         }
         if (multi) {
@@ -3346,9 +3525,9 @@ struct garage_bm {
         std::vector<Hash> todo;
         {
             std::lock_guard<std::mutex> lk(nd.mu);
-            todo.assign(nd.resync_queue.begin(), nd.resync_queue.end());
+            for (const auto &q : nd.resync_queue) todo.push_back(q.second);
             nd.resync_queue.clear();
-            nd.queued.clear();
+            nd.resync_due.clear();
         }
         std::atomic<size_t> next{0};
         std::atomic<uint64_t> ok{0};
@@ -3370,6 +3549,8 @@ struct garage_bm {
                     }
                     if (r == GARAGE_BM_OK) {
                         ok++;
+                        std::lock_guard<std::mutex> lk(nd.mu);
+                        nd.resync_errors.erase(todo[i]);  // an error entry never outlives a success
                     } else {
                         std::lock_guard<std::mutex> lk(failed_mu);
                         failed.push_back(todo[i]);
@@ -3380,6 +3561,207 @@ struct garage_bm {
         for (const Hash &h : failed) put_to_resync(node, h);  // stays queued (backoff is the caller's)
         if (resynced) *resynced = ok.load();
         return (int)failed.size();
+    }
+
+    // ---- scheduled resync (DESIGN.md section 5.8) ---------------------------------------------
+    // garage_bm_block_info: see include/garage_block_manager.h
+    int block_info(const Hash &h, bool check_tags, garage_bm_block_status *o)
+    {
+        memset(o, 0, sizeof(*o));
+        o->rc = get_block_rc(h);
+        o->code = garage_bm_code{k, m, codes[0].l, codes[0].pb ? 1 : 0, codes[0].clay ? 1 : 0};
+        o->n_shards = tot;
+        uint32_t expect = 0;
+        {
+            std::lock_guard<std::mutex> lk(refs_mu);
+            auto it = refs.find(h);
+            if (it != refs.end()) expect = it->second;
+        }
+        int who[64];
+        storage_nodes_of(h, who);
+        std::vector<uint8_t> buf(check_tags ? slot_stride : 0);
+        uint8_t present[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
+        bool all = true;
+        for (int i = 0; i < tot; i++) {
+            Node &nd = *nodes[who[i]];
+            o->node[i] = who[i];
+            uint32_t len = 0;
+            std::string file;
+            Node::ShardPtr sp;
+            {
+                std::lock_guard<std::mutex> lk(nd.mu);  // headers only: the node's writes wait for no shard read
+                o->state[i] = nd.up ? nd.shard_state(h, i, expect, &len, &file, &sp) : GARAGE_BM_SHARD_DOWN;
+                auto e = nd.resync_errors.find(h);
+                o->resync_errors[i] = e == nd.resync_errors.end() ? 0 : e->second.errors;
+            }
+            if (check_tags && o->state[i] == GARAGE_BM_SHARD_VALID) o->state[i] = nd.tag_state(i, expect, file, sp, buf);
+            present[i] = o->state[i] == GARAGE_BM_SHARD_VALID;
+            all = all && present[i];
+            if (present[i] && !o->block_len) o->block_len = len;
+        }
+        // what a rebuild of every shard that is not valid would read: the code's own planner decides recoverability
+        uint8_t rd[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
+        o->recoverable = all || garage_ec_read_set(codes[0].ctx, present, nullptr, rd) == GARAGE_EC_OK;
+        if (!all && o->recoverable) memcpy(o->read_set, rd, tot);
+        return GARAGE_BM_OK;
+    }
+
+    // <node dir>/resync rewritten from the node's queue and error table (file store, once the node persists them)
+    bool save_resync(int node)
+    {
+        Node &nd = *nodes[node];
+        if (nd.dir.empty()) return true;
+        std::lock_guard<std::mutex> fl(nd.resync_file_mu);
+        std::string img;
+        {
+            std::lock_guard<std::mutex> lk(nd.mu);
+            if (!nd.resync_persist) return true;
+            img = nd.resync_image();
+        }
+        return write_file_atomic(nd.resync_path(), img.data(), img.size(), nullptr, 0, nd.fsync_data, nd.fsync_data);
+    }
+
+    // ResyncWorker's iterations (resync.rs:258-336) over the entries of node's queue due now
+    int resync_step(int node, int workers, size_t max_blocks, uint64_t *resynced, uint64_t *failed, uint64_t *deferred,
+                    int64_t *wait_ms)
+    {
+        Node &nd = *nodes[node];
+        std::lock_guard<std::mutex> sl(nd.resync_step_mu);
+        const int64_t now = now_ms();
+        std::vector<Hash> todo;
+        bool first;
+        {
+            std::lock_guard<std::mutex> lk(nd.mu);
+            if (!nd.up) return GARAGE_BM_E_MESSAGE;
+            first = !nd.resync_persist;
+            nd.resync_persist = true;
+            for (auto it = nd.resync_queue.begin(); it != nd.resync_queue.end() && it->first <= now;) {
+                if (max_blocks && todo.size() >= max_blocks) break;
+                todo.push_back(it->second);
+                nd.resync_due.erase(it->second);
+                it = nd.resync_queue.erase(it);
+            }
+        }
+        std::atomic<size_t> next{0};
+        std::atomic<uint64_t> n_ok{0}, n_failed{0}, n_deferred{0};
+        auto run = [&] {
+            garage_ec_bind_thread(ec);
+            for (size_t i; (i = next++) < todo.size();) {
+                const Hash &h = todo[i];
+                {
+                    std::lock_guard<std::mutex> lk(nd.mu);
+                    auto e = nd.resync_errors.find(h);
+                    if (e != nd.resync_errors.end() && (uint64_t)now < e->second.next_try()) {  // backing off
+                        nd.schedule(h, (int64_t)e->second.next_try());
+                        n_deferred++;
+                        continue;
+                    }
+                }
+                int64_t gc_wait = 0;
+                int r;
+                try {
+                    r = resync_block(node, h, &gc_wait);
+                } catch (...) {
+                    r = GARAGE_EC_E_NOMEM;
+                }
+                std::lock_guard<std::mutex> lk(nd.mu);
+                if (r == GARAGE_BM_OK && gc_wait > 0) {  // inside its GC delay: due when it becomes deletable
+                    nd.schedule(h, now + gc_wait);
+                    n_deferred++;
+                } else if (r == GARAGE_BM_OK) {
+                    nd.resync_errors.erase(h);
+                    n_ok++;
+                } else {
+                    // Garage stamps last_try = now + 1 so that its re-queue key differs from the entry it removes; this
+                    // queue replaces the entry in place, so last_try is the time of the try
+                    Node::ResyncError &e = nd.resync_errors[h];
+                    e.errors++;
+                    e.last_try = (uint64_t)now;
+                    e.status = r;
+                    nd.schedule(h, (int64_t)e.next_try());
+                    n_failed++;
+                }
+            }
+        };
+        // every worker is a thread of its own: garage_ec_bind_thread narrows the affinity of the thread it runs on, and
+        // the caller's thread keeps its own
+        const int nth = (int)std::min<size_t>((size_t)workers, todo.size());
+        std::vector<std::thread> th;
+        for (int w = 0; w < nth; w++) th.emplace_back(run);
+        for (auto &t : th) t.join();
+        int64_t wait;
+        {
+            std::lock_guard<std::mutex> lk(nd.mu);
+            // IdleFor: until the next entry falls due; 10 s with an empty queue (resync.rs:326-334)
+            wait = nd.resync_queue.empty() ? 10000 : std::max<int64_t>(0, nd.resync_queue.begin()->first - now);
+        }
+        resync_steps++;
+        resync_deferred += n_deferred;
+        if (resynced) *resynced = n_ok;
+        if (failed) *failed = n_failed;
+        if (deferred) *deferred = n_deferred;
+        if (wait_ms) *wait_ms = wait;
+        // a step that took nothing changed nothing the file does not already hold: entries queued since are due now,
+        // and the next step that takes them writes
+        if (todo.empty() && !first) return GARAGE_BM_OK;
+        return save_resync(node) ? GARAGE_BM_OK : GARAGE_BM_E_MESSAGE;
+    }
+
+    // list_resync_errors (manager.rs:429-449) of node (-1: every node), in node then hash order
+    int list_resync_errors(int node, garage_bm_resync_error *out, size_t cap, size_t *n)
+    {
+        std::vector<garage_bm_resync_error> all;
+        for (int x = node < 0 ? 0 : node; x < (node < 0 ? (int)nodes.size() : node + 1); x++) {
+            Node &nd = *nodes[x];
+            std::vector<std::pair<Hash, Node::ResyncError>> errs;
+            {
+                std::lock_guard<std::mutex> lk(nd.mu);
+                errs.assign(nd.resync_errors.begin(), nd.resync_errors.end());
+            }
+            std::sort(errs.begin(), errs.end(), [](const auto &a, const auto &b) { return a.first < b.first; });
+            for (const auto &e : errs) {
+                garage_bm_resync_error r;
+                memset(&r, 0, sizeof(r));
+                r.node = x;
+                memcpy(r.hash, e.first.data(), 32);
+                r.rc = get_block_rc(e.first);
+                r.errors = e.second.errors;
+                r.last_try_ms = e.second.last_try;
+                r.next_try_ms = e.second.next_try();
+                r.last_status = e.second.status;
+                all.push_back(r);
+            }
+        }
+        *n = all.size();
+        if (out && cap) memcpy(out, all.data(), std::min(cap, all.size()) * sizeof(all[0]));
+        return GARAGE_BM_OK;
+    }
+
+    // clear_backoff (resync.rs:119-134): h (NULL: every errored hash of node) due now, its error count kept
+    int resync_retry_now(int node, const Hash *h, uint64_t *n)
+    {
+        Node &nd = *nodes[node];
+        const int64_t now = now_ms();
+        uint64_t c = 0;
+        {
+            std::lock_guard<std::mutex> lk(nd.mu);
+            auto clear = [&](const Hash &x, Node::ResyncError &e) {
+                e.last_try = (uint64_t)now - e.delay_ms();
+                nd.schedule(x, now);
+                c++;
+            };
+            if (h) {
+                auto it = nd.resync_errors.find(*h);
+                if (it == nd.resync_errors.end() || it->second.errors == 0) return GARAGE_BM_E_MESSAGE;  // not errored
+                clear(*h, it->second);
+            } else {
+                for (auto &e : nd.resync_errors) clear(e.first, e.second);
+            }
+            nd.resync_persist = true;
+        }
+        resync_retry_nows += c;
+        if (n) *n = c;
+        return save_resync(node) ? GARAGE_BM_OK : GARAGE_BM_E_MESSAGE;
     }
 
     int repair_enqueue_missing(int node, uint64_t *enq)
@@ -3845,6 +4227,7 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg, const garage_
             }
             // restart: what is on disk is what exists (the block_ref table would say the same), shards of previous
             // codes and replicas included
+            nd.resync_persist = nd.load_resync();  // the scheduled queue and error table of an earlier run
             std::vector<Hash> have;
             nd.store_list(have);
             std::vector<uint8_t> tmp(bm->slot_stride);
@@ -3938,6 +4321,12 @@ int garage_bm_create_with_drives(garage_bm **out, const garage_bm_config *cfg, c
 void garage_bm_destroy(garage_bm *bm)
 {
     if (!bm) return;
+    for (int i = 0; i < (int)bm->nodes.size(); i++) {  // the scheduled queues of the nodes that keep them
+        try {
+            bm->save_resync(i);
+        } catch (...) {
+        }
+    }
     bm->enc_batcher.reset();
     bm->rec_batcher.reset();
     garage_ec_ctx *ec = bm->ec;
@@ -4019,6 +4408,56 @@ int garage_bm_repair_enqueue_missing(garage_bm *bm, int node, uint64_t *enqueued
 {
     if (!bm || node < 0 || node >= (int)bm->nodes.size()) return GARAGE_EC_E_INVALID;
     BM_GUARD(bm->repair_enqueue_missing(node, enqueued));
+}
+
+int garage_bm_resync_step(garage_bm *bm, int node, int workers, size_t max_blocks, uint64_t *resynced, uint64_t *failed,
+                          uint64_t *deferred, int64_t *wait_ms)
+{
+    if (!bm || node < 0 || node >= (int)bm->nodes.size() || workers < 1 || workers > 8) return GARAGE_EC_E_INVALID;
+    BM_GUARD(bm->resync_step(node, workers, max_blocks, resynced, failed, deferred, wait_ms));
+}
+
+int garage_bm_list_resync_errors(garage_bm *bm, int node, garage_bm_resync_error *out, size_t cap, size_t *n)
+{
+    if (!bm || node < -1 || node >= (int)bm->nodes.size() || !n || (!out && cap)) return GARAGE_EC_E_INVALID;
+    BM_GUARD(bm->list_resync_errors(node, out, cap, n));
+}
+
+int garage_bm_resync_retry_now(garage_bm *bm, int node, const uint8_t *hash32, uint64_t *n)
+{
+    if (!bm || node < 0 || node >= (int)bm->nodes.size()) return GARAGE_EC_E_INVALID;
+    BM_GUARD(([&] {
+        const Hash h = hash32 ? to_hash(hash32) : Hash{};
+        return bm->resync_retry_now(node, hash32 ? &h : nullptr, n);
+    }()));
+}
+
+int garage_bm_block_info(garage_bm *bm, const uint8_t hash[32], int check_tags, garage_bm_block_status *out)
+{
+    if (!bm || !hash || !out) return GARAGE_EC_E_INVALID;
+    BM_GUARD(bm->block_info(to_hash(hash), check_tags != 0, out));
+}
+
+int garage_bm_debug_set_clock_ms(garage_bm *bm, uint64_t now_ms)
+{
+    if (!bm || now_ms > (uint64_t)INT64_MAX) return GARAGE_EC_E_INVALID;
+    bm->debug_clock_ms.store((int64_t)now_ms);
+    return GARAGE_BM_OK;
+}
+
+void garage_bm_get_resync_metrics(garage_bm *bm, garage_bm_resync_metrics *o)
+{
+    if (!bm || !o) return;
+    uint64_t entries = 0;
+    for (auto &n : bm->nodes) {
+        std::lock_guard<std::mutex> lk(n->mu);
+        entries += n->resync_errors.size();
+    }
+    o->resync_error_entries = entries;
+    o->resync_deferred = bm->resync_deferred;
+    o->resync_steps = bm->resync_steps;
+    o->resync_retry_nows = bm->resync_retry_nows;
+    o->resync_failed_bytes_read = bm->resync_failed_bytes_read;
 }
 
 int garage_bm_scrub(garage_bm *bm, int node, uint64_t *checked, uint64_t *corrupt)

@@ -19,6 +19,8 @@
  *   ScrubWorker             src/block/repair.rs:438-490    (sweep of one node's shards)
  *   write_block             src/block/manager.rs:517-530, 720-805 (local durable store)
  *   block_incref/decref     src/block/manager.rs:452-500, get_block_rc :421-449 (src/block/rc.rs)
+ *   ResyncWorker / backoff  src/block/resync.rs:119-134, 241-336, 605-655 (scheduled queue, ErrorCounter,
+ *                           clear_backoff), list_resync_errors manager.rs:429-449
  *   batching front-end      (row f1) concurrent PUT / resync calls coalesced into GPU batches,
  *                           back-pressure like buffer_kb_semaphore (manager.rs:156,380-385)
  */
@@ -205,6 +207,49 @@ typedef struct garage_bm_drive_metrics {
     uint64_t drive_marker_errors;   /* marker checks that failed (at create or garage_bm_set_data_dirs)             */
 } garage_bm_drive_metrics;
 
+/* Counters of the scheduled resync (DESIGN.md section 5.8), in a struct of their own for the same reason. */
+typedef struct garage_bm_resync_metrics {
+    uint64_t resync_error_entries;     /* (node, hash) entries of the error table, all nodes                        */
+    uint64_t resync_deferred;          /* entries garage_bm_resync_step queued again without a try: backoff, GC delay */
+    uint64_t resync_steps;             /* garage_bm_resync_step calls that ran                                      */
+    uint64_t resync_retry_nows;        /* entries garage_bm_resync_retry_now made due                               */
+    uint64_t resync_failed_bytes_read; /* bytes read by resyncs that failed (part of resync_bytes_read)             */
+} garage_bm_resync_metrics;
+
+/* One entry of a node's resync error table (Garage's BlockResyncErrorInfo, manager.rs:429-449).                    */
+typedef struct garage_bm_resync_error {
+    int32_t node;
+    uint8_t hash[32];
+    long long rc;          /* garage_bm_get_block_rc                                                            */
+    uint64_t errors;       /* failed tries since the last success                                               */
+    uint64_t last_try_ms;  /* time of the last failed try (or as set by retry-now)                              */
+    uint64_t next_try_ms;  /* last_try_ms + 60 000 << min(errors - 1, 6): 1 minute up to 64 minutes             */
+    int32_t last_status;   /* what the last failed try returned (GARAGE_BM_E_* / GARAGE_EC_E_*)                 */
+} garage_bm_resync_error;
+
+/* The state of one index of a block's stripe in garage_bm_block_info */
+#define GARAGE_BM_SHARD_VALID 0       /* header checks out (and, with check_tags, the shard tag)                     */
+#define GARAGE_BM_SHARD_ABSENT 1      /* no file of this index                                                        */
+#define GARAGE_BM_SHARD_DOWN 2        /* the holder is down                                                           */
+#define GARAGE_BM_SHARD_BAD_HEADER 3  /* damaged header, or one naming another code, index or block length           */
+#define GARAGE_BM_SHARD_BAD_TAG 4     /* header fine, bytes fail the tag (only with check_tags)                       */
+#define GARAGE_BM_SHARD_QUARANTINED 5 /* no shard, a quarantined .corrupted file                                      */
+#define GARAGE_BM_SHARD_PREVIOUS 6    /* no shard of the configured code, a previous code's shard or a replica        */
+#define GARAGE_BM_MAX_SHARDS 40       /* GARAGE_EC_MAX_K + GARAGE_EC_MAX_M                                            */
+
+typedef struct garage_bm_block_status {
+    long long rc;                                /* garage_bm_get_block_rc                                            */
+    garage_bm_code code;                         /* the configured code                                               */
+    uint32_t block_len;                          /* from a valid shard's header; 0 if there is none                   */
+    int32_t n_shards;                            /* k + m: the entries below that are set                             */
+    int32_t node[GARAGE_BM_MAX_SHARDS];          /* holder of index i in the newest layout version                    */
+    int32_t state[GARAGE_BM_MAX_SHARDS];         /* GARAGE_BM_SHARD_*                                                 */
+    uint64_t resync_errors[GARAGE_BM_MAX_SHARDS];/* that holder's resync error count for the block                    */
+    int32_t recoverable;                         /* every index that is not valid can be rebuilt from the valid ones  */
+    uint8_t read_set[GARAGE_BM_MAX_SHARDS];      /* recoverable with some index not valid: the indices that rebuild
+                                                    reads (garage_ec_read_set); all 0 otherwise                        */
+} garage_bm_block_status;
+
 void garage_bm_default_config(garage_bm_config *cfg);
 int garage_bm_create(garage_bm **out, const garage_bm_config *cfg);
 /* garage_bm_create with several drives per node (file store; DESIGN.md section 5.7); garage_bm_config keeps the size
@@ -255,10 +300,50 @@ long long garage_bm_get_block_rc(garage_bm *bm, const uint8_t hash[32]);
 int garage_bm_resync_block(garage_bm *bm, int node, const uint8_t hash[32]);
 /* drain node's resync queue with `workers` concurrent workers (resync.rs:43: up to 8);
  * returns the number of blocks that could not be resynced (they stay queued, with backoff
- * semantics left to the caller).                                                                */
+ * semantics left to the caller; garage_bm_resync_step below applies Garage's).                  */
 int garage_bm_resync_all(garage_bm *bm, int node, int workers, uint64_t *resynced);
 /* RepairWorker (repair.rs:35-155): enqueue every hash this node should hold but does not.        */
 int garage_bm_repair_enqueue_missing(garage_bm *bm, int node, uint64_t *enqueued);
+
+/* Scheduled resync (DESIGN.md section 5.8).  Each node's resync queue holds one entry per hash with the time it falls
+ * due; everything queued by the calls above is due at once, and garage_bm_resync_all still drains the whole queue
+ * (its successes also clear their error entries).  Times are ms since the epoch, or garage_bm_debug_set_clock_ms's.
+ *
+ * garage_bm_resync_step is one pass of Garage's ResyncWorker (resync.rs:258-336) over node's queue: the entries due
+ * now, in (due time, hash) order, at most max_blocks of them (0 = all), run by `workers` threads (1..8):
+ *   - an entry whose error entry's next_try_ms is later than now is queued again at next_try_ms, read nothing
+ *     (*deferred);
+ *   - a block still inside block_gc_delay_ms is queued again at the time it becomes deletable (*deferred);
+ *   - a failed resync_block adds one to the entry's errors, sets last_try_ms = now and queues it at next_try_ms
+ *     (*failed); a success removes the error entry (*resynced).
+ * *wait_ms = ms until the queue's first entry falls due (0 if one is due), 10 000 for an empty queue (IdleFor).
+ * File store: from the first step or retry-now on, the node's queue and error table are kept in <data_dir>/node<N>/resync
+ * (written at the end of each step that took an entry, on retry-now and at destroy; tmp file, fsync and rename under
+ * data_fsync) and
+ * loaded at create; a node that never ran either writes no file.  GARAGE_EC_E_INVALID for a bad node or workers
+ * outside 1..8; GARAGE_BM_E_MESSAGE if the node is down or the file cannot be written.  Output pointers may be NULL.
+ * Steps of different nodes may run together and with PUTs and resync_all; a node's own steps run one at a time.
+ * The workers are threads of the step's own; the calling thread's CPU affinity is left as it was.                  */
+int garage_bm_resync_step(garage_bm *bm, int node, int workers, size_t max_blocks, uint64_t *resynced, uint64_t *failed,
+                          uint64_t *deferred, int64_t *wait_ms);
+/* garage block list-errors: the error entries of `node` (-1: every node) in node then hash order.  *n = their number
+ * and at most cap of them are written to out, so *n > cap means the list was cut (out NULL, cap 0: a size query).
+ * GARAGE_EC_E_INVALID only for a bad node, n NULL, or out NULL with cap > 0.                                       */
+int garage_bm_list_resync_errors(garage_bm *bm, int node, garage_bm_resync_error *out, size_t cap, size_t *n);
+/* garage block retry-now (clear_backoff, resync.rs:119-134): the entry of hash (NULL: every error entry of node) keeps
+ * its error count, gets last_try_ms = now - its delay and is due now.  GARAGE_BM_E_MESSAGE for a hash without an
+ * error entry on node.  *n (nullable) = entries made due.                                                         */
+int garage_bm_resync_retry_now(garage_bm *bm, int node, const uint8_t *hash32, uint64_t *n);
+/* garage block info under erasure coding: for each index of the block's row in the newest layout version, its holder
+ * and GARAGE_BM_SHARD_* state, and that holder's resync error count; whether the stripe can be rebuilt, decided by
+ * garage_ec_read_set over the valid indices, and the read set of that rebuild.  Read-only: nothing is quarantined,
+ * queued or written.  check_tags = 0: "valid" means the header checks out; 1: every shard is read and its tag
+ * checked, outside the holder's lock (only the header look holds it).  GARAGE_EC_E_INVALID for NULL hash or out.  */
+int garage_bm_block_info(garage_bm *bm, const uint8_t hash[32], int check_tags, garage_bm_block_status *out);
+/* Test clock of the scheduled queue and the error table (not of block_gc_delay_ms): now_ms > 0 is "now", 0 the real
+ * clock.  Set it before anything is queued: entries queued earlier carry real-clock due times.                  */
+int garage_bm_debug_set_clock_ms(garage_bm *bm, uint64_t now_ms);
+void garage_bm_get_resync_metrics(garage_bm *bm, garage_bm_resync_metrics *out);
 
 /* ScrubWorker sweep over all shards stored on `node` (repair.rs:438-490): GPU blake2sum of each
  * shard; a mismatch quarantines the shard (.corrupted, manager.rs:807-819) and queues a resync
