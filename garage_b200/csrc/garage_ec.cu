@@ -608,23 +608,25 @@ int run_reconstruct(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *present,
     return GARAGE_EC_OK;
 }
 
-// The half-shards plan_kernel reads for one stripe (present / want: k+m bytes, want nullable = every absent
-// shard): bit 2i / 2i+1 of *halves = a- / b-half of shard i, both for every shard read by RS and LRC.  False if a
-// wanted shard cannot be rebuilt.  HOST paths upload only these.
-bool stripe_read_plan(const garage_ec_ctx *ctx, const uint8_t *present, const uint8_t *want, uint64_t *halves)
+// The rows plan_kernel reads for one stripe (present / want: k+m bytes, want nullable = every absent shard): for PB
+// bit 2i / 2i+1 of *rows = a- / b-half of shard i, for RS, LRC and Clay bit i = shard i (up to 40 shards: two bits
+// each do not fit in 64).  read_halves gives the halves of shard i either way.  False if a wanted shard cannot be
+// rebuilt.  HOST paths upload only these.
+bool stripe_read_plan(const garage_ec_ctx *ctx, const uint8_t *present, const uint8_t *want, uint64_t *rows)
 {
     uint64_t pm = 0, wm = 0;
     for (int i = 0; i < ctx->k + ctx->m; i++) {
         pm |= (uint64_t)(present[i] != 0) << i;
         wm |= (uint64_t)(!want || want[i] != 0) << i;
     }
-    uint64_t rows = 0;
-    const bool ok = ctx->clay ? clay_read_set(ctx->k, ctx->m, pm, wm, &rows)
-                              : h_read_plan(PlanCode{ctx->k, ctx->m, ctx->l, ctx->pb, ctx->P}, pm, wm, &rows);
-    *halves = rows;
-    if (!ctx->pb)  // RS and LRC rows are shards
-        for (*halves = 0; rows; rows &= rows - 1) *halves |= 3ull << (2 * ctz64(rows));
-    return ok;
+    *rows = 0;
+    return ctx->clay ? clay_read_set(ctx->k, ctx->m, pm, wm, rows)
+                     : h_read_plan(PlanCode{ctx->k, ctx->m, ctx->l, ctx->pb, ctx->P}, pm, wm, rows);
+}
+// bit 0 / 1: the a- / b-half of shard i is read (3 for every shard RS, LRC and Clay read)
+unsigned read_halves(const garage_ec_ctx *ctx, uint64_t rows, size_t i)
+{
+    return ctx->pb ? (unsigned)(rows >> (2 * i)) & 3u : ((rows >> i) & 1) ? 3u : 0u;
 }
 bool stripe_read_set(const garage_ec_ctx *ctx, const uint8_t *present, const uint8_t *want, uint64_t *read)
 {
@@ -632,22 +634,22 @@ bool stripe_read_set(const garage_ec_ctx *ctx, const uint8_t *present, const uin
     const bool ok = stripe_read_plan(ctx, present, want, &hv);
     *read = 0;
     for (int i = 0; i < ctx->k + ctx->m; i++)
-        if ((hv >> (2 * i)) & 3) *read |= 1ull << i;
+        if (read_halves(ctx, hv, i)) *read |= 1ull << i;
     return ok;
 }
 // The pieces of shard i a HOST upload copies, as f(offset, bytes): `whole` bytes from 0 for a shard of the read set,
 // (PB) each planned half of shard_len/2 bytes, or (Clay repair: every shard but one is read) the runs of the repair
 // layers {z : z_y0 = x0} of the one absent shard f = (x0, y0), q^y0 sub-chunks every q^(y0+1)
 template <class F>
-void for_each_read_piece(const garage_ec_ctx *ctx, uint64_t halves, size_t i, size_t len, size_t whole, F &&f)
+void for_each_read_piece(const garage_ec_ctx *ctx, uint64_t rows, size_t i, size_t len, size_t whole, F &&f)
 {
-    const unsigned b = (unsigned)(halves >> (2 * i)) & 3u;
+    const unsigned b = read_halves(ctx, rows, i);
     if (!b) return;
     if (ctx->clay) {
         const int tot = ctx->k + ctx->m;
         int nread = 0, f_shard = 0;
         for (int j = 0; j < tot; j++) {
-            if ((halves >> (2 * j)) & 3) nread++;
+            if (read_halves(ctx, rows, j)) nread++;
             else f_shard = j;
         }
         if (nread != tot - 1) return f((size_t)0, whole);
@@ -1086,7 +1088,7 @@ int garage_ec_read_plan(const garage_ec_ctx *ctx, const uint8_t *present, const 
     if (!ctx || !present || !halves_out || ctx->clay) return GARAGE_EC_E_INVALID;
     uint64_t hv = 0;
     const bool ok = stripe_read_plan(ctx, present, want, &hv);
-    for (int i = 0; i < ctx->k + ctx->m; i++) halves_out[i] = (uint8_t)((hv >> (2 * i)) & 3);
+    for (int i = 0; i < ctx->k + ctx->m; i++) halves_out[i] = (uint8_t)read_halves(ctx, hv, i);
     return ok ? GARAGE_EC_OK : GARAGE_EC_E_UNRECOVERABLE;
 }
 
@@ -1966,6 +1968,9 @@ static int sums_common(garage_ec_ctx *ctx, const uint8_t *shards, const uint8_t 
     if (!shards || (!sums_out && !bad_out)) return GARAGE_EC_E_INVALID;
     if (!aligned16(shards)) return GARAGE_EC_E_ALIGN;
     if (n * (size_t)per > 0xffffffffull) return GARAGE_EC_E_INVALID;
+    if (mem_kind == GARAGE_EC_MEM_HOST && shard_len)  // tags of any length are legal, but not past the stride
+        for (size_t s = 0; s < n; s++)
+            if (shard_len[s] > stride) return GARAGE_EC_E_INVALID;
     CU_TRY(ctx, cudaSetDevice(ctx->device));
     if (mem_kind == GARAGE_EC_MEM_DEVICE)
         return run_sums(ctx, shards, expect, shard_len, stride, n * per, per, sums_out, bad_out,

@@ -1300,7 +1300,7 @@ struct PlanParams {
     uint32_t l;               // LRC local groups; 0 for RS and PB
     uint32_t pb;              // 1: PB(k, m), planned over half-rows
     uint32_t present_is_bad;  // 1: `present` holds "bad" flags (scrub): a shard is present iff flag == 0
-    const uint32_t *shard_len;  // PB: per stripe, nullable (=> stride); a length % 32 != 0 is malformed
+    const uint32_t *shard_len;  // per stripe, nullable (=> stride); > stride (PB: or % 32 != 0) is malformed
     uint32_t stride;
     alignas(16) uint8_t P[kMaxM * kMaxK];  // parity rows, P[i*k + j] (16-byte aligned: staged with uint4 loads)
 };
@@ -1316,8 +1316,9 @@ static_assert(2 * kPbMaxM <= kMaxM && 2 * kPbMaxK <= kMaxK, "PB half-rows fit a 
 // every earlier pivot.  The data rows come first and are identity rows, so the candidate data rows enter the basis
 // as they are (pivot = their column, T = e_position), and reducing a row against all of them is one lane-parallel
 // step.  Only parity rows and wanted rows are reduced serially, against the parity rows of the basis: fewer than the
-// absent data columns and at most kMaxM.  A PB stripe whose shard_len is not a multiple of 32 has no 16-byte aligned
-// halves: status GARAGE_EC_E_INVALID (-1), nothing is rebuilt.  16 CTAs per SM keep it at 32 registers, no spills.
+// absent data columns and at most kMaxM.  A stripe whose shard_len exceeds the stride, or a PB stripe whose shard_len
+// is not a multiple of 32 (no 16-byte aligned halves), is malformed: status GARAGE_EC_E_INVALID (-1), no rows, so the
+// apply kernel reads and writes nothing of it.  16 CTAs per SM keep it at 32 registers, no spills.
 __global__ void __launch_bounds__(kPlanWarps * 32, 16) plan_kernel(const __grid_constant__ PlanParams q)
 {
     __shared__ __align__(16) uint8_t s_gf[sizeof(GfTables)];
@@ -1358,7 +1359,8 @@ __global__ void __launch_bounds__(kPlanWarps * 32, 16) plan_kernel(const __grid_
     const bool w1 = lane + 32 < tot && !p1 && (!wn || wn[lane + 32] != 0);
     const unsigned long long outmask =
         (unsigned long long)__ballot_sync(0xffffffffu, w0) | ((unsigned long long)__ballot_sync(0xffffffffu, w1) << 32);
-    if (q.pb && ((q.shard_len ? q.shard_len[s] : q.stride) & 31)) {
+    const uint32_t slen = q.shard_len ? q.shard_len[s] : q.stride;
+    if (slen > q.stride || (q.pb && (slen & 31))) {
         if (lane == 0) {
             pl->key_present = present;
             pl->key_out = outmask;
@@ -1627,8 +1629,10 @@ struct SumParams {
     uint32_t out_off2;
 };
 
-// where shard i of a launch lives, which stripe's length applies, and its slot in sums/expect/bad
-__device__ __forceinline__ void locate_shard(const SumParams &q, uint32_t i, const uint8_t *&p, uint32_t &len,
+// where shard i of a launch lives, which stripe's length applies, and its slot in sums/expect/bad.  False for a shard
+// whose length exceeds the stride: it is malformed, the kernels read none of it, check mode flags it bad and sums mode
+// leaves its 32 bytes alone.
+__device__ __forceinline__ bool locate_shard(const SumParams &q, uint32_t i, const uint8_t *&p, uint32_t &len,
                                              size_t &oi)
 {
     uint32_t stripe;
@@ -1643,6 +1647,7 @@ __device__ __forceinline__ void locate_shard(const SumParams &q, uint32_t i, con
         oi = (size_t)stripe * q.out_per_stripe + q.out_off2 + (j - stripe * q.per_stripe2);
     }
     len = q.shard_len ? __ldg(q.shard_len + stripe) : q.stride;
+    return len <= q.stride;
 }
 
 __global__ void __launch_bounds__(128) blake2sum_shards_kernel(const __grid_constant__ SumParams q)
@@ -1652,7 +1657,10 @@ __global__ void __launch_bounds__(128) blake2sum_shards_kernel(const __grid_cons
     const uint8_t *p;
     uint32_t len;
     size_t oi;
-    locate_shard(q, i, p, len, oi);
+    if (!locate_shard(q, i, p, len, oi)) {
+        if (q.expect && q.bad) q.bad[oi] = 1;
+        return;
+    }
     Blake2bState S;
     blake2b_init512(S);
     uint64_t m[16];
@@ -1795,7 +1803,10 @@ __global__ void __launch_bounds__(kQuadThreads) blake2sum_shards_quad_kernel(con
     const uint8_t *p;
     uint32_t len;
     size_t oi;
-    locate_shard(q, i, p, len, oi);
+    if (!locate_shard(q, i, p, len, oi)) {  // the same for the whole quad: it leaves together
+        if (c == 0 && q.expect && q.bad) q.bad[oi] = 1;
+        return;
+    }
 
     // this lane's 32 bytes of the shard starting at byte `o` (zero beyond len)
     auto load32 = [&](uint32_t o, uint4 &x, uint4 &y) {
@@ -2095,11 +2106,11 @@ __global__ void __launch_bounds__(256) adler8_shards_kernel(const __grid_constan
         const uint8_t *p;
         uint32_t len;
         size_t oi;
-        locate_shard(q, i, p, len, oi);
+        const bool ok = locate_shard(q, i, p, len, oi);  // warp-uniform: one unit per warp
         const uint32_t seg = adler8_seg_bytes(len);
         const uint32_t start = sgi * seg;
         uint32_t tag = 1;  // Adler-32 of an empty segment
-        if (start < len) {
+        if (ok && start < len) {
             const uint32_t end = min(len, start + seg), n = end - start;
             unsigned long long A = 0, B = 0, T = 0;
             // 8 vectors per lane in flight: rel = byte offset of the vector inside the segment
@@ -2141,8 +2152,8 @@ __global__ void __launch_bounds__(256) adler8_shards_kernel(const __grid_constan
             tag = (b << 16) | a;
         }
         if (lane == 0) {
-            if (q.sums) reinterpret_cast<uint32_t *>(q.sums + oi * 32)[sgi] = tag;
-            if (q.expect && q.bad && reinterpret_cast<const uint32_t *>(q.expect + oi * 32)[sgi] != tag) {
+            if (ok && q.sums) reinterpret_cast<uint32_t *>(q.sums + oi * 32)[sgi] = tag;
+            if (q.expect && q.bad && (!ok || reinterpret_cast<const uint32_t *>(q.expect + oi * 32)[sgi] != tag)) {
                 // set byte `oi` of bad[] to 1 through the aligned 32-bit word that contains it
                 const unsigned long long addr = reinterpret_cast<unsigned long long>(q.bad + oi);
                 atomicOr(reinterpret_cast<unsigned int *>(addr & ~3ull), 1u << (8 * (unsigned)(addr & 3ull)));

@@ -181,7 +181,10 @@ int garage_ec_encode(garage_ec_ctx *ctx, const uint8_t *data, uint8_t *parity,
  *             present; stripe untouched)
  * Survivors used: those of garage_ec_read_set (RS: the first k present shards in index order); only
  * they are read, and HOST calls copy only them to the GPU.  HOST calls return
- * GARAGE_EC_E_UNRECOVERABLE if any stripe was; DEVICE calls only fill status[].            */
+ * GARAGE_EC_E_UNRECOVERABLE if any stripe was; DEVICE calls only fill status[].  A stripe
+ * whose shard_len exceeds `stride` is malformed, for every code: a HOST call returns
+ * GARAGE_EC_E_INVALID before any GPU work; a DEVICE call reports GARAGE_EC_E_INVALID in its
+ * status[], reads and writes nothing of it, and rebuilds the other stripes.                 */
 int garage_ec_reconstruct(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *present,
                           const uint8_t *want, int32_t *status, const uint32_t *shard_len,
                           size_t stride, size_t n_stripes, int mem_kind, void *cuda_stream);
@@ -230,7 +233,10 @@ int garage_ec_deep_check(garage_ec_ctx *ctx, const uint8_t *shards, const uint32
  *   shards          : n_stripes * shards_per_stripe shards, `stride` apart (shard layout)
  *   shards_per_stripe: k (a data array), m (a parity array) or k+m
  *   sums_out        : 32 bytes per shard
- * garage_ec_check_sums compares with `expect` instead: bad_out[i] = 1 iff shard i differs.     */
+ * garage_ec_check_sums compares with `expect` instead: bad_out[i] = 1 iff shard i differs.
+ * shard_len may be any length up to `stride`.  A stripe whose shard_len exceeds `stride` is
+ * malformed: a HOST call returns GARAGE_EC_E_INVALID before any GPU work; a DEVICE call reads
+ * nothing of its shards, leaves their sums_out bytes untouched and sets their bad_out to 1.    */
 int garage_ec_shard_sums(garage_ec_ctx *ctx, const uint8_t *shards, const uint32_t *shard_len,
                          size_t stride, size_t n_stripes, int shards_per_stripe, uint8_t *sums_out,
                          int mem_kind, void *cuda_stream);
@@ -241,7 +247,10 @@ int garage_ec_check_sums(garage_ec_ctx *ctx, const uint8_t *shards, const uint8_
  * feeding resync (src/block/resync.rs:354-503) in one pass: blake2sum every shard, treat the ones
  * whose sum differs from `expect_sums` as erased, rebuild them in place from the first k intact
  * shards.  bad_out[s*(k+m)+i] = 1 iff shard i was corrupt; status[s] = 0 or
- * GARAGE_EC_E_UNRECOVERABLE (> m corrupt shards: reported, never fatal -- resync.rs:300-315).     */
+ * GARAGE_EC_E_UNRECOVERABLE (> m corrupt shards: reported, never fatal -- resync.rs:300-315).
+ * A stripe whose shard_len exceeds `stride` is malformed, for every code: a HOST call returns
+ * GARAGE_EC_E_INVALID before any GPU work; a DEVICE call reads and writes nothing of it, sets
+ * bad_out of all its k+m shards to 1 and reports GARAGE_EC_E_INVALID in its status[].         */
 int garage_ec_scrub_repair(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *expect_sums,
                            uint8_t *bad_out, int32_t *status, const uint32_t *shard_len,
                            size_t stride, size_t n_stripes, int mem_kind, void *cuda_stream);
