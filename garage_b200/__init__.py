@@ -19,7 +19,7 @@ __all__ = ["GarageEc", "EcError", "load_library", "lib_path", "ABI_SYMBOLS",
            "MEM_HOST", "MEM_DEVICE", "VANDERMONDE", "CAUCHY"]
 
 OK = 0
-E_INVALID, E_CUDA, E_NOMEM, E_UNRECOVERABLE, E_NODEVICE, E_ALIGN = -1, -2, -3, -4, -5, -6
+E_INVALID, E_CUDA, E_NOMEM, E_UNRECOVERABLE, E_NODEVICE, E_ALIGN, E_AUTH = -1, -2, -3, -4, -5, -6, -7
 VANDERMONDE, CAUCHY = 0, 1
 MEM_HOST, MEM_DEVICE = 0, 1
 MAX_K, MAX_M = 32, 8
@@ -43,6 +43,7 @@ ABI_SYMBOLS = [
     "garage_ec_deep_check",
     "garage_ec_tag_span", "garage_ec_check_shard_span_host", "garage_ec_range_plan", "garage_ec_decode_range",
     "garage_ec_decode_range_stripes",
+    "garage_ec_sealed_len", "garage_ec_seal", "garage_ec_seal_blocks", "garage_ec_open", "garage_ec_open_stripes",
 ]
 
 
@@ -137,8 +138,22 @@ def load_library(build=True):
     L.garage_ec_range_plan.argtypes = [vp, vp, u32, u32, u32, vp, sz, C.POINTER(sz), C.POINTER(i32)]
     L.garage_ec_decode_range.argtypes = [vp, vp, vp, vp, vp, vp, sz, vp, sz, vp, sz, i32, vp]
     L.garage_ec_decode_range_stripes.argtypes = [vp, vp, vp, vp, vp, vp, sz, vp, vp, sz]
+    L.garage_ec_sealed_len.argtypes = [u32, C.POINTER(u32)]
+    L.garage_ec_seal.argtypes = [vp, vp, sz, vp, vp, vp, vp, sz, vp, vp, sz, i32, vp]
+    L.garage_ec_seal_blocks.argtypes = [vp, vp, vp, vp, vp, vp, sz, vp, vp, sz]
+    L.garage_ec_open.argtypes = [vp, vp, vp, vp, vp, vp, vp, sz, vp, vp, vp, sz, sz, i32, vp]
+    L.garage_ec_open_stripes.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, sz]
     _lib = L
     return L
+
+
+def sealed_len(plain_len) -> int:
+    """garage_ec_sealed_len: 8 + plain_len + 16 * max(1, ceil(plain_len / 4096))"""
+    v = C.c_uint32(0)
+    rc = load_library().garage_ec_sealed_len(plain_len, C.byref(v))
+    if rc:
+        raise EcError(rc, "sealed_len")
+    return v.value
 
 
 def blake2sum(data) -> bytes:
@@ -491,6 +506,44 @@ class GarageEc:
                                                        _ptr(src_present), _ptr(block_lens), src_stride, _ptr(dst_shards),
                                                        dst_stride, _ptr(dst_sums), _ptr(status), n, kind, st),
                            (E_UNRECOVERABLE,))
+
+    # -- SSE-C (AES-256-GCM STREAM chunks, DESIGN.md 2.6)
+    def seal(self, plain, plain_stride, plain_len, keys, nonces, shards, stride, hashes, sums=None, n=None):
+        """garage_ec_seal of n = len(plain_len) blocks; keys = nonces = None stores them as plaintext"""
+        kind, st = self._stream(plain, shards)
+        n = len(plain_len) if n is None else n
+        return self._check(self._L.garage_ec_seal(self._h, _ptr(plain), plain_stride, _ptr(plain_len), _ptr(keys),
+                                                  _ptr(nonces), _ptr(shards), stride, _ptr(hashes), _ptr(sums), n,
+                                                  kind, st))
+
+    def seal_blocks(self, blocks, keys, nonces, shards, stride, hashes, sums=None):
+        """HOST gather form: `blocks` is a list of 1-D uint8 numpy arrays"""
+        n = len(blocks)
+        ptrs = (C.c_void_p * n)(*[b.ctypes.data if b.size else None for b in blocks])
+        lens = np.array([b.size for b in blocks], dtype=np.uint32)
+        return self._check(self._L.garage_ec_seal_blocks(self._h, C.cast(ptrs, C.c_void_p), _ptr(lens), _ptr(keys),
+                                                         _ptr(nonces), _ptr(shards), stride, _ptr(hashes), _ptr(sums), n))
+
+    def open(self, shards, present, sealed_len, hashes, keys, plain, plain_stride, plain_len_out, hash_bad, status,
+             stride, n=None):
+        """garage_ec_open; returns 0, E_UNRECOVERABLE or E_AUTH (HOST mode)"""
+        kind, st = self._stream(shards)
+        n = len(sealed_len) if n is None else n
+        return self._check(self._L.garage_ec_open(self._h, _ptr(shards), _ptr(present), _ptr(sealed_len), _ptr(hashes),
+                                                  _ptr(keys), _ptr(plain), plain_stride, _ptr(plain_len_out),
+                                                  _ptr(hash_bad), _ptr(status), stride, n, kind, st),
+                           (E_UNRECOVERABLE, E_AUTH))
+
+    def open_stripes(self, stripes, present, sealed_len, hashes, keys, plains, plain_len_out, hash_bad, status, stride):
+        """HOST gather form: `stripes` / `plains` are lists of numpy arrays, one per block"""
+        n = len(stripes)
+        sp = (C.c_void_p * n)(*[a.ctypes.data for a in stripes])
+        op = (C.c_void_p * n)(*[a.ctypes.data for a in plains])
+        return self._check(self._L.garage_ec_open_stripes(self._h, C.cast(sp, C.c_void_p), _ptr(present),
+                                                          _ptr(sealed_len), _ptr(hashes), _ptr(keys),
+                                                          C.cast(op, C.c_void_p), _ptr(plain_len_out), _ptr(hash_bad),
+                                                          _ptr(status), stride, n),
+                           (E_UNRECOVERABLE, E_AUTH))
 
     # -- harness utilities
     def fill_random(self, dst, nbytes, seed, offset=0):

@@ -8,7 +8,7 @@ ROOT = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, "csrc")
 SO = os.path.join(PKG, "libgarage_ec.so")
 SOURCES = ["garage_ec.cu"]
-DEPS = ["garage_ec.cu", "rs_kernels.cuh", "clay_kernels.cuh", "gf256.h", "gf256_tables.inc", "blake2b.h"]
+DEPS = ["garage_ec.cu", "rs_kernels.cuh", "clay_kernels.cuh", "sse_kernels.cuh", "gf256.h", "gf256_tables.inc", "blake2b.h"]
 
 
 def nvcc_path():

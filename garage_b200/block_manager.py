@@ -24,6 +24,7 @@ SYMBOLS = [
     "garage_bm_set_data_dirs", "garage_bm_rebalance_step", "garage_bm_get_drive_metrics", "garage_bm_create_with_drives",
     "garage_bm_resync_step", "garage_bm_list_resync_errors", "garage_bm_resync_retry_now", "garage_bm_block_info",
     "garage_bm_debug_set_clock_ms", "garage_bm_get_resync_metrics",
+    "garage_bm_rpc_put_block_sealed", "garage_bm_rpc_get_block_opened", "garage_bm_get_sealed_metrics",
 ]
 SUM_BLAKE2, SUM_ADLER8 = 0, 1
 
@@ -105,6 +106,12 @@ class StripeRepairMetrics(C.Structure):
 class ResyncMetrics(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in (
         "resync_error_entries", "resync_deferred", "resync_steps", "resync_retry_nows", "resync_failed_bytes_read")]
+
+
+class SealedMetrics(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in (
+        "sealed_puts", "sealed_batches", "opened_gets", "opened_auth_failures", "opened_fallbacks", "seal_call_us",
+        "open_call_us")]
 
 
 class ResyncError(C.Structure):
@@ -191,6 +198,10 @@ def load_library():
         L.garage_bm_debug_set_clock_ms.argtypes = [vp, C.c_uint64]
         L.garage_bm_get_resync_metrics.argtypes = [vp, C.POINTER(ResyncMetrics)]
         L.garage_bm_get_resync_metrics.restype = None
+        L.garage_bm_rpc_put_block_sealed.argtypes = [vp, vp, vp, sz, vp]
+        L.garage_bm_rpc_get_block_opened.argtypes = [vp, vp, vp, vp, sz, C.POINTER(sz)]
+        L.garage_bm_get_sealed_metrics.argtypes = [vp, C.POINTER(SealedMetrics)]
+        L.garage_bm_get_sealed_metrics.restype = None
         _lib = L
     return _lib
 
@@ -286,6 +297,27 @@ class BlockManager:
         n = C.c_size_t(0)
         rc = self._L.garage_bm_rpc_get_block(self._h, self._hp(hash32), C.c_void_p(out.ctypes.data), cap, C.byref(n))
         return rc, (out[: n.value].copy() if rc == OK else None)
+
+    def rpc_put_block_sealed(self, key32, data):
+        """(rc, content address) of an SSE-C PUT; key32 None stores the block as plaintext"""
+        a = np.ascontiguousarray(data, dtype=np.uint8)
+        h = (C.c_uint8 * 32)()
+        rc = self._L.garage_bm_rpc_put_block_sealed(self._h, None if key32 is None else C.c_char_p(bytes(key32)),
+                                                    C.c_void_p(a.ctypes.data) if a.size else None, a.size, h)
+        return rc, bytes(h)
+
+    def rpc_get_block_opened(self, hash32, key32, cap=1 << 20):
+        """(rc, plaintext or None) of an SSE-C GET"""
+        out = np.empty(max(cap, 1), dtype=np.uint8)
+        n = C.c_size_t(0)
+        rc = self._L.garage_bm_rpc_get_block_opened(self._h, self._hp(hash32), C.c_char_p(bytes(key32)),
+                                                    C.c_void_p(out.ctypes.data), cap, C.byref(n))
+        return rc, (out[: n.value].copy() if rc == OK else None)
+
+    def sealed_metrics(self):
+        mt = SealedMetrics()
+        self._L.garage_bm_get_sealed_metrics(self._h, C.byref(mt))
+        return {n: getattr(mt, n) for n, _ in SealedMetrics._fields_}
 
     def rpc_get_block_range(self, hash32, offset, length):
         """(rc, bytes [offset, offset + length) of the block or None)"""

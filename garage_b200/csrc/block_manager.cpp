@@ -44,6 +44,7 @@
 
 #include <fcntl.h>
 #include <sys/mman.h>
+#include <sys/random.h>
 #include <sys/stat.h>
 #include <unistd.h>
 
@@ -1484,6 +1485,14 @@ struct EncodeItem {
     size_t pstride = 0;
     const uint8_t *sums = nullptr;
     EncBatchBuf *buf = nullptr;  // to be released (done_one) once the shards are stored
+    // a sealed PUT (rpc_put_block_sealed): the block is sealed under `key` (NULL: stored as plaintext) and `nonce`; the
+    // dispatcher fills `shards` (all k+m, `pstride` apart, kept alive by `sealed_out`) and the content address `hash`
+    bool sealed = false;
+    const uint8_t *key = nullptr;
+    uint8_t nonce[8] = {0};
+    std::shared_ptr<std::vector<uint8_t>> sealed_out;
+    const uint8_t *shards = nullptr;
+    Hash hash{};
     bool fulfilled = false;
     std::promise<int> done;
 };
@@ -1500,6 +1509,11 @@ struct ReconItem {
     uint32_t off = 0, len = 0;
     uint8_t *out = nullptr;
     std::atomic<uint64_t> *call_us = nullptr;  // non-NULL: also gets the wall time of the call that rebuilt this stripe
+    // an opened GET (garage_ec_open_stripes): `block_len` is the sealed length, the plaintext goes to `out`
+    bool open = false;
+    const uint8_t *key = nullptr;
+    Hash hash{};
+    uint32_t plain_len = 0;
     bool fulfilled = false;
     std::promise<int> done;
 };
@@ -1597,6 +1611,8 @@ struct garage_bm {
     std::atomic<uint64_t> convert_blocks{0}, convert_bytes_read{0}, convert_bytes_written{0}, convert_errors{0},
         convert_call_us{0}, legacy_gets{0}, legacy_deleted{0}, range_gets{0}, range_degraded{0}, range_bytes_read{0},
         range_bytes_fetched{0};
+    std::atomic<uint64_t> sealed_puts{0}, sealed_batches{0}, opened_gets{0}, opened_auth_failures{0}, opened_fallbacks{0},
+        seal_call_us{0}, open_call_us{0};
     std::atomic<uint64_t> layout_shards_copied{0}, layout_shards_rebuilt{0}, layout_bytes_read{0}, layout_bytes_written{0},
         layout_deleted{0}, layout_sync_errors{0}, layout_bytes_fetched{0};
     std::atomic<uint64_t> stripe_repairs{0}, stripe_repair_shards{0}, stripe_repair_bytes_read{0},
@@ -1818,8 +1834,76 @@ struct garage_bm {
     }
 
     // ---- batch runners (dispatcher threads) -------------------------------------------------
-    void run_encode(int w, std::vector<EncodeItem *> &b)
+    // the largest stored block: a block_size plaintext sealed (DESIGN.md section 2.6)
+    uint32_t stored_max() const
     {
+        uint32_t s = 0;
+        return garage_ec_sealed_len(cfg.block_size, &s) == GARAGE_EC_OK ? s : cfg.block_size;
+    }
+
+    static void wipe_secret(void *p, size_t n)
+    {
+        volatile uint8_t *v = static_cast<volatile uint8_t *>(p);
+        while (n--) *v++ = 0;
+    }
+
+    // the sealed PUTs of a batch, keyed or stored as plaintext: one garage_ec_seal_blocks call
+    void run_seal(int w, std::vector<EncodeItem *> &b, bool keyed)
+    {
+        const size_t n = b.size();
+        uint32_t max_len = 0;
+        std::vector<const uint8_t *> ptrs(n);
+        std::vector<uint32_t> lens(n);
+        std::vector<uint8_t> keys(keyed ? n * 32 : 0), nonces(keyed ? n * 8 : 0);
+        for (size_t i = 0; i < n; i++) {
+            ptrs[i] = b[i]->data;
+            lens[i] = b[i]->len;
+            max_len = std::max(max_len, b[i]->len);
+            if (keyed) {
+                memcpy(keys.data() + i * 32, b[i]->key, 32);
+                memcpy(nonces.data() + i * 8, b[i]->nonce, 8);
+            }
+        }
+        uint32_t max_b = max_len;
+        if (keyed) garage_ec_sealed_len(max_len, &max_b);
+        const size_t stride = garage_ec_stride_for((uint32_t)shard_len_of(max_b));
+        std::shared_ptr<std::vector<uint8_t>> out;
+        int rc = GARAGE_EC_OK;
+        try {
+            out = std::make_shared<std::vector<uint8_t>>(n * tot * stride + n * 32 + n * tot * 32);
+        } catch (const std::bad_alloc &) {
+            rc = GARAGE_EC_E_NOMEM;
+        }
+        uint8_t *sh = out ? out->data() : nullptr, *hashes = sh ? sh + n * tot * stride : nullptr,
+                *sums = hashes ? hashes + n * 32 : nullptr;
+        const auto t0 = Clock::now();
+        if (rc == GARAGE_EC_OK)
+            rc = garage_ec_seal_blocks(enc_ctx[w], ptrs.data(), lens.data(), keyed ? keys.data() : nullptr,
+                                       keyed ? nonces.data() : nullptr, sh, stride, hashes, sums, n);
+        seal_call_us += (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count();
+        sealed_batches++;
+        if (keyed) wipe_secret(keys.data(), keys.size());
+        for (size_t i = 0; i < n; i++) {
+            if (rc == GARAGE_EC_OK) {
+                b[i]->sealed_out = out;
+                b[i]->shards = sh + i * tot * stride;
+                b[i]->pstride = stride;
+                b[i]->sums = sums + i * tot * 32;
+                memcpy(b[i]->hash.data(), hashes + i * 32, 32);
+            }
+            b[i]->fulfilled = true;
+            b[i]->done.set_value(rc);
+        }
+    }
+
+    void run_encode(int w, std::vector<EncodeItem *> &all)
+    {
+        // sealed PUTs go to their own calls, as run_reconstruct keeps ranged GETs apart
+        std::vector<EncodeItem *> b, keyed, unkeyed;
+        for (EncodeItem *it : all) (it->sealed ? (it->key ? keyed : unkeyed) : b).push_back(it);
+        if (!keyed.empty()) run_seal(w, keyed, true);
+        if (!unkeyed.empty()) run_seal(w, unkeyed, false);
+        if (b.empty()) return;
         const size_t n = b.size();
         uint32_t max_len = 0;
         std::vector<const uint8_t *> ptrs(n);
@@ -1854,9 +1938,10 @@ struct garage_bm {
 
     void run_reconstruct(int w, std::vector<ReconItem *> &all)
     {
-        std::vector<ReconItem *> b, rb;  // whole-shard rebuilds, ranged GETs
-        for (ReconItem *it : all) (it->range ? rb : b).push_back(it);
+        std::vector<ReconItem *> b, rb, ob;  // whole-shard rebuilds, ranged GETs, opened GETs
+        for (ReconItem *it : all) (it->open ? ob : it->range ? rb : b).push_back(it);
         if (!rb.empty()) run_decode_range(w, rb);
+        if (!ob.empty()) run_open(w, ob);
         if (b.empty()) return;
         const size_t n = b.size();
         std::vector<uint8_t *> stripes(n);
@@ -1883,6 +1968,44 @@ struct garage_bm {
         for (size_t i = 0; i < n; i++) {
             int r = rc;
             if (rc == GARAGE_EC_OK || rc == GARAGE_EC_E_UNRECOVERABLE) r = status[i] ? GARAGE_BM_E_MISSING_BLOCK : GARAGE_BM_OK;
+            b[i]->fulfilled = true;
+            b[i]->done.set_value(r);
+        }
+    }
+
+    // the opened GETs of a dispatcher batch: one garage_ec_open_stripes on their stripe slots -- rebuild, content hash,
+    // every chunk's tag, decryption.  Per item: OK, GARAGE_EC_E_AUTH, GARAGE_BM_E_MISSING_BLOCK, or
+    // GARAGE_BM_E_CORRUPT_DATA for a block that does not hash to its address (the caller hunts the stale shard)
+    void run_open(int w, std::vector<ReconItem *> &b)
+    {
+        const size_t n = b.size();
+        std::vector<uint8_t *> stripes(n), outs(n);
+        std::vector<uint8_t> present(n * tot), hashes(n * 32), keys(n * 32), bad(n, 0);
+        std::vector<uint32_t> sealed(n), plen(n, 0);
+        std::vector<int32_t> status(n, 0);
+        for (size_t i = 0; i < n; i++) {
+            stripes[i] = b[i]->stripe;
+            outs[i] = b[i]->out;
+            sealed[i] = b[i]->block_len;
+            memcpy(present.data() + i * tot, b[i]->present, tot);
+            memcpy(hashes.data() + i * 32, b[i]->hash.data(), 32);
+            memcpy(keys.data() + i * 32, b[i]->key, 32);
+        }
+        const auto t0 = Clock::now();
+        const int rc = garage_ec_open_stripes(rec_ctx[w], stripes.data(), present.data(), sealed.data(), hashes.data(),
+                                              keys.data(), outs.data(), plen.data(), bad.data(), status.data(), slot_stride, n);
+        open_call_us += (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count();
+        wipe_secret(keys.data(), keys.size());
+        for (size_t i = 0; i < n; i++) {
+            int r = rc;
+            if (rc == GARAGE_EC_OK || rc == GARAGE_EC_E_UNRECOVERABLE || rc == GARAGE_EC_E_AUTH)
+                // a block that does not hash to its address is the wrong block (a stale shard): its tags say
+                // nothing about the key, so the caller hunts the shard before any verdict on authentication
+                r = status[i] == GARAGE_EC_E_UNRECOVERABLE ? GARAGE_BM_E_MISSING_BLOCK
+                    : bad[i]                             ? GARAGE_BM_E_CORRUPT_DATA
+                    : status[i]                          ? status[i]
+                                                         : GARAGE_BM_OK;
+            b[i]->plain_len = plen[i];
             b[i]->fulfilled = true;
             b[i]->done.set_value(r);
         }
@@ -2138,8 +2261,6 @@ struct garage_bm {
     int rpc_put_block(const Hash &h, const uint8_t *data, size_t len)
     {
         if (len == 0 || len > cfg.block_size) return GARAGE_BM_E_MESSAGE;  // blocks are at most block_size (put.rs:583-617)
-        int who[64];
-        storage_nodes_of(h, who);  // manager.rs:373
         // DataBlock::from_buffer (manager.rs:376): compression is 'none' in this mirror
         const uint64_t permits = (uint64_t)len * tot / k;  // manager.rs:380-385, x (k+m)/k for the parity
         ram->acquire(permits);
@@ -2190,18 +2311,125 @@ struct garage_bm {
             if (have) memcpy(pad.data(), slot.p + off, have);
             return pad.data();
         };
+        return store_block(h, (uint32_t)len, L, shard_bytes, it.sums);
+    }
+    // the k+m shards of a block of len stored bytes: every active layout version, the write quorum, the block's ref
+    int store_block(const Hash &h, uint32_t len, size_t L, const std::function<const uint8_t *(int)> &shard_bytes,
+                    const uint8_t *sums)
+    {
+        int who[64];
+        storage_nodes_of(h, who);  // manager.rs:373
         const int quorum = garage_ec_write_quorum(k, m, GARAGE_CONSISTENT);  // k+1 capped at k+m (row f4, garage_placement.h)
         auto ls = layouts();
-        if (ls->v.size() > 1) return put_many_sets(*ls, h, (uint32_t)len, L, shard_bytes, it.sums, quorum);
+        if (ls->v.size() > 1) return put_many_sets(*ls, h, len, L, shard_bytes, sums, quorum);
         int stored = 0;
         for (int i = 0; i < tot; i++)  // try_write_many_sets (manager.rs:395-405): all at once
             // only a shard that is durably stored counts towards the quorum
-            if (write_shard(who[i], h, i, (uint32_t)len, shard_bytes(i), L, it.sums + (size_t)i * 32)) stored++;
+            if (write_shard(who[i], h, i, len, shard_bytes(i), L, sums + (size_t)i * 32)) stored++;
         {
             std::lock_guard<std::mutex> lk(refs_mu);
-            refs[h] = (uint32_t)len;
+            refs[h] = len;
         }
         return stored >= quorum ? GARAGE_BM_OK : GARAGE_BM_E_QUORUM;
+    }
+
+    // An SSE-C PUT (put.rs:441-466): the plaintext (up to block_size bytes) lands in a put slot and goes through the
+    // encode batcher, whose sealed items become one garage_ec_seal_blocks call; key NULL stores it as plaintext.  The
+    // nonce prefix is 8 bytes of getrandom(2) (Garage: OsRng).  The k+m shards are stored as rpc_put_block stores a
+    // block of sealed_len bytes; *hash_out = the block's content address.
+    int rpc_put_block_sealed(const uint8_t *key, const uint8_t *data, size_t len, uint8_t *hash_out)
+    {
+        if (len > cfg.block_size || (!key && len == 0)) return GARAGE_BM_E_MESSAGE;
+        uint32_t blen = (uint32_t)len;
+        if (key && garage_ec_sealed_len((uint32_t)len, &blen) != GARAGE_EC_OK) return GARAGE_BM_E_MESSAGE;
+        const uint64_t permits = (uint64_t)blen * tot / k;
+        ram->acquire(permits);
+        struct Permit {
+            ByteSemaphore &s;
+            uint64_t n;
+            ~Permit() { s.release(n); }
+        } permit{*ram, permits};
+        SlotLease slot(put_slots);
+        if (len) copy_for_dma(slot.p, data, len);
+        EncodeItem it;
+        it.data = slot.p;
+        it.len = (uint32_t)len;
+        it.sealed = true;
+        it.key = key;
+        for (size_t got = 0; key && got < sizeof(it.nonce);) {
+            const ssize_t r = getrandom(it.nonce + got, sizeof(it.nonce) - got, 0);
+            if (r < 0 && errno != EINTR) return GARAGE_BM_E_MESSAGE;
+            if (r > 0) got += (size_t)r;
+        }
+        const int rc = enc_batcher->submit(it);
+        if (rc != GARAGE_EC_OK) return rc;
+        sealed_puts++;
+        memcpy(hash_out, it.hash.data(), 32);
+        const uint8_t *sh = it.shards;
+        const size_t stride = it.pstride;
+        return store_block(it.hash, blen, shard_len_of(blen), [&](int i) { return sh + (size_t)i * stride; }, it.sums);
+    }
+
+    // One opened GET of the stripe in `slot` (its shards `have`, the stored length block_len) through the reconstruct
+    // dispatchers
+    int open_in_slot(const Hash &h, const uint8_t *key, uint8_t *slot, uint32_t block_len, const uint8_t *have, uint8_t *out,
+                     size_t cap, size_t *out_len)
+    {
+        const uint32_t n = block_len >= 24 ? (block_len - 8 + 4111) / 4112 : 1;
+        if (block_len >= 24 && block_len - 8 - 16ull * n > cap) return GARAGE_EC_E_INVALID;
+        ReconItem it;
+        it.open = true;
+        it.stripe = slot;
+        it.stride = slot_stride;
+        it.block_len = block_len;
+        memcpy(it.present, have, tot);
+        it.key = key;
+        it.hash = h;
+        it.out = out;
+        const int rc = rec_batcher->submit(it);
+        if (rc == GARAGE_BM_OK) {
+            opened_gets++;
+            *out_len = it.plain_len;
+        } else if (rc == GARAGE_EC_E_AUTH) {
+            opened_auth_failures++;
+        }
+        return rc;
+    }
+
+    // An SSE-C GET (EncryptionParams::get_block, encryption.rs:269-279): gathered like rpc_get_block, then the rebuild,
+    // the content-hash check and the decryption in one garage_ec_open_stripes call -- no CPU blake2 on this path.  A
+    // block that does not hash to h, or that the configured stripe cannot serve (previous codes, replicas), goes
+    // through rpc_get_block, with its stale-shard hunt, and the block it returns is opened.
+    int rpc_get_block_opened(const Hash &h, const uint8_t *key, uint8_t *out, size_t cap, size_t *out_len)
+    {
+        {
+            SlotLease slot(stripe_slots);
+            uint8_t have[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
+            uint32_t block_len = 0;
+            bool ok = false;
+            gather_into(h, -1, slot.p, have, block_len, false, false, nullptr, &ok, nullptr, 0);
+            if (ok) {
+                const int rc = open_in_slot(h, key, slot.p, block_len, have, out, cap, out_len);
+                if (rc != GARAGE_BM_E_CORRUPT_DATA) return rc;
+            }
+        }
+        opened_fallbacks++;
+        std::vector<uint8_t> blk(stored_max());
+        size_t blen = 0;
+        int rc = rpc_get_block(h, blk.data(), blk.size(), &blen);
+        if (rc != GARAGE_BM_OK) return rc;
+        SlotLease slot(stripe_slots);
+        uint8_t have[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
+        const size_t L = shard_len_of((uint32_t)blen);
+        for (int j = 0; j < k; j++) {
+            have[j] = 1;
+            uint8_t *row = slot.p + (size_t)j * slot_stride;
+            memset(row, 0, slot_stride);
+            const size_t off = (size_t)j * L;
+            if (off < blen) memcpy(row, blk.data() + off, std::min(L, blen - off));
+        }
+        rc = open_in_slot(h, key, slot.p, (uint32_t)blen, have, out, cap, out_len);
+        return rc == GARAGE_BM_E_CORRUPT_DATA ? GARAGE_BM_E_CORRUPT_DATA : rc;
     }
     // PUT during a layout change: one shard per (node, index) request of garage_layout_write_plan, and the write quorum
     // in the node set of every active version (try_write_many_sets, rpc_helper.rs:432-538)
@@ -2225,7 +2453,7 @@ struct garage_bm {
         return garage_quorum_tracker_state(t) == GARAGE_QUORUM_OK ? GARAGE_BM_OK : GARAGE_BM_E_QUORUM;
     }
 
-    // manager.rs:344-363 + 276-339.  `out` must hold block_size bytes; *out_len = the block's length.
+    // manager.rs:344-363 + 276-339.  `out` must hold stored_max() bytes (a sealed block_size block); *out_len = the block's length.
     int rpc_get_block(const Hash &h, uint8_t *out, size_t cap, size_t *out_len)
     {
         const int rc = get_from_stripe(h, out, cap, out_len, 0);
@@ -2292,7 +2520,7 @@ struct garage_bm {
             }
         }
         auto sliced = [&]() -> int {  // the whole block through rpc_get_block, then the range of it
-            std::vector<uint8_t> whole(cfg.block_size);
+            std::vector<uint8_t> whole(stored_max());
             size_t n = 0;
             const int rc = rpc_get_block(h, whole.data(), whole.size(), &n);
             if (rc != GARAGE_BM_OK) return rc;
@@ -3031,7 +3259,7 @@ struct garage_bm {
         std::lock_guard<std::mutex> cl(convert_mu);
         const size_t bmax = std::max<uint32_t>(cfg.batch_max_blocks, 1);
         const int nsrc = (int)codes.size() + (legacy_rf > 0 ? 1 : 0);  // source codes.size(): the replicas
-        const size_t rep_stride = garage_ec_stride_for(cfg.block_size);
+        const size_t rep_stride = garage_ec_stride_for(stored_max());
         const int quorum = garage_ec_write_quorum(k, m, GARAGE_CONSISTENT);
         uint8_t *blk = conv_blk.get(rep_stride);
         if (!blk) return 0;
@@ -3073,7 +3301,7 @@ struct garage_bm {
                     }
                     convert_bytes_read += nbytes;
                     lens[j] = len;
-                    got_src[j] = ok && len > 0 && len <= cfg.block_size;
+                    got_src[j] = ok && len > 0 && len <= stored_max();
                 });
                 // ... then the readable ones packed to the front
                 std::vector<size_t> which;  // batch position -> block
@@ -3114,7 +3342,7 @@ struct garage_bm {
                         size_t olen = 0;
                         uint32_t l32 = lens[q];
                         int32_t st = 0;
-                        if (get_from_stripe(h, blk, cfg.block_size, &olen, c) == GARAGE_BM_OK && olen == lens[q]) {
+                        if (get_from_stripe(h, blk, stored_max(), &olen, c) == GARAGE_BM_OK && olen == lens[q]) {
                             t0 = Clock::now();
                             rc = garage_ec_transcode(ec, nullptr, blk, nullptr, &l32, rep_stride, dst + q * tot * slot_stride,
                                                      slot_stride, sums + q * tot * 32, &st, 1, GARAGE_EC_MEM_HOST, nullptr);
@@ -3283,7 +3511,7 @@ struct garage_bm {
                 }
                 // the block is wrong: the GET path's hunt finds and quarantines the stale shard, if one set of k is
                 // consistent (the stripe's region of the batch buffer is free by now)
-                blk.resize(std::max<size_t>(cfg.block_size, lens[s]));
+                blk.resize(std::max<size_t>(stored_max(), lens[s]));
                 size_t out_len = 0;
                 if (hunt_stale_shard(h, buf + s * sbytes, blk.data(), blk.size(), &out_len, 0) == GARAGE_BM_OK) nrep++;
                 else deep_content_errors++;
@@ -3834,7 +4062,7 @@ struct garage_bm {
                     const int kind = items[c0 + i].second;
                     ReadResult r;
                     if (kind == Node::kReplicaFile) {  // a replica is checked against its content hash
-                        replica.resize(cfg.block_size);
+                        replica.resize(stored_max());
                         uint32_t len = 0;
                         r = nd.replica_read_into(h, replica.data(), replica.size(), len);
                         if (r == kReadMissing) continue;
@@ -4165,7 +4393,7 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg, const garage_
             c.quantum = 16u * (uint32_t)alpha;
         }
         // slots and the scrub buffer hold a shard of the largest code in play
-        bm->slot_stride = std::max(bm->slot_stride, garage_ec_stride_for((uint32_t)bm->shard_len_of(bm->cfg.block_size, i)));
+        bm->slot_stride = std::max(bm->slot_stride, garage_ec_stride_for((uint32_t)bm->shard_len_of(bm->stored_max(), i)));
     }
     if (lays->v.empty() && cfg->n_nodes <= GARAGE_LAYOUT_MAX_NODES) {
         const int n = cfg->n_nodes, tot = k + m;
@@ -4233,7 +4461,7 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg, const garage_
             std::vector<uint8_t> tmp(bm->slot_stride);
             for (const Hash &h : have) {
                 uint32_t len = 0;
-                if (nd.block_len_of(h, tmp, bm->cfg.block_size, bm->refs.count(h) != 0, len)) bm->refs[h] = len;
+                if (nd.block_len_of(h, tmp, bm->stored_max(), bm->refs.count(h) != 0, len)) bm->refs[h] = len;
             }
         }
     }
@@ -4365,6 +4593,31 @@ int garage_bm_rpc_get_block(garage_bm *bm, const uint8_t hash[32], uint8_t *out,
 {
     if (!bm || !hash || !out_len || !out) return GARAGE_EC_E_INVALID;
     BM_GUARD(bm->rpc_get_block(to_hash(hash), out, cap, out_len));
+}
+
+int garage_bm_rpc_put_block_sealed(garage_bm *bm, const uint8_t *key32, const uint8_t *data, size_t len, uint8_t hash_out[32])
+{
+    if (!bm || !hash_out || (!data && len)) return GARAGE_EC_E_INVALID;
+    BM_GUARD(bm->rpc_put_block_sealed(key32, data, len, hash_out));
+}
+
+int garage_bm_rpc_get_block_opened(garage_bm *bm, const uint8_t hash[32], const uint8_t *key32, uint8_t *out, size_t cap,
+                                   size_t *out_len)
+{
+    if (!bm || !hash || !key32 || !out || !out_len) return GARAGE_EC_E_INVALID;
+    BM_GUARD(bm->rpc_get_block_opened(to_hash(hash), key32, out, cap, out_len));
+}
+
+void garage_bm_get_sealed_metrics(garage_bm *bm, garage_bm_sealed_metrics *o)
+{
+    if (!bm || !o) return;
+    o->sealed_puts = bm->sealed_puts;
+    o->sealed_batches = bm->sealed_batches;
+    o->opened_gets = bm->opened_gets;
+    o->opened_auth_failures = bm->opened_auth_failures;
+    o->opened_fallbacks = bm->opened_fallbacks;
+    o->seal_call_us = bm->seal_call_us;
+    o->open_call_us = bm->open_call_us;
 }
 
 int garage_bm_rpc_get_block_range(garage_bm *bm, const uint8_t hash[32], uint32_t offset, uint32_t len, uint8_t *out,

@@ -30,6 +30,7 @@
 
 #include "rs_kernels.cuh"
 #include "clay_kernels.cuh"
+#include "sse_kernels.cuh"
 
 using namespace garage_ec;
 
@@ -48,6 +49,8 @@ struct HostLane {
     uint8_t *d_small = nullptr;  // shard_len / present / want / status / mismatch / plan
     size_t small_cap = 0;
     cudaEvent_t done = nullptr;  // blocking-sync event (garage_ec_set_wait_mode)
+    uint8_t *h_key = nullptr;    // pinned staging of SSE-C keys and nonces (zeroed once their upload completed)
+    size_t h_key_cap = 0;
 };
 // One HOST-mode call owns one set of lanes for its duration; concurrent callers (tokio
 // spawn_blocking threads, src/block/block.rs:86) get different sets, up to kMaxLaneSets.
@@ -798,6 +801,7 @@ public:
     static constexpr size_t kHostChunkBytes = 48ull << 20;  // target source bytes per chunk
     const size_t n, cs;
     CopyBatch up, down;  // the chunk being issued (or, in a retire step, the chunk being retired)
+    std::function<void()> before_release;  // runs once every lane stream is idle, before the set goes back to the pool
 
     HostPipeline(garage_ec_ctx *ctx, size_t n, size_t bytes_per_stripe)
         : n(n), cs(bytes_per_stripe ? std::min(std::max<size_t>(kHostChunkBytes / bytes_per_stripe, 1), n) : n),
@@ -812,6 +816,7 @@ public:
         for (HostLane &L : set_->lanes)
             if (L.stream) (void)cudaStreamSynchronize(L.stream);
         (void)cudaGetLastError();
+        if (before_release) before_release();  // the lanes are idle and still ours
         {
             std::lock_guard<std::mutex> lk(ctx_->pool_mu);
             ctx_->free_sets.push_back(set_);
@@ -985,6 +990,7 @@ const char *garage_ec_strerror(int code)
     case GARAGE_EC_E_UNRECOVERABLE: return "stripe unrecoverable: the present shards do not determine a wanted shard";
     case GARAGE_EC_E_NODEVICE: return "no usable sm_90 CUDA device (no CPU fallback)";
     case GARAGE_EC_E_ALIGN: return "pointer or stride not 16-byte aligned";
+    case GARAGE_EC_E_AUTH: return "block failed authentication (GCM tag or chunk framing)";
     default: return "unknown error";
     }
 }
@@ -1132,6 +1138,7 @@ void garage_ec_destroy(garage_ec_ctx *ctx)
             if (L.d_buf) cudaFree(L.d_buf);
             if (L.d_small) cudaFree(L.d_small);
             if (L.done) cudaEventDestroy(L.done);
+            if (L.h_key) cudaFreeHost(L.h_key);
         }
         delete set;
     }
@@ -2675,6 +2682,558 @@ int garage_ec_transcode(garage_ec_ctx *dst, garage_ec_ctx *src, uint8_t *src_sha
         return run_transcode(dst, src, src_shards, src_stride, src_present, block_len, dst_shards, dst_stride, dst_sums,
                              status, n_stripes, scratch, st);
     });
+}
+
+// --------------------------------------------------------------------------- SSE-C SEAL / OPEN (DESIGN.md 2.6, 4.9)
+}  // extern "C"
+namespace {
+
+// Device scratch of a seal or open of n blocks: key material | len(B) | L | (open) reconstruct status | want | plan.
+// The key material comes first so that one memset clears every secret.
+struct SseScratch {
+    size_t o_keys, o_blen, o_len, o_rec, o_want, o_plan, bytes;
+    SseScratch(const garage_ec_ctx *ctx, size_t n, bool open)
+    {
+        size_t b = 0;
+        auto take = [&](size_t x) {
+            const size_t o = b;
+            b += align_up(x, 256);
+            return o;
+        };
+        o_keys = take(n * sizeof(sse::SseKey));
+        o_blen = take(n * 4);
+        o_len = take(n * 4);
+        o_rec = open ? take(n * 4) : 0;
+        o_want = open ? take(n * (size_t)(ctx->k + ctx->m)) : 0;
+        o_plan = open ? take(plan_scratch_bytes(ctx, n)) : 0;
+        bytes = b;
+    }
+};
+
+int sse_launch_lens(garage_ec_ctx *ctx, const sse::LensParams &q, size_t n, cudaStream_t st)
+{
+    sse::sse_lens_kernel<<<(unsigned)std::min<size_t>((n + 255) / 256, (size_t)ctx->sm_count * 4), 256, 0, st>>>(q);
+    ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? GARAGE_EC_OK : set_cuda_error(ctx, e, "sse_lens_kernel launch");
+}
+
+int sse_launch_setup(garage_ec_ctx *ctx, const uint8_t *keys, sse::SseKey *ks, size_t n, cudaStream_t st)
+{
+    sse::SetupParams q;
+    q.keys = keys;
+    q.ks = ks;
+    q.n = (uint32_t)n;
+    sse::sse_setup_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(q);
+    ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? GARAGE_EC_OK : set_cuda_error(ctx, e, "sse_setup_kernel launch");
+}
+
+template <int MODE>
+int sse_launch_chunks(garage_ec_ctx *ctx, sse::ChunkParams q, cudaStream_t st)
+{
+    // work items are (block, chunk) pairs over the chunks a block of plain_stride bytes can have
+    q.cmax = (uint32_t)std::max<unsigned long long>(1, (q.plain_stride + sse::kChunk - 1) / sse::kChunk);
+    const unsigned long long items = (unsigned long long)q.n * q.cmax;
+    const unsigned grid = (unsigned)std::min<unsigned long long>((items + sse::kWarps - 1) / sse::kWarps,
+                                                                 (unsigned long long)ctx->sm_count * 4);
+    TimedLaunch tl(ctx, st);
+    sse::sse_chunk_kernel<MODE><<<grid, sse::kWarps * 32, 0, st>>>(q);
+    ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? GARAGE_EC_OK : set_cuda_error(ctx, e, "sse_chunk_kernel launch");
+}
+
+int sse_launch_block_sums(garage_ec_ctx *ctx, const uint8_t *shards, const uint32_t *blen, const uint8_t *hashes,
+                          uint8_t *hash_bad, uint8_t *digest, size_t stride, size_t n, cudaStream_t st)
+{
+    BlockSumParams q;
+    memset(&q, 0, sizeof(q));
+    q.shards = shards;
+    q.block_len = blen;
+    q.hashes = hashes;
+    q.hash_bad = hash_bad;
+    q.digest = digest;
+    q.stride = (uint32_t)stride;
+    q.k = (uint32_t)ctx->k;
+    q.m = (uint32_t)ctx->m;
+    q.n = (uint32_t)n;
+    q.quantum = ctx->quantum;
+    blake2sum_blocks_kernel<<<(unsigned)((n + kQuadThreads / 4 - 1) / (kQuadThreads / 4)), kQuadThreads, 0, st>>>(q);
+    ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? GARAGE_EC_OK : set_cuda_error(ctx, e, "blake2sum_blocks_kernel launch");
+}
+
+// Seal n blocks on the device: lengths, key schedules, the GCM chunks into the data shards, the code's encode, the
+// content hash and (sums != NULL) the shard tags.  The caller zeroes the key material of `scratch`.
+int run_seal(garage_ec_ctx *ctx, const uint8_t *plain, size_t plain_stride, const uint32_t *plain_len,
+             const uint8_t *keys, const uint8_t *nonces, uint8_t *shards, size_t stride, uint8_t *hashes, uint8_t *sums,
+             size_t n, uint8_t *scratch, cudaStream_t st)
+{
+    const SseScratch sc(ctx, n, false);
+    sse::SseKey *ks = keys ? reinterpret_cast<sse::SseKey *>(scratch + sc.o_keys) : nullptr;
+    uint32_t *blen = reinterpret_cast<uint32_t *>(scratch + sc.o_blen), *L = reinterpret_cast<uint32_t *>(scratch + sc.o_len);
+    const size_t tot = ctx->k + ctx->m;
+    sse::LensParams lp;
+    memset(&lp, 0, sizeof(lp));
+    lp.plain_len = plain_len;
+    lp.blen = blen;
+    lp.shard_len = L;
+    lp.plain_stride = plain_stride;
+    lp.stride = (uint32_t)stride;
+    lp.k = (uint32_t)ctx->k;
+    lp.m = (uint32_t)ctx->m;
+    lp.n = (uint32_t)n;
+    lp.quantum = ctx->quantum;
+    lp.keyed = keys ? 1u : 0u;
+    int rc = sse_launch_lens(ctx, lp, n, st);
+    if (!rc && keys) rc = sse_launch_setup(ctx, keys, ks, n, st);
+    if (rc) return rc;
+    sse::ChunkParams q;
+    memset(&q, 0, sizeof(q));
+    q.plain_in = plain;
+    q.plain_stride = plain_stride;
+    q.plain_len = plain_len;
+    q.blen = blen;
+    q.shard_len = L;
+    q.nonces = nonces;
+    q.ks = ks;
+    q.shards = shards;
+    q.stride = (uint32_t)stride;
+    q.k = (uint32_t)ctx->k;
+    q.m = (uint32_t)ctx->m;
+    q.n = (uint32_t)n;
+    rc = sse_launch_chunks<sse::kSeal>(ctx, q, st);
+    if (!rc)
+        rc = run_uniform(ctx, kModeEncode, shards, tot * stride, shards + (size_t)ctx->k * stride, tot * stride, nullptr, L,
+                         stride, n, st);
+    if (!rc) rc = sse_launch_block_sums(ctx, shards, blen, nullptr, nullptr, hashes, stride, n, st);
+    if (!rc && sums) rc = run_sums(ctx, shards, nullptr, L, stride, n * tot, (int)tot, sums, nullptr, st);
+    return rc;
+}
+
+// Open n stored blocks on the device: framing, key schedules, the rebuild of absent data shards, the content hash,
+// every chunk's tag, then the plaintext of the blocks that passed.
+int run_open(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *present, const uint32_t *sealed, const uint8_t *hashes,
+             const uint8_t *keys, uint8_t *plain, size_t plain_stride, uint32_t *plain_len_out, uint8_t *hash_bad,
+             int32_t *status, size_t stride, size_t n, uint8_t *scratch, cudaStream_t st)
+{
+    const SseScratch sc(ctx, n, true);
+    sse::SseKey *ks = reinterpret_cast<sse::SseKey *>(scratch + sc.o_keys);
+    uint32_t *L = reinterpret_cast<uint32_t *>(scratch + sc.o_len);
+    int32_t *rec = reinterpret_cast<int32_t *>(scratch + sc.o_rec);
+    uint8_t *want = scratch + sc.o_want;
+    sse::LensParams lp;
+    memset(&lp, 0, sizeof(lp));
+    lp.sealed_in = sealed;
+    lp.shard_len = L;
+    lp.status = status;
+    lp.want = want;
+    lp.plain_stride = plain_stride;
+    lp.stride = (uint32_t)stride;
+    lp.k = (uint32_t)ctx->k;
+    lp.m = (uint32_t)ctx->m;
+    lp.n = (uint32_t)n;
+    lp.quantum = ctx->quantum;
+    lp.keyed = 1;
+    lp.open = 1;
+    int rc = sse_launch_lens(ctx, lp, n, st);
+    if (!rc) rc = sse_launch_setup(ctx, keys, ks, n, st);
+    if (!rc) rc = run_reconstruct(ctx, shards, present, want, rec, L, stride, n, scratch + sc.o_plan, st);
+    if (!rc) rc = sse_launch_block_sums(ctx, shards, sealed, hashes, hash_bad, nullptr, stride, n, st);
+    if (rc) return rc;
+    sse::ChunkParams q;
+    memset(&q, 0, sizeof(q));
+    q.plain_out = plain;
+    q.plain_stride = plain_stride;
+    q.plain_len_out = plain_len_out;
+    q.blen = sealed;
+    q.shard_len = L;
+    q.ks = ks;
+    q.shards = shards;
+    q.status = status;
+    q.rec_status = rec;
+    q.hash_bad = hash_bad;
+    q.stride = (uint32_t)stride;
+    q.k = (uint32_t)ctx->k;
+    q.m = (uint32_t)ctx->m;
+    q.n = (uint32_t)n;
+    rc = sse_launch_chunks<sse::kCheck>(ctx, q, st);
+    if (!rc) rc = sse_launch_chunks<sse::kOpen>(ctx, q, st);
+    return rc;
+}
+
+// plaintext length of a sealed length, or -1 if the STREAM framing cannot hold it
+int64_t sse_plain_len(uint32_t sealed)
+{
+    if (sealed < sse::kPrefix + 16) return -1;
+    const uint32_t r = (sealed - sse::kPrefix) % sse::kFrame;
+    if (r >= 1 && r < 16) return -1;
+    return (int64_t)sealed - sse::kPrefix - 16 * (int64_t)((sealed - sse::kPrefix + sse::kFrame - 1) / sse::kFrame);
+}
+
+// a lane's pinned key staging of at least `bytes`
+int lane_key_staging(garage_ec_ctx *ctx, HostLane &L, size_t bytes)
+{
+    if (L.h_key_cap >= bytes) return GARAGE_EC_OK;
+    if (L.h_key) cudaFreeHost(L.h_key);
+    L.h_key = nullptr;
+    L.h_key_cap = 0;
+    bytes = std::max<size_t>(bytes, 64 << 10);
+    CU_TRY(ctx, cudaHostAlloc(reinterpret_cast<void **>(&L.h_key), bytes, cudaHostAllocDefault));
+    memset(L.h_key, 0, bytes);
+    L.h_key_cap = bytes;
+    return GARAGE_EC_OK;
+}
+
+// Clears the secrets a HOST call left in its lanes once nothing queued reads them any more and before another call
+// can lease the lanes: wipe() is the call's HostPipeline::before_release.  `dev_off` / `dev_bytes`: the keys, nonces
+// and key material in each lane's small buffer (already cleared on the stream unless the call failed half-way).
+struct LaneKeyWipe {
+    std::vector<HostLane *> lanes;
+    size_t dev_off = 0, dev_bytes = 0;
+    bool failed = true;
+    void use(HostLane *L)
+    {
+        if (std::find(lanes.begin(), lanes.end(), L) == lanes.end()) lanes.push_back(L);
+    }
+    void wipe()
+    {
+        for (HostLane *L : lanes) {
+            if (L->h_key) memset(L->h_key, 0, L->h_key_cap);
+            if (failed && L->d_small && dev_bytes) (void)cudaMemset(L->d_small + dev_off, 0, dev_bytes);
+        }
+        (void)cudaGetLastError();
+    }
+};
+
+int seal_host(garage_ec_ctx *ctx, const uint8_t *plain, size_t plain_stride, const uint8_t *const *blocks,
+              const uint32_t *plain_len, const uint8_t *keys, const uint8_t *nonces, uint8_t *shards, size_t stride,
+              uint8_t *hashes, uint8_t *sums, size_t n)
+{
+    const size_t tot = ctx->k + ctx->m;
+    auto block_at = [&](size_t s) { return blocks ? blocks[s] : plain + s * plain_stride; };
+    uint32_t max_len = 0;
+    for (size_t s = 0; s < n; s++) max_len = std::max(max_len, plain_len[s]);
+    const size_t pitch = align_up((size_t)max_len + 16, 16);
+    LaneKeyWipe wipe;
+    HostPipeline p(ctx, n, pitch + tot * stride);
+    p.before_release = [&wipe] { wipe.wipe(); };
+    const size_t cs = p.cs;
+    SmallLayout sl;
+    const SseScratch sc(ctx, cs, false);
+    const size_t o_scr = sl.take(sc.bytes), o_key = sl.take(cs * 40), o_len = sl.take(cs * 4), o_hash = sl.take(cs * 32),
+                 o_sums = sl.take(sums ? cs * tot * 32 : 0);
+    wipe.dev_off = o_scr;
+    wipe.dev_bytes = o_len - o_scr;  // key material, keys and nonces
+    const size_t blk_b = align_up(cs * pitch, 256);
+    int rc = p.reserve(blk_b + cs * tot * stride, sl.bytes);
+    if (rc) return rc;
+    // batched copies for pinned buffers only, as in reconstruct_host
+    bool pinned = true;
+    for (size_t s = 0; pinned && s < (blocks ? n : 1); s++) pinned = !plain_len[s] || device_addressable_host(block_at(s));
+    p.up.use_batch = pinned;
+    p.down.use_batch = device_addressable_host(shards);
+    const Retire clear_keys = [&](const HostChunk &ch) -> int {
+        memset(ch.L->h_key, 0, ch.L->h_key_cap);
+        return GARAGE_EC_OK;
+    };
+    rc = p.run(
+        [&](const HostChunk &ch) -> int {
+            HostLane &L = *ch.L;
+            wipe.use(&L);
+            const size_t s0 = ch.s0, cnt = ch.cnt;
+            uint8_t *d_blk = L.d_buf, *d_sh = L.d_buf + blk_b;
+            for (size_t q = 0; q < cnt; q++) p.up.add(d_blk + q * pitch, block_at(s0 + q), plain_len[s0 + q]);
+            int r = p.up.flush(ctx, cudaMemcpyHostToDevice, L.stream);
+            if (r) return r;
+            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_len, plain_len + s0, cnt * 4, cudaMemcpyHostToDevice, L.stream));
+            const uint8_t *d_keys = nullptr, *d_nonces = nullptr;
+            if (keys) {
+                r = lane_key_staging(ctx, L, cs * 40);
+                if (r) return r;
+                memcpy(L.h_key, keys + s0 * 32, cnt * 32);
+                memcpy(L.h_key + cs * 32, nonces + s0 * 8, cnt * 8);
+                CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_key, L.h_key, cs * 40, cudaMemcpyHostToDevice, L.stream));
+                d_keys = L.d_small + o_key;
+                d_nonces = L.d_small + o_key + cs * 32;
+            }
+            r = run_seal(ctx, d_blk, pitch, reinterpret_cast<const uint32_t *>(L.d_small + o_len), d_keys, d_nonces, d_sh,
+                         stride, L.d_small + o_hash, sums ? L.d_small + o_sums : nullptr, cnt, L.d_small + o_scr, L.stream);
+            if (r) return r;
+            if (keys) CU_TRY(ctx, cudaMemsetAsync(L.d_small + o_scr, 0, o_len - o_scr, L.stream));
+            // D2H: roundup16(L) bytes of all k+m shards (the data shards are ciphertext now)
+            for (size_t q = 0; q < cnt; q++) {
+                const uint64_t b = keys ? sse::sealed_len(plain_len[s0 + q]) : plain_len[s0 + q];
+                const size_t bytes = align_up(code_shard_len(ctx, (uint32_t)b), 16);
+                for (size_t i = 0; i < tot; i++)
+                    p.down.add(shards + ((s0 + q) * tot + i) * stride, d_sh + (q * tot + i) * stride, bytes);
+            }
+            r = p.down.flush(ctx, cudaMemcpyDeviceToHost, L.stream);
+            if (r) return r;
+            CU_TRY(ctx, cudaMemcpyAsync(hashes + s0 * 32, L.d_small + o_hash, cnt * 32, cudaMemcpyDeviceToHost, L.stream));
+            if (sums)
+                CU_TRY(ctx, cudaMemcpyAsync(sums + s0 * tot * 32, L.d_small + o_sums, cnt * tot * 32, cudaMemcpyDeviceToHost,
+                                            L.stream));
+            return GARAGE_EC_OK;
+        },
+        keys ? clear_keys : Retire());
+    if (!rc) rc = p.drain(keys ? clear_keys : Retire());
+    wipe.failed = rc != 0;
+    return rc;
+}
+
+int open_host(garage_ec_ctx *ctx, uint8_t *shards, uint8_t *const *stripes, const uint8_t *present,
+              const uint32_t *sealed, const uint8_t *hashes, const uint8_t *keys, uint8_t *plain, size_t plain_stride,
+              uint8_t *const *outs, uint32_t *plain_len_out, uint8_t *hash_bad, int32_t *status, size_t stride, size_t n)
+{
+    const size_t k = ctx->k, tot = ctx->k + ctx->m;
+    auto shard_at = [&](size_t s, size_t i) { return stripes ? stripes[s] + i * stride : shards + (s * tot + i) * stride; };
+    auto out_at = [&](size_t s) { return outs ? outs[s] : plain + s * plain_stride; };
+    int64_t max_plain = 0;
+    for (size_t s = 0; s < n; s++) max_plain = std::max(max_plain, sse_plain_len(sealed[s]));
+    const size_t pitch = align_up((size_t)max_plain + 16, 16);
+    std::vector<uint8_t> want(tot);
+    for (size_t i = 0; i < tot; i++) want[i] = i < k;
+    LaneKeyWipe wipe;
+    HostPipeline p(ctx, n, tot * stride + pitch);
+    p.before_release = [&wipe] { wipe.wipe(); };
+    const size_t cs = p.cs;
+    SmallLayout sl;
+    const SseScratch sc(ctx, cs, true);
+    const size_t o_scr = sl.take(sc.bytes), o_key = sl.take(cs * 32), o_present = sl.take(cs * tot),
+                 o_sealed = sl.take(cs * 4), o_hash = sl.take(cs * 32), o_bad = sl.take(cs), o_status = sl.take(cs * 4),
+                 o_plen = sl.take(cs * 4);
+    wipe.dev_off = o_scr;
+    wipe.dev_bytes = o_key + cs * 32 - o_scr;
+    const size_t sh_b = align_up(cs * tot * stride, 256);
+    int rc = p.reserve(sh_b + cs * pitch, sl.bytes, cs * 4);
+    if (rc) return rc;
+    bool pinned = true;
+    for (size_t s = 0; pinned && s < (stripes ? n : 1); s++) pinned = device_addressable_host(shard_at(s, 0));
+    for (size_t s = 0; pinned && s < (outs ? n : 1); s++) pinned = device_addressable_host(out_at(s));
+    p.up.use_batch = p.down.use_batch = pinned;
+    const Retire retire = [&](const HostChunk &ch) -> int {
+        memset(ch.L->h_key, 0, ch.L->h_key_cap);
+        const uint32_t *plen = reinterpret_cast<const uint32_t *>(ch.host);
+        for (size_t q = 0; q < ch.cnt; q++) {
+            const size_t s = ch.s0 + q;
+            if (status[s] || hash_bad[s]) continue;
+            plain_len_out[s] = plen[q];
+            p.down.add(out_at(s), ch.L->d_buf + sh_b + q * pitch, plen[q]);
+        }
+        int r = p.down.flush(ctx, cudaMemcpyDeviceToHost, ch.L->stream);
+        if (r) return r;
+        CU_TRY(ctx, lane_wait(ctx, *ch.L));
+        return GARAGE_EC_OK;
+    };
+    rc = p.run(
+        [&](const HostChunk &ch) -> int {
+            HostLane &L = *ch.L;
+            wipe.use(&L);
+            const size_t s0 = ch.s0, cnt = ch.cnt;
+            uint8_t *d_sh = L.d_buf;
+            // H2D: the present data shards (the block's bytes) and what the code's plan reads to rebuild the others
+            for (size_t s = s0; s < s0 + cnt; s++) {
+                uint64_t hv = 0;
+                const uint8_t *pr = present + s * tot;
+                const size_t len = code_shard_len(ctx, sealed[s]);
+                const bool ok = stripe_read_plan(ctx, pr, want.data(), &hv);
+                for (size_t i = 0; i < tot; i++) {
+                    uint8_t *d = d_sh + ((s - s0) * tot + i) * stride;
+                    if (i < k && pr[i]) p.up.add(d, shard_at(s, i), align_up(len, 16));
+                    else if (ok && i >= k)
+                        for_each_read_piece(ctx, hv, i, len, align_up(len, 16),
+                                            [&](size_t off, size_t bytes) { p.up.add(d + off, shard_at(s, i) + off, bytes); });
+                }
+            }
+            int r = p.up.flush(ctx, cudaMemcpyHostToDevice, L.stream);
+            if (r) return r;
+            r = lane_key_staging(ctx, L, cs * 32);
+            if (r) return r;
+            memcpy(L.h_key, keys + s0 * 32, cnt * 32);
+            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_key, L.h_key, cnt * 32, cudaMemcpyHostToDevice, L.stream));
+            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_present, present + s0 * tot, cnt * tot, cudaMemcpyHostToDevice, L.stream));
+            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_sealed, sealed + s0, cnt * 4, cudaMemcpyHostToDevice, L.stream));
+            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_hash, hashes + s0 * 32, cnt * 32, cudaMemcpyHostToDevice, L.stream));
+            int32_t *d_status = reinterpret_cast<int32_t *>(L.d_small + o_status);
+            r = run_open(ctx, d_sh, L.d_small + o_present, reinterpret_cast<const uint32_t *>(L.d_small + o_sealed),
+                         L.d_small + o_hash, L.d_small + o_key, d_sh + sh_b, pitch,
+                         reinterpret_cast<uint32_t *>(L.d_small + o_plen), L.d_small + o_bad, d_status, stride, cnt,
+                         L.d_small + o_scr, L.stream);
+            if (r) return r;
+            CU_TRY(ctx, cudaMemsetAsync(L.d_small + o_scr, 0, wipe.dev_bytes, L.stream));
+            CU_TRY(ctx, cudaMemcpyAsync(status + s0, d_status, cnt * 4, cudaMemcpyDeviceToHost, L.stream));
+            CU_TRY(ctx, cudaMemcpyAsync(hash_bad + s0, L.d_small + o_bad, cnt, cudaMemcpyDeviceToHost, L.stream));
+            CU_TRY(ctx, cudaMemcpyAsync(ch.host, L.d_small + o_plen, cnt * 4, cudaMemcpyDeviceToHost, L.stream));
+            return GARAGE_EC_OK;
+        },
+        retire);
+    if (!rc) rc = p.drain(retire);
+    wipe.failed = rc != 0;
+    if (rc) return rc;
+    int worst = GARAGE_EC_OK;
+    for (size_t s = 0; s < n; s++) {
+        if (status[s] == GARAGE_EC_E_UNRECOVERABLE) return GARAGE_EC_E_UNRECOVERABLE;
+        if (status[s]) worst = status[s];
+    }
+    return worst;
+}
+
+// checks shared by every seal form; plain_len values are host memory (HOST) or not looked at (DEVICE)
+int seal_args(garage_ec_ctx *ctx, const uint8_t *keys, const uint8_t *nonces, const uint8_t *shards, size_t stride,
+              const uint8_t *hashes, const uint8_t *sums, size_t n)
+{
+    if (!ctx) return GARAGE_EC_E_INVALID;
+    int rc = check_geometry(ctx, stride, n, ctx->k + ctx->m);
+    if (rc) return rc;
+    if (n == 0) return GARAGE_EC_OK;
+    if (!shards || !hashes || (!keys) != (!nonces)) return GARAGE_EC_E_INVALID;
+    if (sums && n * (size_t)(ctx->k + ctx->m) > 0xffffffffull) return GARAGE_EC_E_INVALID;
+    if (!aligned16(shards)) return GARAGE_EC_E_ALIGN;
+    return GARAGE_EC_OK;
+}
+
+// HOST: every block's shard length must fit the stride
+int seal_host_lens_ok(garage_ec_ctx *ctx, const uint32_t *plain_len, bool keyed, size_t stride, size_t n)
+{
+    for (size_t s = 0; s < n; s++) {
+        const uint64_t b = keyed ? sse::sealed_len(plain_len[s]) : plain_len[s];
+        if (b > 0xffffffffull || code_shard_len(ctx, (uint32_t)b) > stride) return GARAGE_EC_E_INVALID;
+    }
+    return GARAGE_EC_OK;
+}
+
+}  // namespace
+extern "C" {
+
+int garage_ec_sealed_len(uint32_t plain_len, uint32_t *sealed_len)
+{
+    if (!sealed_len) return GARAGE_EC_E_INVALID;
+    const uint64_t b = sse::sealed_len(plain_len);
+    if (b > 0xffffffffull) return GARAGE_EC_E_INVALID;
+    *sealed_len = (uint32_t)b;
+    return GARAGE_EC_OK;
+}
+
+int garage_ec_seal(garage_ec_ctx *ctx, const uint8_t *plain, size_t plain_stride, const uint32_t *plain_len,
+                   const uint8_t *keys, const uint8_t *nonces, uint8_t *shards, size_t stride, uint8_t *hashes,
+                   uint8_t *sums, size_t n, int mem_kind, void *cuda_stream)
+{
+    if (mem_kind != GARAGE_EC_MEM_HOST && mem_kind != GARAGE_EC_MEM_DEVICE) return GARAGE_EC_E_INVALID;
+    int rc = seal_args(ctx, keys, nonces, shards, stride, hashes, sums, n);
+    if (rc || n == 0) return rc;
+    if (!plain || !plain_len || (plain_stride & 15)) return GARAGE_EC_E_INVALID;
+    if (!aligned16(plain)) return GARAGE_EC_E_ALIGN;
+    if (mem_kind == GARAGE_EC_MEM_HOST) {
+        for (size_t s = 0; s < n; s++)
+            if (plain_len[s] > plain_stride) return GARAGE_EC_E_INVALID;
+        rc = seal_host_lens_ok(ctx, plain_len, keys != nullptr, stride, n);
+        if (rc) return rc;
+        CU_TRY(ctx, cudaSetDevice(ctx->device));
+        return seal_host(ctx, plain, plain_stride, nullptr, plain_len, keys, nonces, shards, stride, hashes, sums, n);
+    }
+    if ((reinterpret_cast<uintptr_t>(plain_len) & 3) || (reinterpret_cast<uintptr_t>(hashes) & 7) ||
+        (reinterpret_cast<uintptr_t>(sums) & 7))
+        return GARAGE_EC_E_ALIGN;
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    const SseScratch sc(ctx, n, false);
+    return with_stream_scratch(ctx, sc.bytes, st, [&](uint8_t *scratch) {
+        const int r = run_seal(ctx, plain, plain_stride, plain_len, keys, nonces, shards, stride, hashes, sums, n, scratch, st);
+        const cudaError_t e = keys ? cudaMemsetAsync(scratch + sc.o_keys, 0, n * sizeof(sse::SseKey), st) : cudaSuccess;
+        if (r) return r;
+        return e == cudaSuccess ? GARAGE_EC_OK : set_cuda_error(ctx, e, "cudaMemsetAsync(key material)");
+    });
+}
+
+int garage_ec_seal_blocks(garage_ec_ctx *ctx, const uint8_t *const *blocks, const uint32_t *plain_len, const uint8_t *keys,
+                          const uint8_t *nonces, uint8_t *shards, size_t stride, uint8_t *hashes, uint8_t *sums, size_t n)
+{
+    int rc = seal_args(ctx, keys, nonces, shards, stride, hashes, sums, n);
+    if (rc || n == 0) return rc;
+    if (!blocks || !plain_len) return GARAGE_EC_E_INVALID;
+    for (size_t s = 0; s < n; s++)
+        if (!blocks[s] && plain_len[s]) return GARAGE_EC_E_INVALID;
+    rc = seal_host_lens_ok(ctx, plain_len, keys != nullptr, stride, n);
+    if (rc) return rc;
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    return seal_host(ctx, nullptr, 0, blocks, plain_len, keys, nonces, shards, stride, hashes, sums, n);
+}
+
+static int open_args(garage_ec_ctx *ctx, const void *shards, const uint8_t *present, const uint32_t *sealed,
+                     const uint8_t *hashes, const uint8_t *keys, const uint32_t *plain_len_out, const uint8_t *hash_bad,
+                     const int32_t *status, size_t stride, size_t n)
+{
+    if (!ctx) return GARAGE_EC_E_INVALID;
+    int rc = check_geometry(ctx, stride, n, ctx->k + ctx->m);
+    if (rc) return rc;
+    if (n == 0) return GARAGE_EC_OK;
+    if (!shards || !present || !sealed || !hashes || !keys || !plain_len_out || !hash_bad || !status)
+        return GARAGE_EC_E_INVALID;
+    return GARAGE_EC_OK;
+}
+
+// HOST: a stored block whose shard length does not fit the stride is a caller error, not a verdict on the data
+static int open_host_lens_ok(garage_ec_ctx *ctx, const uint32_t *sealed, size_t stride, size_t n)
+{
+    for (size_t s = 0; s < n; s++)
+        if (code_shard_len(ctx, sealed[s]) > stride) return GARAGE_EC_E_INVALID;
+    return GARAGE_EC_OK;
+}
+
+int garage_ec_open(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *present, const uint32_t *sealed_len,
+                   const uint8_t *hashes, const uint8_t *keys, uint8_t *plain, size_t plain_stride,
+                   uint32_t *plain_len_out, uint8_t *hash_bad, int32_t *status, size_t stride, size_t n, int mem_kind,
+                   void *cuda_stream)
+{
+    if (mem_kind != GARAGE_EC_MEM_HOST && mem_kind != GARAGE_EC_MEM_DEVICE) return GARAGE_EC_E_INVALID;
+    int rc = open_args(ctx, shards, present, sealed_len, hashes, keys, plain_len_out, hash_bad, status, stride, n);
+    if (rc || n == 0) return rc;
+    if (!plain || (plain_stride & 15)) return GARAGE_EC_E_INVALID;
+    if (!aligned16(shards) || !aligned16(plain)) return GARAGE_EC_E_ALIGN;
+    if (mem_kind == GARAGE_EC_MEM_HOST) {
+        rc = open_host_lens_ok(ctx, sealed_len, stride, n);
+        if (rc) return rc;
+        for (size_t s = 0; s < n; s++)
+            if (sse_plain_len(sealed_len[s]) > (int64_t)plain_stride) return GARAGE_EC_E_INVALID;
+        CU_TRY(ctx, cudaSetDevice(ctx->device));
+        return open_host(ctx, shards, nullptr, present, sealed_len, hashes, keys, plain, plain_stride, nullptr,
+                         plain_len_out, hash_bad, status, stride, n);
+    }
+    if ((reinterpret_cast<uintptr_t>(sealed_len) & 3) || (reinterpret_cast<uintptr_t>(hashes) & 7) ||
+        (reinterpret_cast<uintptr_t>(plain_len_out) & 3) || (reinterpret_cast<uintptr_t>(status) & 3))
+        return GARAGE_EC_E_ALIGN;
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    const SseScratch sc(ctx, n, true);
+    return with_stream_scratch(ctx, sc.bytes, st, [&](uint8_t *scratch) {
+        const int r = run_open(ctx, shards, present, sealed_len, hashes, keys, plain, plain_stride, plain_len_out, hash_bad,
+                               status, stride, n, scratch, st);
+        const cudaError_t e = cudaMemsetAsync(scratch + sc.o_keys, 0, n * sizeof(sse::SseKey), st);
+        if (r) return r;
+        return e == cudaSuccess ? GARAGE_EC_OK : set_cuda_error(ctx, e, "cudaMemsetAsync(key material)");
+    });
+}
+
+int garage_ec_open_stripes(garage_ec_ctx *ctx, uint8_t *const *stripes, const uint8_t *present, const uint32_t *sealed_len,
+                           const uint8_t *hashes, const uint8_t *keys, uint8_t *const *plains, uint32_t *plain_len_out,
+                           uint8_t *hash_bad, int32_t *status, size_t stride, size_t n)
+{
+    int rc = open_args(ctx, stripes, present, sealed_len, hashes, keys, plain_len_out, hash_bad, status, stride, n);
+    if (rc || n == 0) return rc;
+    if (!plains) return GARAGE_EC_E_INVALID;
+    for (size_t s = 0; s < n; s++) {
+        if (!stripes[s] || !plains[s]) return GARAGE_EC_E_INVALID;
+        if (!aligned16(stripes[s])) return GARAGE_EC_E_ALIGN;
+    }
+    rc = open_host_lens_ok(ctx, sealed_len, stride, n);
+    if (rc) return rc;
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    return open_host(ctx, nullptr, stripes, present, sealed_len, hashes, keys, nullptr, 0, plains, plain_len_out,
+                     hash_bad, status, stride, n);
 }
 
 // ---- test hook -------------------------------------------------------------------------------

@@ -1842,6 +1842,8 @@ struct BlockSumParams {
     uint8_t *hash_bad;            // out: 1 iff the block's blake2sum differs from hashes[s]
     uint32_t *shard_len;          // out: L, or 0 for a stripe whose L does not fit its stride
     uint32_t *mismatch;           // out: 0, or every parity bit for such a stripe (the verify launch ORs into it)
+    uint8_t *digest;              // out, nullable: 32 bytes per stripe, the block's blake2sum (hashes, hash_bad,
+                                  // shard_len and mismatch are then nullable too)
     uint32_t stride, k, m, n, quantum;
 };
 
@@ -1894,12 +1896,12 @@ __global__ void __launch_bounds__(kQuadThreads) blake2sum_blocks_kernel(const __
     const uint64_t L64 = code_shard_len(len, (int)q.k, q.quantum);
     const bool bad_geo = L64 > q.stride;  // DEVICE mode reports it; nothing of the stripe is read
     const uint32_t L = bad_geo ? 0u : (uint32_t)L64;
-    if (c == 0) {
+    if (c == 0 && q.shard_len) {
         q.shard_len[s] = L;
         q.mismatch[s] = bad_geo ? (1u << q.m) - 1 : 0u;
     }
     if (bad_geo) {
-        if (c == 0) q.hash_bad[s] = 1;
+        if (c == 0 && q.hash_bad) q.hash_bad[s] = 1;
         return;
     }
     const uint8_t *stripe = q.shards + (size_t)s * (q.k + q.m) * q.stride;
@@ -1922,6 +1924,8 @@ __global__ void __launch_bounds__(kQuadThreads) blake2sum_blocks_kernel(const __
         y = block_vec16(stripe, q.stride, L, j, off, ny);
     };
     const uint64_t h0 = blake2b_quad(len, &s_msg[tid >> 2][0], load32);
+    if (q.digest) *reinterpret_cast<unsigned long long *>(q.digest + (size_t)s * 32 + 8 * c) = h0;
+    if (!q.hashes) return;
     const unsigned long long e = *reinterpret_cast<const unsigned long long *>(q.hashes + (size_t)s * 32 + 8 * c);
     const uint32_t diff = __ballot_sync(qmask, e != h0) & qmask;
     if (c == 0) q.hash_bad[s] = diff ? 1 : 0;

@@ -1,0 +1,547 @@
+// sse_kernels.cuh -- SSE-C blocks on the device (DESIGN.md sections 2.6 and 4.9): AES-256-GCM in the STREAM-LE31
+// chunk framing of Garage's EncryptionParams::encrypt_block, written straight into and read straight out of the
+// shard layout.
+//
+// A plain block P of len bytes, key K, 8-byte nonce prefix N:  B = N || C_0 || ... || C_{n-1}, n = max(1,
+// ceil(len / 4096)), C_c = AES-256-GCM(K, N || LE32(c | (c == n-1) << 31), P[4096c, 4096c + 4096)) = ciphertext ||
+// 16-byte tag.  Chunk c starts at byte 8 + 4112c of B, 8 bytes off a 16-byte boundary, and B is cut into data shards
+// of L bytes (data shard j = B[jL, (j+1)L)), so chunks straddle shards at arbitrary offsets.
+//
+// One warp per chunk.  The warp stages its chunk's bytes of B in shared memory: seal writes ciphertext and tag there
+// and then stores them to the shard layout with 16-byte stores aligned in shard space (bytes a vector shares with
+// the neighbouring chunk are stored one by one, so two warps never write the same byte); open loads the chunk's
+// bytes of every shard it touches with aligned 16-byte loads.  No pass over HBM stages B anywhere else.
+//
+// GHASH is split across the lanes: the chunk's nb data blocks are right-aligned in 256 slots, lane l runs Horner's
+// rule (4-bit tables of H) over slots [8l, 8l+8), and its partial sum is multiplied by H^(8(31-l)) -- the same power
+// for every chunk length, precomputed per key -- before a warp reduction.  Open checks every tag in one launch and
+// decrypts in a second one, so that no plaintext of a block is written unless all of its tags passed.
+#pragma once
+
+#include <stdint.h>
+
+namespace garage_ec {
+namespace sse {
+
+constexpr uint32_t kChunk = 4096;          // STREAM_ENC_PLAIN_CHUNK_SIZE
+constexpr uint32_t kFrame = kChunk + 16;   // one sealed chunk: ciphertext + tag
+constexpr uint32_t kPrefix = 8;            // the nonce prefix at the head of B
+constexpr int kWarps = 8;                  // warps per CTA of the chunk kernel
+constexpr uint32_t kStage = kFrame + kPrefix + 24;  // per-warp staging: [0, 8) nonce, [8, 8 + 4112) chunk, slack
+
+// sealed length of a len-byte block (64-bit: the caller checks it fits 32 bits)
+__host__ __device__ inline uint64_t sealed_len(uint64_t len)
+{
+    const uint64_t n = len ? (len + kChunk - 1) / kChunk : 1;
+    return kPrefix + len + 16 * n;
+}
+
+// Per-key material, built by sse_setup_kernel: the AES-256 round keys (FIPS-197 5.2), the 4-bit multiplication
+// table of H = E_K(0^128) and H^(8(31-l)) for lane l.  Secret: zeroed on the stream after the call's last kernel.
+struct SseKey {
+    uint32_t rk[60];
+    uint32_t pad[4];
+    unsigned long long hh[16], hl[16];   // i * H, GCM bit order (hi, lo words big-endian)
+    unsigned long long pw[32][2];        // lane powers
+};
+static_assert(sizeof(SseKey) == 1024, "SseKey layout");
+
+struct SseTables {
+    uint32_t te[4][256];
+    uint8_t sbox[256];
+    uint32_t r4[16];   // reduction of the four bits a 4-bit shift drops (Shoup's table)
+};
+
+__device__ __forceinline__ uint8_t gf8_mul(uint8_t a, uint8_t b)
+{
+    uint8_t r = 0;
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+        if (b & 1) r ^= a;
+        const uint8_t hi = a & 0x80;
+        a = (uint8_t)(a << 1);
+        if (hi) a ^= 0x1b;
+        b >>= 1;
+    }
+    return r;
+}
+
+// the S-box (FIPS-197 5.1.1: inverse in GF(2^8) mod x^8+x^4+x^3+x+1, then the affine map) and the encryption T
+// tables, built by the CTA's threads (blockDim.x >= 256)
+__device__ __forceinline__ void build_tables(SseTables &t)
+{
+    const uint32_t x = threadIdx.x;
+    if (x < 256) {
+        uint8_t inv = 0;
+        if (x) {  // x^254
+            uint8_t r = 1, b = (uint8_t)x;
+            for (int e = 254; e; e >>= 1) {
+                if (e & 1) r = gf8_mul(r, b);
+                b = gf8_mul(b, b);
+            }
+            inv = r;
+        }
+        uint32_t s = inv;
+        s ^= ((inv << 1) | (inv >> 7)) ^ ((inv << 2) | (inv >> 6)) ^ ((inv << 3) | (inv >> 5)) ^
+             ((inv << 4) | (inv >> 4)) ^ 0x63;
+        s &= 0xff;
+        t.sbox[x] = (uint8_t)s;
+        const uint32_t s2 = gf8_mul((uint8_t)s, 2), s3 = s2 ^ s;
+        const uint32_t w = (s2 << 24) | (s << 16) | (s << 8) | s3;
+        t.te[0][x] = w;
+        t.te[1][x] = (w >> 8) | (w << 24);
+        t.te[2][x] = (w >> 16) | (w << 16);
+        t.te[3][x] = (w >> 24) | (w << 8);
+    }
+    if (x < 16) {
+        uint32_t r = 0;
+        for (int b = 0; b < 4; b++)
+            if (x & (1u << b)) r ^= 0xE100u >> (3 - b);
+        t.r4[x] = r;
+    }
+}
+
+__device__ __forceinline__ uint32_t sub_word(const SseTables &t, uint32_t w)
+{
+    return ((uint32_t)t.sbox[w >> 24] << 24) | ((uint32_t)t.sbox[(w >> 16) & 0xff] << 16) |
+           ((uint32_t)t.sbox[(w >> 8) & 0xff] << 8) | (uint32_t)t.sbox[w & 0xff];
+}
+
+// one AES-256 block; state as four big-endian column words
+__device__ __forceinline__ void aes256_encrypt(const SseTables &t, const uint32_t *rk, uint32_t &s0, uint32_t &s1,
+                                               uint32_t &s2, uint32_t &s3)
+{
+    s0 ^= rk[0];
+    s1 ^= rk[1];
+    s2 ^= rk[2];
+    s3 ^= rk[3];
+#pragma unroll
+    for (int r = 1; r < 14; r++) {
+        const uint32_t t0 = t.te[0][s0 >> 24] ^ t.te[1][(s1 >> 16) & 0xff] ^ t.te[2][(s2 >> 8) & 0xff] ^
+                            t.te[3][s3 & 0xff] ^ rk[4 * r];
+        const uint32_t t1 = t.te[0][s1 >> 24] ^ t.te[1][(s2 >> 16) & 0xff] ^ t.te[2][(s3 >> 8) & 0xff] ^
+                            t.te[3][s0 & 0xff] ^ rk[4 * r + 1];
+        const uint32_t t2 = t.te[0][s2 >> 24] ^ t.te[1][(s3 >> 16) & 0xff] ^ t.te[2][(s0 >> 8) & 0xff] ^
+                            t.te[3][s1 & 0xff] ^ rk[4 * r + 2];
+        const uint32_t t3 = t.te[0][s3 >> 24] ^ t.te[1][(s0 >> 16) & 0xff] ^ t.te[2][(s1 >> 8) & 0xff] ^
+                            t.te[3][s2 & 0xff] ^ rk[4 * r + 3];
+        s0 = t0;
+        s1 = t1;
+        s2 = t2;
+        s3 = t3;
+    }
+    const uint8_t *S = t.sbox;
+    const uint32_t o0 = ((uint32_t)S[s0 >> 24] << 24) | ((uint32_t)S[(s1 >> 16) & 0xff] << 16) |
+                        ((uint32_t)S[(s2 >> 8) & 0xff] << 8) | S[s3 & 0xff];
+    const uint32_t o1 = ((uint32_t)S[s1 >> 24] << 24) | ((uint32_t)S[(s2 >> 16) & 0xff] << 16) |
+                        ((uint32_t)S[(s3 >> 8) & 0xff] << 8) | S[s0 & 0xff];
+    const uint32_t o2 = ((uint32_t)S[s2 >> 24] << 24) | ((uint32_t)S[(s3 >> 16) & 0xff] << 16) |
+                        ((uint32_t)S[(s0 >> 8) & 0xff] << 8) | S[s1 & 0xff];
+    const uint32_t o3 = ((uint32_t)S[s3 >> 24] << 24) | ((uint32_t)S[(s0 >> 16) & 0xff] << 16) |
+                        ((uint32_t)S[(s1 >> 8) & 0xff] << 8) | S[s2 & 0xff];
+    s0 = o0 ^ rk[56];
+    s1 = o1 ^ rk[57];
+    s2 = o2 ^ rk[58];
+    s3 = o3 ^ rk[59];
+}
+
+// X * Y in GF(2^128), GCM bit order, bit by bit (NIST SP 800-38D, Algorithm 1)
+__device__ __forceinline__ void gf128_mul_bits(unsigned long long &xh, unsigned long long &xl, unsigned long long yh,
+                                               unsigned long long yl)
+{
+    unsigned long long zh = 0, zl = 0, vh = yh, vl = yl;
+    for (int i = 0; i < 128; i++) {
+        const unsigned long long bit = i < 64 ? (xh >> (63 - i)) & 1 : (xl >> (127 - i)) & 1;
+        const unsigned long long msk = 0ull - bit;
+        zh ^= vh & msk;
+        zl ^= vl & msk;
+        const unsigned long long lsb = vl & 1;
+        vl = (vl >> 1) | (vh << 63);
+        vh = (vh >> 1) ^ ((0ull - lsb) & 0xE100000000000000ull);
+    }
+    xh = zh;
+    xl = zl;
+}
+
+// X * H by the 4-bit table of H (hh / hl: i * H for the nibble i read most significant bit first)
+__device__ __forceinline__ void gf128_mul_h(const unsigned long long *hh, const unsigned long long *hl,
+                                            const uint32_t *r4, unsigned long long &xh, unsigned long long &xl)
+{
+    unsigned long long zh = 0, zl = 0;
+#pragma unroll
+    for (int i = 31; i >= 0; i--) {  // nibbles from the last (x^124..x^127) to the first
+        const uint32_t nib = (uint32_t)((i < 16 ? xh >> (60 - 4 * i) : xl >> (60 - 4 * (i - 16))) & 0xf);
+        if (i != 31) {
+            const uint32_t rem = (uint32_t)(zl & 0xf);
+            zl = (zh << 60) | (zl >> 4);
+            zh = (zh >> 4) ^ ((unsigned long long)r4[rem] << 48);
+        }
+        zh ^= hh[nib];
+        zl ^= hl[nib];
+    }
+    xh = zh;
+    xl = zl;
+}
+
+__device__ __forceinline__ unsigned long long load_be64(const uint8_t *p)
+{
+    unsigned long long v = 0;
+#pragma unroll
+    for (int i = 0; i < 8; i++) v = (v << 8) | p[i];
+    return v;
+}
+__device__ __forceinline__ uint32_t bswap32(uint32_t v) { return __byte_perm(v, 0, 0x0123); }
+__device__ __forceinline__ unsigned long long bswap64(unsigned long long v)
+{
+    return ((unsigned long long)bswap32((uint32_t)v) << 32) | bswap32((uint32_t)(v >> 32));
+}
+
+// ---- key setup: one thread per block --------------------------------------------------------------------------
+struct SetupParams {
+    const uint8_t *keys;   // 32 bytes per block
+    SseKey *ks;            // out
+    uint32_t n;
+};
+__global__ void __launch_bounds__(256) sse_setup_kernel(const __grid_constant__ SetupParams q)
+{
+    __shared__ SseTables t;
+    build_tables(t);
+    __syncthreads();
+    const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= q.n) return;
+    SseKey &K = q.ks[s];
+    uint32_t w[60];
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+        const uint8_t *k = q.keys + (size_t)s * 32 + 4 * i;
+        w[i] = ((uint32_t)k[0] << 24) | ((uint32_t)k[1] << 16) | ((uint32_t)k[2] << 8) | k[3];
+    }
+    uint32_t rcon = 1;
+#pragma unroll
+    for (int i = 8; i < 60; i++) {
+        uint32_t tmp = w[i - 1];
+        if (i % 8 == 0) {
+            tmp = sub_word(t, (tmp << 8) | (tmp >> 24)) ^ (rcon << 24);
+            rcon = gf8_mul((uint8_t)rcon, 2);
+        } else if (i % 8 == 4) {
+            tmp = sub_word(t, tmp);
+        }
+        w[i] = w[i - 8] ^ tmp;
+    }
+#pragma unroll
+    for (int i = 0; i < 60; i++) K.rk[i] = w[i];
+    uint32_t h0 = 0, h1 = 0, h2 = 0, h3 = 0;
+    aes256_encrypt(t, w, h0, h1, h2, h3);
+#pragma unroll
+    for (int i = 0; i < 60; i++) w[i] = 0;
+    unsigned long long vh = ((unsigned long long)h0 << 32) | h1, vl = ((unsigned long long)h2 << 32) | h3;
+    const unsigned long long Hh = vh, Hl = vl;
+    // table: entry 8 = H, 4 = H*x, 2 = H*x^2, 1 = H*x^3 (x = a right shift in GCM order), then the sums
+    K.hh[0] = K.hl[0] = 0;
+    K.hh[8] = vh;
+    K.hl[8] = vl;
+    for (int i = 4; i > 0; i >>= 1) {
+        const unsigned long long lsb = vl & 1;
+        vl = (vl >> 1) | (vh << 63);
+        vh = (vh >> 1) ^ ((0ull - lsb) & 0xE100000000000000ull);
+        K.hh[i] = vh;
+        K.hl[i] = vl;
+    }
+    for (int i = 2; i <= 8; i <<= 1)
+        for (int j = 1; j < i; j++) {
+            K.hh[i + j] = K.hh[i] ^ K.hh[j];
+            K.hl[i + j] = K.hl[i] ^ K.hl[j];
+        }
+    // H^8, then lane 31-i gets H^(8i); lane 31: the identity (bit 0 set)
+    unsigned long long p8h = Hh, p8l = Hl;
+    for (int i = 0; i < 3; i++) gf128_mul_bits(p8h, p8l, p8h, p8l);
+    unsigned long long ph = 1ull << 63, pl = 0;
+    for (int i = 0; i < 32; i++) {
+        K.pw[31 - i][0] = ph;
+        K.pw[31 - i][1] = pl;
+        gf128_mul_bits(ph, pl, p8h, p8l);
+    }
+}
+
+// ---- the chunk kernel -----------------------------------------------------------------------------------------
+enum { kSeal = 0, kCheck = 1, kOpen = 2 };
+
+struct ChunkParams {
+    const uint8_t *plain_in;        // seal: block s at plain_in + s*plain_stride
+    uint8_t *plain_out;             // open: block s at plain_out + s*plain_stride
+    unsigned long long plain_stride;
+    const uint32_t *plain_len;      // seal: per block
+    uint32_t *plain_len_out;        // open: per block
+    const uint32_t *blen;           // len(B) per block: sealed length (plain_len when unkeyed)
+    const uint32_t *shard_len;      // L per block; 0 = nothing of the block is touched
+    const uint8_t *nonces;          // seal: 8 bytes per block
+    const SseKey *ks;               // nullable (seal only): B = P
+    uint8_t *shards;                // stripe s at shards + s*(k+m)*stride, data shard j at + j*stride
+    int32_t *status;                // check / open
+    const int32_t *rec_status;      // check: verdict of the reconstruct
+    const uint8_t *hash_bad;        // open: skip the block when set
+    uint32_t stride, k, m, n;
+    uint32_t cmax;                  // chunks per block this launch covers (work item = block * cmax + chunk)
+};
+
+struct ChunkSmem {
+    SseTables t;
+    __align__(16) uint8_t stage[kWarps][kStage];
+    uint32_t rk[kWarps][60];
+    unsigned long long hh[kWarps][16], hl[kWarps][16];
+};
+
+template <int MODE>
+__global__ void __launch_bounds__(kWarps * 32) sse_chunk_kernel(const __grid_constant__ ChunkParams q)
+{
+    __shared__ ChunkSmem sm;
+    build_tables(sm.t);
+    __syncthreads();
+    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    uint8_t *st = sm.stage[wid];
+    const unsigned long long total = (unsigned long long)q.n * q.cmax;
+    for (unsigned long long w = (unsigned long long)blockIdx.x * kWarps + wid; w < total;
+         w += (unsigned long long)gridDim.x * kWarps) {
+        const uint32_t s = (uint32_t)(w / q.cmax), c = (uint32_t)(w - (unsigned long long)s * q.cmax);
+        const uint32_t L = q.shard_len[s];
+        if (!L) continue;
+        const bool keyed = MODE != kSeal || q.ks;
+        const uint32_t blen = q.blen[s];
+        const uint32_t prefix = keyed ? kPrefix : 0, pitch = keyed ? kFrame : kChunk;
+        uint32_t plen, nch;
+        if (MODE == kSeal) {
+            plen = q.plain_len[s];
+        } else {
+            if (MODE == kCheck && c == 0) {
+                const int32_t rs = q.rec_status[s];
+                if (rs && lane == 0) q.status[s] = rs;  // an unrecoverable stripe reports that, not its framing
+            }
+            if (q.status[s] != 0 || q.rec_status[s] != 0) continue;
+            if (MODE == kOpen && q.hash_bad[s]) continue;
+            const uint32_t nn = (blen - kPrefix + kFrame - 1) / kFrame;  // framing checked by sse_lens_kernel
+            plen = blen - kPrefix - 16 * nn;
+        }
+        nch = plen ? (plen + kChunk - 1) / kChunk : 1;
+        if (c >= nch) continue;
+        const bool last = c == nch - 1;
+        const uint32_t clen = last ? plen - kChunk * c : kChunk;  // plaintext bytes of this chunk
+        const uint32_t nb = (clen + 15) >> 4;
+        const uint32_t base = pitch * c;  // B position of stage[0]
+        uint8_t *stripe = q.shards + (size_t)s * (q.k + q.m) * q.stride;
+        const SseKey *K = keyed ? q.ks + s : nullptr;
+        if (keyed) {
+            for (uint32_t i = lane; i < 60; i += 32) sm.rk[wid][i] = K->rk[i];
+            if (lane < 16) {
+                sm.hh[wid][lane] = K->hh[lane];
+                sm.hl[wid][lane] = K->hl[lane];
+            }
+        }
+        uint32_t nw0 = 0, nw1 = 0;  // the nonce prefix, big-endian words
+        if (keyed) {
+            if (MODE == kSeal) {
+                const uint8_t *np = q.nonces + (size_t)s * 8;
+                nw0 = ((uint32_t)np[0] << 24) | ((uint32_t)np[1] << 16) | ((uint32_t)np[2] << 8) | np[3];
+                nw1 = ((uint32_t)np[4] << 24) | ((uint32_t)np[5] << 16) | ((uint32_t)np[6] << 8) | np[7];
+            } else {
+                // B[0, 8): byte i of B is byte i % L of data shard i / L
+                uint8_t nb8[8];
+#pragma unroll
+                for (int i = 0; i < 8; i++) nb8[i] = stripe[(size_t)(i / L) * q.stride + i % L];
+                nw0 = ((uint32_t)nb8[0] << 24) | ((uint32_t)nb8[1] << 16) | ((uint32_t)nb8[2] << 8) | nb8[3];
+                nw1 = ((uint32_t)nb8[4] << 24) | ((uint32_t)nb8[5] << 16) | ((uint32_t)nb8[6] << 8) | nb8[7];
+            }
+        }
+        const uint32_t nw2 = bswap32(c | (last ? 0x80000000u : 0u));  // LE32(c | last << 31) as a big-endian word
+
+        if (MODE != kSeal) {
+            // load this chunk's ciphertext and tag, B[base + 8, base + 8 + clen + 16), into stage[8..]
+            const uint32_t r0 = base + kPrefix, r1 = r0 + clen + 16;
+            for (uint32_t j = r0 / L; j * L < r1 && j < q.k; j++) {
+                const uint32_t x0 = max(r0, j * L) - j * L, x1 = min(r1, (j + 1) * L) - j * L;
+                const uint8_t *sh = stripe + (size_t)j * q.stride;
+                for (uint32_t v = (x0 & ~15u) + 16 * lane; v < x1; v += 512) {
+                    const uint4 d = *reinterpret_cast<const uint4 *>(sh + v);
+                    const uint32_t wds[4] = {d.x, d.y, d.z, d.w};
+#pragma unroll
+                    for (int b = 0; b < 16; b++) {
+                        const uint32_t x = v + b;
+                        if (x >= x0 && x < x1) st[j * L + x - base] = (uint8_t)(wds[b >> 2] >> (8 * (b & 3)));
+                    }
+                }
+            }
+        }
+        __syncwarp();
+
+        // this lane's slots: data blocks b = 8*lane + i - (256 - nb)
+        unsigned long long yh = 0, yl = 0;
+        if (MODE == kSeal && !keyed) {
+            // B = P: copy the chunk into the stage
+            const uint8_t *src = q.plain_in + (size_t)s * q.plain_stride + (size_t)kChunk * c;
+            for (uint32_t b = lane; b < nb; b += 32)
+                *reinterpret_cast<uint4 *>(st + 16 * b) = *reinterpret_cast<const uint4 *>(src + 16 * b);
+        } else {
+#pragma unroll 1
+            for (uint32_t i = 0; i < 8; i++) {
+                const int b = (int)(8 * lane + i) - (int)(256 - nb);
+                if (b < 0) continue;
+                const uint32_t valid = min(16u, clen - 16u * (uint32_t)b);
+                unsigned long long ch, cl;
+                if (MODE == kCheck) {
+                    ch = *reinterpret_cast<const unsigned long long *>(st + kPrefix + 16 * b);
+                    cl = *reinterpret_cast<const unsigned long long *>(st + kPrefix + 16 * b + 8);
+                } else {
+                    uint32_t k0 = nw0, k1 = nw1, k2 = nw2, k3 = (uint32_t)b + 2;
+                    aes256_encrypt(sm.t, sm.rk[wid], k0, k1, k2, k3);
+                    // keystream in memory byte order (little-endian 64-bit words of the block)
+                    const unsigned long long ksa = bswap64(((unsigned long long)k0 << 32) | k1),
+                                             ksb = bswap64(((unsigned long long)k2 << 32) | k3);
+                    unsigned long long pa, pb;
+                    if (MODE == kSeal) {
+                        const uint4 p = *reinterpret_cast<const uint4 *>(q.plain_in + (size_t)s * q.plain_stride +
+                                                                         (size_t)kChunk * c + 16 * b);
+                        pa = ((unsigned long long)p.y << 32) | p.x;
+                        pb = ((unsigned long long)p.w << 32) | p.z;
+                    } else {
+                        pa = *reinterpret_cast<const unsigned long long *>(st + kPrefix + 16 * b);
+                        pb = *reinterpret_cast<const unsigned long long *>(st + kPrefix + 16 * b + 8);
+                    }
+                    // mask to the valid bytes
+                    const unsigned long long ma = valid >= 8 ? ~0ull : ((1ull << (8 * valid)) - 1),
+                                             mb = valid >= 16 ? ~0ull : valid <= 8 ? 0ull : ((1ull << (8 * (valid - 8))) - 1);
+                    const unsigned long long oa = (pa ^ ksa) & ma, ob = (pb ^ ksb) & mb;
+                    if (MODE == kSeal) {
+                        *reinterpret_cast<unsigned long long *>(st + kPrefix + 16 * b) = oa;
+                        *reinterpret_cast<unsigned long long *>(st + kPrefix + 16 * b + 8) = ob;
+                        ch = oa;
+                        cl = ob;
+                    } else {
+                        uint8_t *dst = q.plain_out + (size_t)s * q.plain_stride + (size_t)kChunk * c + 16 * b;
+                        *reinterpret_cast<uint4 *>(dst) =
+                            make_uint4((uint32_t)oa, (uint32_t)(oa >> 32), (uint32_t)ob, (uint32_t)(ob >> 32));
+                        continue;
+                    }
+                }
+                if (MODE == kCheck && valid < 16) {  // zero-pad the last block for GHASH
+                    const unsigned long long ma = valid >= 8 ? ~0ull : ((1ull << (8 * valid)) - 1),
+                                             mb = valid <= 8 ? 0ull : ((1ull << (8 * (valid - 8))) - 1);
+                    ch &= ma;
+                    cl &= mb;
+                }
+                // Horner: Y = (Y ^ C_b) * H, blocks as big-endian 128-bit values
+                yh ^= bswap64(ch);
+                yl ^= bswap64(cl);
+                gf128_mul_h(sm.hh[wid], sm.hl[wid], sm.t.r4, yh, yl);
+            }
+        }
+
+        if (MODE != kOpen && keyed) {
+            if (lane != 31) gf128_mul_bits(yh, yl, K->pw[lane][0], K->pw[lane][1]);
+            __syncwarp();  // the last data block's zero tail is in the stage before lane 0 writes the tag over it
+#pragma unroll
+            for (int o = 16; o; o >>= 1) {
+                yh ^= __shfl_xor_sync(0xffffffffu, yh, o);
+                yl ^= __shfl_xor_sync(0xffffffffu, yl, o);
+            }
+            if (lane == 0) {
+                // S = (D ^ lengths) * H; T = E_K(J0) ^ S, J0 = nonce || 1
+                yl ^= (unsigned long long)clen * 8;
+                gf128_mul_h(sm.hh[wid], sm.hl[wid], sm.t.r4, yh, yl);
+                uint32_t j0 = nw0, j1 = nw1, j2 = nw2, j3 = 1;
+                aes256_encrypt(sm.t, sm.rk[wid], j0, j1, j2, j3);
+                const unsigned long long th = yh ^ (((unsigned long long)j0 << 32) | j1),
+                                         tl = yl ^ (((unsigned long long)j2 << 32) | j3);
+                uint8_t *tp = st + kPrefix + clen;
+                if (MODE == kSeal) {
+#pragma unroll
+                    for (int i = 0; i < 8; i++) {
+                        tp[i] = (uint8_t)(th >> (56 - 8 * i));
+                        tp[8 + i] = (uint8_t)(tl >> (56 - 8 * i));
+                    }
+                    if (c == 0) {
+#pragma unroll
+                        for (int i = 0; i < 4; i++) {
+                            st[i] = (uint8_t)(nw0 >> (24 - 8 * i));
+                            st[4 + i] = (uint8_t)(nw1 >> (24 - 8 * i));
+                        }
+                    }
+                } else {
+                    const unsigned long long gh = load_be64(tp), gl = load_be64(tp + 8);
+                    if (gh != th || gl != tl) q.status[s] = -7;  // GARAGE_EC_E_AUTH
+                }
+            }
+        }
+        if (MODE == kOpen && c == 0 && lane == 0) q.plain_len_out[s] = plen;
+
+        if (MODE == kSeal) {
+            __syncwarp();
+            // store this chunk's part of B: [start, end) -- chunk 0 from 0 (the nonce), the last chunk to k*L (the
+            // zero tail); bytes past L of a shard, up to roundup16(L), are zero and belong to the chunk that owns
+            // the shard's last byte
+            const uint32_t start = c == 0 ? 0 : prefix + pitch * c;
+            const uint32_t end = last ? q.k * L : prefix + pitch * (c + 1);
+            const uint32_t Lr = (L + 15) & ~15u;
+            for (uint32_t j = start / L; j * L < end && j < q.k; j++) {
+                const uint32_t x0 = max(start, j * L) - j * L;
+                uint32_t x1 = min(end, (j + 1) * L) - j * L;
+                if (x1 == L) x1 = Lr;
+                uint8_t *sh = stripe + (size_t)j * q.stride;
+                auto byte_at = [&](uint32_t x) -> uint8_t {
+                    const uint32_t p = j * L + x;
+                    return (x >= L || p >= blen) ? (uint8_t)0 : st[p - base];
+                };
+                for (uint32_t v = (x0 & ~15u) + 16 * lane; v < x1; v += 512) {
+                    if (v >= x0 && v + 16 <= x1) {
+                        uint32_t wds[4] = {0, 0, 0, 0};
+                        if (j * L + v < blen && v < L) {
+#pragma unroll
+                            for (int b = 0; b < 16; b++) wds[b >> 2] |= (uint32_t)byte_at(v + b) << (8 * (b & 3));
+                        }
+                        *reinterpret_cast<uint4 *>(sh + v) = make_uint4(wds[0], wds[1], wds[2], wds[3]);
+                    } else {
+                        for (uint32_t x = max(v, x0); x < min(v + 16, x1); x++) sh[x] = byte_at(x);
+                    }
+                }
+            }
+        }
+        __syncwarp();
+    }
+}
+
+// ---- per-block lengths and framing ----------------------------------------------------------------------------
+struct LensParams {
+    const uint32_t *plain_len;   // seal: per block
+    const uint32_t *sealed_in;   // open: per block
+    uint32_t *blen;              // out: len(B) (seal)
+    uint32_t *shard_len;         // out: L, 0 for a block that is skipped
+    int32_t *status;             // open: out, 0 / GARAGE_EC_E_AUTH (framing) / GARAGE_EC_E_INVALID (geometry)
+    uint8_t *want;               // open: out, (k+m) bytes per block, the data shards
+    unsigned long long plain_stride;
+    uint32_t stride, k, m, n, quantum, keyed, open;
+};
+__global__ void __launch_bounds__(256) sse_lens_kernel(const __grid_constant__ LensParams q)
+{
+    for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < q.n; s += gridDim.x * blockDim.x) {
+        if (!q.open) {
+            const uint32_t len = q.plain_len[s];
+            const uint64_t b = q.keyed ? sealed_len(len) : len;
+            const uint64_t L = b > 0xffffffffull ? ~0ull : code_shard_len((uint32_t)b, (int)q.k, q.quantum);
+            const bool bad = L > q.stride || len > q.plain_stride;
+            q.blen[s] = bad ? 0u : (uint32_t)b;
+            q.shard_len[s] = bad ? 0u : (uint32_t)L;
+            continue;
+        }
+        const uint32_t b = q.sealed_in[s];
+        const uint64_t L = code_shard_len(b, (int)q.k, q.quantum);
+        const uint32_t r = (b - kPrefix) % kFrame;
+        const bool framed = b >= kPrefix + 16 && !(r >= 1 && r < 16);
+        uint64_t plen = 0;
+        if (framed) plen = b - kPrefix - 16ull * ((b - kPrefix + kFrame - 1) / kFrame);
+        const bool bad = L > q.stride || plen > q.plain_stride;
+        q.status[s] = bad ? -1 /* GARAGE_EC_E_INVALID */ : framed ? 0 : -7 /* GARAGE_EC_E_AUTH */;
+        q.shard_len[s] = bad ? 0u : (uint32_t)L;
+        for (uint32_t i = 0; i < q.k + q.m; i++) q.want[(size_t)s * (q.k + q.m) + i] = i < q.k;
+    }
+}
+
+}  // namespace sse
+}  // namespace garage_ec

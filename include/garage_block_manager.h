@@ -216,6 +216,18 @@ typedef struct garage_bm_resync_metrics {
     uint64_t resync_failed_bytes_read; /* bytes read by resyncs that failed (part of resync_bytes_read)             */
 } garage_bm_resync_metrics;
 
+/* Counters of the SSE-C calls (DESIGN.md section 5.9), in a struct of their own for the same reason. */
+typedef struct garage_bm_sealed_metrics {
+    uint64_t sealed_puts;          /* garage_bm_rpc_put_block_sealed calls that sealed their block               */
+    uint64_t sealed_batches;       /* garage_ec_seal_blocks calls of the encode dispatchers                      */
+    uint64_t opened_gets;          /* garage_bm_rpc_get_block_opened calls that returned a plaintext             */
+    uint64_t opened_auth_failures; /* opened GETs that ended in GARAGE_EC_E_AUTH                                 */
+    uint64_t opened_fallbacks;     /* opened GETs that went through rpc_get_block (stale shard, previous code,
+                                      replica or missing stripe) before the block was opened                   */
+    uint64_t seal_call_us;         /* wall time inside garage_ec_seal_blocks                                    */
+    uint64_t open_call_us;         /* wall time inside garage_ec_open_stripes                                   */
+} garage_bm_sealed_metrics;
+
 /* One entry of a node's resync error table (Garage's BlockResyncErrorInfo, manager.rs:429-449).                    */
 typedef struct garage_bm_resync_error {
     int32_t node;
@@ -275,6 +287,22 @@ int garage_bm_rpc_put_block(garage_bm *bm, const uint8_t hash[32], const uint8_t
  * GARAGE_BM_E_MISSING_BLOCK if fewer than k valid shards can be gathered.                       */
 int garage_bm_rpc_get_block(garage_bm *bm, const uint8_t hash[32], uint8_t *out, size_t cap,
                             size_t *out_len);
+/* SSE-C PUT (src/api/s3/put.rs:441-466, DESIGN.md sections 2.6 and 5.9): the plaintext (len <= block_size) is sealed
+ * with AES-256-GCM STREAM chunks under key32 and a fresh 8-byte nonce prefix from getrandom(2) -- key32 NULL: stored
+ * as plaintext (len >= 1) -- by the encode batcher, then stored exactly as garage_bm_rpc_put_block stores a block of
+ * sealed_len bytes.  hash_out = the block's content address, blake2sum of the sealed block.  No key is kept or logged. */
+int garage_bm_rpc_put_block_sealed(garage_bm *bm, const uint8_t *key32, const uint8_t *data, size_t len,
+                                   uint8_t hash_out[32]);
+/* SSE-C GET (EncryptionParams::get_block, src/api/s3/encryption.rs:269-279): the plaintext of block `hash` sealed
+ * under key32.  Gathered like garage_bm_rpc_get_block; the rebuild, the content-hash check and the decryption are one
+ * garage_ec_open_stripes call of the reconstruct dispatchers.  A block that does not hash to its address, or that only
+ * a previous code or a replica holds, is read by garage_bm_rpc_get_block (stale-shard hunt included) and then opened.
+ * GARAGE_EC_E_AUTH if a tag or the framing fails (wrong key, tampered block); GARAGE_BM_E_MISSING_BLOCK as
+ * garage_bm_rpc_get_block; GARAGE_EC_E_INVALID if the plaintext exceeds cap.                                        */
+int garage_bm_rpc_get_block_opened(garage_bm *bm, const uint8_t hash[32], const uint8_t *key32, uint8_t *out, size_t cap,
+                                   size_t *out_len);
+void garage_bm_get_sealed_metrics(garage_bm *bm, garage_bm_sealed_metrics *out);
+
 /* Bytes [offset, offset + len) of a block (body_from_blocks_range, src/api/s3/get.rs:650-743; the source range of
  * UploadPartCopy, src/api/s3/copy.rs:396-469), reading only the shards and columns garage_ec_range_plan names, each as
  * the adler8 tag span that covers its runs (BLAKE2 stores: whole shards).  *out_len = len.  A range whose touched data

@@ -58,6 +58,7 @@ extern "C" {
 #define GARAGE_EC_E_UNRECOVERABLE (-4) /* >= 1 stripe could not be rebuilt; see status[] */
 #define GARAGE_EC_E_NODEVICE (-5)      /* no CUDA device / wrong architecture */
 #define GARAGE_EC_E_ALIGN (-6)         /* pointer or stride alignment violated */
+#define GARAGE_EC_E_AUTH (-7)          /* a block failed authentication (a GCM tag, or its framing); see status[] */
 
 /* matrix kinds */
 #define GARAGE_EC_VANDERMONDE 0 /* systematic Vandermonde (default), G = V * inv(V[0..k)) */
@@ -379,6 +380,56 @@ int garage_ec_decode_range_stripes(garage_ec_ctx *ctx, const uint8_t *const *str
 int garage_ec_transcode(garage_ec_ctx *dst, garage_ec_ctx *src, uint8_t *src_shards, const uint8_t *src_present,
                         const uint32_t *block_len, size_t src_stride, uint8_t *dst_shards, size_t dst_stride,
                         uint8_t *dst_sums, int32_t *status, size_t n_stripes, int mem_kind, void *cuda_stream);
+
+/* ---- SSE-C -- call sites: the "Encrypt and hash (blake2) block" stage of PutObject (src/api/s3/put.rs:441-466:
+ * EncryptionParams::encrypt_block, then blake2sum) and EncryptionParams::get_block (src/api/s3/encryption.rs:269-279,
+ * DecryptStream, encryption.rs:431-540).  DESIGN.md section 2.6 is normative.  A plain block P of len bytes sealed
+ * under a 32-byte key K and an 8-byte nonce prefix N is B = N || C_0 || ... || C_{n-1}, n = max(1, ceil(len/4096)),
+ * C_c = AES-256-GCM(K, nonce = N || LE32(c | (c == n-1) << 31), aad = empty, P[4096c, min(4096(c+1), len))) =
+ * ciphertext || 16-byte tag: aead's StreamLE31 over Garage's 4096-byte chunks.  sealed_len = 8 + len + 16n.  The stored
+ * block is B: its content address is blake2sum(B), and data shard j = B[jL, (j+1)L) zero padded, L =
+ * garage_ec_code_shard_len(sealed_len), so every other call of this header works on it unchanged.
+ * Keys are secrets: the library's device and pinned copies of keys and key schedules are zeroed before a HOST call
+ * returns and before the stream work of a DEVICE call ends, and no key reaches garage_ec_last_error.
+ *
+ * garage_ec_sealed_len: 8 + plain_len + 16 * max(1, ceil(plain_len / 4096)); GARAGE_EC_E_INVALID past 32 bits.
+ *
+ * garage_ec_seal: block s is plain_len[s] bytes at plain + s*plain_stride (plain_stride a multiple of 16 >= every
+ * plain_len; the whole row may be read).  keys / nonces: 32 / 8 bytes per block, or both NULL: B = P (Garage's
+ * Plaintext).  shards (shard layout, k+m shards per block) gets exactly the context's encode of B -- nothing is written
+ * past roundup16(L) of a shard --, hashes[32 s] = blake2sum(B), sums (nullable) the context's tag of every shard, as
+ * garage_ec_encode_blocks_with_sums.  DEVICE: all pointers device memory (plain_len 4-byte, hashes and sums 8-byte
+ * aligned); only kernels and stream-ordered scratch are enqueued (capturable in a CUDA graph); a block whose L exceeds
+ * `stride` or whose plain_len exceeds plain_stride is malformed: nothing of its shards is written and its hash and tags
+ * are unspecified.  HOST: synchronous, GARAGE_EC_E_INVALID before any GPU work for such a block; downloads
+ * roundup16(L) bytes of all k+m shards.  garage_ec_seal_blocks is the HOST gather form: block s at blocks[s].
+ *
+ * garage_ec_open: the inverse for stored blocks (shard layout, present: n*(k+m) bytes, sealed_len / hashes / keys: n
+ * values).  Absent data shards are rebuilt by the code's own plan, reading only what garage_ec_read_set names for the
+ * data shards (HOST: only those and the present data shards are uploaded; DEVICE: the absent data shards of `shards`
+ * are OVERWRITTEN with their rebuilt bytes).  hash_bad[s] = 1 iff blake2sum(B) != hashes[s].  Every chunk's tag is
+ * checked.  status[s]: 0; GARAGE_EC_E_UNRECOVERABLE; GARAGE_EC_E_AUTH for a failed tag or a sealed_len the framing cannot
+ * hold (< 24, or (sealed_len - 8) mod 4112 in 1..15); DEVICE only: GARAGE_EC_E_INVALID for an L past `stride` or a
+ * plaintext past plain_stride.  Only a block with status 0 and hash_bad 0 has its plaintext written (at plain +
+ * s*plain_stride; DEVICE writes zeros up to roundup16 of its length) and plain_len_out[s] set.  keys is required.
+ * DEVICE: as for seal (sealed_len and plain_len_out 4-byte, status 4-byte, hashes 8-byte aligned).  HOST: synchronous;
+ * GARAGE_EC_E_INVALID before any GPU work for an L past `stride` or a plaintext past plain_stride; returns
+ * GARAGE_EC_E_UNRECOVERABLE if any block was, else GARAGE_EC_E_AUTH if any block failed authentication; hash_bad does not
+ * fail the call.  garage_ec_open_stripes is the HOST gather form: stripe s at stripes[s] (its k+m shards `stride`
+ * apart), plaintext s written to plains[s] (room for sealed_len[s] - 24 bytes suffices).                            */
+int garage_ec_sealed_len(uint32_t plain_len, uint32_t *sealed_len);
+int garage_ec_seal(garage_ec_ctx *ctx, const uint8_t *plain, size_t plain_stride, const uint32_t *plain_len,
+                   const uint8_t *keys, const uint8_t *nonces, uint8_t *shards, size_t stride, uint8_t *hashes,
+                   uint8_t *sums, size_t n, int mem_kind, void *cuda_stream);
+int garage_ec_seal_blocks(garage_ec_ctx *ctx, const uint8_t *const *blocks, const uint32_t *plain_len, const uint8_t *keys,
+                          const uint8_t *nonces, uint8_t *shards, size_t stride, uint8_t *hashes, uint8_t *sums, size_t n);
+int garage_ec_open(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *present, const uint32_t *sealed_len,
+                   const uint8_t *hashes, const uint8_t *keys, uint8_t *plain, size_t plain_stride,
+                   uint32_t *plain_len_out, uint8_t *hash_bad, int32_t *status, size_t stride, size_t n, int mem_kind,
+                   void *cuda_stream);
+int garage_ec_open_stripes(garage_ec_ctx *ctx, uint8_t *const *stripes, const uint8_t *present, const uint32_t *sealed_len,
+                           const uint8_t *hashes, const uint8_t *keys, uint8_t *const *plains, uint32_t *plain_len_out,
+                           uint8_t *hash_bad, int32_t *status, size_t stride, size_t n);
 
 /* ---- utilities used by the harness ------------------------------------------------------
  * device-side synthetic data (same splitmix64 counter stream as the oracle's

@@ -140,5 +140,40 @@ impl ErasureCoder {
         check(self.ctx, rc)?;
         Ok((bad.into_iter().map(|b| b != 0).collect(), mm))
     }
+
+    /// put.rs:441-466: seal every block (None: stored as plaintext) into the shard layout; returns the content
+    /// addresses.  `keys` and `nonces` hold one entry per block.
+    pub fn seal_blocks(&self, blocks: &[&[u8]], keys: Option<(&[[u8; 32]], &[[u8; 8]])>, shards_out: &mut [u8],
+                       stride: usize) -> Result<Vec<[u8; 32]>, Error> {
+        let n = blocks.len();
+        let ptrs: Vec<*const u8> = blocks.iter().map(|b| b.as_ptr()).collect();
+        let lens: Vec<u32> = blocks.iter().map(|b| b.len() as u32).collect();
+        let (kp, np) = match keys {
+            Some((k, nn)) => { assert!(k.len() == n && nn.len() == n); (k.as_ptr() as *const u8, nn.as_ptr() as *const u8) }
+            None => (std::ptr::null(), std::ptr::null()),
+        };
+        let mut hashes = vec![[0u8; 32]; n];
+        let rc = unsafe { sys::garage_ec_seal_blocks(self.ctx, ptrs.as_ptr(), lens.as_ptr(), kp, np,
+                          shards_out.as_mut_ptr(), stride, hashes.as_mut_ptr() as *mut u8, std::ptr::null_mut(), n) };
+        check(self.ctx, rc)?;
+        Ok(hashes)
+    }
+
+    /// EncryptionParams::get_block for SSE-C: rebuild, check the content hash and every chunk tag, decrypt.  Per
+    /// stripe: Ok(plaintext length), or the stripe's status (GARAGE_EC_E_AUTH, GARAGE_EC_E_UNRECOVERABLE, or
+    /// GARAGE_EC_E_INVALID for a block that does not hash to its address).
+    pub fn open_stripes(&self, stripes: &[*mut u8], present: &[u8], sealed_len: &[u32], hashes: &[[u8; 32]],
+                        keys: &[[u8; 32]], outs: &[*mut u8], stride: usize) -> Result<Vec<Result<u32, i32>>, Error> {
+        let n = stripes.len();
+        assert!(sealed_len.len() == n && hashes.len() == n && keys.len() == n && outs.len() == n);
+        let (mut plen, mut bad, mut status) = (vec![0u32; n], vec![0u8; n], vec![0i32; n]);
+        let rc = unsafe { sys::garage_ec_open_stripes(self.ctx, stripes.as_ptr(), present.as_ptr(), sealed_len.as_ptr(),
+                          hashes.as_ptr() as *const u8, keys.as_ptr() as *const u8, outs.as_ptr(), plen.as_mut_ptr(),
+                          bad.as_mut_ptr(), status.as_mut_ptr(), stride, n) };
+        if rc != sys::GARAGE_EC_E_AUTH && rc != sys::GARAGE_EC_E_UNRECOVERABLE { check(self.ctx, rc)?; }
+        Ok((0..n).map(|s| if status[s] == sys::GARAGE_EC_E_UNRECOVERABLE { Err(status[s]) }
+                          else if bad[s] != 0 { Err(sys::GARAGE_EC_E_INVALID) }
+                          else if status[s] != 0 { Err(status[s]) } else { Ok(plen[s]) }).collect())
+    }
 }
 impl Drop for ErasureCoder { fn drop(&mut self) { unsafe { sys::garage_ec_destroy(self.ctx) } } }

@@ -14,6 +14,7 @@ pub const GARAGE_EC_E_NOMEM: c_int = -3;
 pub const GARAGE_EC_E_UNRECOVERABLE: c_int = -4;
 pub const GARAGE_EC_E_NODEVICE: c_int = -5;
 pub const GARAGE_EC_E_ALIGN: c_int = -6;
+pub const GARAGE_EC_E_AUTH: c_int = -7;
 pub const GARAGE_EC_VANDERMONDE: c_int = 0;
 pub const GARAGE_EC_CAUCHY: c_int = 1;
 pub const GARAGE_EC_MEM_HOST: c_int = 0;
@@ -62,6 +63,21 @@ extern "C" {
     pub fn garage_ec_decode_range_stripes(ctx: *mut garage_ec_ctx, stripes: *const *const u8, present: *const u8,
                             block_len: *const u32, offset: *const u32, len: *const u32, stride: usize,
                             outs: *const *mut u8, status: *mut i32, n: usize) -> c_int;
+    pub fn garage_ec_sealed_len(plain_len: u32, sealed_len: *mut u32) -> c_int;
+    pub fn garage_ec_seal(ctx: *mut garage_ec_ctx, plain: *const u8, plain_stride: usize, plain_len: *const u32,
+                          keys: *const u8, nonces: *const u8, shards: *mut u8, stride: usize, hashes: *mut u8,
+                          sums: *mut u8, n: usize, mem_kind: c_int, stream: *mut c_void) -> c_int;
+    pub fn garage_ec_seal_blocks(ctx: *mut garage_ec_ctx, blocks: *const *const u8, plain_len: *const u32,
+                                 keys: *const u8, nonces: *const u8, shards: *mut u8, stride: usize, hashes: *mut u8,
+                                 sums: *mut u8, n: usize) -> c_int;
+    pub fn garage_ec_open(ctx: *mut garage_ec_ctx, shards: *mut u8, present: *const u8, sealed_len: *const u32,
+                          hashes: *const u8, keys: *const u8, plain: *mut u8, plain_stride: usize,
+                          plain_len_out: *mut u32, hash_bad: *mut u8, status: *mut i32, stride: usize, n: usize,
+                          mem_kind: c_int, stream: *mut c_void) -> c_int;
+    pub fn garage_ec_open_stripes(ctx: *mut garage_ec_ctx, stripes: *const *mut u8, present: *const u8,
+                                  sealed_len: *const u32, hashes: *const u8, keys: *const u8, plains: *const *mut u8,
+                                  plain_len_out: *mut u32, hash_bad: *mut u8, status: *mut i32, stride: usize,
+                                  n: usize) -> c_int;
     pub fn garage_ec_strerror(code: c_int) -> *const c_char;
     pub fn garage_ec_last_error(ctx: *const garage_ec_ctx) -> *const c_char;
     pub fn garage_ec_abi_version() -> c_int;
