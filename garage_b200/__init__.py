@@ -44,6 +44,7 @@ ABI_SYMBOLS = [
     "garage_ec_tag_span", "garage_ec_check_shard_span_host", "garage_ec_range_plan", "garage_ec_decode_range",
     "garage_ec_decode_range_stripes",
     "garage_ec_sealed_len", "garage_ec_seal", "garage_ec_seal_blocks", "garage_ec_open", "garage_ec_open_stripes",
+    "garage_ec_sealed_range", "garage_ec_open_range_plan", "garage_ec_open_range", "garage_ec_open_range_stripes",
 ]
 
 
@@ -143,6 +144,10 @@ def load_library(build=True):
     L.garage_ec_seal_blocks.argtypes = [vp, vp, vp, vp, vp, vp, sz, vp, vp, sz]
     L.garage_ec_open.argtypes = [vp, vp, vp, vp, vp, vp, vp, sz, vp, vp, vp, sz, sz, i32, vp]
     L.garage_ec_open_stripes.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, sz]
+    L.garage_ec_sealed_range.argtypes = [u32, u32, u32, C.POINTER(u32), C.POINTER(u32), C.POINTER(u32), C.POINTER(u32)]
+    L.garage_ec_open_range_plan.argtypes = [vp, vp, u32, u32, u32, vp, sz, C.POINTER(sz), C.POINTER(i32)]
+    L.garage_ec_open_range.argtypes = [vp, vp, vp, vp, vp, vp, vp, sz, vp, sz, vp, sz, i32, vp]
+    L.garage_ec_open_range_stripes.argtypes = [vp, vp, vp, vp, vp, vp, vp, sz, vp, vp, sz]
     _lib = L
     return L
 
@@ -543,6 +548,50 @@ class GarageEc:
                                                           _ptr(sealed_len), _ptr(hashes), _ptr(keys),
                                                           C.cast(op, C.c_void_p), _ptr(plain_len_out), _ptr(hash_bad),
                                                           _ptr(status), stride, n),
+                           (E_UNRECOVERABLE, E_AUTH))
+
+    # -- SSE-C ranged opens (DESIGN.md 2.7)
+    @staticmethod
+    def sealed_range(sealed_len, offset, length):
+        """garage_ec_sealed_range (host only, no context): (span_off, span_len, c0, n_chunks) of plaintext bytes
+        [offset, offset + length) of a block sealed to sealed_len bytes; raises EcError (E_AUTH / E_INVALID)"""
+        v = [C.c_uint32(0) for _ in range(4)]
+        rc = load_library().garage_ec_sealed_range(sealed_len, offset, length, *[C.byref(x) for x in v])
+        if rc:
+            raise EcError(rc, "sealed_range")
+        return tuple(x.value for x in v)
+
+    def open_range_plan(self, present, sealed_len, offset, length):
+        """(runs [(shard, offset, len)], needs_gpu) for the prefix and span of a plaintext range of one sealed block,
+        or (None, needs_gpu) if an absent touched data shard cannot be rebuilt"""
+        pr = np.ascontiguousarray(present, dtype=np.uint8)
+        assert pr.shape == (self.k + self.m,)
+        cap = (self.k + self.m) * 1024
+        out = np.zeros(cap * 3, dtype=np.uint32)
+        n, g = C.c_size_t(0), C.c_int(0)
+        rc = self._check(self._L.garage_ec_open_range_plan(self._h, _ptr(pr), sealed_len, offset, length, _ptr(out),
+                                                           cap, C.byref(n), C.byref(g)), (E_UNRECOVERABLE,))
+        if rc == E_UNRECOVERABLE:
+            return None, g.value
+        return [tuple(int(v) for v in out[3 * i:3 * i + 3]) for i in range(n.value)], g.value
+
+    def open_range(self, shards, present, sealed_len, keys, offset, length, stride, out, out_stride, status):
+        """garage_ec_open_range of n = len(sealed_len) requests; returns 0, E_UNRECOVERABLE or E_AUTH (HOST mode)"""
+        kind, st = self._stream(shards)
+        return self._check(self._L.garage_ec_open_range(self._h, _ptr(shards), _ptr(present), _ptr(sealed_len),
+                                                        _ptr(keys), _ptr(offset), _ptr(length), stride, _ptr(out),
+                                                        out_stride, _ptr(status), len(sealed_len), kind, st),
+                           (E_UNRECOVERABLE, E_AUTH))
+
+    def open_range_stripes(self, stripes, present, sealed_len, keys, offset, length, stride, outs, status):
+        """HOST gather form: `stripes` / `outs` are lists of numpy arrays, one per request"""
+        n = len(stripes)
+        sp = (C.c_void_p * n)(*[a.ctypes.data for a in stripes])
+        op = (C.c_void_p * n)(*[a.ctypes.data for a in outs])
+        return self._check(self._L.garage_ec_open_range_stripes(self._h, C.cast(sp, C.c_void_p), _ptr(present),
+                                                                _ptr(sealed_len), _ptr(keys), _ptr(offset),
+                                                                _ptr(length), stride, C.cast(op, C.c_void_p),
+                                                                _ptr(status), n),
                            (E_UNRECOVERABLE, E_AUTH))
 
     # -- harness utilities

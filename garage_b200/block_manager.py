@@ -25,6 +25,7 @@ SYMBOLS = [
     "garage_bm_resync_step", "garage_bm_list_resync_errors", "garage_bm_resync_retry_now", "garage_bm_block_info",
     "garage_bm_debug_set_clock_ms", "garage_bm_get_resync_metrics",
     "garage_bm_rpc_put_block_sealed", "garage_bm_rpc_get_block_opened", "garage_bm_get_sealed_metrics",
+    "garage_bm_rpc_get_block_range_opened", "garage_bm_get_sealed_range_metrics",
 ]
 SUM_BLAKE2, SUM_ADLER8 = 0, 1
 
@@ -112,6 +113,12 @@ class SealedMetrics(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in (
         "sealed_puts", "sealed_batches", "opened_gets", "opened_auth_failures", "opened_fallbacks", "seal_call_us",
         "open_call_us")]
+
+
+class SealedRangeMetrics(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in (
+        "gets", "degraded_gets", "bytes_read", "bytes_fetched", "auth_failures", "fallbacks", "call_us",
+        "open_range_call_us")]
 
 
 class ResyncError(C.Structure):
@@ -202,6 +209,9 @@ def load_library():
         L.garage_bm_rpc_get_block_opened.argtypes = [vp, vp, vp, vp, sz, C.POINTER(sz)]
         L.garage_bm_get_sealed_metrics.argtypes = [vp, C.POINTER(SealedMetrics)]
         L.garage_bm_get_sealed_metrics.restype = None
+        L.garage_bm_rpc_get_block_range_opened.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, vp, sz, C.POINTER(sz)]
+        L.garage_bm_get_sealed_range_metrics.argtypes = [vp, C.POINTER(SealedRangeMetrics)]
+        L.garage_bm_get_sealed_range_metrics.restype = None
         _lib = L
     return _lib
 
@@ -318,6 +328,19 @@ class BlockManager:
         mt = SealedMetrics()
         self._L.garage_bm_get_sealed_metrics(self._h, C.byref(mt))
         return {n: getattr(mt, n) for n, _ in SealedMetrics._fields_}
+
+    def rpc_get_block_range_opened(self, hash32, key32, offset, length):
+        """(rc, plaintext bytes [offset, offset + length) of an SSE-C block or None)"""
+        out = np.empty(max(length, 1), dtype=np.uint8)
+        n = C.c_size_t(0)
+        rc = self._L.garage_bm_rpc_get_block_range_opened(self._h, self._hp(hash32), C.c_char_p(bytes(key32)), offset,
+                                                          length, C.c_void_p(out.ctypes.data), length, C.byref(n))
+        return rc, (out[: n.value].copy() if rc == OK else None)
+
+    def get_sealed_range_metrics(self):
+        mt = SealedRangeMetrics()
+        self._L.garage_bm_get_sealed_range_metrics(self._h, C.byref(mt))
+        return {n: getattr(mt, n) for n, _ in SealedRangeMetrics._fields_}
 
     def rpc_get_block_range(self, hash32, offset, length):
         """(rc, bytes [offset, offset + length) of the block or None)"""

@@ -1611,6 +1611,9 @@ struct garage_bm {
     std::atomic<uint64_t> convert_blocks{0}, convert_bytes_read{0}, convert_bytes_written{0}, convert_errors{0},
         convert_call_us{0}, legacy_gets{0}, legacy_deleted{0}, range_gets{0}, range_degraded{0}, range_bytes_read{0},
         range_bytes_fetched{0};
+    std::atomic<uint64_t> sealed_range_gets{0}, sealed_range_degraded{0}, sealed_range_bytes_read{0},
+        sealed_range_bytes_fetched{0}, sealed_range_auth_failures{0}, sealed_range_fallbacks{0}, sealed_range_us{0},
+        sealed_range_call_us{0};
     std::atomic<uint64_t> sealed_puts{0}, sealed_batches{0}, opened_gets{0}, opened_auth_failures{0}, opened_fallbacks{0},
         seal_call_us{0}, open_call_us{0};
     std::atomic<uint64_t> layout_shards_copied{0}, layout_shards_rebuilt{0}, layout_bytes_read{0}, layout_bytes_written{0},
@@ -1938,10 +1941,11 @@ struct garage_bm {
 
     void run_reconstruct(int w, std::vector<ReconItem *> &all)
     {
-        std::vector<ReconItem *> b, rb, ob;  // whole-shard rebuilds, ranged GETs, opened GETs
-        for (ReconItem *it : all) (it->open ? ob : it->range ? rb : b).push_back(it);
+        std::vector<ReconItem *> b, rb, ob, orb;  // whole-shard rebuilds, ranged GETs, opened GETs, ranged opened GETs
+        for (ReconItem *it : all) (it->open && it->range ? orb : it->open ? ob : it->range ? rb : b).push_back(it);
         if (!rb.empty()) run_decode_range(w, rb);
         if (!ob.empty()) run_open(w, ob);
+        if (!orb.empty()) run_open_range(w, orb);
         if (b.empty()) return;
         const size_t n = b.size();
         std::vector<uint8_t *> stripes(n);
@@ -2006,6 +2010,39 @@ struct garage_bm {
                     : status[i]                          ? status[i]
                                                          : GARAGE_BM_OK;
             b[i]->plain_len = plen[i];
+            b[i]->fulfilled = true;
+            b[i]->done.set_value(r);
+        }
+    }
+
+    // the ranged opened GETs of a dispatcher batch: one garage_ec_open_range_stripes on their stripe slots.  Per item:
+    // OK, GARAGE_EC_E_AUTH or GARAGE_BM_E_MISSING_BLOCK
+    void run_open_range(int w, std::vector<ReconItem *> &b)
+    {
+        const size_t n = b.size();
+        std::vector<const uint8_t *> stripes(n);
+        std::vector<uint8_t *> outs(n);
+        std::vector<uint8_t> present(n * tot), keys(n * 32);
+        std::vector<uint32_t> sealed(n), offs(n), lens(n);
+        std::vector<int32_t> status(n, 0);
+        for (size_t i = 0; i < n; i++) {
+            stripes[i] = b[i]->stripe;
+            outs[i] = b[i]->out;
+            sealed[i] = b[i]->block_len;
+            offs[i] = b[i]->off;
+            lens[i] = b[i]->len;
+            memcpy(present.data() + i * tot, b[i]->present, tot);
+            memcpy(keys.data() + i * 32, b[i]->key, 32);
+        }
+        const auto t0 = Clock::now();
+        const int rc = garage_ec_open_range_stripes(rec_ctx[w], stripes.data(), present.data(), sealed.data(), keys.data(),
+                                                    offs.data(), lens.data(), slot_stride, outs.data(), status.data(), n);
+        sealed_range_call_us += (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count();
+        wipe_secret(keys.data(), keys.size());
+        for (size_t i = 0; i < n; i++) {
+            int r = rc;
+            if (rc == GARAGE_EC_OK || rc == GARAGE_EC_E_UNRECOVERABLE || rc == GARAGE_EC_E_AUTH)
+                r = status[i] == GARAGE_EC_E_UNRECOVERABLE ? GARAGE_BM_E_MISSING_BLOCK : status[i] ? status[i] : GARAGE_BM_OK;
             b[i]->fulfilled = true;
             b[i]->done.set_value(r);
         }
@@ -2473,19 +2510,19 @@ struct garage_bm {
         return rc;
     }
 
-    // Bytes [off, off + len) of block h into out (S3 GetObject with a Range header, body_from_blocks_range; the
-    // source ranges of UploadPartCopy).  The block length comes from the first configured-code shard header that
-    // reads.  garage_ec_range_plan names the runs to fetch; each holder reads only the tag span covering its runs
-    // (garage_ec_tag_span) and checks it against the shard's tag; a span that fails quarantines its shard, queues its
-    // resync, and the plan is recomputed without it.  A range whose touched data shards are all present never
-    // touches the GPU; the others go through the reconstruct dispatchers (garage_ec_decode_range_stripes).
-    // Integrity: a ranged read is proven by the shard tags only.  The block's blake2sum needs the whole block, so a
-    // self-consistent stale shard is found by the deep scrub (DESIGN.md section 5.4), not here.  A range equal to the
-    // whole block is rpc_get_block, with its content-hash check and stale-shard hunt; so is a block held only under a
-    // previous code or as replicas, which is then sliced.
-    int rpc_get_block_range(const Hash &h, uint32_t off, uint32_t len, uint8_t *out, size_t cap, size_t *out_len)
+    // The gather of the ranged GETs.  The block length and tag kind come from the first configured-code shard header
+    // that reads (a bad one quarantines its shard); pre(block_len) then returns 0 to go on, kRangeWhole or an error to
+    // stop with.  plan(present, block_len, runs, cap, &n, &gpu) names the runs to fetch (garage_ec_range_plan's format);
+    // each holder reads only the tag span covering its runs (garage_ec_tag_span) into `slot` and checks it against the
+    // shard's tag; a span that fails, or a shard whose header does not match, quarantines its shard and the plan is
+    // recomputed without it.  On GARAGE_BM_OK: `present` is the final plan's presence map, *gpu its needs_gpu, and
+    // `fetched_ctr` has the planned run bytes added.  kRangeNoHeader if no configured-code header reads.
+    static constexpr int kRangeWhole = 1, kRangeNoHeader = 2;
+    using RangePlanFn = std::function<int(const uint8_t *, uint32_t, garage_ec_range *, size_t, size_t *, int *)>;
+    int gather_ranged(const Hash &h, uint8_t *slot, const std::function<int(uint32_t)> &pre, const RangePlanFn &plan,
+                      uint32_t &block_len, uint8_t *present, int *gpu, std::atomic<uint64_t> &read_ctr,
+                      std::atomic<uint64_t> &fetched_ctr)
     {
-        range_gets++;
         const Code &cd = codes[0];
         const int tot = cd.tot;
         constexpr int kMaxSrc = GARAGE_BM_MAX_LAYOUT_VERSIONS;
@@ -2493,7 +2530,6 @@ struct garage_bm {
             cur[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
         const bool by_index = shard_sources(h, 0, src, nsrc);
         auto left = [&](int i) { return cur[i] < nsrc[i]; };
-        // the block length and tag kind: the first header that reads (a bad one quarantines its shard)
         ShardMeta m0;
         bool have_len = false;
         for (int i = 0; i < tot && !have_len; i++) {
@@ -2519,29 +2555,18 @@ struct garage_bm {
                 cur[i]++;
             }
         }
-        auto sliced = [&]() -> int {  // the whole block through rpc_get_block, then the range of it
-            std::vector<uint8_t> whole(stored_max());
-            size_t n = 0;
-            const int rc = rpc_get_block(h, whole.data(), whole.size(), &n);
-            if (rc != GARAGE_BM_OK) return rc;
-            if ((uint64_t)off + len > n || len > cap) return GARAGE_EC_E_INVALID;
-            memcpy(out, whole.data() + off, len);
-            *out_len = len;
-            return GARAGE_BM_OK;
-        };
-        if (!have_len) return has_legacy() ? sliced() : GARAGE_BM_E_MISSING_BLOCK;
-        const uint32_t block_len = m0.block_len, L = (uint32_t)shard_len_of(block_len);
-        if ((uint64_t)off + len > block_len || len > cap) return GARAGE_EC_E_INVALID;
-        if (off == 0 && len == block_len) return sliced();
-        SlotLease slot(stripe_slots);
-        uint8_t fetched[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0}, guess[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
+        if (!have_len) return kRangeNoHeader;
+        block_len = m0.block_len;
+        const uint32_t L = (uint32_t)shard_len_of(block_len);
+        int rc = pre(block_len);
+        if (rc) return rc;
+        uint8_t fetched[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
         uint32_t f_lo[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M], f_hi[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
-        std::vector<garage_ec_range> runs((size_t)tot * ((cd.clay ? cd.quantum / 16 : 1) + 2));
+        std::vector<garage_ec_range> runs((size_t)tot * ((cd.clay ? cd.quantum / 16 : 1) + 2) * 2);
         size_t nr = 0;
-        int gpu = 0;
         for (;;) {
-            for (int i = 0; i < tot; i++) guess[i] = fetched[i] || left(i);
-            const int rc = garage_ec_range_plan(cd.ctx, guess, block_len, off, len, runs.data(), runs.size(), &nr, &gpu);
+            for (int i = 0; i < tot; i++) present[i] = fetched[i] || left(i);
+            rc = plan(present, block_len, runs.data(), runs.size(), &nr, gpu);
             if (rc == GARAGE_EC_E_UNRECOVERABLE) return GARAGE_BM_E_MISSING_BLOCK;
             if (rc != GARAGE_EC_OK) return rc;
             uint32_t lo[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M], hi[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
@@ -2559,9 +2584,9 @@ struct garage_bm {
                 while (left(i)) {  // a shard's runs come from one source
                     const int node = src[i][cur[i]], fidx = by_index ? i : -1;
                     ShardMeta mt;
-                    bool got = read_shard_into(node, h, slot.p + (size_t)i * slot_stride + so, slot_stride - so, mt, true, 0,
+                    bool got = read_shard_into(node, h, slot + (size_t)i * slot_stride + so, slot_stride - so, mt, true, 0,
                                                fidx, ShardSpan::bytes(so, sl));
-                    if (got) range_bytes_read += sl;
+                    if (got) read_ctr += sl;
                     if (got && (mt.index != i || mt.block_len != block_len || mt.shard_len != L)) {
                         quarantine(node, h, 0, fidx);  // a stale or misplaced shard with a self-consistent tag
                         got = false;
@@ -2578,26 +2603,149 @@ struct garage_bm {
             }
             if (!replan) break;
         }
-        for (size_t x = 0; x < nr; x++) range_bytes_fetched += runs[x].len;
-        *out_len = len;
-        if (!gpu) {  // every touched data shard is present: their range bytes, no GPU
-            for (uint64_t j = off / L, end = (uint64_t)off + len; j * L < end; j++) {
-                const uint64_t base = j * L, c0 = std::max<uint64_t>(off, base) - base, c1 = std::min<uint64_t>(end, base + L) - base;
-                memcpy(out + (base + c0 - off), slot.p + j * slot_stride + c0, c1 - c0);
+        for (size_t x = 0; x < nr; x++) fetched_ctr += runs[x].len;
+        return GARAGE_BM_OK;
+    }
+
+    // Bytes [off, off + len) of block h into out (S3 GetObject with a Range header, body_from_blocks_range; the
+    // source ranges of UploadPartCopy), gathered by gather_ranged with garage_ec_range_plan.  A range whose touched data
+    // shards are all present never touches the GPU; the others go through the reconstruct dispatchers
+    // (garage_ec_decode_range_stripes).
+    // Integrity: a ranged read is proven by the shard tags only.  The block's blake2sum needs the whole block, so a
+    // self-consistent stale shard is found by the deep scrub (DESIGN.md section 5.4), not here.  A range equal to the
+    // whole block is rpc_get_block, with its content-hash check and stale-shard hunt; so is a block held only under a
+    // previous code or as replicas, which is then sliced.
+    int rpc_get_block_range(const Hash &h, uint32_t off, uint32_t len, uint8_t *out, size_t cap, size_t *out_len)
+    {
+        range_gets++;
+        auto sliced = [&]() -> int {  // the whole block through rpc_get_block, then the range of it
+            std::vector<uint8_t> whole(stored_max());
+            size_t n = 0;
+            const int rc = rpc_get_block(h, whole.data(), whole.size(), &n);
+            if (rc != GARAGE_BM_OK) return rc;
+            if ((uint64_t)off + len > n || len > cap) return GARAGE_EC_E_INVALID;
+            memcpy(out, whole.data() + off, len);
+            *out_len = len;
+            return GARAGE_BM_OK;
+        };
+        uint8_t present[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
+        uint32_t block_len = 0;
+        int gpu = 0;
+        {
+            SlotLease slot(stripe_slots);
+            const int rc = gather_ranged(
+                h, slot.p,
+                [&](uint32_t bl) -> int {
+                    if ((uint64_t)off + len > bl || len > cap) return GARAGE_EC_E_INVALID;
+                    return off == 0 && len == bl ? kRangeWhole : 0;
+                },
+                [&](const uint8_t *pr, uint32_t bl, garage_ec_range *r, size_t c, size_t *nr, int *g) {
+                    return garage_ec_range_plan(codes[0].ctx, pr, bl, off, len, r, c, nr, g);
+                },
+                block_len, present, &gpu, range_bytes_read, range_bytes_fetched);
+            if (rc == GARAGE_BM_OK) {
+                *out_len = len;
+                if (!gpu) {  // every touched data shard is present: their range bytes, no GPU
+                    const uint64_t L = shard_len_of(block_len);
+                    for (uint64_t j = off / L, end = (uint64_t)off + len; j * L < end; j++) {
+                        const uint64_t base = j * L, c0 = std::max<uint64_t>(off, base) - base,
+                                       c1 = std::min<uint64_t>(end, base + L) - base;
+                        memcpy(out + (base + c0 - off), slot.p + j * slot_stride + c0, c1 - c0);
+                    }
+                    return GARAGE_BM_OK;
+                }
+                range_degraded++;
+                ReconItem it;
+                it.stripe = slot.p;
+                it.stride = slot_stride;
+                it.block_len = block_len;
+                memcpy(it.present, present, tot);
+                it.range = true;
+                it.off = off;
+                it.len = len;
+                it.out = out;
+                return rec_batcher->submit(it);
             }
+            if (rc == kRangeNoHeader && !has_legacy()) return GARAGE_BM_E_MISSING_BLOCK;
+            if (rc != kRangeWhole && rc != kRangeNoHeader) return rc;
+        }
+        return sliced();
+    }
+
+    // Plaintext bytes [off, off + len) of SSE-C block h sealed under key (a ranged GET or UploadPartCopy of an SSE-C
+    // object, DESIGN.md sections 2.7 and 5.10), gathered by gather_ranged with garage_ec_open_range_plan: only the
+    // nonce prefix and the chunks the range touches are fetched, and one garage_ec_open_range_stripes call of the
+    // reconstruct dispatchers rebuilds, checks and decrypts them.  The whole plaintext, and blocks held only under a
+    // previous code or as replicas, go through rpc_get_block_opened (content hash checked) and are sliced.  A touched
+    // chunk that fails its tag is either a wrong key or a self-consistent stale shard, and at range level the two look
+    // alike: one whole-block rpc_get_block_opened tells them apart (its hash check hunts and quarantines a stale
+    // shard); its E_AUTH is the answer.
+    int rpc_get_block_range_opened(const Hash &h, const uint8_t *key, uint32_t off, uint32_t len, uint8_t *out,
+                                   size_t cap, size_t *out_len)
+    {
+        const auto t0 = Clock::now();
+        struct Timer {
+            std::atomic<uint64_t> &us;
+            Clock::time_point t0;
+            ~Timer() { us += (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count(); }
+        } timer{sealed_range_us, t0};
+        sealed_range_gets++;
+        auto sliced = [&]() -> int {  // the whole plaintext through rpc_get_block_opened, then the range of it
+            std::vector<uint8_t> whole(stored_max());
+            size_t n = 0;
+            const int rc = rpc_get_block_opened(h, key, whole.data(), whole.size(), &n);
+            if (rc != GARAGE_BM_OK) return rc;
+            if ((uint64_t)off + len > n || len > cap) return GARAGE_EC_E_INVALID;
+            memcpy(out, whole.data() + off, len);
+            *out_len = len;
+            return GARAGE_BM_OK;
+        };
+        uint8_t present[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
+        uint32_t block_len = 0;
+        int gpu = 0, rc;
+        {
+            SlotLease slot(stripe_slots);
+            rc = gather_ranged(
+                h, slot.p,
+                [&](uint32_t bl) -> int {
+                    uint32_t so, sl, c0, nch;
+                    const int r = garage_ec_sealed_range(bl, off, len, &so, &sl, &c0, &nch);
+                    if (r) return r;
+                    if (len > cap) return GARAGE_EC_E_INVALID;
+                    const uint64_t P = bl - 8 - 16ull * ((bl - 8 + 4111) / 4112);
+                    return (off == 0 && len == P) || !len ? kRangeWhole : 0;
+                },
+                [&](const uint8_t *pr, uint32_t bl, garage_ec_range *r, size_t c, size_t *nr, int *g) {
+                    return garage_ec_open_range_plan(codes[0].ctx, pr, bl, off, len, r, c, nr, g);
+                },
+                block_len, present, &gpu, sealed_range_bytes_read, sealed_range_bytes_fetched);
+            if (rc == GARAGE_BM_OK) {
+                if (gpu) sealed_range_degraded++;
+                ReconItem it;
+                it.stripe = slot.p;
+                it.stride = slot_stride;
+                it.block_len = block_len;
+                memcpy(it.present, present, tot);
+                it.open = it.range = true;
+                it.key = key;
+                it.off = off;
+                it.len = len;
+                it.out = out;
+                rc = rec_batcher->submit(it);
+                if (rc == GARAGE_BM_OK) *out_len = len;
+            }
+        }
+        if (rc == kRangeWhole && !len) {  // a well-framed block's empty range
+            *out_len = 0;
             return GARAGE_BM_OK;
         }
-        range_degraded++;
-        ReconItem it;
-        it.stripe = slot.p;
-        it.stride = slot_stride;
-        it.block_len = block_len;
-        memcpy(it.present, guess, tot);
-        it.range = true;
-        it.off = off;
-        it.len = len;
-        it.out = out;
-        return rec_batcher->submit(it);
+        if (rc == GARAGE_EC_E_AUTH || rc == kRangeWhole || (rc == kRangeNoHeader && has_legacy())) {
+            if (rc == GARAGE_EC_E_AUTH) sealed_range_fallbacks++;
+            rc = sliced();
+            if (rc == GARAGE_EC_E_AUTH) sealed_range_auth_failures++;
+            return rc;
+        }
+        return rc == kRangeNoHeader ? GARAGE_BM_E_MISSING_BLOCK : rc;
     }
 
     // the block from the first of its first legacy_rf ring nodes whose replica matches its content hash (a replica
@@ -4618,6 +4766,26 @@ void garage_bm_get_sealed_metrics(garage_bm *bm, garage_bm_sealed_metrics *o)
     o->opened_fallbacks = bm->opened_fallbacks;
     o->seal_call_us = bm->seal_call_us;
     o->open_call_us = bm->open_call_us;
+}
+
+int garage_bm_rpc_get_block_range_opened(garage_bm *bm, const uint8_t hash[32], const uint8_t *key32, uint32_t offset,
+                                         uint32_t len, uint8_t *out, size_t cap, size_t *out_len)
+{
+    if (!bm || !hash || !key32 || !out_len || (!out && len)) return GARAGE_EC_E_INVALID;
+    BM_GUARD(bm->rpc_get_block_range_opened(to_hash(hash), key32, offset, len, out, cap, out_len));
+}
+
+void garage_bm_get_sealed_range_metrics(garage_bm *bm, garage_bm_sealed_range_metrics *o)
+{
+    if (!bm || !o) return;
+    o->gets = bm->sealed_range_gets;
+    o->degraded_gets = bm->sealed_range_degraded;
+    o->bytes_read = bm->sealed_range_bytes_read;
+    o->bytes_fetched = bm->sealed_range_bytes_fetched;
+    o->auth_failures = bm->sealed_range_auth_failures;
+    o->fallbacks = bm->sealed_range_fallbacks;
+    o->call_us = bm->sealed_range_us;
+    o->open_range_call_us = bm->sealed_range_call_us;
 }
 
 int garage_bm_rpc_get_block_range(garage_bm *bm, const uint8_t hash[32], uint32_t offset, uint32_t len, uint8_t *out,

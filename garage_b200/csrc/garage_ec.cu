@@ -1689,21 +1689,17 @@ void for_each_rebuilt_piece(const RangeWindow &r, size_t c0, size_t bytes, F &&f
     }
 }
 
-}  // namespace
-extern "C" {
 
-int garage_ec_range_plan(const garage_ec_ctx *ctx, const uint8_t *present, uint32_t block_len, uint32_t offset,
-                         uint32_t len, garage_ec_range *ranges, size_t cap, size_t *n_ranges, int *needs_gpu)
+// The unmerged runs garage_ec_range_plan names for one request, appended to `runs`; *needs_gpu |= an absent touched
+// data shard.
+int range_runs(const garage_ec_ctx *ctx, const uint8_t *present, uint32_t block_len, uint32_t offset, uint32_t len,
+               std::vector<garage_ec_range> &runs, int *needs_gpu)
 {
-    if (!ctx || !present || !n_ranges || (cap && !ranges)) return GARAGE_EC_E_INVALID;
-    *n_ranges = 0;
-    if (needs_gpu) *needs_gpu = 0;
     RangeReq q;
     int rc = range_request(ctx, present, block_len, offset, len, UINT64_MAX, &q);
     if (rc) return rc;
-    if (needs_gpu) *needs_gpu = q.r.w ? 1 : 0;
+    if (q.r.w) *needs_gpu = 1;
     if (!q.ok) return GARAGE_EC_E_UNRECOVERABLE;
-    std::vector<garage_ec_range> runs;
     for_each_range_piece(q.r, offset, len, [&](size_t j, size_t c, size_t, size_t bytes) {
         if (present[j]) runs.push_back(garage_ec_range{(uint32_t)j, (uint32_t)c, (uint32_t)bytes});
     });
@@ -1711,6 +1707,12 @@ int garage_ec_range_plan(const garage_ec_ctx *ctx, const uint8_t *present, uint3
         for_each_window_run(ctx, q, (size_t)i, [&](size_t off, size_t, size_t bytes) {
             runs.push_back(garage_ec_range{(uint32_t)i, (uint32_t)off, (uint32_t)bytes});
         });
+    return GARAGE_EC_OK;
+}
+
+// runs in shard then offset order, overlapping or adjacent runs merged, into ranges[0, cap)
+int merge_runs(std::vector<garage_ec_range> &runs, garage_ec_range *ranges, size_t cap, size_t *n_ranges)
+{
     std::sort(runs.begin(), runs.end(), [](const garage_ec_range &a, const garage_ec_range &b) {
         return a.shard != b.shard ? a.shard < b.shard : a.offset < b.offset;
     });
@@ -1725,6 +1727,23 @@ int garage_ec_range_plan(const garage_ec_ctx *ctx, const uint8_t *present, uint3
     for (size_t x = 0; x < merged.size() && x < cap; x++) ranges[x] = merged[x];
     *n_ranges = merged.size();
     return merged.size() > cap ? GARAGE_EC_E_INVALID : GARAGE_EC_OK;
+}
+
+}  // namespace
+extern "C" {
+
+int garage_ec_range_plan(const garage_ec_ctx *ctx, const uint8_t *present, uint32_t block_len, uint32_t offset,
+                         uint32_t len, garage_ec_range *ranges, size_t cap, size_t *n_ranges, int *needs_gpu)
+{
+    if (!ctx || !present || !n_ranges || (cap && !ranges)) return GARAGE_EC_E_INVALID;
+    *n_ranges = 0;
+    if (needs_gpu) *needs_gpu = 0;
+    std::vector<garage_ec_range> runs;
+    int gpu = 0;
+    const int rc = range_runs(ctx, present, block_len, offset, len, runs, &gpu);
+    if (needs_gpu) *needs_gpu = gpu;
+    if (rc) return rc;
+    return merge_runs(runs, ranges, cap, n_ranges);
 }
 
 // HOST ranged decode.  stripes / outs != NULL: the gather form (garage_ec_decode_range_stripes).  Only the window runs
@@ -1830,51 +1849,75 @@ static int decode_range_host(garage_ec_ctx *ctx, const uint8_t *shards, const ui
     return any_bad ? GARAGE_EC_E_UNRECOVERABLE : GARAGE_EC_OK;
 }
 
-// DEVICE ranged decode: geometry, pack the window runs into sub-stripes, the code's own decode on them, join
+// DEVICE ranged decode: geometry, pack the window runs into sub-stripes, the code's own decode on them, join.  Request
+// s reads stripe s >> shift of `shards`; `sc` holds a RangeScratch.
+struct RangeScratch {
+    size_t o_sub, o_geo, o_len, o_want, o_st, o_plan, bytes;
+    RangeScratch(const garage_ec_ctx *ctx, size_t n, size_t stride)
+    {
+        const size_t tot = ctx->k + ctx->m;
+        SmallLayout sl;
+        o_sub = sl.take(n * tot * stride);
+        o_geo = sl.take(n * 16);
+        o_len = sl.take(n * 4);
+        o_want = sl.take(n * tot);
+        o_st = sl.take(n * 4);
+        o_plan = sl.take(plan_scratch_bytes(ctx, n));
+        bytes = sl.bytes;
+    }
+};
+static int run_decode_range(garage_ec_ctx *ctx, const uint8_t *shards, uint32_t shift, const uint8_t *present,
+                            const uint32_t *block_len, const uint32_t *offset, const uint32_t *len, size_t stride,
+                            uint8_t *out, size_t out_stride, int32_t *status, size_t n, uint8_t *sc, cudaStream_t st)
+{
+    const size_t pitch = (size_t)(ctx->k + ctx->m) * stride;
+    const RangeScratch rs(ctx, n, stride);
+    const size_t o_sub = rs.o_sub, o_geo = rs.o_geo, o_len = rs.o_len, o_want = rs.o_want, o_st = rs.o_st,
+                 o_plan = rs.o_plan;
+    RangeParams q;
+    memset(&q, 0, sizeof(q));
+    q.shards = shards;
+    q.sub = sc + o_sub;
+    q.present = present;
+    q.block_len = block_len;
+    q.offset = offset;
+    q.len = len;
+    q.out = out;
+    q.geo = reinterpret_cast<uint4 *>(sc + o_geo);
+    q.sub_len = reinterpret_cast<uint32_t *>(sc + o_len);
+    q.want = sc + o_want;
+    q.plan_status = reinterpret_cast<const int32_t *>(sc + o_st);
+    q.status = status;
+    q.pitch = pitch;
+    q.out_stride = out_stride;
+    q.stride = (uint32_t)stride;
+    q.k = (uint32_t)ctx->k;
+    q.m = (uint32_t)ctx->m;
+    q.n = (uint32_t)n;
+    q.quantum = ctx->quantum;
+    q.alpha = ctx->clay ? (uint32_t)ctx->cg.alpha : 1u;
+    q.pb = ctx->pb ? 1u : 0u;
+    q.shift = shift;
+    const unsigned per_req = (unsigned)std::min<size_t>(n, (size_t)ctx->sm_count * 8);
+    range_geo_kernel<<<(unsigned)std::min<size_t>((n + 255) / 256, (size_t)ctx->sm_count * 4), 256, 0, st>>>(q);
+    range_pack_kernel<<<per_req, 256, 0, st>>>(q);
+    ctx->launches.fetch_add(2, std::memory_order_relaxed);
+    CU_TRY(ctx, cudaGetLastError());
+    int r = run_reconstruct(ctx, q.sub, present, q.want, reinterpret_cast<int32_t *>(sc + o_st), q.sub_len, stride, n,
+                            sc + o_plan, st);
+    if (r) return r;
+    range_join_kernel<<<per_req, 256, 0, st>>>(q);
+    ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    CU_TRY(ctx, cudaGetLastError());
+    return GARAGE_EC_OK;
+}
 static int decode_range_device(garage_ec_ctx *ctx, const uint8_t *shards, const uint8_t *present,
                                const uint32_t *block_len, const uint32_t *offset, const uint32_t *len, size_t stride,
                                uint8_t *out, size_t out_stride, int32_t *status, size_t n, cudaStream_t st)
 {
-    const size_t tot = ctx->k + ctx->m, pitch = tot * stride;
-    SmallLayout sl;
-    const size_t o_sub = sl.take(n * pitch), o_geo = sl.take(n * 16), o_len = sl.take(n * 4), o_want = sl.take(n * tot),
-                 o_st = sl.take(n * 4), o_plan = sl.take(plan_scratch_bytes(ctx, n));
-    return with_stream_scratch(ctx, sl.bytes, st, [&](uint8_t *sc) -> int {
-        RangeParams q;
-        memset(&q, 0, sizeof(q));
-        q.shards = shards;
-        q.sub = sc + o_sub;
-        q.present = present;
-        q.block_len = block_len;
-        q.offset = offset;
-        q.len = len;
-        q.out = out;
-        q.geo = reinterpret_cast<uint4 *>(sc + o_geo);
-        q.sub_len = reinterpret_cast<uint32_t *>(sc + o_len);
-        q.want = sc + o_want;
-        q.plan_status = reinterpret_cast<const int32_t *>(sc + o_st);
-        q.status = status;
-        q.pitch = pitch;
-        q.out_stride = out_stride;
-        q.stride = (uint32_t)stride;
-        q.k = (uint32_t)ctx->k;
-        q.m = (uint32_t)ctx->m;
-        q.n = (uint32_t)n;
-        q.quantum = ctx->quantum;
-        q.alpha = ctx->clay ? (uint32_t)ctx->cg.alpha : 1u;
-        q.pb = ctx->pb ? 1u : 0u;
-        const unsigned per_req = (unsigned)std::min<size_t>(n, (size_t)ctx->sm_count * 8);
-        range_geo_kernel<<<(unsigned)std::min<size_t>((n + 255) / 256, (size_t)ctx->sm_count * 4), 256, 0, st>>>(q);
-        range_pack_kernel<<<per_req, 256, 0, st>>>(q);
-        ctx->launches.fetch_add(2, std::memory_order_relaxed);
-        CU_TRY(ctx, cudaGetLastError());
-        int r = run_reconstruct(ctx, q.sub, present, q.want, reinterpret_cast<int32_t *>(sc + o_st), q.sub_len, stride, n,
-                                sc + o_plan, st);
-        if (r) return r;
-        range_join_kernel<<<per_req, 256, 0, st>>>(q);
-        ctx->launches.fetch_add(1, std::memory_order_relaxed);
-        CU_TRY(ctx, cudaGetLastError());
-        return GARAGE_EC_OK;
+    return with_stream_scratch(ctx, RangeScratch(ctx, n, stride).bytes, st, [&](uint8_t *sc) -> int {
+        return run_decode_range(ctx, shards, 0, present, block_len, offset, len, stride, out, out_stride, status, n, sc,
+                                st);
     });
 }
 
@@ -2733,8 +2776,8 @@ int sse_launch_setup(garage_ec_ctx *ctx, const uint8_t *keys, sse::SseKey *ks, s
 template <int MODE>
 int sse_launch_chunks(garage_ec_ctx *ctx, sse::ChunkParams q, cudaStream_t st)
 {
-    // work items are (block, chunk) pairs over the chunks a block of plain_stride bytes can have
-    q.cmax = (uint32_t)std::max<unsigned long long>(1, (q.plain_stride + sse::kChunk - 1) / sse::kChunk);
+    // work items are (block, chunk) pairs over the chunks a block of plain_stride bytes can have (ranged: the caller's)
+    if (!q.cmax) q.cmax = (uint32_t)std::max<unsigned long long>(1, (q.plain_stride + sse::kChunk - 1) / sse::kChunk);
     const unsigned long long items = (unsigned long long)q.n * q.cmax;
     const unsigned grid = (unsigned)std::min<unsigned long long>((items + sse::kWarps - 1) / sse::kWarps,
                                                                  (unsigned long long)ctx->sm_count * 4);
@@ -3234,6 +3277,286 @@ int garage_ec_open_stripes(garage_ec_ctx *ctx, uint8_t *const *stripes, const ui
     CU_TRY(ctx, cudaSetDevice(ctx->device));
     return open_host(ctx, nullptr, stripes, present, sealed_len, hashes, keys, nullptr, 0, plains, plain_len_out,
                      hash_bad, status, stride, n);
+}
+
+// --------------------------------------------------------------------------- SSE-C RANGED OPEN (DESIGN.md 2.7, 4.10)
+}  // extern "C"
+namespace {
+
+// The unmerged runs of the prefix B[0, 8) and the span of plaintext bytes [o, o + len) of a block sealed to S bytes,
+// appended to `runs` (garage_ec_range_plan's runs of each); nothing for an empty range.
+int open_range_runs(const garage_ec_ctx *ctx, const uint8_t *present, uint32_t S, uint32_t o, uint32_t len,
+                    std::vector<garage_ec_range> &runs, int *needs_gpu)
+{
+    uint32_t so, sl, c0, nch;
+    int rc = sse::sealed_range(S, o, len, &so, &sl, &c0, &nch);
+    if (rc || !len) return rc;
+    rc = range_runs(ctx, present, S, 0, sse::kPrefix, runs, needs_gpu);
+    return rc ? rc : range_runs(ctx, present, S, so, sl, runs, needs_gpu);
+}
+
+// Device scratch of a ranged open of n requests: key material first (one memset clears every secret), then the rows
+// (2s: the prefix, 2s + 1: the span), the two decodes per request and their arguments.  A range of at most out_stride
+// bytes touches at most out_stride / 4096 + 2 chunks: that bounds a span row.
+struct OpenRangeScratch {
+    size_t cmax, row_pitch, o_keys, o_rows, o_dec, o_blen2, o_off2, o_len2, o_present2, o_st2, bytes;
+    OpenRangeScratch(const garage_ec_ctx *ctx, size_t n, size_t stride, size_t out_stride)
+    {
+        cmax = out_stride / sse::kChunk + 2;
+        row_pitch = align_up(cmax * sse::kFrame, 16);
+        SmallLayout sl;
+        o_keys = sl.take(n * sizeof(sse::SseKey));
+        o_rows = sl.take(2 * n * row_pitch);
+        o_dec = sl.take(RangeScratch(ctx, 2 * n, stride).bytes);
+        o_blen2 = sl.take(2 * n * 4);
+        o_off2 = sl.take(2 * n * 4);
+        o_len2 = sl.take(2 * n * 4);
+        o_present2 = sl.take(2 * n * (size_t)(ctx->k + ctx->m));
+        o_st2 = sl.take(2 * n * 4);
+        bytes = sl.bytes;
+    }
+};
+
+// Open plaintext ranges of n stored blocks on the device: framing and geometry, key schedules, each request's prefix
+// and span decoded into its two rows, every touched chunk's tag, then the range bytes of the requests that passed.
+// The caller zeroes the key material of `sc`.
+int run_open_range(garage_ec_ctx *ctx, const uint8_t *shards, const uint8_t *present, const uint32_t *sealed,
+                   const uint8_t *keys, const uint32_t *offset, const uint32_t *len, size_t stride, uint8_t *out,
+                   size_t out_stride, int32_t *status, size_t n, uint8_t *sc, cudaStream_t st)
+{
+    const OpenRangeScratch o(ctx, n, stride, out_stride);
+    sse::SseKey *ks = reinterpret_cast<sse::SseKey *>(sc + o.o_keys);
+    uint32_t *blen2 = reinterpret_cast<uint32_t *>(sc + o.o_blen2), *off2 = reinterpret_cast<uint32_t *>(sc + o.o_off2),
+             *len2 = reinterpret_cast<uint32_t *>(sc + o.o_len2);
+    int32_t *st2 = reinterpret_cast<int32_t *>(sc + o.o_st2);
+    sse::RangeLensParams lp;
+    memset(&lp, 0, sizeof(lp));
+    lp.sealed = sealed;
+    lp.offset = offset;
+    lp.len = len;
+    lp.present = present;
+    lp.status = status;
+    lp.blen2 = blen2;
+    lp.off2 = off2;
+    lp.len2 = len2;
+    lp.present2 = sc + o.o_present2;
+    lp.out_stride = out_stride;
+    lp.stride = (uint32_t)stride;
+    lp.k = (uint32_t)ctx->k;
+    lp.m = (uint32_t)ctx->m;
+    lp.n = (uint32_t)n;
+    lp.quantum = ctx->quantum;
+    sse::sse_range_lens_kernel<<<(unsigned)std::min<size_t>((n + 255) / 256, (size_t)ctx->sm_count * 4), 256, 0, st>>>(lp);
+    ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    CU_TRY(ctx, cudaGetLastError());
+    int rc = sse_launch_setup(ctx, keys, ks, n, st);
+    if (!rc)
+        rc = run_decode_range(ctx, shards, 1, sc + o.o_present2, blen2, off2, len2, stride, sc + o.o_rows, o.row_pitch,
+                              st2, 2 * n, sc + o.o_dec, st);
+    if (rc) return rc;
+    sse::ChunkParams q;
+    memset(&q, 0, sizeof(q));
+    q.plain_out = out;
+    q.plain_stride = out_stride;
+    q.rows = sc + o.o_rows;
+    q.row_pitch = o.row_pitch;
+    q.offset = offset;
+    q.len = len;
+    q.blen = sealed;
+    q.ks = ks;
+    q.status = status;
+    q.rec_status = st2;
+    q.stride = (uint32_t)stride;
+    q.k = (uint32_t)ctx->k;
+    q.m = (uint32_t)ctx->m;
+    q.n = (uint32_t)n;
+    q.cmax = (uint32_t)o.cmax;
+    rc = sse_launch_chunks<sse::kRangeCheck>(ctx, q, st);
+    if (!rc) rc = sse_launch_chunks<sse::kRangeOpen>(ctx, q, st);
+    return rc;
+}
+
+// HOST ranged open.  stripes / outs != NULL: the gather form.  Only the planned runs of the prefix and the span go up
+// (ciphertext: the present ones too), into a stripe of the lane's buffer; only the len plaintext bytes come down.
+int open_range_host(garage_ec_ctx *ctx, const uint8_t *shards, const uint8_t *const *stripes, const uint8_t *present,
+                    const uint32_t *sealed, const uint8_t *keys, const uint32_t *offset, const uint32_t *len,
+                    size_t stride, uint8_t *out, size_t out_stride, uint8_t *const *outs, int32_t *status, size_t n)
+{
+    const size_t tot = ctx->k + ctx->m;
+    auto shard_at = [&](size_t s, size_t i) { return stripes ? stripes[s] + i * stride : shards + (s * tot + i) * stride; };
+    auto out_at = [&](size_t s) { return outs ? outs[s] : out + s * out_stride; };
+    uint32_t max_len = 0;
+    for (size_t s = 0; s < n; s++) {
+        uint32_t so, sl, c0, nch;
+        if (code_shard_len(ctx, sealed[s]) > stride ||
+            sse::sealed_range(sealed[s], offset[s], len[s], &so, &sl, &c0, &nch) == GARAGE_EC_E_INVALID ||
+            (len[s] && !out_at(s)))
+            return GARAGE_EC_E_INVALID;
+        max_len = std::max(max_len, len[s]);
+    }
+    const size_t opitch = align_up(std::max<size_t>(max_len, 16), 16);
+    LaneKeyWipe wipe;
+    HostPipeline p(ctx, n, tot * stride + opitch);
+    p.before_release = [&wipe] { wipe.wipe(); };
+    const size_t cs = p.cs;
+    SmallLayout sl;
+    const size_t o_key = sl.take(cs * 32), o_present = sl.take(cs * tot), o_sealed = sl.take(cs * 4),
+                 o_off = sl.take(cs * 4), o_len = sl.take(cs * 4), o_status = sl.take(cs * 4);
+    wipe.dev_off = o_key;
+    wipe.dev_bytes = cs * 32;
+    const size_t sh_b = align_up(cs * tot * stride, 256);
+    int rc = p.reserve(sh_b + cs * opitch, sl.bytes);
+    if (rc) return rc;
+    bool pinned = true;
+    for (size_t s = 0; pinned && s < (stripes ? n : 1); s++) pinned = device_addressable_host(shard_at(s, 0));
+    for (size_t s = 0; pinned && outs && s < n; s++) pinned = !len[s] || device_addressable_host(outs[s]);
+    if (!outs) pinned = pinned && device_addressable_host(out);
+    p.up.use_batch = p.down.use_batch = pinned;
+    const OpenRangeScratch osc(ctx, cs, stride, opitch);
+    const Retire retire = [&](const HostChunk &ch) -> int {
+        memset(ch.L->h_key, 0, ch.L->h_key_cap);
+        for (size_t q = 0; q < ch.cnt; q++) {
+            const size_t s = ch.s0 + q;
+            if (!status[s]) p.down.add(out_at(s), ch.L->d_buf + sh_b + q * opitch, len[s]);
+        }
+        int r = p.down.flush(ctx, cudaMemcpyDeviceToHost, ch.L->stream);
+        if (r) return r;
+        CU_TRY(ctx, lane_wait(ctx, *ch.L));
+        return GARAGE_EC_OK;
+    };
+    std::vector<garage_ec_range> runs;
+    rc = p.run(
+        [&](const HostChunk &ch) -> int {
+            HostLane &L = *ch.L;
+            wipe.use(&L);
+            const size_t s0 = ch.s0, cnt = ch.cnt;
+            uint8_t *d_sh = L.d_buf;
+            // H2D: the planned runs; a request the plan cannot serve uploads nothing and fails on the device too
+            for (size_t s = s0; s < s0 + cnt; s++) {
+                int gpu = 0;
+                runs.clear();
+                if (open_range_runs(ctx, present + s * tot, sealed[s], offset[s], len[s], runs, &gpu)) continue;
+                for (const garage_ec_range &r : runs)
+                    p.up.add(d_sh + ((s - s0) * tot + r.shard) * stride + r.offset, shard_at(s, r.shard) + r.offset, r.len);
+            }
+            int r = p.up.flush(ctx, cudaMemcpyHostToDevice, L.stream);
+            if (r) return r;
+            r = lane_key_staging(ctx, L, cs * 32);
+            if (r) return r;
+            memcpy(L.h_key, keys + s0 * 32, cnt * 32);
+            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_key, L.h_key, cnt * 32, cudaMemcpyHostToDevice, L.stream));
+            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_present, present + s0 * tot, cnt * tot, cudaMemcpyHostToDevice, L.stream));
+            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_sealed, sealed + s0, cnt * 4, cudaMemcpyHostToDevice, L.stream));
+            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_off, offset + s0, cnt * 4, cudaMemcpyHostToDevice, L.stream));
+            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_len, len + s0, cnt * 4, cudaMemcpyHostToDevice, L.stream));
+            int32_t *d_status = reinterpret_cast<int32_t *>(L.d_small + o_status);
+            r = with_stream_scratch(ctx, osc.bytes, L.stream, [&](uint8_t *sc) {
+                const int e = run_open_range(ctx, d_sh, L.d_small + o_present,
+                                             reinterpret_cast<const uint32_t *>(L.d_small + o_sealed), L.d_small + o_key,
+                                             reinterpret_cast<const uint32_t *>(L.d_small + o_off),
+                                             reinterpret_cast<const uint32_t *>(L.d_small + o_len), stride, d_sh + sh_b,
+                                             opitch, d_status, cnt, sc, L.stream);
+                const cudaError_t z = cudaMemsetAsync(sc + osc.o_keys, 0, cnt * sizeof(sse::SseKey), L.stream);
+                if (e) return e;
+                return z == cudaSuccess ? GARAGE_EC_OK : set_cuda_error(ctx, z, "cudaMemsetAsync(key material)");
+            });
+            if (r) return r;
+            CU_TRY(ctx, cudaMemsetAsync(L.d_small + o_key, 0, wipe.dev_bytes, L.stream));
+            CU_TRY(ctx, cudaMemcpyAsync(status + s0, d_status, cnt * 4, cudaMemcpyDeviceToHost, L.stream));
+            return GARAGE_EC_OK;
+        },
+        retire);
+    if (!rc) rc = p.drain(retire);
+    wipe.failed = rc != 0;
+    if (rc) return rc;
+    int worst = GARAGE_EC_OK;
+    for (size_t s = 0; s < n; s++) {
+        if (status[s] == GARAGE_EC_E_UNRECOVERABLE) return GARAGE_EC_E_UNRECOVERABLE;
+        if (status[s]) worst = status[s];
+    }
+    return worst;
+}
+
+int open_range_args(garage_ec_ctx *ctx, const void *shards, const uint8_t *present, const uint32_t *sealed,
+                    const uint8_t *keys, const uint32_t *offset, const uint32_t *len, const int32_t *status,
+                    size_t stride, size_t n)
+{
+    if (!ctx) return GARAGE_EC_E_INVALID;
+    int rc = check_geometry(ctx, stride, n, ctx->k + ctx->m);
+    if (rc) return rc;
+    if (n == 0) return GARAGE_EC_OK;
+    if (!shards || !present || !sealed || !keys || !offset || !len || !status) return GARAGE_EC_E_INVALID;
+    return GARAGE_EC_OK;
+}
+
+}  // namespace
+extern "C" {
+
+int garage_ec_sealed_range(uint32_t sealed_len, uint32_t offset, uint32_t len, uint32_t *span_off, uint32_t *span_len,
+                           uint32_t *c0, uint32_t *n_chunks)
+{
+    if (!span_off || !span_len || !c0 || !n_chunks) return GARAGE_EC_E_INVALID;
+    return sse::sealed_range(sealed_len, offset, len, span_off, span_len, c0, n_chunks);
+}
+
+int garage_ec_open_range_plan(const garage_ec_ctx *ctx, const uint8_t *present, uint32_t sealed_len, uint32_t offset,
+                              uint32_t len, garage_ec_range *ranges, size_t cap, size_t *n_ranges, int *needs_gpu)
+{
+    if (!ctx || !present || !n_ranges || (cap && !ranges)) return GARAGE_EC_E_INVALID;
+    *n_ranges = 0;
+    if (needs_gpu) *needs_gpu = 0;
+    std::vector<garage_ec_range> runs;
+    int gpu = 0;
+    const int rc = open_range_runs(ctx, present, sealed_len, offset, len, runs, &gpu);
+    if (needs_gpu) *needs_gpu = gpu;
+    if (rc) return rc;
+    return merge_runs(runs, ranges, cap, n_ranges);
+}
+
+int garage_ec_open_range(garage_ec_ctx *ctx, const uint8_t *shards, const uint8_t *present, const uint32_t *sealed_len,
+                         const uint8_t *keys, const uint32_t *offset, const uint32_t *len, size_t stride, uint8_t *out,
+                         size_t out_stride, int32_t *status, size_t n, int mem_kind, void *cuda_stream)
+{
+    if (mem_kind != GARAGE_EC_MEM_HOST && mem_kind != GARAGE_EC_MEM_DEVICE) return GARAGE_EC_E_INVALID;
+    int rc = open_range_args(ctx, shards, present, sealed_len, keys, offset, len, status, stride, n);
+    if (rc || n == 0) return rc;
+    if (!out) return GARAGE_EC_E_INVALID;
+    if (!aligned16(shards)) return GARAGE_EC_E_ALIGN;
+    if (mem_kind == GARAGE_EC_MEM_HOST) {
+        CU_TRY(ctx, cudaSetDevice(ctx->device));
+        return open_range_host(ctx, shards, nullptr, present, sealed_len, keys, offset, len, stride, out, out_stride,
+                               nullptr, status, n);
+    }
+    if (!aligned16(out) || (out_stride & 15) || (reinterpret_cast<uintptr_t>(sealed_len) & 3) ||
+        (reinterpret_cast<uintptr_t>(offset) & 3) || (reinterpret_cast<uintptr_t>(len) & 3) ||
+        (reinterpret_cast<uintptr_t>(status) & 3))
+        return GARAGE_EC_E_ALIGN;
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    const OpenRangeScratch sc(ctx, n, stride, out_stride);
+    return with_stream_scratch(ctx, sc.bytes, st, [&](uint8_t *scratch) {
+        const int r = run_open_range(ctx, shards, present, sealed_len, keys, offset, len, stride, out, out_stride, status,
+                                     n, scratch, st);
+        const cudaError_t e = cudaMemsetAsync(scratch + sc.o_keys, 0, n * sizeof(sse::SseKey), st);
+        if (r) return r;
+        return e == cudaSuccess ? GARAGE_EC_OK : set_cuda_error(ctx, e, "cudaMemsetAsync(key material)");
+    });
+}
+
+int garage_ec_open_range_stripes(garage_ec_ctx *ctx, const uint8_t *const *stripes, const uint8_t *present,
+                                 const uint32_t *sealed_len, const uint8_t *keys, const uint32_t *offset,
+                                 const uint32_t *len, size_t stride, uint8_t *const *outs, int32_t *status, size_t n)
+{
+    int rc = open_range_args(ctx, stripes, present, sealed_len, keys, offset, len, status, stride, n);
+    if (rc || n == 0) return rc;
+    if (!outs) return GARAGE_EC_E_INVALID;
+    for (size_t s = 0; s < n; s++) {
+        if (!stripes[s]) return GARAGE_EC_E_INVALID;
+        if (!aligned16(stripes[s])) return GARAGE_EC_E_ALIGN;
+    }
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    return open_range_host(ctx, nullptr, stripes, present, sealed_len, keys, offset, len, stride, nullptr, 0, outs,
+                           status, n);
 }
 
 // ---- test hook -------------------------------------------------------------------------------

@@ -2210,7 +2210,8 @@ __host__ __device__ inline RangeWindow range_window(uint32_t L, uint32_t unit, u
 }
 
 struct RangeParams {
-    const uint8_t *shards;          // the caller's shard layout: stripe s at shards + s*pitch, shard i at + i*stride
+    const uint8_t *shards;          // the caller's shard layout: request s reads stripe s >> shift at
+                                    // shards + (s >> shift)*pitch, shard i at + i*stride
     uint8_t *sub;                   // the sub-stripes, same layout (a window never exceeds its shard)
     const uint8_t *present;         // n*(k+m)
     const uint32_t *block_len, *offset, *len;  // per request
@@ -2221,7 +2222,7 @@ struct RangeParams {
     const int32_t *plan_status;     // the decode's status of the sub-stripes
     int32_t *status;                // nullable, out
     unsigned long long pitch, out_stride;
-    uint32_t stride, k, m, n, quantum, alpha, pb;
+    uint32_t stride, k, m, n, quantum, alpha, pb, shift;
 };
 
 // one thread per request: the window, the decode's want map and sub-stripe length
@@ -2254,7 +2255,7 @@ __global__ void __launch_bounds__(256) range_pack_kernel(const __grid_constant__
         const uint4 g = q.geo[s];
         if (!g.w) continue;
         const uint32_t nz = g.x / g.y, nv = (g.w + 15) >> 4, per = nz * nv;
-        const uint8_t *src = q.shards + s * q.pitch, *pr = q.present + (size_t)s * tot;
+        const uint8_t *src = q.shards + (s >> q.shift) * q.pitch, *pr = q.present + (size_t)s * tot;
         uint8_t *dst = q.sub + s * q.pitch;
         for (uint32_t idx = threadIdx.x; idx < tot * per; idx += blockDim.x) {
             const uint32_t i = idx / per, r = idx - i * per, z = r / nv, v = r - z * nv;
@@ -2273,7 +2274,7 @@ __device__ __forceinline__ const uint8_t *range_src(const RangeParams &q, uint32
     const uint32_t j = o / g.x, c = o - j * g.x;
     if (q.present[(size_t)s * (q.k + q.m) + j]) {
         *rem = g.x - c;
-        return q.shards + s * q.pitch + (size_t)j * q.stride + c;
+        return q.shards + (s >> q.shift) * q.pitch + (size_t)j * q.stride + c;
     }
     const uint32_t z = c / g.y, cc = c - z * g.y;
     *rem = g.z + g.w - cc;

@@ -36,6 +36,26 @@ __host__ __device__ inline uint64_t sealed_len(uint64_t len)
     return kPrefix + len + 16 * n;
 }
 
+// DESIGN.md 2.7: the chunks c0 .. c0 + nch - 1 that plaintext bytes [o, o + len) of a block sealed to S bytes lie in,
+// and their run of B, [span_off, span_off + span_len).  0; -7 (GARAGE_EC_E_AUTH) for an S the framing cannot hold;
+// -1 (GARAGE_EC_E_INVALID) for a range past the plaintext.  An empty range touches nothing: nch = span_len = 0.
+__host__ __device__ inline int sealed_range(uint32_t S, uint32_t o, uint32_t len, uint32_t *span_off,
+                                            uint32_t *span_len, uint32_t *c0, uint32_t *nch)
+{
+    if (S < kPrefix + 16) return -7;
+    const uint32_t r = (S - kPrefix) % kFrame;
+    if (r >= 1 && r < 16) return -7;
+    const uint64_t n = ((uint64_t)S - kPrefix + kFrame - 1) / kFrame, P = S - kPrefix - 16 * n;
+    if ((uint64_t)o + len > P) return -1;
+    const uint64_t a = o / kChunk, b = len ? ((uint64_t)o + len - 1) / kChunk + 1 : a;
+    const uint64_t s0 = kPrefix + kFrame * a, s1 = kPrefix + kFrame * b;
+    *c0 = (uint32_t)a;
+    *nch = (uint32_t)(b - a);
+    *span_off = (uint32_t)(s0 < S ? s0 : S);
+    *span_len = (uint32_t)((s1 < S ? s1 : S) - *span_off);
+    return 0;
+}
+
 // Per-key material, built by sse_setup_kernel: the AES-256 round keys (FIPS-197 5.2), the 4-bit multiplication
 // table of H = E_K(0^128) and H^(8(31-l)) for lane l.  Secret: zeroed on the stream after the call's last kernel.
 struct SseKey {
@@ -264,11 +284,17 @@ __global__ void __launch_bounds__(256) sse_setup_kernel(const __grid_constant__ 
 }
 
 // ---- the chunk kernel -----------------------------------------------------------------------------------------
-enum { kSeal = 0, kCheck = 1, kOpen = 2 };
+// kRangeCheck / kRangeOpen: ranged opens (DESIGN.md 4.10).  Request s reads its nonce prefix from row 2s of `rows`
+// and chunks c0 .. c1 of its range, back to back from a 16-byte boundary, from row 2s + 1; the open writes only the
+// plaintext bytes [offset, offset + len) to plain_out + s*plain_stride, zero up to roundup16(len).
+enum { kSeal = 0, kCheck = 1, kOpen = 2, kRangeCheck = 3, kRangeOpen = 4 };
 
 struct ChunkParams {
     const uint8_t *plain_in;        // seal: block s at plain_in + s*plain_stride
     uint8_t *plain_out;             // open: block s at plain_out + s*plain_stride
+    const uint8_t *rows;            // ranged: row r at rows + r*row_pitch
+    const uint32_t *offset, *len;   // ranged: the plaintext range per request
+    unsigned long long row_pitch;
     unsigned long long plain_stride;
     const uint32_t *plain_len;      // seal: per block
     uint32_t *plain_len_out;        // open: per block
@@ -278,10 +304,11 @@ struct ChunkParams {
     const SseKey *ks;               // nullable (seal only): B = P
     uint8_t *shards;                // stripe s at shards + s*(k+m)*stride, data shard j at + j*stride
     int32_t *status;                // check / open
-    const int32_t *rec_status;      // check: verdict of the reconstruct
+    const int32_t *rec_status;      // check: verdict of the reconstruct (ranged: of the two row decodes, 2s and 2s + 1)
     const uint8_t *hash_bad;        // open: skip the block when set
     uint32_t stride, k, m, n;
-    uint32_t cmax;                  // chunks per block this launch covers (work item = block * cmax + chunk)
+    uint32_t cmax;                  // chunks per block this launch covers (work item = block * cmax + chunk; ranged:
+                                    // + chunk - c0)
 };
 
 struct ChunkSmem {
@@ -302,24 +329,35 @@ __global__ void __launch_bounds__(kWarps * 32) sse_chunk_kernel(const __grid_con
     const unsigned long long total = (unsigned long long)q.n * q.cmax;
     for (unsigned long long w = (unsigned long long)blockIdx.x * kWarps + wid; w < total;
          w += (unsigned long long)gridDim.x * kWarps) {
-        const uint32_t s = (uint32_t)(w / q.cmax), c = (uint32_t)(w - (unsigned long long)s * q.cmax);
-        const uint32_t L = q.shard_len[s];
-        if (!L) continue;
+        constexpr bool ranged = MODE == kRangeCheck || MODE == kRangeOpen;
+        constexpr bool checking = MODE == kCheck || MODE == kRangeCheck;
+        const uint32_t s = (uint32_t)(w / q.cmax), ci = (uint32_t)(w - (unsigned long long)s * q.cmax);
+        const uint32_t L = ranged ? 0u : q.shard_len[s];
+        if (!ranged && !L) continue;
         const bool keyed = MODE != kSeal || q.ks;
         const uint32_t blen = q.blen[s];
         const uint32_t prefix = keyed ? kPrefix : 0, pitch = keyed ? kFrame : kChunk;
-        uint32_t plen, nch;
+        uint32_t plen, nch, c = ci, off = 0, len = 0, c1 = 0;
         if (MODE == kSeal) {
             plen = q.plain_len[s];
         } else {
-            if (MODE == kCheck && c == 0) {
-                const int32_t rs = q.rec_status[s];
+            const int32_t rs = ranged ? (q.rec_status[2 * s] ? q.rec_status[2 * s] : q.rec_status[2 * s + 1])
+                                      : q.rec_status[s];
+            if (checking && ci == 0) {
                 if (rs && lane == 0) q.status[s] = rs;  // an unrecoverable stripe reports that, not its framing
             }
-            if (q.status[s] != 0 || q.rec_status[s] != 0) continue;
+            if (q.status[s] != 0 || rs != 0) continue;
             if (MODE == kOpen && q.hash_bad[s]) continue;
             const uint32_t nn = (blen - kPrefix + kFrame - 1) / kFrame;  // framing checked by sse_lens_kernel
             plen = blen - kPrefix - 16 * nn;
+            if (ranged) {  // range checked by sse_range_lens_kernel
+                off = q.offset[s];
+                len = q.len[s];
+                if (!len) continue;
+                c = off / kChunk + ci;
+                c1 = (off + len - 1) / kChunk;
+                if (c > c1) continue;
+            }
         }
         nch = plen ? (plen + kChunk - 1) / kChunk : 1;
         if (c >= nch) continue;
@@ -343,17 +381,27 @@ __global__ void __launch_bounds__(kWarps * 32) sse_chunk_kernel(const __grid_con
                 nw0 = ((uint32_t)np[0] << 24) | ((uint32_t)np[1] << 16) | ((uint32_t)np[2] << 8) | np[3];
                 nw1 = ((uint32_t)np[4] << 24) | ((uint32_t)np[5] << 16) | ((uint32_t)np[6] << 8) | np[7];
             } else {
-                // B[0, 8): byte i of B is byte i % L of data shard i / L
+                // B[0, 8): byte i of B is byte i % L of data shard i / L (ranged: the first 8 bytes of row 2s)
+                const uint8_t *row = q.rows + 2ull * s * q.row_pitch;
                 uint8_t nb8[8];
 #pragma unroll
-                for (int i = 0; i < 8; i++) nb8[i] = stripe[(size_t)(i / L) * q.stride + i % L];
+                for (int i = 0; i < 8; i++) nb8[i] = ranged ? row[i] : stripe[(size_t)(i / L) * q.stride + i % L];
                 nw0 = ((uint32_t)nb8[0] << 24) | ((uint32_t)nb8[1] << 16) | ((uint32_t)nb8[2] << 8) | nb8[3];
                 nw1 = ((uint32_t)nb8[4] << 24) | ((uint32_t)nb8[5] << 16) | ((uint32_t)nb8[6] << 8) | nb8[7];
             }
         }
         const uint32_t nw2 = bswap32(c | (last ? 0x80000000u : 0u));  // LE32(c | last << 31) as a big-endian word
 
-        if (MODE != kSeal) {
+        if (ranged) {
+            // the chunk's ciphertext and tag, 16-byte aligned in row 2s + 1, into stage[8..]; the row is zero past
+            // the span up to its roundup16, and a vector past clen + 16 lands in the stage's slack
+            const uint8_t *src = q.rows + (2ull * s + 1) * q.row_pitch + (size_t)kFrame * ci;
+            for (uint32_t v = 16 * lane; v < clen + 16; v += 512) {
+                const uint4 d = *reinterpret_cast<const uint4 *>(src + v);
+                *reinterpret_cast<unsigned long long *>(st + kPrefix + v) = ((unsigned long long)d.y << 32) | d.x;
+                *reinterpret_cast<unsigned long long *>(st + kPrefix + v + 8) = ((unsigned long long)d.w << 32) | d.z;
+            }
+        } else if (MODE != kSeal) {
             // load this chunk's ciphertext and tag, B[base + 8, base + 8 + clen + 16), into stage[8..]
             const uint32_t r0 = base + kPrefix, r1 = r0 + clen + 16;
             for (uint32_t j = r0 / L; j * L < r1 && j < q.k; j++) {
@@ -384,9 +432,12 @@ __global__ void __launch_bounds__(kWarps * 32) sse_chunk_kernel(const __grid_con
             for (uint32_t i = 0; i < 8; i++) {
                 const int b = (int)(8 * lane + i) - (int)(256 - nb);
                 if (b < 0) continue;
+                // ranged open: only the counter blocks that overlap the range
+                if (MODE == kRangeOpen && (kChunk * c + 16 * (uint32_t)b >= off + len || kChunk * c + 16 * (uint32_t)b + 16 <= off))
+                    continue;
                 const uint32_t valid = min(16u, clen - 16u * (uint32_t)b);
                 unsigned long long ch, cl;
-                if (MODE == kCheck) {
+                if (checking) {
                     ch = *reinterpret_cast<const unsigned long long *>(st + kPrefix + 16 * b);
                     cl = *reinterpret_cast<const unsigned long long *>(st + kPrefix + 16 * b + 8);
                 } else {
@@ -409,9 +460,10 @@ __global__ void __launch_bounds__(kWarps * 32) sse_chunk_kernel(const __grid_con
                     const unsigned long long ma = valid >= 8 ? ~0ull : ((1ull << (8 * valid)) - 1),
                                              mb = valid >= 16 ? ~0ull : valid <= 8 ? 0ull : ((1ull << (8 * (valid - 8))) - 1);
                     const unsigned long long oa = (pa ^ ksa) & ma, ob = (pb ^ ksb) & mb;
-                    if (MODE == kSeal) {
+                    if (MODE == kSeal || MODE == kRangeOpen) {
                         *reinterpret_cast<unsigned long long *>(st + kPrefix + 16 * b) = oa;
                         *reinterpret_cast<unsigned long long *>(st + kPrefix + 16 * b + 8) = ob;
+                        if (MODE == kRangeOpen) continue;
                         ch = oa;
                         cl = ob;
                     } else {
@@ -421,7 +473,7 @@ __global__ void __launch_bounds__(kWarps * 32) sse_chunk_kernel(const __grid_con
                         continue;
                     }
                 }
-                if (MODE == kCheck && valid < 16) {  // zero-pad the last block for GHASH
+                if (checking && valid < 16) {  // zero-pad the last block for GHASH
                     const unsigned long long ma = valid >= 8 ? ~0ull : ((1ull << (8 * valid)) - 1),
                                              mb = valid <= 8 ? 0ull : ((1ull << (8 * (valid - 8))) - 1);
                     ch &= ma;
@@ -434,7 +486,7 @@ __global__ void __launch_bounds__(kWarps * 32) sse_chunk_kernel(const __grid_con
             }
         }
 
-        if (MODE != kOpen && keyed) {
+        if (MODE != kOpen && MODE != kRangeOpen && keyed) {
             if (lane != 31) gf128_mul_bits(yh, yl, K->pw[lane][0], K->pw[lane][1]);
             __syncwarp();  // the last data block's zero tail is in the stage before lane 0 writes the tag over it
 #pragma unroll
@@ -471,6 +523,26 @@ __global__ void __launch_bounds__(kWarps * 32) sse_chunk_kernel(const __grid_con
             }
         }
         if (MODE == kOpen && c == 0 && lane == 0) q.plain_len_out[s] = plen;
+
+        if (MODE == kRangeOpen) {
+            __syncwarp();
+            // out positions [a, e) come from this chunk; the last chunk also writes the zero tail up to roundup16(len).
+            // A vector shared with the neighbouring chunk is stored byte by byte, so two warps never write one byte.
+            const uint32_t cb = kChunk * c, a = max(off, cb) - off, e = min(off + len, cb + clen) - off;
+            const uint32_t ew = c == c1 ? (len + 15) & ~15u : e;
+            uint8_t *dst = q.plain_out + (size_t)s * q.plain_stride;
+            auto byte_at = [&](uint32_t x) -> uint8_t { return x < len ? st[kPrefix + off + x - cb] : (uint8_t)0; };
+            for (uint32_t v = (a & ~15u) + 16 * lane; v < ew; v += 512) {
+                if (v >= a && v + 16 <= ew) {
+                    uint32_t wds[4] = {0, 0, 0, 0};
+#pragma unroll
+                    for (int b = 0; b < 16; b++) wds[b >> 2] |= (uint32_t)byte_at(v + b) << (8 * (b & 3));
+                    *reinterpret_cast<uint4 *>(dst + v) = make_uint4(wds[0], wds[1], wds[2], wds[3]);
+                } else {
+                    for (uint32_t x = max(v, a); x < min(v + 16, ew); x++) dst[x] = byte_at(x);
+                }
+            }
+        }
 
         if (MODE == kSeal) {
             __syncwarp();
@@ -540,6 +612,36 @@ __global__ void __launch_bounds__(256) sse_lens_kernel(const __grid_constant__ L
         q.status[s] = bad ? -1 /* GARAGE_EC_E_INVALID */ : framed ? 0 : -7 /* GARAGE_EC_E_AUTH */;
         q.shard_len[s] = bad ? 0u : (uint32_t)L;
         for (uint32_t i = 0; i < q.k + q.m; i++) q.want[(size_t)s * (q.k + q.m) + i] = i < q.k;
+    }
+}
+
+// ---- ranged open: per-request framing and the two row decodes --------------------------------------------------
+struct RangeLensParams {
+    const uint32_t *sealed, *offset, *len;  // per request
+    const uint8_t *present;                 // n*(k+m)
+    int32_t *status;                        // out: 0 / GARAGE_EC_E_AUTH (framing) / GARAGE_EC_E_INVALID (geometry)
+    uint32_t *blen2, *off2, *len2;          // out: decode 2s = the prefix B[0, 8), 2s + 1 = the span (empty if failed)
+    uint8_t *present2;                      // out: 2n*(k+m), request s's map twice
+    unsigned long long out_stride;
+    uint32_t stride, k, m, n, quantum;
+};
+__global__ void __launch_bounds__(256) sse_range_lens_kernel(const __grid_constant__ RangeLensParams q)
+{
+    const uint32_t tot = q.k + q.m;
+    for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < q.n; s += gridDim.x * blockDim.x) {
+        const uint32_t S = q.sealed[s], o = q.offset[s], len = q.len[s];
+        uint32_t so = 0, sl = 0, c0, nch;
+        int32_t st = code_shard_len(S, (int)q.k, q.quantum) > q.stride ? -1 : sealed_range(S, o, len, &so, &sl, &c0, &nch);
+        if (!st && ((uint64_t)len + 15) / 16 * 16 > q.out_stride) st = -1;
+        q.status[s] = st;
+        const bool go = !st && len;
+        q.blen2[2 * s] = q.blen2[2 * s + 1] = go ? S : 0u;
+        q.off2[2 * s] = 0;
+        q.len2[2 * s] = go ? kPrefix : 0u;
+        q.off2[2 * s + 1] = go ? so : 0u;
+        q.len2[2 * s + 1] = go ? sl : 0u;
+        for (uint32_t i = 0; i < tot; i++)
+            q.present2[(2 * (size_t)s) * tot + i] = q.present2[(2 * (size_t)s + 1) * tot + i] = q.present[(size_t)s * tot + i];
     }
 }
 

@@ -227,6 +227,18 @@ typedef struct garage_bm_sealed_metrics {
     uint64_t seal_call_us;         /* wall time inside garage_ec_seal_blocks                                    */
     uint64_t open_call_us;         /* wall time inside garage_ec_open_stripes                                   */
 } garage_bm_sealed_metrics;
+/* Counters of garage_bm_rpc_get_block_range_opened (DESIGN.md section 5.10), in a struct of their own for the same
+ * reason. */
+typedef struct garage_bm_sealed_range_metrics {
+    uint64_t gets;               /* garage_bm_rpc_get_block_range_opened calls                                      */
+    uint64_t degraded_gets;      /* of those, ranges whose prefix or span needed an absent data shard rebuilt       */
+    uint64_t bytes_read;         /* tag-span bytes those GETs read from shard files                                */
+    uint64_t bytes_fetched;      /* the planned run bytes: what would cross the network in Garage                  */
+    uint64_t auth_failures;      /* calls that ended in GARAGE_EC_E_AUTH                                            */
+    uint64_t fallbacks;          /* ranges that failed a tag and went through one whole-block opened GET            */
+    uint64_t call_us;            /* wall time inside garage_bm_rpc_get_block_range_opened                           */
+    uint64_t open_range_call_us; /* wall time inside garage_ec_open_range_stripes                                   */
+} garage_bm_sealed_range_metrics;
 
 /* One entry of a node's resync error table (Garage's BlockResyncErrorInfo, manager.rs:429-449).                    */
 typedef struct garage_bm_resync_error {
@@ -302,6 +314,21 @@ int garage_bm_rpc_put_block_sealed(garage_bm *bm, const uint8_t *key32, const ui
 int garage_bm_rpc_get_block_opened(garage_bm *bm, const uint8_t hash[32], const uint8_t *key32, uint8_t *out, size_t cap,
                                    size_t *out_len);
 void garage_bm_get_sealed_metrics(garage_bm *bm, garage_bm_sealed_metrics *out);
+
+/* Ranged SSE-C GET (body_from_blocks_range, src/api/s3/get.rs:650-743, and UploadPartCopy with a source range,
+ * src/api/s3/copy.rs:396-469, of an SSE-C object): plaintext bytes [offset, offset + len) of block `hash` sealed under
+ * key32.  Gathered like garage_bm_rpc_get_block_range, with the runs of garage_ec_open_range_plan (the nonce prefix and
+ * the touched chunks); one garage_ec_open_range_stripes call of the reconstruct dispatchers rebuilds, checks and
+ * decrypts them.  *out_len = len.  The whole plaintext, and blocks held only under a previous code or as replicas, are
+ * served by garage_bm_rpc_get_block_opened and sliced.  A touched chunk that fails its tag is retried once as a
+ * whole-block garage_bm_rpc_get_block_opened, whose content-hash check finds and quarantines a stale shard: its bytes
+ * are served if it succeeds, GARAGE_EC_E_AUTH is returned if it fails authentication (a wrong key).  Integrity: as
+ * DESIGN.md section 2.7 -- the touched chunks are proven, untouched chunks and the content hash are not.
+ * GARAGE_EC_E_INVALID if offset + len exceeds the plaintext or len > cap; GARAGE_BM_E_MISSING_BLOCK as
+ * garage_bm_rpc_get_block.                                                                                         */
+int garage_bm_rpc_get_block_range_opened(garage_bm *bm, const uint8_t hash[32], const uint8_t *key32, uint32_t offset,
+                                         uint32_t len, uint8_t *out, size_t cap, size_t *out_len);
+void garage_bm_get_sealed_range_metrics(garage_bm *bm, garage_bm_sealed_range_metrics *out);
 
 /* Bytes [offset, offset + len) of a block (body_from_blocks_range, src/api/s3/get.rs:650-743; the source range of
  * UploadPartCopy, src/api/s3/copy.rs:396-469), reading only the shards and columns garage_ec_range_plan names, each as

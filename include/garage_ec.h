@@ -431,6 +431,51 @@ int garage_ec_open_stripes(garage_ec_ctx *ctx, uint8_t *const *stripes, const ui
                            const uint8_t *hashes, const uint8_t *keys, uint8_t *const *plains, uint32_t *plain_len_out,
                            uint8_t *hash_bad, int32_t *status, size_t stride, size_t n);
 
+/* ---- SSE-C RANGED OPEN -- call sites: body_from_blocks_range (src/api/s3/get.rs:650-743) and UploadPartCopy with a
+ * source range (src/api/s3/copy.rs:396-469, 511-540) when the object is SSE-C, through EncryptionParams::get_block:
+ * plaintext bytes [offset, offset + len) of a sealed block, proven from the chunks they touch and the nonce prefix
+ * alone (DESIGN.md section 2.7 is normative).  A block sealed to S bytes has n = (S - 8 + 4111) / 4112 chunks and
+ * P = S - 8 - 16n plaintext bytes; the range touches chunks c0 = offset / 4096 .. c1 = (offset + len - 1) / 4096 and needs
+ * the prefix B[0, 8) and the span B[8 + 4112 c0, min(S, 8 + 4112 (c1 + 1))).  Chunk c is opened under nonce
+ * N || LE32(c | (c == n-1) << 31).  What a ranged open proves: every touched chunk is the authentic chunk c of a block
+ * sealed under this key with this N.  It does not prove that untouched chunks are intact or that the block still
+ * hashes to its address (the deep scrub does).
+ *
+ * garage_ec_sealed_range (host only): *span_off / *span_len, *c0 and *n_chunks = c1 - c0 + 1 of one range; an empty
+ * range touches nothing (n_chunks = span_len = 0, span_off = min(S, 8 + 4112 * (offset / 4096))).  GARAGE_EC_E_AUTH for
+ * an S the framing cannot hold (as garage_ec_open), GARAGE_EC_E_INVALID for offset + len > P.
+ *
+ * garage_ec_open_range_plan (host only, one request): the byte runs a gatherer fetches, in garage_ec_range_plan's
+ * format and merge rule: its runs for the prefix and for the span, merged.  Nothing for an empty range.  *needs_gpu
+ * (nullable) = 1 iff a data shard the prefix or the span touches is absent.  Errors as garage_ec_sealed_range, then as
+ * garage_ec_range_plan.
+ *
+ * garage_ec_open_range: n requests on the shard layout (stride rules of reconstruct; only the planned runs need hold
+ * valid bytes; shards is never written).  sealed_len / offset / len: n values; keys: 32 bytes per request.  Request s
+ * writes its len[s] plaintext bytes at out + s*out_stride only if every chunk it touches passed its tag.  status (n
+ * int32, required): 0; GARAGE_EC_E_UNRECOVERABLE; GARAGE_EC_E_AUTH (a touched chunk's tag or the prefix fails, or S is
+ * malformed); DEVICE only: GARAGE_EC_E_INVALID for a range past P, an L past `stride` or roundup16(len) past
+ * out_stride.  An empty range of a well-framed block is status 0 and writes nothing.
+ *   DEVICE: all pointers device memory; out 16-byte aligned, out_stride a multiple of 16, bytes [len, roundup16(len))
+ *           written as zero; sealed_len / offset / len / status 4-byte aligned.  Only kernels and stream-ordered
+ *           scratch of about 2n((k+m)*stride + out_stride) bytes are enqueued (capturable in a CUDA graph).
+ *   HOST:   synchronous; any output alignment.  GARAGE_EC_E_INVALID before any GPU work for a range past P or an L past
+ *           `stride`.  Uploads only the planned runs (present span and prefix bytes too: they are ciphertext),
+ *           downloads only the len plaintext bytes; returns GARAGE_EC_E_UNRECOVERABLE if any request was, else
+ *           GARAGE_EC_E_AUTH if any request failed authentication.
+ * Key schedules and the library's copies of keys are zeroed as for garage_ec_open.  garage_ec_open_range_stripes is
+ * the HOST gather form: stripe s at stripes[s] (its k+m shards `stride` apart), request s writes at outs[s].          */
+int garage_ec_sealed_range(uint32_t sealed_len, uint32_t offset, uint32_t len, uint32_t *span_off, uint32_t *span_len,
+                           uint32_t *c0, uint32_t *n_chunks);
+int garage_ec_open_range_plan(const garage_ec_ctx *ctx, const uint8_t *present, uint32_t sealed_len, uint32_t offset,
+                              uint32_t len, garage_ec_range *ranges, size_t cap, size_t *n_ranges, int *needs_gpu);
+int garage_ec_open_range(garage_ec_ctx *ctx, const uint8_t *shards, const uint8_t *present, const uint32_t *sealed_len,
+                         const uint8_t *keys, const uint32_t *offset, const uint32_t *len, size_t stride, uint8_t *out,
+                         size_t out_stride, int32_t *status, size_t n, int mem_kind, void *cuda_stream);
+int garage_ec_open_range_stripes(garage_ec_ctx *ctx, const uint8_t *const *stripes, const uint8_t *present,
+                                 const uint32_t *sealed_len, const uint8_t *keys, const uint32_t *offset,
+                                 const uint32_t *len, size_t stride, uint8_t *const *outs, int32_t *status, size_t n);
+
 /* ---- utilities used by the harness ------------------------------------------------------
  * device-side synthetic data (same splitmix64 counter stream as the oracle's
  * generator): fills dst[0..len) (device) with stream bytes at `offset`

@@ -88,6 +88,7 @@ impl ErasureCoder {
     pub fn range_plan(&self, hash: &Hash, present: &[bool], block_len: usize, offset: usize, len: usize)
         -> Result<(Vec<(u32, u32, u32)>, bool), Error>
     {
+        assert!(present.len() == self.k + self.m);
         let pr: Vec<u8> = present.iter().map(|p| *p as u8).collect();
         let cap = (self.k + self.m) * 512;
         let mut runs: Vec<sys::garage_ec_range> = (0..cap).map(|_| sys::garage_ec_range { shard: 0, offset: 0, len: 0 }).collect();
@@ -105,6 +106,7 @@ impl ErasureCoder {
     pub fn read_range(&self, hash: &Hash, stripe: &[u8], stride: usize, present: &[bool], block_len: usize,
                       offset: usize, len: usize) -> Result<Vec<u8>, Error>
     {
+        assert!(present.len() == self.k + self.m);
         let pr: Vec<u8> = present.iter().map(|p| *p as u8).collect();
         let mut out = vec![0u8; len];
         let (bl, off, ln, mut st) = ([block_len as u32], [offset as u32], [len as u32], [0i32]);
@@ -165,7 +167,8 @@ impl ErasureCoder {
     pub fn open_stripes(&self, stripes: &[*mut u8], present: &[u8], sealed_len: &[u32], hashes: &[[u8; 32]],
                         keys: &[[u8; 32]], outs: &[*mut u8], stride: usize) -> Result<Vec<Result<u32, i32>>, Error> {
         let n = stripes.len();
-        assert!(sealed_len.len() == n && hashes.len() == n && keys.len() == n && outs.len() == n);
+        assert!(present.len() == n * (self.k + self.m) && sealed_len.len() == n && hashes.len() == n && keys.len() == n
+                && outs.len() == n);
         let (mut plen, mut bad, mut status) = (vec![0u32; n], vec![0u8; n], vec![0i32; n]);
         let rc = unsafe { sys::garage_ec_open_stripes(self.ctx, stripes.as_ptr(), present.as_ptr(), sealed_len.as_ptr(),
                           hashes.as_ptr() as *const u8, keys.as_ptr() as *const u8, outs.as_ptr(), plen.as_mut_ptr(),
@@ -174,6 +177,24 @@ impl ErasureCoder {
         Ok((0..n).map(|s| if status[s] == sys::GARAGE_EC_E_UNRECOVERABLE { Err(status[s]) }
                           else if bad[s] != 0 { Err(sys::GARAGE_EC_E_INVALID) }
                           else if status[s] != 0 { Err(status[s]) } else { Ok(plen[s]) }).collect())
+    }
+
+    /// A byte range of SSE-C blocks (body_from_blocks_range, UploadPartCopy with a source range): check and decrypt
+    /// only the chunks plaintext bytes [offset, offset + len) touch.  `stripes` hold at least the runs of
+    /// garage_ec_open_range_plan.  Per request: Ok(()) with its len bytes in outs[s], or its status
+    /// (GARAGE_EC_E_AUTH, GARAGE_EC_E_UNRECOVERABLE).
+    pub fn open_range_stripes(&self, stripes: &[*const u8], present: &[u8], sealed_len: &[u32], keys: &[[u8; 32]],
+                              offset: &[u32], len: &[u32], outs: &[*mut u8], stride: usize)
+                              -> Result<Vec<Result<(), i32>>, Error> {
+        let n = stripes.len();
+        assert!(present.len() == n * (self.k + self.m) && sealed_len.len() == n && keys.len() == n && offset.len() == n
+                && len.len() == n && outs.len() == n);
+        let mut status = vec![0i32; n];
+        let rc = unsafe { sys::garage_ec_open_range_stripes(self.ctx, stripes.as_ptr(), present.as_ptr(),
+                          sealed_len.as_ptr(), keys.as_ptr() as *const u8, offset.as_ptr(), len.as_ptr(), stride,
+                          outs.as_ptr(), status.as_mut_ptr(), n) };
+        if rc != sys::GARAGE_EC_E_AUTH && rc != sys::GARAGE_EC_E_UNRECOVERABLE { check(self.ctx, rc)?; }
+        Ok(status.iter().map(|&st| if st != 0 { Err(st) } else { Ok(()) }).collect())
     }
 }
 impl Drop for ErasureCoder { fn drop(&mut self) { unsafe { sys::garage_ec_destroy(self.ctx) } } }

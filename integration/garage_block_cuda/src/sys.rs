@@ -78,6 +78,18 @@ extern "C" {
                                   sealed_len: *const u32, hashes: *const u8, keys: *const u8, plains: *const *mut u8,
                                   plain_len_out: *mut u32, hash_bad: *mut u8, status: *mut i32, stride: usize,
                                   n: usize) -> c_int;
+    pub fn garage_ec_sealed_range(sealed_len: u32, offset: u32, len: u32, span_off: *mut u32, span_len: *mut u32,
+                                  c0: *mut u32, n_chunks: *mut u32) -> c_int;
+    pub fn garage_ec_open_range_plan(ctx: *const garage_ec_ctx, present: *const u8, sealed_len: u32, offset: u32,
+                                     len: u32, ranges: *mut garage_ec_range, cap: usize, n_ranges: *mut usize,
+                                     needs_gpu: *mut c_int) -> c_int;
+    pub fn garage_ec_open_range(ctx: *mut garage_ec_ctx, shards: *const u8, present: *const u8, sealed_len: *const u32,
+                                keys: *const u8, offset: *const u32, len: *const u32, stride: usize, out: *mut u8,
+                                out_stride: usize, status: *mut i32, n: usize, mem_kind: c_int,
+                                stream: *mut c_void) -> c_int;
+    pub fn garage_ec_open_range_stripes(ctx: *mut garage_ec_ctx, stripes: *const *const u8, present: *const u8,
+                                        sealed_len: *const u32, keys: *const u8, offset: *const u32, len: *const u32,
+                                        stride: usize, outs: *const *mut u8, status: *mut i32, n: usize) -> c_int;
     pub fn garage_ec_strerror(code: c_int) -> *const c_char;
     pub fn garage_ec_last_error(ctx: *const garage_ec_ctx) -> *const c_char;
     pub fn garage_ec_abi_version() -> c_int;
