@@ -52,6 +52,11 @@ namespace {
 
 using Hash = std::array<uint8_t, 32>;
 using Clock = std::chrono::steady_clock;
+// the microseconds since t0: what a call adds to its *_us counter
+inline uint64_t us_since(Clock::time_point t0)
+{
+    return (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count();
+}
 struct HashHasher {
     size_t operator()(const Hash &h) const
     {
@@ -1259,6 +1264,14 @@ private:
     std::mutex mu_;
     std::condition_variable cv_;
 };
+struct ByteLease {  // RAII: the bytes go back to the semaphore on every path
+    ByteSemaphore &sem;
+    const uint64_t n;
+    ByteLease(ByteSemaphore &s, uint64_t bytes) : sem(s), n(bytes) { sem.acquire(n); }
+    ~ByteLease() { sem.release(n); }
+    ByteLease(const ByteLease &) = delete;
+    ByteLease &operator=(const ByteLease &) = delete;
+};
 
 // ---------------------------------------------------------------- generic batcher (row f1)
 template <class Item>
@@ -1498,22 +1511,22 @@ struct EncodeItem {
 };
 
 struct ReconItem {
-    uint8_t *stripe = nullptr;  // pinned slot: k+m shards, `stride` apart, survivors filled in by the caller
-    size_t stride = 0;
-    uint32_t block_len = 0;
-    uint8_t present[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
-    uint8_t want[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
-    // a ranged GET (garage_ec_decode_range_stripes): `present` is the plan's presence map, bytes [off, off + len) of
-    // the block go to `out`
-    bool range = false;
-    uint32_t off = 0, len = 0;
-    uint8_t *out = nullptr;
-    std::atomic<uint64_t> *call_us = nullptr;  // non-NULL: also gets the wall time of the call that rebuilt this stripe
-    // an opened GET (garage_ec_open_stripes): `block_len` is the sealed length, the plaintext goes to `out`
-    bool open = false;
-    const uint8_t *key = nullptr;
-    Hash hash{};
-    uint32_t plain_len = 0;
+    // what the dispatcher does with the stripe, in the order a batch runs them: a ranged GET
+    // (garage_ec_decode_range_stripes), an opened GET (garage_ec_open_stripes), a ranged opened GET
+    // (garage_ec_open_range_stripes), a whole-shard rebuild (garage_ec_reconstruct_stripes)
+    enum Kind { kRange, kOpen, kOpenRange, kRebuild };
+    static constexpr int kKinds = kRebuild + 1;
+    Kind kind = kRebuild;
+    uint8_t *stripe = nullptr;  // pinned slot: k+m shards, slot_stride apart, survivors filled in by the caller
+    uint32_t block_len = 0;     // the stored length: the sealed length for the opened kinds
+    uint8_t present[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};  // the ranged kinds: the plan's presence map
+    uint8_t want[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};     // rebuild: the shards to rebuild
+    std::atomic<uint64_t> *call_us = nullptr;  // rebuild, non-NULL: also gets the wall time of the call that rebuilt it
+    uint32_t off = 0, len = 0;  // the ranged kinds: bytes [off, off + len) of the block or plaintext go to `out`
+    uint8_t *out = nullptr;     // the ranged kinds and open: where the bytes go
+    const uint8_t *key = nullptr;  // the opened kinds
+    Hash hash{};                   // open: the content address to check
+    uint32_t plain_len = 0;        // open: set by the dispatcher
     bool fulfilled = false;
     std::promise<int> done;
 };
@@ -1607,7 +1620,6 @@ struct garage_bm {
         scrub_checked{0}, scrub_corrupt{0}, enc_gpu_us{0}, rec_gpu_us{0}, corrupt_data_errors{0}, write_errors{0},
         resync_shards_read{0}, resync_bytes_read{0}, resync_bytes_fetched{0};
     std::atomic<uint64_t> resync_deferred{0}, resync_steps{0}, resync_retry_nows{0}, resync_failed_bytes_read{0};
-    std::atomic<uint64_t> put_ns_slot{0}, put_ns_land{0}, put_ns_wait{0}, put_ns_store{0};
     std::atomic<uint64_t> convert_blocks{0}, convert_bytes_read{0}, convert_bytes_written{0}, convert_errors{0},
         convert_call_us{0}, legacy_gets{0}, legacy_deleted{0}, range_gets{0}, range_degraded{0}, range_bytes_read{0},
         range_bytes_fetched{0};
@@ -1795,7 +1807,8 @@ struct garage_bm {
     // `for_dma`: the GPU reads `dst` next (degraded GET, resync): see copy_for_dma
     // index >= 0: the node's shard of that index (several active layout versions)
     // span other than the whole shard (a PB half, or the tag span of a ranged GET): a ranged read of its bytes into
-    // dst, checked against the tag segments it covers (garage_ec_check_shard_span_host)
+    // dst, checked against the tag segments it covers (garage_ec_check_shard_span_host); an empty span reads and checks
+    // the header alone (dst may be NULL)
     bool read_shard_into(int node, const Hash &h, uint8_t *dst, size_t cap, ShardMeta &mt, bool for_dma = false, int code = 0,
                          int index = -1, ShardSpan span = {})
     {
@@ -1822,8 +1835,8 @@ struct garage_bm {
                 size_t off = 0, n = 0;
                 span.resolve(mt.shard_len, off, n);
                 bytes_read += n;
-                if (garage_ec_check_shard_span_host(mt.sum_kind, dst, mt.shard_len, (uint32_t)off, (uint32_t)n,
-                                                    mt.sum.data()) == GARAGE_EC_OK)
+                if (!n || garage_ec_check_shard_span_host(mt.sum_kind, dst, mt.shard_len, (uint32_t)off, (uint32_t)n,
+                                                          mt.sum.data()) == GARAGE_EC_OK)
                     return true;
             } else {
                 bytes_read += mt.shard_len;
@@ -1842,6 +1855,16 @@ struct garage_bm {
     {
         uint32_t s = 0;
         return garage_ec_sealed_len(cfg.block_size, &s) == GARAGE_EC_OK ? s : cfg.block_size;
+    }
+    // the plaintext length of a block sealed to S bytes (DESIGN.md section 2.6: S = 8 + P + 16 n for its n chunks of at
+    // most 4096 plaintext bytes and a tag each); false for an S the framing cannot hold (garage_ec_sealed_range's rule)
+    static bool plain_len_of(uint32_t S, uint32_t &P)
+    {
+        uint32_t so, sl, c0, nch;
+        if (garage_ec_sealed_range(S, 0, 0, &so, &sl, &c0, &nch) != GARAGE_EC_OK) return false;
+        constexpr uint64_t kSealedChunk = 4096 + 16;
+        P = (uint32_t)(S - 8 - 16 * ((S - 8 + kSealedChunk - 1) / kSealedChunk));
+        return true;
     }
 
     static void wipe_secret(void *p, size_t n)
@@ -1883,7 +1906,7 @@ struct garage_bm {
         if (rc == GARAGE_EC_OK)
             rc = garage_ec_seal_blocks(enc_ctx[w], ptrs.data(), lens.data(), keyed ? keys.data() : nullptr,
                                        keyed ? nonces.data() : nullptr, sh, stride, hashes, sums, n);
-        seal_call_us += (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count();
+        seal_call_us += us_since(t0);
         sealed_batches++;
         if (keyed) wipe_secret(keys.data(), keys.size());
         for (size_t i = 0; i < n; i++) {
@@ -1925,7 +1948,7 @@ struct garage_bm {
         const auto t0 = Clock::now();
         if (rc == GARAGE_EC_OK)
             rc = garage_ec_encode_blocks_with_sums(enc_ctx[w], ptrs.data(), lens.data(), n, par, sums, stride);
-        enc_gpu_us += (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count();
+        enc_gpu_us += us_since(t0);
         if (rc == GARAGE_EC_OK) bb.set_pending((int)n);
         for (size_t i = 0; i < n; i++) {
             if (rc == GARAGE_EC_OK) {
@@ -1939,121 +1962,22 @@ struct garage_bm {
         }
     }
 
+    // a dispatcher batch: one call per kind of item in it
     void run_reconstruct(int w, std::vector<ReconItem *> &all)
     {
-        std::vector<ReconItem *> b, rb, ob, orb;  // whole-shard rebuilds, ranged GETs, opened GETs, ranged opened GETs
-        for (ReconItem *it : all) (it->open && it->range ? orb : it->open ? ob : it->range ? rb : b).push_back(it);
-        if (!rb.empty()) run_decode_range(w, rb);
-        if (!ob.empty()) run_open(w, ob);
-        if (!orb.empty()) run_open_range(w, orb);
-        if (b.empty()) return;
-        const size_t n = b.size();
-        std::vector<uint8_t *> stripes(n);
-        std::vector<uint8_t> present(n * tot), want(n * tot);
-        std::vector<uint32_t> lens(n);
-        std::vector<int32_t> status(n, 0);
-        for (size_t i = 0; i < n; i++) {
-            stripes[i] = b[i]->stripe;
-            lens[i] = (uint32_t)shard_len_of(b[i]->block_len);
-            memcpy(present.data() + i * tot, b[i]->present, tot);
-            memcpy(want.data() + i * tot, b[i]->want, tot);
-        }
-        const auto t0 = Clock::now();
-        int rc = garage_ec_reconstruct_stripes(rec_ctx[w], stripes.data(), present.data(), want.data(), status.data(),
-                                               lens.data(), slot_stride, n);
-        const uint64_t us = (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count();
-        rec_gpu_us += us;
-        std::vector<std::atomic<uint64_t> *> counted;  // each extra counter gets the call's time once
-        for (size_t i = 0; i < n; i++)
-            if (b[i]->call_us && std::find(counted.begin(), counted.end(), b[i]->call_us) == counted.end()) {
-                counted.push_back(b[i]->call_us);
-                *b[i]->call_us += us;
-            }
-        for (size_t i = 0; i < n; i++) {
-            int r = rc;
-            if (rc == GARAGE_EC_OK || rc == GARAGE_EC_E_UNRECOVERABLE) r = status[i] ? GARAGE_BM_E_MISSING_BLOCK : GARAGE_BM_OK;
-            b[i]->fulfilled = true;
-            b[i]->done.set_value(r);
-        }
+        std::vector<ReconItem *> by_kind[ReconItem::kKinds];
+        for (ReconItem *it : all) by_kind[it->kind].push_back(it);
+        for (auto &b : by_kind)
+            if (!b.empty()) run_kind(w, b);
     }
 
-    // the opened GETs of a dispatcher batch: one garage_ec_open_stripes on their stripe slots -- rebuild, content hash,
-    // every chunk's tag, decryption.  Per item: OK, GARAGE_EC_E_AUTH, GARAGE_BM_E_MISSING_BLOCK, or
-    // GARAGE_BM_E_CORRUPT_DATA for a block that does not hash to its address (the caller hunts the stale shard)
-    void run_open(int w, std::vector<ReconItem *> &b)
+    // The items of one kind: one garage_ec_* call on their stripe slots.  The columns every kind passes are packed
+    // here; each kind adds its own, makes its call, adds the call's time to its counter and fulfils the items with its
+    // verdict: an item's result when the call's rc is one the kind lists (any other rc is every item's result).
+    void run_kind(int w, std::vector<ReconItem *> &b)
     {
         const size_t n = b.size();
         std::vector<uint8_t *> stripes(n), outs(n);
-        std::vector<uint8_t> present(n * tot), hashes(n * 32), keys(n * 32), bad(n, 0);
-        std::vector<uint32_t> sealed(n), plen(n, 0);
-        std::vector<int32_t> status(n, 0);
-        for (size_t i = 0; i < n; i++) {
-            stripes[i] = b[i]->stripe;
-            outs[i] = b[i]->out;
-            sealed[i] = b[i]->block_len;
-            memcpy(present.data() + i * tot, b[i]->present, tot);
-            memcpy(hashes.data() + i * 32, b[i]->hash.data(), 32);
-            memcpy(keys.data() + i * 32, b[i]->key, 32);
-        }
-        const auto t0 = Clock::now();
-        const int rc = garage_ec_open_stripes(rec_ctx[w], stripes.data(), present.data(), sealed.data(), hashes.data(),
-                                              keys.data(), outs.data(), plen.data(), bad.data(), status.data(), slot_stride, n);
-        open_call_us += (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count();
-        wipe_secret(keys.data(), keys.size());
-        for (size_t i = 0; i < n; i++) {
-            int r = rc;
-            if (rc == GARAGE_EC_OK || rc == GARAGE_EC_E_UNRECOVERABLE || rc == GARAGE_EC_E_AUTH)
-                // a block that does not hash to its address is the wrong block (a stale shard): its tags say
-                // nothing about the key, so the caller hunts the shard before any verdict on authentication
-                r = status[i] == GARAGE_EC_E_UNRECOVERABLE ? GARAGE_BM_E_MISSING_BLOCK
-                    : bad[i]                             ? GARAGE_BM_E_CORRUPT_DATA
-                    : status[i]                          ? status[i]
-                                                         : GARAGE_BM_OK;
-            b[i]->plain_len = plen[i];
-            b[i]->fulfilled = true;
-            b[i]->done.set_value(r);
-        }
-    }
-
-    // the ranged opened GETs of a dispatcher batch: one garage_ec_open_range_stripes on their stripe slots.  Per item:
-    // OK, GARAGE_EC_E_AUTH or GARAGE_BM_E_MISSING_BLOCK
-    void run_open_range(int w, std::vector<ReconItem *> &b)
-    {
-        const size_t n = b.size();
-        std::vector<const uint8_t *> stripes(n);
-        std::vector<uint8_t *> outs(n);
-        std::vector<uint8_t> present(n * tot), keys(n * 32);
-        std::vector<uint32_t> sealed(n), offs(n), lens(n);
-        std::vector<int32_t> status(n, 0);
-        for (size_t i = 0; i < n; i++) {
-            stripes[i] = b[i]->stripe;
-            outs[i] = b[i]->out;
-            sealed[i] = b[i]->block_len;
-            offs[i] = b[i]->off;
-            lens[i] = b[i]->len;
-            memcpy(present.data() + i * tot, b[i]->present, tot);
-            memcpy(keys.data() + i * 32, b[i]->key, 32);
-        }
-        const auto t0 = Clock::now();
-        const int rc = garage_ec_open_range_stripes(rec_ctx[w], stripes.data(), present.data(), sealed.data(), keys.data(),
-                                                    offs.data(), lens.data(), slot_stride, outs.data(), status.data(), n);
-        sealed_range_call_us += (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count();
-        wipe_secret(keys.data(), keys.size());
-        for (size_t i = 0; i < n; i++) {
-            int r = rc;
-            if (rc == GARAGE_EC_OK || rc == GARAGE_EC_E_UNRECOVERABLE || rc == GARAGE_EC_E_AUTH)
-                r = status[i] == GARAGE_EC_E_UNRECOVERABLE ? GARAGE_BM_E_MISSING_BLOCK : status[i] ? status[i] : GARAGE_BM_OK;
-            b[i]->fulfilled = true;
-            b[i]->done.set_value(r);
-        }
-    }
-
-    // the ranged GETs of a dispatcher batch: one garage_ec_decode_range_stripes on their stripe slots
-    void run_decode_range(int w, std::vector<ReconItem *> &b)
-    {
-        const size_t n = b.size();
-        std::vector<const uint8_t *> stripes(n);
-        std::vector<uint8_t *> outs(n);
         std::vector<uint8_t> present(n * tot);
         std::vector<uint32_t> blen(n), offs(n), lens(n);
         std::vector<int32_t> status(n, 0);
@@ -2065,43 +1989,118 @@ struct garage_bm {
             lens[i] = b[i]->len;
             memcpy(present.data() + i * tot, b[i]->present, tot);
         }
-        const auto t0 = Clock::now();
-        int rc = garage_ec_decode_range_stripes(rec_ctx[w], stripes.data(), present.data(), blen.data(), offs.data(),
+        std::vector<uint8_t> keys;  // the opened kinds: wiped right after their call
+        auto pack_keys = [&] {
+            keys.resize(n * 32);
+            for (size_t i = 0; i < n; i++) memcpy(keys.data() + i * 32, b[i]->key, 32);
+        };
+        int rc = GARAGE_EC_E_INVALID;
+        auto fulfil = [&](bool listed, const std::function<int(size_t)> &verdict) {
+            for (size_t i = 0; i < n; i++) {
+                b[i]->fulfilled = true;
+                b[i]->done.set_value(listed ? verdict(i) : rc);
+            }
+        };
+        switch (b[0]->kind) {
+        case ReconItem::kRebuild: {
+            std::vector<uint8_t> want(n * tot);
+            for (size_t i = 0; i < n; i++) {
+                blen[i] = (uint32_t)shard_len_of(blen[i]);  // this call takes shard lengths
+                memcpy(want.data() + i * tot, b[i]->want, tot);
+            }
+            const auto t0 = Clock::now();
+            rc = garage_ec_reconstruct_stripes(rec_ctx[w], stripes.data(), present.data(), want.data(), status.data(),
+                                               blen.data(), slot_stride, n);
+            const uint64_t us = us_since(t0);
+            rec_gpu_us += us;
+            std::set<std::atomic<uint64_t> *> counters;  // each extra counter gets the call's time once
+            for (ReconItem *it : b)
+                if (it->call_us) counters.insert(it->call_us);
+            for (auto *c : counters) *c += us;
+            fulfil(rc == GARAGE_EC_OK || rc == GARAGE_EC_E_UNRECOVERABLE,
+                   [&](size_t i) { return status[i] ? GARAGE_BM_E_MISSING_BLOCK : GARAGE_BM_OK; });
+            break;
+        }
+        case ReconItem::kRange: {
+            const auto t0 = Clock::now();
+            rc = garage_ec_decode_range_stripes(rec_ctx[w], stripes.data(), present.data(), blen.data(), offs.data(),
                                                 lens.data(), slot_stride, outs.data(), status.data(), n);
-        rec_gpu_us += (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count();
-        for (size_t i = 0; i < n; i++) {
-            int r = rc;
-            if (rc == GARAGE_EC_OK || rc == GARAGE_EC_E_UNRECOVERABLE) r = status[i] ? GARAGE_BM_E_MISSING_BLOCK : GARAGE_BM_OK;
-            b[i]->fulfilled = true;
-            b[i]->done.set_value(r);
+            rec_gpu_us += us_since(t0);
+            fulfil(rc == GARAGE_EC_OK || rc == GARAGE_EC_E_UNRECOVERABLE,
+                   [&](size_t i) { return status[i] ? GARAGE_BM_E_MISSING_BLOCK : GARAGE_BM_OK; });
+            break;
+        }
+        case ReconItem::kOpen: {
+            std::vector<uint8_t> hashes(n * 32), bad(n, 0);
+            std::vector<uint32_t> plen(n, 0);
+            for (size_t i = 0; i < n; i++) memcpy(hashes.data() + i * 32, b[i]->hash.data(), 32);
+            pack_keys();
+            const auto t0 = Clock::now();
+            rc = garage_ec_open_stripes(rec_ctx[w], stripes.data(), present.data(), blen.data(), hashes.data(), keys.data(),
+                                        outs.data(), plen.data(), bad.data(), status.data(), slot_stride, n);
+            open_call_us += us_since(t0);
+            wipe_secret(keys.data(), keys.size());
+            for (size_t i = 0; i < n; i++) b[i]->plain_len = plen[i];
+            // a block that does not hash to its address is the wrong block (a stale shard): its tags say nothing about
+            // the key, so the caller hunts the shard before any verdict on authentication
+            fulfil(rc == GARAGE_EC_OK || rc == GARAGE_EC_E_UNRECOVERABLE || rc == GARAGE_EC_E_AUTH, [&](size_t i) {
+                return status[i] == GARAGE_EC_E_UNRECOVERABLE ? GARAGE_BM_E_MISSING_BLOCK
+                       : bad[i]                             ? GARAGE_BM_E_CORRUPT_DATA
+                       : status[i]                          ? status[i]
+                                                            : GARAGE_BM_OK;
+            });
+            break;
+        }
+        case ReconItem::kOpenRange: {
+            pack_keys();
+            const auto t0 = Clock::now();
+            rc = garage_ec_open_range_stripes(rec_ctx[w], stripes.data(), present.data(), blen.data(), keys.data(),
+                                              offs.data(), lens.data(), slot_stride, outs.data(), status.data(), n);
+            sealed_range_call_us += us_since(t0);
+            wipe_secret(keys.data(), keys.size());
+            fulfil(rc == GARAGE_EC_OK || rc == GARAGE_EC_E_UNRECOVERABLE || rc == GARAGE_EC_E_AUTH, [&](size_t i) {
+                return status[i] == GARAGE_EC_E_UNRECOVERABLE ? GARAGE_BM_E_MISSING_BLOCK : status[i] ? status[i] : GARAGE_BM_OK;
+            });
+            break;
+        }
         }
     }
 
-    // The sources of every index of h's stripe of `code`, in the order to try them: with several active layout
-    // versions (code 0) those garage_layout_read_plan lists, and true (read each source's file of that index); else the
-    // index's ring node.
-    bool shard_sources(const Hash &h, int code, int (*src)[GARAGE_BM_MAX_LAYOUT_VERSIONS], int *nsrc)
+    // The sources of every index of h's stripe of `code`, in the order to try them, and per index a cursor on the next
+    // one: with several active layout versions (code 0) the sources garage_layout_read_plan lists, each read for its file
+    // of that index (by_index); else the index's ring node.  Node `skip` is left out of the indices `skip_for` names
+    // (NULL: of every index).
+    struct ShardSources {
+        int src[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M][GARAGE_BM_MAX_LAYOUT_VERSIONS];
+        int nsrc[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0}, cur[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
+        bool by_index = false;
+        bool left(int i) const { return cur[i] < nsrc[i]; }  // a source of index i is left to try
+        int node(int i) const { return src[i][cur[i]]; }
+        int file(int i) const { return by_index ? i : -1; }  // the index argument of read_shard_into and quarantine
+        void next(int i) { cur[i]++; }
+    };
+    ShardSources shard_sources(const Hash &h, int code, int skip = -1, const uint8_t *skip_for = nullptr)
     {
-        constexpr int kMaxSrc = GARAGE_BM_MAX_LAYOUT_VERSIONS;
         const int k = codes[code].k, tot = codes[code].tot;
-        for (int i = 0; i < tot; i++) nsrc[i] = 0;
+        ShardSources s;
+        auto add = [&](int i, int node) {
+            if (i < tot && s.nsrc[i] < GARAGE_BM_MAX_LAYOUT_VERSIONS && !(node == skip && (!skip_for || skip_for[i])))
+                s.src[i][s.nsrc[i]++] = node;
+        };
         auto ls = layouts();
         if (code == 0 && ls->v.size() > 1) {
-            garage_shard_source plan[(GARAGE_EC_MAX_K + GARAGE_EC_MAX_M) * kMaxSrc];
+            garage_shard_source plan[(GARAGE_EC_MAX_K + GARAGE_EC_MAX_M) * GARAGE_BM_MAX_LAYOUT_VERSIONS];
             const auto act = ls->raw();
             const int np = garage_layout_read_plan(act.data(), (int)act.size(), nullptr, 0, h.data(), k, -1, nullptr, plan,
                                                    (int)(sizeof(plan) / sizeof(plan[0])));
-            for (int s = 0; s < np; s++)
-                if (plan[s].index < tot && nsrc[plan[s].index] < kMaxSrc) src[plan[s].index][nsrc[plan[s].index]++] = plan[s].node;
-            return true;
+            for (int x = 0; x < np; x++) add(plan[x].index, plan[x].node);
+            s.by_index = true;
+            return s;
         }
         int who[64];
         nodes_of(h, code, who);
-        for (int i = 0; i < tot; i++) {
-            src[i][0] = who[i];
-            nsrc[i] = 1;
-        }
-        return false;
+        for (int i = 0; i < tot; i++) add(i, who[i]);
+        return s;
     }
 
     // Read the valid shards of `h` from every up node except `skip_node` into the stripe slot
@@ -2136,15 +2135,7 @@ struct garage_bm {
             for (int i = 0; i < tot; i++) rd[i] = rd[i] ? 3 : 0;
             return rc;
         };
-        constexpr int kMaxSrc = GARAGE_BM_MAX_LAYOUT_VERSIONS;
-        int src[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M][kMaxSrc], nsrc[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0},
-            cur[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
-        const bool by_index = shard_sources(h, code, src, nsrc);  // read each source's file of that index
-        // a source of index i is left to try
-        auto left = [&](int i) {
-            while (cur[i] < nsrc[i] && src[i][cur[i]] == skip_node && (!want_in || want_in[i])) cur[i]++;
-            return cur[i] < nsrc[i];
-        };
+        ShardSources srcs = shard_sources(h, code, skip_node, want_in);
         memset(have, 0, tot);
         uint32_t expect = 0;
         bool have_expect = false;
@@ -2161,8 +2152,8 @@ struct garage_bm {
         uint8_t have_h[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};  // halves held: bit 0 a, bit 1 b (3 = whole shard)
         // whole shard (half < 0) or one half of it
         auto try_shard = [&](int i, int half = -1) {
-            if (!left(i) || have_h[i] == 3) return;
-            const int node = src[i][cur[i]], fidx = by_index ? i : -1;
+            if (!srcs.left(i) || have_h[i] == 3) return;
+            const int node = srcs.node(i), fidx = srcs.file(i);
             ShardMeta mt;
             uint8_t *dst = slot + (size_t)i * slot_stride;
             bool got;
@@ -2181,7 +2172,7 @@ struct garage_bm {
                     have[i] = 0;
                     count--;
                 }
-                cur[i]++;
+                srcs.next(i);
                 return;
             }
             if (mt.index != i || (have_expect && mt.block_len != expect)) {
@@ -2189,7 +2180,7 @@ struct garage_bm {
                 if (have_h[i]) count--;
                 have_h[i] = 0;
                 have[i] = 0;
-                cur[i]++;
+                srcs.next(i);
                 return;
             }
             if (from_out) from_out[i] = node;
@@ -2205,7 +2196,7 @@ struct garage_bm {
         uint8_t want[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
         auto attempt = [&](int i) {  // whole shard i from its sources in order, until one is good
             do try_shard(i);
-            while (!have[i] && left(i));
+            while (!have[i] && srcs.left(i));
         };
         if (all) {
             for (int i = 0; i < tot; i++) attempt(i);
@@ -2223,7 +2214,7 @@ struct garage_bm {
                 // assume every shard with a source not yet tried is there, a wanted one excepted; fetch what the read
                 // plan still lacks (RS / LRC: whole shards of the read set; PB: the planned halves)
                 uint8_t guess[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M], rd[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
-                for (int i = 0; i < tot; i++) guess[i] = have[i] || (!want[i] && left(i));
+                for (int i = 0; i < tot; i++) guess[i] = have[i] || (!want[i] && srcs.left(i));
                 if (plan(guess, want, rd) != GARAGE_EC_OK) break;
                 bool fetched = false, missing = false;
                 for (int i = 0; i < tot; i++) {
@@ -2264,13 +2255,12 @@ struct garage_bm {
             int32_t st = 0;
             const auto t0 = Clock::now();
             int rc = garage_ec_reconstruct_stripes(codes[code].ctx, &slot, have, want, &st, &L, slot_stride, 1);
-            rec_gpu_us += (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count();
+            rec_gpu_us += us_since(t0);
             if (rc == GARAGE_EC_OK || rc == GARAGE_EC_E_UNRECOVERABLE) rc = st ? GARAGE_BM_E_MISSING_BLOCK : GARAGE_BM_OK;
             return rc;
         }
         ReconItem it;
         it.stripe = slot;
-        it.stride = slot_stride;
         it.block_len = block_len;
         memcpy(it.present, have, tot);
         memcpy(it.want, want, tot);
@@ -2299,40 +2289,16 @@ struct garage_bm {
     {
         if (len == 0 || len > cfg.block_size) return GARAGE_BM_E_MESSAGE;  // blocks are at most block_size (put.rs:583-617)
         // DataBlock::from_buffer (manager.rs:376): compression is 'none' in this mirror
-        const uint64_t permits = (uint64_t)len * tot / k;  // manager.rs:380-385, x (k+m)/k for the parity
-        ram->acquire(permits);
-        struct Permit {
-            ByteSemaphore &s;
-            uint64_t n;
-            ~Permit() { s.release(n); }
-        } permit{*ram, permits};
+        ByteLease permit(*ram, (uint64_t)len * tot / k);  // manager.rs:380-385, x (k+m)/k for the parity
         put_calls++;
         // land the block in pinned memory (caller's thread, so copies of concurrent PUTs overlap)
-        const auto t_in = Clock::now();
         SlotLease slot(put_slots);
-        const auto t_slot = Clock::now();
         copy_for_dma(slot.p, data, len);  // landing copy: the GPU reads the slot next
         EncodeItem it;
         it.data = slot.p;
         it.len = (uint32_t)len;
-        const auto t_sub = Clock::now();
         int rc = enc_batcher->submit(it);
         if (rc != GARAGE_EC_OK) return rc;
-        const auto t_enc = Clock::now();
-        struct PhaseNote {  // where a PUT's wall time goes (GARAGE_BM_TRACE prints the sums after a bench run)
-            garage_bm &bm;
-            Clock::time_point a, b, c, d;
-            ~PhaseNote()
-            {
-                auto us = [](Clock::time_point x, Clock::time_point y) {
-                    return (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(y - x).count();
-                };
-                bm.put_ns_slot += us(a, b);
-                bm.put_ns_land += us(b, c);
-                bm.put_ns_wait += us(c, d);
-                bm.put_ns_store += us(d, Clock::now());
-            }
-        } note{*this, t_in, t_slot, t_sub, t_enc};
         struct BufRelease {
             EncBatchBuf *b;
             ~BufRelease() { b->done_one(); }
@@ -2379,13 +2345,7 @@ struct garage_bm {
         if (len > cfg.block_size || (!key && len == 0)) return GARAGE_BM_E_MESSAGE;
         uint32_t blen = (uint32_t)len;
         if (key && garage_ec_sealed_len((uint32_t)len, &blen) != GARAGE_EC_OK) return GARAGE_BM_E_MESSAGE;
-        const uint64_t permits = (uint64_t)blen * tot / k;
-        ram->acquire(permits);
-        struct Permit {
-            ByteSemaphore &s;
-            uint64_t n;
-            ~Permit() { s.release(n); }
-        } permit{*ram, permits};
+        ByteLease permit(*ram, (uint64_t)blen * tot / k);
         SlotLease slot(put_slots);
         if (len) copy_for_dma(slot.p, data, len);
         EncodeItem it;
@@ -2412,12 +2372,11 @@ struct garage_bm {
     int open_in_slot(const Hash &h, const uint8_t *key, uint8_t *slot, uint32_t block_len, const uint8_t *have, uint8_t *out,
                      size_t cap, size_t *out_len)
     {
-        const uint32_t n = block_len >= 24 ? (block_len - 8 + 4111) / 4112 : 1;
-        if (block_len >= 24 && block_len - 8 - 16ull * n > cap) return GARAGE_EC_E_INVALID;
+        uint32_t plain = 0;
+        if (plain_len_of(block_len, plain) && plain > cap) return GARAGE_EC_E_INVALID;
         ReconItem it;
-        it.open = true;
+        it.kind = ReconItem::kOpen;
         it.stripe = slot;
-        it.stride = slot_stride;
         it.block_len = block_len;
         memcpy(it.present, have, tot);
         it.key = key;
@@ -2465,8 +2424,7 @@ struct garage_bm {
             const size_t off = (size_t)j * L;
             if (off < blen) memcpy(row, blk.data() + off, std::min(L, blen - off));
         }
-        rc = open_in_slot(h, key, slot.p, (uint32_t)blen, have, out, cap, out_len);
-        return rc == GARAGE_BM_E_CORRUPT_DATA ? GARAGE_BM_E_CORRUPT_DATA : rc;
+        return open_in_slot(h, key, slot.p, (uint32_t)blen, have, out, cap, out_len);
     }
     // PUT during a layout change: one shard per (node, index) request of garage_layout_write_plan, and the write quorum
     // in the node set of every active version (try_write_many_sets, rpc_helper.rs:432-538)
@@ -2512,49 +2470,35 @@ struct garage_bm {
 
     // The gather of the ranged GETs.  The block length and tag kind come from the first configured-code shard header
     // that reads (a bad one quarantines its shard); pre(block_len) then returns 0 to go on, kRangeWhole or an error to
-    // stop with.  plan(present, block_len, runs, cap, &n, &gpu) names the runs to fetch (garage_ec_range_plan's format);
-    // each holder reads only the tag span covering its runs (garage_ec_tag_span) into `slot` and checks it against the
-    // shard's tag; a span that fails, or a shard whose header does not match, quarantines its shard and the plan is
+    // stop with.  plan (garage_ec_range_plan or garage_ec_open_range_plan) names the runs of range [off, off + len) to
+    // fetch; each holder reads only the tag span covering its runs (garage_ec_tag_span) into `slot` and checks it against
+    // the shard's tag; a span that fails, or a shard whose header does not match, quarantines its shard and the plan is
     // recomputed without it.  On GARAGE_BM_OK: `present` is the final plan's presence map, *gpu its needs_gpu, and
     // `fetched_ctr` has the planned run bytes added.  kRangeNoHeader if no configured-code header reads.
     static constexpr int kRangeWhole = 1, kRangeNoHeader = 2;
-    using RangePlanFn = std::function<int(const uint8_t *, uint32_t, garage_ec_range *, size_t, size_t *, int *)>;
-    int gather_ranged(const Hash &h, uint8_t *slot, const std::function<int(uint32_t)> &pre, const RangePlanFn &plan,
-                      uint32_t &block_len, uint8_t *present, int *gpu, std::atomic<uint64_t> &read_ctr,
+    using RangePlanFn = int (*)(const garage_ec_ctx *, const uint8_t *, uint32_t, uint32_t, uint32_t, garage_ec_range *,
+                                size_t, size_t *, int *);
+    int gather_ranged(const Hash &h, uint8_t *slot, const std::function<int(uint32_t)> &pre, RangePlanFn plan, uint32_t off,
+                      uint32_t len, uint32_t &block_len, uint8_t *present, int *gpu, std::atomic<uint64_t> &read_ctr,
                       std::atomic<uint64_t> &fetched_ctr)
     {
         const Code &cd = codes[0];
         const int tot = cd.tot;
-        constexpr int kMaxSrc = GARAGE_BM_MAX_LAYOUT_VERSIONS;
-        int src[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M][kMaxSrc], nsrc[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0},
-            cur[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
-        const bool by_index = shard_sources(h, 0, src, nsrc);
-        auto left = [&](int i) { return cur[i] < nsrc[i]; };
+        ShardSources srcs = shard_sources(h, 0);
         ShardMeta m0;
         bool have_len = false;
-        for (int i = 0; i < tot && !have_len; i++) {
-            while (left(i) && !have_len) {
-                Node &nd = *nodes[src[i][cur[i]]];
-                ReadResult r = kReadMissing;
+        for (int i = 0; i < tot && !have_len; i++)
+            for (; srcs.left(i); srcs.next(i)) {  // a down holder or a missing file: the next source
                 ShardMeta mt;
-                Node::ShardPtr sp;
-                {
-                    std::lock_guard<std::mutex> lk(nd.mu);
-                    if (nd.up) {
-                        if (nd.dir.empty()) sp = nd.store_find(h);
-                        else r = nd.store_read_into(h, nullptr, 0, mt, ShardSpan::bytes(0, 0), 0, by_index ? i : -1);
-                    }
-                }
-                if (sp) r = nd.copy_out(*sp, nullptr, 0, mt, false, ShardSpan::bytes(0, 0));
-                if (r == kReadOk && mt.index == i) {
+                if (!read_shard_into(srcs.node(i), h, nullptr, 0, mt, false, 0, srcs.file(i), ShardSpan::bytes(0, 0)))
+                    continue;
+                if (mt.index == i) {
                     m0 = mt;
                     have_len = true;
                     break;
                 }
-                if (r != kReadMissing) quarantine(src[i][cur[i]], h, 0, by_index ? i : -1);
-                cur[i]++;
+                quarantine(srcs.node(i), h, 0, srcs.file(i));  // a misplaced shard
             }
-        }
         if (!have_len) return kRangeNoHeader;
         block_len = m0.block_len;
         const uint32_t L = (uint32_t)shard_len_of(block_len);
@@ -2565,8 +2509,8 @@ struct garage_bm {
         std::vector<garage_ec_range> runs((size_t)tot * ((cd.clay ? cd.quantum / 16 : 1) + 2) * 2);
         size_t nr = 0;
         for (;;) {
-            for (int i = 0; i < tot; i++) present[i] = fetched[i] || left(i);
-            rc = plan(present, block_len, runs.data(), runs.size(), &nr, gpu);
+            for (int i = 0; i < tot; i++) present[i] = fetched[i] || srcs.left(i);
+            rc = plan(cd.ctx, present, block_len, off, len, runs.data(), runs.size(), &nr, gpu);
             if (rc == GARAGE_EC_E_UNRECOVERABLE) return GARAGE_BM_E_MISSING_BLOCK;
             if (rc != GARAGE_EC_OK) return rc;
             uint32_t lo[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M], hi[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
@@ -2581,8 +2525,8 @@ struct garage_bm {
                 uint32_t so = 0, sl = 0;
                 if (garage_ec_tag_span(m0.sum_kind, L, lo[i], hi[i] - lo[i], &so, &sl) != GARAGE_EC_OK) return GARAGE_EC_E_INVALID;
                 fetched[i] = 0;
-                while (left(i)) {  // a shard's runs come from one source
-                    const int node = src[i][cur[i]], fidx = by_index ? i : -1;
+                for (; srcs.left(i); srcs.next(i)) {  // a shard's runs come from one source
+                    const int node = srcs.node(i), fidx = srcs.file(i);
                     ShardMeta mt;
                     bool got = read_shard_into(node, h, slot + (size_t)i * slot_stride + so, slot_stride - so, mt, true, 0,
                                                fidx, ShardSpan::bytes(so, sl));
@@ -2597,7 +2541,6 @@ struct garage_bm {
                         f_hi[i] = so + sl;
                         break;
                     }
-                    cur[i]++;
                 }
                 replan = !fetched[i];  // the shard is out: the plan changes
             }
@@ -2605,6 +2548,37 @@ struct garage_bm {
         }
         for (size_t x = 0; x < nr; x++) fetched_ctr += runs[x].len;
         return GARAGE_BM_OK;
+    }
+
+    // bytes [off, off + len) of the whole block (or plaintext) that `whole` -- rpc_get_block or rpc_get_block_opened --
+    // writes into a stored_max() buffer: the ranged GETs' route through a whole-block GET
+    int slice_whole(const std::function<int(uint8_t *, size_t, size_t *)> &whole, uint32_t off, uint32_t len, uint8_t *out,
+                    size_t cap, size_t *out_len)
+    {
+        std::vector<uint8_t> buf(stored_max());
+        size_t n = 0;
+        const int rc = whole(buf.data(), buf.size(), &n);
+        if (rc != GARAGE_BM_OK) return rc;
+        if ((uint64_t)off + len > n || len > cap) return GARAGE_EC_E_INVALID;
+        memcpy(out, buf.data() + off, len);
+        *out_len = len;
+        return GARAGE_BM_OK;
+    }
+    // a ranged item on the stripe gather_ranged left in `slot`, through the reconstruct dispatchers: a ranged GET, or
+    // with a key a ranged opened GET
+    int submit_range(uint8_t *slot, uint32_t block_len, const uint8_t *present, const uint8_t *key, uint32_t off,
+                     uint32_t len, uint8_t *out)
+    {
+        ReconItem it;
+        it.kind = key ? ReconItem::kOpenRange : ReconItem::kRange;
+        it.stripe = slot;
+        it.block_len = block_len;
+        memcpy(it.present, present, tot);
+        it.key = key;
+        it.off = off;
+        it.len = len;
+        it.out = out;
+        return rec_batcher->submit(it);
     }
 
     // Bytes [off, off + len) of block h into out (S3 GetObject with a Range header, body_from_blocks_range; the
@@ -2618,16 +2592,6 @@ struct garage_bm {
     int rpc_get_block_range(const Hash &h, uint32_t off, uint32_t len, uint8_t *out, size_t cap, size_t *out_len)
     {
         range_gets++;
-        auto sliced = [&]() -> int {  // the whole block through rpc_get_block, then the range of it
-            std::vector<uint8_t> whole(stored_max());
-            size_t n = 0;
-            const int rc = rpc_get_block(h, whole.data(), whole.size(), &n);
-            if (rc != GARAGE_BM_OK) return rc;
-            if ((uint64_t)off + len > n || len > cap) return GARAGE_EC_E_INVALID;
-            memcpy(out, whole.data() + off, len);
-            *out_len = len;
-            return GARAGE_BM_OK;
-        };
         uint8_t present[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
         uint32_t block_len = 0;
         int gpu = 0;
@@ -2639,10 +2603,7 @@ struct garage_bm {
                     if ((uint64_t)off + len > bl || len > cap) return GARAGE_EC_E_INVALID;
                     return off == 0 && len == bl ? kRangeWhole : 0;
                 },
-                [&](const uint8_t *pr, uint32_t bl, garage_ec_range *r, size_t c, size_t *nr, int *g) {
-                    return garage_ec_range_plan(codes[0].ctx, pr, bl, off, len, r, c, nr, g);
-                },
-                block_len, present, &gpu, range_bytes_read, range_bytes_fetched);
+                garage_ec_range_plan, off, len, block_len, present, &gpu, range_bytes_read, range_bytes_fetched);
             if (rc == GARAGE_BM_OK) {
                 *out_len = len;
                 if (!gpu) {  // every touched data shard is present: their range bytes, no GPU
@@ -2655,21 +2616,13 @@ struct garage_bm {
                     return GARAGE_BM_OK;
                 }
                 range_degraded++;
-                ReconItem it;
-                it.stripe = slot.p;
-                it.stride = slot_stride;
-                it.block_len = block_len;
-                memcpy(it.present, present, tot);
-                it.range = true;
-                it.off = off;
-                it.len = len;
-                it.out = out;
-                return rec_batcher->submit(it);
+                return submit_range(slot.p, block_len, present, nullptr, off, len, out);
             }
             if (rc == kRangeNoHeader && !has_legacy()) return GARAGE_BM_E_MISSING_BLOCK;
             if (rc != kRangeWhole && rc != kRangeNoHeader) return rc;
         }
-        return sliced();
+        return slice_whole([&](uint8_t *b, size_t c, size_t *n) { return rpc_get_block(h, b, c, n); }, off, len, out, cap,
+                           out_len);
     }
 
     // Plaintext bytes [off, off + len) of SSE-C block h sealed under key (a ranged GET or UploadPartCopy of an SSE-C
@@ -2683,23 +2636,12 @@ struct garage_bm {
     int rpc_get_block_range_opened(const Hash &h, const uint8_t *key, uint32_t off, uint32_t len, uint8_t *out,
                                    size_t cap, size_t *out_len)
     {
-        const auto t0 = Clock::now();
         struct Timer {
             std::atomic<uint64_t> &us;
             Clock::time_point t0;
-            ~Timer() { us += (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count(); }
-        } timer{sealed_range_us, t0};
+            ~Timer() { us += us_since(t0); }
+        } timer{sealed_range_us, Clock::now()};
         sealed_range_gets++;
-        auto sliced = [&]() -> int {  // the whole plaintext through rpc_get_block_opened, then the range of it
-            std::vector<uint8_t> whole(stored_max());
-            size_t n = 0;
-            const int rc = rpc_get_block_opened(h, key, whole.data(), whole.size(), &n);
-            if (rc != GARAGE_BM_OK) return rc;
-            if ((uint64_t)off + len > n || len > cap) return GARAGE_EC_E_INVALID;
-            memcpy(out, whole.data() + off, len);
-            *out_len = len;
-            return GARAGE_BM_OK;
-        };
         uint8_t present[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
         uint32_t block_len = 0;
         int gpu = 0, rc;
@@ -2708,30 +2650,16 @@ struct garage_bm {
             rc = gather_ranged(
                 h, slot.p,
                 [&](uint32_t bl) -> int {
-                    uint32_t so, sl, c0, nch;
-                    const int r = garage_ec_sealed_range(bl, off, len, &so, &sl, &c0, &nch);
-                    if (r) return r;
-                    if (len > cap) return GARAGE_EC_E_INVALID;
-                    const uint64_t P = bl - 8 - 16ull * ((bl - 8 + 4111) / 4112);
+                    uint32_t P = 0;
+                    if (!plain_len_of(bl, P)) return GARAGE_EC_E_AUTH;  // as garage_ec_sealed_range
+                    if ((uint64_t)off + len > P || len > cap) return GARAGE_EC_E_INVALID;
                     return (off == 0 && len == P) || !len ? kRangeWhole : 0;
                 },
-                [&](const uint8_t *pr, uint32_t bl, garage_ec_range *r, size_t c, size_t *nr, int *g) {
-                    return garage_ec_open_range_plan(codes[0].ctx, pr, bl, off, len, r, c, nr, g);
-                },
-                block_len, present, &gpu, sealed_range_bytes_read, sealed_range_bytes_fetched);
+                garage_ec_open_range_plan, off, len, block_len, present, &gpu, sealed_range_bytes_read,
+                sealed_range_bytes_fetched);
             if (rc == GARAGE_BM_OK) {
                 if (gpu) sealed_range_degraded++;
-                ReconItem it;
-                it.stripe = slot.p;
-                it.stride = slot_stride;
-                it.block_len = block_len;
-                memcpy(it.present, present, tot);
-                it.open = it.range = true;
-                it.key = key;
-                it.off = off;
-                it.len = len;
-                it.out = out;
-                rc = rec_batcher->submit(it);
+                rc = submit_range(slot.p, block_len, present, key, off, len, out);
                 if (rc == GARAGE_BM_OK) *out_len = len;
             }
         }
@@ -2741,7 +2669,8 @@ struct garage_bm {
         }
         if (rc == GARAGE_EC_E_AUTH || rc == kRangeWhole || (rc == kRangeNoHeader && has_legacy())) {
             if (rc == GARAGE_EC_E_AUTH) sealed_range_fallbacks++;
-            rc = sliced();
+            rc = slice_whole([&](uint8_t *b, size_t c, size_t *n) { return rpc_get_block_opened(h, key, b, c, n); }, off, len,
+                             out, cap, out_len);
             if (rc == GARAGE_EC_E_AUTH) sealed_range_auth_failures++;
             return rc;
         }
@@ -3019,7 +2948,6 @@ struct garage_bm {
                 const RebuildJob &jb = jobs[b0 + j];
                 ReconItem &it = items[j];
                 it.stripe = slots.p[j];
-                it.stride = slot_stride;
                 it.call_us = c.call_us;
                 memcpy(it.want, jb.want, tot);
                 for (;;) {
@@ -3469,7 +3397,7 @@ struct garage_bm {
                 auto t0 = Clock::now();
                 int rc = garage_ec_transcode(ec, rep ? nullptr : codes[c].ctx, src, rep ? nullptr : present.data(), lens.data(),
                                              s_stride, dst, slot_stride, sums, status.data(), n, GARAGE_EC_MEM_HOST, nullptr);
-                convert_call_us += (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count();
+                convert_call_us += us_since(t0);
                 if (rc != GARAGE_EC_OK && rc != GARAGE_EC_E_UNRECOVERABLE) continue;
                 // the new data shards must hash to the block before anything is written
                 std::vector<uint8_t> good(n, 0);
@@ -3494,8 +3422,7 @@ struct garage_bm {
                             t0 = Clock::now();
                             rc = garage_ec_transcode(ec, nullptr, blk, nullptr, &l32, rep_stride, dst + q * tot * slot_stride,
                                                      slot_stride, sums + q * tot * 32, &st, 1, GARAGE_EC_MEM_HOST, nullptr);
-                            convert_call_us +=
-                                (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count();
+                            convert_call_us += us_since(t0);
                             std::vector<uint8_t> tmp(lens[q]);
                             assemble(dst + q * tot * slot_stride, lens[q], tmp.data());
                             Hash got;
@@ -3640,7 +3567,7 @@ struct garage_bm {
             const auto t0 = Clock::now();
             const int rc_ = garage_ec_deep_check(ec, buf, lens.data(), hashes, hash_bad.data(), mm.data(), slot_stride, nc,
                                                  GARAGE_EC_MEM_HOST, nullptr);
-            deep_check_us += (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(Clock::now() - t0).count();
+            deep_check_us += us_since(t0);
             if (rc_ != GARAGE_EC_OK) return rc_;
             nchecked += nc;
             deep_blocks += nc;
@@ -4343,10 +4270,6 @@ struct garage_bm {
         go.store(true, std::memory_order_release);
         for (auto &x : th) x.join();
         const double el = std::chrono::duration<double>(Clock::now() - t0).count();
-        if (mode == 0 && getenv("GARAGE_BM_TRACE"))
-            fprintf(stderr, "[garage_bm] PUT x%zu, %d threads, %.3f s: per block ms  slot-wait %.3f  landing copy %.3f  batch+GPU %.3f  "
-                            "store %d shards %.3f\n", nb, threads, el, put_ns_slot.exchange(0) / 1e6 / nb, put_ns_land.exchange(0) / 1e6 / nb,
-                    put_ns_wait.exchange(0) / 1e6 / nb, tot, put_ns_store.exchange(0) / 1e6 / nb);
         if (gib_per_s) *gib_per_s = (double)nb * block_len / el / (double)(1ull << 30);
         if (errors) *errors = errs.load();
         return GARAGE_BM_OK;
