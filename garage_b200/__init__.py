@@ -45,6 +45,7 @@ ABI_SYMBOLS = [
     "garage_ec_decode_range_stripes",
     "garage_ec_sealed_len", "garage_ec_seal", "garage_ec_seal_blocks", "garage_ec_open", "garage_ec_open_stripes",
     "garage_ec_sealed_range", "garage_ec_open_range_plan", "garage_ec_open_range", "garage_ec_open_range_stripes",
+    "garage_ec_reseal", "garage_ec_reseal_stripes",
 ]
 
 
@@ -148,6 +149,8 @@ def load_library(build=True):
     L.garage_ec_open_range_plan.argtypes = [vp, vp, u32, u32, u32, vp, sz, C.POINTER(sz), C.POINTER(i32)]
     L.garage_ec_open_range.argtypes = [vp, vp, vp, vp, vp, vp, vp, sz, vp, sz, vp, sz, i32, vp]
     L.garage_ec_open_range_stripes.argtypes = [vp, vp, vp, vp, vp, vp, vp, sz, vp, vp, sz]
+    L.garage_ec_reseal.argtypes = [vp, vp, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, sz, i32, vp]
+    L.garage_ec_reseal_stripes.argtypes = [vp, vp, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, sz]
     _lib = L
     return L
 
@@ -592,6 +595,39 @@ class GarageEc:
                                                                 _ptr(sealed_len), _ptr(keys), _ptr(offset),
                                                                 _ptr(length), stride, C.cast(op, C.c_void_p),
                                                                 _ptr(status), n),
+                           (E_UNRECOVERABLE, E_AUTH))
+
+    # -- SSE-C copies with re-encryption (DESIGN.md 2.8)
+    def reseal(self, src_shards, src_present, src_len, src_hashes, src_keys, pieces, piece_start, dst_keys, dst_nonces,
+               dst_shards, dst_hashes, dst_len_out, src_hash_bad, src_status, status, stride, dst_sums=None,
+               n_src=None, n_dst=None):
+        """garage_ec_reseal: destination d = the pieces [piece_start[d], piece_start[d+1]) of `pieces` ((src, offset,
+        len) uint32 triples), sealed under dst_keys / dst_nonces; src_keys = None: plaintext sources.  Returns 0,
+        E_UNRECOVERABLE or E_AUTH (HOST mode)"""
+        kind, st = self._stream(src_shards, dst_shards)
+        n_src = len(src_len) if n_src is None else n_src
+        n_dst = len(piece_start) - 1 if n_dst is None else n_dst
+        return self._check(self._L.garage_ec_reseal(self._h, _ptr(src_shards), _ptr(src_present), _ptr(src_len),
+                                                    _ptr(src_hashes), _ptr(src_keys), n_src, _ptr(pieces),
+                                                    _ptr(piece_start), _ptr(dst_keys), _ptr(dst_nonces),
+                                                    _ptr(dst_shards), _ptr(dst_hashes), _ptr(dst_sums),
+                                                    _ptr(dst_len_out), _ptr(src_hash_bad), _ptr(src_status),
+                                                    _ptr(status), stride, n_dst, kind, st),
+                           (E_UNRECOVERABLE, E_AUTH))
+
+    def reseal_stripes(self, src_stripes, src_present, src_len, src_hashes, src_keys, pieces, piece_start, dst_keys,
+                       dst_nonces, dst_shards, dst_hashes, dst_len_out, src_hash_bad, src_status, status, stride,
+                       dst_sums=None):
+        """HOST gather form: `src_stripes` is a list of numpy arrays, one (k+m)*stride stripe per source"""
+        n = len(src_stripes)
+        sp = (C.c_void_p * max(n, 1))(*[a.ctypes.data for a in src_stripes])
+        return self._check(self._L.garage_ec_reseal_stripes(self._h, C.cast(sp, C.c_void_p), _ptr(src_present),
+                                                            _ptr(src_len), _ptr(src_hashes), _ptr(src_keys), n,
+                                                            _ptr(pieces), _ptr(piece_start), _ptr(dst_keys),
+                                                            _ptr(dst_nonces), _ptr(dst_shards), _ptr(dst_hashes),
+                                                            _ptr(dst_sums), _ptr(dst_len_out), _ptr(src_hash_bad),
+                                                            _ptr(src_status), _ptr(status), stride,
+                                                            len(piece_start) - 1),
                            (E_UNRECOVERABLE, E_AUTH))
 
     # -- harness utilities

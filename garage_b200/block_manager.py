@@ -26,7 +26,9 @@ SYMBOLS = [
     "garage_bm_debug_set_clock_ms", "garage_bm_get_resync_metrics",
     "garage_bm_rpc_put_block_sealed", "garage_bm_rpc_get_block_opened", "garage_bm_get_sealed_metrics",
     "garage_bm_rpc_get_block_range_opened", "garage_bm_get_sealed_range_metrics",
+    "garage_bm_rpc_put_block_resealed", "garage_bm_get_reseal_metrics",
 ]
+MAX_PIECES = 64
 SUM_BLAKE2, SUM_ADLER8 = 0, 1
 
 
@@ -121,6 +123,16 @@ class SealedRangeMetrics(C.Structure):
         "open_range_call_us")]
 
 
+class ResealMetrics(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in (
+        "calls", "batches", "sources_gathered", "bytes_read", "auth_failures", "fallbacks", "call_us", "reseal_call_us")]
+
+
+class Piece(C.Structure):
+    """garage_bm_piece: plaintext bytes [offset, offset + len) of stored block `hash`"""
+    _fields_ = [("hash", C.c_uint8 * 32), ("offset", C.c_uint32), ("len", C.c_uint32)]
+
+
 class ResyncError(C.Structure):
     """garage_bm_resync_error: one entry of a node's resync error table"""
     _fields_ = [("node", C.c_int32), ("hash", C.c_uint8 * 32), ("rc", C.c_longlong), ("errors", C.c_uint64),
@@ -212,6 +224,9 @@ def load_library():
         L.garage_bm_rpc_get_block_range_opened.argtypes = [vp, vp, vp, C.c_uint32, C.c_uint32, vp, sz, C.POINTER(sz)]
         L.garage_bm_get_sealed_range_metrics.argtypes = [vp, C.POINTER(SealedRangeMetrics)]
         L.garage_bm_get_sealed_range_metrics.restype = None
+        L.garage_bm_rpc_put_block_resealed.argtypes = [vp, vp, C.c_int, vp, vp, vp, C.POINTER(C.c_uint32)]
+        L.garage_bm_get_reseal_metrics.argtypes = [vp, C.POINTER(ResealMetrics)]
+        L.garage_bm_get_reseal_metrics.restype = None
         _lib = L
     return _lib
 
@@ -341,6 +356,26 @@ class BlockManager:
         mt = SealedRangeMetrics()
         self._L.garage_bm_get_sealed_range_metrics(self._h, C.byref(mt))
         return {n: getattr(mt, n) for n, _ in SealedRangeMetrics._fields_}
+
+    def put_block_resealed(self, pieces, src_key32, dst_key32):
+        """(rc, content address, stored length) of a copy with re-encryption: `pieces` is a list of (hash, offset,
+        len) plaintext ranges of stored blocks, sealed into one new block under dst_key32; src_key32 None: the sources
+        are plaintext blocks"""
+        arr = (Piece * max(1, len(pieces)))()
+        for i, (h, off, n) in enumerate(pieces):
+            arr[i].hash[:] = list(bytes(h))
+            arr[i].offset, arr[i].len = off, n
+        h = (C.c_uint8 * 32)()
+        ln = C.c_uint32(0)
+        rc = self._L.garage_bm_rpc_put_block_resealed(
+            self._h, arr, len(pieces), None if src_key32 is None else C.c_char_p(bytes(src_key32)),
+            None if dst_key32 is None else C.c_char_p(bytes(dst_key32)), h, C.byref(ln))
+        return rc, bytes(h), ln.value
+
+    def reseal_metrics(self):
+        mt = ResealMetrics()
+        self._L.garage_bm_get_reseal_metrics(self._h, C.byref(mt))
+        return {n: getattr(mt, n) for n, _ in ResealMetrics._fields_}
 
     def rpc_get_block_range(self, hash32, offset, length):
         """(rc, bytes [offset, offset + length) of the block or None)"""

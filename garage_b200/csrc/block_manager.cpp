@@ -1510,12 +1510,32 @@ struct EncodeItem {
     std::promise<int> done;
 };
 
+// A copy with re-encryption (rpc_put_block_resealed): the destination's pieces over the gathered source stripes.  The
+// dispatcher fills the outputs; `out` keeps the batch's destination shards and tags alive.
+struct ResealJob {
+    std::vector<uint8_t *> stripes;  // one per distinct source: k+m shards, slot_stride apart (ciphertext)
+    std::vector<uint8_t> present;    // k+m per source
+    std::vector<uint32_t> src_len;
+    std::vector<Hash> src_hash;
+    std::vector<garage_ec_piece> pieces;  // src: an index into `stripes`
+    const uint8_t *src_key = nullptr;     // NULL: the sources are plaintext
+    const uint8_t *dst_key = nullptr;
+    uint8_t nonce[8] = {0};
+    std::vector<uint8_t> src_bad;       // out, per source
+    std::vector<int32_t> src_status;    // out, per source
+    std::shared_ptr<std::vector<uint8_t>> out;
+    const uint8_t *shards = nullptr, *sums = nullptr;  // out: k+m shards slot_stride apart, their tags
+    Hash hash{};
+    uint32_t stored_len = 0;
+};
+
 struct ReconItem {
     // what the dispatcher does with the stripe, in the order a batch runs them: a ranged GET
     // (garage_ec_decode_range_stripes), an opened GET (garage_ec_open_stripes), a ranged opened GET
-    // (garage_ec_open_range_stripes), a whole-shard rebuild (garage_ec_reconstruct_stripes)
-    enum Kind { kRange, kOpen, kOpenRange, kRebuild };
-    static constexpr int kKinds = kRebuild + 1;
+    // (garage_ec_open_range_stripes), a whole-shard rebuild (garage_ec_reconstruct_stripes), a copy with
+    // re-encryption (garage_ec_reseal_stripes, its stripes in `reseal`)
+    enum Kind { kRange, kOpen, kOpenRange, kRebuild, kReseal };
+    static constexpr int kKinds = kReseal + 1;
     Kind kind = kRebuild;
     uint8_t *stripe = nullptr;  // pinned slot: k+m shards, slot_stride apart, survivors filled in by the caller
     uint32_t block_len = 0;     // the stored length: the sealed length for the opened kinds
@@ -1527,6 +1547,7 @@ struct ReconItem {
     const uint8_t *key = nullptr;  // the opened kinds
     Hash hash{};                   // open: the content address to check
     uint32_t plain_len = 0;        // open: set by the dispatcher
+    ResealJob *reseal = nullptr;   // reseal
     bool fulfilled = false;
     std::promise<int> done;
 };
@@ -1628,6 +1649,8 @@ struct garage_bm {
         sealed_range_call_us{0};
     std::atomic<uint64_t> sealed_puts{0}, sealed_batches{0}, opened_gets{0}, opened_auth_failures{0}, opened_fallbacks{0},
         seal_call_us{0}, open_call_us{0};
+    std::atomic<uint64_t> reseal_calls{0}, reseal_batches{0}, reseal_sources{0}, reseal_bytes_read{0},
+        reseal_auth_failures{0}, reseal_fallbacks{0}, reseal_us{0}, reseal_call_us{0};
     std::atomic<uint64_t> layout_shards_copied{0}, layout_shards_rebuilt{0}, layout_bytes_read{0}, layout_bytes_written{0},
         layout_deleted{0}, layout_sync_errors{0}, layout_bytes_fetched{0};
     std::atomic<uint64_t> stripe_repairs{0}, stripe_repair_shards{0}, stripe_repair_bytes_read{0},
@@ -2002,6 +2025,15 @@ struct garage_bm {
             }
         };
         switch (b[0]->kind) {
+        case ReconItem::kReseal: {  // keyed and plaintext sources cannot share one call
+            for (const bool keyed : {true, false}) {
+                std::vector<ReconItem *> g;
+                for (ReconItem *it : b)
+                    if ((it->reseal->src_key != nullptr) == keyed) g.push_back(it);
+                if (!g.empty()) run_reseal(w, g, keyed);
+            }
+            break;
+        }
         case ReconItem::kRebuild: {
             std::vector<uint8_t> want(n * tot);
             for (size_t i = 0; i < n; i++) {
@@ -2063,6 +2095,65 @@ struct garage_bm {
             });
             break;
         }
+        }
+    }
+
+    // The reseals of a batch: their sources back to back and their pieces renumbered, one garage_ec_reseal_stripes
+    // call; its status per destination is each item's result (any other rc is every item's).  The destination shards
+    // and tags stay in one buffer the items share.  The dispatcher's copies of the keys are wiped after the call.
+    void run_reseal(int w, std::vector<ReconItem *> &g, bool keyed)
+    {
+        const size_t n = g.size();
+        std::vector<uint8_t *> stripes;
+        std::vector<uint8_t> present, shash, skeys, dkeys(n * 32), nonces(n * 8);
+        std::vector<uint32_t> slen, start(1, 0);
+        std::vector<garage_ec_piece> pieces;
+        std::vector<size_t> base(n);
+        for (size_t i = 0; i < n; i++) {
+            const ResealJob &J = *g[i]->reseal;
+            base[i] = stripes.size();
+            for (size_t j = 0; j < J.stripes.size(); j++) {
+                stripes.push_back(J.stripes[j]);
+                slen.push_back(J.src_len[j]);
+                shash.insert(shash.end(), J.src_hash[j].begin(), J.src_hash[j].end());
+                if (keyed) skeys.insert(skeys.end(), J.src_key, J.src_key + 32);
+            }
+            present.insert(present.end(), J.present.begin(), J.present.end());
+            for (const garage_ec_piece &p : J.pieces) pieces.push_back({(uint32_t)(base[i] + p.src), p.offset, p.len});
+            start.push_back((uint32_t)pieces.size());
+            memcpy(dkeys.data() + i * 32, J.dst_key, 32);
+            memcpy(nonces.data() + i * 8, J.nonce, 8);
+        }
+        const size_t ns = stripes.size(), sh_bytes = n * tot * slot_stride;
+        auto out = std::make_shared<std::vector<uint8_t>>(sh_bytes + n * tot * 32 + n * 32);
+        uint8_t *dsh = out->data(), *dsums = dsh + sh_bytes, *dhash = dsums + n * tot * 32;
+        std::vector<uint32_t> dlen(n, 0);
+        std::vector<uint8_t> bad(ns, 0);
+        std::vector<int32_t> sst(ns, 0), st(n, 0);
+        const auto t0 = Clock::now();
+        const int rc = garage_ec_reseal_stripes(rec_ctx[w], stripes.data(), present.data(), slen.data(), shash.data(),
+                                                keyed ? skeys.data() : nullptr, ns, pieces.data(), start.data(),
+                                                dkeys.data(), nonces.data(), dsh, dhash, dsums, dlen.data(), bad.data(),
+                                                sst.data(), st.data(), slot_stride, n);
+        reseal_call_us += us_since(t0);
+        reseal_batches++;
+        wipe_secret(skeys.data(), skeys.size());
+        wipe_secret(dkeys.data(), dkeys.size());
+        const bool listed = rc == GARAGE_EC_OK || rc == GARAGE_EC_E_UNRECOVERABLE || rc == GARAGE_EC_E_AUTH;
+        for (size_t i = 0; i < n; i++) {
+            ResealJob &J = *g[i]->reseal;
+            const size_t nj = J.stripes.size();
+            J.src_bad.assign(bad.begin() + base[i], bad.begin() + base[i] + nj);
+            J.src_status.assign(sst.begin() + base[i], sst.begin() + base[i] + nj);
+            if (listed && !st[i]) {
+                J.out = out;
+                J.shards = dsh + i * tot * slot_stride;
+                J.sums = dsums + i * tot * 32;
+                memcpy(J.hash.data(), dhash + i * 32, 32);
+                J.stored_len = dlen[i];
+            }
+            g[i]->fulfilled = true;
+            g[i]->done.set_value(listed ? st[i] : rc);
         }
     }
 
@@ -2365,6 +2456,119 @@ struct garage_bm {
         const uint8_t *sh = it.shards;
         const size_t stride = it.pstride;
         return store_block(it.hash, blen, shard_len_of(blen), [&](int i) { return sh + (size_t)i * stride; }, it.sums);
+    }
+
+    // A copy with re-encryption into an SSE-C block (handle_copy_reencrypt, copy.rs:320-349; UploadPartCopy,
+    // copy.rs:506-636; DESIGN.md section 5.11).  Each distinct source is gathered once, as rpc_get_block_opened gathers,
+    // into a buffer of its own (the sources count against the RAM budget); one garage_ec_reseal_stripes call of the
+    // reconstruct dispatchers proves the sources and seals the destination.  A source that the configured stripe cannot
+    // serve (a previous code, replicas) or that does not hash to its address is read by rpc_get_block -- the stale-shard
+    // hunt quarantines the culprit -- and its stored bytes (ciphertext for keyed sources) are framed into its buffer with
+    // every data shard present; the copy is retried once.  No plaintext is in host memory on any path.  The result is
+    // stored as rpc_put_block stores a block of its sealed length; refcounts are not touched.
+    int rpc_put_block_resealed(const garage_bm_piece *in, int n_in, const uint8_t *src_key, const uint8_t *dst_key,
+                               uint8_t *hash_out, uint32_t *stored_len_out)
+    {
+        const auto t0 = Clock::now();
+        struct AddTime {
+            std::atomic<uint64_t> &c;
+            Clock::time_point t;
+            ~AddTime() { c += us_since(t); }
+        } add_time{reseal_us, t0};
+        reseal_calls++;
+        uint64_t total = 0;
+        ResealJob J;
+        std::vector<Hash> hs;
+        for (int p = 0; p < n_in; p++) {
+            if (!in[p].len) return GARAGE_EC_E_INVALID;
+            total += in[p].len;
+            const Hash h = to_hash(in[p].hash);
+            const size_t j = std::find(hs.begin(), hs.end(), h) - hs.begin();
+            if (j == hs.size()) hs.push_back(h);
+            J.pieces.push_back({(uint32_t)j, in[p].offset, in[p].len});
+        }
+        if (total > cfg.block_size) return GARAGE_EC_E_INVALID;
+        const size_t ns = hs.size(), sbytes = (size_t)tot * slot_stride;
+        ByteLease permit(*ram, (uint64_t)(ns + 1) * sbytes);  // the source buffers and the destination's shards
+        std::vector<std::unique_ptr<uint8_t[]>> bufs(ns);
+        J.stripes.resize(ns);
+        J.present.assign(ns * tot, 0);
+        J.src_len.assign(ns, 0);
+        J.src_hash = hs;
+        J.src_key = src_key;
+        J.dst_key = dst_key;
+        // the stored block through rpc_get_block, framed into the source's buffer with all data shards present
+        auto frame = [&](size_t j) -> int {
+            reseal_fallbacks++;
+            std::vector<uint8_t> blk(stored_max());
+            size_t blen = 0;
+            const int rc = rpc_get_block(hs[j], blk.data(), blk.size(), &blen);
+            if (rc != GARAGE_BM_OK) return rc;
+            reseal_bytes_read += blen;
+            const size_t L = shard_len_of((uint32_t)blen);
+            uint8_t *slot = J.stripes[j];
+            memset(&J.present[j * tot], 0, tot);
+            for (int i = 0; i < k; i++) {
+                J.present[j * tot + i] = 1;
+                uint8_t *row = slot + (size_t)i * slot_stride;
+                memset(row, 0, slot_stride);
+                const size_t off = (size_t)i * L;
+                if (off < blen) memcpy(row, blk.data() + off, std::min(L, blen - off));
+            }
+            J.src_len[j] = (uint32_t)blen;
+            return GARAGE_BM_OK;
+        };
+        for (size_t j = 0; j < ns; j++) {
+            bufs[j].reset(new (std::nothrow) uint8_t[sbytes]);
+            if (!bufs[j]) return GARAGE_EC_E_NOMEM;
+            J.stripes[j] = bufs[j].get();
+            bool ok = false;
+            uint64_t bytes = 0;
+            uint32_t bl = 0;
+            gather_into(hs[j], -1, J.stripes[j], &J.present[j * tot], bl, false, false, nullptr, &ok, &bytes);
+            reseal_sources++;
+            reseal_bytes_read += bytes;
+            J.src_len[j] = bl;
+            if (!ok) {
+                const int rc = frame(j);
+                if (rc != GARAGE_BM_OK) return rc;
+            }
+        }
+        for (const garage_ec_piece &p : J.pieces) {  // a source the framing cannot hold fails AUTH on the GPU
+            uint32_t P = J.src_len[p.src];
+            if ((!src_key || plain_len_of(P, P)) && (uint64_t)p.offset + p.len > P) return GARAGE_EC_E_INVALID;
+        }
+        for (size_t got = 0; got < sizeof(J.nonce);) {
+            const ssize_t r = getrandom(J.nonce + got, sizeof(J.nonce) - got, 0);
+            if (r < 0 && errno != EINTR) return GARAGE_BM_E_MESSAGE;
+            if (r > 0) got += (size_t)r;
+        }
+        int rc = GARAGE_BM_OK;
+        for (int attempt = 0; attempt < 2; attempt++) {
+            ReconItem it;
+            it.kind = ReconItem::kReseal;
+            it.reseal = &J;
+            rc = rec_batcher->submit(it);
+            if (rc != GARAGE_EC_E_UNRECOVERABLE || attempt) break;
+            // a source that does not hash to its address, or that its stripe cannot rebuild: once through rpc_get_block
+            bool again = false;
+            for (size_t j = 0; j < ns && j < J.src_bad.size(); j++)
+                if (J.src_bad[j] || J.src_status[j] == GARAGE_EC_E_UNRECOVERABLE) {
+                    const int r = frame(j);
+                    if (r != GARAGE_BM_OK) return r;
+                    again = true;
+                }
+            if (!again) break;
+        }
+        if (rc == GARAGE_EC_E_AUTH) reseal_auth_failures++;
+        if (rc == GARAGE_EC_E_UNRECOVERABLE) return GARAGE_BM_E_MISSING_BLOCK;
+        if (rc != GARAGE_BM_OK) return rc;
+        memcpy(hash_out, J.hash.data(), 32);
+        if (stored_len_out) *stored_len_out = J.stored_len;
+        const uint8_t *sh = J.shards;
+        const size_t stride = slot_stride;
+        return store_block(J.hash, J.stored_len, shard_len_of(J.stored_len), [&](int i) { return sh + (size_t)i * stride; },
+                           J.sums);
     }
 
     // One opened GET of the stripe in `slot` (its shards `have`, the stored length block_len) through the reconstruct
@@ -4696,6 +4900,27 @@ int garage_bm_rpc_get_block_range_opened(garage_bm *bm, const uint8_t hash[32], 
 {
     if (!bm || !hash || !key32 || !out_len || (!out && len)) return GARAGE_EC_E_INVALID;
     BM_GUARD(bm->rpc_get_block_range_opened(to_hash(hash), key32, offset, len, out, cap, out_len));
+}
+
+int garage_bm_rpc_put_block_resealed(garage_bm *bm, const garage_bm_piece *pieces, int n_pieces, const uint8_t *src_key32,
+                                     const uint8_t *dst_key32, uint8_t hash_out[32], uint32_t *stored_len_out)
+{
+    if (!bm || !pieces || !dst_key32 || !hash_out || n_pieces < 1 || n_pieces > GARAGE_BM_MAX_PIECES)
+        return GARAGE_EC_E_INVALID;
+    BM_GUARD(bm->rpc_put_block_resealed(pieces, n_pieces, src_key32, dst_key32, hash_out, stored_len_out));
+}
+
+void garage_bm_get_reseal_metrics(garage_bm *bm, garage_bm_reseal_metrics *o)
+{
+    if (!bm || !o) return;
+    o->calls = bm->reseal_calls;
+    o->batches = bm->reseal_batches;
+    o->sources_gathered = bm->reseal_sources;
+    o->bytes_read = bm->reseal_bytes_read;
+    o->auth_failures = bm->reseal_auth_failures;
+    o->fallbacks = bm->reseal_fallbacks;
+    o->call_us = bm->reseal_us;
+    o->reseal_call_us = bm->reseal_call_us;
 }
 
 void garage_bm_get_sealed_range_metrics(garage_bm *bm, garage_bm_sealed_range_metrics *o)

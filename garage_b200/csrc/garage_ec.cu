@@ -3559,6 +3559,422 @@ int garage_ec_open_range_stripes(garage_ec_ctx *ctx, const uint8_t *const *strip
                            status, n);
 }
 
+// --------------------------------------------------------------------------- SSE-C RESEAL (DESIGN.md 2.8, 4.11)
+}  // extern "C"
+namespace {
+
+static_assert(sizeof(garage_ec_piece) == 12, "garage_ec_piece is three uint32 words");
+
+// Device scratch of a reseal of n_src sources into n_dst destinations: key material (sources, then destinations) |
+// source L | reconstruct status | want | plan | destination |Q|, len(B'), L'.  The key material comes first so that
+// one memset clears every secret.
+struct ResealScratch {
+    size_t o_keys, keys_bytes, o_src_L, o_rec, o_want, o_plan, o_plen, o_blen, o_dst_L, bytes;
+    ResealScratch(const garage_ec_ctx *ctx, size_t n_src, size_t n_dst)
+    {
+        size_t b = 0;
+        auto take = [&](size_t x) {
+            const size_t o = b;
+            b += align_up(x, 256);
+            return o;
+        };
+        keys_bytes = (n_src + n_dst) * sizeof(sse::SseKey);
+        o_keys = take(keys_bytes);
+        o_src_L = take(n_src * 4);
+        o_rec = take(n_src * 4);
+        o_want = take(n_src * (size_t)(ctx->k + ctx->m));
+        o_plan = take(plan_scratch_bytes(ctx, n_src));
+        o_plen = take(n_dst * 4);
+        o_blen = take(n_dst * 4);
+        o_dst_L = take(n_dst * 4);
+        bytes = b;
+    }
+};
+
+// Reseal on the device: framing, piece lists and lengths, key schedules, the rebuild of absent source data shards,
+// the sources' content hashes and (keyed) every chunk tag, the destinations' verdicts, the fused decrypt-and-seal
+// into the destination data shards, the code's encode, the destinations' content hashes and (sums != NULL) their
+// shard tags.  The caller zeroes the key material of `scratch`.
+int run_reseal(garage_ec_ctx *ctx, uint8_t *src_shards, const uint8_t *src_present, const uint32_t *src_len,
+               const uint8_t *src_hashes, const uint8_t *src_keys, size_t n_src, const uint32_t *pieces,
+               const uint32_t *piece_start, const uint8_t *dst_keys, const uint8_t *dst_nonces, uint8_t *dst_shards,
+               uint8_t *dst_hashes, uint8_t *dst_sums, uint32_t *dst_len_out, uint8_t *src_hash_bad,
+               int32_t *src_status, int32_t *status, size_t stride, size_t n_dst, uint8_t *scratch, cudaStream_t st)
+{
+    const ResealScratch sc(ctx, n_src, n_dst);
+    const size_t tot = ctx->k + ctx->m, nmax = std::max(n_src, n_dst);
+    sse::SseKey *ks = reinterpret_cast<sse::SseKey *>(scratch + sc.o_keys);
+    uint32_t *src_L = reinterpret_cast<uint32_t *>(scratch + sc.o_src_L), *plen = reinterpret_cast<uint32_t *>(scratch + sc.o_plen),
+             *blen = reinterpret_cast<uint32_t *>(scratch + sc.o_blen), *dst_L = reinterpret_cast<uint32_t *>(scratch + sc.o_dst_L);
+    int32_t *rec = reinterpret_cast<int32_t *>(scratch + sc.o_rec);
+    const unsigned grid = (unsigned)std::min<size_t>((nmax + 255) / 256, (size_t)ctx->sm_count * 4);
+    sse::ResealLensParams lp;
+    memset(&lp, 0, sizeof(lp));
+    lp.src_len = src_len;
+    lp.pieces = pieces;
+    lp.piece_start = piece_start;
+    lp.src_status = src_status;
+    lp.src_L = src_L;
+    lp.want = scratch + sc.o_want;
+    lp.status = status;
+    lp.dst_plen = plen;
+    lp.dst_blen = blen;
+    lp.dst_L = dst_L;
+    lp.stride = (uint32_t)stride;
+    lp.k = (uint32_t)ctx->k;
+    lp.m = (uint32_t)ctx->m;
+    lp.n_src = (uint32_t)n_src;
+    lp.n_dst = (uint32_t)n_dst;
+    lp.quantum = ctx->quantum;
+    lp.keyed = src_keys ? 1u : 0u;
+    sse::sse_reseal_lens_kernel<<<grid, 256, 0, st>>>(lp);
+    ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    CU_TRY(ctx, cudaGetLastError());
+    int rc = src_keys && n_src ? sse_launch_setup(ctx, src_keys, ks, n_src, st) : GARAGE_EC_OK;
+    if (!rc) rc = sse_launch_setup(ctx, dst_keys, ks + n_src, n_dst, st);
+    if (!rc && n_src)
+        rc = run_reconstruct(ctx, src_shards, src_present, scratch + sc.o_want, rec, src_L, stride, n_src,
+                             scratch + sc.o_plan, st);
+    if (!rc && n_src) rc = sse_launch_block_sums(ctx, src_shards, src_len, src_hashes, src_hash_bad, nullptr, stride, n_src, st);
+    if (rc) return rc;
+    const uint32_t cmax = (uint32_t)std::max<size_t>(1, ((size_t)ctx->k * stride + sse::kChunk - 1) / sse::kChunk);
+    sse::ChunkParams q;
+    memset(&q, 0, sizeof(q));
+    q.stride = (uint32_t)stride;
+    q.k = (uint32_t)ctx->k;
+    q.m = (uint32_t)ctx->m;
+    q.cmax = cmax;
+    if (src_keys && n_src) {
+        q.blen = src_len;
+        q.shard_len = src_L;
+        q.ks = ks;
+        q.shards = src_shards;
+        q.status = src_status;
+        q.rec_status = rec;
+        q.n = (uint32_t)n_src;
+        rc = sse_launch_chunks<sse::kCheck>(ctx, q, st);
+        if (rc) return rc;
+    }
+    sse::ResealVerdictParams vp;
+    memset(&vp, 0, sizeof(vp));
+    vp.pieces = pieces;
+    vp.piece_start = piece_start;
+    vp.rec = rec;
+    vp.hash_bad = src_hash_bad;
+    vp.src_status = src_status;
+    vp.status = status;
+    vp.dst_blen = blen;
+    vp.dst_L = dst_L;
+    vp.dst_len_out = dst_len_out;
+    vp.n_src = (uint32_t)n_src;
+    vp.n_dst = (uint32_t)n_dst;
+    sse::sse_reseal_verdict_kernel<<<grid, 256, 0, st>>>(vp);
+    ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    CU_TRY(ctx, cudaGetLastError());
+    memset(&q, 0, sizeof(q));
+    q.plain_len = plen;
+    q.blen = blen;
+    q.shard_len = dst_L;
+    q.nonces = dst_nonces;
+    q.ks = ks + n_src;
+    q.shards = dst_shards;
+    q.stride = (uint32_t)stride;
+    q.k = (uint32_t)ctx->k;
+    q.m = (uint32_t)ctx->m;
+    q.n = (uint32_t)n_dst;
+    q.cmax = cmax;
+    q.pieces = pieces;
+    q.piece_start = piece_start;
+    q.src_shards = src_shards;
+    q.src_len = src_len;
+    q.src_L = src_L;
+    q.src_ks = src_keys ? ks : nullptr;
+    rc = sse_launch_chunks<sse::kReseal>(ctx, q, st);
+    if (!rc)
+        rc = run_uniform(ctx, kModeEncode, dst_shards, tot * stride, dst_shards + (size_t)ctx->k * stride, tot * stride,
+                         nullptr, dst_L, stride, n_dst, st);
+    if (!rc) rc = sse_launch_block_sums(ctx, dst_shards, blen, nullptr, nullptr, dst_hashes, stride, n_dst, st);
+    if (!rc && dst_sums) rc = run_sums(ctx, dst_shards, nullptr, dst_L, stride, n_dst * tot, (int)tot, dst_sums, nullptr, st);
+    return rc;
+}
+
+// The checks a HOST reseal makes before any GPU work: every source's L fits the stride and some piece names it, every
+// destination has a well-formed piece list inside its sources' plaintext, and every L' fits the stride
+int reseal_host_args_ok(garage_ec_ctx *ctx, const uint32_t *src_len, bool keyed, size_t n_src,
+                        const garage_ec_piece *pieces, const uint32_t *piece_start, size_t stride, size_t n_dst)
+{
+    for (size_t i = 0; i < n_src; i++)
+        if (code_shard_len(ctx, src_len[i]) > stride) return GARAGE_EC_E_INVALID;
+    std::vector<uint8_t> named(n_src, 0);
+    for (size_t d = 0; d < n_dst; d++) {
+        if (piece_start[d + 1] <= piece_start[d]) return GARAGE_EC_E_INVALID;
+        uint64_t Q = 0;
+        for (uint32_t p = piece_start[d]; p < piece_start[d + 1]; p++) {
+            const garage_ec_piece &x = pieces[p];
+            if (x.src >= n_src || !x.len) return GARAGE_EC_E_INVALID;
+            named[x.src] = 1;
+            const int64_t P = keyed ? sse_plain_len(src_len[x.src]) : (int64_t)src_len[x.src];
+            if (P >= 0 && (int64_t)x.offset + x.len > P) return GARAGE_EC_E_INVALID;  // P < 0: the source fails AUTH
+            Q += x.len;
+        }
+        const uint64_t B = sse::sealed_len(Q);
+        if (B > 0xffffffffull || code_shard_len(ctx, (uint32_t)B) > stride) return GARAGE_EC_E_INVALID;
+    }
+    for (size_t i = 0; i < n_src; i++)
+        if (!named[i]) return GARAGE_EC_E_INVALID;  // a chunk uploads only the sources its pieces name
+    return GARAGE_EC_OK;
+}
+
+// HOST reseal.  src_stripes != NULL: the gather form.  The pipeline chunks the destinations; a chunk uploads the
+// distinct sources its pieces name (a source two chunks name is uploaded and proven by both), renumbers their pieces,
+// and uploads only what garage_ec_open would upload of each: ciphertext.  Only roundup16(L') bytes of the k+m shards of the destinations that passed come down.
+int reseal_host(garage_ec_ctx *ctx, const uint8_t *src_shards, const uint8_t *const *src_stripes,
+                const uint8_t *src_present, const uint32_t *src_len, const uint8_t *src_hashes, const uint8_t *src_keys,
+                size_t n_src, const garage_ec_piece *pieces, const uint32_t *piece_start, const uint8_t *dst_keys,
+                const uint8_t *dst_nonces, uint8_t *dst_shards, uint8_t *dst_hashes, uint8_t *dst_sums,
+                uint32_t *dst_len_out, uint8_t *src_hash_bad, int32_t *src_status, int32_t *status, size_t stride,
+                size_t n_dst)
+{
+    const size_t k = ctx->k, tot = ctx->k + ctx->m;
+    auto shard_at = [&](size_t i, size_t j) {
+        return src_stripes ? src_stripes[i] + j * stride : src_shards + (i * tot + j) * stride;
+    };
+    // per destination: its own shards and those of the most distinct sources one destination names, so that a
+    // chunk's sources and destinations fit the pipeline's chunk budget (or one destination's worth when that is more)
+    std::vector<size_t> last(n_src, SIZE_MAX);
+    size_t per_dst = 1;
+    for (size_t d = 0; d < n_dst; d++) {
+        size_t cnt = 0;
+        for (uint32_t x = piece_start[d]; x < piece_start[d + 1]; x++)
+            if (last[pieces[x].src] != d) {
+                last[pieces[x].src] = d;
+                cnt++;
+            }
+        per_dst = std::max(per_dst, cnt);
+    }
+    LaneKeyWipe wipe;  // outlives p: p's destructor runs wipe.wipe()
+    HostPipeline p(ctx, n_dst, (1 + per_dst) * tot * stride);
+    const size_t cs = p.cs, nch = (n_dst + cs - 1) / cs;
+    std::vector<std::vector<uint32_t>> srcs(nch);
+    last.assign(n_src, SIZE_MAX);
+    size_t max_src = 1, max_pieces = 1;
+    for (size_t c = 0; c < nch; c++) {
+        const size_t d0 = c * cs, d1 = std::min(n_dst, d0 + cs);
+        for (uint32_t x = piece_start[d0]; x < piece_start[d1]; x++)
+            if (last[pieces[x].src] != c) {
+                last[pieces[x].src] = c;
+                srcs[c].push_back(pieces[x].src);
+            }
+        max_pieces = std::max<size_t>(max_pieces, piece_start[d1] - piece_start[d0]);
+    }
+    for (const auto &v : srcs) max_src = std::max(max_src, v.size());
+    std::vector<uint32_t> local(n_src);
+    std::vector<uint8_t> want(tot);
+    for (size_t j = 0; j < tot; j++) want[j] = j < k;
+
+    p.before_release = [&wipe] { wipe.wipe(); };
+    SmallLayout sl;
+    const ResealScratch sc(ctx, max_src, cs);
+    // device small buffer: scratch | keys and nonces | the uploaded tables | the downloaded verdicts | hashes | sums;
+    // the lane's pageable staging mirrors [o_present, o_dhash)
+    const size_t o_scr = sl.take(sc.bytes), o_key = sl.take(max_src * 32 + cs * 40), o_present = sl.take(max_src * tot),
+                 o_slen = sl.take(max_src * 4), o_shash = sl.take(max_src * 32), o_pieces = sl.take(max_pieces * 12),
+                 o_pstart = sl.take((cs + 1) * 4), o_sbad = sl.take(max_src), o_sstatus = sl.take(max_src * 4),
+                 o_dlen = sl.take(cs * 4), o_status = sl.take(cs * 4), o_dhash = sl.take(cs * 32),
+                 o_dsums = sl.take(dst_sums ? cs * tot * 32 : 0);
+    wipe.dev_off = o_scr;
+    wipe.dev_bytes = o_present - o_scr;
+    const size_t src_b = align_up(max_src * tot * stride, 256);
+    int rc = p.reserve(src_b + cs * tot * stride, sl.bytes, o_dhash - o_present);
+    if (rc) return rc;
+    bool pinned = true;
+    for (size_t i = 0; pinned && i < (src_stripes ? n_src : 1); i++) pinned = device_addressable_host(shard_at(i, 0));
+    p.up.use_batch = pinned;
+    p.down.use_batch = device_addressable_host(dst_shards);
+    auto at = [](const HostChunk &ch, size_t o, size_t base) { return ch.host + (o - base); };
+    const Retire retire = [&](const HostChunk &ch) -> int {
+        memset(ch.L->h_key, 0, ch.L->h_key_cap);
+        const std::vector<uint32_t> &S = srcs[ch.s0 / cs];
+        const uint8_t *sbad = at(ch, o_sbad, o_present);
+        const int32_t *sst = reinterpret_cast<const int32_t *>(at(ch, o_sstatus, o_present)),
+                      *dst = reinterpret_cast<const int32_t *>(at(ch, o_status, o_present));
+        const uint32_t *dlen = reinterpret_cast<const uint32_t *>(at(ch, o_dlen, o_present));
+        for (size_t li = 0; li < S.size(); li++) {
+            src_hash_bad[S[li]] = sbad[li];
+            src_status[S[li]] = sst[li];
+        }
+        const uint8_t *d_dst = ch.L->d_buf + src_b;
+        for (size_t q = 0; q < ch.cnt; q++) {
+            const size_t d = ch.s0 + q;
+            status[d] = dst[q];
+            if (dst[q]) continue;
+            dst_len_out[d] = dlen[q];
+            const size_t bytes = align_up(code_shard_len(ctx, dlen[q]), 16);
+            for (size_t j = 0; j < tot; j++) p.down.add(dst_shards + (d * tot + j) * stride, d_dst + (q * tot + j) * stride, bytes);
+        }
+        int r = p.down.flush(ctx, cudaMemcpyDeviceToHost, ch.L->stream);
+        if (r) return r;
+        CU_TRY(ctx, lane_wait(ctx, *ch.L));
+        return GARAGE_EC_OK;
+    };
+    rc = p.run(
+        [&](const HostChunk &ch) -> int {
+            HostLane &L = *ch.L;
+            wipe.use(&L);
+            const size_t s0 = ch.s0, cnt = ch.cnt;
+            const std::vector<uint32_t> &S = srcs[s0 / cs];
+            uint8_t *d_src = L.d_buf, *d_dst = L.d_buf + src_b;
+            int r = lane_key_staging(ctx, L, max_src * 32 + cs * 40);
+            if (r) return r;
+            uint8_t *h_present = at(ch, o_present, o_present), *h_shash = at(ch, o_shash, o_present);
+            uint32_t *h_slen = reinterpret_cast<uint32_t *>(at(ch, o_slen, o_present)),
+                     *h_pieces = reinterpret_cast<uint32_t *>(at(ch, o_pieces, o_present)),
+                     *h_pstart = reinterpret_cast<uint32_t *>(at(ch, o_pstart, o_present));
+            // H2D: the present data shards of each source and what the code's plan reads to rebuild the others
+            for (size_t li = 0; li < S.size(); li++) {
+                const size_t i = S[li];
+                local[i] = (uint32_t)li;
+                const uint8_t *pr = src_present + i * tot;
+                memcpy(h_present + li * tot, pr, tot);
+                h_slen[li] = src_len[i];
+                memcpy(h_shash + li * 32, src_hashes + i * 32, 32);
+                if (src_keys) memcpy(L.h_key + li * 32, src_keys + i * 32, 32);
+                uint64_t hv = 0;
+                const size_t len = code_shard_len(ctx, src_len[i]);
+                const bool ok = stripe_read_plan(ctx, pr, want.data(), &hv);
+                for (size_t j = 0; j < tot; j++) {
+                    uint8_t *dp = d_src + (li * tot + j) * stride;
+                    if (j < k && pr[j]) p.up.add(dp, shard_at(i, j), align_up(len, 16));
+                    else if (ok && j >= k)
+                        for_each_read_piece(ctx, hv, j, len, align_up(len, 16),
+                                            [&](size_t off, size_t bytes) { p.up.add(dp + off, shard_at(i, j) + off, bytes); });
+                }
+            }
+            const uint32_t pbase = piece_start[s0];
+            for (size_t q = 0; q <= cnt; q++) h_pstart[q] = piece_start[s0 + q] - pbase;
+            for (uint32_t x = pbase; x < piece_start[s0 + cnt]; x++) {
+                h_pieces[3 * (x - pbase)] = local[pieces[x].src];
+                h_pieces[3 * (x - pbase) + 1] = pieces[x].offset;
+                h_pieces[3 * (x - pbase) + 2] = pieces[x].len;
+            }
+            memcpy(L.h_key + max_src * 32, dst_keys + s0 * 32, cnt * 32);
+            memcpy(L.h_key + max_src * 32 + cs * 32, dst_nonces + s0 * 8, cnt * 8);
+            r = p.up.flush(ctx, cudaMemcpyHostToDevice, L.stream);
+            if (r) return r;
+            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_key, L.h_key, max_src * 32 + cs * 40, cudaMemcpyHostToDevice, L.stream));
+            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_present, ch.host, o_sbad - o_present, cudaMemcpyHostToDevice, L.stream));
+            auto u32 = [&](size_t o) { return reinterpret_cast<uint32_t *>(L.d_small + o); };
+            r = run_reseal(ctx, d_src, L.d_small + o_present, u32(o_slen), L.d_small + o_shash,
+                           src_keys ? L.d_small + o_key : nullptr, S.size(), u32(o_pieces), u32(o_pstart),
+                           L.d_small + o_key + max_src * 32, L.d_small + o_key + max_src * 32 + cs * 32, d_dst,
+                           L.d_small + o_dhash, dst_sums ? L.d_small + o_dsums : nullptr, u32(o_dlen), L.d_small + o_sbad,
+                           reinterpret_cast<int32_t *>(u32(o_sstatus)), reinterpret_cast<int32_t *>(u32(o_status)), stride,
+                           cnt, L.d_small + o_scr, L.stream);
+            if (r) return r;
+            CU_TRY(ctx, cudaMemsetAsync(L.d_small + o_scr, 0, wipe.dev_bytes, L.stream));
+            CU_TRY(ctx, cudaMemcpyAsync(at(ch, o_sbad, o_present), L.d_small + o_sbad, o_dhash - o_sbad,
+                                        cudaMemcpyDeviceToHost, L.stream));
+            CU_TRY(ctx, cudaMemcpyAsync(dst_hashes + s0 * 32, L.d_small + o_dhash, cnt * 32, cudaMemcpyDeviceToHost, L.stream));
+            if (dst_sums)
+                CU_TRY(ctx, cudaMemcpyAsync(dst_sums + s0 * tot * 32, L.d_small + o_dsums, cnt * tot * 32,
+                                            cudaMemcpyDeviceToHost, L.stream));
+            return GARAGE_EC_OK;
+        },
+        retire);
+    if (!rc) rc = p.drain(retire);
+    wipe.failed = rc != 0;
+    if (rc) return rc;
+    int worst = GARAGE_EC_OK;
+    for (size_t d = 0; d < n_dst; d++) {
+        if (status[d] == GARAGE_EC_E_UNRECOVERABLE) return GARAGE_EC_E_UNRECOVERABLE;
+        if (status[d]) worst = status[d];
+    }
+    return worst;
+}
+
+int reseal_args(garage_ec_ctx *ctx, const void *src_shards, const uint8_t *src_present, const uint32_t *src_len,
+                const uint8_t *src_hashes, size_t n_src, const garage_ec_piece *pieces, const uint32_t *piece_start,
+                const uint8_t *dst_keys, const uint8_t *dst_nonces, const uint8_t *dst_shards, const uint8_t *dst_hashes,
+                const uint32_t *dst_len_out, const uint8_t *src_hash_bad, const int32_t *src_status,
+                const int32_t *status, size_t stride, size_t n_dst)
+{
+    if (!ctx) return GARAGE_EC_E_INVALID;
+    int rc = check_geometry(ctx, stride, std::max(n_src, n_dst), ctx->k + ctx->m);
+    if (rc) return rc;
+    if (n_dst == 0) return GARAGE_EC_OK;
+    if (!piece_start || !pieces || !dst_keys || !dst_nonces || !dst_shards || !dst_hashes || !dst_len_out || !status)
+        return GARAGE_EC_E_INVALID;
+    if (n_src && (!src_shards || !src_present || !src_len || !src_hashes || !src_hash_bad || !src_status))
+        return GARAGE_EC_E_INVALID;
+    if (!aligned16(dst_shards)) return GARAGE_EC_E_ALIGN;
+    return GARAGE_EC_OK;
+}
+
+}  // namespace
+extern "C" {
+
+int garage_ec_reseal(garage_ec_ctx *ctx, uint8_t *src_shards, const uint8_t *src_present, const uint32_t *src_len,
+                     const uint8_t *src_hashes, const uint8_t *src_keys, size_t n_src, const garage_ec_piece *pieces,
+                     const uint32_t *piece_start, const uint8_t *dst_keys, const uint8_t *dst_nonces,
+                     uint8_t *dst_shards, uint8_t *dst_hashes, uint8_t *dst_sums, uint32_t *dst_len_out,
+                     uint8_t *src_hash_bad, int32_t *src_status, int32_t *status, size_t stride, size_t n_dst,
+                     int mem_kind, void *cuda_stream)
+{
+    if (mem_kind != GARAGE_EC_MEM_HOST && mem_kind != GARAGE_EC_MEM_DEVICE) return GARAGE_EC_E_INVALID;
+    int rc = reseal_args(ctx, src_shards, src_present, src_len, src_hashes, n_src, pieces, piece_start, dst_keys,
+                         dst_nonces, dst_shards, dst_hashes, dst_len_out, src_hash_bad, src_status, status, stride, n_dst);
+    if (rc || n_dst == 0) return rc;
+    if (n_src && !aligned16(src_shards)) return GARAGE_EC_E_ALIGN;
+    if (mem_kind == GARAGE_EC_MEM_HOST) {
+        rc = reseal_host_args_ok(ctx, src_len, src_keys != nullptr, n_src, pieces, piece_start, stride, n_dst);
+        if (rc) return rc;
+        CU_TRY(ctx, cudaSetDevice(ctx->device));
+        return reseal_host(ctx, src_shards, nullptr, src_present, src_len, src_hashes, src_keys, n_src, pieces,
+                           piece_start, dst_keys, dst_nonces, dst_shards, dst_hashes, dst_sums, dst_len_out,
+                           src_hash_bad, src_status, status, stride, n_dst);
+    }
+    for (const void *p : {(const void *)src_len, (const void *)pieces, (const void *)piece_start, (const void *)dst_len_out,
+                          (const void *)src_status, (const void *)status})
+        if (reinterpret_cast<uintptr_t>(p) & 3) return GARAGE_EC_E_ALIGN;
+    if ((reinterpret_cast<uintptr_t>(src_hashes) & 7) || (reinterpret_cast<uintptr_t>(dst_hashes) & 7) ||
+        (reinterpret_cast<uintptr_t>(dst_sums) & 7))
+        return GARAGE_EC_E_ALIGN;
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    const ResealScratch sc(ctx, n_src, n_dst);
+    return with_stream_scratch(ctx, sc.bytes, st, [&](uint8_t *scratch) {
+        const int r = run_reseal(ctx, src_shards, src_present, src_len, src_hashes, src_keys, n_src,
+                                 reinterpret_cast<const uint32_t *>(pieces), piece_start, dst_keys, dst_nonces, dst_shards,
+                                 dst_hashes, dst_sums, dst_len_out, src_hash_bad, src_status, status, stride, n_dst,
+                                 scratch, st);
+        const cudaError_t e = cudaMemsetAsync(scratch + sc.o_keys, 0, sc.keys_bytes, st);
+        if (r) return r;
+        return e == cudaSuccess ? GARAGE_EC_OK : set_cuda_error(ctx, e, "cudaMemsetAsync(key material)");
+    });
+}
+
+int garage_ec_reseal_stripes(garage_ec_ctx *ctx, uint8_t *const *src_stripes, const uint8_t *src_present,
+                             const uint32_t *src_len, const uint8_t *src_hashes, const uint8_t *src_keys, size_t n_src,
+                             const garage_ec_piece *pieces, const uint32_t *piece_start, const uint8_t *dst_keys,
+                             const uint8_t *dst_nonces, uint8_t *dst_shards, uint8_t *dst_hashes, uint8_t *dst_sums,
+                             uint32_t *dst_len_out, uint8_t *src_hash_bad, int32_t *src_status, int32_t *status,
+                             size_t stride, size_t n_dst)
+{
+    int rc = reseal_args(ctx, src_stripes, src_present, src_len, src_hashes, n_src, pieces, piece_start, dst_keys,
+                         dst_nonces, dst_shards, dst_hashes, dst_len_out, src_hash_bad, src_status, status, stride, n_dst);
+    if (rc || n_dst == 0) return rc;
+    for (size_t i = 0; i < n_src; i++) {
+        if (!src_stripes[i]) return GARAGE_EC_E_INVALID;
+        if (!aligned16(src_stripes[i])) return GARAGE_EC_E_ALIGN;
+    }
+    rc = reseal_host_args_ok(ctx, src_len, src_keys != nullptr, n_src, pieces, piece_start, stride, n_dst);
+    if (rc) return rc;
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    return reseal_host(ctx, nullptr, src_stripes, src_present, src_len, src_hashes, src_keys, n_src, pieces, piece_start,
+                       dst_keys, dst_nonces, dst_shards, dst_hashes, dst_sums, dst_len_out, src_hash_bad, src_status,
+                       status, stride, n_dst);
+}
+
 // ---- test hook -------------------------------------------------------------------------------
 int garage_ec_debug_fail_after(garage_ec_ctx *ctx, long n_calls)
 {

@@ -287,7 +287,9 @@ __global__ void __launch_bounds__(256) sse_setup_kernel(const __grid_constant__ 
 // kRangeCheck / kRangeOpen: ranged opens (DESIGN.md 4.10).  Request s reads its nonce prefix from row 2s of `rows`
 // and chunks c0 .. c1 of its range, back to back from a 16-byte boundary, from row 2s + 1; the open writes only the
 // plaintext bytes [offset, offset + len) to plain_out + s*plain_stride, zero up to roundup16(len).
-enum { kSeal = 0, kCheck = 1, kOpen = 2, kRangeCheck = 3, kRangeOpen = 4 };
+// kReseal: copies with re-encryption (DESIGN.md 4.11).  Work item (d, c) is chunk c of destination d: the warp
+// decrypts the source CTR blocks its pieces cover straight into the stage, then seals the stage in place as kSeal does.
+enum { kSeal = 0, kCheck = 1, kOpen = 2, kRangeCheck = 3, kRangeOpen = 4, kReseal = 5 };
 
 struct ChunkParams {
     const uint8_t *plain_in;        // seal: block s at plain_in + s*plain_stride
@@ -309,6 +311,13 @@ struct ChunkParams {
     uint32_t stride, k, m, n;
     uint32_t cmax;                  // chunks per block this launch covers (work item = block * cmax + chunk; ranged:
                                     // + chunk - c0)
+    // reseal: block s is destination s (plain_len = |Q_s|, blen its sealed length, shard_len 0 = not proven, ks its
+    // key), made of pieces [piece_start[s], piece_start[s + 1]) = {src, offset, len} words of the sources
+    const uint32_t *pieces, *piece_start;
+    const uint8_t *src_shards;      // source i at src_shards + i*(k+m)*stride
+    const uint32_t *src_len;        // stored length S_i
+    const uint32_t *src_L;          // its L
+    const SseKey *src_ks;           // nullable: the sources are plaintext
 };
 
 struct ChunkSmem {
@@ -317,6 +326,45 @@ struct ChunkSmem {
     uint32_t rk[kWarps][60];
     unsigned long long hh[kWarps][16], hl[kWarps][16];
 };
+
+// kReseal: plaintext bytes [x0, x1) of source i into to[0, x1 - x0), lanes splitting its 16-byte blocks.  Block g of a
+// keyed source is decrypted from its ciphertext at B position 8 + 4112 (g / 256) + 16 (g mod 256), counter block
+// N_i || LE32(c | last << 31) || BE32(g mod 256 + 2); an unkeyed source's block is B[16g, 16g + 16).  The source's
+// round keys are read from its key material in global memory, so the mode needs no shared memory of its own.
+__device__ __forceinline__ void reseal_piece(const ChunkParams &q, const SseTables &t, uint8_t *to, uint32_t i,
+                                             uint32_t x0, uint32_t x1, uint32_t lane)
+{
+    const uint32_t S = q.src_len[i], L = q.src_L[i];
+    const uint8_t *stripe = q.src_shards + (size_t)i * (q.k + q.m) * q.stride;
+    const SseKey *K = q.src_ks ? q.src_ks + i : nullptr;
+    uint32_t P = S, nch = 1, nw0 = 0, nw1 = 0;
+    if (K) {  // framing checked by sse_reseal_lens_kernel
+        nch = (S - kPrefix + kFrame - 1) / kFrame;
+        P = S - kPrefix - 16 * nch;
+        uint8_t nb8[8];
+#pragma unroll
+        for (int b = 0; b < 8; b++) nb8[b] = stripe[(size_t)(b / L) * q.stride + b % L];
+        nw0 = ((uint32_t)nb8[0] << 24) | ((uint32_t)nb8[1] << 16) | ((uint32_t)nb8[2] << 8) | nb8[3];
+        nw1 = ((uint32_t)nb8[4] << 24) | ((uint32_t)nb8[5] << 16) | ((uint32_t)nb8[6] << 8) | nb8[7];
+    }
+    const uint32_t g1 = (x1 + 15) / 16;
+    for (uint32_t g = x0 / 16 + lane; g < g1; g += 32) {
+        const uint32_t c = g >> 8, pos = K ? kPrefix + kFrame * c + 16 * (g & 255) : 16 * g, j = pos / L;
+        const uint4 v = block_vec16(stripe, q.stride, L, j, pos - j * L, min(16u, P - 16 * g));
+        unsigned long long a = ((unsigned long long)v.y << 32) | v.x, b = ((unsigned long long)v.w << 32) | v.z;
+        if (K) {
+            uint32_t k0 = nw0, k1 = nw1, k2 = bswap32(c | (c == nch - 1 ? 0x80000000u : 0u)), k3 = (g & 255) + 2;
+            aes256_encrypt(t, K->rk, k0, k1, k2, k3);
+            a ^= bswap64(((unsigned long long)k0 << 32) | k1);
+            b ^= bswap64(((unsigned long long)k2 << 32) | k3);
+        }
+        const uint32_t lo = max(16 * g, x0), hi = min(16 * g + 16, x1);
+        for (uint32_t x = lo; x < hi; x++) {
+            const uint32_t o = x - 16 * g;
+            to[x - x0] = (uint8_t)(o < 8 ? a >> (8 * o) : b >> (8 * (o - 8)));
+        }
+    }
+}
 
 template <int MODE>
 __global__ void __launch_bounds__(kWarps * 32) sse_chunk_kernel(const __grid_constant__ ChunkParams q)
@@ -331,6 +379,7 @@ __global__ void __launch_bounds__(kWarps * 32) sse_chunk_kernel(const __grid_con
          w += (unsigned long long)gridDim.x * kWarps) {
         constexpr bool ranged = MODE == kRangeCheck || MODE == kRangeOpen;
         constexpr bool checking = MODE == kCheck || MODE == kRangeCheck;
+        constexpr bool sealing = MODE == kSeal || MODE == kReseal;
         const uint32_t s = (uint32_t)(w / q.cmax), ci = (uint32_t)(w - (unsigned long long)s * q.cmax);
         const uint32_t L = ranged ? 0u : q.shard_len[s];
         if (!ranged && !L) continue;
@@ -338,7 +387,7 @@ __global__ void __launch_bounds__(kWarps * 32) sse_chunk_kernel(const __grid_con
         const uint32_t blen = q.blen[s];
         const uint32_t prefix = keyed ? kPrefix : 0, pitch = keyed ? kFrame : kChunk;
         uint32_t plen, nch, c = ci, off = 0, len = 0, c1 = 0;
-        if (MODE == kSeal) {
+        if (sealing) {
             plen = q.plain_len[s];
         } else {
             const int32_t rs = ranged ? (q.rec_status[2 * s] ? q.rec_status[2 * s] : q.rec_status[2 * s + 1])
@@ -376,7 +425,7 @@ __global__ void __launch_bounds__(kWarps * 32) sse_chunk_kernel(const __grid_con
         }
         uint32_t nw0 = 0, nw1 = 0;  // the nonce prefix, big-endian words
         if (keyed) {
-            if (MODE == kSeal) {
+            if (sealing) {
                 const uint8_t *np = q.nonces + (size_t)s * 8;
                 nw0 = ((uint32_t)np[0] << 24) | ((uint32_t)np[1] << 16) | ((uint32_t)np[2] << 8) | np[3];
                 nw1 = ((uint32_t)np[4] << 24) | ((uint32_t)np[5] << 16) | ((uint32_t)np[6] << 8) | np[7];
@@ -400,6 +449,37 @@ __global__ void __launch_bounds__(kWarps * 32) sse_chunk_kernel(const __grid_con
                 const uint4 d = *reinterpret_cast<const uint4 *>(src + v);
                 *reinterpret_cast<unsigned long long *>(st + kPrefix + v) = ((unsigned long long)d.y << 32) | d.x;
                 *reinterpret_cast<unsigned long long *>(st + kPrefix + v + 8) = ((unsigned long long)d.w << 32) | d.z;
+            }
+        } else if (MODE == kReseal) {
+            // destination bytes [X0, X1) of Q_s: the pieces' destination offsets are an exclusive scan of their
+            // lengths, formed 32 pieces at a time; every piece that overlaps the chunk is decrypted by the whole warp
+            const uint32_t X0 = kChunk * c, X1 = X0 + clen, p1 = q.piece_start[s + 1];
+            uint32_t run = 0;
+            for (uint32_t pb = q.piece_start[s]; pb < p1 && run < X1; pb += 32) {
+                const uint32_t p = pb + lane;
+                uint32_t src = 0, po = 0, pl = 0;
+                if (p < p1) {
+                    src = q.pieces[3 * (size_t)p];
+                    po = q.pieces[3 * (size_t)p + 1];
+                    pl = q.pieces[3 * (size_t)p + 2];
+                }
+                uint32_t incl = pl;
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) {
+                    const uint32_t v = __shfl_up_sync(0xffffffffu, incl, o);
+                    if (lane >= (uint32_t)o) incl += v;
+                }
+                const uint32_t at = run + incl - pl;
+                uint32_t hit = __ballot_sync(0xffffffffu, pl && at < X1 && at + pl > X0);
+                run += __shfl_sync(0xffffffffu, incl, 31);
+                while (hit) {
+                    const int l = __ffs(hit) - 1;
+                    hit &= hit - 1;
+                    const uint32_t hs = __shfl_sync(0xffffffffu, src, l), ho = __shfl_sync(0xffffffffu, po, l),
+                                   hl = __shfl_sync(0xffffffffu, pl, l), ha = __shfl_sync(0xffffffffu, at, l);
+                    const uint32_t a = max(X0, ha), e = min(X1, ha + hl);
+                    reseal_piece(q, sm.t, st + kPrefix + (a - X0), hs, ho + a - ha, ho + e - ha, lane);
+                }
             }
         } else if (MODE != kSeal) {
             // load this chunk's ciphertext and tag, B[base + 8, base + 8 + clen + 16), into stage[8..]
@@ -460,7 +540,7 @@ __global__ void __launch_bounds__(kWarps * 32) sse_chunk_kernel(const __grid_con
                     const unsigned long long ma = valid >= 8 ? ~0ull : ((1ull << (8 * valid)) - 1),
                                              mb = valid >= 16 ? ~0ull : valid <= 8 ? 0ull : ((1ull << (8 * (valid - 8))) - 1);
                     const unsigned long long oa = (pa ^ ksa) & ma, ob = (pb ^ ksb) & mb;
-                    if (MODE == kSeal || MODE == kRangeOpen) {
+                    if (sealing || MODE == kRangeOpen) {
                         *reinterpret_cast<unsigned long long *>(st + kPrefix + 16 * b) = oa;
                         *reinterpret_cast<unsigned long long *>(st + kPrefix + 16 * b + 8) = ob;
                         if (MODE == kRangeOpen) continue;
@@ -503,7 +583,7 @@ __global__ void __launch_bounds__(kWarps * 32) sse_chunk_kernel(const __grid_con
                 const unsigned long long th = yh ^ (((unsigned long long)j0 << 32) | j1),
                                          tl = yl ^ (((unsigned long long)j2 << 32) | j3);
                 uint8_t *tp = st + kPrefix + clen;
-                if (MODE == kSeal) {
+                if (sealing) {
 #pragma unroll
                     for (int i = 0; i < 8; i++) {
                         tp[i] = (uint8_t)(th >> (56 - 8 * i));
@@ -544,7 +624,7 @@ __global__ void __launch_bounds__(kWarps * 32) sse_chunk_kernel(const __grid_con
             }
         }
 
-        if (MODE == kSeal) {
+        if (sealing) {
             __syncwarp();
             // store this chunk's part of B: [start, end) -- chunk 0 from 0 (the nonce), the last chunk to k*L (the
             // zero tail); bytes past L of a shard, up to roundup16(L), are zero and belong to the chunk that owns
@@ -642,6 +722,104 @@ __global__ void __launch_bounds__(256) sse_range_lens_kernel(const __grid_consta
         q.len2[2 * s + 1] = go ? sl : 0u;
         for (uint32_t i = 0; i < tot; i++)
             q.present2[(2 * (size_t)s) * tot + i] = q.present2[(2 * (size_t)s + 1) * tot + i] = q.present[(size_t)s * tot + i];
+    }
+}
+
+// ---- reseal: source framing, piece lists and destination lengths (DESIGN.md 4.11) ---------------------------------
+// plaintext length of a source stored as S bytes, or ~0u when a keyed S cannot be framed (no piece is checked then:
+// the source fails with GARAGE_EC_E_AUTH)
+__device__ __forceinline__ uint32_t reseal_src_plain(uint32_t S, bool keyed)
+{
+    if (!keyed) return S;
+    const uint32_t r = (S - kPrefix) % kFrame;
+    if (S < kPrefix + 16 || (r >= 1 && r < 16)) return ~0u;
+    return S - kPrefix - 16 * ((S - kPrefix + kFrame - 1) / kFrame);
+}
+
+struct ResealLensParams {
+    const uint32_t *src_len, *pieces, *piece_start;
+    int32_t *src_status;        // out: 0 / GARAGE_EC_E_AUTH (framing) / GARAGE_EC_E_INVALID (L past stride)
+    uint32_t *src_L;            // out: L, 0 for a source that is not read
+    uint8_t *want;              // out: n_src*(k+m), the data shards
+    int32_t *status;            // out: 0 / GARAGE_EC_E_INVALID (piece list, L' past stride)
+    uint32_t *dst_plen, *dst_blen, *dst_L;  // out: |Q_d|, sealed_len(|Q_d|), L' (0 when invalid)
+    uint32_t stride, k, m, n_src, n_dst, quantum, keyed;
+};
+__global__ void __launch_bounds__(256) sse_reseal_lens_kernel(const __grid_constant__ ResealLensParams q)
+{
+    const uint32_t tot = q.k + q.m;
+    for (uint32_t x = blockIdx.x * blockDim.x + threadIdx.x; x < max(q.n_src, q.n_dst); x += gridDim.x * blockDim.x) {
+        if (x < q.n_src) {
+            const uint32_t S = q.src_len[x];
+            const uint64_t L = code_shard_len(S, (int)q.k, q.quantum);
+            const bool bad = L > q.stride;
+            q.src_status[x] = bad ? -1 : reseal_src_plain(S, q.keyed) == ~0u ? -7 : 0;
+            q.src_L[x] = bad ? 0u : (uint32_t)L;
+            for (uint32_t i = 0; i < tot; i++) q.want[(size_t)x * tot + i] = i < q.k;
+        }
+        if (x < q.n_dst) {
+            const uint32_t p0 = q.piece_start[x], p1 = q.piece_start[x + 1];
+            bool ok = p1 > p0;
+            uint64_t Q = 0;
+            for (uint32_t p = p0; ok && p < p1; p++) {
+                const uint32_t src = q.pieces[3 * (size_t)p], off = q.pieces[3 * (size_t)p + 1],
+                               len = q.pieces[3 * (size_t)p + 2];
+                ok = src < q.n_src && len > 0;
+                if (ok) {
+                    const uint32_t P = reseal_src_plain(q.src_len[src], q.keyed);
+                    ok = P == ~0u || (uint64_t)off + len <= P;
+                }
+                Q += len;
+            }
+            const uint64_t B = sealed_len(Q);
+            const uint64_t L = ok && B <= 0xffffffffull ? code_shard_len((uint32_t)B, (int)q.k, q.quantum) : ~0ull;
+            ok = ok && L <= q.stride;
+            q.status[x] = ok ? 0 : -1;
+            q.dst_plen[x] = ok ? (uint32_t)Q : 0u;
+            q.dst_blen[x] = ok ? (uint32_t)B : 0u;
+            q.dst_L[x] = ok ? (uint32_t)L : 0u;
+        }
+    }
+}
+
+// A destination is resealed only if every source it names is proven: status[d] becomes GARAGE_EC_E_UNRECOVERABLE if
+// one is unrecoverable or does not hash to its address, else GARAGE_EC_E_AUTH, else GARAGE_EC_E_INVALID (its own
+// lens verdict or a named source's geometry).  A destination that fails gets L' = len(B') = 0, so that no later
+// kernel writes its shards; one that passes gets dst_len_out.  Sources: the reconstruct's verdict joins src_status.
+struct ResealVerdictParams {
+    const uint32_t *pieces, *piece_start;
+    const int32_t *rec;           // n_src: the reconstruct's status
+    const uint8_t *hash_bad;
+    int32_t *src_status, *status;
+    uint32_t *dst_blen, *dst_L, *dst_len_out;
+    uint32_t n_src, n_dst;
+};
+__device__ __forceinline__ int32_t reseal_src_verdict(const ResealVerdictParams &q, uint32_t i)
+{
+    const int32_t st = q.rec[i] ? q.rec[i] : q.src_status[i];
+    return st == -1 ? -1 : q.hash_bad[i] ? -4 /* GARAGE_EC_E_UNRECOVERABLE */ : st;
+}
+__global__ void __launch_bounds__(256) sse_reseal_verdict_kernel(const __grid_constant__ ResealVerdictParams q)
+{
+    for (uint32_t x = blockIdx.x * blockDim.x + threadIdx.x; x < max(q.n_src, q.n_dst); x += gridDim.x * blockDim.x) {
+        if (x < q.n_src && q.rec[x]) q.src_status[x] = q.rec[x];
+        if (x >= q.n_dst) continue;
+        bool unrec = false, auth = false, inval = q.status[x] != 0;
+        for (uint32_t p = q.piece_start[x]; p < q.piece_start[x + 1]; p++) {
+            const uint32_t i = q.pieces[3 * (size_t)p];
+            if (i >= q.n_src) continue;  // the lens verdict already says GARAGE_EC_E_INVALID
+            const int32_t v = reseal_src_verdict(q, i);
+            unrec |= v == -4;
+            auth |= v == -7;
+            inval |= v == -1;
+        }
+        const int32_t st = unrec ? -4 : auth ? -7 : inval ? -1 : 0;
+        q.status[x] = st;
+        if (st) {
+            q.dst_blen[x] = q.dst_L[x] = 0;
+        } else {
+            q.dst_len_out[x] = q.dst_blen[x];
+        }
     }
 }
 

@@ -239,6 +239,18 @@ typedef struct garage_bm_sealed_range_metrics {
     uint64_t call_us;            /* wall time inside garage_bm_rpc_get_block_range_opened                           */
     uint64_t open_range_call_us; /* wall time inside garage_ec_open_range_stripes                                   */
 } garage_bm_sealed_range_metrics;
+/* Counters of garage_bm_rpc_put_block_resealed (DESIGN.md section 5.11), in a struct of their own for the same
+ * reason. */
+typedef struct garage_bm_reseal_metrics {
+    uint64_t calls;            /* garage_bm_rpc_put_block_resealed calls                                            */
+    uint64_t batches;          /* garage_ec_reseal_stripes calls of the reconstruct dispatchers                    */
+    uint64_t sources_gathered; /* source blocks gathered from their stripes                                        */
+    uint64_t bytes_read;       /* shard bytes those gathers and the fallbacks read                                 */
+    uint64_t auth_failures;    /* calls that ended in GARAGE_EC_E_AUTH                                              */
+    uint64_t fallbacks;        /* sources read through garage_bm_rpc_get_block (stale shard, previous code, replica) */
+    uint64_t call_us;          /* wall time inside garage_bm_rpc_put_block_resealed                                 */
+    uint64_t reseal_call_us;   /* wall time inside garage_ec_reseal_stripes                                         */
+} garage_bm_reseal_metrics;
 
 /* One entry of a node's resync error table (Garage's BlockResyncErrorInfo, manager.rs:429-449).                    */
 typedef struct garage_bm_resync_error {
@@ -329,6 +341,29 @@ void garage_bm_get_sealed_metrics(garage_bm *bm, garage_bm_sealed_metrics *out);
 int garage_bm_rpc_get_block_range_opened(garage_bm *bm, const uint8_t hash[32], const uint8_t *key32, uint32_t offset,
                                          uint32_t len, uint8_t *out, size_t cap, size_t *out_len);
 void garage_bm_get_sealed_range_metrics(garage_bm *bm, garage_bm_sealed_range_metrics *out);
+
+/* Copy with re-encryption into an SSE-C block (handle_copy_reencrypt, src/api/s3/copy.rs:320-349, through save_stream's
+ * block loop; UploadPartCopy, copy.rs:506-636, one call per Defragmenter output; DESIGN.md sections 2.8 and 5.11): the
+ * destination block is the plaintext pieces[0..n_pieces) -- bytes [offset, offset + len) of the plaintext of stored
+ * block `hash` -- concatenated and sealed under dst_key32 and a fresh nonce prefix from getrandom(2).  src_key32: the
+ * key every source is sealed under, or NULL: the sources are plaintext blocks.  Each distinct source is gathered once,
+ * as garage_bm_rpc_get_block_opened gathers it, and proven whole (content hash, every chunk tag); a batch of copies
+ * is one garage_ec_reseal_stripes call of the reconstruct dispatchers.  No plaintext is in host memory on any path.  A
+ * source that does not hash to its address or that only a previous code or a replica holds is read by
+ * garage_bm_rpc_get_block (stale-shard hunt included) and the copy is retried once.  The result is stored exactly as
+ * garage_bm_rpc_put_block stores a block of its sealed length; refcounts are not touched.  hash_out = its content
+ * address, *stored_len_out (nullable) = its sealed length.  GARAGE_EC_E_INVALID for NULL dst_key32, n_pieces outside
+ * 1..GARAGE_BM_MAX_PIECES, an empty piece, a total length over block_size or a piece past its source's plaintext;
+ * GARAGE_EC_E_AUTH if a source fails a tag or its framing (nothing is stored); GARAGE_BM_E_MISSING_BLOCK as
+ * garage_bm_rpc_get_block.                                                                                         */
+#define GARAGE_BM_MAX_PIECES 64
+typedef struct garage_bm_piece {
+    uint8_t hash[32];
+    uint32_t offset, len;
+} garage_bm_piece;
+int garage_bm_rpc_put_block_resealed(garage_bm *bm, const garage_bm_piece *pieces, int n_pieces, const uint8_t *src_key32,
+                                     const uint8_t *dst_key32, uint8_t hash_out[32], uint32_t *stored_len_out);
+void garage_bm_get_reseal_metrics(garage_bm *bm, garage_bm_reseal_metrics *out);
 
 /* Bytes [offset, offset + len) of a block (body_from_blocks_range, src/api/s3/get.rs:650-743; the source range of
  * UploadPartCopy, src/api/s3/copy.rs:396-469), reading only the shards and columns garage_ec_range_plan names, each as

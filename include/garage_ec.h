@@ -476,6 +476,53 @@ int garage_ec_open_range_stripes(garage_ec_ctx *ctx, const uint8_t *const *strip
                                  const uint32_t *sealed_len, const uint8_t *keys, const uint32_t *offset,
                                  const uint32_t *len, size_t stride, uint8_t *const *outs, int32_t *status, size_t n);
 
+/* ---- SSE-C RESEAL -- call sites: CopyObject with re-encryption (handle_copy_reencrypt, src/api/s3/copy.rs:320-349,
+ * through save_stream's block loop) and UploadPartCopy with an encrypted source or destination (copy.rs:506-636, one
+ * call per Defragmenter output) when the destination is SSE-C: stored source blocks are opened and their plaintext,
+ * cut into pieces, is sealed into new blocks under new keys, without the plaintext ever leaving the chunk kernel's
+ * registers and shared memory (DESIGN.md section 2.8 is normative).
+ *
+ * Sources: n_src stored blocks (shard layout, present: n_src*(k+m) bytes, src_len = the stored length S_i, src_hashes
+ * the content addresses).  src_keys: 32 bytes per source, or NULL: every source is Garage Plaintext (P_i = B_i).
+ * Destinations: destination d is the pieces [piece_start[d], piece_start[d+1]) of `pieces` (piece_start has n_dst + 1
+ * entries); piece {src, offset, len} is plaintext bytes P_src[offset, offset + len), and Q_d is the concatenation of
+ * d's pieces.  B'_d = the seal (garage_ec_seal) of Q_d under dst_keys[32 d] and dst_nonces[8 d]; both are required.
+ *
+ * Every source is proven whole as garage_ec_open proves a block: absent data shards rebuilt by the code's own plan,
+ * src_hash_bad[i] = blake2sum(B_i) != src_hashes[i], every chunk tag of a keyed source checked; src_status[i] = 0,
+ * GARAGE_EC_E_UNRECOVERABLE, GARAGE_EC_E_AUTH (a tag or the framing), or (DEVICE) GARAGE_EC_E_INVALID (L past stride).
+ * Destination d is written only if every source it names has status 0 and hash_bad 0: dst_shards gets exactly the
+ * context's encode of B'_d (nothing past roundup16(L') of a shard), dst_hashes[32 d] = blake2sum(B'_d), dst_sums
+ * (nullable) its shard tags and dst_len_out[d] = len(B'_d).  Otherwise no byte of its shards is written, its hash and
+ * tags are unspecified, and status[d] = GARAGE_EC_E_UNRECOVERABLE if a named source is unrecoverable or does not hash
+ * to its address, else GARAGE_EC_E_AUTH, else (DEVICE) GARAGE_EC_E_INVALID for an empty piece list, an empty piece, a
+ * piece past its source's plaintext or an L' past `stride`.  n_dst == 0 does nothing.
+ *   DEVICE: all pointers device memory; shards 16-byte aligned, src_len / pieces / piece_start / dst_len_out / the
+ *           status arrays 4-byte, hashes and sums 8-byte aligned.  Absent source data shards are OVERWRITTEN with their
+ *           rebuilt bytes.  Only kernels and stream-ordered scratch are enqueued (capturable in a CUDA graph).
+ *   HOST:   synchronous.  GARAGE_EC_E_INVALID before any GPU work for a bad piece list, a source no piece names, a
+ *           piece past its source's plaintext, or an L or L' past `stride`.  Destinations are staged in chunks; each uploads only the source
+ *           bytes garage_ec_open would upload for the sources its pieces name (ciphertext: no plaintext crosses PCIe)
+ *           and downloads roundup16(L') bytes of the k+m shards of its destinations that passed.  Returns
+ *           GARAGE_EC_E_UNRECOVERABLE if any destination was, else GARAGE_EC_E_AUTH if any failed authentication.
+ * Key schedules and the library's copies of keys are zeroed as for garage_ec_open.  garage_ec_reseal_stripes is the
+ * HOST gather form: source stripe i at src_stripes[i] (its k+m shards `stride` apart).                              */
+typedef struct garage_ec_piece {
+    uint32_t src, offset, len;
+} garage_ec_piece;
+int garage_ec_reseal(garage_ec_ctx *ctx, uint8_t *src_shards, const uint8_t *src_present, const uint32_t *src_len,
+                     const uint8_t *src_hashes, const uint8_t *src_keys, size_t n_src, const garage_ec_piece *pieces,
+                     const uint32_t *piece_start, const uint8_t *dst_keys, const uint8_t *dst_nonces,
+                     uint8_t *dst_shards, uint8_t *dst_hashes, uint8_t *dst_sums, uint32_t *dst_len_out,
+                     uint8_t *src_hash_bad, int32_t *src_status, int32_t *status, size_t stride, size_t n_dst,
+                     int mem_kind, void *cuda_stream);
+int garage_ec_reseal_stripes(garage_ec_ctx *ctx, uint8_t *const *src_stripes, const uint8_t *src_present,
+                             const uint32_t *src_len, const uint8_t *src_hashes, const uint8_t *src_keys, size_t n_src,
+                             const garage_ec_piece *pieces, const uint32_t *piece_start, const uint8_t *dst_keys,
+                             const uint8_t *dst_nonces, uint8_t *dst_shards, uint8_t *dst_hashes, uint8_t *dst_sums,
+                             uint32_t *dst_len_out, uint8_t *src_hash_bad, int32_t *src_status, int32_t *status,
+                             size_t stride, size_t n_dst);
+
 /* ---- utilities used by the harness ------------------------------------------------------
  * device-side synthetic data (same splitmix64 counter stream as the oracle's
  * generator): fills dst[0..len) (device) with stream bytes at `offset`

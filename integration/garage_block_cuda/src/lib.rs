@@ -196,5 +196,30 @@ impl ErasureCoder {
         if rc != sys::GARAGE_EC_E_AUTH && rc != sys::GARAGE_EC_E_UNRECOVERABLE { check(self.ctx, rc)?; }
         Ok(status.iter().map(|&st| if st != 0 { Err(st) } else { Ok(()) }).collect())
     }
+
+    /// Copy with re-encryption (handle_copy_reencrypt, UploadPartCopy) into SSE-C destinations: destination d is the
+    /// plaintext pieces[piece_start[d]..piece_start[d + 1]] of the sources, sealed under dst_keys[d] / dst_nonces[d]
+    /// into `shards_out` (the shard layout, n_dst * (k+m) * stride bytes).  src_keys = None: plaintext sources.  Per
+    /// destination: Ok((content hash, stored length)) or its status (GARAGE_EC_E_AUTH, GARAGE_EC_E_UNRECOVERABLE).
+    pub fn reseal_stripes(&self, stripes: &[*mut u8], present: &[u8], src_len: &[u32], src_hashes: &[[u8; 32]],
+                          src_keys: Option<&[[u8; 32]]>, pieces: &[sys::garage_ec_piece], piece_start: &[u32],
+                          dst_keys: &[[u8; 32]], dst_nonces: &[[u8; 8]], shards_out: &mut [u8], stride: usize)
+                          -> Result<Vec<Result<([u8; 32], u32), i32>>, Error> {
+        let (n_src, n_dst) = (stripes.len(), dst_keys.len());
+        assert!(present.len() == n_src * (self.k + self.m) && src_len.len() == n_src && src_hashes.len() == n_src
+                && piece_start.len() == n_dst + 1 && dst_nonces.len() == n_dst
+                && shards_out.len() >= n_dst * (self.k + self.m) * stride);
+        assert!(piece_start[n_dst] as usize <= pieces.len());
+        let kp = match src_keys { Some(k) => { assert!(k.len() == n_src); k.as_ptr() as *const u8 } None => std::ptr::null() };
+        let (mut hashes, mut lens) = (vec![[0u8; 32]; n_dst], vec![0u32; n_dst]);
+        let (mut bad, mut src_status, mut status) = (vec![0u8; n_src], vec![0i32; n_src], vec![0i32; n_dst]);
+        let rc = unsafe { sys::garage_ec_reseal_stripes(self.ctx, stripes.as_ptr(), present.as_ptr(), src_len.as_ptr(),
+                          src_hashes.as_ptr() as *const u8, kp, n_src, pieces.as_ptr(), piece_start.as_ptr(),
+                          dst_keys.as_ptr() as *const u8, dst_nonces.as_ptr() as *const u8, shards_out.as_mut_ptr(),
+                          hashes.as_mut_ptr() as *mut u8, std::ptr::null_mut(), lens.as_mut_ptr(), bad.as_mut_ptr(),
+                          src_status.as_mut_ptr(), status.as_mut_ptr(), stride, n_dst) };
+        if rc != sys::GARAGE_EC_E_AUTH && rc != sys::GARAGE_EC_E_UNRECOVERABLE { check(self.ctx, rc)?; }
+        Ok((0..n_dst).map(|d| if status[d] != 0 { Err(status[d]) } else { Ok((hashes[d], lens[d])) }).collect())
+    }
 }
 impl Drop for ErasureCoder { fn drop(&mut self) { unsafe { sys::garage_ec_destroy(self.ctx) } } }

@@ -6,6 +6,7 @@ use std::os::raw::{c_char, c_int, c_void};
 
 #[repr(C)] pub struct garage_ec_ctx { _private: [u8; 0] }
 #[repr(C)] pub struct garage_ec_range { pub shard: u32, pub offset: u32, pub len: u32 }
+#[repr(C)] pub struct garage_ec_piece { pub src: u32, pub offset: u32, pub len: u32 }
 
 pub const GARAGE_EC_OK: c_int = 0;
 pub const GARAGE_EC_E_INVALID: c_int = -1;
@@ -90,6 +91,18 @@ extern "C" {
     pub fn garage_ec_open_range_stripes(ctx: *mut garage_ec_ctx, stripes: *const *const u8, present: *const u8,
                                         sealed_len: *const u32, keys: *const u8, offset: *const u32, len: *const u32,
                                         stride: usize, outs: *const *mut u8, status: *mut i32, n: usize) -> c_int;
+    pub fn garage_ec_reseal(ctx: *mut garage_ec_ctx, src_shards: *mut u8, src_present: *const u8, src_len: *const u32,
+                            src_hashes: *const u8, src_keys: *const u8, n_src: usize, pieces: *const garage_ec_piece,
+                            piece_start: *const u32, dst_keys: *const u8, dst_nonces: *const u8, dst_shards: *mut u8,
+                            dst_hashes: *mut u8, dst_sums: *mut u8, dst_len_out: *mut u32, src_hash_bad: *mut u8,
+                            src_status: *mut i32, status: *mut i32, stride: usize, n_dst: usize, mem_kind: c_int,
+                            stream: *mut c_void) -> c_int;
+    pub fn garage_ec_reseal_stripes(ctx: *mut garage_ec_ctx, src_stripes: *const *mut u8, src_present: *const u8,
+                                    src_len: *const u32, src_hashes: *const u8, src_keys: *const u8, n_src: usize,
+                                    pieces: *const garage_ec_piece, piece_start: *const u32, dst_keys: *const u8,
+                                    dst_nonces: *const u8, dst_shards: *mut u8, dst_hashes: *mut u8, dst_sums: *mut u8,
+                                    dst_len_out: *mut u32, src_hash_bad: *mut u8, src_status: *mut i32,
+                                    status: *mut i32, stride: usize, n_dst: usize) -> c_int;
     pub fn garage_ec_strerror(code: c_int) -> *const c_char;
     pub fn garage_ec_last_error(ctx: *const garage_ec_ctx) -> *const c_char;
     pub fn garage_ec_abi_version() -> c_int;
