@@ -46,6 +46,8 @@ ABI_SYMBOLS = [
     "garage_ec_sealed_len", "garage_ec_seal", "garage_ec_seal_blocks", "garage_ec_open", "garage_ec_open_stripes",
     "garage_ec_sealed_range", "garage_ec_open_range_plan", "garage_ec_open_range", "garage_ec_open_range_stripes",
     "garage_ec_reseal", "garage_ec_reseal_stripes",
+    "garage_ec_seal_crc", "garage_ec_seal_blocks_crc", "garage_ec_reseal_crc", "garage_ec_reseal_stripes_crc",
+    "garage_ec_crc_combine",
 ]
 
 
@@ -151,8 +153,28 @@ def load_library(build=True):
     L.garage_ec_open_range_stripes.argtypes = [vp, vp, vp, vp, vp, vp, vp, sz, vp, vp, sz]
     L.garage_ec_reseal.argtypes = [vp, vp, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, sz, i32, vp]
     L.garage_ec_reseal_stripes.argtypes = [vp, vp, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, sz]
+    L.garage_ec_seal_crc.argtypes = [vp, vp, sz, vp, vp, vp, vp, sz, vp, vp, vp, vp, sz, i32, vp]
+    L.garage_ec_seal_blocks_crc.argtypes = [vp, vp, vp, vp, vp, vp, sz, vp, vp, vp, vp, sz]
+    L.garage_ec_reseal_crc.argtypes = [vp, vp, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, sz,
+                                       sz, i32, vp]
+    L.garage_ec_reseal_stripes_crc.argtypes = [vp, vp, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp,
+                                               vp, sz, sz]
+    L.garage_ec_crc_combine.argtypes = [i32, u32, u32, u64, C.POINTER(u32)]
     _lib = L
     return L
+
+
+# S3 checksum kinds of the _crc seal and reseal forms (DESIGN.md 2.9)
+CRC_NONE, CRC32, CRC32C = 0, 1, 2
+
+
+def crc_combine(kind, crc_a, crc_b, len_b) -> int:
+    """garage_ec_crc_combine (host only): the CRC of A || B from CRC(A), CRC(B) and len(B)"""
+    v = C.c_uint32(0)
+    rc = load_library().garage_ec_crc_combine(kind, crc_a, crc_b, len_b, C.byref(v))
+    if rc:
+        raise EcError(rc, "crc_combine")
+    return v.value
 
 
 def sealed_len(plain_len) -> int:
@@ -516,21 +538,24 @@ class GarageEc:
                            (E_UNRECOVERABLE,))
 
     # -- SSE-C (AES-256-GCM STREAM chunks, DESIGN.md 2.6)
-    def seal(self, plain, plain_stride, plain_len, keys, nonces, shards, stride, hashes, sums=None, n=None):
-        """garage_ec_seal of n = len(plain_len) blocks; keys = nonces = None stores them as plaintext"""
+    def seal(self, plain, plain_stride, plain_len, keys, nonces, shards, stride, hashes, sums=None, n=None,
+             crc_kind=None, crcs=None):
+        """garage_ec_seal of n = len(plain_len) blocks; keys = nonces = None stores them as plaintext.  crc_kind (one
+        uint8 CRC_* per block) and crcs (uint32 per block): also the plaintext checksums (garage_ec_seal_crc)"""
         kind, st = self._stream(plain, shards)
         n = len(plain_len) if n is None else n
-        return self._check(self._L.garage_ec_seal(self._h, _ptr(plain), plain_stride, _ptr(plain_len), _ptr(keys),
-                                                  _ptr(nonces), _ptr(shards), stride, _ptr(hashes), _ptr(sums), n,
-                                                  kind, st))
+        return self._check(self._L.garage_ec_seal_crc(self._h, _ptr(plain), plain_stride, _ptr(plain_len), _ptr(keys),
+                                                      _ptr(nonces), _ptr(shards), stride, _ptr(hashes), _ptr(sums),
+                                                      _ptr(crc_kind), _ptr(crcs), n, kind, st))
 
-    def seal_blocks(self, blocks, keys, nonces, shards, stride, hashes, sums=None):
+    def seal_blocks(self, blocks, keys, nonces, shards, stride, hashes, sums=None, crc_kind=None, crcs=None):
         """HOST gather form: `blocks` is a list of 1-D uint8 numpy arrays"""
         n = len(blocks)
         ptrs = (C.c_void_p * n)(*[b.ctypes.data if b.size else None for b in blocks])
         lens = np.array([b.size for b in blocks], dtype=np.uint32)
-        return self._check(self._L.garage_ec_seal_blocks(self._h, C.cast(ptrs, C.c_void_p), _ptr(lens), _ptr(keys),
-                                                         _ptr(nonces), _ptr(shards), stride, _ptr(hashes), _ptr(sums), n))
+        return self._check(self._L.garage_ec_seal_blocks_crc(self._h, C.cast(ptrs, C.c_void_p), _ptr(lens), _ptr(keys),
+                                                             _ptr(nonces), _ptr(shards), stride, _ptr(hashes),
+                                                             _ptr(sums), _ptr(crc_kind), _ptr(crcs), n))
 
     def open(self, shards, present, sealed_len, hashes, keys, plain, plain_stride, plain_len_out, hash_bad, status,
              stride, n=None):
@@ -600,34 +625,36 @@ class GarageEc:
     # -- SSE-C copies with re-encryption (DESIGN.md 2.8)
     def reseal(self, src_shards, src_present, src_len, src_hashes, src_keys, pieces, piece_start, dst_keys, dst_nonces,
                dst_shards, dst_hashes, dst_len_out, src_hash_bad, src_status, status, stride, dst_sums=None,
-               n_src=None, n_dst=None):
+               n_src=None, n_dst=None, crc_kind=None, crcs=None):
         """garage_ec_reseal: destination d = the pieces [piece_start[d], piece_start[d+1]) of `pieces` ((src, offset,
-        len) uint32 triples), sealed under dst_keys / dst_nonces; src_keys = None: plaintext sources.  Returns 0,
-        E_UNRECOVERABLE or E_AUTH (HOST mode)"""
+        len) uint32 triples), sealed under dst_keys / dst_nonces; src_keys = None: plaintext sources.  crc_kind / crcs
+        per destination: also the checksums of their plaintext (garage_ec_reseal_crc).  Returns 0, E_UNRECOVERABLE or
+        E_AUTH (HOST mode)"""
         kind, st = self._stream(src_shards, dst_shards)
         n_src = len(src_len) if n_src is None else n_src
         n_dst = len(piece_start) - 1 if n_dst is None else n_dst
-        return self._check(self._L.garage_ec_reseal(self._h, _ptr(src_shards), _ptr(src_present), _ptr(src_len),
-                                                    _ptr(src_hashes), _ptr(src_keys), n_src, _ptr(pieces),
-                                                    _ptr(piece_start), _ptr(dst_keys), _ptr(dst_nonces),
-                                                    _ptr(dst_shards), _ptr(dst_hashes), _ptr(dst_sums),
-                                                    _ptr(dst_len_out), _ptr(src_hash_bad), _ptr(src_status),
-                                                    _ptr(status), stride, n_dst, kind, st),
+        return self._check(self._L.garage_ec_reseal_crc(self._h, _ptr(src_shards), _ptr(src_present), _ptr(src_len),
+                                                        _ptr(src_hashes), _ptr(src_keys), n_src, _ptr(pieces),
+                                                        _ptr(piece_start), _ptr(dst_keys), _ptr(dst_nonces),
+                                                        _ptr(dst_shards), _ptr(dst_hashes), _ptr(dst_sums),
+                                                        _ptr(dst_len_out), _ptr(src_hash_bad), _ptr(src_status),
+                                                        _ptr(status), _ptr(crc_kind), _ptr(crcs), stride, n_dst, kind,
+                                                        st),
                            (E_UNRECOVERABLE, E_AUTH))
 
     def reseal_stripes(self, src_stripes, src_present, src_len, src_hashes, src_keys, pieces, piece_start, dst_keys,
                        dst_nonces, dst_shards, dst_hashes, dst_len_out, src_hash_bad, src_status, status, stride,
-                       dst_sums=None):
+                       dst_sums=None, crc_kind=None, crcs=None):
         """HOST gather form: `src_stripes` is a list of numpy arrays, one (k+m)*stride stripe per source"""
         n = len(src_stripes)
         sp = (C.c_void_p * max(n, 1))(*[a.ctypes.data for a in src_stripes])
-        return self._check(self._L.garage_ec_reseal_stripes(self._h, C.cast(sp, C.c_void_p), _ptr(src_present),
-                                                            _ptr(src_len), _ptr(src_hashes), _ptr(src_keys), n,
-                                                            _ptr(pieces), _ptr(piece_start), _ptr(dst_keys),
-                                                            _ptr(dst_nonces), _ptr(dst_shards), _ptr(dst_hashes),
-                                                            _ptr(dst_sums), _ptr(dst_len_out), _ptr(src_hash_bad),
-                                                            _ptr(src_status), _ptr(status), stride,
-                                                            len(piece_start) - 1),
+        return self._check(self._L.garage_ec_reseal_stripes_crc(self._h, C.cast(sp, C.c_void_p), _ptr(src_present),
+                                                                _ptr(src_len), _ptr(src_hashes), _ptr(src_keys), n,
+                                                                _ptr(pieces), _ptr(piece_start), _ptr(dst_keys),
+                                                                _ptr(dst_nonces), _ptr(dst_shards), _ptr(dst_hashes),
+                                                                _ptr(dst_sums), _ptr(dst_len_out), _ptr(src_hash_bad),
+                                                                _ptr(src_status), _ptr(status), _ptr(crc_kind),
+                                                                _ptr(crcs), stride, len(piece_start) - 1),
                            (E_UNRECOVERABLE, E_AUTH))
 
     # -- harness utilities

@@ -27,8 +27,10 @@ SYMBOLS = [
     "garage_bm_rpc_put_block_sealed", "garage_bm_rpc_get_block_opened", "garage_bm_get_sealed_metrics",
     "garage_bm_rpc_get_block_range_opened", "garage_bm_get_sealed_range_metrics",
     "garage_bm_rpc_put_block_resealed", "garage_bm_get_reseal_metrics",
+    "garage_bm_rpc_put_block_sealed_crc", "garage_bm_rpc_put_block_resealed_crc",
 ]
 MAX_PIECES = 64
+CRC_NONE, CRC32, CRC32C = 0, 1, 2  # checksum kinds of the _crc writes (DESIGN.md 2.9)
 SUM_BLAKE2, SUM_ADLER8 = 0, 1
 
 
@@ -227,6 +229,9 @@ def load_library():
         L.garage_bm_rpc_put_block_resealed.argtypes = [vp, vp, C.c_int, vp, vp, vp, C.POINTER(C.c_uint32)]
         L.garage_bm_get_reseal_metrics.argtypes = [vp, C.POINTER(ResealMetrics)]
         L.garage_bm_get_reseal_metrics.restype = None
+        L.garage_bm_rpc_put_block_sealed_crc.argtypes = [vp, vp, vp, sz, C.c_uint8, vp, C.POINTER(C.c_uint32)]
+        L.garage_bm_rpc_put_block_resealed_crc.argtypes = [vp, vp, C.c_int, vp, vp, C.c_uint8, vp,
+                                                           C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
         _lib = L
     return _lib
 
@@ -331,6 +336,17 @@ class BlockManager:
                                                     C.c_void_p(a.ctypes.data) if a.size else None, a.size, h)
         return rc, bytes(h)
 
+    def rpc_put_block_sealed_crc(self, key32, data, crc_kind):
+        """(rc, content address, CRC) of an SSE-C PUT that also returns the S3 checksum of kind crc_kind (CRC_*) of
+        the plaintext"""
+        a = np.ascontiguousarray(data, dtype=np.uint8)
+        h = (C.c_uint8 * 32)()
+        crc = C.c_uint32(0)
+        rc = self._L.garage_bm_rpc_put_block_sealed_crc(self._h, None if key32 is None else C.c_char_p(bytes(key32)),
+                                                        C.c_void_p(a.ctypes.data) if a.size else None, a.size,
+                                                        crc_kind, h, C.byref(crc))
+        return rc, bytes(h), crc.value
+
     def rpc_get_block_opened(self, hash32, key32, cap=1 << 20):
         """(rc, plaintext or None) of an SSE-C GET"""
         out = np.empty(max(cap, 1), dtype=np.uint8)
@@ -371,6 +387,20 @@ class BlockManager:
             self._h, arr, len(pieces), None if src_key32 is None else C.c_char_p(bytes(src_key32)),
             None if dst_key32 is None else C.c_char_p(bytes(dst_key32)), h, C.byref(ln))
         return rc, bytes(h), ln.value
+
+    def put_block_resealed_crc(self, pieces, src_key32, dst_key32, crc_kind):
+        """put_block_resealed that also returns the S3 checksum of kind crc_kind (CRC_*) of the new block's plaintext:
+        (rc, content address, stored length, CRC)"""
+        arr = (Piece * max(1, len(pieces)))()
+        for i, (h, off, n) in enumerate(pieces):
+            arr[i].hash[:] = list(bytes(h))
+            arr[i].offset, arr[i].len = off, n
+        h = (C.c_uint8 * 32)()
+        ln, crc = C.c_uint32(0), C.c_uint32(0)
+        rc = self._L.garage_bm_rpc_put_block_resealed_crc(
+            self._h, arr, len(pieces), None if src_key32 is None else C.c_char_p(bytes(src_key32)),
+            None if dst_key32 is None else C.c_char_p(bytes(dst_key32)), crc_kind, h, C.byref(ln), C.byref(crc))
+        return rc, bytes(h), ln.value, crc.value
 
     def reseal_metrics(self):
         mt = ResealMetrics()

@@ -1503,6 +1503,8 @@ struct EncodeItem {
     bool sealed = false;
     const uint8_t *key = nullptr;
     uint8_t nonce[8] = {0};
+    uint8_t crc_kind = GARAGE_EC_CRC_NONE;  // the S3 checksum of the plaintext to compute (DESIGN.md 2.9); out: crc
+    uint32_t crc = 0;
     std::shared_ptr<std::vector<uint8_t>> sealed_out;
     const uint8_t *shards = nullptr;
     Hash hash{};
@@ -1521,6 +1523,8 @@ struct ResealJob {
     const uint8_t *src_key = nullptr;     // NULL: the sources are plaintext
     const uint8_t *dst_key = nullptr;
     uint8_t nonce[8] = {0};
+    uint8_t crc_kind = GARAGE_EC_CRC_NONE;  // the S3 checksum of the destination's plaintext; out: crc
+    uint32_t crc = 0;
     std::vector<uint8_t> src_bad;       // out, per source
     std::vector<int32_t> src_status;    // out, per source
     std::shared_ptr<std::vector<uint8_t>> out;
@@ -1896,17 +1900,19 @@ struct garage_bm {
         while (n--) *v++ = 0;
     }
 
-    // the sealed PUTs of a batch, keyed or stored as plaintext: one garage_ec_seal_blocks call
+    // the sealed PUTs of a batch, keyed or stored as plaintext: one garage_ec_seal_blocks_crc call, each block with
+    // its own checksum kind
     void run_seal(int w, std::vector<EncodeItem *> &b, bool keyed)
     {
         const size_t n = b.size();
         uint32_t max_len = 0;
         std::vector<const uint8_t *> ptrs(n);
-        std::vector<uint32_t> lens(n);
-        std::vector<uint8_t> keys(keyed ? n * 32 : 0), nonces(keyed ? n * 8 : 0);
+        std::vector<uint32_t> lens(n), crcs(n, 0);
+        std::vector<uint8_t> keys(keyed ? n * 32 : 0), nonces(keyed ? n * 8 : 0), kinds(n);
         for (size_t i = 0; i < n; i++) {
             ptrs[i] = b[i]->data;
             lens[i] = b[i]->len;
+            kinds[i] = b[i]->crc_kind;
             max_len = std::max(max_len, b[i]->len);
             if (keyed) {
                 memcpy(keys.data() + i * 32, b[i]->key, 32);
@@ -1927,8 +1933,9 @@ struct garage_bm {
                 *sums = hashes ? hashes + n * 32 : nullptr;
         const auto t0 = Clock::now();
         if (rc == GARAGE_EC_OK)
-            rc = garage_ec_seal_blocks(enc_ctx[w], ptrs.data(), lens.data(), keyed ? keys.data() : nullptr,
-                                       keyed ? nonces.data() : nullptr, sh, stride, hashes, sums, n);
+            rc = garage_ec_seal_blocks_crc(enc_ctx[w], ptrs.data(), lens.data(), keyed ? keys.data() : nullptr,
+                                           keyed ? nonces.data() : nullptr, sh, stride, hashes, sums, kinds.data(),
+                                           crcs.data(), n);
         seal_call_us += us_since(t0);
         sealed_batches++;
         if (keyed) wipe_secret(keys.data(), keys.size());
@@ -1938,6 +1945,7 @@ struct garage_bm {
                 b[i]->shards = sh + i * tot * stride;
                 b[i]->pstride = stride;
                 b[i]->sums = sums + i * tot * 32;
+                b[i]->crc = crcs[i];
                 memcpy(b[i]->hash.data(), hashes + i * 32, 32);
             }
             b[i]->fulfilled = true;
@@ -2098,15 +2106,16 @@ struct garage_bm {
         }
     }
 
-    // The reseals of a batch: their sources back to back and their pieces renumbered, one garage_ec_reseal_stripes
-    // call; its status per destination is each item's result (any other rc is every item's).  The destination shards
-    // and tags stay in one buffer the items share.  The dispatcher's copies of the keys are wiped after the call.
+    // The reseals of a batch: their sources back to back and their pieces renumbered, one
+    // garage_ec_reseal_stripes_crc call with each destination's checksum kind; its status per destination is each
+    // item's result (any other rc is every item's).  The destination shards and tags stay in one buffer the items share.
+    // The dispatcher's copies of the keys are wiped after the call.
     void run_reseal(int w, std::vector<ReconItem *> &g, bool keyed)
     {
         const size_t n = g.size();
         std::vector<uint8_t *> stripes;
-        std::vector<uint8_t> present, shash, skeys, dkeys(n * 32), nonces(n * 8);
-        std::vector<uint32_t> slen, start(1, 0);
+        std::vector<uint8_t> present, shash, skeys, dkeys(n * 32), nonces(n * 8), kinds(n);
+        std::vector<uint32_t> slen, start(1, 0), crcs(n, 0);
         std::vector<garage_ec_piece> pieces;
         std::vector<size_t> base(n);
         for (size_t i = 0; i < n; i++) {
@@ -2123,6 +2132,7 @@ struct garage_bm {
             start.push_back((uint32_t)pieces.size());
             memcpy(dkeys.data() + i * 32, J.dst_key, 32);
             memcpy(nonces.data() + i * 8, J.nonce, 8);
+            kinds[i] = J.crc_kind;
         }
         const size_t ns = stripes.size(), sh_bytes = n * tot * slot_stride;
         auto out = std::make_shared<std::vector<uint8_t>>(sh_bytes + n * tot * 32 + n * 32);
@@ -2131,10 +2141,11 @@ struct garage_bm {
         std::vector<uint8_t> bad(ns, 0);
         std::vector<int32_t> sst(ns, 0), st(n, 0);
         const auto t0 = Clock::now();
-        const int rc = garage_ec_reseal_stripes(rec_ctx[w], stripes.data(), present.data(), slen.data(), shash.data(),
-                                                keyed ? skeys.data() : nullptr, ns, pieces.data(), start.data(),
-                                                dkeys.data(), nonces.data(), dsh, dhash, dsums, dlen.data(), bad.data(),
-                                                sst.data(), st.data(), slot_stride, n);
+        const int rc = garage_ec_reseal_stripes_crc(rec_ctx[w], stripes.data(), present.data(), slen.data(),
+                                                    shash.data(), keyed ? skeys.data() : nullptr, ns, pieces.data(),
+                                                    start.data(), dkeys.data(), nonces.data(), dsh, dhash, dsums,
+                                                    dlen.data(), bad.data(), sst.data(), st.data(), kinds.data(),
+                                                    crcs.data(), slot_stride, n);
         reseal_call_us += us_since(t0);
         reseal_batches++;
         wipe_secret(skeys.data(), skeys.size());
@@ -2151,6 +2162,7 @@ struct garage_bm {
                 J.sums = dsums + i * tot * 32;
                 memcpy(J.hash.data(), dhash + i * 32, 32);
                 J.stored_len = dlen[i];
+                J.crc = crcs[i];
             }
             g[i]->fulfilled = true;
             g[i]->done.set_value(listed ? st[i] : rc);
@@ -2430,8 +2442,10 @@ struct garage_bm {
     // An SSE-C PUT (put.rs:441-466): the plaintext (up to block_size bytes) lands in a put slot and goes through the
     // encode batcher, whose sealed items become one garage_ec_seal_blocks call; key NULL stores it as plaintext.  The
     // nonce prefix is 8 bytes of getrandom(2) (Garage: OsRng).  The k+m shards are stored as rpc_put_block stores a
-    // block of sealed_len bytes; *hash_out = the block's content address.
-    int rpc_put_block_sealed(const uint8_t *key, const uint8_t *data, size_t len, uint8_t *hash_out)
+    // block of sealed_len bytes; *hash_out = the block's content address.  crc_kind (GARAGE_EC_CRC_*): *crc_out = the
+    // S3 checksum of the plaintext, from the same seal call.
+    int rpc_put_block_sealed(const uint8_t *key, const uint8_t *data, size_t len, uint8_t *hash_out,
+                             uint8_t crc_kind = GARAGE_EC_CRC_NONE, uint32_t *crc_out = nullptr)
     {
         if (len > cfg.block_size || (!key && len == 0)) return GARAGE_BM_E_MESSAGE;
         uint32_t blen = (uint32_t)len;
@@ -2444,6 +2458,7 @@ struct garage_bm {
         it.len = (uint32_t)len;
         it.sealed = true;
         it.key = key;
+        it.crc_kind = crc_kind;
         for (size_t got = 0; key && got < sizeof(it.nonce);) {
             const ssize_t r = getrandom(it.nonce + got, sizeof(it.nonce) - got, 0);
             if (r < 0 && errno != EINTR) return GARAGE_BM_E_MESSAGE;
@@ -2453,6 +2468,7 @@ struct garage_bm {
         if (rc != GARAGE_EC_OK) return rc;
         sealed_puts++;
         memcpy(hash_out, it.hash.data(), 32);
+        if (crc_out) *crc_out = it.crc;
         const uint8_t *sh = it.shards;
         const size_t stride = it.pstride;
         return store_block(it.hash, blen, shard_len_of(blen), [&](int i) { return sh + (size_t)i * stride; }, it.sums);
@@ -2465,9 +2481,11 @@ struct garage_bm {
     // serve (a previous code, replicas) or that does not hash to its address is read by rpc_get_block -- the stale-shard
     // hunt quarantines the culprit -- and its stored bytes (ciphertext for keyed sources) are framed into its buffer with
     // every data shard present; the copy is retried once.  No plaintext is in host memory on any path.  The result is
-    // stored as rpc_put_block stores a block of its sealed length; refcounts are not touched.
+    // stored as rpc_put_block stores a block of its sealed length; refcounts are not touched.  crc_kind: *crc_out = the
+    // S3 checksum of the destination's plaintext, from the GPU call that sealed it (the retry's, after a fallback).
     int rpc_put_block_resealed(const garage_bm_piece *in, int n_in, const uint8_t *src_key, const uint8_t *dst_key,
-                               uint8_t *hash_out, uint32_t *stored_len_out)
+                               uint8_t *hash_out, uint32_t *stored_len_out, uint8_t crc_kind = GARAGE_EC_CRC_NONE,
+                               uint32_t *crc_out = nullptr)
     {
         const auto t0 = Clock::now();
         struct AddTime {
@@ -2497,6 +2515,7 @@ struct garage_bm {
         J.src_hash = hs;
         J.src_key = src_key;
         J.dst_key = dst_key;
+        J.crc_kind = crc_kind;
         // the stored block through rpc_get_block, framed into the source's buffer with all data shards present
         auto frame = [&](size_t j) -> int {
             reseal_fallbacks++;
@@ -2565,6 +2584,7 @@ struct garage_bm {
         if (rc != GARAGE_BM_OK) return rc;
         memcpy(hash_out, J.hash.data(), 32);
         if (stored_len_out) *stored_len_out = J.stored_len;
+        if (crc_out) *crc_out = J.crc;
         const uint8_t *sh = J.shards;
         const size_t stride = slot_stride;
         return store_block(J.hash, J.stored_len, shard_len_of(J.stored_len), [&](int i) { return sh + (size_t)i * stride; },
@@ -4876,6 +4896,13 @@ int garage_bm_rpc_put_block_sealed(garage_bm *bm, const uint8_t *key32, const ui
     BM_GUARD(bm->rpc_put_block_sealed(key32, data, len, hash_out));
 }
 
+int garage_bm_rpc_put_block_sealed_crc(garage_bm *bm, const uint8_t *key32, const uint8_t *data, size_t len,
+                                       uint8_t crc_kind, uint8_t hash_out[32], uint32_t *crc_out)
+{
+    if (!bm || !hash_out || !crc_out || (!data && len) || crc_kind > GARAGE_EC_CRC_CRC32C) return GARAGE_EC_E_INVALID;
+    BM_GUARD(bm->rpc_put_block_sealed(key32, data, len, hash_out, crc_kind, crc_out));
+}
+
 int garage_bm_rpc_get_block_opened(garage_bm *bm, const uint8_t hash[32], const uint8_t *key32, uint8_t *out, size_t cap,
                                    size_t *out_len)
 {
@@ -4908,6 +4935,17 @@ int garage_bm_rpc_put_block_resealed(garage_bm *bm, const garage_bm_piece *piece
     if (!bm || !pieces || !dst_key32 || !hash_out || n_pieces < 1 || n_pieces > GARAGE_BM_MAX_PIECES)
         return GARAGE_EC_E_INVALID;
     BM_GUARD(bm->rpc_put_block_resealed(pieces, n_pieces, src_key32, dst_key32, hash_out, stored_len_out));
+}
+
+int garage_bm_rpc_put_block_resealed_crc(garage_bm *bm, const garage_bm_piece *pieces, int n_pieces,
+                                         const uint8_t *src_key32, const uint8_t *dst_key32, uint8_t crc_kind,
+                                         uint8_t hash_out[32], uint32_t *stored_len_out, uint32_t *crc_out)
+{
+    if (!bm || !pieces || !dst_key32 || !hash_out || !crc_out || n_pieces < 1 || n_pieces > GARAGE_BM_MAX_PIECES ||
+        crc_kind > GARAGE_EC_CRC_CRC32C)
+        return GARAGE_EC_E_INVALID;
+    BM_GUARD(bm->rpc_put_block_resealed(pieces, n_pieces, src_key32, dst_key32, hash_out, stored_len_out, crc_kind,
+                                        crc_out));
 }
 
 void garage_bm_get_reseal_metrics(garage_bm *bm, garage_bm_reseal_metrics *o)

@@ -2731,10 +2731,10 @@ int garage_ec_transcode(garage_ec_ctx *dst, garage_ec_ctx *src, uint8_t *src_sha
 }  // extern "C"
 namespace {
 
-// Device scratch of a seal or open of n blocks: key material | len(B) | L | (open) reconstruct status | want | plan.
-// The key material comes first so that one memset clears every secret.
+// Device scratch of a seal or open of n blocks: key material | len(B) | L | (seal) checksum accumulators | (open)
+// reconstruct status | want | plan.  The key material comes first so that one memset clears every secret.
 struct SseScratch {
-    size_t o_keys, o_blen, o_len, o_rec, o_want, o_plan, bytes;
+    size_t o_keys, o_blen, o_len, o_crc, o_rec, o_want, o_plan, bytes;
     SseScratch(const garage_ec_ctx *ctx, size_t n, bool open)
     {
         size_t b = 0;
@@ -2746,6 +2746,7 @@ struct SseScratch {
         o_keys = take(n * sizeof(sse::SseKey));
         o_blen = take(n * 4);
         o_len = take(n * 4);
+        o_crc = open ? 0 : take(n * 4);
         o_rec = open ? take(n * 4) : 0;
         o_want = open ? take(n * (size_t)(ctx->k + ctx->m)) : 0;
         o_plan = open ? take(plan_scratch_bytes(ctx, n)) : 0;
@@ -2788,6 +2789,15 @@ int sse_launch_chunks(garage_ec_ctx *ctx, sse::ChunkParams q, cudaStream_t st)
     return e == cudaSuccess ? GARAGE_EC_OK : set_cuda_error(ctx, e, "sse_chunk_kernel launch");
 }
 
+// the checksum passes around a kCrc chunk kernel (sse_crc_pass_kernel)
+int sse_launch_crc_pass(garage_ec_ctx *ctx, const sse::CrcPassParams &q, cudaStream_t st)
+{
+    sse::sse_crc_pass_kernel<<<(unsigned)std::min<size_t>((q.n + 255) / 256, (size_t)ctx->sm_count * 4), 256, 0, st>>>(q);
+    ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? GARAGE_EC_OK : set_cuda_error(ctx, e, "sse_crc_pass_kernel launch");
+}
+
 int sse_launch_block_sums(garage_ec_ctx *ctx, const uint8_t *shards, const uint32_t *blen, const uint8_t *hashes,
                           uint8_t *hash_bad, uint8_t *digest, size_t stride, size_t n, cudaStream_t st)
 {
@@ -2809,11 +2819,12 @@ int sse_launch_block_sums(garage_ec_ctx *ctx, const uint8_t *shards, const uint3
     return e == cudaSuccess ? GARAGE_EC_OK : set_cuda_error(ctx, e, "blake2sum_blocks_kernel launch");
 }
 
-// Seal n blocks on the device: lengths, key schedules, the GCM chunks into the data shards, the code's encode, the
-// content hash and (sums != NULL) the shard tags.  The caller zeroes the key material of `scratch`.
+// Seal n blocks on the device: lengths, key schedules, the GCM chunks into the data shards (crc_kind != NULL: and the
+// plaintext checksums into crcs), the code's encode, the content hash and (sums != NULL) the shard tags.  The caller
+// zeroes the key material of `scratch`.
 int run_seal(garage_ec_ctx *ctx, const uint8_t *plain, size_t plain_stride, const uint32_t *plain_len,
              const uint8_t *keys, const uint8_t *nonces, uint8_t *shards, size_t stride, uint8_t *hashes, uint8_t *sums,
-             size_t n, uint8_t *scratch, cudaStream_t st)
+             const uint8_t *crc_kind, uint32_t *crcs, size_t n, uint8_t *scratch, cudaStream_t st)
 {
     const SseScratch sc(ctx, n, false);
     sse::SseKey *ks = keys ? reinterpret_cast<sse::SseKey *>(scratch + sc.o_keys) : nullptr;
@@ -2832,6 +2843,16 @@ int run_seal(garage_ec_ctx *ctx, const uint8_t *plain, size_t plain_stride, cons
     lp.quantum = ctx->quantum;
     lp.keyed = keys ? 1u : 0u;
     int rc = sse_launch_lens(ctx, lp, n, st);
+    sse::CrcPassParams cp;
+    memset(&cp, 0, sizeof(cp));
+    cp.kind = crc_kind;
+    cp.acc = reinterpret_cast<uint32_t *>(scratch + sc.o_crc);
+    cp.shard_len = L;
+    cp.blen = blen;
+    cp.plain_len = plain_len;
+    cp.crcs = crcs;
+    cp.n = (uint32_t)n;
+    if (!rc && crc_kind) rc = sse_launch_crc_pass(ctx, cp, st);
     if (!rc && keys) rc = sse_launch_setup(ctx, keys, ks, n, st);
     if (rc) return rc;
     sse::ChunkParams q;
@@ -2848,7 +2869,11 @@ int run_seal(garage_ec_ctx *ctx, const uint8_t *plain, size_t plain_stride, cons
     q.k = (uint32_t)ctx->k;
     q.m = (uint32_t)ctx->m;
     q.n = (uint32_t)n;
-    rc = sse_launch_chunks<sse::kSeal>(ctx, q, st);
+    q.crc_kind = crc_kind;
+    q.crc_acc = cp.acc;
+    rc = crc_kind ? sse_launch_chunks<sse::kSeal | sse::kCrc>(ctx, q, st) : sse_launch_chunks<sse::kSeal>(ctx, q, st);
+    cp.final = 1;
+    if (!rc && crc_kind) rc = sse_launch_crc_pass(ctx, cp, st);
     if (!rc)
         rc = run_uniform(ctx, kModeEncode, shards, tot * stride, shards + (size_t)ctx->k * stride, tot * stride, nullptr, L,
                          stride, n, st);
@@ -2954,7 +2979,7 @@ struct LaneKeyWipe {
 
 int seal_host(garage_ec_ctx *ctx, const uint8_t *plain, size_t plain_stride, const uint8_t *const *blocks,
               const uint32_t *plain_len, const uint8_t *keys, const uint8_t *nonces, uint8_t *shards, size_t stride,
-              uint8_t *hashes, uint8_t *sums, size_t n)
+              uint8_t *hashes, uint8_t *sums, const uint8_t *crc_kind, uint32_t *crcs, size_t n)
 {
     const size_t tot = ctx->k + ctx->m;
     auto block_at = [&](size_t s) { return blocks ? blocks[s] : plain + s * plain_stride; };
@@ -2968,7 +2993,8 @@ int seal_host(garage_ec_ctx *ctx, const uint8_t *plain, size_t plain_stride, con
     SmallLayout sl;
     const SseScratch sc(ctx, cs, false);
     const size_t o_scr = sl.take(sc.bytes), o_key = sl.take(cs * 40), o_len = sl.take(cs * 4), o_hash = sl.take(cs * 32),
-                 o_sums = sl.take(sums ? cs * tot * 32 : 0);
+                 o_sums = sl.take(sums ? cs * tot * 32 : 0), o_kind = sl.take(crc_kind ? cs : 0),
+                 o_crcs = sl.take(crc_kind ? cs * 4 : 0);
     wipe.dev_off = o_scr;
     wipe.dev_bytes = o_len - o_scr;  // key material, keys and nonces
     const size_t blk_b = align_up(cs * pitch, 256);
@@ -3003,8 +3029,12 @@ int seal_host(garage_ec_ctx *ctx, const uint8_t *plain, size_t plain_stride, con
                 d_keys = L.d_small + o_key;
                 d_nonces = L.d_small + o_key + cs * 32;
             }
+            if (crc_kind)
+                CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_kind, crc_kind + s0, cnt, cudaMemcpyHostToDevice, L.stream));
+            uint32_t *d_crcs = reinterpret_cast<uint32_t *>(L.d_small + o_crcs);
             r = run_seal(ctx, d_blk, pitch, reinterpret_cast<const uint32_t *>(L.d_small + o_len), d_keys, d_nonces, d_sh,
-                         stride, L.d_small + o_hash, sums ? L.d_small + o_sums : nullptr, cnt, L.d_small + o_scr, L.stream);
+                         stride, L.d_small + o_hash, sums ? L.d_small + o_sums : nullptr,
+                         crc_kind ? L.d_small + o_kind : nullptr, d_crcs, cnt, L.d_small + o_scr, L.stream);
             if (r) return r;
             if (keys) CU_TRY(ctx, cudaMemsetAsync(L.d_small + o_scr, 0, o_len - o_scr, L.stream));
             // D2H: roundup16(L) bytes of all k+m shards (the data shards are ciphertext now)
@@ -3020,6 +3050,7 @@ int seal_host(garage_ec_ctx *ctx, const uint8_t *plain, size_t plain_stride, con
             if (sums)
                 CU_TRY(ctx, cudaMemcpyAsync(sums + s0 * tot * 32, L.d_small + o_sums, cnt * tot * 32, cudaMemcpyDeviceToHost,
                                             L.stream));
+            if (crc_kind) CU_TRY(ctx, cudaMemcpyAsync(crcs + s0, d_crcs, cnt * 4, cudaMemcpyDeviceToHost, L.stream));
             return GARAGE_EC_OK;
         },
         keys ? clear_keys : Retire());
@@ -3127,15 +3158,23 @@ int open_host(garage_ec_ctx *ctx, uint8_t *shards, uint8_t *const *stripes, cons
 
 // checks shared by every seal form; plain_len values are host memory (HOST) or not looked at (DEVICE)
 int seal_args(garage_ec_ctx *ctx, const uint8_t *keys, const uint8_t *nonces, const uint8_t *shards, size_t stride,
-              const uint8_t *hashes, const uint8_t *sums, size_t n)
+              const uint8_t *hashes, const uint8_t *sums, const uint8_t *crc_kind, const uint32_t *crcs, size_t n)
 {
     if (!ctx) return GARAGE_EC_E_INVALID;
     int rc = check_geometry(ctx, stride, n, ctx->k + ctx->m);
     if (rc) return rc;
     if (n == 0) return GARAGE_EC_OK;
-    if (!shards || !hashes || (!keys) != (!nonces)) return GARAGE_EC_E_INVALID;
+    if (!shards || !hashes || (!keys) != (!nonces) || (crc_kind && !crcs)) return GARAGE_EC_E_INVALID;
     if (sums && n * (size_t)(ctx->k + ctx->m) > 0xffffffffull) return GARAGE_EC_E_INVALID;
     if (!aligned16(shards)) return GARAGE_EC_E_ALIGN;
+    return GARAGE_EC_OK;
+}
+
+// HOST: every checksum kind is known
+int crc_kinds_ok(const uint8_t *crc_kind, size_t n)
+{
+    for (size_t s = 0; crc_kind && s < n; s++)
+        if (crc_kind[s] > GARAGE_EC_CRC_CRC32C) return GARAGE_EC_E_INVALID;
     return GARAGE_EC_OK;
 }
 
@@ -3161,12 +3200,12 @@ int garage_ec_sealed_len(uint32_t plain_len, uint32_t *sealed_len)
     return GARAGE_EC_OK;
 }
 
-int garage_ec_seal(garage_ec_ctx *ctx, const uint8_t *plain, size_t plain_stride, const uint32_t *plain_len,
-                   const uint8_t *keys, const uint8_t *nonces, uint8_t *shards, size_t stride, uint8_t *hashes,
-                   uint8_t *sums, size_t n, int mem_kind, void *cuda_stream)
+int garage_ec_seal_crc(garage_ec_ctx *ctx, const uint8_t *plain, size_t plain_stride, const uint32_t *plain_len,
+                       const uint8_t *keys, const uint8_t *nonces, uint8_t *shards, size_t stride, uint8_t *hashes,
+                       uint8_t *sums, const uint8_t *crc_kind, uint32_t *crcs, size_t n, int mem_kind, void *cuda_stream)
 {
     if (mem_kind != GARAGE_EC_MEM_HOST && mem_kind != GARAGE_EC_MEM_DEVICE) return GARAGE_EC_E_INVALID;
-    int rc = seal_args(ctx, keys, nonces, shards, stride, hashes, sums, n);
+    int rc = seal_args(ctx, keys, nonces, shards, stride, hashes, sums, crc_kind, crcs, n);
     if (rc || n == 0) return rc;
     if (!plain || !plain_len || (plain_stride & 15)) return GARAGE_EC_E_INVALID;
     if (!aligned16(plain)) return GARAGE_EC_E_ALIGN;
@@ -3174,36 +3213,63 @@ int garage_ec_seal(garage_ec_ctx *ctx, const uint8_t *plain, size_t plain_stride
         for (size_t s = 0; s < n; s++)
             if (plain_len[s] > plain_stride) return GARAGE_EC_E_INVALID;
         rc = seal_host_lens_ok(ctx, plain_len, keys != nullptr, stride, n);
+        if (!rc) rc = crc_kinds_ok(crc_kind, n);
         if (rc) return rc;
         CU_TRY(ctx, cudaSetDevice(ctx->device));
-        return seal_host(ctx, plain, plain_stride, nullptr, plain_len, keys, nonces, shards, stride, hashes, sums, n);
+        return seal_host(ctx, plain, plain_stride, nullptr, plain_len, keys, nonces, shards, stride, hashes, sums,
+                         crc_kind, crcs, n);
     }
     if ((reinterpret_cast<uintptr_t>(plain_len) & 3) || (reinterpret_cast<uintptr_t>(hashes) & 7) ||
-        (reinterpret_cast<uintptr_t>(sums) & 7))
+        (reinterpret_cast<uintptr_t>(sums) & 7) || (crc_kind && (reinterpret_cast<uintptr_t>(crcs) & 3)))
         return GARAGE_EC_E_ALIGN;
     CU_TRY(ctx, cudaSetDevice(ctx->device));
     cudaStream_t st = (cudaStream_t)cuda_stream;
     const SseScratch sc(ctx, n, false);
     return with_stream_scratch(ctx, sc.bytes, st, [&](uint8_t *scratch) {
-        const int r = run_seal(ctx, plain, plain_stride, plain_len, keys, nonces, shards, stride, hashes, sums, n, scratch, st);
+        const int r = run_seal(ctx, plain, plain_stride, plain_len, keys, nonces, shards, stride, hashes, sums, crc_kind,
+                               crcs, n, scratch, st);
         const cudaError_t e = keys ? cudaMemsetAsync(scratch + sc.o_keys, 0, n * sizeof(sse::SseKey), st) : cudaSuccess;
         if (r) return r;
         return e == cudaSuccess ? GARAGE_EC_OK : set_cuda_error(ctx, e, "cudaMemsetAsync(key material)");
     });
 }
 
-int garage_ec_seal_blocks(garage_ec_ctx *ctx, const uint8_t *const *blocks, const uint32_t *plain_len, const uint8_t *keys,
-                          const uint8_t *nonces, uint8_t *shards, size_t stride, uint8_t *hashes, uint8_t *sums, size_t n)
+int garage_ec_seal(garage_ec_ctx *ctx, const uint8_t *plain, size_t plain_stride, const uint32_t *plain_len,
+                   const uint8_t *keys, const uint8_t *nonces, uint8_t *shards, size_t stride, uint8_t *hashes,
+                   uint8_t *sums, size_t n, int mem_kind, void *cuda_stream)
 {
-    int rc = seal_args(ctx, keys, nonces, shards, stride, hashes, sums, n);
+    return garage_ec_seal_crc(ctx, plain, plain_stride, plain_len, keys, nonces, shards, stride, hashes, sums, nullptr,
+                              nullptr, n, mem_kind, cuda_stream);
+}
+
+int garage_ec_seal_blocks_crc(garage_ec_ctx *ctx, const uint8_t *const *blocks, const uint32_t *plain_len,
+                              const uint8_t *keys, const uint8_t *nonces, uint8_t *shards, size_t stride, uint8_t *hashes,
+                              uint8_t *sums, const uint8_t *crc_kind, uint32_t *crcs, size_t n)
+{
+    int rc = seal_args(ctx, keys, nonces, shards, stride, hashes, sums, crc_kind, crcs, n);
     if (rc || n == 0) return rc;
     if (!blocks || !plain_len) return GARAGE_EC_E_INVALID;
     for (size_t s = 0; s < n; s++)
         if (!blocks[s] && plain_len[s]) return GARAGE_EC_E_INVALID;
     rc = seal_host_lens_ok(ctx, plain_len, keys != nullptr, stride, n);
+    if (!rc) rc = crc_kinds_ok(crc_kind, n);
     if (rc) return rc;
     CU_TRY(ctx, cudaSetDevice(ctx->device));
-    return seal_host(ctx, nullptr, 0, blocks, plain_len, keys, nonces, shards, stride, hashes, sums, n);
+    return seal_host(ctx, nullptr, 0, blocks, plain_len, keys, nonces, shards, stride, hashes, sums, crc_kind, crcs, n);
+}
+
+int garage_ec_seal_blocks(garage_ec_ctx *ctx, const uint8_t *const *blocks, const uint32_t *plain_len, const uint8_t *keys,
+                          const uint8_t *nonces, uint8_t *shards, size_t stride, uint8_t *hashes, uint8_t *sums, size_t n)
+{
+    return garage_ec_seal_blocks_crc(ctx, blocks, plain_len, keys, nonces, shards, stride, hashes, sums, nullptr, nullptr,
+                                     n);
+}
+
+int garage_ec_crc_combine(int kind, uint32_t crc_a, uint32_t crc_b, uint64_t len_b, uint32_t *out)
+{
+    if (!out || kind < GARAGE_EC_CRC_CRC32 || kind > GARAGE_EC_CRC_CRC32C) return GARAGE_EC_E_INVALID;
+    *out = sse::crc_shift(sse::kCrcHost, kind - 1, crc_a, len_b) ^ crc_b;
+    return GARAGE_EC_OK;
 }
 
 static int open_args(garage_ec_ctx *ctx, const void *shards, const uint8_t *present, const uint32_t *sealed,
@@ -3566,10 +3632,10 @@ namespace {
 static_assert(sizeof(garage_ec_piece) == 12, "garage_ec_piece is three uint32 words");
 
 // Device scratch of a reseal of n_src sources into n_dst destinations: key material (sources, then destinations) |
-// source L | reconstruct status | want | plan | destination |Q|, len(B'), L'.  The key material comes first so that
-// one memset clears every secret.
+// source L | reconstruct status | want | plan | destination |Q|, len(B'), L', checksum accumulator.  The key material
+// comes first so that one memset clears every secret.
 struct ResealScratch {
-    size_t o_keys, keys_bytes, o_src_L, o_rec, o_want, o_plan, o_plen, o_blen, o_dst_L, bytes;
+    size_t o_keys, keys_bytes, o_src_L, o_rec, o_want, o_plan, o_plen, o_blen, o_dst_L, o_crc, bytes;
     ResealScratch(const garage_ec_ctx *ctx, size_t n_src, size_t n_dst)
     {
         size_t b = 0;
@@ -3587,19 +3653,21 @@ struct ResealScratch {
         o_plen = take(n_dst * 4);
         o_blen = take(n_dst * 4);
         o_dst_L = take(n_dst * 4);
+        o_crc = take(n_dst * 4);
         bytes = b;
     }
 };
 
 // Reseal on the device: framing, piece lists and lengths, key schedules, the rebuild of absent source data shards,
 // the sources' content hashes and (keyed) every chunk tag, the destinations' verdicts, the fused decrypt-and-seal
-// into the destination data shards, the code's encode, the destinations' content hashes and (sums != NULL) their
-// shard tags.  The caller zeroes the key material of `scratch`.
+// into the destination data shards (crc_kind != NULL: and the checksums of Q_d into crcs), the code's encode, the
+// destinations' content hashes and (sums != NULL) their shard tags.  The caller zeroes the key material of `scratch`.
 int run_reseal(garage_ec_ctx *ctx, uint8_t *src_shards, const uint8_t *src_present, const uint32_t *src_len,
                const uint8_t *src_hashes, const uint8_t *src_keys, size_t n_src, const uint32_t *pieces,
                const uint32_t *piece_start, const uint8_t *dst_keys, const uint8_t *dst_nonces, uint8_t *dst_shards,
                uint8_t *dst_hashes, uint8_t *dst_sums, uint32_t *dst_len_out, uint8_t *src_hash_bad,
-               int32_t *src_status, int32_t *status, size_t stride, size_t n_dst, uint8_t *scratch, cudaStream_t st)
+               int32_t *src_status, int32_t *status, const uint8_t *crc_kind, uint32_t *crcs, size_t stride,
+               size_t n_dst, uint8_t *scratch, cudaStream_t st)
 {
     const ResealScratch sc(ctx, n_src, n_dst);
     const size_t tot = ctx->k + ctx->m, nmax = std::max(n_src, n_dst);
@@ -3630,7 +3698,17 @@ int run_reseal(garage_ec_ctx *ctx, uint8_t *src_shards, const uint8_t *src_prese
     sse::sse_reseal_lens_kernel<<<grid, 256, 0, st>>>(lp);
     ctx->launches.fetch_add(1, std::memory_order_relaxed);
     CU_TRY(ctx, cudaGetLastError());
-    int rc = src_keys && n_src ? sse_launch_setup(ctx, src_keys, ks, n_src, st) : GARAGE_EC_OK;
+    sse::CrcPassParams cp;
+    memset(&cp, 0, sizeof(cp));
+    cp.kind = crc_kind;
+    cp.acc = reinterpret_cast<uint32_t *>(scratch + sc.o_crc);
+    cp.shard_len = dst_L;
+    cp.status = status;
+    cp.plain_len = plen;
+    cp.crcs = crcs;
+    cp.n = (uint32_t)n_dst;
+    int rc = crc_kind ? sse_launch_crc_pass(ctx, cp, st) : GARAGE_EC_OK;
+    if (!rc && src_keys && n_src) rc = sse_launch_setup(ctx, src_keys, ks, n_src, st);
     if (!rc) rc = sse_launch_setup(ctx, dst_keys, ks + n_src, n_dst, st);
     if (!rc && n_src)
         rc = run_reconstruct(ctx, src_shards, src_present, scratch + sc.o_want, rec, src_L, stride, n_src,
@@ -3689,7 +3767,12 @@ int run_reseal(garage_ec_ctx *ctx, uint8_t *src_shards, const uint8_t *src_prese
     q.src_len = src_len;
     q.src_L = src_L;
     q.src_ks = src_keys ? ks : nullptr;
-    rc = sse_launch_chunks<sse::kReseal>(ctx, q, st);
+    q.crc_kind = crc_kind;
+    q.crc_acc = cp.acc;
+    rc = crc_kind ? sse_launch_chunks<sse::kReseal | sse::kCrc>(ctx, q, st) : sse_launch_chunks<sse::kReseal>(ctx, q, st);
+    cp.final = 1;
+    cp.status = nullptr;
+    if (!rc && crc_kind) rc = sse_launch_crc_pass(ctx, cp, st);
     if (!rc)
         rc = run_uniform(ctx, kModeEncode, dst_shards, tot * stride, dst_shards + (size_t)ctx->k * stride, tot * stride,
                          nullptr, dst_L, stride, n_dst, st);
@@ -3732,8 +3815,8 @@ int reseal_host(garage_ec_ctx *ctx, const uint8_t *src_shards, const uint8_t *co
                 const uint8_t *src_present, const uint32_t *src_len, const uint8_t *src_hashes, const uint8_t *src_keys,
                 size_t n_src, const garage_ec_piece *pieces, const uint32_t *piece_start, const uint8_t *dst_keys,
                 const uint8_t *dst_nonces, uint8_t *dst_shards, uint8_t *dst_hashes, uint8_t *dst_sums,
-                uint32_t *dst_len_out, uint8_t *src_hash_bad, int32_t *src_status, int32_t *status, size_t stride,
-                size_t n_dst)
+                uint32_t *dst_len_out, uint8_t *src_hash_bad, int32_t *src_status, int32_t *status,
+                const uint8_t *crc_kind, uint32_t *crcs, size_t stride, size_t n_dst)
 {
     const size_t k = ctx->k, tot = ctx->k + ctx->m;
     auto shard_at = [&](size_t i, size_t j) {
@@ -3781,7 +3864,8 @@ int reseal_host(garage_ec_ctx *ctx, const uint8_t *src_shards, const uint8_t *co
                  o_slen = sl.take(max_src * 4), o_shash = sl.take(max_src * 32), o_pieces = sl.take(max_pieces * 12),
                  o_pstart = sl.take((cs + 1) * 4), o_sbad = sl.take(max_src), o_sstatus = sl.take(max_src * 4),
                  o_dlen = sl.take(cs * 4), o_status = sl.take(cs * 4), o_dhash = sl.take(cs * 32),
-                 o_dsums = sl.take(dst_sums ? cs * tot * 32 : 0);
+                 o_dsums = sl.take(dst_sums ? cs * tot * 32 : 0), o_kind = sl.take(crc_kind ? cs : 0),
+                 o_crcs = sl.take(crc_kind ? cs * 4 : 0);
     wipe.dev_off = o_scr;
     wipe.dev_bytes = o_present - o_scr;
     const size_t src_b = align_up(max_src * tot * stride, 256);
@@ -3863,13 +3947,15 @@ int reseal_host(garage_ec_ctx *ctx, const uint8_t *src_shards, const uint8_t *co
             if (r) return r;
             CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_key, L.h_key, max_src * 32 + cs * 40, cudaMemcpyHostToDevice, L.stream));
             CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_present, ch.host, o_sbad - o_present, cudaMemcpyHostToDevice, L.stream));
+            if (crc_kind)
+                CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_kind, crc_kind + s0, cnt, cudaMemcpyHostToDevice, L.stream));
             auto u32 = [&](size_t o) { return reinterpret_cast<uint32_t *>(L.d_small + o); };
             r = run_reseal(ctx, d_src, L.d_small + o_present, u32(o_slen), L.d_small + o_shash,
                            src_keys ? L.d_small + o_key : nullptr, S.size(), u32(o_pieces), u32(o_pstart),
                            L.d_small + o_key + max_src * 32, L.d_small + o_key + max_src * 32 + cs * 32, d_dst,
                            L.d_small + o_dhash, dst_sums ? L.d_small + o_dsums : nullptr, u32(o_dlen), L.d_small + o_sbad,
-                           reinterpret_cast<int32_t *>(u32(o_sstatus)), reinterpret_cast<int32_t *>(u32(o_status)), stride,
-                           cnt, L.d_small + o_scr, L.stream);
+                           reinterpret_cast<int32_t *>(u32(o_sstatus)), reinterpret_cast<int32_t *>(u32(o_status)),
+                           crc_kind ? L.d_small + o_kind : nullptr, u32(o_crcs), stride, cnt, L.d_small + o_scr, L.stream);
             if (r) return r;
             CU_TRY(ctx, cudaMemsetAsync(L.d_small + o_scr, 0, wipe.dev_bytes, L.stream));
             CU_TRY(ctx, cudaMemcpyAsync(at(ch, o_sbad, o_present), L.d_small + o_sbad, o_dhash - o_sbad,
@@ -3878,6 +3964,7 @@ int reseal_host(garage_ec_ctx *ctx, const uint8_t *src_shards, const uint8_t *co
             if (dst_sums)
                 CU_TRY(ctx, cudaMemcpyAsync(dst_sums + s0 * tot * 32, L.d_small + o_dsums, cnt * tot * 32,
                                             cudaMemcpyDeviceToHost, L.stream));
+            if (crc_kind) CU_TRY(ctx, cudaMemcpyAsync(crcs + s0, u32(o_crcs), cnt * 4, cudaMemcpyDeviceToHost, L.stream));
             return GARAGE_EC_OK;
         },
         retire);
@@ -3896,13 +3983,14 @@ int reseal_args(garage_ec_ctx *ctx, const void *src_shards, const uint8_t *src_p
                 const uint8_t *src_hashes, size_t n_src, const garage_ec_piece *pieces, const uint32_t *piece_start,
                 const uint8_t *dst_keys, const uint8_t *dst_nonces, const uint8_t *dst_shards, const uint8_t *dst_hashes,
                 const uint32_t *dst_len_out, const uint8_t *src_hash_bad, const int32_t *src_status,
-                const int32_t *status, size_t stride, size_t n_dst)
+                const int32_t *status, const uint8_t *crc_kind, const uint32_t *crcs, size_t stride, size_t n_dst)
 {
     if (!ctx) return GARAGE_EC_E_INVALID;
     int rc = check_geometry(ctx, stride, std::max(n_src, n_dst), ctx->k + ctx->m);
     if (rc) return rc;
     if (n_dst == 0) return GARAGE_EC_OK;
-    if (!piece_start || !pieces || !dst_keys || !dst_nonces || !dst_shards || !dst_hashes || !dst_len_out || !status)
+    if (!piece_start || !pieces || !dst_keys || !dst_nonces || !dst_shards || !dst_hashes || !dst_len_out || !status ||
+        (crc_kind && !crcs))
         return GARAGE_EC_E_INVALID;
     if (n_src && (!src_shards || !src_present || !src_len || !src_hashes || !src_hash_bad || !src_status))
         return GARAGE_EC_E_INVALID;
@@ -3913,28 +4001,30 @@ int reseal_args(garage_ec_ctx *ctx, const void *src_shards, const uint8_t *src_p
 }  // namespace
 extern "C" {
 
-int garage_ec_reseal(garage_ec_ctx *ctx, uint8_t *src_shards, const uint8_t *src_present, const uint32_t *src_len,
-                     const uint8_t *src_hashes, const uint8_t *src_keys, size_t n_src, const garage_ec_piece *pieces,
-                     const uint32_t *piece_start, const uint8_t *dst_keys, const uint8_t *dst_nonces,
-                     uint8_t *dst_shards, uint8_t *dst_hashes, uint8_t *dst_sums, uint32_t *dst_len_out,
-                     uint8_t *src_hash_bad, int32_t *src_status, int32_t *status, size_t stride, size_t n_dst,
-                     int mem_kind, void *cuda_stream)
+int garage_ec_reseal_crc(garage_ec_ctx *ctx, uint8_t *src_shards, const uint8_t *src_present, const uint32_t *src_len,
+                         const uint8_t *src_hashes, const uint8_t *src_keys, size_t n_src, const garage_ec_piece *pieces,
+                         const uint32_t *piece_start, const uint8_t *dst_keys, const uint8_t *dst_nonces,
+                         uint8_t *dst_shards, uint8_t *dst_hashes, uint8_t *dst_sums, uint32_t *dst_len_out,
+                         uint8_t *src_hash_bad, int32_t *src_status, int32_t *status, const uint8_t *crc_kind,
+                         uint32_t *crcs, size_t stride, size_t n_dst, int mem_kind, void *cuda_stream)
 {
     if (mem_kind != GARAGE_EC_MEM_HOST && mem_kind != GARAGE_EC_MEM_DEVICE) return GARAGE_EC_E_INVALID;
     int rc = reseal_args(ctx, src_shards, src_present, src_len, src_hashes, n_src, pieces, piece_start, dst_keys,
-                         dst_nonces, dst_shards, dst_hashes, dst_len_out, src_hash_bad, src_status, status, stride, n_dst);
+                         dst_nonces, dst_shards, dst_hashes, dst_len_out, src_hash_bad, src_status, status, crc_kind, crcs,
+                         stride, n_dst);
     if (rc || n_dst == 0) return rc;
     if (n_src && !aligned16(src_shards)) return GARAGE_EC_E_ALIGN;
     if (mem_kind == GARAGE_EC_MEM_HOST) {
         rc = reseal_host_args_ok(ctx, src_len, src_keys != nullptr, n_src, pieces, piece_start, stride, n_dst);
+        if (!rc) rc = crc_kinds_ok(crc_kind, n_dst);
         if (rc) return rc;
         CU_TRY(ctx, cudaSetDevice(ctx->device));
         return reseal_host(ctx, src_shards, nullptr, src_present, src_len, src_hashes, src_keys, n_src, pieces,
                            piece_start, dst_keys, dst_nonces, dst_shards, dst_hashes, dst_sums, dst_len_out,
-                           src_hash_bad, src_status, status, stride, n_dst);
+                           src_hash_bad, src_status, status, crc_kind, crcs, stride, n_dst);
     }
     for (const void *p : {(const void *)src_len, (const void *)pieces, (const void *)piece_start, (const void *)dst_len_out,
-                          (const void *)src_status, (const void *)status})
+                          (const void *)src_status, (const void *)status, (const void *)crcs})
         if (reinterpret_cast<uintptr_t>(p) & 3) return GARAGE_EC_E_ALIGN;
     if ((reinterpret_cast<uintptr_t>(src_hashes) & 7) || (reinterpret_cast<uintptr_t>(dst_hashes) & 7) ||
         (reinterpret_cast<uintptr_t>(dst_sums) & 7))
@@ -3945,12 +4035,48 @@ int garage_ec_reseal(garage_ec_ctx *ctx, uint8_t *src_shards, const uint8_t *src
     return with_stream_scratch(ctx, sc.bytes, st, [&](uint8_t *scratch) {
         const int r = run_reseal(ctx, src_shards, src_present, src_len, src_hashes, src_keys, n_src,
                                  reinterpret_cast<const uint32_t *>(pieces), piece_start, dst_keys, dst_nonces, dst_shards,
-                                 dst_hashes, dst_sums, dst_len_out, src_hash_bad, src_status, status, stride, n_dst,
-                                 scratch, st);
+                                 dst_hashes, dst_sums, dst_len_out, src_hash_bad, src_status, status, crc_kind, crcs,
+                                 stride, n_dst, scratch, st);
         const cudaError_t e = cudaMemsetAsync(scratch + sc.o_keys, 0, sc.keys_bytes, st);
         if (r) return r;
         return e == cudaSuccess ? GARAGE_EC_OK : set_cuda_error(ctx, e, "cudaMemsetAsync(key material)");
     });
+}
+
+int garage_ec_reseal(garage_ec_ctx *ctx, uint8_t *src_shards, const uint8_t *src_present, const uint32_t *src_len,
+                     const uint8_t *src_hashes, const uint8_t *src_keys, size_t n_src, const garage_ec_piece *pieces,
+                     const uint32_t *piece_start, const uint8_t *dst_keys, const uint8_t *dst_nonces,
+                     uint8_t *dst_shards, uint8_t *dst_hashes, uint8_t *dst_sums, uint32_t *dst_len_out,
+                     uint8_t *src_hash_bad, int32_t *src_status, int32_t *status, size_t stride, size_t n_dst,
+                     int mem_kind, void *cuda_stream)
+{
+    return garage_ec_reseal_crc(ctx, src_shards, src_present, src_len, src_hashes, src_keys, n_src, pieces, piece_start,
+                                dst_keys, dst_nonces, dst_shards, dst_hashes, dst_sums, dst_len_out, src_hash_bad,
+                                src_status, status, nullptr, nullptr, stride, n_dst, mem_kind, cuda_stream);
+}
+
+int garage_ec_reseal_stripes_crc(garage_ec_ctx *ctx, uint8_t *const *src_stripes, const uint8_t *src_present,
+                                 const uint32_t *src_len, const uint8_t *src_hashes, const uint8_t *src_keys, size_t n_src,
+                                 const garage_ec_piece *pieces, const uint32_t *piece_start, const uint8_t *dst_keys,
+                                 const uint8_t *dst_nonces, uint8_t *dst_shards, uint8_t *dst_hashes, uint8_t *dst_sums,
+                                 uint32_t *dst_len_out, uint8_t *src_hash_bad, int32_t *src_status, int32_t *status,
+                                 const uint8_t *crc_kind, uint32_t *crcs, size_t stride, size_t n_dst)
+{
+    int rc = reseal_args(ctx, src_stripes, src_present, src_len, src_hashes, n_src, pieces, piece_start, dst_keys,
+                         dst_nonces, dst_shards, dst_hashes, dst_len_out, src_hash_bad, src_status, status, crc_kind, crcs,
+                         stride, n_dst);
+    if (rc || n_dst == 0) return rc;
+    for (size_t i = 0; i < n_src; i++) {
+        if (!src_stripes[i]) return GARAGE_EC_E_INVALID;
+        if (!aligned16(src_stripes[i])) return GARAGE_EC_E_ALIGN;
+    }
+    rc = reseal_host_args_ok(ctx, src_len, src_keys != nullptr, n_src, pieces, piece_start, stride, n_dst);
+    if (!rc) rc = crc_kinds_ok(crc_kind, n_dst);
+    if (rc) return rc;
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    return reseal_host(ctx, nullptr, src_stripes, src_present, src_len, src_hashes, src_keys, n_src, pieces, piece_start,
+                       dst_keys, dst_nonces, dst_shards, dst_hashes, dst_sums, dst_len_out, src_hash_bad, src_status,
+                       status, crc_kind, crcs, stride, n_dst);
 }
 
 int garage_ec_reseal_stripes(garage_ec_ctx *ctx, uint8_t *const *src_stripes, const uint8_t *src_present,
@@ -3960,19 +4086,9 @@ int garage_ec_reseal_stripes(garage_ec_ctx *ctx, uint8_t *const *src_stripes, co
                              uint32_t *dst_len_out, uint8_t *src_hash_bad, int32_t *src_status, int32_t *status,
                              size_t stride, size_t n_dst)
 {
-    int rc = reseal_args(ctx, src_stripes, src_present, src_len, src_hashes, n_src, pieces, piece_start, dst_keys,
-                         dst_nonces, dst_shards, dst_hashes, dst_len_out, src_hash_bad, src_status, status, stride, n_dst);
-    if (rc || n_dst == 0) return rc;
-    for (size_t i = 0; i < n_src; i++) {
-        if (!src_stripes[i]) return GARAGE_EC_E_INVALID;
-        if (!aligned16(src_stripes[i])) return GARAGE_EC_E_ALIGN;
-    }
-    rc = reseal_host_args_ok(ctx, src_len, src_keys != nullptr, n_src, pieces, piece_start, stride, n_dst);
-    if (rc) return rc;
-    CU_TRY(ctx, cudaSetDevice(ctx->device));
-    return reseal_host(ctx, nullptr, src_stripes, src_present, src_len, src_hashes, src_keys, n_src, pieces, piece_start,
-                       dst_keys, dst_nonces, dst_shards, dst_hashes, dst_sums, dst_len_out, src_hash_bad, src_status,
-                       status, stride, n_dst);
+    return garage_ec_reseal_stripes_crc(ctx, src_stripes, src_present, src_len, src_hashes, src_keys, n_src, pieces,
+                                        piece_start, dst_keys, dst_nonces, dst_shards, dst_hashes, dst_sums, dst_len_out,
+                                        src_hash_bad, src_status, status, nullptr, nullptr, stride, n_dst);
 }
 
 // ---- test hook -------------------------------------------------------------------------------

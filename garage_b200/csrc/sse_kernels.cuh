@@ -20,6 +20,8 @@
 
 #include <stdint.h>
 
+#include <type_traits>
+
 namespace garage_ec {
 namespace sse {
 
@@ -289,7 +291,8 @@ __global__ void __launch_bounds__(256) sse_setup_kernel(const __grid_constant__ 
 // plaintext bytes [offset, offset + len) to plain_out + s*plain_stride, zero up to roundup16(len).
 // kReseal: copies with re-encryption (DESIGN.md 4.11).  Work item (d, c) is chunk c of destination d: the warp
 // decrypts the source CTR blocks its pieces cover straight into the stage, then seals the stage in place as kSeal does.
-enum { kSeal = 0, kCheck = 1, kOpen = 2, kRangeCheck = 3, kRangeOpen = 4, kReseal = 5 };
+// kCrc (added to kSeal or kReseal): also the CRC32 / CRC32C of each block's plaintext, per q.crc_kind (DESIGN.md 4.12).
+enum { kSeal = 0, kCheck = 1, kOpen = 2, kRangeCheck = 3, kRangeOpen = 4, kReseal = 5, kCrc = 8 };
 
 struct ChunkParams {
     const uint8_t *plain_in;        // seal: block s at plain_in + s*plain_stride
@@ -318,6 +321,9 @@ struct ChunkParams {
     const uint32_t *src_len;        // stored length S_i
     const uint32_t *src_L;          // its L
     const SseKey *src_ks;           // nullable: the sources are plaintext
+    // the kCrc instantiations: checksum kind per block (GARAGE_EC_CRC_*, 0 = none) and its accumulator (DESIGN.md 4.12)
+    const uint8_t *crc_kind;
+    uint32_t *crc_acc;
 };
 
 struct ChunkSmem {
@@ -326,6 +332,98 @@ struct ChunkSmem {
     uint32_t rk[kWarps][60];
     unsigned long long hh[kWarps][16], hl[kWarps][16];
 };
+
+// ---- CRC32 / CRC32C of the plaintext (DESIGN.md 2.9 and 4.12) ----------------------------------------------------
+// Values mod P in the reflected order of zlib: bit 31 is the coefficient of x^0, bit 0 that of x^31.  Kind index t =
+// GARAGE_EC_CRC_* - 1: 0 = CRC32 (0xEDB88320), 1 = CRC32C (0x82F63B78).  "raw" is the CRC with zero init and no final
+// XOR, which is linear: raw(A || B) = raw(A) * x^(8|B|) + raw(B), and leading zero bytes leave it unchanged.
+__host__ __device__ constexpr uint32_t crc_poly(int t) { return t ? 0x82F63B78u : 0xEDB88320u; }
+__host__ __device__ constexpr uint32_t crc_mulx(uint32_t v, uint32_t poly) { return (v >> 1) ^ ((v & 1u) ? poly : 0u); }
+// v / x: P has a constant term, so x is invertible
+__host__ __device__ constexpr uint32_t crc_divx(uint32_t v, uint32_t poly)
+{
+    return (v >> 31) ? ((v ^ poly) << 1) | 1u : v << 1;
+}
+// a * b mod P, branch-free over the 32 coefficients of a
+__host__ __device__ constexpr uint32_t crc_mul(uint32_t a, uint32_t b, uint32_t poly)
+{
+    uint32_t p = 0;
+    for (int i = 0; i < 32; i++) {
+        p ^= b & (0u - ((a >> (31 - i)) & 1u));
+        b = crc_mulx(b, poly);
+    }
+    return p;
+}
+
+struct CrcConsts {
+    uint32_t slice[2][2][256];  // slicing-by-2: slice[t][j][b] = raw(b followed by j zero bytes)
+    uint32_t slot[2][257];      // x^(-128 j): a lane value whose 16-byte slots end j slots into the chunk's grid
+    uint32_t chunk[2][256];     // x^(-32768 c): chunk c's place in the block's grid of 4096-byte chunks
+    uint32_t chunk_hi[2][12];   // x^(-32768 * 256 * 2^i), for chunks from 256 on (a block has fewer than 2^20)
+    uint32_t x8[2][64];         // x^(8 * 2^i): a shift by a byte count
+};
+constexpr CrcConsts make_crc_consts()
+{
+    CrcConsts c{};
+    for (int t = 0; t < 2; t++) {
+        const uint32_t P = crc_poly(t);
+        for (uint32_t b = 0; b < 256; b++) {
+            uint32_t v = b;
+            for (int i = 0; i < 8; i++) v = crc_mulx(v, P);
+            c.slice[t][0][b] = v;
+        }
+        for (uint32_t b = 0; b < 256; b++) c.slice[t][1][b] = (c.slice[t][0][b] >> 8) ^ c.slice[t][0][c.slice[t][0][b] & 0xff];
+        uint32_t h = 0x80000000u;  // x^-128
+        for (int i = 0; i < 128; i++) h = crc_divx(h, P);
+        c.slot[t][0] = 0x80000000u;
+        for (int j = 1; j <= 256; j++) c.slot[t][j] = crc_mul(c.slot[t][j - 1], h, P);
+        c.chunk[t][0] = 0x80000000u;
+        for (int j = 1; j < 256; j++) c.chunk[t][j] = crc_mul(c.chunk[t][j - 1], c.slot[t][256], P);
+        c.chunk_hi[t][0] = crc_mul(c.chunk[t][255], c.slot[t][256], P);
+        for (int i = 1; i < 12; i++) c.chunk_hi[t][i] = crc_mul(c.chunk_hi[t][i - 1], c.chunk_hi[t][i - 1], P);
+        c.x8[t][0] = 0x00800000u;  // x^8
+        for (int i = 1; i < 64; i++) c.x8[t][i] = crc_mul(c.x8[t][i - 1], c.x8[t][i - 1], P);
+    }
+    return c;
+}
+// global, not __constant__, memory: the constant bank layout of every other kernel stays as it was
+__device__ const CrcConsts kCrcDev = make_crc_consts();
+constexpr CrcConsts kCrcHost = make_crc_consts();
+
+// v * x^(8n): square-and-multiply over x8
+__host__ __device__ inline uint32_t crc_shift(const CrcConsts &c, int t, uint32_t v, unsigned long long n)
+{
+    for (int i = 0; n; i++, n >>= 1)
+        if (n & 1) v = crc_mul(c.x8[t][i], v, crc_poly(t));
+    return v;
+}
+// The CRC (init and final XOR 0xFFFFFFFF) of a len-byte message M from acc = raw(M) * x^(-8 len), the form the chunk
+// kernel accumulates: the init's contribution is 0xFFFFFFFF * x^(8 len), so CRC = (acc + 0xFFFFFFFF) * x^(8 len) + 0xFFFFFFFF.
+__host__ __device__ inline uint32_t crc_finish(const CrcConsts &c, int t, uint32_t acc, unsigned long long len)
+{
+    return crc_shift(c, t, acc ^ 0xFFFFFFFFu, len) ^ 0xFFFFFFFFu;
+}
+
+// 6152 bytes on top of ChunkSmem's 41984, under the 48 KiB of static shared memory a CTA may have: slicing-by-4
+// tables for both kinds (8 KiB) would not fit (DESIGN.md 4.12)
+struct CrcChunkSmem : ChunkSmem {
+    uint32_t crc_slice[2][2][256];
+    uint32_t crc_slot[2][257];
+};
+
+// one lane's raw CRC continued over 16 plaintext bytes (two little-endian words, zero past the chunk's end)
+__device__ __forceinline__ uint32_t crc_block16(const uint32_t (*T)[256], uint32_t c, unsigned long long a,
+                                                unsigned long long b)
+{
+    const uint32_t w[4] = {(uint32_t)a, (uint32_t)(a >> 32), (uint32_t)b, (uint32_t)(b >> 32)};
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+        c ^= w[i];
+        c = (c >> 16) ^ T[1][c & 0xff] ^ T[0][(c >> 8) & 0xff];
+        c = (c >> 16) ^ T[1][c & 0xff] ^ T[0][(c >> 8) & 0xff];
+    }
+    return c;
+}
 
 // kReseal: plaintext bytes [x0, x1) of source i into to[0, x1 - x0), lanes splitting its 16-byte blocks.  Block g of a
 // keyed source is decrypted from its ciphertext at B position 8 + 4112 (g / 256) + 16 (g mod 256), counter block
@@ -366,11 +464,22 @@ __device__ __forceinline__ void reseal_piece(const ChunkParams &q, const SseTabl
     }
 }
 
-template <int MODE>
-__global__ void __launch_bounds__(kWarps * 32) sse_chunk_kernel(const __grid_constant__ ChunkParams q)
+// Launch bounds: the checksumming modes are held to the CTAs per SM that kSeal (4) and kReseal (3) reach by their
+// register counts -- unbounded, ptxas gives the checksumming seal 92 registers and 2 CTAs per SM (DESIGN.md 4.12).  A
+// minimum of 0 leaves the other modes as they were built before the checksums existed.
+template <int KMODE>
+__global__ void __launch_bounds__(kWarps * 32, KMODE == (kSeal | kCrc) ? 4 : KMODE == (kReseal | kCrc) ? 3 : 0)
+    sse_chunk_kernel(const __grid_constant__ ChunkParams q)
 {
-    __shared__ ChunkSmem sm;
+    constexpr int MODE = KMODE & ~kCrc;
+    constexpr bool crc = (KMODE & kCrc) != 0;
+    static_assert(!crc || MODE == kSeal || MODE == kReseal, "checksums are computed by the sealing modes only");
+    __shared__ std::conditional_t<crc, CrcChunkSmem, ChunkSmem> sm;
     build_tables(sm.t);
+    if constexpr (crc) {
+        for (uint32_t i = threadIdx.x; i < 2 * 2 * 256; i += blockDim.x) (&sm.crc_slice[0][0][0])[i] = (&kCrcDev.slice[0][0][0])[i];
+        for (uint32_t i = threadIdx.x; i < 2 * 257; i += blockDim.x) (&sm.crc_slot[0][0])[i] = (&kCrcDev.slot[0][0])[i];
+    }
     __syncthreads();
     const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     uint8_t *st = sm.stage[wid];
@@ -383,6 +492,8 @@ __global__ void __launch_bounds__(kWarps * 32) sse_chunk_kernel(const __grid_con
         const uint32_t s = (uint32_t)(w / q.cmax), ci = (uint32_t)(w - (unsigned long long)s * q.cmax);
         const uint32_t L = ranged ? 0u : q.shard_len[s];
         if (!ranged && !L) continue;
+        const uint32_t ckind = crc ? q.crc_kind[s] : 0u;  // 0 or GARAGE_EC_CRC_*: other kinds were given L = 0
+        uint32_t cv = 0;                                   // this lane's raw CRC of its slots
         const bool keyed = MODE != kSeal || q.ks;
         const uint32_t blen = q.blen[s];
         const uint32_t prefix = keyed ? kPrefix : 0, pitch = keyed ? kFrame : kChunk;
@@ -507,6 +618,21 @@ __global__ void __launch_bounds__(kWarps * 32) sse_chunk_kernel(const __grid_con
             const uint8_t *src = q.plain_in + (size_t)s * q.plain_stride + (size_t)kChunk * c;
             for (uint32_t b = lane; b < nb; b += 32)
                 *reinterpret_cast<uint4 *>(st + 16 * b) = *reinterpret_cast<const uint4 *>(src + 16 * b);
+            if constexpr (crc) {
+                if (ckind) {  // the lane's slots, as the keyed path below visits them, back out of the stage
+                    __syncwarp();
+                    for (uint32_t i = 0; i < 8; i++) {
+                        const int b = (int)(8 * lane + i) - (int)(256 - nb);
+                        if (b < 0) continue;
+                        const uint32_t valid = min(16u, clen - 16u * (uint32_t)b);
+                        const unsigned long long ma = valid >= 8 ? ~0ull : ((1ull << (8 * valid)) - 1),
+                                                 mb = valid >= 16 ? ~0ull : valid <= 8 ? 0ull : ((1ull << (8 * (valid - 8))) - 1);
+                        cv = crc_block16(sm.crc_slice[ckind - 1], cv,
+                                         *reinterpret_cast<const unsigned long long *>(st + 16 * b) & ma,
+                                         *reinterpret_cast<const unsigned long long *>(st + 16 * b + 8) & mb);
+                    }
+                }
+            }
         } else {
 #pragma unroll 1
             for (uint32_t i = 0; i < 8; i++) {
@@ -539,6 +665,9 @@ __global__ void __launch_bounds__(kWarps * 32) sse_chunk_kernel(const __grid_con
                     // mask to the valid bytes
                     const unsigned long long ma = valid >= 8 ? ~0ull : ((1ull << (8 * valid)) - 1),
                                              mb = valid >= 16 ? ~0ull : valid <= 8 ? 0ull : ((1ull << (8 * (valid - 8))) - 1);
+                    if constexpr (crc) {
+                        if (ckind) cv = crc_block16(sm.crc_slice[ckind - 1], cv, pa & ma, pb & mb);
+                    }
                     const unsigned long long oa = (pa ^ ksa) & ma, ob = (pb ^ ksb) & mb;
                     if (sealing || MODE == kRangeOpen) {
                         *reinterpret_cast<unsigned long long *>(st + kPrefix + 16 * b) = oa;
@@ -563,6 +692,25 @@ __global__ void __launch_bounds__(kWarps * 32) sse_chunk_kernel(const __grid_con
                 yh ^= bswap64(ch);
                 yl ^= bswap64(cl);
                 gf128_mul_h(sm.hh[wid], sm.hl[wid], sm.t.r4, yh, yl);
+            }
+        }
+
+        if constexpr (crc) {
+            // Fold (DESIGN.md 4.12): lane l's slots end at slot j = nb - 8(31 - l) of the chunk, and the chunk's grid at
+            // slot 256c of the block's, so its share of acc = raw(P) * x^(-8 len(P)) is cv * x^(-128 (256c + j)).
+            if (ckind) {
+                const int t = (int)ckind - 1;
+                const uint32_t poly = crc_poly(t);
+                const int j = (int)nb - 8 * (31 - (int)lane);  // <= 0: no slot of the lane holds a byte, cv = 0
+                cv = crc_mul(sm.crc_slot[t][max(j, 0)], cv, poly);
+#pragma unroll
+                for (int o = 16; o; o >>= 1) cv ^= __shfl_xor_sync(0xffffffffu, cv, o);
+                if (lane == 0) {
+                    cv = crc_mul(kCrcDev.chunk[t][c & 255], cv, poly);
+                    for (uint32_t h = c >> 8, i = 0; h; h >>= 1, i++)
+                        if (h & 1) cv = crc_mul(kCrcDev.chunk_hi[t][i], cv, poly);
+                    atomicXor(q.crc_acc + s, cv);  // XOR: the order in which the chunks finish does not matter
+                }
             }
         }
 
@@ -819,6 +967,40 @@ __global__ void __launch_bounds__(256) sse_reseal_verdict_kernel(const __grid_co
             q.dst_blen[x] = q.dst_L[x] = 0;
         } else {
             q.dst_len_out[x] = q.dst_blen[x];
+        }
+    }
+}
+
+// ---- checksums: before and after the kCrc chunk kernel (DESIGN.md 4.12) ------------------------------------------
+// Before (final = 0): zero each block's accumulator, and make a block of unknown kind malformed as an L past the
+// stride makes it -- seal: L = len(B) = 0; reseal (status != NULL, ahead of the verdict): GARAGE_EC_E_INVALID.
+// After (final = 1): crcs[s] = the CRC of a written block with a kind, 0 for every other block.
+struct CrcPassParams {
+    const uint8_t *kind;
+    uint32_t *acc;
+    uint32_t *shard_len;        // L, 0 = not written
+    uint32_t *blen;             // before, seal
+    int32_t *status;            // before, reseal
+    const uint32_t *plain_len;  // after
+    uint32_t *crcs;             // after
+    uint32_t n, final;
+};
+__global__ void __launch_bounds__(256) sse_crc_pass_kernel(const __grid_constant__ CrcPassParams q)
+{
+    for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < q.n; s += gridDim.x * blockDim.x) {
+        const uint32_t k = q.kind[s];
+        if (!q.final) {
+            q.acc[s] = 0;
+            if (k > 2) {
+                if (q.status) {
+                    q.status[s] = -1;  // GARAGE_EC_E_INVALID
+                } else {
+                    q.shard_len[s] = 0;
+                    q.blen[s] = 0;
+                }
+            }
+        } else {
+            q.crcs[s] = k && k <= 2 && q.shard_len[s] ? crc_finish(kCrcDev, (int)k - 1, q.acc[s], q.plain_len[s]) : 0u;
         }
     }
 }

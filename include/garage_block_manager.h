@@ -363,6 +363,17 @@ typedef struct garage_bm_piece {
 } garage_bm_piece;
 int garage_bm_rpc_put_block_resealed(garage_bm *bm, const garage_bm_piece *pieces, int n_pieces, const uint8_t *src_key32,
                                      const uint8_t *dst_key32, uint8_t hash_out[32], uint32_t *stored_len_out);
+/* The two SSE-C writes with the S3 checksum of the block's plaintext (DESIGN.md sections 2.9 and 5.12): crc_kind
+ * GARAGE_EC_CRC_NONE / _CRC32 / _CRC32C, *crc_out = the CRC32 or CRC32C of the plaintext (0 for NONE), computed by the
+ * same GPU call that seals the block -- for a copy that falls back to garage_bm_rpc_get_block, by the retry's -- so the
+ * plaintext still never reaches host memory.  The caller folds the blocks' values into the object's checksum with
+ * garage_ec_crc_combine.  Otherwise exactly garage_bm_rpc_put_block_sealed / _resealed; GARAGE_EC_E_INVALID also for
+ * an unknown kind or a NULL crc_out.                                                                               */
+int garage_bm_rpc_put_block_sealed_crc(garage_bm *bm, const uint8_t *key32, const uint8_t *data, size_t len,
+                                       uint8_t crc_kind, uint8_t hash_out[32], uint32_t *crc_out);
+int garage_bm_rpc_put_block_resealed_crc(garage_bm *bm, const garage_bm_piece *pieces, int n_pieces,
+                                         const uint8_t *src_key32, const uint8_t *dst_key32, uint8_t crc_kind,
+                                         uint8_t hash_out[32], uint32_t *stored_len_out, uint32_t *crc_out);
 void garage_bm_get_reseal_metrics(garage_bm *bm, garage_bm_reseal_metrics *out);
 
 /* Bytes [offset, offset + len) of a block (body_from_blocks_range, src/api/s3/get.rs:650-743; the source range of

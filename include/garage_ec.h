@@ -523,6 +523,52 @@ int garage_ec_reseal_stripes(garage_ec_ctx *ctx, uint8_t *const *src_stripes, co
                              uint32_t *dst_len_out, uint8_t *src_hash_bad, int32_t *src_status, int32_t *status,
                              size_t stride, size_t n_dst);
 
+/* ---- SSE-C CHECKSUMS -- call sites: the Checksummer of PutObject / UploadPart (src/api/s3/put.rs:413-437,
+ * checksum.rs) for an SSE-C object whose checksum is CRC32 or CRC32C, and of CopyObject / UploadPartCopy into an SSE-C
+ * destination (copy.rs:76-79, 143-147, 507-508, 656-658): the S3 checksum of each block's plaintext, computed in the
+ * chunk kernel from the plaintext it already holds, so that it never reaches host memory (DESIGN.md section 2.9 is
+ * normative).  Kinds, one byte per block: GARAGE_EC_CRC_NONE, GARAGE_EC_CRC_CRC32 (zlib's CRC-32, reflected 0xEDB88320)
+ * or GARAGE_EC_CRC_CRC32C (Castagnoli, reflected 0x82F63B78); both init and final XOR 0xFFFFFFFF, the CRC of the empty
+ * string 0.  A batch may mix kinds.  S3 stores the value as its 4 big-endian bytes.
+ *
+ * garage_ec_seal_crc / garage_ec_seal_blocks_crc: garage_ec_seal / garage_ec_seal_blocks plus crc_kind (n bytes, NULL:
+ * no checksums) and crcs (n uint32, required when crc_kind is not NULL).  crcs[s] = the CRC of plaintext block s for
+ * every block with a kind that is written, 0 for every other block; all other outputs are byte-identical to the call
+ * without checksums.  A kind above GARAGE_EC_CRC_CRC32C is refused as the other per-block input errors are: HOST
+ * returns GARAGE_EC_E_INVALID before any GPU work, DEVICE treats the block as malformed (nothing of its shards is
+ * written).  DEVICE: crc_kind and crcs are device memory, crcs 4-byte aligned; still only kernels and stream-ordered
+ * scratch (one 32-bit accumulator per block) are enqueued.  HOST: uploads n more bytes and downloads 4n more.
+ *
+ * garage_ec_reseal_crc / garage_ec_reseal_stripes_crc: the reseal calls with the same two arguments, indexed by
+ * destination: crcs[d] = the CRC of Q_d for a destination with a kind that passes (dst_len_out[d] set); unspecified
+ * otherwise.  An unknown kind: HOST GARAGE_EC_E_INVALID before any GPU work; DEVICE status[d] = GARAGE_EC_E_INVALID.
+ *
+ * garage_ec_crc_combine (host only, no device): *out = CRC(A || B) from crc_a = CRC(A), crc_b = CRC(B) and len_b =
+ * |B| (zlib's crc32_combine; len_b = 0 gives crc_a) -- how a caller folds block checksums into a part's or an
+ * object's.  GARAGE_EC_E_INVALID for a kind other than CRC32 / CRC32C or a NULL out.                                */
+#define GARAGE_EC_CRC_NONE 0
+#define GARAGE_EC_CRC_CRC32 1
+#define GARAGE_EC_CRC_CRC32C 2
+int garage_ec_seal_crc(garage_ec_ctx *ctx, const uint8_t *plain, size_t plain_stride, const uint32_t *plain_len,
+                       const uint8_t *keys, const uint8_t *nonces, uint8_t *shards, size_t stride, uint8_t *hashes,
+                       uint8_t *sums, const uint8_t *crc_kind, uint32_t *crcs, size_t n, int mem_kind, void *cuda_stream);
+int garage_ec_seal_blocks_crc(garage_ec_ctx *ctx, const uint8_t *const *blocks, const uint32_t *plain_len,
+                              const uint8_t *keys, const uint8_t *nonces, uint8_t *shards, size_t stride, uint8_t *hashes,
+                              uint8_t *sums, const uint8_t *crc_kind, uint32_t *crcs, size_t n);
+int garage_ec_reseal_crc(garage_ec_ctx *ctx, uint8_t *src_shards, const uint8_t *src_present, const uint32_t *src_len,
+                         const uint8_t *src_hashes, const uint8_t *src_keys, size_t n_src, const garage_ec_piece *pieces,
+                         const uint32_t *piece_start, const uint8_t *dst_keys, const uint8_t *dst_nonces,
+                         uint8_t *dst_shards, uint8_t *dst_hashes, uint8_t *dst_sums, uint32_t *dst_len_out,
+                         uint8_t *src_hash_bad, int32_t *src_status, int32_t *status, const uint8_t *crc_kind,
+                         uint32_t *crcs, size_t stride, size_t n_dst, int mem_kind, void *cuda_stream);
+int garage_ec_reseal_stripes_crc(garage_ec_ctx *ctx, uint8_t *const *src_stripes, const uint8_t *src_present,
+                                 const uint32_t *src_len, const uint8_t *src_hashes, const uint8_t *src_keys, size_t n_src,
+                                 const garage_ec_piece *pieces, const uint32_t *piece_start, const uint8_t *dst_keys,
+                                 const uint8_t *dst_nonces, uint8_t *dst_shards, uint8_t *dst_hashes, uint8_t *dst_sums,
+                                 uint32_t *dst_len_out, uint8_t *src_hash_bad, int32_t *src_status, int32_t *status,
+                                 const uint8_t *crc_kind, uint32_t *crcs, size_t stride, size_t n_dst);
+int garage_ec_crc_combine(int kind, uint32_t crc_a, uint32_t crc_b, uint64_t len_b, uint32_t *out);
+
 /* ---- utilities used by the harness ------------------------------------------------------
  * device-side synthetic data (same splitmix64 counter stream as the oracle's
  * generator): fills dst[0..len) (device) with stream bytes at `offset`

@@ -221,5 +221,57 @@ impl ErasureCoder {
         if rc != sys::GARAGE_EC_E_AUTH && rc != sys::GARAGE_EC_E_UNRECOVERABLE { check(self.ctx, rc)?; }
         Ok((0..n_dst).map(|d| if status[d] != 0 { Err(status[d]) } else { Ok((hashes[d], lens[d])) }).collect())
     }
+
+    /// seal_blocks, also returning each block's S3 checksum of kind crc_kind[s] (GARAGE_EC_CRC_*; 0 for
+    /// GARAGE_EC_CRC_NONE): read_and_put_blocks' Checksummer for CRC32 / CRC32C, folded by crc_combine.
+    pub fn seal_blocks_crc(&self, blocks: &[&[u8]], keys: Option<(&[[u8; 32]], &[[u8; 8]])>, crc_kind: &[u8],
+                           shards_out: &mut [u8], stride: usize) -> Result<(Vec<[u8; 32]>, Vec<u32>), Error> {
+        let n = blocks.len();
+        assert!(crc_kind.len() == n);
+        let ptrs: Vec<*const u8> = blocks.iter().map(|b| b.as_ptr()).collect();
+        let lens: Vec<u32> = blocks.iter().map(|b| b.len() as u32).collect();
+        let (kp, np) = match keys {
+            Some((k, nn)) => { assert!(k.len() == n && nn.len() == n); (k.as_ptr() as *const u8, nn.as_ptr() as *const u8) }
+            None => (std::ptr::null(), std::ptr::null()),
+        };
+        let (mut hashes, mut crcs) = (vec![[0u8; 32]; n], vec![0u32; n]);
+        let rc = unsafe { sys::garage_ec_seal_blocks_crc(self.ctx, ptrs.as_ptr(), lens.as_ptr(), kp, np,
+                          shards_out.as_mut_ptr(), stride, hashes.as_mut_ptr() as *mut u8, std::ptr::null_mut(),
+                          crc_kind.as_ptr(), crcs.as_mut_ptr(), n) };
+        check(self.ctx, rc)?;
+        Ok((hashes, crcs))
+    }
+
+    /// reseal_stripes, also returning the S3 checksum of kind crc_kind[d] of each destination's plaintext (copies
+    /// into a destination with a CRC32 / CRC32C checksum).
+    pub fn reseal_stripes_crc(&self, stripes: &[*mut u8], present: &[u8], src_len: &[u32], src_hashes: &[[u8; 32]],
+                              src_keys: Option<&[[u8; 32]]>, pieces: &[sys::garage_ec_piece], piece_start: &[u32],
+                              dst_keys: &[[u8; 32]], dst_nonces: &[[u8; 8]], crc_kind: &[u8], shards_out: &mut [u8],
+                              stride: usize) -> Result<Vec<Result<([u8; 32], u32, u32), i32>>, Error> {
+        let (n_src, n_dst) = (stripes.len(), dst_keys.len());
+        assert!(present.len() == n_src * (self.k + self.m) && src_len.len() == n_src && src_hashes.len() == n_src
+                && piece_start.len() == n_dst + 1 && dst_nonces.len() == n_dst && crc_kind.len() == n_dst
+                && shards_out.len() >= n_dst * (self.k + self.m) * stride);
+        assert!(piece_start[n_dst] as usize <= pieces.len());
+        let kp = match src_keys { Some(k) => { assert!(k.len() == n_src); k.as_ptr() as *const u8 } None => std::ptr::null() };
+        let (mut hashes, mut lens, mut crcs) = (vec![[0u8; 32]; n_dst], vec![0u32; n_dst], vec![0u32; n_dst]);
+        let (mut bad, mut src_status, mut status) = (vec![0u8; n_src], vec![0i32; n_src], vec![0i32; n_dst]);
+        let rc = unsafe { sys::garage_ec_reseal_stripes_crc(self.ctx, stripes.as_ptr(), present.as_ptr(),
+                          src_len.as_ptr(), src_hashes.as_ptr() as *const u8, kp, n_src, pieces.as_ptr(),
+                          piece_start.as_ptr(), dst_keys.as_ptr() as *const u8, dst_nonces.as_ptr() as *const u8,
+                          shards_out.as_mut_ptr(), hashes.as_mut_ptr() as *mut u8, std::ptr::null_mut(),
+                          lens.as_mut_ptr(), bad.as_mut_ptr(), src_status.as_mut_ptr(), status.as_mut_ptr(),
+                          crc_kind.as_ptr(), crcs.as_mut_ptr(), stride, n_dst) };
+        if rc != sys::GARAGE_EC_E_AUTH && rc != sys::GARAGE_EC_E_UNRECOVERABLE { check(self.ctx, rc)?; }
+        Ok((0..n_dst).map(|d| if status[d] != 0 { Err(status[d]) } else { Ok((hashes[d], lens[d], crcs[d])) }).collect())
+    }
+
+    /// CRC(A || B) from CRC(A), CRC(B) and |B| (host only): folds block checksums, in order, into a part's.
+    pub fn crc_combine(kind: u8, crc_a: u32, crc_b: u32, len_b: u64) -> Result<u32, Error> {
+        let mut out = 0u32;
+        let rc = unsafe { sys::garage_ec_crc_combine(kind as i32, crc_a, crc_b, len_b, &mut out) };
+        if rc != sys::GARAGE_EC_OK { return Err(Error::Message(format!("garage_ec_crc_combine: {}", rc))); }
+        Ok(out)
+    }
 }
 impl Drop for ErasureCoder { fn drop(&mut self) { unsafe { sys::garage_ec_destroy(self.ctx) } } }

@@ -20,6 +20,9 @@ pub const GARAGE_EC_VANDERMONDE: c_int = 0;
 pub const GARAGE_EC_CAUCHY: c_int = 1;
 pub const GARAGE_EC_MEM_HOST: c_int = 0;
 pub const GARAGE_EC_MEM_DEVICE: c_int = 1;
+pub const GARAGE_EC_CRC_NONE: u8 = 0;
+pub const GARAGE_EC_CRC_CRC32: u8 = 1;
+pub const GARAGE_EC_CRC_CRC32C: u8 = 2;
 
 #[link(name = "garage_ec")]
 extern "C" {
@@ -103,6 +106,29 @@ extern "C" {
                                     dst_nonces: *const u8, dst_shards: *mut u8, dst_hashes: *mut u8, dst_sums: *mut u8,
                                     dst_len_out: *mut u32, src_hash_bad: *mut u8, src_status: *mut i32,
                                     status: *mut i32, stride: usize, n_dst: usize) -> c_int;
+    pub fn garage_ec_seal_crc(ctx: *mut garage_ec_ctx, plain: *const u8, plain_stride: usize, plain_len: *const u32,
+                              keys: *const u8, nonces: *const u8, shards: *mut u8, stride: usize, hashes: *mut u8,
+                              sums: *mut u8, crc_kind: *const u8, crcs: *mut u32, n: usize, mem_kind: c_int,
+                              stream: *mut c_void) -> c_int;
+    pub fn garage_ec_seal_blocks_crc(ctx: *mut garage_ec_ctx, blocks: *const *const u8, plain_len: *const u32,
+                                     keys: *const u8, nonces: *const u8, shards: *mut u8, stride: usize,
+                                     hashes: *mut u8, sums: *mut u8, crc_kind: *const u8, crcs: *mut u32,
+                                     n: usize) -> c_int;
+    pub fn garage_ec_reseal_crc(ctx: *mut garage_ec_ctx, src_shards: *mut u8, src_present: *const u8,
+                                src_len: *const u32, src_hashes: *const u8, src_keys: *const u8, n_src: usize,
+                                pieces: *const garage_ec_piece, piece_start: *const u32, dst_keys: *const u8,
+                                dst_nonces: *const u8, dst_shards: *mut u8, dst_hashes: *mut u8, dst_sums: *mut u8,
+                                dst_len_out: *mut u32, src_hash_bad: *mut u8, src_status: *mut i32, status: *mut i32,
+                                crc_kind: *const u8, crcs: *mut u32, stride: usize, n_dst: usize, mem_kind: c_int,
+                                stream: *mut c_void) -> c_int;
+    pub fn garage_ec_reseal_stripes_crc(ctx: *mut garage_ec_ctx, src_stripes: *const *mut u8, src_present: *const u8,
+                                        src_len: *const u32, src_hashes: *const u8, src_keys: *const u8, n_src: usize,
+                                        pieces: *const garage_ec_piece, piece_start: *const u32, dst_keys: *const u8,
+                                        dst_nonces: *const u8, dst_shards: *mut u8, dst_hashes: *mut u8,
+                                        dst_sums: *mut u8, dst_len_out: *mut u32, src_hash_bad: *mut u8,
+                                        src_status: *mut i32, status: *mut i32, crc_kind: *const u8, crcs: *mut u32,
+                                        stride: usize, n_dst: usize) -> c_int;
+    pub fn garage_ec_crc_combine(kind: c_int, crc_a: u32, crc_b: u32, len_b: u64, out: *mut u32) -> c_int;
     pub fn garage_ec_strerror(code: c_int) -> *const c_char;
     pub fn garage_ec_last_error(ctx: *const garage_ec_ctx) -> *const c_char;
     pub fn garage_ec_abi_version() -> c_int;
