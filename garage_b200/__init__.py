@@ -34,7 +34,7 @@ ABI_SYMBOLS = [
     "garage_ec_launch_count", "garage_ec_set_timing", "garage_ec_timing_read",
     "garage_ec_shard_sums", "garage_ec_check_sums", "garage_ec_blake2sum",
     "garage_ec_encode_blocks_with_sums", "garage_ec_scrub_repair",
-    "garage_ec_numa_info", "garage_ec_bind_thread", "garage_ec_debug_fail_after",
+    "garage_ec_numa_info", "garage_ec_bind_thread", "garage_ec_device_count", "garage_ec_debug_fail_after",
     "garage_ec_set_sum_kind", "garage_ec_set_wait_mode", "garage_ec_copy_for_dma", "garage_ec_shard_sum_host", "garage_ec_reconstruct_stripes",
     "garage_ec_create_lrc", "garage_ec_code_info", "garage_ec_read_set",
     "garage_ec_create_piggyback", "garage_ec_piggyback_info", "garage_ec_code_shard_len", "garage_ec_read_plan",
@@ -117,6 +117,7 @@ def load_library(build=True):
     L.garage_ec_timing_read.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(u64)]
     L.garage_ec_numa_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32)]
     L.garage_ec_bind_thread.argtypes = [vp]
+    L.garage_ec_device_count.argtypes = []
     L.garage_ec_debug_fail_after.argtypes = [vp, C.c_long]
     L.garage_ec_reconstruct_stripes.argtypes = [vp, vp, vp, vp, vp, vp, sz, sz]
     L.garage_ec_set_sum_kind.argtypes = [vp, i32]

@@ -28,7 +28,9 @@ SYMBOLS = [
     "garage_bm_rpc_get_block_range_opened", "garage_bm_get_sealed_range_metrics",
     "garage_bm_rpc_put_block_resealed", "garage_bm_get_reseal_metrics",
     "garage_bm_rpc_put_block_sealed_crc", "garage_bm_rpc_put_block_resealed_crc",
+    "garage_bm_create_on_devices", "garage_bm_get_device_metrics",
 ]
+MAX_DEVICES = 16
 MAX_PIECES = 64
 CRC_NONE, CRC32, CRC32C = 0, 1, 2  # checksum kinds of the _crc writes (DESIGN.md 2.9)
 SUM_BLAKE2, SUM_ADLER8 = 0, 1
@@ -130,6 +132,12 @@ class ResealMetrics(C.Structure):
         "calls", "batches", "sources_gathered", "bytes_read", "auth_failures", "fallbacks", "call_us", "reseal_call_us")]
 
 
+class DeviceMetrics(C.Structure):
+    """garage_bm_device_metrics: one dispatcher group"""
+    _fields_ = [("cuda_device", C.c_int), ("numa_node", C.c_int)] + [(n, C.c_uint64) for n in (
+        "batches", "blocks", "bytes", "routed_local", "routed_remote")] + [("pool_numa_node", C.c_int)]
+
+
 class Piece(C.Structure):
     """garage_bm_piece: plaintext bytes [offset, offset + len) of stored block `hash`"""
     _fields_ = [("hash", C.c_uint8 * 32), ("offset", C.c_uint32), ("len", C.c_uint32)]
@@ -207,6 +215,9 @@ def load_library():
         L.garage_bm_get_stripe_repair_metrics.argtypes = [vp, C.POINTER(StripeRepairMetrics)]
         L.garage_bm_get_stripe_repair_metrics.restype = None
         L.garage_bm_create_with_drives.argtypes = [C.POINTER(vp), C.POINTER(Config), C.POINTER(DataDir), i32]
+        L.garage_bm_create_on_devices.argtypes = [C.POINTER(vp), C.POINTER(Config), C.POINTER(DataDir), i32,
+                                                  C.POINTER(C.c_int), i32]
+        L.garage_bm_get_device_metrics.argtypes = [vp, C.POINTER(DeviceMetrics), i32, C.POINTER(i32)]
         L.garage_bm_set_data_dirs.argtypes = [vp, i32, C.POINTER(DataDir), i32]
         L.garage_bm_rebalance_step.argtypes = [vp, i32, vp, sz, vp, C.POINTER(i32), C.POINTER(C.c_uint64)]
         L.garage_bm_get_drive_metrics.argtypes = [vp, C.POINTER(DriveMetrics)]
@@ -256,7 +267,7 @@ class BlockManager:
     def __init__(self, k=10, m=4, n_nodes=None, cuda_device=0, batch_max_blocks=64, batch_linger_us=100,
                  block_ram_buffer_max=256 << 20, data_dir=None, shard_sum_kind=SUM_ADLER8, verify_content_hash=True,
                  data_fsync=False, block_gc_delay_ms=0, local_groups=0, piggyback=False, previous_codes=(),
-                 legacy_replicas=0, layout=None, clay=False, clay_layout=False, data_dirs=None):
+                 legacy_replicas=0, layout=None, clay=False, clay_layout=False, data_dirs=None, cuda_devices=None):
         """block_gc_delay_ms defaults to 0 HERE (tests delete at once); the library's default is the
         reference's BLOCK_GC_DELAY of 10 minutes.  local_groups > 0: LRC(k, local_groups, m - local_groups).
         piggyback: PB(k, m), half-shard repair reads.  clay: Clay(k, m), a lost shard rebuilt from 1/m of the others; clay_layout: that store may change its
@@ -264,7 +275,8 @@ class BlockManager:
         layout: None (partition p on nodes (p mod n_nodes) + i) or a dict with zone, capacity and optionally
         zone_redundancy, max_per_zone: version 1 of the cluster layout.  data_dirs: None (one directory per node) or a list
         of (path, capacity[, read_only]) tuples or {path, capacity, read_only} dicts, paths relative to each node's
-        directory: the drives every node spreads its files over."""
+        directory: the drives every node spreads its files over.  cuda_devices: None (cuda_device alone) or the list of
+        devices to run one dispatcher group each on (garage_bm_create_on_devices; a device may repeat)."""
         self._L = load_library()
         cfg = Config()
         self._L.garage_bm_default_config(C.byref(cfg))
@@ -287,7 +299,11 @@ class BlockManager:
             self._spec, self._spec_arrays = _layout_spec(**layout)  # kept alive
             cfg.layout = C.pointer(self._spec)
         h = C.c_void_p()
-        if data_dirs is None:
+        if cuda_devices is not None:
+            devs = (C.c_int * max(1, len(cuda_devices)))(*map(int, cuda_devices))
+            drives, n = _data_dirs(data_dirs) if data_dirs is not None else (None, 0)
+            rc = self._L.garage_bm_create_on_devices(C.byref(h), C.byref(cfg), drives, n, devs, len(cuda_devices))
+        elif data_dirs is None:
             rc = self._L.garage_bm_create(C.byref(h), C.byref(cfg))
         else:
             drives, n = _data_dirs(data_dirs)
@@ -562,6 +578,15 @@ class BlockManager:
             assert finished
             total += n
         return total
+
+    def device_metrics(self):
+        """one dict per dispatcher group, in the order the devices were listed"""
+        n = C.c_int(0)
+        arr = (DeviceMetrics * MAX_DEVICES)()
+        rc = self._L.garage_bm_get_device_metrics(self._h, arr, MAX_DEVICES, C.byref(n))
+        if rc != OK:
+            raise BlockManagerError(rc)
+        return [{f: getattr(arr[i], f) for f, _ in DeviceMetrics._fields_} for i in range(n.value)]
 
     def drive_metrics(self):
         mt = DriveMetrics()

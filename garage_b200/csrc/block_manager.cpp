@@ -34,6 +34,7 @@
 #include <memory>
 #include <mutex>
 #include <new>
+#include <numeric>
 #include <random>
 #include <set>
 #include <string>
@@ -46,6 +47,7 @@
 #include <sys/mman.h>
 #include <sys/random.h>
 #include <sys/stat.h>
+#include <sys/syscall.h>
 #include <unistd.h>
 
 namespace {
@@ -1581,6 +1583,61 @@ struct PinnedBuf {
     ~PinnedBuf() { release(); }
 };
 
+// Everything one listed device runs (DESIGN.md section 5.13): the dispatcher contexts and threads of both batchers,
+// one context per code for the sweeps' own calls, and the pinned memory its callers land blocks and stripes in,
+// allocated on the device's NUMA node.  A call routed to a group takes its slots from the group's pools and submits to
+// its batchers only, so a batch never spans devices.
+struct DeviceGroup {
+    static constexpr int kWorkers = 3;  // dispatcher threads per batcher (overlap PCIe / GPU / collection)
+    static constexpr int kEncBufs = 4;  // pinned output buffers per dispatcher: a batch's callers store their shards
+                                        // out of one while the dispatcher fills the next ones
+    int device = 0;
+    int numa_node = -1;  // the GPU's node (garage_ec_numa_info), -1 = unknown
+    int pool_node = -1;  // the node its pools landed on
+    garage_ec_ctx *enc_ctx[kWorkers] = {nullptr};  // one context (= its own staging lanes) per worker
+    garage_ec_ctx *rec_ctx[kWorkers] = {nullptr};
+    std::vector<garage_ec_ctx *> code_ctx;  // per code of garage_bm::codes; the first group's are the codes' own
+    SlotPool put_slots;     // one block each
+    SlotPool stripe_slots;  // (k+m) x slot_stride each: degraded GETs, resync workers
+    EncBatchBuf enc_out[kWorkers][kEncBufs];
+    int enc_next[kWorkers] = {0};
+    std::unique_ptr<Batcher<EncodeItem>> enc_batcher;
+    std::unique_ptr<Batcher<ReconItem>> rec_batcher;
+    PinnedBuf scrub_buf;
+    std::mutex scrub_mu;
+    PinnedBuf deep_buf;  // the deep scrub's batch of stripes (not stripe_slots: DESIGN.md section 5.2's pool rule)
+    std::mutex deep_mu;
+    PinnedBuf conv_src, conv_dst, conv_blk;  // a conversion batch: old shards / replicas in, new shards + tags out
+    std::mutex rebuild_mu;                   // garage_bm::rebuild_batch: one batch of the pool at a time
+    std::atomic<uint64_t> queued{0};         // calls routed here that have not returned
+    std::atomic<uint64_t> batches{0}, blocks{0}, bytes{0}, routed_local{0}, routed_remote{0};
+    void count(size_t n_blocks, uint64_t n_bytes)  // one GPU call of the group
+    {
+        batches++;
+        blocks += n_blocks;
+        bytes += n_bytes;
+    }
+    // threads and pinned memory, before the contexts they use are destroyed
+    void stop()
+    {
+        enc_batcher.reset();
+        rec_batcher.reset();
+        for (auto &w : enc_out)
+            for (auto &eb : w) eb.release();
+        for (PinnedBuf *b : {&scrub_buf, &deep_buf, &conv_src, &conv_dst, &conv_blk}) b->release();
+        put_slots.destroy();
+        stripe_slots.destroy();
+    }
+};
+
+// The group the calling thread's GPU work goes to: set by garage_bm::Route for the length of one call, and for good
+// in a group's dispatcher threads.  Keyed by the manager, as one process may run several.
+struct RouteTls {
+    const void *bm = nullptr;
+    DeviceGroup *g = nullptr;
+};
+thread_local RouteTls tl_route;
+
 struct RcEntry {
     int64_t count = 0;
     Clock::time_point zero_since{};  // when the count last dropped to 0 (BLOCK_GC_DELAY, manager.rs:49-52)
@@ -1612,12 +1669,52 @@ struct garage_bm {
     int k = 0, m = 0, tot = 0;
     int sum_kind = GARAGE_EC_SUM_ADLER8;
     size_t slot_stride = 0;  // stride of the largest block's shards: geometry of every stripe slot
-    static constexpr int kWorkers = 3;  // dispatcher threads per batcher (overlap PCIe / GPU / collection)
-    garage_ec_ctx *ec = nullptr;                   // scrub + geometry helpers
-    garage_ec_ctx *enc_ctx[kWorkers] = {nullptr};  // one context (= its own staging lanes) per worker
-    garage_ec_ctx *rec_ctx[kWorkers] = {nullptr};
-    SlotPool put_slots;     // one block each
-    SlotPool stripe_slots;  // (k+m) x slot_stride each: degraded GETs, resync workers
+    // one group per listed device, in list order (DESIGN.md section 5.13)
+    std::vector<std::unique_ptr<DeviceGroup>> groups;
+    std::atomic<uint64_t> route_rr{0};  // round robin among equally loaded candidates
+
+    // The routing rule: the groups whose GPU is on the calling thread's NUMA node (getcpu(2)) are the candidates, all
+    // groups if none is; the candidate with the fewest calls in flight wins, ties going round robin.
+    DeviceGroup &pick_group()
+    {
+        unsigned cpu = 0, node = 0;
+        const int here = syscall(SYS_getcpu, &cpu, &node, nullptr) == 0 ? (int)node : -1;
+        bool local = false;
+        for (const auto &g : groups) local = local || (here >= 0 && g->numa_node == here);
+        const size_t n = groups.size(), start = (size_t)(route_rr++ % n);
+        DeviceGroup *best = nullptr;
+        for (size_t i = 0; i < n; i++) {
+            DeviceGroup &g = *groups[(start + i) % n];
+            if (local && g.numa_node != here) continue;
+            if (!best || g.queued.load() < best->queued.load()) best = &g;
+        }
+        (local ? best->routed_local : best->routed_remote)++;
+        return *best;
+    }
+    // Every call that reaches the GPU holds one: it routes the calling thread for the length of the call, so the
+    // call's slots, batches and sweep buffers all come from one group.  A call made inside another (a GET's fallback,
+    // a resync of a layout sync) keeps the outer call's group.
+    struct Route {
+        RouteTls saved;
+        bool own;
+        explicit Route(garage_bm &bm) : saved(tl_route), own(tl_route.bm != &bm)
+        {
+            if (!own) return;
+            DeviceGroup &g = bm.pick_group();
+            g.queued++;
+            tl_route = {&bm, &g};
+        }
+        ~Route()
+        {
+            if (!own) return;
+            tl_route.g->queued--;
+            tl_route = saved;
+        }
+        Route(const Route &) = delete;
+        Route &operator=(const Route &) = delete;
+    };
+    // the calling thread's group: its Route's, its dispatcher's, else the first
+    DeviceGroup &grp() const { return tl_route.bm == this ? *tl_route.g : *groups[0]; }
     std::vector<std::unique_ptr<Node>> nodes;
     // stands in for the block_ref / rc tables (src/model/s3/block_ref_table.rs, src/block/rc.rs):
     // which blocks exist and how long they are.  Lock order: refs_mu before any Node::mu.
@@ -1627,16 +1724,6 @@ struct garage_bm {
     // block_decref have an entry; a block without entry is treated as needed (rc > 0)
     std::unordered_map<Hash, RcEntry, HashHasher> rc;
     std::unique_ptr<ByteSemaphore> ram;
-    std::unique_ptr<Batcher<EncodeItem>> enc_batcher;
-    std::unique_ptr<Batcher<ReconItem>> rec_batcher;
-    static constexpr int kEncBufs = 4;  // pinned output buffers per dispatcher: a batch's callers store their shards
-                                        // out of one while the dispatcher fills the next ones
-    EncBatchBuf enc_out[kWorkers][kEncBufs];
-    int enc_next[kWorkers] = {0};
-    PinnedBuf scrub_buf;
-    std::mutex scrub_mu;
-    PinnedBuf deep_buf;  // the deep scrub's batch of stripes (not stripe_slots: DESIGN.md section 5.2's pool rule)
-    std::mutex deep_mu;
     std::atomic<uint64_t> deep_blocks{0}, deep_skipped{0}, deep_parity_bad{0}, deep_content_errors{0}, deep_check_us{0};
     std::atomic<bool> warmed{false};
     // metrics (src/block/metrics.rs)
@@ -1680,8 +1767,9 @@ struct garage_bm {
         for (size_t i = 0; i < n; i++) b += runs[i].len;
         return b;
     }
-    // codes[0]: the configured code (ctx = ec); codes[1..]: garage_bm_config.previous_codes, one context each.  Shard i
-    // of every code lives on the i-th node of the block's ring row.
+    // codes[0]: the configured code; codes[1..]: garage_bm_config.previous_codes, one context each, on the
+    // first listed device (each group has its own for its GPU calls).  Shard i of every code lives on the i-th node of
+    // the block's ring row.
     struct Code : CodeDesc {
         int tot = 0;
         garage_ec_ctx *ctx = nullptr;
@@ -1699,8 +1787,7 @@ struct garage_bm {
         }
         return true;
     }
-    std::mutex convert_mu;         // one conversion batch at a time (owns the pinned batch buffers)
-    PinnedBuf conv_src, conv_dst, conv_blk;  // old shards / replicas in, new shards + tags out, one block
+    std::mutex convert_mu;         // one conversion batch at a time (in its group's pinned batch buffers)
     size_t shard_len_of(uint32_t block_len, int code = 0) const
     {
         uint32_t L = 0;  // a length that does not fit in 32 bits is larger than any slot: every caller rejects it
@@ -1933,7 +2020,7 @@ struct garage_bm {
                 *sums = hashes ? hashes + n * 32 : nullptr;
         const auto t0 = Clock::now();
         if (rc == GARAGE_EC_OK)
-            rc = garage_ec_seal_blocks_crc(enc_ctx[w], ptrs.data(), lens.data(), keyed ? keys.data() : nullptr,
+            rc = garage_ec_seal_blocks_crc(grp().enc_ctx[w], ptrs.data(), lens.data(), keyed ? keys.data() : nullptr,
                                            keyed ? nonces.data() : nullptr, sh, stride, hashes, sums, kinds.data(),
                                            crcs.data(), n);
         seal_call_us += us_since(t0);
@@ -1957,7 +2044,12 @@ struct garage_bm {
     {
         // sealed PUTs go to their own calls, as run_reconstruct keeps ranged GETs apart
         std::vector<EncodeItem *> b, keyed, unkeyed;
-        for (EncodeItem *it : all) (it->sealed ? (it->key ? keyed : unkeyed) : b).push_back(it);
+        uint64_t bytes = 0;
+        for (EncodeItem *it : all) {
+            (it->sealed ? (it->key ? keyed : unkeyed) : b).push_back(it);
+            bytes += it->len;
+        }
+        grp().count(all.size(), bytes);
         if (!keyed.empty()) run_seal(w, keyed, true);
         if (!unkeyed.empty()) run_seal(w, unkeyed, false);
         if (b.empty()) return;
@@ -1971,14 +2063,15 @@ struct garage_bm {
             max_len = std::max(max_len, b[i]->len);
         }
         const size_t stride = garage_ec_stride_for((uint32_t)shard_len_of(max_len));
-        EncBatchBuf &bb = enc_out[w][enc_next[w] = (enc_next[w] + 1) % kEncBufs];
+        DeviceGroup &g = grp();
+        EncBatchBuf &bb = g.enc_out[w][g.enc_next[w] = (g.enc_next[w] + 1) % DeviceGroup::kEncBufs];
         bb.wait_idle();  // the callers of the batch that last used this buffer have stored their shards
         uint8_t *par = bb.get(n * m * stride + n * tot * 32);
         int rc = par ? GARAGE_EC_OK : GARAGE_EC_E_NOMEM;
         uint8_t *sums = par ? par + n * m * stride : nullptr;
         const auto t0 = Clock::now();
         if (rc == GARAGE_EC_OK)
-            rc = garage_ec_encode_blocks_with_sums(enc_ctx[w], ptrs.data(), lens.data(), n, par, sums, stride);
+            rc = garage_ec_encode_blocks_with_sums(g.enc_ctx[w], ptrs.data(), lens.data(), n, par, sums, stride);
         enc_gpu_us += us_since(t0);
         if (rc == GARAGE_EC_OK) bb.set_pending((int)n);
         for (size_t i = 0; i < n; i++) {
@@ -1997,7 +2090,15 @@ struct garage_bm {
     void run_reconstruct(int w, std::vector<ReconItem *> &all)
     {
         std::vector<ReconItem *> by_kind[ReconItem::kKinds];
-        for (ReconItem *it : all) by_kind[it->kind].push_back(it);
+        uint64_t bytes = 0;
+        for (ReconItem *it : all) {
+            by_kind[it->kind].push_back(it);
+            if (it->reseal)
+                for (uint32_t l : it->reseal->src_len) bytes += l;
+            else
+                bytes += it->block_len;
+        }
+        grp().count(all.size(), bytes);
         for (auto &b : by_kind)
             if (!b.empty()) run_kind(w, b);
     }
@@ -2049,7 +2150,7 @@ struct garage_bm {
                 memcpy(want.data() + i * tot, b[i]->want, tot);
             }
             const auto t0 = Clock::now();
-            rc = garage_ec_reconstruct_stripes(rec_ctx[w], stripes.data(), present.data(), want.data(), status.data(),
+            rc = garage_ec_reconstruct_stripes(grp().rec_ctx[w], stripes.data(), present.data(), want.data(), status.data(),
                                                blen.data(), slot_stride, n);
             const uint64_t us = us_since(t0);
             rec_gpu_us += us;
@@ -2063,7 +2164,7 @@ struct garage_bm {
         }
         case ReconItem::kRange: {
             const auto t0 = Clock::now();
-            rc = garage_ec_decode_range_stripes(rec_ctx[w], stripes.data(), present.data(), blen.data(), offs.data(),
+            rc = garage_ec_decode_range_stripes(grp().rec_ctx[w], stripes.data(), present.data(), blen.data(), offs.data(),
                                                 lens.data(), slot_stride, outs.data(), status.data(), n);
             rec_gpu_us += us_since(t0);
             fulfil(rc == GARAGE_EC_OK || rc == GARAGE_EC_E_UNRECOVERABLE,
@@ -2076,7 +2177,7 @@ struct garage_bm {
             for (size_t i = 0; i < n; i++) memcpy(hashes.data() + i * 32, b[i]->hash.data(), 32);
             pack_keys();
             const auto t0 = Clock::now();
-            rc = garage_ec_open_stripes(rec_ctx[w], stripes.data(), present.data(), blen.data(), hashes.data(), keys.data(),
+            rc = garage_ec_open_stripes(grp().rec_ctx[w], stripes.data(), present.data(), blen.data(), hashes.data(), keys.data(),
                                         outs.data(), plen.data(), bad.data(), status.data(), slot_stride, n);
             open_call_us += us_since(t0);
             wipe_secret(keys.data(), keys.size());
@@ -2094,7 +2195,7 @@ struct garage_bm {
         case ReconItem::kOpenRange: {
             pack_keys();
             const auto t0 = Clock::now();
-            rc = garage_ec_open_range_stripes(rec_ctx[w], stripes.data(), present.data(), blen.data(), keys.data(),
+            rc = garage_ec_open_range_stripes(grp().rec_ctx[w], stripes.data(), present.data(), blen.data(), keys.data(),
                                               offs.data(), lens.data(), slot_stride, outs.data(), status.data(), n);
             sealed_range_call_us += us_since(t0);
             wipe_secret(keys.data(), keys.size());
@@ -2141,7 +2242,7 @@ struct garage_bm {
         std::vector<uint8_t> bad(ns, 0);
         std::vector<int32_t> sst(ns, 0), st(n, 0);
         const auto t0 = Clock::now();
-        const int rc = garage_ec_reseal_stripes_crc(rec_ctx[w], stripes.data(), present.data(), slen.data(),
+        const int rc = garage_ec_reseal_stripes_crc(grp().rec_ctx[w], stripes.data(), present.data(), slen.data(),
                                                     shash.data(), keyed ? skeys.data() : nullptr, ns, pieces.data(),
                                                     start.data(), dkeys.data(), nonces.data(), dsh, dhash, dsums,
                                                     dlen.data(), bad.data(), sst.data(), st.data(), kinds.data(),
@@ -2357,8 +2458,10 @@ struct garage_bm {
             const uint32_t L = (uint32_t)shard_len_of(block_len, code);
             int32_t st = 0;
             const auto t0 = Clock::now();
-            int rc = garage_ec_reconstruct_stripes(codes[code].ctx, &slot, have, want, &st, &L, slot_stride, 1);
+            DeviceGroup &g = grp();
+            int rc = garage_ec_reconstruct_stripes(g.code_ctx[code], &slot, have, want, &st, &L, slot_stride, 1);
             rec_gpu_us += us_since(t0);
+            g.count(1, block_len);
             if (rc == GARAGE_EC_OK || rc == GARAGE_EC_E_UNRECOVERABLE) rc = st ? GARAGE_BM_E_MISSING_BLOCK : GARAGE_BM_OK;
             return rc;
         }
@@ -2367,7 +2470,7 @@ struct garage_bm {
         it.block_len = block_len;
         memcpy(it.present, have, tot);
         memcpy(it.want, want, tot);
-        return rec_batcher->submit(it);
+        return grp().rec_batcher->submit(it);
     }
 
     void assemble(const uint8_t *slot, uint32_t block_len, uint8_t *out, int code = 0) const
@@ -2390,17 +2493,18 @@ struct garage_bm {
 
     int rpc_put_block(const Hash &h, const uint8_t *data, size_t len)
     {
+        Route route(*this);
         if (len == 0 || len > cfg.block_size) return GARAGE_BM_E_MESSAGE;  // blocks are at most block_size (put.rs:583-617)
         // DataBlock::from_buffer (manager.rs:376): compression is 'none' in this mirror
         ByteLease permit(*ram, (uint64_t)len * tot / k);  // manager.rs:380-385, x (k+m)/k for the parity
         put_calls++;
         // land the block in pinned memory (caller's thread, so copies of concurrent PUTs overlap)
-        SlotLease slot(put_slots);
+        SlotLease slot(grp().put_slots);
         copy_for_dma(slot.p, data, len);  // landing copy: the GPU reads the slot next
         EncodeItem it;
         it.data = slot.p;
         it.len = (uint32_t)len;
-        int rc = enc_batcher->submit(it);
+        int rc = grp().enc_batcher->submit(it);
         if (rc != GARAGE_EC_OK) return rc;
         struct BufRelease {
             EncBatchBuf *b;
@@ -2447,11 +2551,12 @@ struct garage_bm {
     int rpc_put_block_sealed(const uint8_t *key, const uint8_t *data, size_t len, uint8_t *hash_out,
                              uint8_t crc_kind = GARAGE_EC_CRC_NONE, uint32_t *crc_out = nullptr)
     {
+        Route route(*this);
         if (len > cfg.block_size || (!key && len == 0)) return GARAGE_BM_E_MESSAGE;
         uint32_t blen = (uint32_t)len;
         if (key && garage_ec_sealed_len((uint32_t)len, &blen) != GARAGE_EC_OK) return GARAGE_BM_E_MESSAGE;
         ByteLease permit(*ram, (uint64_t)blen * tot / k);
-        SlotLease slot(put_slots);
+        SlotLease slot(grp().put_slots);
         if (len) copy_for_dma(slot.p, data, len);
         EncodeItem it;
         it.data = slot.p;
@@ -2464,7 +2569,7 @@ struct garage_bm {
             if (r < 0 && errno != EINTR) return GARAGE_BM_E_MESSAGE;
             if (r > 0) got += (size_t)r;
         }
-        const int rc = enc_batcher->submit(it);
+        const int rc = grp().enc_batcher->submit(it);
         if (rc != GARAGE_EC_OK) return rc;
         sealed_puts++;
         memcpy(hash_out, it.hash.data(), 32);
@@ -2487,6 +2592,7 @@ struct garage_bm {
                                uint8_t *hash_out, uint32_t *stored_len_out, uint8_t crc_kind = GARAGE_EC_CRC_NONE,
                                uint32_t *crc_out = nullptr)
     {
+        Route route(*this);
         const auto t0 = Clock::now();
         struct AddTime {
             std::atomic<uint64_t> &c;
@@ -2567,7 +2673,7 @@ struct garage_bm {
             ReconItem it;
             it.kind = ReconItem::kReseal;
             it.reseal = &J;
-            rc = rec_batcher->submit(it);
+            rc = grp().rec_batcher->submit(it);
             if (rc != GARAGE_EC_E_UNRECOVERABLE || attempt) break;
             // a source that does not hash to its address, or that its stripe cannot rebuild: once through rpc_get_block
             bool again = false;
@@ -2606,7 +2712,7 @@ struct garage_bm {
         it.key = key;
         it.hash = h;
         it.out = out;
-        const int rc = rec_batcher->submit(it);
+        const int rc = grp().rec_batcher->submit(it);
         if (rc == GARAGE_BM_OK) {
             opened_gets++;
             *out_len = it.plain_len;
@@ -2622,8 +2728,9 @@ struct garage_bm {
     // through rpc_get_block, with its stale-shard hunt, and the block it returns is opened.
     int rpc_get_block_opened(const Hash &h, const uint8_t *key, uint8_t *out, size_t cap, size_t *out_len)
     {
+        Route route(*this);
         {
-            SlotLease slot(stripe_slots);
+            SlotLease slot(grp().stripe_slots);
             uint8_t have[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
             uint32_t block_len = 0;
             bool ok = false;
@@ -2638,7 +2745,7 @@ struct garage_bm {
         size_t blen = 0;
         int rc = rpc_get_block(h, blk.data(), blk.size(), &blen);
         if (rc != GARAGE_BM_OK) return rc;
-        SlotLease slot(stripe_slots);
+        SlotLease slot(grp().stripe_slots);
         uint8_t have[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
         const size_t L = shard_len_of((uint32_t)blen);
         for (int j = 0; j < k; j++) {
@@ -2675,6 +2782,7 @@ struct garage_bm {
     // manager.rs:344-363 + 276-339.  `out` must hold stored_max() bytes (a sealed block_size block); *out_len = the block's length.
     int rpc_get_block(const Hash &h, uint8_t *out, size_t cap, size_t *out_len)
     {
+        Route route(*this);
         const int rc = get_from_stripe(h, out, cap, out_len, 0);
         if (rc == GARAGE_BM_OK || !has_legacy()) return rc;
         // the configured stripe cannot serve it (yet): a block stored before the code changed
@@ -2802,7 +2910,7 @@ struct garage_bm {
         it.off = off;
         it.len = len;
         it.out = out;
-        return rec_batcher->submit(it);
+        return grp().rec_batcher->submit(it);
     }
 
     // Bytes [off, off + len) of block h into out (S3 GetObject with a Range header, body_from_blocks_range; the
@@ -2815,12 +2923,13 @@ struct garage_bm {
     // previous code or as replicas, which is then sliced.
     int rpc_get_block_range(const Hash &h, uint32_t off, uint32_t len, uint8_t *out, size_t cap, size_t *out_len)
     {
+        Route route(*this);
         range_gets++;
         uint8_t present[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
         uint32_t block_len = 0;
         int gpu = 0;
         {
-            SlotLease slot(stripe_slots);
+            SlotLease slot(grp().stripe_slots);
             const int rc = gather_ranged(
                 h, slot.p,
                 [&](uint32_t bl) -> int {
@@ -2860,6 +2969,7 @@ struct garage_bm {
     int rpc_get_block_range_opened(const Hash &h, const uint8_t *key, uint32_t off, uint32_t len, uint8_t *out,
                                    size_t cap, size_t *out_len)
     {
+        Route route(*this);
         struct Timer {
             std::atomic<uint64_t> &us;
             Clock::time_point t0;
@@ -2870,7 +2980,7 @@ struct garage_bm {
         uint32_t block_len = 0;
         int gpu = 0, rc;
         {
-            SlotLease slot(stripe_slots);
+            SlotLease slot(grp().stripe_slots);
             rc = gather_ranged(
                 h, slot.p,
                 [&](uint32_t bl) -> int {
@@ -2934,7 +3044,7 @@ struct garage_bm {
     int get_from_stripe(const Hash &h, uint8_t *out, size_t cap, size_t *out_len, int code)
     {
         const int k = codes[code].k;
-        SlotLease slot(stripe_slots);
+        SlotLease slot(grp().stripe_slots);
         uint8_t have[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M], want[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
         uint32_t block_len = 0;
         bool ok = false;
@@ -2969,7 +3079,7 @@ struct garage_bm {
         const int avail = gather_into(h, -1, sp, have, block_len, /*all=*/true, /*for_gpu=*/true, nullptr, nullptr,
                                       nullptr, code, who);
         if (avail > k && block_len <= cap) {
-            SlotLease trial(stripe_slots);
+            SlotLease trial(grp().stripe_slots);
             for (int x = 0; x < tot; x++) {
                 if (!have[x]) continue;
                 uint8_t h2[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M], w2[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
@@ -3012,6 +3122,7 @@ struct garage_bm {
     // it is not such a block)
     int resync_block(int node, const Hash &h, int64_t *gc_wait_ms = nullptr)
     {
+        Route route(*this);
         if (gc_wait_ms) *gc_wait_ms = 0;
         const auto ls = layouts();
         const bool multi = ls->v.size() > 1;
@@ -3043,7 +3154,7 @@ struct garage_bm {
             if (exists) return GARAGE_BM_OK;
         }
         if (!known || unneeded) return GARAGE_BM_OK;  // rc == 0: nothing to fetch
-        SlotLease slot(stripe_slots);
+        SlotLease slot(grp().stripe_slots);
         if (multi) {  // a layout change: the shard's holder in an older version is asked first (DESIGN.md section 5.2)
             const int c = copy_from_older(node, h, idx, *ls, false, slot.p);
             if (c != 0) {
@@ -3152,11 +3263,11 @@ struct garage_bm {
     // Rebuild the jobs' stripes from their survivors, like resync_block's fetch branch, batch_max_blocks stripes per
     // garage_ec_reconstruct_stripes.  Returns the number of shards written; *errors = the errors counted.
     // Concurrent callers run their batches one at a time (rebuild_mu), and a batch takes its stripe slots from the
-    // shared pool in one step, so it never holds part of the pool while it waits for the rest.
-    std::mutex rebuild_mu;
+    // group's pool in one step, so it never holds part of the pool while it waits for the rest.
     size_t rebuild_batch(std::vector<RebuildJob> &jobs, const RebuildCounters &c, size_t *errors = nullptr)
     {
-        std::lock_guard<std::mutex> rl(rebuild_mu);
+        DeviceGroup &dg = grp();
+        std::lock_guard<std::mutex> rl(dg.rebuild_mu);
         const size_t bmax = std::max<uint32_t>(cfg.batch_max_blocks, 1);
         std::atomic<size_t> written{0}, nerr{0};
         for (size_t b0 = 0; b0 < jobs.size(); b0 += bmax) {
@@ -3165,7 +3276,7 @@ struct garage_bm {
                 SlotPool &pool;
                 std::vector<uint8_t *> p;
                 ~Slots() { pool.release_n(p); }
-            } slots{stripe_slots, stripe_slots.acquire_n(n)};
+            } slots{dg.stripe_slots, dg.stripe_slots.acquire_n(n)};
             std::vector<ReconItem> items(n);
             std::vector<uint8_t> ok(n, 0);
             parallel_for(n, [&](size_t j, std::vector<uint8_t> &) {
@@ -3196,7 +3307,7 @@ struct garage_bm {
                 if (ok[j]) batch.push_back(&items[j]);
             std::vector<int> rc;
             reconstruct_calls += batch.size();
-            if (!batch.empty()) rec_batcher->submit_all(batch, rc);
+            if (!batch.empty()) dg.rec_batcher->submit_all(batch, rc);
             for (size_t q = 0, j = 0; j < n; j++)
                 if (ok[j]) ok[j] = rc[q++] == GARAGE_BM_OK;
             parallel_for(n, [&](size_t j, std::vector<uint8_t> &) {
@@ -3290,6 +3401,7 @@ struct garage_bm {
     // garage_bm_layout_sync_step: see include/garage_block_manager.h
     int layout_sync_step(int node, const Hash *cursor, size_t max_blocks, Hash *cursor_out, int *finished, uint64_t *moved)
     {
+        Route route(*this);
         Node &nd = *nodes[node];
         const auto ls = layouts();
         const uint64_t newest_v = garage_layout_version(ls->newest());
@@ -3315,7 +3427,7 @@ struct garage_bm {
         std::vector<std::pair<Hash, int>> receive;
         std::vector<Hash> offload;  // blocks of which the node holds an index the newest version does not give it
         {
-            SlotLease scratch(stripe_slots);
+            SlotLease scratch(grp().stripe_slots);
             for (const Hash &h : hs) {
                 {
                     // rc 0: nothing is received; the node's shards go once the GC delay has passed, decided and deleted
@@ -3557,11 +3669,12 @@ struct garage_bm {
     size_t convert_batch(const std::vector<Hash> &hs)
     {
         std::lock_guard<std::mutex> cl(convert_mu);
+        DeviceGroup &dg = grp();
         const size_t bmax = std::max<uint32_t>(cfg.batch_max_blocks, 1);
         const int nsrc = (int)codes.size() + (legacy_rf > 0 ? 1 : 0);  // source codes.size(): the replicas
         const size_t rep_stride = garage_ec_stride_for(stored_max());
         const int quorum = garage_ec_write_quorum(k, m, GARAGE_CONSISTENT);
-        uint8_t *blk = conv_blk.get(rep_stride);
+        uint8_t *blk = dg.conv_blk.get(rep_stride);
         if (!blk) return 0;
         std::atomic<size_t> converted{0};
         for (size_t b0 = 0; b0 < hs.size(); b0 += bmax) {
@@ -3571,8 +3684,8 @@ struct garage_bm {
                 const bool rep = c == (int)codes.size();
                 const int s_tot = rep ? 1 : codes[c].tot;
                 const size_t s_stride = rep ? rep_stride : slot_stride;
-                uint8_t *src = conv_src.get(nb * s_tot * s_stride);
-                uint8_t *dst = conv_dst.get(nb * tot * (slot_stride + 32));
+                uint8_t *src = dg.conv_src.get(nb * s_tot * s_stride);
+                uint8_t *dst = dg.conv_dst.get(nb * tot * (slot_stride + 32));
                 if (!src || !dst) break;
                 uint8_t *sums = dst + nb * tot * slot_stride;
                 std::vector<uint8_t> present(nb * s_tot);
@@ -3619,9 +3732,11 @@ struct garage_bm {
                 if (n == 0) continue;
                 std::vector<int32_t> status(n, GARAGE_EC_E_UNRECOVERABLE);
                 auto t0 = Clock::now();
-                int rc = garage_ec_transcode(ec, rep ? nullptr : codes[c].ctx, src, rep ? nullptr : present.data(), lens.data(),
-                                             s_stride, dst, slot_stride, sums, status.data(), n, GARAGE_EC_MEM_HOST, nullptr);
+                int rc = garage_ec_transcode(dg.code_ctx[0], rep ? nullptr : dg.code_ctx[c], src, rep ? nullptr : present.data(),
+                                             lens.data(), s_stride, dst, slot_stride, sums, status.data(), n,
+                                             GARAGE_EC_MEM_HOST, nullptr);
                 convert_call_us += us_since(t0);
+                dg.count(n, std::accumulate(lens.begin(), lens.begin() + n, (uint64_t)0));
                 if (rc != GARAGE_EC_OK && rc != GARAGE_EC_E_UNRECOVERABLE) continue;
                 // the new data shards must hash to the block before anything is written
                 std::vector<uint8_t> good(n, 0);
@@ -3644,9 +3759,11 @@ struct garage_bm {
                         int32_t st = 0;
                         if (get_from_stripe(h, blk, stored_max(), &olen, c) == GARAGE_BM_OK && olen == lens[q]) {
                             t0 = Clock::now();
-                            rc = garage_ec_transcode(ec, nullptr, blk, nullptr, &l32, rep_stride, dst + q * tot * slot_stride,
-                                                     slot_stride, sums + q * tot * 32, &st, 1, GARAGE_EC_MEM_HOST, nullptr);
+                            rc = garage_ec_transcode(dg.code_ctx[0], nullptr, blk, nullptr, &l32, rep_stride,
+                                                     dst + q * tot * slot_stride, slot_stride, sums + q * tot * 32, &st, 1,
+                                                     GARAGE_EC_MEM_HOST, nullptr);
                             convert_call_us += us_since(t0);
+                            dg.count(1, l32);
                             std::vector<uint8_t> tmp(lens[q]);
                             assemble(dst + q * tot * slot_stride, lens[q], tmp.data());
                             Hash got;
@@ -3692,7 +3809,9 @@ struct garage_bm {
     {
         const size_t nt = std::min<size_t>(n, std::min(16u, std::max(1u, std::thread::hardware_concurrency())));
         std::atomic<size_t> next{0};
+        const RouteTls route = tl_route;  // the workers' GPU work goes to the caller's group
         auto run = [&] {
+            tl_route = route;
             std::vector<uint8_t> tmp;
             for (size_t i; (i = next++) < n;) fn(i, tmp);
         };
@@ -3736,6 +3855,7 @@ struct garage_bm {
     int deep_scrub_step(int node, const Hash *cursor, size_t max_blocks, Hash *cursor_out, int *finished,
                         uint64_t *checked, uint64_t *repaired)
     {
+        Route route(*this);
         {
             Node &nd = *nodes[node];
             std::lock_guard<std::mutex> lk(nd.mu);
@@ -3744,9 +3864,10 @@ struct garage_bm {
         std::vector<Hash> mine = owned_blocks(node);
         sweep_page(mine, cursor, max_blocks, cursor_out, finished);
         uint64_t nchecked = 0, nrep = 0;
-        std::lock_guard<std::mutex> dl(deep_mu);
+        DeviceGroup &dg = grp();
+        std::lock_guard<std::mutex> dl(dg.deep_mu);
         const size_t bmax = std::max<uint32_t>(cfg.batch_max_blocks, 1), sbytes = (size_t)tot * slot_stride;
-        uint8_t *buf = mine.empty() ? nullptr : deep_buf.get(bmax * (sbytes + 32));
+        uint8_t *buf = mine.empty() ? nullptr : dg.deep_buf.get(bmax * (sbytes + 32));
         if (!mine.empty() && !buf) return GARAGE_EC_E_NOMEM;
         const bool multi = multi_version();
         std::vector<uint8_t> blk;
@@ -3789,9 +3910,10 @@ struct garage_bm {
             std::vector<uint8_t> hash_bad(nc);
             std::vector<uint32_t> mm(nc);
             const auto t0 = Clock::now();
-            const int rc_ = garage_ec_deep_check(ec, buf, lens.data(), hashes, hash_bad.data(), mm.data(), slot_stride, nc,
-                                                 GARAGE_EC_MEM_HOST, nullptr);
+            const int rc_ = garage_ec_deep_check(dg.code_ctx[0], buf, lens.data(), hashes, hash_bad.data(), mm.data(),
+                                                 slot_stride, nc, GARAGE_EC_MEM_HOST, nullptr);
             deep_check_us += us_since(t0);
+            dg.count(nc, std::accumulate(lens.begin(), lens.end(), (uint64_t)0));
             if (rc_ != GARAGE_EC_OK) return rc_;
             nchecked += nc;
             deep_blocks += nc;
@@ -3923,6 +4045,7 @@ struct garage_bm {
     int stripe_repair_step(int node, const Hash *cursor, size_t max_blocks, int min_missing, Hash *cursor_out,
                            int *finished, uint64_t *repaired, uint64_t *rebuilt)
     {
+        Route route(*this);
         {
             Node &nd = *nodes[node];
             std::lock_guard<std::mutex> lk(nd.mu);
@@ -3967,6 +4090,7 @@ struct garage_bm {
     // garage_bm_convert_step: see include/garage_block_manager.h
     int convert_step(int node, const Hash *cursor, size_t max_blocks, Hash *cursor_out, int *finished, uint64_t *converted)
     {
+        Route route(*this);
         Node &nd = *nodes[node];
         std::vector<Hash> hs;
         {
@@ -3982,7 +4106,7 @@ struct garage_bm {
         sweep_page(hs, cursor, max_blocks, cursor_out, finished);
         std::vector<Hash> todo;
         {
-            SlotLease scratch(stripe_slots);  // the quorum check's reads
+            SlotLease scratch(grp().stripe_slots);  // the quorum check's reads
             for (const Hash &h : hs) {
                 {
                     // rc 0: never converted; the legacy copies go once the GC delay has passed, decided and deleted
@@ -4063,8 +4187,8 @@ struct garage_bm {
         workers = std::max(1, std::min(workers, 64));
         std::vector<std::thread> th;
         for (int w = 0; w < workers; w++)
-            th.emplace_back([&] {
-                garage_ec_bind_thread(ec);
+            th.emplace_back([&, w] {
+                bind_worker(w);
                 for (;;) {
                     const size_t i = next++;
                     if (i >= todo.size()) return;
@@ -4171,8 +4295,8 @@ struct garage_bm {
         }
         std::atomic<size_t> next{0};
         std::atomic<uint64_t> n_ok{0}, n_failed{0}, n_deferred{0};
-        auto run = [&] {
-            garage_ec_bind_thread(ec);
+        auto run = [&](int w) {
+            bind_worker(w);
             for (size_t i; (i = next++) < todo.size();) {
                 const Hash &h = todo[i];
                 {
@@ -4214,7 +4338,7 @@ struct garage_bm {
         // the caller's thread keeps its own
         const int nth = (int)std::min<size_t>((size_t)workers, todo.size());
         std::vector<std::thread> th;
-        for (int w = 0; w < nth; w++) th.emplace_back(run);
+        for (int w = 0; w < nth; w++) th.emplace_back(run, w);
         for (auto &t : th) t.join();
         int64_t wait;
         {
@@ -4326,7 +4450,9 @@ struct garage_bm {
     int scrub(int node, uint64_t *checked, uint64_t *corrupt, const Hash *cursor = nullptr, size_t max_shards = 0,
               Hash *cursor_out = nullptr, int *finished = nullptr)
     {
-        std::lock_guard<std::mutex> sl(scrub_mu);
+        Route route(*this);
+        DeviceGroup &dg = grp();
+        std::lock_guard<std::mutex> sl(dg.scrub_mu);
         Node &nd = *nodes[node];
         std::vector<Hash> hashes;
         {
@@ -4347,7 +4473,7 @@ struct garage_bm {
         std::vector<uint8_t> replica;
         for (size_t c0 = 0; c0 < items.size(); c0 += chunk) {
             const size_t n = std::min(chunk, items.size() - c0);
-            uint8_t *buf = scrub_buf.get(n * stride + n * 32 + n + n * 4);
+            uint8_t *buf = dg.scrub_buf.get(n * stride + n * 32 + n + n * 4);
             if (!buf) return GARAGE_EC_E_NOMEM;
             uint8_t *expect = buf + n * stride, *bad = expect + n * 32;
             std::vector<uint32_t> lens(n, 0);
@@ -4392,8 +4518,10 @@ struct garage_bm {
                     }
                 }
             }
-            int rc = garage_ec_check_sums(ec, buf, expect, lens.data(), stride, n, 1, bad, GARAGE_EC_MEM_HOST, nullptr);
+            int rc = garage_ec_check_sums(dg.code_ctx[0], buf, expect, lens.data(), stride, n, 1, bad, GARAGE_EC_MEM_HOST,
+                                          nullptr);
             if (rc != GARAGE_EC_OK) return rc;
+            dg.count(n, std::accumulate(lens.begin(), lens.end(), (uint64_t)0));
             for (size_t i = 0; i < n; i++) {
                 if (!state[i]) continue;
                 nchecked++;
@@ -4408,6 +4536,10 @@ struct garage_bm {
         if (corrupt) *corrupt = nbad;
         return GARAGE_BM_OK;
     }
+
+    // worker thread w of a resync pass or a load run: on the CPUs of the node of group w mod n, so that the workers of
+    // a pass spread over the listed devices' sockets and each is routed to a group of its own socket
+    void bind_worker(int w) const { garage_ec_bind_thread(groups[(size_t)w % groups.size()]->code_ctx[0]); }
 
     // ---- native closed-loop load generator (tools/bm_bench.py drives it): `threads` client threads,
     // each PUTs (mode 0) or GETs (mode 1) `per_thread` blocks of `block_len` bytes.  Blocks are the
@@ -4451,8 +4583,9 @@ struct garage_bm {
             Hash wh;
             garage_ec_blake2sum(wblk.data(), block_len, wh.data());
             std::vector<std::thread> wt;
-            for (int t = 0; t < 3 * kWorkers; t++)
-                wt.emplace_back([&] {
+            for (int t = 0; t < 3 * DeviceGroup::kWorkers * (int)groups.size(); t++)
+                wt.emplace_back([&, t] {
+                    bind_worker(t);
                     try {
                         rpc_put_block(wh, wblk.data(), block_len);
                     } catch (...) {
@@ -4468,7 +4601,7 @@ struct garage_bm {
         std::vector<std::thread> th;
         for (int t = 0; t < threads; t++)
             th.emplace_back([&, t] {
-                garage_ec_bind_thread(ec);
+                bind_worker(t);
                 std::vector<uint8_t> out(mode == 1 ? block_len : 0);
                 ready++;
                 while (!go.load(std::memory_order_acquire)) std::this_thread::yield();
@@ -4603,7 +4736,91 @@ static int create_ctx(const CodeDesc &c, int device, int sum_kind, garage_ec_ctx
     return rc;
 }
 
-static int bm_create(garage_bm **out, const garage_bm_config *cfg, const garage_bm_data_dir *data_dirs, int n_data_dirs)
+// The group of bm on `device` (DESIGN.md section 5.13): a context per code (the first group takes the codes' own), the
+// dispatcher contexts and their parity buffers, the pools on the device's NUMA node, every context warmed, then the
+// dispatcher threads.  What it built before a failure is torn down with the manager.
+static int create_group(garage_bm *bm, int device, bool first)
+{
+    bm->groups.emplace_back(new DeviceGroup());
+    DeviceGroup &g = *bm->groups.back();
+    g.device = device;
+    const garage_bm_config &cfg = bm->cfg;
+    const int m = bm->m;
+    int rc = GARAGE_EC_OK;
+    for (const auto &c : bm->codes) {
+        garage_ec_ctx *x = first ? c.ctx : nullptr;
+        if (!first && (rc = create_ctx(c, device, bm->sum_kind, &x)) != GARAGE_EC_OK) return rc;
+        g.code_ctx.push_back(x);
+    }
+    garage_ec_ctx *const ec = g.code_ctx[0];
+    garage_ec_numa_info(ec, &g.numa_node, nullptr);
+    for (PinnedBuf *b : {&g.scrub_buf, &g.deep_buf, &g.conv_src, &g.conv_dst, &g.conv_blk}) b->ctx = ec;
+    for (int w = 0; w < DeviceGroup::kWorkers; w++) {
+        rc = create_ctx(bm->codes[0], device, bm->sum_kind, &g.enc_ctx[w]);
+        if (rc == GARAGE_EC_OK) rc = create_ctx(bm->codes[0], device, bm->sum_kind, &g.rec_ctx[w]);
+        if (rc != GARAGE_EC_OK) return rc;
+        // Dispatchers wait for their batch spinning in the driver (default) or sleeping on an event
+        // (GARAGE_BM_SLEEP_WAIT=1).  With 32 client threads on a 16-CPU host PUT is faster spinning: the wake-up
+        // latency costs more than the three CPUs.
+        const int sleep_wait = getenv("GARAGE_BM_SLEEP_WAIT") ? 1 : 0;
+        garage_ec_set_wait_mode(g.enc_ctx[w], sleep_wait);
+        garage_ec_set_wait_mode(g.rec_ctx[w], sleep_wait);
+        for (auto &eb : g.enc_out[w]) eb.ctx = g.enc_ctx[w];
+        // the pinned parity buffers at their final size now, not on the first large batch
+        const size_t out_bytes = (size_t)std::max<uint32_t>(cfg.batch_max_blocks, 1) * ((size_t)m * bm->slot_stride + (size_t)bm->tot * 32);
+        for (auto &eb : g.enc_out[w])
+            if (!eb.get(out_bytes)) return GARAGE_EC_E_NOMEM;
+    }
+    const size_t nslots = (size_t)std::max<uint32_t>(cfg.batch_max_blocks, 1) * (DeviceGroup::kWorkers + 1);
+    if (!g.put_slots.init(ec, nslots, cfg.block_size)) return GARAGE_EC_E_NOMEM;
+    int max_tot = bm->tot;  // a stripe slot holds a stripe of any code in play
+    for (const auto &c : bm->codes) max_tot = std::max(max_tot, c.tot);
+    if (!g.stripe_slots.init(ec, nslots, (size_t)max_tot * bm->slot_stride)) return GARAGE_EC_E_NOMEM;
+    garage_ec_numa_info(ec, nullptr, &g.pool_node);
+    // Warm every dispatcher's context now: streams, lane buffers, and the first launch of each kernel (CUDA
+    // loads kernels lazily) cost tens of milliseconds that would otherwise land on the first real batches.
+    {
+        SlotLease blk(g.put_slots), stripe(g.stripe_slots);
+        const uint32_t wlen = cfg.block_size;
+        memset(blk.p, 0x5a, wlen);
+        memset(stripe.p, 0, (size_t)bm->tot * bm->slot_stride);
+        for (int w = 0; w < DeviceGroup::kWorkers; w++) {
+            const uint8_t *ptrs[1] = {blk.p};
+            uint8_t *par = g.enc_out[w][0].get(1);
+            rc = garage_ec_encode_blocks_with_sums(g.enc_ctx[w], ptrs, &wlen, 1, par, par + (size_t)m * bm->slot_stride, bm->slot_stride);
+            if (rc != GARAGE_EC_OK) return rc;
+            uint8_t present[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M], want[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
+            memset(present, 1, sizeof(present));
+            present[0] = 0;
+            want[0] = 1;
+            uint8_t *stripes[1] = {stripe.p};
+            const uint32_t slen = (uint32_t)bm->shard_len_of(wlen);
+            int32_t st = 0;
+            rc = garage_ec_reconstruct_stripes(g.rec_ctx[w], stripes, present, want, &st, &slen, bm->slot_stride, 1);
+            if (rc != GARAGE_EC_OK) return rc;
+        }
+        uint8_t bad1 = 0, exp1[32] = {0};
+        const uint32_t slen = (uint32_t)bm->shard_len_of(wlen);
+        rc = garage_ec_check_sums(ec, stripe.p, exp1, &slen, bm->slot_stride, 1, 1, &bad1, GARAGE_EC_MEM_HOST, nullptr);
+        if (rc != GARAGE_EC_OK) return rc;
+    }
+    // the dispatchers run on the device's node and route their own work to their group
+    DeviceGroup *gp = &g;
+    auto start = [bm, gp] {
+        garage_ec_bind_thread(gp->code_ctx[0]);
+        tl_route = {bm, gp};
+    };
+    g.enc_batcher.reset(new Batcher<EncodeItem>(cfg.batch_max_blocks, cfg.batch_linger_us, DeviceGroup::kWorkers,
+                                                [bm](int w, std::vector<EncodeItem *> &b) { bm->run_encode(w, b); }, start));
+    g.rec_batcher.reset(new Batcher<ReconItem>(cfg.batch_max_blocks, cfg.batch_linger_us, DeviceGroup::kWorkers,
+                                               [bm](int w, std::vector<ReconItem *> &b) { bm->run_reconstruct(w, b); }, start));
+    return GARAGE_EC_OK;
+}
+
+// devices: the listed devices, one group each.  check_range: a device past garage_ec_device_count is refused before any
+// CUDA context exists (garage_bm_create leaves that to the context's own NODEVICE, as it always has).
+static int bm_create(garage_bm **out, const garage_bm_config *cfg, const garage_bm_data_dir *data_dirs, int n_data_dirs,
+                     const int *devices, int n_devices, bool check_range)
 {
     *out = nullptr;
     const int k = cfg->data_shards, m = cfg->parity_shards, l = cfg->local_groups;
@@ -4653,6 +4870,10 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg, const garage_
     // a store changes its layout or its code, not both at once
     if (lays->v.size() > 1 && (np > 0 || cfg->legacy_replicas > 0)) return GARAGE_EC_E_INVALID;
     if (clay && layout_file && !cfg->clay_layout) return GARAGE_EC_E_INVALID;  // a Clay store keeps the fixed ring
+    // with no device at all, the first context's NODEVICE is the answer, as for garage_bm_create
+    const int ndev = check_range ? garage_ec_device_count() : 0;
+    for (int i = 0; i < n_devices; i++)
+        if (ndev > 0 && devices[i] >= ndev) return GARAGE_EC_E_INVALID;
     std::unique_ptr<garage_bm> bm(new garage_bm());
     bm->cfg = *cfg;
     if (!bm->cfg.block_size) bm->cfg.block_size = 1u << 20;
@@ -4675,12 +4896,11 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg, const garage_
         c.pb = p.piggyback != 0;
         c.clay = p.clay != 0;
         c.tot = p.k + p.m;
-        rc = create_ctx(c, cfg->cuda_device, bm->sum_kind, &c.ctx);
+        rc = create_ctx(c, devices[0], bm->sum_kind, &c.ctx);
         if (rc != GARAGE_EC_OK) {  // no GPU => no block manager: there is no CPU fallback
             garage_bm_destroy(bm.release());
             return rc;
         }
-        if (i == 0) bm->ec = c.ctx;
         c.quantum = c.pb ? 128u : 1u;
         if (c.clay) {
             int alpha = 0;
@@ -4761,69 +4981,16 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg, const garage_
         }
     }
     bm->ram.reset(new ByteSemaphore(cfg->block_ram_buffer_max ? cfg->block_ram_buffer_max : (256ull << 20)));
-    bm->scrub_buf.ctx = bm->ec;
-    bm->deep_buf.ctx = bm->ec;
     auto destroy_on_error = [&](int code) {
         garage_bm_destroy(bm.release());
         return code;
     };
     // a layout given in the configuration is recorded, so that a restart keeps it and its later versions
     if (layout_file && !std::filesystem::exists(layout_path) && !bm->save_layout(*lays)) return destroy_on_error(GARAGE_BM_E_MESSAGE);
-    for (int w = 0; w < garage_bm::kWorkers; w++) {
-        rc = create_ctx(bm->codes[0], cfg->cuda_device, bm->sum_kind, &bm->enc_ctx[w]);
-        if (rc == GARAGE_EC_OK) rc = create_ctx(bm->codes[0], cfg->cuda_device, bm->sum_kind, &bm->rec_ctx[w]);
-        if (rc != GARAGE_EC_OK) return destroy_on_error(rc);
-        // Dispatchers wait for their batch spinning in the driver (default) or sleeping on an event
-        // (GARAGE_BM_SLEEP_WAIT=1).  With 32 client threads on a 16-CPU host PUT is faster spinning: the wake-up
-        // latency costs more than the three CPUs.
-        const int sleep_wait = getenv("GARAGE_BM_SLEEP_WAIT") ? 1 : 0;
-        garage_ec_set_wait_mode(bm->enc_ctx[w], sleep_wait);
-        garage_ec_set_wait_mode(bm->rec_ctx[w], sleep_wait);
-        for (auto &eb : bm->enc_out[w]) eb.ctx = bm->enc_ctx[w];
-        // the pinned parity buffers at their final size now, not on the first large batch
-        const size_t out_bytes = (size_t)std::max<uint32_t>(cfg->batch_max_blocks, 1) * ((size_t)m * bm->slot_stride + (size_t)(k + m) * 32);
-        for (auto &eb : bm->enc_out[w])
-            if (!eb.get(out_bytes)) return destroy_on_error(GARAGE_EC_E_NOMEM);
+    for (int i = 0; i < n_devices; i++) {
+        rc = create_group(bm.get(), devices[i], i == 0);
+        if (rc != GARAGE_EC_OK) return destroy_on_error(rc);  // no group left out: all of them or no manager
     }
-    const size_t nslots = (size_t)std::max<uint32_t>(cfg->batch_max_blocks, 1) * (garage_bm::kWorkers + 1);
-    if (!bm->put_slots.init(bm->ec, nslots, bm->cfg.block_size)) return destroy_on_error(GARAGE_EC_E_NOMEM);
-    int max_tot = bm->tot;  // a stripe slot holds a stripe of any code in play
-    for (const auto &c : bm->codes) max_tot = std::max(max_tot, c.tot);
-    if (!bm->stripe_slots.init(bm->ec, nslots, (size_t)max_tot * bm->slot_stride)) return destroy_on_error(GARAGE_EC_E_NOMEM);
-    bm->conv_src.ctx = bm->conv_dst.ctx = bm->conv_blk.ctx = bm->ec;
-    // Warm every dispatcher's context now: streams, lane buffers, and the first launch of each kernel (CUDA
-    // loads kernels lazily) cost tens of milliseconds that would otherwise land on the first real batches.
-    {
-        SlotLease blk(bm->put_slots), stripe(bm->stripe_slots);
-        const uint32_t wlen = bm->cfg.block_size;
-        memset(blk.p, 0x5a, wlen);
-        memset(stripe.p, 0, (size_t)bm->tot * bm->slot_stride);
-        for (int w = 0; w < garage_bm::kWorkers; w++) {
-            const uint8_t *ptrs[1] = {blk.p};
-            uint8_t *par = bm->enc_out[w][0].get(1);
-            rc = garage_ec_encode_blocks_with_sums(bm->enc_ctx[w], ptrs, &wlen, 1, par, par + (size_t)m * bm->slot_stride, bm->slot_stride);
-            if (rc != GARAGE_EC_OK) return destroy_on_error(rc);
-            uint8_t present[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M], want[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
-            memset(present, 1, sizeof(present));
-            present[0] = 0;
-            want[0] = 1;
-            uint8_t *stripes[1] = {stripe.p};
-            const uint32_t slen = (uint32_t)bm->shard_len_of(wlen);
-            int32_t st = 0;
-            rc = garage_ec_reconstruct_stripes(bm->rec_ctx[w], stripes, present, want, &st, &slen, bm->slot_stride, 1);
-            if (rc != GARAGE_EC_OK) return destroy_on_error(rc);
-        }
-        uint8_t bad1 = 0, exp1[32] = {0};
-        const uint32_t slen = (uint32_t)bm->shard_len_of(wlen);
-        rc = garage_ec_check_sums(bm->ec, stripe.p, exp1, &slen, bm->slot_stride, 1, 1, &bad1, GARAGE_EC_MEM_HOST, nullptr);
-        if (rc != GARAGE_EC_OK) return destroy_on_error(rc);
-    }
-    garage_bm *raw = bm.get();
-    auto bind = [raw] { garage_ec_bind_thread(raw->ec); };
-    bm->enc_batcher.reset(new Batcher<EncodeItem>(cfg->batch_max_blocks, cfg->batch_linger_us, garage_bm::kWorkers,
-                                                  [raw](int w, std::vector<EncodeItem *> &b) { raw->run_encode(w, b); }, bind));
-    bm->rec_batcher.reset(new Batcher<ReconItem>(cfg->batch_max_blocks, cfg->batch_linger_us, garage_bm::kWorkers,
-                                                 [raw](int w, std::vector<ReconItem *> &b) { raw->run_reconstruct(w, b); }, bind));
     *out = bm.release();
     return GARAGE_BM_OK;
 }
@@ -4831,14 +4998,25 @@ static int bm_create(garage_bm **out, const garage_bm_config *cfg, const garage_
 int garage_bm_create(garage_bm **out, const garage_bm_config *cfg)
 {
     if (!out || !cfg) return GARAGE_EC_E_INVALID;
-    BM_GUARD(bm_create(out, cfg, nullptr, 0));
+    BM_GUARD(bm_create(out, cfg, nullptr, 0, &cfg->cuda_device, 1, false));
 }
 
 int garage_bm_create_with_drives(garage_bm **out, const garage_bm_config *cfg, const garage_bm_data_dir *data_dirs,
                                  int n_data_dirs)
 {
     if (!out || !cfg) return GARAGE_EC_E_INVALID;
-    BM_GUARD(bm_create(out, cfg, data_dirs, n_data_dirs));
+    BM_GUARD(bm_create(out, cfg, data_dirs, n_data_dirs, &cfg->cuda_device, 1, false));
+}
+
+int garage_bm_create_on_devices(garage_bm **out, const garage_bm_config *cfg, const garage_bm_data_dir *data_dirs,
+                                int n_data_dirs, const int *cuda_devices, int n_devices)
+{
+    if (!out || !cfg) return GARAGE_EC_E_INVALID;
+    *out = nullptr;
+    if (!cuda_devices || n_devices < 1 || n_devices > GARAGE_BM_MAX_DEVICES) return GARAGE_EC_E_INVALID;
+    for (int i = 0; i < n_devices; i++)
+        if (cuda_devices[i] < 0) return GARAGE_EC_E_INVALID;
+    BM_GUARD(bm_create(out, cfg, data_dirs, n_data_dirs, cuda_devices, n_devices, true));
 }
 
 void garage_bm_destroy(garage_bm *bm)
@@ -4850,30 +5028,42 @@ void garage_bm_destroy(garage_bm *bm)
         } catch (...) {
         }
     }
-    bm->enc_batcher.reset();
-    bm->rec_batcher.reset();
-    garage_ec_ctx *ec = bm->ec;
-    garage_ec_ctx *ctxs[2 * garage_bm::kWorkers];
-    for (int w = 0; w < garage_bm::kWorkers; w++) {
-        for (auto &eb : bm->enc_out[w]) eb.release();  // pinned buffers go before their context
-        ctxs[2 * w] = bm->enc_ctx[w];
-        ctxs[2 * w + 1] = bm->rec_ctx[w];
+    for (auto &g : bm->groups) {  // every dispatcher joined before any pinned memory goes
+        g->enc_batcher.reset();
+        g->rec_batcher.reset();
     }
-    bm->scrub_buf.release();
-    bm->deep_buf.release();
-    bm->conv_src.release();
-    bm->conv_dst.release();
-    bm->conv_blk.release();
-    bm->put_slots.destroy();
-    bm->stripe_slots.destroy();
-    std::vector<garage_ec_ctx *> previous;
-    for (size_t c = 1; c < bm->codes.size(); c++) previous.push_back(bm->codes[c].ctx);
+    std::vector<garage_ec_ctx *> ctxs;  // each once: the first group's code contexts are the codes' own
+    for (auto &g : bm->groups) {
+        g->stop();  // pinned memory goes before its context
+        ctxs.insert(ctxs.end(), std::begin(g->enc_ctx), std::end(g->enc_ctx));
+        ctxs.insert(ctxs.end(), std::begin(g->rec_ctx), std::end(g->rec_ctx));
+        ctxs.insert(ctxs.end(), g->code_ctx.begin(), g->code_ctx.end());
+    }
+    for (const auto &c : bm->codes) ctxs.push_back(c.ctx);
     delete bm;
+    std::sort(ctxs.begin(), ctxs.end());
+    ctxs.erase(std::unique(ctxs.begin(), ctxs.end()), ctxs.end());
     for (garage_ec_ctx *c : ctxs)
         if (c) garage_ec_destroy(c);
-    for (garage_ec_ctx *c : previous)
-        if (c) garage_ec_destroy(c);
-    if (ec) garage_ec_destroy(ec);
+}
+
+int garage_bm_get_device_metrics(garage_bm *bm, garage_bm_device_metrics *out, int cap, int *n)
+{
+    if (!bm || !n || cap < 0 || (!out && cap > 0)) return GARAGE_EC_E_INVALID;
+    *n = (int)bm->groups.size();
+    for (int i = 0; i < *n && i < cap; i++) {
+        const DeviceGroup &g = *bm->groups[i];
+        garage_bm_device_metrics &o = out[i];
+        o.cuda_device = g.device;
+        o.numa_node = g.numa_node;
+        o.batches = g.batches;
+        o.blocks = g.blocks;
+        o.bytes = g.bytes;
+        o.routed_local = g.routed_local;
+        o.routed_remote = g.routed_remote;
+        o.pool_numa_node = g.pool_node;
+    }
+    return GARAGE_BM_OK;
 }
 
 void garage_bm_blake2sum(const uint8_t *data, size_t len, uint8_t hash_out[32]) { garage_ec_blake2sum(data, len, hash_out); }
@@ -5252,9 +5442,11 @@ void garage_bm_get_metrics(garage_bm *bm, garage_bm_metrics *o)
     o->resync_recv_counter = bm->resync_recv_counter;
     o->delete_counter = bm->delete_counter;
     o->put_calls = bm->put_calls;
-    o->put_batches = bm->enc_batcher ? bm->enc_batcher->batches() : 0;
+    for (const auto &g : bm->groups) {
+        o->put_batches += g->enc_batcher ? g->enc_batcher->batches() : 0;
+        o->reconstruct_batches += g->rec_batcher ? g->rec_batcher->batches() : 0;
+    }
     o->reconstruct_calls = bm->reconstruct_calls;
-    o->reconstruct_batches = bm->rec_batcher ? bm->rec_batcher->batches() : 0;
     o->scrub_shards_checked = bm->scrub_checked;
     o->scrub_corruptions = bm->scrub_corrupt;
     o->encode_call_us = bm->enc_gpu_us;

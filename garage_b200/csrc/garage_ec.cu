@@ -1280,6 +1280,16 @@ int garage_ec_bind_thread(const garage_ec_ctx *ctx)
     return sched_setaffinity(0, sizeof(want), &want) == 0 ? GARAGE_EC_OK : 1;
 }
 
+int garage_ec_device_count(void)
+{
+    int n = 0;
+    if (cudaGetDeviceCount(&n) != cudaSuccess) {
+        (void)cudaGetLastError();
+        return 0;
+    }
+    return n;
+}
+
 void garage_ec_host_free(garage_ec_ctx *ctx, void *ptr)
 {
     if (!ctx || !ptr) return;

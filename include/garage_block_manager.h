@@ -298,7 +298,36 @@ int garage_bm_create(garage_bm **out, const garage_bm_config *cfg);
  * repeated path or one outside the node directory, capacity 0 without read_only, or no drive with capacity.        */
 int garage_bm_create_with_drives(garage_bm **out, const garage_bm_config *cfg, const garage_bm_data_dir *data_dirs,
                                  int n_data_dirs);
+/* garage_bm_create_with_drives on several GPUs of the host (DESIGN.md section 5.13); cfg->cuda_device is not read.  One
+ * dispatcher group per listed device: its encode and reconstruct dispatchers, a context per code for the sweeps, and
+ * its pinned slot pools on the device's NUMA node.  Every call that reaches the GPU is routed to one group by the
+ * calling thread's NUMA node: among the groups whose GPU is on that node (all groups if none is) the one with the
+ * fewest calls in flight, ties round robin.  A batch never spans groups.  The same device may be listed more than
+ * once (two groups on one GPU).  data_dirs NULL / n_data_dirs 0: every file under the node directory, as
+ * garage_bm_create.  GARAGE_EC_E_INVALID before any context is created or thread started for a NULL list, n_devices
+ * outside 1..GARAGE_BM_MAX_DEVICES, a negative device, one at or past garage_ec_device_count, or anything
+ * garage_bm_create_with_drives refuses; GARAGE_EC_E_NODEVICE on a host with no device.  A group that cannot be built
+ * fails the whole call, and what was built is torn down.  garage_bm_create(_with_drives) are this call on
+ * {cfg->cuda_device}.                                                                                            */
+#define GARAGE_BM_MAX_DEVICES 16
+int garage_bm_create_on_devices(garage_bm **out, const garage_bm_config *cfg, const garage_bm_data_dir *data_dirs,
+                                int n_data_dirs, const int *cuda_devices, int n_devices);
 void garage_bm_destroy(garage_bm *bm);
+
+/* One dispatcher group (garage_bm_create_on_devices), in list order. */
+typedef struct {
+    int cuda_device;
+    int numa_node;          /* the GPU's NUMA node (garage_ec_numa_info), -1 = unknown                             */
+    uint64_t batches;       /* GPU calls of the group: dispatcher batches and the sweeps' own calls                */
+    uint64_t blocks;        /* blocks (or shards, for the scrub) those calls carried                               */
+    uint64_t bytes;         /* their stored bytes                                                                  */
+    uint64_t routed_local;  /* calls routed here from a thread on the GPU's node                                   */
+    uint64_t routed_remote; /* calls routed here from any other node (no group on the caller's node)               */
+    int pool_numa_node;     /* the node the group's pinned pools landed on (garage_ec_numa_info), -1 = unknown     */
+} garage_bm_device_metrics;
+/* *n = the number of groups; at most cap entries are written to out.  GARAGE_EC_E_INVALID for NULL bm or n, cap < 0,
+ * or out NULL with cap > 0.                                                                                      */
+int garage_bm_get_device_metrics(garage_bm *bm, garage_bm_device_metrics *out, int cap, int *n);
 
 /* util/data.rs:130-138 */
 void garage_bm_blake2sum(const uint8_t *data, size_t len, uint8_t hash_out[32]);

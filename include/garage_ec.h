@@ -600,6 +600,9 @@ void garage_ec_host_free(garage_ec_ctx *ctx, void *ptr);
  * permitted).                                                                               */
 int garage_ec_numa_info(const garage_ec_ctx *ctx, int *gpu_node, int *last_alloc_node);
 int garage_ec_bind_thread(const garage_ec_ctx *ctx);
+/* the number of CUDA devices this process sees (cudaGetDeviceCount); 0 if there is none or no driver.  Creates no
+ * context: the block manager checks a device list with it before it creates any.                              */
+int garage_ec_device_count(void);
 
 /* number of kernel launches issued by this context so far (bench.py's gpu_launches)        */
 uint64_t garage_ec_launch_count(const garage_ec_ctx *ctx);

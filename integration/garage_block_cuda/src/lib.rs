@@ -275,3 +275,75 @@ impl ErasureCoder {
     }
 }
 impl Drop for ErasureCoder { fn drop(&mut self) { unsafe { sys::garage_ec_destroy(self.ctx) } } }
+
+/// `cuda_devices = [...]` (DESIGN.md section 5.13): one coder per listed GPU with its NUMA node, and the block
+/// manager's routing rule.  The coders whose GPU is on the calling thread's node are the candidates (all of them if
+/// none is); the one with the fewest calls in flight wins, ties round robin.  A batch is handed to one coder only, so
+/// no batch spans GPUs; the batcher and pinned pools of each coder live next to it (one batch::EcBatcher per coder).
+pub struct DeviceCoders {
+    coders: Vec<(ErasureCoder, i32)>,
+    in_flight: Vec<std::sync::atomic::AtomicUsize>,
+    rr: std::sync::atomic::AtomicUsize,
+}
+
+extern "C" {
+    fn getcpu(cpu: *mut u32, node: *mut u32) -> std::os::raw::c_int;  // glibc >= 2.29
+}
+
+pub const MAX_DEVICES: usize = 16;
+
+/// A routed call: the coder it runs on, released (one call less in flight) when dropped.
+pub struct Routed<'a> { owner: &'a DeviceCoders, i: usize }
+impl<'a> std::ops::Deref for Routed<'a> {
+    type Target = ErasureCoder;
+    fn deref(&self) -> &ErasureCoder { &self.owner.coders[self.i].0 }
+}
+impl<'a> Drop for Routed<'a> {
+    fn drop(&mut self) { self.owner.in_flight[self.i].fetch_sub(1, std::sync::atomic::Ordering::Relaxed); }
+}
+
+impl DeviceCoders {
+    /// One coder per entry of `devices` (a device may repeat).  Refused before any context exists: an empty list, more
+    /// than MAX_DEVICES entries, or a device outside 0..garage_ec_device_count().  A coder that cannot be created fails
+    /// the whole call (the ones already created are dropped): a node never runs on fewer GPUs than configured.
+    pub fn new(devices: &[i32], k: usize, m: usize) -> Result<Self, Error> {
+        let n = unsafe { sys::garage_ec_device_count() };
+        if devices.is_empty() || devices.len() > MAX_DEVICES || devices.iter().any(|&d| d < 0 || d >= n) {
+            return Err(Error::Message(format!("cuda_devices {:?}: {} device(s) visible", devices, n)));
+        }
+        let mut coders = Vec::with_capacity(devices.len());
+        for &d in devices {
+            let ec = ErasureCoder::new(d, k, m)?;
+            let mut node = -1;
+            unsafe { sys::garage_ec_numa_info(ec.ctx, &mut node, std::ptr::null_mut()) };
+            coders.push((ec, node));
+        }
+        let in_flight = devices.iter().map(|_| std::sync::atomic::AtomicUsize::new(0)).collect();
+        Ok(Self { coders, in_flight, rr: std::sync::atomic::AtomicUsize::new(0) })
+    }
+
+    /// The coder a call from this thread runs on (see the type's documentation).
+    pub fn route(&self) -> Routed<'_> {
+        use std::sync::atomic::Ordering::Relaxed;
+        let (mut cpu, mut node) = (0u32, 0u32);
+        let here = if unsafe { getcpu(&mut cpu, &mut node) } == 0 { node as i32 } else { -1 };
+        let local = here >= 0 && self.coders.iter().any(|c| c.1 == here);
+        let n = self.coders.len();
+        let start = self.rr.fetch_add(1, Relaxed) % n;
+        let mut best: Option<usize> = None;
+        for j in 0..n {
+            let i = (start + j) % n;
+            if local && self.coders[i].1 != here { continue; }
+            if best.map_or(true, |b| self.in_flight[i].load(Relaxed) < self.in_flight[b].load(Relaxed)) { best = Some(i); }
+        }
+        let i = best.unwrap();
+        self.in_flight[i].fetch_add(1, Relaxed);
+        Routed { owner: self, i }
+    }
+
+    /// Pin the calling thread (a resync worker, an API worker) to the CPUs of coder w mod n's node, so that a pool of
+    /// workers spreads over the GPUs' sockets.
+    pub fn bind_worker(&self, w: usize) {
+        unsafe { sys::garage_ec_bind_thread(self.coders[w % self.coders.len()].0.ctx) };
+    }
+}

@@ -180,6 +180,7 @@ extern "C" {
     pub fn garage_ec_timing_read(ctx: *mut garage_ec_ctx, total_ms: *mut f64, launches: *mut u64) -> c_int;
     pub fn garage_ec_numa_info(ctx: *const garage_ec_ctx, gpu_node: *mut c_int, last_alloc_node: *mut c_int) -> c_int;
     pub fn garage_ec_bind_thread(ctx: *const garage_ec_ctx) -> c_int;
+    pub fn garage_ec_device_count() -> c_int;
     pub fn garage_ec_reconstruct_stripes(ctx: *mut garage_ec_ctx, stripes: *const *mut u8, present: *const u8,
                             want: *const u8, status: *mut i32, shard_len: *const u32, stride: usize,
                             n_stripes: usize) -> c_int;
