@@ -48,6 +48,7 @@ ABI_SYMBOLS = [
     "garage_ec_reseal", "garage_ec_reseal_stripes",
     "garage_ec_seal_crc", "garage_ec_seal_blocks_crc", "garage_ec_reseal_crc", "garage_ec_reseal_stripes_crc",
     "garage_ec_crc_combine",
+    "garage_ec_reconstruct_segments", "garage_ec_reconstruct_segments_stripes",
 ]
 
 
@@ -120,6 +121,8 @@ def load_library(build=True):
     L.garage_ec_device_count.argtypes = []
     L.garage_ec_debug_fail_after.argtypes = [vp, C.c_long]
     L.garage_ec_reconstruct_stripes.argtypes = [vp, vp, vp, vp, vp, vp, sz, sz]
+    L.garage_ec_reconstruct_segments.argtypes = [vp, vp, vp, vp, vp, vp, sz, sz, i32, vp]
+    L.garage_ec_reconstruct_segments_stripes.argtypes = [vp, vp, vp, vp, vp, vp, sz, sz]
     L.garage_ec_set_sum_kind.argtypes = [vp, i32]
     L.garage_ec_set_wait_mode.argtypes = [vp, i32]
     L.garage_ec_copy_for_dma.argtypes = [vp, vp, C.c_size_t]
@@ -477,6 +480,19 @@ class GarageEc:
         ptrs = (C.c_void_p * n)(*[a.ctypes.data for a in stripes])
         return self._check(self._L.garage_ec_reconstruct_stripes(self._h, C.cast(ptrs, C.c_void_p), _ptr(present),
                                                                  _ptr(want), _ptr(status), _ptr(shard_len), stride, n),
+                           (E_UNRECOVERABLE,))
+
+    def reconstruct_segments(self, shards, seg_present, stride, n, want=None, status=None, shard_len=None):
+        """garage_ec_reconstruct_segments: seg_present holds one byte per shard, bit g = adler8 segment g is valid.
+        `shards` a list of numpy arrays: the gather form (one (k+m)*stride buffer per stripe)"""
+        if isinstance(shards, list):
+            ptrs = (C.c_void_p * n)(*[a.ctypes.data for a in shards])
+            return self._check(self._L.garage_ec_reconstruct_segments_stripes(
+                self._h, C.cast(ptrs, C.c_void_p), _ptr(seg_present), _ptr(want), _ptr(status), _ptr(shard_len),
+                stride, n), (E_UNRECOVERABLE,))
+        kind, st = self._stream(shards)
+        return self._check(self._L.garage_ec_reconstruct_segments(self._h, _ptr(shards), _ptr(seg_present), _ptr(want),
+                                                                  _ptr(status), _ptr(shard_len), stride, n, kind, st),
                            (E_UNRECOVERABLE,))
 
     def verify(self, shards, mismatch, stride, n, shard_len=None):

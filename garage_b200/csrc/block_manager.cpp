@@ -944,6 +944,18 @@ struct Node {
         if (index >= 0 && by_index) return file_read_into(path_at(h, index), 0, dst, cap, mt, span);
         return file_read_into(path_for(h, code), code, dst, cap, mt, span);
     }
+    // Salvage (DESIGN.md section 5.14): h's configured-code shard whole into dst, from its live file or, `quarantined`,
+    // from its ".corrupted" copy (memory store: Node::corrupted).  The header is checked as on every read (file store:
+    // its Adler-32 check, the code it names, its lengths); the tag is not, and nothing is moved or queued.
+    ReadResult salvage_read(const Hash &h, bool quarantined, uint8_t *dst, size_t cap, ShardMeta &mt) const
+    {
+        if (dir.empty()) {
+            const auto &map = quarantined ? corrupted : shards;
+            auto it = map.find(h);
+            return it == map.end() ? kReadMissing : copy_out(*it->second, dst, cap, mt);
+        }
+        return quarantined ? file_read_into(path_of(h, ".corrupted"), 0, dst, cap, mt) : store_read_into(h, dst, cap, mt);
+    }
     // one shard file read as a shard of `code`
     ReadResult file_read_into(const std::string &path, int code, uint8_t *dst, size_t cap, ShardMeta &mt, ShardSpan span = {}) const
     {
@@ -1744,6 +1756,8 @@ struct garage_bm {
         reseal_auth_failures{0}, reseal_fallbacks{0}, reseal_us{0}, reseal_call_us{0};
     std::atomic<uint64_t> layout_shards_copied{0}, layout_shards_rebuilt{0}, layout_bytes_read{0}, layout_bytes_written{0},
         layout_deleted{0}, layout_sync_errors{0}, layout_bytes_fetched{0};
+    std::atomic<uint64_t> salvage_attempts{0}, salvage_blocks{0}, salvage_failures{0}, salvage_units_rebuilt{0},
+        salvage_quarantined_segments{0}, salvage_bytes_read{0}, salvage_call_us{0};
     std::atomic<uint64_t> stripe_repairs{0}, stripe_repair_shards{0}, stripe_repair_bytes_read{0},
         stripe_repair_bytes_fetched{0}, stripe_repair_bytes_written{0}, stripe_repair_errors{0}, stripe_repair_call_us{0};
     std::atomic<uint64_t> rebalance_files_moved{0}, rebalance_bytes_moved{0}, rebalance_errors{0}, drive_marker_errors{0};
@@ -2927,10 +2941,10 @@ struct garage_bm {
         range_gets++;
         uint8_t present[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
         uint32_t block_len = 0;
-        int gpu = 0;
+        int gpu = 0, rc;
         {
             SlotLease slot(grp().stripe_slots);
-            const int rc = gather_ranged(
+            rc = gather_ranged(
                 h, slot.p,
                 [&](uint32_t bl) -> int {
                     if ((uint64_t)off + len > bl || len > cap) return GARAGE_EC_E_INVALID;
@@ -2952,10 +2966,13 @@ struct garage_bm {
                 return submit_range(slot.p, block_len, present, nullptr, off, len, out);
             }
             if (rc == kRangeNoHeader && !has_legacy()) return GARAGE_BM_E_MISSING_BLOCK;
-            if (rc != kRangeWhole && rc != kRangeNoHeader) return rc;
+            if (rc != kRangeWhole && rc != kRangeNoHeader && !(rc == GARAGE_BM_E_MISSING_BLOCK && salvage_possible()))
+                return rc;
         }
-        return slice_whole([&](uint8_t *b, size_t c, size_t *n) { return rpc_get_block(h, b, c, n); }, off, len, out, cap,
-                           out_len);
+        const int r2 = slice_whole([&](uint8_t *b, size_t c, size_t *n) { return rpc_get_block(h, b, c, n); }, off, len, out,
+                                   cap, out_len);
+        // a range whose shards gave up: the whole GET's salvage (DESIGN.md section 5.14) serves it, else today's error
+        return rc == GARAGE_BM_E_MISSING_BLOCK && r2 != GARAGE_BM_OK ? rc : r2;
     }
 
     // Plaintext bytes [off, off + len) of SSE-C block h sealed under key (a ranged GET or UploadPartCopy of an SSE-C
@@ -3039,6 +3056,150 @@ struct garage_bm {
         return false;
     }
 
+    // ---- salvage (DESIGN.md section 5.14) ------------------------------------------------------
+    // Where the configured stripe has too few whole valid shards, an adler8 store can still hold every byte: each segment
+    // of every index from the live shard or, failing that, from its quarantined copy, and each unit rebuilt on its own
+    // (garage_ec_reconstruct_segments).  RS, LRC and PB stores with one active layout version only.
+    bool salvage_possible() const { return sum_kind == GARAGE_EC_SUM_ADLER8 && !codes[0].clay && !multi_version(); }
+
+    // The stripe of h rebuilt by segment into `slot` (a stripe slot) and proven by its content hash; the block goes to
+    // blk (block_len bytes, nullable).  live_ok[i]: index i's live shard was whole and valid.  GARAGE_BM_OK, or
+    // GARAGE_BM_E_MISSING_BLOCK when salvage does not apply or fails (never wrong bytes).
+    int salvage_stripe(const Hash &h, uint8_t *slot, uint32_t &block_len, uint8_t *live_ok, uint8_t *blk = nullptr)
+    {
+        if (!salvage_possible()) return GARAGE_BM_E_MISSING_BLOCK;
+        uint32_t expect = 0;
+        {
+            std::lock_guard<std::mutex> lk(refs_mu);
+            auto it = refs.find(h);
+            if (it == refs.end()) return GARAGE_BM_E_MISSING_BLOCK;
+            expect = it->second;
+        }
+        salvage_attempts++;
+        const size_t L = shard_len_of(expect);
+        if (L > slot_stride) {
+            salvage_failures++;
+            return GARAGE_BM_E_MISSING_BLOCK;
+        }
+        const uint32_t S = (uint32_t)((L + 7) / 8 + 15) / 16 * 16;  // the adler8 segment length
+        int who[64];
+        storage_nodes_of(h, who);
+        uint8_t seg[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
+        std::vector<uint8_t> tmp(slot_stride);
+        uint64_t nread = 0, from_q = 0;
+        // the header must name this index, the block length the others agree on (refs) and the adler8 tag
+        auto fits = [&](const ShardMeta &mt, int i) {
+            return mt.index == i && mt.block_len == expect && mt.shard_len == L && mt.sum_kind == GARAGE_EC_SUM_ADLER8;
+        };
+        auto seg_bits = [&](const uint8_t *b, const ShardMeta &mt) {  // bit g: segment g passes its tag (empty: set)
+            uint8_t bits = 0;
+            for (uint32_t g = 0, o = 0; g < 8; g++, o += S)
+                if (o >= L || garage_ec_check_shard_span_host(GARAGE_EC_SUM_ADLER8, b + o, (uint32_t)L, o,
+                                                              (uint32_t)std::min<size_t>(S, L - o), mt.sum.data()) == GARAGE_EC_OK)
+                    bits |= (uint8_t)(1u << g);
+            return bits;
+        };
+        for (int i = 0; i < tot; i++) {
+            seg[i] = 0;
+            live_ok[i] = 0;
+            Node &nd = *nodes[who[i]];
+            uint8_t *dst = slot + (size_t)i * slot_stride;
+            for (int q = 0; q < 2 && seg[i] != 0xFF; q++) {  // the live copy first, then the quarantined one
+                ShardMeta mt;
+                ReadResult r;
+                {
+                    std::lock_guard<std::mutex> lk(nd.mu);
+                    if (!nd.up) break;
+                    r = nd.salvage_read(h, q == 1, q ? tmp.data() : dst, slot_stride, mt);
+                }
+                if (r != kReadOk || !fits(mt, i)) continue;
+                nread += L;
+                const uint8_t bits = (uint8_t)(seg_bits(q ? tmp.data() : dst, mt) & ~seg[i]);
+                if (q == 0) live_ok[i] = bits == 0xFF;
+                for (uint32_t g = 0, o = 0; q && g < 8; g++, o += S)
+                    if ((bits >> g) & 1 && o < L) {
+                        memcpy(dst + o, tmp.data() + o, std::min<size_t>(S, L - o));
+                        from_q++;
+                    }
+                seg[i] |= bits;
+            }
+        }
+        salvage_bytes_read += nread;
+        salvage_quarantined_segments += from_q;
+        bool work = false;
+        for (int i = 0; i < tot; i++) work |= seg[i] != 0xFF;
+        if (work) {
+            const uint32_t L32 = (uint32_t)L;
+            int32_t st = 0;
+            const auto t0 = Clock::now();
+            const int rc = garage_ec_reconstruct_segments_stripes(grp().code_ctx[0], &slot, seg, nullptr, &st, &L32,
+                                                                  slot_stride, 1);
+            salvage_call_us += us_since(t0);
+            if (rc != GARAGE_EC_OK || st != 0) {
+                salvage_failures++;
+                return GARAGE_BM_E_MISSING_BLOCK;
+            }
+            const bool pb = codes[0].pb;
+            for (uint32_t g = 0; g < (pb ? 4u : 8u); g++)
+                for (int i = 0; i < tot && (pb || (size_t)g * S < L); i++)
+                    salvage_units_rebuilt += pb ? !((seg[i] >> g) & (seg[i] >> (g + 4)) & 1) : !((seg[i] >> g) & 1);
+        }
+        std::vector<uint8_t> own;
+        if (!blk) {
+            own.resize(expect);
+            blk = own.data();
+        }
+        assemble(slot, expect, blk);
+        if (!content_ok(h, blk, expect)) {  // e.g. a stale quarantined copy consistent with its own tag
+            salvage_failures++;
+            return GARAGE_BM_E_MISSING_BLOCK;
+        }
+        block_len = expect;
+        salvage_blocks++;
+        return GARAGE_BM_OK;
+    }
+    // A GET whose gather gave up: the salvaged block, or GARAGE_BM_E_MISSING_BLOCK as before.  Nothing is written: the
+    // damaged indices were queued for resync when they were quarantined.
+    int salvage_get(const Hash &h, uint8_t *slot, uint8_t *out, size_t cap, size_t *out_len)
+    {
+        uint8_t live[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
+        uint32_t bl = 0;
+        std::vector<uint8_t> blk;
+        {
+            std::lock_guard<std::mutex> lk(refs_mu);
+            auto it = refs.find(h);
+            if (it == refs.end() || it->second > cap) return GARAGE_BM_E_MISSING_BLOCK;
+        }
+        if (salvage_stripe(h, slot, bl, live, out) != GARAGE_BM_OK) return GARAGE_BM_E_MISSING_BLOCK;
+        *out_len = bl;
+        return GARAGE_BM_OK;
+    }
+    // A resync or stripe repair whose survivors could not rebuild: salvage the stripe and write every shard whose live
+    // copy was not whole and valid to its holder, with a fresh header and tag (.corrupted files stay).  Returns the shards
+    // written (*bytes_out += their bytes); -1 if salvage failed; -2 if the write of index `must` failed.
+    int salvage_heal(const Hash &h, uint8_t *slot, int must = -1, uint64_t *bytes_out = nullptr)
+    {
+        uint8_t live[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
+        uint32_t bl = 0;
+        if (salvage_stripe(h, slot, bl, live) != GARAGE_BM_OK) return -1;
+        int who[64];
+        storage_nodes_of(h, who);
+        const size_t L = shard_len_of(bl);
+        int n = 0;
+        bool must_ok = must < 0;
+        for (int i = 0; i < tot; i++) {
+            if (live[i]) continue;
+            const uint8_t *bytes = slot + (size_t)i * slot_stride;
+            Hash sum;
+            shard_tag(bytes, L, sum);
+            if (!write_shard(who[i], h, i, bl, bytes, L, sum.data())) continue;
+            n++;
+            if (bytes_out) *bytes_out += L;
+            must_ok |= i == must;
+        }
+        return must_ok ? n : -2;
+    }
+
     // manager.rs:344-363 + 276-339 on the stripe of `code`: gather, rebuild missing data shards, check the content
     // hash, and on a mismatch hunt the shard that is stale
     int get_from_stripe(const Hash &h, uint8_t *out, size_t cap, size_t *out_len, int code)
@@ -3049,7 +3210,8 @@ struct garage_bm {
         uint32_t block_len = 0;
         bool ok = false;
         gather_into(h, -1, slot.p, have, block_len, false, false, nullptr, &ok, nullptr, code);
-        if (!ok) return GARAGE_BM_E_MISSING_BLOCK;  // manager.rs:336-338
+        if (!ok)  // manager.rs:336-338, unless the stripe can be salvaged segment by segment
+            return code == 0 ? salvage_get(h, slot.p, out, cap, out_len) : GARAGE_BM_E_MISSING_BLOCK;
         *out_len = block_len;
         if (block_len > cap) return GARAGE_EC_E_INVALID;
         bool all_data = true;
@@ -3181,6 +3343,18 @@ struct garage_bm {
             if (has_legacy() && convert_batch({h}) == 1) {
                 resync_counter++;
                 return GARAGE_BM_OK;
+            }
+            // rebuild by segment from the survivors and the quarantined copies (DESIGN.md section 5.14)
+            if (salvage_possible()) {
+                const int w = salvage_heal(h, slot.p, idx);
+                if (w >= 0) {
+                    resync_counter++;
+                    return GARAGE_BM_OK;
+                }
+                if (w == -2) {
+                    resync_error_counter++;
+                    return GARAGE_BM_E_MESSAGE;  // as a failed write of the fetch branch
+                }
             }
             resync_error_counter++;
             resync_failed_bytes_read += nbytes;
@@ -4075,6 +4249,18 @@ struct garage_bm {
         }
         rebuild_batch(jobs, {stripe_repair_bytes_read, stripe_repair_bytes_fetched, stripe_repair_shards,
                              stripe_repair_bytes_written, stripe_repair_errors, &stripe_repair_call_us, false});
+        // stripes their survivors could not rebuild: salvage by segment (DESIGN.md section 5.14)
+        for (RebuildJob &jb : jobs) {
+            if (jb.written >= 0 || !salvage_possible()) continue;
+            SlotLease slot(grp().stripe_slots);
+            uint64_t nb = 0;
+            const int w = salvage_heal(jb.h, slot.p, -1, &nb);
+            if (w > 0) {
+                jb.written = w;
+                stripe_repair_shards += (uint64_t)w;
+                stripe_repair_bytes_written += nb;
+            }
+        }
         uint64_t nrep = 0, nshards = 0;
         for (const RebuildJob &jb : jobs)
             if (jb.written > 0) {
@@ -5514,6 +5700,18 @@ void garage_bm_get_drive_metrics(garage_bm *bm, garage_bm_drive_metrics *o)
     o->rebalance_bytes_moved = bm->rebalance_bytes_moved;
     o->rebalance_errors = bm->rebalance_errors;
     o->drive_marker_errors = bm->drive_marker_errors;
+}
+
+void garage_bm_get_salvage_metrics(garage_bm *bm, garage_bm_salvage_metrics *o)
+{
+    if (!bm || !o) return;
+    o->salvage_attempts = bm->salvage_attempts;
+    o->salvage_blocks = bm->salvage_blocks;
+    o->salvage_failures = bm->salvage_failures;
+    o->salvage_units_rebuilt = bm->salvage_units_rebuilt;
+    o->salvage_quarantined_segments = bm->salvage_quarantined_segments;
+    o->salvage_bytes_read = bm->salvage_bytes_read;
+    o->salvage_call_us = bm->salvage_call_us;
 }
 
 void garage_bm_get_stripe_repair_metrics(garage_bm *bm, garage_bm_stripe_repair_metrics *o)

@@ -257,7 +257,7 @@ template <int K, int MODE>
 cudaError_t launch_apply_t(const garage_ec_ctx *ctx, const ApplyParams &p, cudaStream_t st)
 {
     static std::atomic<int> configured_for_device{-1};  // per instantiation
-    using CFG = StreamCfg<K, MODE>;
+    using CFG = StreamCfg<K, cfg_mode(MODE)>;
     auto kern = rs_apply_kernel<K, MODE>;
     if ((size_t)CFG::kSmem > ctx->smem_optin) return cudaErrorInvalidConfiguration;
     // opt-in shared memory size is a per-function, per-device attribute; setting it is cheap
@@ -1643,6 +1643,281 @@ int garage_ec_reconstruct_stripes(garage_ec_ctx *ctx, uint8_t *const *stripes, c
     if (!shard_lens_ok(ctx, shard_len, stride, n_stripes)) return GARAGE_EC_E_INVALID;
     CU_TRY(ctx, cudaSetDevice(ctx->device));
     return reconstruct_host(ctx, nullptr, stripes, present, want, status, shard_len, stride, n_stripes);
+}
+
+// --------------------------------------------------------------------------- RECONSTRUCT BY SEGMENT (DESIGN.md 2.10)
+}  // extern "C"
+
+namespace {
+
+// Device scratch of run_segments for n stripes: unit plans | apply counter (16 B) | unit presence | unit want |
+// unit status | work list
+struct SegScratch {
+    size_t plan, counter, present, want, ustatus, units, bytes;
+    SegScratch(const garage_ec_ctx *ctx, size_t n)
+    {
+        const size_t nu = n * units_per_stripe(ctx->pb), tot = ctx->k + ctx->m;
+        plan = 0;
+        counter = nu * sizeof(StripePlan);
+        present = counter + 16;
+        want = present + align_up(nu * tot, 16);
+        ustatus = want + align_up(nu * tot, 16);
+        units = ustatus + nu * 4;
+        bytes = units + align_up((1 + nu) * 4, 16);
+    }
+};
+
+// n * U unit rows of k+m shards must stay below 2^32 (plan rows and work-list ids are 32-bit)
+bool seg_count_ok(const garage_ec_ctx *ctx, size_t n)
+{
+    return (unsigned long long)n * units_per_stripe(ctx->pb) * (ctx->k + ctx->m) < (1ull << 32);
+}
+
+// Device-resident reconstruct by unit.  scratch: SegScratch(ctx, n).bytes of device memory.
+int run_segments(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *seg_present, const uint8_t *want, int32_t *status,
+                 const uint32_t *shard_len, size_t stride, size_t n, uint8_t *scratch, cudaStream_t st)
+{
+    const SegScratch sc(ctx, n);
+    const size_t nu = n * units_per_stripe(ctx->pb), tot = ctx->k + ctx->m;
+    StripePlan *plan = reinterpret_cast<StripePlan *>(scratch + sc.plan);
+    uint32_t *counter = reinterpret_cast<uint32_t *>(scratch + sc.counter);
+    uint32_t *units = reinterpret_cast<uint32_t *>(scratch + sc.units);
+    int32_t *ustatus = reinterpret_cast<int32_t *>(scratch + sc.ustatus);
+    cudaError_t e = cudaMemsetAsync(units, 0, sizeof(uint32_t), st);
+    if (e != cudaSuccess) return set_cuda_error(ctx, e, "cudaMemsetAsync(units)");
+    UnitParams u;
+    memset(&u, 0, sizeof(u));
+    u.seg_present = seg_present;
+    u.want = want;
+    u.shard_len = shard_len;
+    u.unit_present = scratch + sc.present;
+    u.unit_want = want ? scratch + sc.want : nullptr;
+    u.unit_status = ustatus;
+    u.plan = plan;
+    u.status = status;
+    u.units = units;
+    u.n = (uint32_t)n;
+    u.tot = (uint32_t)tot;
+    u.stride = (uint32_t)stride;
+    u.pb = ctx->pb ? 1u : 0u;
+    unit_prep_kernel<<<(unsigned)((nu * tot + 255) / 256), 256, 0, st>>>(u);
+    ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return set_cuda_error(ctx, e, "unit_prep_kernel launch");
+    // the one survivor planner, over unit rows; shard_len NULL with stride 0: unit_prep_kernel already judged the
+    // stripe's geometry, and a malformed stripe's units are all present
+    PlanParams q;
+    memset(&q, 0, sizeof(q));
+    q.present = scratch + sc.present;
+    q.want = u.unit_want;
+    q.status = ustatus;
+    q.plan = plan;
+    q.counter = counter;
+    q.n = (uint32_t)nu;
+    q.k = (uint32_t)ctx->k;
+    q.m = (uint32_t)ctx->m;
+    q.l = (uint32_t)ctx->l;
+    q.pb = ctx->pb ? 1u : 0u;
+    memcpy(q.P, ctx->P, (size_t)ctx->k * ctx->m);
+    plan_kernel<<<(unsigned)((nu + kPlanWarps - 1) / kPlanWarps), kPlanWarps * 32, 0, st>>>(q);
+    ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return set_cuda_error(ctx, e, "plan_kernel launch");
+    unit_fold_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(u);
+    ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return set_cuda_error(ctx, e, "unit_fold_kernel launch");
+
+    TimedLaunch tl(ctx, st);
+    const int nout = ctx->pb ? 2 * ctx->m : ctx->m;
+    for (int r0 = 0; r0 < nout; r0 += kRowsPerPass) {
+        if (r0 > 0) {
+            e = cudaMemsetAsync(counter, 0, sizeof(uint32_t), st);
+            if (e != cudaSuccess) return set_cuda_error(ctx, e, "cudaMemsetAsync(counter)");
+        }
+        ApplyParams p;
+        memset(&p, 0, sizeof(p));
+        p.src = shards;
+        p.dst = shards;
+        p.src_pitch = p.dst_pitch = tot * stride;
+        p.shard_len = shard_len;
+        p.plan = plan;
+        p.units = units;
+        p.counter = counter;
+        p.stride = (uint32_t)stride;
+        p.n = (uint32_t)n;
+        p.k = (uint32_t)(ctx->pb ? 2 * ctx->k : ctx->k);
+        p.half = ctx->pb ? 1u : 0u;
+        p.row_off = (uint32_t)r0;
+        p.row_bytes = 128;
+        e = launch_apply<kModeUnits>(ctx, p, st);
+        if (e != cudaSuccess) return set_cuda_error(ctx, e, "rs_apply_kernel<units> launch");
+    }
+    return GARAGE_EC_OK;
+}
+
+// HOST form (garage_ec_reconstruct_segments(MEM_HOST) / _stripes): the chunk pipeline of reconstruct_host, by unit.  Up:
+// the read-set pieces of every unit that has work, of stripes whose every unit is recoverable.  Down: the rebuilt units
+// of those stripes (RS / LRC: with the zero tail of the shard's last unit).
+int segments_host(garage_ec_ctx *ctx, uint8_t *shards, uint8_t *const *stripes, const uint8_t *seg_present,
+                  const uint8_t *want, int32_t *status, const uint32_t *shard_len, size_t stride, size_t n)
+{
+    const size_t tot = ctx->k + ctx->m;
+    const uint32_t U = units_per_stripe(ctx->pb);
+    auto shard_at = [&](size_t s, size_t i) -> uint8_t * {
+        return stripes ? stripes[s] + i * stride : shards + (s * tot + i) * stride;
+    };
+    const bool zero_copy = !stripes && device_addressable_host(shards);
+    HostPipeline p(ctx, n, zero_copy ? 0 : tot * stride);
+    bool pinned = !zero_copy;
+    for (size_t s = 0; pinned && s < (stripes ? n : 1); s++) pinned = device_addressable_host(stripes ? stripes[s] : shards);
+    p.up.use_batch = p.down.use_batch = pinned;
+    SmallLayout sl;
+    const SegScratch sc(ctx, p.cs);
+    const size_t o_present = sl.take(p.cs * tot), o_want = sl.take(p.cs * tot), o_status = sl.take(p.cs * 4),
+                 o_len = sl.take(p.cs * 4), o_scratch = sl.take(sc.bytes);
+    int rc = p.reserve(zero_copy ? 0 : p.cs * tot * stride, sl.bytes);
+    if (rc) return rc;
+    int32_t *st_out = p.status_out(status);
+    // per unit of the chunk: the read plan (0 = no work or a stripe that will not be rebuilt)
+    std::vector<uint64_t> rows(p.cs * U);
+    std::vector<uint8_t> has_work(p.cs * U);
+    rc = p.run([&](const HostChunk &ch) -> int {
+        HostLane &L = *ch.L;
+        const size_t s0 = ch.s0, cnt = ch.cnt;
+        uint8_t *d_sh = zero_copy ? shards : L.d_buf;
+        for (size_t s = s0; s < s0 + cnt; s++) {
+            const uint32_t len = shard_len ? shard_len[s] : (uint32_t)stride;
+            const uint8_t *sp = seg_present + s * tot, *wn = want ? want + s * tot : nullptr;
+            bool ok = true;
+            for (uint32_t g = 0; g < U; g++) {
+                uint8_t up[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
+                bool work = false;  // a wanted shard is absent in this unit
+                for (size_t i = 0; i < tot; i++) {
+                    up[i] = unit_present(sp[i], len, g, ctx->pb) ? 1 : 0;
+                    work |= !up[i] && (!wn || wn[i]);
+                }
+                uint64_t hv = 0;
+                ok &= stripe_read_plan(ctx, up, wn, &hv);
+                rows[(s - s0) * U + g] = hv;
+                has_work[(s - s0) * U + g] = work;
+            }
+            if (!ok)
+                for (uint32_t g = 0; g < U; g++) has_work[(s - s0) * U + g] = 0;
+        }
+        // H2D: the pieces of each unit's read set
+        for (size_t s = s0; s < s0 + cnt && !zero_copy; s++) {
+            const uint32_t len = shard_len ? shard_len[s] : (uint32_t)stride;
+            for (uint32_t g = 0; g < U; g++) {
+                if (!has_work[(s - s0) * U + g]) continue;
+                uint32_t base, ulen;
+                unit_columns(len, g, ctx->pb, &base, &ulen);
+                const uint64_t hv = rows[(s - s0) * U + g];
+                for (size_t i = 0; i < tot; i++) {
+                    const unsigned b = read_halves(ctx, hv, i);
+                    for (unsigned h = 0; h < 2; h++) {
+                        if (!(b >> h & 1) || (!ctx->pb && h)) continue;
+                        const size_t off = base + (ctx->pb ? h * (size_t)(len / 2) : 0);
+                        p.up.add(d_sh + ((s - s0) * tot + i) * stride + off, shard_at(s, i) + off, align_up(ulen, 16));
+                    }
+                }
+            }
+        }
+        int r = p.up.flush(ctx, cudaMemcpyHostToDevice, L.stream);
+        if (r) return r;
+        CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_present, seg_present + s0 * tot, cnt * tot, cudaMemcpyHostToDevice,
+                                    L.stream));
+        const uint8_t *d_want = nullptr;
+        if (want) {
+            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_want, want + s0 * tot, cnt * tot, cudaMemcpyHostToDevice, L.stream));
+            d_want = L.d_small + o_want;
+        }
+        const uint32_t *d_len = nullptr;
+        if (shard_len) {
+            CU_TRY(ctx, cudaMemcpyAsync(L.d_small + o_len, shard_len + s0, cnt * 4, cudaMemcpyHostToDevice, L.stream));
+            d_len = reinterpret_cast<const uint32_t *>(L.d_small + o_len);
+        }
+        r = run_segments(ctx, d_sh, L.d_small + o_present, d_want, reinterpret_cast<int32_t *>(L.d_small + o_status), d_len,
+                         stride, cnt, L.d_small + o_scratch, L.stream);
+        if (r) return r;
+        CU_TRY(ctx, cudaMemcpyAsync(st_out + s0, L.d_small + o_status, cnt * 4, cudaMemcpyDeviceToHost, L.stream));
+        // D2H: exactly the rebuilt units
+        for (size_t s = s0; s < s0 + cnt && !zero_copy; s++) {
+            const uint32_t len = shard_len ? shard_len[s] : (uint32_t)stride;
+            const uint8_t *sp = seg_present + s * tot, *wn = want ? want + s * tot : nullptr;
+            for (uint32_t g = 0; g < U; g++) {
+                if (!has_work[(s - s0) * U + g]) continue;
+                uint32_t base, ulen;
+                unit_columns(len, g, ctx->pb, &base, &ulen);
+                for (size_t i = 0; i < tot; i++) {
+                    if (unit_present(sp[i], len, g, ctx->pb) || (wn && !wn[i])) continue;
+                    for (unsigned h = 0; h < (ctx->pb ? 2u : 1u); h++) {
+                        const size_t off = base + h * (size_t)(len / 2);
+                        p.down.add(shard_at(s, i) + off, d_sh + ((s - s0) * tot + i) * stride + off, align_up(ulen, 16));
+                    }
+                }
+            }
+        }
+        return p.down.flush(ctx, cudaMemcpyDeviceToHost, L.stream);
+    });
+    if (!rc) rc = p.drain();
+    if (rc) return rc;
+    for (size_t s = 0; s < n; s++)
+        if (st_out[s] != 0) return GARAGE_EC_E_UNRECOVERABLE;
+    return GARAGE_EC_OK;
+}
+
+// every stripe's L within the stride and, for PB, a multiple of 128 (HOST forms check before any GPU work)
+bool seg_lens_ok(const garage_ec_ctx *ctx, const uint32_t *shard_len, size_t stride, size_t n)
+{
+    const size_t unit = ctx->pb ? 128 : 1;
+    if (!shard_len) return stride % unit == 0;
+    for (size_t s = 0; s < n; s++)
+        if (shard_len[s] % unit || shard_len[s] > stride) return false;
+    return true;
+}
+
+}  // namespace
+
+extern "C" {
+
+int garage_ec_reconstruct_segments(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *seg_present, const uint8_t *want,
+                                   int32_t *status, const uint32_t *shard_len, size_t stride, size_t n_stripes,
+                                   int mem_kind, void *cuda_stream)
+{
+    if (!ctx || ctx->clay || (mem_kind != GARAGE_EC_MEM_HOST && mem_kind != GARAGE_EC_MEM_DEVICE))
+        return GARAGE_EC_E_INVALID;
+    int rc = check_geometry(ctx, stride, n_stripes, ctx->k + ctx->m);
+    if (rc) return rc;
+    if (n_stripes == 0) return GARAGE_EC_OK;
+    if (!shards || !seg_present || !seg_count_ok(ctx, n_stripes)) return GARAGE_EC_E_INVALID;
+    if (!aligned16(shards)) return GARAGE_EC_E_ALIGN;
+    if (mem_kind == GARAGE_EC_MEM_HOST && !seg_lens_ok(ctx, shard_len, stride, n_stripes)) return GARAGE_EC_E_INVALID;
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    if (mem_kind == GARAGE_EC_MEM_HOST)
+        return segments_host(ctx, shards, nullptr, seg_present, want, status, shard_len, stride, n_stripes);
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    return with_stream_scratch(ctx, SegScratch(ctx, n_stripes).bytes, st, [&](uint8_t *scratch) {
+        return run_segments(ctx, shards, seg_present, want, status, shard_len, stride, n_stripes, scratch, st);
+    });
+}
+
+int garage_ec_reconstruct_segments_stripes(garage_ec_ctx *ctx, uint8_t *const *stripes, const uint8_t *seg_present,
+                                           const uint8_t *want, int32_t *status, const uint32_t *shard_len,
+                                           size_t stride, size_t n_stripes)
+{
+    if (!ctx || ctx->clay) return GARAGE_EC_E_INVALID;
+    int rc = check_geometry(ctx, stride, n_stripes, ctx->k + ctx->m);
+    if (rc) return rc;
+    if (n_stripes == 0) return GARAGE_EC_OK;
+    if (!stripes || !seg_present || !seg_count_ok(ctx, n_stripes)) return GARAGE_EC_E_INVALID;
+    for (size_t s = 0; s < n_stripes; s++) {
+        if (!stripes[s]) return GARAGE_EC_E_INVALID;
+        if (!aligned16(stripes[s])) return GARAGE_EC_E_ALIGN;
+    }
+    if (!seg_lens_ok(ctx, shard_len, stride, n_stripes)) return GARAGE_EC_E_INVALID;
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    return segments_host(ctx, nullptr, stripes, seg_present, want, status, shard_len, stride, n_stripes);
 }
 
 // --------------------------------------------------------------------------- RANGED READS (DESIGN.md 2.5)

@@ -114,7 +114,10 @@ constexpr int kMaxGroups = 6;
 constexpr uint32_t kStageRowBytes = 512;  // 32 columns x 16 B of one shard
 constexpr uint32_t kSmemLimit = 227 * 1024;
 
-enum ApplyMode { kModeEncode = 0, kModePlan = 1, kModeVerify = 2 };
+enum ApplyMode { kModeEncode = 0, kModePlan = 1, kModeVerify = 2, kModeUnits = 3 };
+// kModeUnits (garage_ec_reconstruct_segments, DESIGN.md 4.13) is kModePlan over a list of adler8 units instead of
+// stripes: the same launch shape, tables and consumer warps, only the builder addresses a unit
+__host__ __device__ constexpr int cfg_mode(int mode) { return mode == kModeUnits ? kModePlan : mode; }
 
 // ---- table layout: k sources -> groups of 2^lg tables ---------------------------------------
 struct TabLayout {
@@ -317,6 +320,30 @@ struct __align__(16) StripePlan {
     uint8_t coef[kMaxM][kMaxK];  // out[r] = XOR_j coef[r][j] * row[surv[j]]
 };
 
+// adler8 tag segment length of a len-byte shard (the tag is described with adler8_shards_kernel below)
+__host__ __device__ inline uint32_t adler8_seg_bytes(uint32_t len)
+{
+    return (((len + 7) / 8) + 15) / 16 * 16;
+}
+// Columns of unit g of a stripe of shard length L (DESIGN.md 2.10): RS and LRC, adler8 segment g,
+// [g*S, min(L, (g+1)*S)) with S = adler8_seg_bytes(L); PB (L % 128 == 0), columns [g*L/8, (g+1)*L/8) of each half, which
+// are segments g and g+4.  An empty unit has len 0.
+__host__ __device__ inline void unit_columns(uint32_t L, uint32_t g, bool pb, uint32_t *base, uint32_t *len)
+{
+    const uint32_t S = pb ? L / 8 : adler8_seg_bytes(L), a = g * S;
+    *base = a;
+    *len = pb ? S : (a >= L ? 0u : (L - a < S ? L - a : S));
+}
+// Is shard i present in unit g, from its seg_present byte b (bit g: segment g holds valid bytes)?  A PB unit needs
+// both of its segments; an empty unit is present in every shard.
+__host__ __device__ inline bool unit_present(uint8_t b, uint32_t L, uint32_t g, bool pb)
+{
+    uint32_t base, len;
+    unit_columns(L, g, pb, &base, &len);
+    if (!len) return true;
+    return pb ? ((b >> g) & (b >> (g + 4)) & 1) != 0 : ((b >> g) & 1) != 0;
+}
+
 struct ApplyParams {
     const uint8_t *src;            // stripe s source base = src + s*src_pitch
     uint8_t *dst;                  // stripe s output base = dst + s*dst_pitch
@@ -337,10 +364,14 @@ struct ApplyParams {
     uint32_t rows_per_stripe;   // shards per stripe in `src` (k for encode, k+m for verify): tensor row of (s, j) = s*rows_per_stripe + j
     uint32_t half;              // kModePlan, PB contexts: plan indices are half-rows q = 2*shard + half (DESIGN.md 2.2)
     uint8_t coef[kRowsPerPass * kMaxK];  // uniform modes: coef[i*k + j]
+    // kModeUnits: units[0] = work units, units[1 + w] = unit id s*U + g (U = 8, PB: 4); plan is per unit id.  It sits
+    // in the padding before `tmap`, so the parameter block of the other modes keeps its size
+    const uint32_t *units;
     // 2-D view of `src` for TMA: dim0 = stride/4 uint32 elements, dim1 = n*rows_per_stripe shards
     // (pitch `stride`), box = 128 elements (512 B = 32 columns) x k rows
     alignas(64) CUtensorMap tmap;
 };
+static_assert(sizeof(ApplyParams) == 384, "ApplyParams layout");
 
 // ------------------------------------------------------------------ small device helpers
 template <int I, int N, class F> __device__ __forceinline__ void static_for(F &&f)
@@ -761,12 +792,12 @@ __device__ __forceinline__ void group_lookup(uint32_t (&acc)[16], uint4 (&d)[16]
 }
 
 // ------------------------------------------------------------------ the streaming kernel
-template <int K, int MODE> struct KernelCfg : StreamCfg<K, MODE> {
+template <int K, int MODE> struct KernelCfg : StreamCfg<K, cfg_mode(MODE)> {
     static constexpr int kK = K;
 };
 
 template <int K, int MODE>
-__global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kernel(const __grid_constant__ ApplyParams p)
+__global__ void __launch_bounds__(StreamCfg<K, cfg_mode(MODE)>::kThreads, 1) rs_apply_kernel(const __grid_constant__ ApplyParams p)
 {
     using CFG = KernelCfg<K, MODE>;
     constexpr int S = CFG::S;
@@ -792,7 +823,7 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
     uint32_t stage_parity = 0;
 
     // TMA: lane 0 arms the warp's stage with `nrow` x `rb` bytes; the copies are issued by the caller
-    if constexpr (MODE != kModePlan) {
+    if constexpr (cfg_mode(MODE) != kModePlan) {
         // ---- uniform coefficient matrix: build once, then warps stream items ----------------
         build_tables<CFG>(tab, p.coef, K, p.rows, warp, (uint32_t)NW, K);
         __syncthreads();
@@ -1047,7 +1078,12 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
             // chunk ranges each (4096 stripes on 132 SMs are 31.03 stripes per SM: with whole stripes only, a
             // few SMs streamed a 32nd stripe alone at the end).  The parts of a stripe have the same erasure
             // pattern: a table buffer that gets another part of the stripe it already holds skips the build.
-            const uint32_t whole = p.n > 2 * gridDim.x ? p.n - 2 * gridDim.x : 0;
+            // kModeUnits: work unit w is unit units[1 + w], its plan p.plan[unit], its rows the unit's columns.
+            // kModePlan compares with p.n itself below, not with nwork: a register copy of the count held across the
+            // loop changes that mode's register allocation (RS(4, m) reconstruct's spills)
+            constexpr bool kUnits = MODE == kModeUnits;
+            const uint32_t nwork = kUnits ? __ldg(p.units) : p.n;
+            const uint32_t whole = nwork > 2 * gridDim.x ? nwork - 2 * gridDim.x : 0;
             uint32_t claimed = 0;
             if (lane == 0) claimed = atomicAdd(p.counter, 1u);
             // pattern whose tables each buffer holds (scalars, not arrays: `b` is a run-time index)
@@ -1066,13 +1102,23 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
                 int rows = 0;
                 uint32_t ns = 0;
                 unsigned long long kp = 0, ko = 0;
-                const uint32_t slen = s < p.n ? (p.shard_len ? __ldg(p.shard_len + s) : p.stride) : 0;
+                uint32_t sid = s, pid = s, ubase = 0, ulen = 0;  // kModeUnits: the unit's stripe, plan and columns
+                if constexpr (kUnits) {
+                    if (s < nwork) {
+                        pid = __ldg(p.units + 1 + s);
+                        sid = pid / (p.half ? 4u : 8u);
+                    }
+                }
+                const uint32_t slen = s < (kUnits ? nwork : p.n) ? (p.shard_len ? __ldg(p.shard_len + sid) : p.stride) : 0;
+                if constexpr (kUnits) unit_columns(slen, pid % (p.half ? 4u : 8u), p.half != 0, &ubase, &ulen);
                 // source / output index -> byte offset: a shard, or (PB) the half-row q = 2*shard + half
                 auto idx_off = [&](uint32_t i) -> uint32_t {
-                    return p.half ? (i >> 1) * p.stride + (i & 1) * (slen >> 1) : i * p.stride;
+                    const uint32_t o = p.half ? (i >> 1) * p.stride + (i & 1) * (slen >> 1) : i * p.stride;
+                    if constexpr (kUnits) return o + ubase;
+                    else return o;
                 };
-                if (s < p.n) {
-                    const StripePlan *pl = p.plan + s;
+                if (s < (kUnits ? nwork : p.n)) {
+                    const StripePlan *pl = p.plan + pid;
                     rows = pl->unrecoverable ? 0 : min(kRowsPerPass, (int)pl->nrows - (int)p.row_off);
                     if (rows > 0) {
                         ns = pl->nsurv;
@@ -1085,9 +1131,11 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
                     }
                 }
                 if (lane == 0) {
-                    const uint32_t len = p.half ? slen >> 1 : slen;  // PB: chunks of one half
+                    uint32_t len = p.half ? slen >> 1 : slen;  // PB: chunks of one half
+                    if constexpr (kUnits) len = ulen;
                     const uint32_t nch = (((len + 15) >> 4) + 31) >> 5;  // 32-column chunks of the stripe
                     ps.sid = s;
+                    if constexpr (kUnits) ps.sid = s < nwork ? sid : p.n;
                     ps.rows = rows;
                     ps.chunk_next = part * nch / parts;
                     ps.chunk_end = (part + 1) * nch / parts;
@@ -1109,7 +1157,7 @@ __global__ void __launch_bounds__(StreamCfg<K, MODE>::kThreads, 1) rs_apply_kern
                     }
                 }
                 mbar_arrive(bar_full + 8 * b);  // all 32 lanes: each lane's table stores are released by its own arrive
-                if (s >= p.n) break;
+                if (s >= (kUnits ? nwork : p.n)) break;
             }
             return;
         }
@@ -1440,6 +1488,65 @@ __global__ void __launch_bounds__(kPlanWarps * 32, 16) plan_kernel(const __grid_
         pl->nsurv = (uint8_t)nsurv;
         if (q.status) q.status[s] = ok ? 0 : -4;
     }
+}
+
+// ---- reconstruct by adler8 unit (garage_ec_reconstruct_segments, DESIGN.md 2.10 / 4.13) -------------------------
+// unit_prep_kernel turns the per-shard segment bits into one presence row per unit, plan_kernel plans the n*U rows,
+// unit_fold_kernel gives each stripe its status and lists the units with work, and rs_apply_kernel<kModeUnits>
+// rebuilds only those units' columns.
+struct UnitParams {
+    const uint8_t *seg_present;  // n*(k+m): bit g = segment g of shard i holds valid bytes
+    const uint8_t *want;         // n*(k+m), nullable
+    const uint32_t *shard_len;   // n, nullable (=> stride)
+    uint8_t *unit_present;       // n*U*(k+m) out (prep)
+    uint8_t *unit_want;          // n*U*(k+m) out (prep), when want != NULL
+    const int32_t *unit_status;  // n*U, plan_kernel's verdict per unit (fold)
+    const StripePlan *plan;      // n*U (fold)
+    int32_t *status;             // n, nullable (fold)
+    uint32_t *units;             // 1 + n*U (fold): units[0] = count (zero at launch), then unit ids
+    uint32_t n, tot, stride, pb;
+};
+__host__ __device__ inline uint32_t units_per_stripe(bool pb) { return pb ? 4u : 8u; }
+// A stripe whose L exceeds the stride, or a PB stripe whose L is not a multiple of 128, is malformed
+__device__ __forceinline__ uint32_t unit_stripe_len(const UnitParams &q, uint32_t s, bool *bad)
+{
+    const uint32_t L = q.shard_len ? __ldg(q.shard_len + s) : q.stride;
+    *bad = L > q.stride || (q.pb && (L & 127));
+    return L;
+}
+// one thread per (unit, shard); a malformed stripe's units are all present (no work)
+__global__ void __launch_bounds__(256) unit_prep_kernel(const __grid_constant__ UnitParams q)
+{
+    const uint32_t U = units_per_stripe(q.pb != 0);
+    const size_t e = (size_t)blockIdx.x * 256 + threadIdx.x;
+    if (e >= (size_t)q.n * U * q.tot) return;
+    const uint32_t unit = (uint32_t)(e / q.tot), i = (uint32_t)(e % q.tot), s = unit / U, g = unit % U;
+    bool bad;
+    const uint32_t L = unit_stripe_len(q, s, &bad);
+    const size_t si = (size_t)s * q.tot + i;
+    q.unit_present[e] = (bad || unit_present(__ldg(q.seg_present + si), L, g, q.pb != 0)) ? 1 : 0;
+    if (q.want) q.unit_want[e] = __ldg(q.want + si);
+}
+// one thread per stripe: status, then the ids of its units that rebuild rows, appended to the work list (any order:
+// every unit writes only its own columns)
+__global__ void __launch_bounds__(256) unit_fold_kernel(const __grid_constant__ UnitParams q)
+{
+    const uint32_t s = blockIdx.x * 256 + threadIdx.x;
+    if (s >= q.n) return;
+    const uint32_t U = units_per_stripe(q.pb != 0);
+    bool bad;
+    (void)unit_stripe_len(q, s, &bad);
+    int32_t st = bad ? GARAGE_EC_E_INVALID : 0;
+    for (uint32_t g = 0; g < U && !st; g++)
+        if (q.unit_status[(size_t)s * U + g] != 0) st = GARAGE_EC_E_UNRECOVERABLE;
+    if (q.status) q.status[s] = st;
+    if (st) return;
+    uint32_t cnt = 0;
+    for (uint32_t g = 0; g < U; g++) cnt += q.plan[(size_t)s * U + g].nrows > 0;
+    if (!cnt) return;
+    uint32_t w = atomicAdd(q.units, cnt);
+    for (uint32_t g = 0; g < U; g++)
+        if (q.plan[(size_t)s * U + g].nrows > 0) q.units[1 + w++] = s * U + g;
 }
 
 // ---- PB(k, m) encode / verify (DESIGN.md section 2.2) -----------------------------------------------------------
@@ -2089,10 +2196,6 @@ __global__ void __launch_bounds__(256) transcode_reframe_kernel(const __grid_con
 // bytes for each, so the kernel streams at HBM speed; one warp per shard, four 16-byte loads per
 // lane in flight.  Pinned by python's zlib.adler32 (tests/test_blake2.py).
 constexpr uint32_t kAdlerMod = 65521;
-__host__ __device__ inline uint32_t adler8_seg_bytes(uint32_t len)
-{
-    return (((len + 7) / 8) + 15) / 16 * 16;
-}
 
 __global__ void __launch_bounds__(256) adler8_shards_kernel(const __grid_constant__ SumParams q)
 {

@@ -199,6 +199,19 @@ typedef struct garage_bm_stripe_repair_metrics {
     uint64_t stripe_repair_errors;        /* unrecoverable stripes + shard writes that failed                   */
     uint64_t stripe_repair_call_us;       /* wall time inside garage_ec_reconstruct_stripes                     */
 } garage_bm_stripe_repair_metrics;
+/* Counters of salvage (DESIGN.md section 5.14): a GET, resync or stripe repair whose survivors could not rebuild the
+ * configured stripe of an adler8 store (RS, LRC or PB) rebuilds it segment by segment from the live shards and their
+ * quarantined copies (garage_ec_reconstruct_segments), proven by the block's content hash.  A struct of its own for
+ * the same reason. */
+typedef struct garage_bm_salvage_metrics {
+    uint64_t salvage_attempts;             /* stripes salvage was tried on                                        */
+    uint64_t salvage_blocks;               /* stripes salvaged: rebuilt and proven by the content hash            */
+    uint64_t salvage_failures;             /* tries that ended in an unrecoverable unit or a content-hash mismatch */
+    uint64_t salvage_units_rebuilt;        /* (shard, unit) pieces rebuilt: a segment, for PB a pair of segments  */
+    uint64_t salvage_quarantined_segments; /* segments taken from quarantined copies                              */
+    uint64_t salvage_bytes_read;           /* shard bytes read, live and quarantined copies                        */
+    uint64_t salvage_call_us;              /* wall time inside garage_ec_reconstruct_segments_stripes              */
+} garage_bm_salvage_metrics;
 /* Counters of the drives (DESIGN.md section 5.7), in a struct of their own for the same reason. */
 typedef struct garage_bm_drive_metrics {
     uint64_t rebalance_files_moved; /* files garage_bm_rebalance_step wrote to their primary drive (old copy removed) */
@@ -600,6 +613,7 @@ int garage_bm_storage_nodes_of(garage_bm *bm, const uint8_t hash[32], int *nodes
 void garage_bm_get_metrics(garage_bm *bm, garage_bm_metrics *out);
 void garage_bm_get_range_metrics(garage_bm *bm, garage_bm_range_metrics *out);
 void garage_bm_get_stripe_repair_metrics(garage_bm *bm, garage_bm_stripe_repair_metrics *out);
+void garage_bm_get_salvage_metrics(garage_bm *bm, garage_bm_salvage_metrics *out);
 
 #ifdef __cplusplus
 }

@@ -199,6 +199,38 @@ int garage_ec_reconstruct_stripes(garage_ec_ctx *ctx, uint8_t *const *stripes, c
                                   const uint8_t *want, int32_t *status, const uint32_t *shard_len,
                                   size_t stride, size_t n_stripes);
 
+/* ---- RECONSTRUCT BY SEGMENT (normative: DESIGN.md section 2.10) -- a stripe with more than m damaged shards whose
+ * damage falls in different adler8 segments: every segment of a stripe covers the same byte columns of all k+m shards,
+ * and each is decoded on its own.  Shard layout, stride and alignment rules: those of garage_ec_reconstruct.
+ *   seg_present : n * (k+m) bytes; bit g set = segment g of shard i holds valid bytes (0x00 a wholly absent shard, 0xFF
+ *                 a whole one).  Segment g of a stripe = [g*S, min(L, (g+1)*S)), S = roundup16(ceil(L/8)): the adler8
+ *                 segments, the runs garage_ec_tag_span names.  An empty segment counts as present.
+ *   want        : NULL = every shard with a cleared bit; else n * (k+m) bytes, only wanted shards are completed.
+ *   Units       : RS and LRC: one segment.  PB: segments g and g+4 (g < 4), with L % 128 == 0 so that S = L/8; a shard
+ *                 is present in a PB unit only if both bits are set.  Each unit is decoded from the code's own read
+ *                 set for the unit's presence map (RS: the first k present shards; LRC: the local group when it
+ *                 suffices; PB: garage_ec_read_plan), and every missing unit of a wanted shard is rebuilt from it.  A
+ *                 unit's verdict is garage_ec_reconstruct's for that presence map and want.
+ *   Writes      : only the bytes of rebuilt units, and the zero tail [L, roundup16(L)) of a shard whose last unit is
+ *                 rebuilt.  A unit whose bytes are present is never written.
+ *   status      : n int32 (nullable in DEVICE mode): 0; GARAGE_EC_E_UNRECOVERABLE if a unit cannot be rebuilt (nothing
+ *                 of the stripe is written); DEVICE only: GARAGE_EC_E_INVALID for an L past `stride` or, for PB, an L
+ *                 that is not a multiple of 128 (nothing of the stripe is read or written).
+ * With every seg_present byte 0x00 or 0xFF the output is byte-identical to garage_ec_reconstruct with
+ * present = (byte == 0xFF).  Clay contexts return GARAGE_EC_E_INVALID before any CUDA call: a Clay shard's layers are
+ * coupled across the whole shard, so its segments are not independent codewords.
+ *   DEVICE: only kernels and stream-ordered scratch are enqueued (capturable in a CUDA graph); reads only the survivor
+ *           bytes of each unit's read set, never past byte n*(k+m)*stride of `shards`.
+ *   HOST:   synchronous; GARAGE_EC_E_INVALID before any GPU work for a malformed L; uploads only the survivor units of
+ *           stripes that have work and downloads only the rebuilt units; returns GARAGE_EC_E_UNRECOVERABLE if any
+ *           stripe was.  The _stripes form is the gather form, as garage_ec_reconstruct_stripes.                    */
+int garage_ec_reconstruct_segments(garage_ec_ctx *ctx, uint8_t *shards, const uint8_t *seg_present,
+                                   const uint8_t *want, int32_t *status, const uint32_t *shard_len,
+                                   size_t stride, size_t n_stripes, int mem_kind, void *cuda_stream);
+int garage_ec_reconstruct_segments_stripes(garage_ec_ctx *ctx, uint8_t *const *stripes,
+                                           const uint8_t *seg_present, const uint8_t *want, int32_t *status,
+                                           const uint32_t *shard_len, size_t stride, size_t n_stripes);
+
 /* ---- VERIFY (scrub) -- call sites: DataBlock::verify via BlockManager::read_block,
  * src/block/manager.rs:554-609 / src/block/block.rs:69-83, driven by ScrubWorker::work,
  * src/block/repair.rs:438-490: recompute parity from the k data shards and compare with

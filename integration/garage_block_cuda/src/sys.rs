@@ -184,6 +184,12 @@ extern "C" {
     pub fn garage_ec_reconstruct_stripes(ctx: *mut garage_ec_ctx, stripes: *const *mut u8, present: *const u8,
                             want: *const u8, status: *mut i32, shard_len: *const u32, stride: usize,
                             n_stripes: usize) -> c_int;
+    pub fn garage_ec_reconstruct_segments(ctx: *mut garage_ec_ctx, shards: *mut u8, seg_present: *const u8,
+                            want: *const u8, status: *mut i32, shard_len: *const u32, stride: usize,
+                            n_stripes: usize, mem_kind: c_int, cuda_stream: *mut c_void) -> c_int;
+    pub fn garage_ec_reconstruct_segments_stripes(ctx: *mut garage_ec_ctx, stripes: *const *mut u8,
+                            seg_present: *const u8, want: *const u8, status: *mut i32,
+                            shard_len: *const u32, stride: usize, n_stripes: usize) -> c_int;
     pub fn garage_ec_set_sum_kind(ctx: *mut garage_ec_ctx, kind: c_int) -> c_int;
     pub fn garage_ec_set_wait_mode(ctx: *mut garage_ec_ctx, blocking: c_int) -> c_int;
     pub fn garage_ec_copy_for_dma(dst_pinned: *mut c_void, src: *const c_void, n: usize);
