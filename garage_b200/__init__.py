@@ -48,7 +48,7 @@ ABI_SYMBOLS = [
     "garage_ec_reseal", "garage_ec_reseal_stripes",
     "garage_ec_seal_crc", "garage_ec_seal_blocks_crc", "garage_ec_reseal_crc", "garage_ec_reseal_stripes_crc",
     "garage_ec_crc_combine",
-    "garage_ec_reconstruct_segments", "garage_ec_reconstruct_segments_stripes",
+    "garage_ec_reconstruct_segments", "garage_ec_reconstruct_segments_stripes", "garage_ec_segment_read_ranges",
 ]
 
 
@@ -123,6 +123,7 @@ def load_library(build=True):
     L.garage_ec_reconstruct_stripes.argtypes = [vp, vp, vp, vp, vp, vp, sz, sz]
     L.garage_ec_reconstruct_segments.argtypes = [vp, vp, vp, vp, vp, vp, sz, sz, i32, vp]
     L.garage_ec_reconstruct_segments_stripes.argtypes = [vp, vp, vp, vp, vp, vp, sz, sz]
+    L.garage_ec_segment_read_ranges.argtypes = [vp, vp, vp, u32, vp, sz, C.POINTER(sz)]
     L.garage_ec_set_sum_kind.argtypes = [vp, i32]
     L.garage_ec_set_wait_mode.argtypes = [vp, i32]
     L.garage_ec_copy_for_dma.argtypes = [vp, vp, C.c_size_t]
@@ -401,6 +402,21 @@ class GarageEc:
         n = C.c_size_t(0)
         rc = self._check(self._L.garage_ec_read_ranges(self._h, _ptr(pr), _ptr(wn), shard_len, _ptr(out), cap,
                                                        C.byref(n)), (E_UNRECOVERABLE,))
+        if rc == E_UNRECOVERABLE:
+            return None
+        return [tuple(int(v) for v in out[3 * i:3 * i + 3]) for i in range(n.value)]
+
+    def segment_read_ranges(self, seg_present, shard_len, want=None, cap=None):
+        """[(shard, offset, len)] byte runs reconstruct_segments reads to complete one stripe's wanted shards, or None
+        if a unit is unrecoverable (DESIGN.md section 2.10)"""
+        sp = np.ascontiguousarray(seg_present, dtype=np.uint8)
+        wn = None if want is None else np.ascontiguousarray(want, dtype=np.uint8)
+        assert sp.shape == (self.k + self.m,) and (wn is None or wn.shape == sp.shape)
+        cap = (self.k + self.m) * 8 if cap is None else cap
+        out = np.zeros(max(1, cap) * 3, dtype=np.uint32)
+        n = C.c_size_t(0)
+        rc = self._check(self._L.garage_ec_segment_read_ranges(self._h, _ptr(sp), _ptr(wn), shard_len, _ptr(out), cap,
+                                                               C.byref(n)), (E_UNRECOVERABLE,))
         if rc == E_UNRECOVERABLE:
             return None
         return [tuple(int(v) for v in out[3 * i:3 * i + 3]) for i in range(n.value)]

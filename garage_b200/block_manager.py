@@ -21,7 +21,7 @@ SYMBOLS = [
     "garage_bm_convert_step", "garage_bm_debug_convert_stop_after", "garage_bm_apply_layout", "garage_bm_layout_sync_step",
     "garage_bm_layout_versions", "garage_bm_deep_scrub_step", "garage_bm_rpc_get_block_range",
     "garage_bm_get_range_metrics", "garage_bm_stripe_repair_step", "garage_bm_get_stripe_repair_metrics",
-    "garage_bm_get_salvage_metrics",
+    "garage_bm_get_salvage_metrics", "garage_bm_get_segment_repair_metrics",
     "garage_bm_set_data_dirs", "garage_bm_rebalance_step", "garage_bm_get_drive_metrics", "garage_bm_create_with_drives",
     "garage_bm_resync_step", "garage_bm_list_resync_errors", "garage_bm_resync_retry_now", "garage_bm_block_info",
     "garage_bm_debug_set_clock_ms", "garage_bm_get_resync_metrics",
@@ -115,6 +115,11 @@ class SalvageMetrics(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in (
         "salvage_attempts", "salvage_blocks", "salvage_failures", "salvage_units_rebuilt", "salvage_quarantined_segments",
         "salvage_bytes_read", "salvage_call_us")]
+
+
+class SegmentRepairMetrics(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in (
+        "repairs", "units_rebuilt", "bytes_read", "bytes_fetched", "fallbacks", "call_us")]
 
 
 class ResyncMetrics(C.Structure):
@@ -223,6 +228,8 @@ def load_library():
         L.garage_bm_get_stripe_repair_metrics.restype = None
         L.garage_bm_get_salvage_metrics.argtypes = [vp, C.POINTER(SalvageMetrics)]
         L.garage_bm_get_salvage_metrics.restype = None
+        L.garage_bm_get_segment_repair_metrics.argtypes = [vp, C.POINTER(SegmentRepairMetrics)]
+        L.garage_bm_get_segment_repair_metrics.restype = None
         L.garage_bm_create_with_drives.argtypes = [C.POINTER(vp), C.POINTER(Config), C.POINTER(DataDir), i32]
         L.garage_bm_create_on_devices.argtypes = [C.POINTER(vp), C.POINTER(Config), C.POINTER(DataDir), i32,
                                                   C.POINTER(C.c_int), i32]
@@ -560,6 +567,12 @@ class BlockManager:
         mt = SalvageMetrics()
         self._L.garage_bm_get_salvage_metrics(self._h, C.byref(mt))
         return {n: getattr(mt, n) for n, _ in SalvageMetrics._fields_}
+
+    def segment_repair_metrics(self):
+        """garage_bm_segment_repair_metrics (DESIGN.md section 5.15) as a dict"""
+        mt = SegmentRepairMetrics()
+        self._L.garage_bm_get_segment_repair_metrics(self._h, C.byref(mt))
+        return {n: getattr(mt, n) for n, _ in SegmentRepairMetrics._fields_}
 
     def set_data_dirs(self, node, dirs):
         """node restarts with this data_dir list ((path, capacity[, read_only]) tuples or dicts) -> rc; a failed marker

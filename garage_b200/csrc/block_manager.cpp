@@ -41,6 +41,7 @@
 #include <type_traits>
 #include <thread>
 #include <unordered_map>
+#include <unordered_set>
 #include <vector>
 
 #include <fcntl.h>
@@ -392,6 +393,11 @@ struct Node {
     using ShardPtr = std::shared_ptr<const StoredShard>;
     std::unordered_map<Hash, ShardPtr, HashHasher> shards;
     std::unordered_map<Hash, ShardPtr, HashHasher> corrupted;  // the ".corrupted" quarantine
+    // repair by segment (DESIGN.md section 5.15): the hashes whose quarantined copy here was quarantined because its
+    // adler8 tag failed -- not named stale by the content-hash hunt or deep scrub, not a bad header.  A stale copy
+    // passes its own tags, so only this verdict lets resync keep a copy's good segments.  Memory only: a restart
+    // forgets it and resync rebuilds the whole shard.  Any write, erase or other quarantine of the hash clears it.
+    std::unordered_set<Hash, HashHasher> tag_failed;
     // block_local_resync_queue (resync.rs:90, put_to_resync_at :241-256): one entry per hash with the time it falls
     // due (ms on the manager's clock), iterated in (due, hash) order
     std::unordered_map<Hash, int64_t, HashHasher> resync_due;
@@ -767,6 +773,7 @@ struct Node {
     // in-memory: the copy was made by the caller; the shard it replaces is returned, to be freed outside the lock
     ShardPtr store_put_ptr(const Hash &h, ShardPtr sp)
     {
+        tag_failed.erase(h);
         shards[h].swap(sp);
         return sp;
     }
@@ -891,6 +898,7 @@ struct Node {
     bool store_put(const Hash &h, const ShardMeta &mt, const uint8_t *bytes, size_t n, int newest = -1,
                    const std::function<bool()> &allow = [] { return true; })
     {
+        tag_failed.erase(h);
         if (dir.empty()) {
             auto sp = std::make_shared<StoredShard>();
             static_cast<ShardMeta &>(*sp) = mt;
@@ -955,6 +963,13 @@ struct Node {
             return it == map.end() ? kReadMissing : copy_out(*it->second, dst, cap, mt);
         }
         return quarantined ? file_read_into(path_of(h, ".corrupted"), 0, dst, cap, mt) : store_read_into(h, dst, cap, mt);
+    }
+    // h has a quarantined copy here (".corrupted", memory store: Node::corrupted)
+    bool has_quarantined(const Hash &h) const
+    {
+        if (dir.empty()) return corrupted.count(h) != 0;
+        std::error_code ec;
+        return std::filesystem::exists(path_of(h, ".corrupted"), ec);
     }
     // one shard file read as a shard of `code`
     ReadResult file_read_into(const std::string &path, int code, uint8_t *dst, size_t cap, ShardMeta &mt, ShardSpan span = {}) const
@@ -1123,13 +1138,17 @@ struct Node {
     }
     bool store_erase(const Hash &h)
     {
+        tag_failed.erase(h);
         if (dir.empty()) return shards.erase(h) != 0;
         return remove_file(h, ".shard");
     }
     // move_block_to_corrupted (manager.rs:807-819): file >= 0 that ShardFile of h; code -1 the replica; index >= 0
-    // (by_index stores) the file holding that index; otherwise the file holding the shard of `code`
-    void store_quarantine(const Hash &h, int code = 0, int index = -1, int file = -1)
+    // (by_index stores) the file holding that index; otherwise the file holding the shard of `code`.  tag: the shard
+    // is quarantined because its adler8 tag failed (Node::tag_failed)
+    void store_quarantine(const Hash &h, int code = 0, int index = -1, int file = -1, bool tag = false)
     {
+        if (tag) tag_failed.insert(h);
+        else tag_failed.erase(h);
         if (dir.empty()) {
             auto it = shards.find(h);
             if (it != shards.end()) {
@@ -1758,6 +1777,8 @@ struct garage_bm {
         layout_deleted{0}, layout_sync_errors{0}, layout_bytes_fetched{0};
     std::atomic<uint64_t> salvage_attempts{0}, salvage_blocks{0}, salvage_failures{0}, salvage_units_rebuilt{0},
         salvage_quarantined_segments{0}, salvage_bytes_read{0}, salvage_call_us{0};
+    std::atomic<uint64_t> segrep_repairs{0}, segrep_units_rebuilt{0}, segrep_bytes_read{0}, segrep_bytes_fetched{0},
+        segrep_fallbacks{0}, segrep_call_us{0};
     std::atomic<uint64_t> stripe_repairs{0}, stripe_repair_shards{0}, stripe_repair_bytes_read{0},
         stripe_repair_bytes_fetched{0}, stripe_repair_bytes_written{0}, stripe_repair_errors{0}, stripe_repair_call_us{0};
     std::atomic<uint64_t> rebalance_files_moved{0}, rebalance_bytes_moved{0}, rebalance_errors{0}, drive_marker_errors{0};
@@ -1918,14 +1939,15 @@ struct garage_bm {
     }
 
     // code -1: the node's replica of h.  index >= 0: the file holding that index (by_index stores).  file >= 0: that
-    // Node::ShardFile of h
-    void quarantine(int node, const Hash &h, int code = 0, int index = -1, int file = -1)
+    // Node::ShardFile of h.  tag_failed: a configured-code shard whose tag failed (a repair by segment may keep its good
+    // segments, DESIGN.md section 5.15)
+    void quarantine(int node, const Hash &h, int code = 0, int index = -1, int file = -1, bool tag_failed = false)
     {
         corruption_counter++;
         {
             Node &nd = *nodes[node];
             std::lock_guard<std::mutex> lk(nd.mu);
-            nd.store_quarantine(h, code, index, file);
+            nd.store_quarantine(h, code, index, file, tag_failed);
         }
         put_to_resync(node, h);
     }
@@ -1973,7 +1995,7 @@ struct garage_bm {
                     return true;
             }
         }
-        quarantine(node, h, code, index);
+        quarantine(node, h, code, index, -1, r == kReadOk && code == 0);  // a tag mismatch, or a bad header
         return false;
     }
 
@@ -3061,6 +3083,20 @@ struct garage_bm {
     // of every index from the live shard or, failing that, from its quarantined copy, and each unit rebuilt on its own
     // (garage_ec_reconstruct_segments).  RS, LRC and PB stores with one active layout version only.
     bool salvage_possible() const { return sum_kind == GARAGE_EC_SUM_ADLER8 && !codes[0].clay && !multi_version(); }
+    // the adler8 segment length of an L-byte shard
+    static uint32_t seg_len(size_t L) { return (uint32_t)((L + 7) / 8 + 15) / 16 * 16; }
+    // bit g: adler8 segment g of the L-byte shard b passes its value in the tag sum32 (an empty segment: set).  Salvage
+    // and repair by segment keep a copy's segment on this proof alone.
+    static uint8_t good_segments(const uint8_t *b, size_t L, const uint8_t *sum32)
+    {
+        const uint32_t S = seg_len(L);
+        uint8_t bits = 0;
+        for (uint32_t g = 0, o = 0; g < 8; g++, o += S)
+            if (o >= L || garage_ec_check_shard_span_host(GARAGE_EC_SUM_ADLER8, b + o, (uint32_t)L, o,
+                                                          (uint32_t)std::min<size_t>(S, L - o), sum32) == GARAGE_EC_OK)
+                bits |= (uint8_t)(1u << g);
+        return bits;
+    }
 
     // The stripe of h rebuilt by segment into `slot` (a stripe slot) and proven by its content hash; the block goes to
     // blk (block_len bytes, nullable).  live_ok[i]: index i's live shard was whole and valid.  GARAGE_BM_OK, or
@@ -3081,7 +3117,7 @@ struct garage_bm {
             salvage_failures++;
             return GARAGE_BM_E_MISSING_BLOCK;
         }
-        const uint32_t S = (uint32_t)((L + 7) / 8 + 15) / 16 * 16;  // the adler8 segment length
+        const uint32_t S = seg_len(L);
         int who[64];
         storage_nodes_of(h, who);
         uint8_t seg[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
@@ -3090,14 +3126,6 @@ struct garage_bm {
         // the header must name this index, the block length the others agree on (refs) and the adler8 tag
         auto fits = [&](const ShardMeta &mt, int i) {
             return mt.index == i && mt.block_len == expect && mt.shard_len == L && mt.sum_kind == GARAGE_EC_SUM_ADLER8;
-        };
-        auto seg_bits = [&](const uint8_t *b, const ShardMeta &mt) {  // bit g: segment g passes its tag (empty: set)
-            uint8_t bits = 0;
-            for (uint32_t g = 0, o = 0; g < 8; g++, o += S)
-                if (o >= L || garage_ec_check_shard_span_host(GARAGE_EC_SUM_ADLER8, b + o, (uint32_t)L, o,
-                                                              (uint32_t)std::min<size_t>(S, L - o), mt.sum.data()) == GARAGE_EC_OK)
-                    bits |= (uint8_t)(1u << g);
-            return bits;
         };
         for (int i = 0; i < tot; i++) {
             seg[i] = 0;
@@ -3114,7 +3142,7 @@ struct garage_bm {
                 }
                 if (r != kReadOk || !fits(mt, i)) continue;
                 nread += L;
-                const uint8_t bits = (uint8_t)(seg_bits(q ? tmp.data() : dst, mt) & ~seg[i]);
+                const uint8_t bits = (uint8_t)(good_segments(q ? tmp.data() : dst, L, mt.sum.data()) & ~seg[i]);
                 if (q == 0) live_ok[i] = bits == 0xFF;
                 for (uint32_t g = 0, o = 0; q && g < 8; g++, o += S)
                     if ((bits >> g) & 1 && o < L) {
@@ -3198,6 +3226,105 @@ struct garage_bm {
             must_ok |= i == must;
         }
         return must_ok ? n : -2;
+    }
+
+    // ---- repair by segment (DESIGN.md section 5.15) -------------------------------------------
+    // Resync of index idx of h on `node`, whose quarantined copy failed its adler8 tag (Node::tag_failed): the copy's
+    // units that pass their segment tags stay, the others are rebuilt from the same columns of the survivors -- the
+    // garage_ec_segment_read_ranges runs, each read through read_shard_into and checked against its holder's tag --
+    // and the shard is written, with the copy's tag, only if all eight segment values match that tag.  `slot`: a
+    // stripe slot.  true: written.  false: not tried (the store does not qualify, or the node holds no quarantined
+    // copy) or failed (a fallback: a missing hint, a copy that does not fit, no good or no bad unit, an absent or bad
+    // survivor span, an unrecoverable unit, a failed post-check or write); the caller rebuilds the whole shard.
+    bool segment_repair(int node, const Hash &h, int idx, uint8_t *slot)
+    {
+        if (!salvage_possible()) return false;
+        uint32_t expect = 0;
+        {
+            std::lock_guard<std::mutex> lk(refs_mu);
+            auto it = refs.find(h);
+            if (it == refs.end()) return false;
+            expect = it->second;
+        }
+        const size_t L = shard_len_of(expect);
+        Node &nd = *nodes[node];
+        uint8_t *own = slot + (size_t)idx * slot_stride;
+        ShardMeta cm;  // the copy's header
+        ReadResult r = kReadMissing;
+        {
+            std::lock_guard<std::mutex> lk(nd.mu);
+            if (!nd.up || !nd.has_quarantined(h)) return false;
+            if (nd.tag_failed.count(h) && L <= slot_stride) r = nd.salvage_read(h, true, own, slot_stride, cm);
+        }
+        uint64_t nread = 0, fetched = 0, nshards = 0;
+        auto count = [&] {
+            segrep_bytes_read += nread;
+            segrep_bytes_fetched += fetched;
+            resync_bytes_read += nread;
+            resync_bytes_fetched += fetched;
+            resync_shards_read += nshards;
+        };
+        auto fallback = [&] {
+            count();
+            segrep_fallbacks++;
+            return false;
+        };
+        if (r != kReadOk) return fallback();
+        nread += L;
+        if (cm.index != idx || cm.block_len != expect || cm.shard_len != L || cm.sum_kind != GARAGE_EC_SUM_ADLER8)
+            return fallback();
+        const bool pb = codes[0].pb;
+        uint8_t bits = good_segments(own, L, cm.sum.data());
+        if (pb) bits &= (uint8_t)((bits >> 4) | (bits << 4));  // a PB unit is segments g and g + 4: both or neither
+        const uint32_t S = seg_len(L);
+        int ngood = 0, nbad = 0;
+        for (uint32_t g = 0; g < (pb ? 4u : 8u); g++)
+            if (pb || (size_t)g * S < L) ((bits >> g) & 1 ? ngood : nbad)++;
+        if (!ngood || !nbad) return fallback();
+        // the survivors: every other index whose holder is up
+        int who[64];
+        storage_nodes_of(h, who);
+        uint8_t seg[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M], want[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
+        for (int i = 0; i < tot; i++) {
+            Node &x = *nodes[who[i]];
+            std::lock_guard<std::mutex> lk(x.mu);
+            seg[i] = x.up ? 0xFF : 0x00;
+        }
+        seg[idx] = bits;
+        want[idx] = 1;
+        garage_ec_range runs[(GARAGE_EC_MAX_K + GARAGE_EC_MAX_M) * 8];
+        size_t nr = 0;
+        if (garage_ec_segment_read_ranges(codes[0].ctx, seg, want, (uint32_t)L, runs, sizeof(runs) / sizeof(runs[0]),
+                                          &nr) != GARAGE_EC_OK)
+            return fallback();
+        for (size_t x = 0; x < nr; x++) {
+            const garage_ec_range &rn = runs[x];
+            ShardMeta mt;
+            if (!read_shard_into(who[rn.shard], h, slot + (size_t)rn.shard * slot_stride + rn.offset,
+                                 slot_stride - rn.offset, mt, /*for_dma=*/true, 0, -1, ShardSpan::bytes(rn.offset, rn.len)))
+                return fallback();  // absent, or a span that failed its holder's tag (quarantined and queued)
+            nread += rn.len;
+            fetched += rn.len;
+            nshards += x == 0 || runs[x - 1].shard != rn.shard;
+            if (mt.index != (int)rn.shard || mt.block_len != expect || mt.shard_len != L) return fallback();
+        }
+        const uint32_t L32 = (uint32_t)L;
+        int32_t st = 0;
+        const auto t0 = Clock::now();
+        const int rc = garage_ec_reconstruct_segments_stripes(grp().code_ctx[0], &slot, seg, want, &st, &L32, slot_stride, 1);
+        segrep_call_us += us_since(t0);
+        if (rc != GARAGE_EC_OK || st != 0) return fallback();
+        Hash sum;
+        shard_tag(own, L, sum);
+        // the eight segment values written at PUT: a stale copy that rotted fails here
+        if (memcmp(sum.data(), cm.sum.data(), 32) != 0) return fallback();
+        if (!write_shard(node, h, idx, expect, own, L, cm.sum.data())) return fallback();
+        count();
+        segrep_repairs++;
+        segrep_units_rebuilt += (uint64_t)nbad;
+        resync_recv_counter++;
+        resync_counter++;
+        return true;
     }
 
     // manager.rs:344-363 + 276-339 on the stripe of `code`: gather, rebuild missing data shards, check the content
@@ -3324,6 +3451,8 @@ struct garage_bm {
                 return c > 0 ? GARAGE_BM_OK : GARAGE_BM_E_MESSAGE;
             }
         }
+        // a shard whose tag failed: only its damaged units, from the same columns of the survivors (DESIGN.md 5.15)
+        if (segment_repair(node, h, idx, slot.p)) return GARAGE_BM_OK;
         uint8_t have[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M], want[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M] = {0};
         uint32_t block_len = 0;
         bool ok = false;
@@ -4713,7 +4842,8 @@ struct garage_bm {
                 nchecked++;
                 if (state[i] == 3 || (state[i] == 1 && !bad[i])) continue;
                 nbad++;
-                quarantine(node, items[c0 + i].first, 0, -1, items[c0 + i].second);
+                quarantine(node, items[c0 + i].first, 0, -1, items[c0 + i].second,
+                           state[i] == 1 && items[c0 + i].second == Node::kShardFile);  // tag failed on the GPU
             }
         }
         scrub_checked += nchecked;
@@ -5712,6 +5842,17 @@ void garage_bm_get_salvage_metrics(garage_bm *bm, garage_bm_salvage_metrics *o)
     o->salvage_quarantined_segments = bm->salvage_quarantined_segments;
     o->salvage_bytes_read = bm->salvage_bytes_read;
     o->salvage_call_us = bm->salvage_call_us;
+}
+
+void garage_bm_get_segment_repair_metrics(garage_bm *bm, garage_bm_segment_repair_metrics *o)
+{
+    if (!bm || !o) return;
+    o->repairs = bm->segrep_repairs;
+    o->units_rebuilt = bm->segrep_units_rebuilt;
+    o->bytes_read = bm->segrep_bytes_read;
+    o->bytes_fetched = bm->segrep_bytes_fetched;
+    o->fallbacks = bm->segrep_fallbacks;
+    o->call_us = bm->segrep_call_us;
 }
 
 void garage_bm_get_stripe_repair_metrics(garage_bm *bm, garage_bm_stripe_repair_metrics *o)

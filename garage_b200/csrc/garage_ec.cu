@@ -667,6 +667,32 @@ void for_each_read_piece(const garage_ec_ctx *ctx, uint64_t rows, size_t i, size
     else if (b == 3) f((size_t)0, len);
     else f(b == 1 ? (size_t)0 : len / 2, len / 2);
 }
+// The plan of unit g (DESIGN.md 2.10) of one stripe of shard length len (sp / wn: its k+m seg_present and want bytes,
+// wn nullable): *rows as stripe_read_plan gives them for the unit's presence map, *work = a wanted shard is absent in
+// the unit.  False if the unit cannot be rebuilt.  The HOST reconstruct by segment uploads, and
+// garage_ec_segment_read_ranges names, the for_each_unit_piece pieces of these rows.
+bool unit_read_plan(const garage_ec_ctx *ctx, const uint8_t *sp, const uint8_t *wn, uint32_t len, uint32_t g,
+                    uint64_t *rows, bool *work)
+{
+    uint8_t up[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
+    *work = false;
+    for (int i = 0; i < ctx->k + ctx->m; i++) {
+        up[i] = unit_present(sp[i], len, g, ctx->pb) ? 1 : 0;
+        *work |= !up[i] && (!wn || wn[i]);
+    }
+    return stripe_read_plan(ctx, up, wn, rows);
+}
+// The pieces of shard i that unit g's plan `rows` reads, as f(offset, bytes): the unit's columns, for PB those of each
+// planned half
+template <class F>
+void for_each_unit_piece(const garage_ec_ctx *ctx, uint64_t rows, size_t i, uint32_t len, uint32_t g, F &&f)
+{
+    uint32_t base, ulen;
+    unit_columns(len, g, ctx->pb, &base, &ulen);
+    const unsigned b = read_halves(ctx, rows, i);
+    for (unsigned h = 0; h < (ctx->pb ? 2u : 1u); h++)
+        if ((b >> h) & 1) f(base + h * (size_t)(len / 2), (size_t)ulen);
+}
 // Every stripe's shard_len (NULL: stride) must be at most the stride and, for PB, a multiple of 32 so that the halves
 // are 16-byte aligned; for Clay, a multiple of 16*alpha, so that every layer's sub-chunk is
 bool shard_lens_ok(const garage_ec_ctx *ctx, const uint32_t *shard_len, size_t stride, size_t n)
@@ -1791,14 +1817,9 @@ int segments_host(garage_ec_ctx *ctx, uint8_t *shards, uint8_t *const *stripes, 
             const uint8_t *sp = seg_present + s * tot, *wn = want ? want + s * tot : nullptr;
             bool ok = true;
             for (uint32_t g = 0; g < U; g++) {
-                uint8_t up[GARAGE_EC_MAX_K + GARAGE_EC_MAX_M];
-                bool work = false;  // a wanted shard is absent in this unit
-                for (size_t i = 0; i < tot; i++) {
-                    up[i] = unit_present(sp[i], len, g, ctx->pb) ? 1 : 0;
-                    work |= !up[i] && (!wn || wn[i]);
-                }
                 uint64_t hv = 0;
-                ok &= stripe_read_plan(ctx, up, wn, &hv);
+                bool work = false;  // a wanted shard is absent in this unit
+                ok &= unit_read_plan(ctx, sp, wn, len, g, &hv, &work);
                 rows[(s - s0) * U + g] = hv;
                 has_work[(s - s0) * U + g] = work;
             }
@@ -1810,17 +1831,10 @@ int segments_host(garage_ec_ctx *ctx, uint8_t *shards, uint8_t *const *stripes, 
             const uint32_t len = shard_len ? shard_len[s] : (uint32_t)stride;
             for (uint32_t g = 0; g < U; g++) {
                 if (!has_work[(s - s0) * U + g]) continue;
-                uint32_t base, ulen;
-                unit_columns(len, g, ctx->pb, &base, &ulen);
-                const uint64_t hv = rows[(s - s0) * U + g];
-                for (size_t i = 0; i < tot; i++) {
-                    const unsigned b = read_halves(ctx, hv, i);
-                    for (unsigned h = 0; h < 2; h++) {
-                        if (!(b >> h & 1) || (!ctx->pb && h)) continue;
-                        const size_t off = base + (ctx->pb ? h * (size_t)(len / 2) : 0);
+                for (size_t i = 0; i < tot; i++)
+                    for_each_unit_piece(ctx, rows[(s - s0) * U + g], i, len, g, [&](size_t off, size_t ulen) {
                         p.up.add(d_sh + ((s - s0) * tot + i) * stride + off, shard_at(s, i) + off, align_up(ulen, 16));
-                    }
-                }
+                    });
             }
         }
         int r = p.up.flush(ctx, cudaMemcpyHostToDevice, L.stream);
@@ -2016,6 +2030,25 @@ int merge_runs(std::vector<garage_ec_range> &runs, garage_ec_range *ranges, size
 
 }  // namespace
 extern "C" {
+
+int garage_ec_segment_read_ranges(const garage_ec_ctx *ctx, const uint8_t *seg_present, const uint8_t *want,
+                                  uint32_t shard_len, garage_ec_range *ranges, size_t cap, size_t *n_ranges)
+{
+    if (!ctx || !seg_present || !n_ranges || (cap && !ranges)) return GARAGE_EC_E_INVALID;
+    *n_ranges = 0;
+    if (ctx->clay || (ctx->pb && shard_len % 128)) return GARAGE_EC_E_INVALID;
+    std::vector<garage_ec_range> runs;
+    for (uint32_t g = 0; g < units_per_stripe(ctx->pb); g++) {
+        uint64_t hv = 0;
+        bool work = false;
+        if (!unit_read_plan(ctx, seg_present, want, shard_len, g, &hv, &work)) return GARAGE_EC_E_UNRECOVERABLE;
+        for (int i = 0; work && i < ctx->k + ctx->m; i++)
+            for_each_unit_piece(ctx, hv, (size_t)i, shard_len, g, [&](size_t off, size_t bytes) {
+                runs.push_back(garage_ec_range{(uint32_t)i, (uint32_t)off, (uint32_t)bytes});
+            });
+    }
+    return merge_runs(runs, ranges, cap, n_ranges);
+}
 
 int garage_ec_range_plan(const garage_ec_ctx *ctx, const uint8_t *present, uint32_t block_len, uint32_t offset,
                          uint32_t len, garage_ec_range *ranges, size_t cap, size_t *n_ranges, int *needs_gpu)

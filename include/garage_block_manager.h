@@ -212,6 +212,19 @@ typedef struct garage_bm_salvage_metrics {
     uint64_t salvage_bytes_read;           /* shard bytes read, live and quarantined copies                        */
     uint64_t salvage_call_us;              /* wall time inside garage_ec_reconstruct_segments_stripes              */
 } garage_bm_salvage_metrics;
+/* Counters of repair by segment (DESIGN.md section 5.15): a resync of a shard its node quarantined because its adler8
+ * tag failed keeps the copy's units that pass their segment tags and rebuilds only the others, from the same columns
+ * of the survivors (garage_ec_segment_read_ranges, garage_ec_reconstruct_segments_stripes).  RS, LRC and PB stores
+ * with adler8 tags and one active layout version.  These bytes are counted in resync_bytes_read and
+ * resync_bytes_fetched too.  A struct of its own for the same reason. */
+typedef struct garage_bm_segment_repair_metrics {
+    uint64_t repairs;       /* shards written by the partial path                                           */
+    uint64_t units_rebuilt; /* (shard, unit) pieces rebuilt: a segment, for PB a pair of segments           */
+    uint64_t bytes_read;    /* quarantined-copy + survivor span bytes read                                  */
+    uint64_t bytes_fetched; /* survivor run bytes: what would cross the network in Garage                   */
+    uint64_t fallbacks;     /* partial tries (the node held a quarantined copy) that ended in the whole-shard path */
+    uint64_t call_us;       /* wall time inside garage_ec_reconstruct_segments_stripes                      */
+} garage_bm_segment_repair_metrics;
 /* Counters of the drives (DESIGN.md section 5.7), in a struct of their own for the same reason. */
 typedef struct garage_bm_drive_metrics {
     uint64_t rebalance_files_moved; /* files garage_bm_rebalance_step wrote to their primary drive (old copy removed) */
@@ -614,6 +627,7 @@ void garage_bm_get_metrics(garage_bm *bm, garage_bm_metrics *out);
 void garage_bm_get_range_metrics(garage_bm *bm, garage_bm_range_metrics *out);
 void garage_bm_get_stripe_repair_metrics(garage_bm *bm, garage_bm_stripe_repair_metrics *out);
 void garage_bm_get_salvage_metrics(garage_bm *bm, garage_bm_salvage_metrics *out);
+void garage_bm_get_segment_repair_metrics(garage_bm *bm, garage_bm_segment_repair_metrics *out);
 
 #ifdef __cplusplus
 }

@@ -230,6 +230,16 @@ int garage_ec_reconstruct_segments(garage_ec_ctx *ctx, uint8_t *shards, const ui
 int garage_ec_reconstruct_segments_stripes(garage_ec_ctx *ctx, uint8_t *const *stripes,
                                            const uint8_t *seg_present, const uint8_t *want, int32_t *status,
                                            const uint32_t *shard_len, size_t stride, size_t n_stripes);
+/* garage_ec_segment_read_ranges (host only, ONE stripe of shard length shard_len; seg_present / want: k+m bytes, as
+ * for garage_ec_reconstruct_segments): the byte runs {shard, offset, len} garage_ec_reconstruct_segments reads to
+ * complete the wanted shards -- for every unit in which a wanted shard is absent, the unit's columns of each shard of
+ * that unit's read set (RS: the first k present; LRC: the local group when it suffices; PB: the garage_ec_read_plan
+ * halves).  Runs are in garage_ec_read_ranges' order and merge rule: by shard, then offset, adjacent runs merged.
+ * Bytes outside them are never read: a stripe holding only these runs (and its own present units) rebuilds to the
+ * same bytes.  GARAGE_EC_E_INVALID on a Clay context, for PB with shard_len % 128 != 0, or when the runs pass `cap`
+ * (*n_ranges = the runs needed); GARAGE_EC_E_UNRECOVERABLE when a unit cannot be rebuilt.                          */
+int garage_ec_segment_read_ranges(const garage_ec_ctx *ctx, const uint8_t *seg_present, const uint8_t *want,
+                                  uint32_t shard_len, garage_ec_range *ranges, size_t cap, size_t *n_ranges);
 
 /* ---- VERIFY (scrub) -- call sites: DataBlock::verify via BlockManager::read_block,
  * src/block/manager.rs:554-609 / src/block/block.rs:69-83, driven by ScrubWorker::work,

@@ -190,6 +190,9 @@ extern "C" {
     pub fn garage_ec_reconstruct_segments_stripes(ctx: *mut garage_ec_ctx, stripes: *const *mut u8,
                             seg_present: *const u8, want: *const u8, status: *mut i32,
                             shard_len: *const u32, stride: usize, n_stripes: usize) -> c_int;
+    pub fn garage_ec_segment_read_ranges(ctx: *const garage_ec_ctx, seg_present: *const u8, want: *const u8,
+                            shard_len: u32, ranges: *mut garage_ec_range, cap: usize,
+                            n_ranges: *mut usize) -> c_int;
     pub fn garage_ec_set_sum_kind(ctx: *mut garage_ec_ctx, kind: c_int) -> c_int;
     pub fn garage_ec_set_wait_mode(ctx: *mut garage_ec_ctx, blocking: c_int) -> c_int;
     pub fn garage_ec_copy_for_dma(dst_pinned: *mut c_void, src: *const c_void, n: usize);
